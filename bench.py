@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- the hot path of rorosen/zeekstd (per-frame compress + decompress of a seekable archive) on B200.
+"""bench.py -- the hot path of rorosen/zeekstd (per-frame compress + decompress of a seekable archive) on H100.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
@@ -24,8 +24,9 @@ configs[1] per rank (data that originates on the host goes H2D per GPU, no NCCL 
 (oracle/libzstd_driver.c; the Rust crate itself cannot be built in this image -- no cargo, no network) on the SAME
 bytes (the generator is counter-based: identical on CPU and GPU), frames spread over every host thread; what one thread
 reaches (zeekstd itself is single-threaded) is reported beside it.  Both arms report the MEAN over the timed steps.
-`roofline.traffic` comes from the committed ncu capture named in `traffic_source`: a bench value is never taken under a
-profiler.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step returned (frame sizes, and a seeded sample of the
+archive and of the decompressed output) as DIR/<name>.npy, so that two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -53,7 +54,6 @@ SEED = 20260924
 METRIC = "GiB/s compress + decompress (2 MiB frames)"
 KERNEL_NAMES = ["zk_scan_kernel", "zk_seq_kernel", "zk_huf_kernel", "zk_exec_kernel", "zk_xxh64_kernel", "zk_match_kernel",
                 "zk_entropy_enc_kernel", "zk_frame_*_kernels"]
-TRAFFIC_FILE = os.path.join(ROOT, "profiles", "traffic_r2.json")
 
 
 def workload_c1():
@@ -70,7 +70,7 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 def whole_direction(n_plain, n_comp, c_ms, d_ms, n_gpus):
@@ -166,7 +166,7 @@ def single_thread_note(data: np.ndarray, level: int, checksum: bool):
             "sample": f"{data.size >> 20} MiB", "note": "what zeekstd's own single-threaded Encoder/Decoder reaches"}
 
 
-L2_NOTE = "GPU arm: a 256 MiB buffer is written between timed iterations and the inputs exceed the 126 MB L2"
+L2_NOTE = "GPU arm: a 256 MiB buffer is written between timed iterations and the inputs exceed the 50 MB L2"
 EXCHANGE_C4 = ("GPU arm: NCCL inside the timed region -- scatter input -> compress -> all_gather(frame sizes) -> gather archive to root; "
                "scatter archive -> decompress -> gather output to root (chunked, pipelined, two communicators)")
 
@@ -180,6 +180,24 @@ def config_c1(n):
 def config_c4(nbytes, world):
     return {"workload": workload_c4(nbytes), "frame_size": FRAME, "level": C4_LEVEL, "checksum": True, "bytes_total": nbytes, "step": "compress+decompress",
             "parallelism": f"frames sharded over {world} GPUs, root-held buffer", "l2": L2_NOTE, "exchange": EXCHANGE_C4}
+
+
+DUMP_SEED = 20261015
+DUMP_SAMPLE = 1 << 21                      # bytes sampled per array: 2 Mi x float32 = 8 MiB, at most four such arrays per run
+
+
+def dump_outputs(d, prefix, archive, c_sizes, d_sizes, output):
+    """--dump-outputs: what the timed path handed back in its last step -- per-frame compressed / decompressed sizes (whole) and a fixed,
+    seeded sample of the archive and of the decompressed output (DUMP_SAMPLE sorted byte positions, the same on every run)"""
+    import torch
+    os.makedirs(d, exist_ok=True)
+    arrays = {"compressed_sizes": np.asarray(c_sizes, dtype=np.float64), "decompressed_sizes": np.asarray(d_sizes, dtype=np.float64)}
+    for name, t in (("archive_sample", archive), ("output_sample", output)):
+        idx = np.sort(np.random.default_rng(DUMP_SEED).integers(0, t.numel(), min(DUMP_SAMPLE, t.numel())))
+        arrays[name] = t[torch.from_numpy(idx).to(t.device)].to(torch.float32).cpu().numpy()
+    for name, a in arrays.items():
+        np.save(os.path.join(d, f"{prefix}_{name}.npy"), a)
+    return sorted(f"{prefix}_{name}.npy" for name in arrays)
 
 
 # ================================================================================================ reference arm
@@ -233,7 +251,7 @@ class Rig:
         self.lib = N.load()
         self.ctx = zk.Context(local, self.lib)
         self.dev = torch.device("cuda", local)
-        self.flush = torch.empty(256 << 20, dtype=torch.uint8, device=self.dev)          # > 126 MB L2: written between steps
+        self.flush = torch.empty(256 << 20, dtype=torch.uint8, device=self.dev)          # > 50 MB L2: written between steps
 
     def device_step_fn(self, x, level, checksum):
         torch, N, lib, ctx = self.torch, self.N, self.lib, self.ctx
@@ -257,7 +275,7 @@ class Rig:
             rc = lib.zk_decompress_frames_dev(ctx._h, comp.data_ptr(), co.ctypes.data_as(N.u64p), do.ctypes.data_as(N.u64p), k, back.data_ptr(), int(checksum), None, None)
             assert rc == 0, rc
             return t_c, ctx.last_device_ms, int(co[-1])
-        step.back, step.cs, step.nf = back, cs, nf
+        step.back, step.comp, step.cs, step.ds, step.nf = back, comp, cs, ds, nf
         return step
 
     def timed_device(self, x, level, checksum, warmup, steps, dist=None):
@@ -386,13 +404,7 @@ def roofline_block(rig, alg_bytes, n):
     peak, peak_src = peaks()
     per = [float(kms[i]) / max(1, int(kcnt[i])) for i in range(8)]
     dom = int(np.argmax(per))
-    traffic, traffic_src = None, None
-    try:
-        tj = json.load(open(TRAFFIC_FILE))
-        if n == (1 << 30) and KERNEL_NAMES[dom] in tj["bytes_per_launch"]:
-            traffic, traffic_src = tj["bytes_per_launch"][KERNEL_NAMES[dom]], tj["source"]
-    except (OSError, ValueError, KeyError):
-        pass
+    traffic, traffic_src = None, None          # no profiler capture is kept with the project: measured DRAM traffic is not reported
     achieved = alg_bytes / (per[dom] / 1e3) / 1e9 if per[dom] > 0 else 0.0
     return {"bound": "hbm", "kernel": KERNEL_NAMES[dom], "achieved": round(achieved, 2), "peak": peak, "unit": "GB/s", "frac": round(achieved / peak, 5),
             "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src, "algorithmic_bytes_per_launch": int(alg_bytes),
@@ -435,6 +447,10 @@ def main_ours(args, rank, world, local, ncores):
     sampler = ClockSampler(local); sampler.start()
     tc_ms, td_ms, clen = rig.timed_device(x, LEVEL, False, W, K, dist)
     clocks = sampler.result()
+    dumped = []
+    if args.dump_outputs and rank == 0:
+        ls = rig.last_step
+        dumped += dump_outputs(args.dump_outputs, "configs1", ls.comp[:clen], ls.cs[:ls.nf.value], ls.ds[:ls.nf.value], ls.back[:n])
     launches = ctx.kernel_launches - launches0
     roof = roofline_block(rig, n + clen, n) if rank == 0 else None
     lib.zk_ctx_profile(ctx._h, 0)
@@ -457,7 +473,10 @@ def main_ours(args, rank, world, local, ncores):
         # ---- configs[3] shape on one GPU: level 3 + checksum (fused into the codec kernels), device-resident
         nb = min(C4_BYTES, C4_ONE_GPU_BYTES)
         x4 = gen_mix(nb, C4_SEED, corpus.CLASS_MIX_MIXED, device=dev)
-        c4c, c4d, c4len = rig.timed_device(x4, C4_LEVEL, True, 3, max(2, K // 2))
+        c4c, c4d, c4len = rig.timed_device(x4, C4_LEVEL, True, 3, K)
+        if args.dump_outputs:
+            ls = rig.last_step
+            dumped += dump_outputs(args.dump_outputs, "configs3_one_gpu", ls.comp[:c4len], ls.cs[:ls.nf.value], ls.ds[:ls.nf.value], ls.back[:nb])
         c4 = {"config": config_c4(nb, 1), "value": round(2 * (nb / gib) / ((c4c + c4d) / 1e3), 3), "compress_GiBps": round(nb / gib / (c4c / 1e3), 3),
               "decompress_GiBps": round(nb / gib / (c4d / 1e3), 3), "ratio": round(nb / c4len, 4)}
         del x4, rig.last_step
@@ -470,6 +489,8 @@ def main_ours(args, rank, world, local, ncores):
                 "ratio": round(n / clen, 4), "gpu_launches": int(launches), "clocks": clocks, "e2e": e2e, "roofline": roof,
                 "roofline_whole_direction": whole_direction(n, clen, tc_ms, td_ms, 1), "config4_one_gpu": c4,
                 "cpu_baseline": cpu_baseline_block(x.cpu().numpy(), ncores, LEVEL, False, f"the {n >> 20} MiB workload")}
+        if dumped:
+            line["dump_outputs"] = {"dir": args.dump_outputs, "files": dumped}
         print(json.dumps(line), flush=True)
         return 0
 
@@ -508,7 +529,7 @@ def main_ours(args, rank, world, local, ncores):
     dist.barrier(); torch.cuda.synchronize()
     tcs = tds = 0.0
     acc = {}
-    for _ in range(K):
+    for it in range(K):
         rig.flush.fill_(1); torch.cuda.synchronize(); dist.barrier()
         st = {}
         ev[0].record()
@@ -520,10 +541,12 @@ def main_ours(args, rank, world, local, ncores):
         for k_, v_ in st.items():
             acc[k_] = acc.get(k_, 0.0) + float(v_)
         clen4 = int(np.sum(cs))
+        if it == K - 1 and args.dump_outputs and rank == 0:
+            dumped += dump_outputs(args.dump_outputs, "configs3", frames[:clen4], cs, ds, back[:nb])
         del frames, back
     torch.cuda.synchronize(); dist.barrier()
     clocks4 = sampler.result()
-    e2e4 = c4_host_leg(parallel, codec, xr, nb, FRAME, C4_LEVEL, dev, rank, max(1, min(2, K)), torch.cuda.synchronize, True)
+    e2e4 = c4_host_leg(parallel, codec, xr, nb, FRAME, C4_LEVEL, dev, rank, K, torch.cuda.synchronize, True)
     if e2e4 is not None:
         e2e4["per_rank_configs1"] = e2e
     launches4 = ctx.kernel_launches - launches0
@@ -562,6 +585,8 @@ def main_ours(args, rank, world, local, ncores):
             "roofline_note": "`roofline` is the dominant kernel in rank 0's configs[1] pass (per-kernel events); `roofline_whole_direction` is THIS job",
             "roofline_whole_direction": whole_direction(nb, clen4, c_ms, d_ms, world),
             "cpu_baseline": cpu_baseline_block(sample, ncores, C4_LEVEL, True, f"the first {sample.size >> 30} GiB of the workload")}
+    if dumped:
+        line["dump_outputs"] = {"dir": args.dump_outputs, "files": dumped}
     print(json.dumps(line), flush=True)
     dist.destroy_process_group()
     return 0
@@ -573,6 +598,8 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed to DIR/<name>.npy (sizes whole, archive and output as a seeded sample)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1")); local = int(os.environ.get("LOCAL_RANK", "0"))
     ncores = os.cpu_count() or 1

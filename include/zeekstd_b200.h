@@ -1,5 +1,5 @@
 /*
- * zeekstd_b200.h -- C ABI of the B200-native seekable-zstd codec.
+ * zeekstd_b200.h -- C ABI of the H100-native seekable-zstd codec.
  *
  * Drop-in boundary for the hot path of rorosen/zeekstd.  The reference crosses into native code
  * (libzstd via zstd-safe) at exactly these call sites, which this ABI replaces:

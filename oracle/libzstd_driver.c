@@ -4,7 +4,7 @@
  * The reference (rorosen/zeekstd) is Rust and cannot be built here (no cargo,
  * no network); all of its codec arithmetic is the third-party libzstd
  * (zstd-sys 2.0.16+zstd.1.5.7, Cargo.lock:1192-1198) which is absent from
- * /root/reference as source but present in the image as a shared object.
+ * the reference tree as source but present on the system as a shared object.
  * This driver dlopen()s that shared object and replays the reference's exact
  * libzstd call sequences:
  *

@@ -5,7 +5,7 @@
  * (RFC 8878) -- the arithmetic that rorosen/zeekstd reaches through
  *   lib/src/decode.rs:243-245   dctx.decompress_stream(...)
  * i.e. libzstd 1.5.7 (zstd-sys 2.0.16+zstd.1.5.7, Cargo.lock:1192-1198),
- * whose sources are NOT in /root/reference.  It is written from the format
+ * whose sources are NOT in the reference tree.  It is written from the format
  * rules restated in SURVEY.md Appendix A and pinned (tests/test_oracle.py)
  * against the real libzstd in the image (oracle/libzstd_driver.c) on the
  * reference's own fixture (assets/dickens.txt -> tests/golden/) and on

@@ -1,5 +1,5 @@
 """Backend-independent test bodies.  Every function takes a zeekstd_b200.Context bound to the library under test
-(the emulated CPU build for `-m "not gpu"`, the real sm_100a build for `-m gpu`) and checks it against the oracle
+(the emulated CPU build for `-m "not gpu"`, the real sm_90a build for `-m gpu`) and checks it against the oracle
 (libzstd through the reference's call sequence / the plain-C restatement).  The API tests are ports of the
 reference's own tests (lib/src/lib.rs:69-357, encode.rs:802-871, decode.rs:581-940, seek_table.rs:1061-1278)."""
 from __future__ import annotations

@@ -1,7 +1,7 @@
 """pytest configuration.
 
 Two builds of the SAME native sources are exercised:
-  * `-m gpu`      : zeekstd_b200/libzeekstd_b200.so (nvcc, sm_100a) on a real B200 -- the parity tests proper;
+  * `-m gpu`      : zeekstd_b200/libzeekstd_b200.so (nvcc, sm_90a) on a real H100 -- the parity tests proper;
   * `-m "not gpu"`: tests/emul/_build/libzeekstd_b200_emul.so, the device code interpreted on the CPU by
                     tests/emul/cuda_emul.h (test infrastructure only) -- host logic + kernel logic on tiny inputs.
 """
@@ -16,7 +16,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a real CUDA device (run on an H100)")
 
 
 def _has_gpu() -> bool:

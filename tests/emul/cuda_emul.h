@@ -1,8 +1,8 @@
 // tests/emul/cuda_emul.h -- TEST INFRASTRUCTURE ONLY.
 //
 // A tiny "CUDA on one CPU thread" execution model so that the *device* code of zeekstd_b200
-// (zeekstd_b200/csrc/*.cu) can be exercised bit-for-bit in this GPU-less container before it is
-// sent to a B200 with gpurun.  The kernels are compiled unmodified by g++ (-x c++ -DZK_EMUL
+// (zeekstd_b200/csrc/*.cu) can be exercised bit-for-bit on a machine without a GPU before it runs
+// on an H100.  The kernels are compiled unmodified by g++ (-x c++ -DZK_EMUL
 // -include cuda_emul.h); every CUDA thread of a CTA becomes a ucontext coroutine, CTAs run one
 // after another, and the warp/block collectives (__shfl_*_sync, __ballot_sync, __syncwarp,
 // __syncthreads) are rendez-vous points between those coroutines.  Scheduling order is
@@ -10,7 +10,7 @@
 //
 // This is NOT a product path: the emulated library is built into tests/emul/_build/ and is only
 // ever loaded explicitly by tests; the shipped zeekstd_b200/libzeekstd_b200.so contains nvcc-built
-// sm_100a code only and refuses to run without a GPU.
+// sm_90a code only and refuses to run without a GPU.
 #pragma once
 #ifndef ZK_EMUL
 #error "cuda_emul.h is only for the ZK_EMUL test build"

@@ -1,6 +1,6 @@
 """Generates the committed golden fixtures from the reference's own corpus (assets/dickens.txt) and the real
-libzstd of this image (oracle/libzstd_driver.c replaying the reference's call sequence).  Run HERE (the reference
-tree does not exist on the GPU box):   python tests/golden/make_golden.py
+libzstd of the system (oracle/libzstd_driver.c replaying the reference's call sequence), from the corpus as committed
+next to this script:   python tests/golden/make_golden.py
 """
 import hashlib, json, os, sys
 import numpy as np
@@ -9,7 +9,7 @@ sys.path.insert(0, ROOT)
 from oracle import oracle as O
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-d = np.fromfile("/root/reference/assets/dickens.txt", dtype=np.uint8)
+d = np.fromfile(os.path.join(HERE, "dickens.txt"), dtype=np.uint8)
 meta = {"libzstd": O.libzstd_version(), "dickens_bytes": int(d.size), "dickens_sha256": hashlib.sha256(d.tobytes()).hexdigest()}
 
 # known answers on the full corpus (BASELINE config 1): frame sizes per level / frame size

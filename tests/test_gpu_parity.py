@@ -1,4 +1,4 @@
-"""`-m gpu`: the parity tests proper, through the C ABI of the real sm_100a library on a B200.
+"""`-m gpu`: the parity tests proper, through the C ABI of the real sm_90a library on an H100.
 Same bodies as the emulated suite (tests/cases.py) at realistic sizes, the committed golden fixtures, and -- at
 BASELINE.json's full sizes -- size-independent properties (round trips, libzstd cross-decoding).
 The oracle is the image's libzstd (1.5.5; the reference pins 1.5.7 through zstd-sys -- same format, same decoder
@@ -27,7 +27,7 @@ def ctx(gpu_lib):
 
 
 def test_native_library_is_the_one_running(ctx, gpu_lib):
-    assert b"sm_100a" in gpu_lib.zk_version()
+    assert b"sm_90a" in gpu_lib.zk_version()
     before = ctx.kernel_launches
     cases.check_compress_roundtrip(ctx, corpus.make_class("text", 100_000, 1).numpy(), 50_000, 3, True)
     assert ctx.kernel_launches > before

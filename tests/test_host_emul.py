@@ -1,6 +1,6 @@
 """`-m "not gpu"` suite: the host layer and the kernel LOGIC, run on the emulated build of the same sources
 (tests/emul: device code interpreted on the CPU).  Inputs are tiny because every CUDA thread is a coroutine here; the
-same bodies (tests/cases.py) run at realistic sizes on the B200 in test_gpu_parity.py."""
+same bodies (tests/cases.py) run at realistic sizes on the H100 in test_gpu_parity.py."""
 import numpy as np
 import pytest
 

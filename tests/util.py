@@ -1,4 +1,4 @@
-"""Shared helpers for the parity tests (both the emulated CPU build and the real sm_100a build)."""
+"""Shared helpers for the parity tests (both the emulated CPU build and the real sm_90a build)."""
 from __future__ import annotations
 
 import json

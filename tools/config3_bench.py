@@ -1,7 +1,7 @@
 """GPU-box measurement of BASELINE configs[2]: 8 GiB of text (dickens.txt slices), 512 KiB frames (16 384 frames), archive
 written by libzstd through the reference's Encoder sequence (level 3, checksums on -- the reference's defaults,
-encode.rs:176-180), DECOMPRESS-ONLY on one B200, output compared bit for bit with the input and timed beside libzstd.
-usage: python tools/config3_bench.py [GiB=8] > profiles/config3_r2.json"""
+encode.rs:176-180), DECOMPRESS-ONLY on one H100, output compared bit for bit with the input and timed beside libzstd.
+usage: python tools/config3_bench.py [GiB=8] > config3.json"""
 import ctypes, json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

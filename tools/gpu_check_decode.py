@@ -1,4 +1,4 @@
-"""Ad-hoc GPU check (run under gpurun): parity + rough timing of the device-resident decode path."""
+"""Ad-hoc GPU check (run on a GPU machine): parity + rough timing of the device-resident decode path."""
 import ctypes, json, os, sys, time
 import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -49,5 +49,5 @@ if os.environ.get("ZK_CHECK_BIG"):
 txt = corpus.make_text(sz, device="cuda").cpu().numpy()
 out.append(run("text-2M-L1", txt, 2 << 20, 1, False))
 out.append(run("text-512K-L1", txt, 512 << 10, 1, False))
-os.makedirs("gpurun_out", exist_ok=True)
-json.dump(out, open("gpurun_out/check_decode.json", "w"), indent=1)
+os.makedirs("tools_out", exist_ok=True)
+json.dump(out, open("tools_out/check_decode.json", "w"), indent=1)

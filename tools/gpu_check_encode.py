@@ -1,4 +1,4 @@
-"""Ad-hoc GPU check (run under gpurun): compress on the GPU, verify with libzstd + our GPU decoder, rough timing."""
+"""Ad-hoc GPU check (run on a GPU machine): compress on the GPU, verify with libzstd + our GPU decoder, rough timing."""
 import ctypes, json, os, sys, time
 import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -52,5 +52,5 @@ out.append(run("mix-256M-2M-L1", corpus.make_mix(256 << 20, device="cuda"), 2 <<
 out.append(run("mix-256M-2M-L3ck", corpus.make_mix(256 << 20, device="cuda"), 2 << 20, 3, 1))
 if os.environ.get("ZK_CHECK_BIG"):
     out.append(run("mix-1G-2M-L1", corpus.make_mix(1 << 30, device="cuda"), 2 << 20, 1, 0, verify_cpu=True))
-os.makedirs("gpurun_out", exist_ok=True)
-json.dump(out, open("gpurun_out/check_encode.json", "w"), indent=1)
+os.makedirs("tools_out", exist_ok=True)
+json.dump(out, open("tools_out/check_encode.json", "w"), indent=1)

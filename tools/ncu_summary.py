@@ -1,5 +1,5 @@
-"""Write the profiles/ summary of an ncu report: per-kernel metrics + top stall lines per CUDA source line.
-   python tools/ncu_summary.py gpurun_out/ncu_<tag>.ncu-rep profiles/ncu_summary_<tag>.txt ["header line"]"""
+"""Write a text summary of an ncu report: per-kernel metrics + top stall lines per CUDA source line.
+   python tools/ncu_summary.py <report>.ncu-rep <summary>.txt ["header line"]"""
 import csv, io, subprocess, sys
 rep, dst = sys.argv[1], sys.argv[2]
 hdr = sys.argv[3] if len(sys.argv) > 3 else ""

@@ -1,4 +1,4 @@
-"""Profile target (run under ncu via gpurun): device-resident compress + decompress of the bench workload (1 GiB mix, 2 MiB frames)."""
+"""Profile target (run under a profiler on a GPU machine): device-resident compress + decompress of the bench workload (1 GiB mix, 2 MiB frames)."""
 import ctypes, os, sys, json
 import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,4 +1,4 @@
-"""Profile target (run under ncu via gpurun): one warm-up + N timed device-resident decodes of a text/mix batch."""
+"""Profile target (run under a profiler on a GPU machine): one warm-up + N timed device-resident decodes of a text/mix batch."""
 import ctypes, os, sys, json
 import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

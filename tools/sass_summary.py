@@ -1,5 +1,5 @@
-"""profiles/sass_summary.txt: per-kernel SASS instruction counts, registers and the opcodes that prove the TMA / mbarrier
-code paths (cuobjdump here, no GPU needed).  usage: python tools/sass_summary.py > profiles/sass_summary.txt"""
+"""Per-kernel SASS instruction counts, registers and the opcodes that prove the TMA / mbarrier
+code paths (cuobjdump here, no GPU needed).  usage: python tools/sass_summary.py > sass_summary.txt"""
 import collections, re, subprocess
 SO = "zeekstd_b200/libzeekstd_b200.so"
 sass = subprocess.run(["cuobjdump", "-sass", SO], capture_output=True, text=True).stdout
@@ -18,7 +18,7 @@ for l in sass.split("\n"):
     if m and kern:
         cnt[kern][m.group(1).split(".")[0]] += 1; cnt[kern]["_total"] += 1
 dem = lambda n: subprocess.run(["c++filt", n], capture_output=True, text=True).stdout.strip().split("(")[0]
-print("# SASS summary of zeekstd_b200/libzeekstd_b200.so (cuobjdump -sass, sm_100a), round 2 -- tools/sass_summary.py")
+print("# SASS summary of zeekstd_b200/libzeekstd_b200.so (cuobjdump -sass, sm_90a) -- tools/sass_summary.py")
 print("# UBLKCP = cp.async.bulk (TMA bulk copy global -> shared; K-D1s stages sequence bitstreams with it), SYNCS = mbarrier operations")
 print("# (arrive / expect_tx / try_wait: the tile barriers of K-D1s and the event waits of zk_exec2_kernel), REDUX = redux.sync, MATCH = match.any")
 print("kernel | SASS instructions | registers | static smem | UBLKCP | SYNCS | REDUX | MATCH | LDS | STS | LDG | STG | ATOM/RED | BAR")

@@ -49,4 +49,4 @@ res = dict(archive_bytes=len(a), frames=st.num_frames(), reads=len(offs), read_b
                         note="every touched frame is decoded once and only as far as the last byte some read wants of it"),
            reference_cpu_single_read_ms=dict(p50=round(float(np.percentile(tl, 50)), 3), p99=round(float(np.percentile(tl, 99)), 3), note="libzstd 1 thread, whole frame(s) decoded"))
 print(json.dumps(res), flush=True)
-os.makedirs("gpurun_out", exist_ok=True); json.dump(res, open("gpurun_out/seek_r2.json", "w"), indent=1)
+os.makedirs("tools_out", exist_ok=True); json.dump(res, open("tools_out/seek.json", "w"), indent=1)

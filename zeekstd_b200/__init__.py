@@ -1,4 +1,4 @@
-"""zeekstd_b200 -- B200-native seekable-Zstandard codec behind rorosen/zeekstd's API surface.
+"""zeekstd_b200 -- H100-native seekable-Zstandard codec behind rorosen/zeekstd's API surface.
 
 Python mirror of the reference's public items (lib/src/lib.rs:38-58) over the C ABI in
 include/zeekstd_b200.h; every codec byte is produced by the CUDA kernels in csrc/.

@@ -1,6 +1,6 @@
 """ctypes binding of the C ABI declared in include/zeekstd_b200.h.
 
-The product library is zeekstd_b200/libzeekstd_b200.so (nvcc, sm_100a).  There is NO fallback:
+The product library is zeekstd_b200/libzeekstd_b200.so (nvcc, sm_90a).  There is NO fallback:
 if it is missing, or no CUDA device is usable, loading / context creation raises.
 Tests may load another build of the SAME sources explicitly by path (tests/emul: device code
 interpreted on the CPU) through `load(path)`; nothing in this package ever does so on its own.
@@ -151,7 +151,7 @@ def load(path: str | None = None, require_all: bool = True) -> ctypes.CDLL:
         return _libs[path]
     if not os.path.exists(path):
         raise ImportError(
-            f"{path} not found: build it with `python -m zeekstd_b200.build` (nvcc, sm_100a). "
+            f"{path} not found: build it with `python -m zeekstd_b200.build` (nvcc, sm_90a). "
             "zeekstd_b200 has no CPU fallback.")
     lib = ctypes.CDLL(path)
     for name, (res, args) in _SIGS.items():

@@ -1,6 +1,6 @@
 """Build the zeekstd_b200 native library IN-TREE.
 
-  python -m zeekstd_b200.build            -> zeekstd_b200/libzeekstd_b200.so   (nvcc, sm_100a; the product)
+  python -m zeekstd_b200.build            -> zeekstd_b200/libzeekstd_b200.so   (nvcc, sm_90a; the product)
   python -m zeekstd_b200.build --emul     -> tests/emul/_build/libzeekstd_b200_emul.so  (g++, TEST ONLY:
                                              device code interpreted by tests/emul/cuda_emul.h)
 """
@@ -18,7 +18,7 @@ PRODUCT_SO = os.path.join(HERE, "libzeekstd_b200.so")
 EMUL_DIR = os.path.join(ROOT, "tests", "emul", "_build")
 EMUL_SO = os.path.join(EMUL_DIR, "libzeekstd_b200_emul.so")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -53,7 +53,7 @@ def build_product(force: bool = False, verbose: bool = False) -> str:
             sys.stderr.write(out)
         if p.returncode:
             raise RuntimeError(f"nvcc failed on {src}")
-    cmd = [nvcc, "-shared", "-o", PRODUCT_SO] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+    cmd = [nvcc, "-shared", "-o", PRODUCT_SO] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
     subprocess.run(cmd, check=True)
     return PRODUCT_SO
 

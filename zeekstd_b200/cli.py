@@ -124,7 +124,7 @@ def _level(s: str) -> int:
 
 
 def build_parser() -> argparse.ArgumentParser:
-    ap = argparse.ArgumentParser(prog="zeekstd_b200", description="Compress and decompress data using the Zstandard Seekable Format (B200 codec).")
+    ap = argparse.ArgumentParser(prog="zeekstd_b200", description="Compress and decompress data using the Zstandard Seekable Format (H100 codec).")
     _add_flags(ap, True)
     sub = ap.add_subparsers(dest="command")
 

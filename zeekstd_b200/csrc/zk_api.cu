@@ -26,7 +26,7 @@ static size_t zk_env_size(const char* name, size_t dflt) {
     return (size_t)strtoull(s, nullptr, 10);
 }
 
-// sub-batches in flight of the host-pointer pipelines (measured on B200, tools/e2e_sweep4.sh): decompress wants many
+// sub-batches in flight of the host-pointer pipelines (tuning knobs, swept by tools/e2e_sweep4.sh): decompress wants many
 // (its exec stage is latency-bound per frame), compress few (its kernels fill the machine from one 128 MiB sub-batch)
 static int zk_host_slots(bool enc) {
     size_t v = zk_env_size(enc ? "ZK_HOST_SLOTS_ENC" : "ZK_HOST_SLOTS", enc ? 4 : 8);
@@ -37,7 +37,7 @@ extern "C" const char* zk_version(void) {
 #ifdef ZK_EMUL
     return "zeekstd_b200 0.1 (ZK_EMUL test build: device code interpreted on the CPU; not a product build)";
 #else
-    return "zeekstd_b200 0.1 (sm_100a)";
+    return "zeekstd_b200 0.1 (sm_90a)";
 #endif
 }
 
@@ -99,7 +99,7 @@ extern "C" int32_t zk_ctx_create(int32_t device_ordinal, uint32_t flags, zk_ctx*
     ZK_RT_OK(cudaGetDeviceProperties(&prop, device_ordinal));
     zk_ctx* c = new zk_ctx();
     c->device = device_ordinal;
-    c->sm_count = prop.multiProcessorCount > 0 ? prop.multiProcessorCount : 148;
+    c->sm_count = prop.multiProcessorCount > 0 ? prop.multiProcessorCount : 132;
     // ZK_HOST_PRIO (default 1): slot i runs at stream priority (greatest + i): concurrent sub-batches of the host pipelines then
     // complete staggered (oldest slot first) instead of all at once, which keeps the D2H engine busy from early on
     int least = 0, greatest = 0;
@@ -282,7 +282,7 @@ extern "C" int32_t zk_decompress_frames_upto(zk_ctx* c, const uint8_t* comp, con
     if (!c || (n && (!comp || !c_off || !d_off || !dst))) return ZK_ERR_INVALID_ARG;
     if (n == 0) return 0;
     ZK_RT_OK(cudaSetDevice(c->device));
-    const size_t sub_bytes = zk_env_size("ZK_HOST_SUB_BYTES", (size_t)128 << 20);     // measured best on B200 (tools/e2e_sweep2.sh)
+    const size_t sub_bytes = zk_env_size("ZK_HOST_SUB_BYTES", (size_t)128 << 20);     // tuning knob (tools/e2e_sweep2.sh sweeps it)
     ZkSubDec sub[ZK_SLOTS];
     const int NS = zk_host_slots(false);
     const uint32_t ramp = (uint32_t)zk_env_size("ZK_HOST_RAMP", 0);            // the first `ramp` sub-batches are 1/2^ramp ... 1/2 of the full size
@@ -294,7 +294,7 @@ extern "C" int32_t zk_decompress_frames_upto(zk_ctx* c, const uint8_t* comp, con
         int rc = zk_dec_sub_finish(c, si, sub[si], comp, c_off, d_off, dst, verify, status, d_need);
         if (rc && !worst) worst = rc;
         // ZK_HOST_RAMP=r (default 0): the first r sub-batches are 1/2^r ... 1/2 of the full size, so that the output copy could start
-        // earlier.  Measured on B200 (profiles/README.md): no gain -- a sub-batch of any size spends about one frame latency in
+        // earlier.  It gave no gain when it was tried: a sub-batch of any size spends about one frame latency in
         // K-D2, so a small first sub-batch is not done much sooner than a full one
         const size_t this_sub = k < ramp ? sub_bytes >> (ramp - k) : sub_bytes;
         uint32_t end = zk_next_sub(d_off, first, n, this_sub, 1u << 20);
@@ -367,7 +367,7 @@ extern "C" int32_t zk_compress_frames(zk_ctx* c, const uint8_t* src, size_t n, u
     const uint32_t nf = zk_frames_of(n, frame_size);
     if (nf > frames_cap) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
     ZK_RT_OK(cudaSetDevice(c->device));
-    const size_t sub_bytes = zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20);    // measured best on B200 (tools/knobs_round.sh)
+    const size_t sub_bytes = zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20);    // tuning knob (tools/knobs_round.sh sweeps it)
     uint32_t per = (uint32_t)(sub_bytes / frame_size); if (per == 0) per = 1;
     // The compressed size of a sub-batch is only known when it completes, so output positions are assigned in
     // order at completion time: H2D and kernels of later sub-batches overlap the D2H of earlier ones.

@@ -2,7 +2,7 @@
 //
 // The codec arithmetic that the reference reaches through zstd-safe -> libzstd
 // (lib/src/encode.rs:341-345,444-448; lib/src/decode.rs:243-245) is implemented here from the
-// Zstandard format (RFC 8878; restated in SURVEY.md Appendix A) as CUDA for sm_100a.
+// Zstandard format (RFC 8878; restated in SURVEY.md Appendix A) as CUDA for sm_90a.
 #pragma once
 
 #ifdef ZK_EMUL
@@ -267,7 +267,7 @@ __device__ inline uint32_t zk_fse_read_ncount(const uint8_t* p, uint32_t n, int 
 // -------------------------------------------------------------------------------------------
 // Event = an mbarrier with an arrival count of one: every arrive completes a phase, so "something changed" wakes
 // whoever sleeps in try_wait on it (hardware sleep: a waiting warp issues nothing, and wakes ~60 cycles after the
-// arrive -- B300_MICROARCH.md, mbarrier).  A waiter re-checks its own condition after every wake-up; it first learns the
+// arrive -- PTX ISA, mbarrier).  A waiter re-checks its own condition after every wake-up; it first learns the
 // parity of the running phase (test_wait), THEN checks the condition, then sleeps on that parity, so a change between the
 // check and the sleep ends the sleep at once.  Two changes in that window would be missed; the time hint bounds that.
 // -------------------------------------------------------------------------------------------

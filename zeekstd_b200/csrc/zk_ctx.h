@@ -16,7 +16,7 @@ struct ZkSlot {
 
 struct zk_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     ZkSlot slot[ZK_SLOTS];
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaStream_t up = nullptr, down = nullptr;            // dedicated copy streams of the host-pointer decompress pipeline

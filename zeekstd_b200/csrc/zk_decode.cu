@@ -1,4 +1,4 @@
-// zk_decode.cu -- batched Zstandard frame decode for sm_100a.
+// zk_decode.cu -- batched Zstandard frame decode for sm_90a.
 //
 // Replaces the reference's only decompression call into libzstd,
 //   lib/src/decode.rs:243-245   self.dctx.decompress_stream(&mut out_buffer, &mut in_buffer)
@@ -1543,7 +1543,7 @@ __device__ __forceinline__ void zk_exec_body(ZkD2Smem& sm, const ZkDecodeArgs& a
 // =============================================================================================
 // K-D2 (second generation): the same job with in-order bookkeeping only.
 //
-// Profiling the dataflow kernel above (profiles/ncu_summary_bench_r1.txt) showed about 3 500 warp instructions per
+// Profiling the dataflow kernel above showed about 3 500 warp instructions per
 // 32-sequence chunk at 15 warps per SM: it was bound by instruction issue, not by the dependency chain of a frame (a
 // frame whose every chunk waits for its predecessor would still finish in ~2 ms at ~1 000 cycles per chunk).  This
 // version keeps the shared-memory ring, the 32-sequence chunks dealt round-robin to the W warps of the CTA and the ring
@@ -2059,7 +2059,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     if (need_blocks < ws->want_blocks) need_blocks = ws->want_blocks;
     if (need_lit < ws->want_lit) need_lit = ws->want_lit;
     if (need_seq < ws->want_seq) need_seq = ws->want_seq;
-    int sms = ws->sm_count > 0 ? ws->sm_count : 148;
+    int sms = ws->sm_count > 0 ? ws->sm_count : 132;
     int rc = zk_decode_ensure(ws, n, need_blocks, need_lit, need_seq);
     if (rc) return rc;
     memcpy(ws->h_off, c_off, (size_t)(n + 1) * 8);
@@ -2156,7 +2156,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
         // second-generation kernel: <= 64 registers, so 32 warps per SM whatever the split; ring = what is left of the
         // SM's shared memory per resident entry
         if (per_sm > 8) per_sm = 8;
-        if (W <= 0) W = 16 / per_sm;        // measured (profiles/README.md): more warps per frame than this make the in-order chain SLOWER
+        if (W <= 0) W = 16 / per_sm;        // more warps per frame than this made the in-order chain SLOWER when this kernel was tuned
         if (W > 32) W = 32;
         if (W < 2) W = 2;
         uint32_t ring = 128 * 1024;
