@@ -67,6 +67,8 @@ int32_t zk_ctx_create(int32_t device_ordinal, uint32_t flags, zk_ctx** out);
 void zk_ctx_destroy(zk_ctx* ctx);
 /* number of CUDA kernels this context has launched so far (bench.py reports it as gpu_launches) */
 uint64_t zk_ctx_kernel_launches(const zk_ctx* ctx);
+/* number of execution segments (independent runs of blocks of a seek-table entry) the decoder has run so far */
+uint64_t zk_ctx_decode_segments(const zk_ctx* ctx);
 /* kernel-only device time (ms, CUDA events on the context's stream) of the most recent batch call */
 float zk_ctx_last_device_ms(const zk_ctx* ctx);
 const char* zk_version(void);

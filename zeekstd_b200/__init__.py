@@ -119,6 +119,11 @@ class Context:
     def kernel_launches(self) -> int: return int(self.lib.zk_ctx_kernel_launches(self._h))
 
     @property
+    def decode_segments(self) -> int:
+        """execution segments the decoder has run so far: independent runs of blocks, several per entry where the data allows"""
+        return int(self.lib.zk_ctx_decode_segments(self._h))
+
+    @property
     def last_device_ms(self) -> float: return float(self.lib.zk_ctx_last_device_ms(self._h))
 
     # ---- batch codec (the hot path) ------------------------------------------------------------

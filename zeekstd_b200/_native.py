@@ -46,6 +46,7 @@ _SIGS = {
     "zk_ctx_create": (c_int32, [c_int32, c_uint32, POINTER(c_void_p)]),
     "zk_ctx_destroy": (None, [c_void_p]),
     "zk_ctx_kernel_launches": (c_uint64, [c_void_p]),
+    "zk_ctx_decode_segments": (c_uint64, [c_void_p]),
     "zk_ctx_last_device_ms": (c_float, [c_void_p]),
     "zk_compress_bound": (c_size_t, [c_size_t, c_uint32]),
     "zk_ctx_profile": (None, [c_void_p, c_int32]),

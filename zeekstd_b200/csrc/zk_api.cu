@@ -146,6 +146,11 @@ extern "C" void zk_ctx_destroy(zk_ctx* c) {
 }
 
 extern "C" uint64_t zk_ctx_kernel_launches(const zk_ctx* c) { return c ? c->launches() : 0; }
+extern "C" uint64_t zk_ctx_decode_segments(const zk_ctx* c) {
+    unsigned long long n = 0;
+    for (int i = 0; c && i < ZK_SLOTS; i++) n += c->slot[i].dws.segments;
+    return n;
+}
 extern "C" float zk_ctx_last_device_ms(const zk_ctx* c) { return c ? c->last_ms : 0.f; }
 extern "C" size_t zk_compress_bound(size_t n, uint32_t frame_size) { return zk_encode_bound(n, frame_size); }
 

@@ -100,11 +100,16 @@ struct ZkBlock {                 // one zstd block of one seek-table entry
     uint32_t hash_start;         // last block: start (rel. to entry output) and length of the zstd frame's content
     uint32_t hash_len;
     uint32_t bmax;               // Block_Maximum_Size of the block's zstd frame: min(Window_Size, 128 KiB)   [scan kernel]
+    uint32_t back;               // how far before its first byte the block's matches read (0: not at all; ZK_BACK_UNKNOWN) [scan / seq kernel]
+    uint32_t out_pos;            // output position, relative to the entry's output          [plan kernel]
+    uint32_t frame_start;        // output position of the first byte of the block's zstd frame [plan kernel]
 };
 #define ZKB_FIRST 1u             // first block of a zstd frame: resets repeat offsets / entropy tables
 #define ZKB_LAST 2u              // Last_Block
 #define ZKB_HAS_CSUM 4u          // 4-byte content checksum follows the last block
 #define ZKB_HAS_FCS 8u
+#define ZKB_SEG 16u              // first block of an execution segment   [plan kernel]
+#define ZK_BACK_UNKNOWN 0xFFFFFFFFu   // a symbolic offset, or sequences that were not (successfully) decoded by the second-generation FSE kernel
 
 // symbolic repeat offset: "incoming repeat slot s (0..2) minus delta" (delta in 0..2^20)
 #define ZK_SYM 0x80000000u
@@ -116,15 +121,25 @@ struct ZkEntry {                 // one seek-table entry (one "frame" of the see
     uint32_t first_block;
     uint32_t n_blocks;
     int32_t status;              // 0, -(zstd code), or ZK_ST_RETRY
-    uint32_t produced;           // bytes written (exec kernel)
+    uint32_t produced;           // bytes written (plan / exec kernel)
+    uint32_t run_blocks;         // the exec kernel runs blocks [0, run_blocks): the serial walk stops there (wanted prefix reached, or a failure)  [plan]
+    uint32_t segs_left;          // segments of the entry not finished yet; whoever finishes the last one writes status  [plan / exec]
+    unsigned long long fail;     // smallest ZK_FAIL_KEY of the failures met (the one the serial walk meets first), ~0 = none  [plan / exec]
 };
 #define ZK_ST_RETRY 0x7FFFFFFF   // scratch capacity exceeded: host grows the workspace and re-runs
+// failure order of the serial walk: by block, then by what it checks first at that block
+#define ZK_FAIL_STATUS 0u        // entropy stage status of the block
+#define ZK_FAIL_DST 1u           // the block does not fit the entry's output
+#define ZK_FAIL_EXEC 2u          // a bad offset while its sequences execute
+#define ZK_FAIL_FCS 3u           // Frame_Content_Size mismatch after the frame's last block
+#define ZK_FAIL_KEY(block, stage, code) (((unsigned long long)(block) << 32) | ((unsigned long long)(stage) << 16) | (unsigned long long)(code))
 
 struct ZkCounters {
     unsigned long long n_blocks, n_lit, n_seq;   // exact needs (accumulated even when over capacity)
     uint32_t overflow;
     uint32_t n_errors;
     uint32_t n_huf_blocks, n_seq_blocks;         // lengths of huf_list / seq_list
+    uint32_t n_segments;                         // length of seg_list: execution segments of the batch (plan kernel)
 };
 
 // -------------------------------------------------------------------------------------------

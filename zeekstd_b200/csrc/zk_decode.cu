@@ -8,7 +8,8 @@
 //   K-D0 zk_scan_kernel     one thread / entry : walk frame + block headers, carve scratch
 //   K-D1s zk_seq_kernel     one LANE  / block  : FSE sequence decode (4-byte cells + state machine in smem)
 //   K-D1h zk_huf_kernel     one LANE  / stream : Huffman literal decode (4 lanes per 4-stream block, two-level table)
-//   K-D2 zk_exec_kernel[_w5] one CTA  / entry  : ordered sequence execution through a shared-memory window
+//   K-D1p zk_plan_kernel    one warp / entry   : output positions, the serial walk's checks, execution segments
+//   K-D2 zk_exec_kernel[_w5] one CTA  / segment : ordered sequence execution through a shared-memory window
 //   K-D3 zk_xxh64_kernel    one warp  / entry  : content checksum (only if requested & present)
 //
 // Format rules: RFC 8878 as restated in SURVEY.md Appendix A (the arithmetic is not in the
@@ -186,6 +187,8 @@ struct ZkFillEmit {
         b.lit_src = 0; b.regen = bi.type == 2 ? 0 : bi.size; b.status = 0; b.lit_status = 0;
         b.rep_out[0] = ZK_SYM_MAKE(0, 0); b.rep_out[1] = ZK_SYM_MAKE(1, 0); b.rep_out[2] = ZK_SYM_MAKE(2, 0);
         b.fcs = bi.fcs; b.hash_start = 0; b.hash_len = 0; b.bmax = bi.bmax;
+        b.back = bi.type == 2 && bi.nseq ? ZK_BACK_UNKNOWN : 0u;   // blocks without sequences read no earlier output
+        b.out_pos = 0; b.frame_start = 0;
         if (bi.flags & ZKB_FIRST) { huf_ref = ll_ref = of_ref = ml_ref = -1; }
         b.huf_ref = -1; b.ll_ref = -1; b.of_ref = -1; b.ml_ref = -1;
         if (bi.type == 2) {
@@ -212,7 +215,7 @@ struct ZkFillEmit {
 __global__ void __launch_bounds__(128) zk_scan_kernel(ZkDecodeArgs a) {
     uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= a.n_entries) return;
-    ZkEntry ent; ent.first_block = 0; ent.n_blocks = 0; ent.status = 0; ent.produced = 0;
+    ZkEntry ent; ent.first_block = 0; ent.n_blocks = 0; ent.status = 0; ent.produced = 0; ent.run_blocks = 0; ent.segs_left = 0; ent.fail = ~0ull;
     unsigned long long c0 = a.c_off[e], c1 = a.c_off[e + 1];
     if (c1 < c0 || c1 - c0 > 0xFFFFFFFFull) { ent.status = -ZKZ_SRC_SIZE_WRONG; a.entries[e] = ent; return; }
     const uint8_t* p = a.comp + c0; uint32_t n = (uint32_t)(c1 - c0);
@@ -464,6 +467,7 @@ struct ZkSeq2Chain {
     uint16_t nxt2[2][64];                  // build scratch of the OF / ML tables (LL uses t.nxt): the three tables are built side by side
     alignas(8) unsigned long long bar[4];  // one mbarrier per tile slot
     uint32_t lit_end, out_end, r0, r1, r2; // carries of the helper phase
+    uint32_t back;                         // ... and the block's ZkBlock::back so far
     int st;
 };
 
@@ -506,7 +510,7 @@ __global__ void __launch_bounds__(32) zk_seq2_kernel(ZkDecodeArgs a) {
         int next_issue = -1, next_wait = -1, top_tile = 0; uint32_t stream_end_off = 0, use0 = 0;
         bool live = false, parsed = false;
         if (chain_lane) {
-            ch.st = 0; ch.lit_end = 0; ch.out_end = 0; ch.r0 = ZK_SYM_MAKE(0, 0); ch.r1 = ZK_SYM_MAKE(1, 0); ch.r2 = ZK_SYM_MAKE(2, 0);
+            ch.st = 0; ch.lit_end = 0; ch.out_end = 0; ch.back = 0; ch.r0 = ZK_SYM_MAKE(0, 0); ch.r1 = ZK_SYM_MAKE(1, 0); ch.r2 = ZK_SYM_MAKE(2, 0);
             const uint32_t my = first + (uint32_t)myc;
             if (my < n) {
                 bidx = a.seq_list[my];
@@ -665,13 +669,17 @@ __global__ void __launch_bounds__(32) zk_seq2_kernel(ZkDecodeArgs a) {
                     if (lane == j) off = o;
                     lastpos = j + 1; m &= m - 1;
                 }
+                uint32_t back = 0;                                                       // how far before the block's first byte this match reads
                 if (act) {
                     const uint32_t at = sbase + sdone + (uint32_t)lane;
                     a.seq_lit_end[at] = le; a.seq_out_end[at] = oe; a.seq_off[at] = off;
+                    const uint32_t md = oe - mlv;                                        // block-relative match destination
+                    back = (off & ZK_SYM) ? ZK_BACK_UNKNOWN : (off > md ? min(off - md, ZK_BACK_UNKNOWN - 1u) : 0u);
                 }
+                back = __reduce_max_sync(0xFFFFFFFFu, back);
                 const bool anybad = __any_sync(0xFFFFFFFFu, badv) || badr;
                 if (lane == (int)ncc - 1) { hc.lit_end = le; hc.out_end = oe; }
-                if (lane == 0) { hc.r0 = r0; hc.r1 = r1; hc.r2 = r2; if (anybad && hc.st == 0) hc.st = ZKZ_CORRUPTION; }
+                if (lane == 0) { hc.r0 = r0; hc.r1 = r1; hc.r2 = r2; hc.back = max(hc.back, back); if (anybad && hc.st == 0) hc.st = ZKZ_CORRUPTION; }
             }
             __syncwarp();
             if (chain_lane) { done += cnt; if (ch.st != 0) remaining = 0; }
@@ -688,6 +696,7 @@ __global__ void __launch_bounds__(32) zk_seq2_kernel(ZkDecodeArgs a) {
             a.blocks[bidx].rep_out[0] = ch.r0; a.blocks[bidx].rep_out[1] = ch.r1; a.blocks[bidx].rep_out[2] = ch.r2;
             a.blocks[bidx].regen = ch.out_end + (lit_size - ch.lit_end);
             a.blocks[bidx].status = st ? -st : 0;
+            a.blocks[bidx].back = st ? ZK_BACK_UNKNOWN : ch.back;
         }
         __syncwarp();
     }
@@ -903,6 +912,133 @@ __global__ void __launch_bounds__(32) zk_huf_kernel(ZkDecodeArgs a) {
 }
 
 // =============================================================================================
+// K-D1p: execution plan -- one warp per entry.
+//
+// The serial walk over an entry's blocks is cut into SEGMENTS: runs of consecutive blocks that read nothing written
+// before their first block.  Segments are independent, so K-D2 runs them on different CTAs, and no CTA ever waits for
+// another.  Block b starts a segment iff it is the entry's first block, or
+//   * no match of b or of any later block (up to where the walk stops) reads before b's first byte -- which also rules
+//     out symbolic offsets from b on (ZkBlock::back is unknown for those), and
+//   * b starts a zstd frame, or its outgoing repeat offsets are concrete,
+// so every repeat offset inside a segment resolves from state created inside it.  The checks the serial walk made as it
+// went (a failed entropy stage, output overflow, Frame_Content_Size, the final size, the wanted prefix of a range read)
+// are made here: they only need the regenerated sizes.  The walk stops at the first of them; the failure is kept as a key
+// ordered like the serial walk (block, then check), and K-D2 adds the bad offsets it meets by atomicMin.
+// =============================================================================================
+__device__ void zk_entry_finish(const ZkDecodeArgs& a, uint32_t e) {
+    ZkEntry& en = a.entries[e];
+    const unsigned long long f = *(volatile unsigned long long*)&en.fail;
+    if (f == ~0ull) { en.status = 0; return; }
+    const uint32_t bi = (uint32_t)(f >> 32), stage = (uint32_t)(f >> 16) & 0xFFu;
+    en.status = -(int32_t)(f & 0xFFFFu);
+    if (bi < en.n_blocks) {             // the walk stopped before the failing block, or after it for a frame size mismatch
+        const ZkBlock& b = a.blocks[en.first_block + bi];
+        en.produced = b.out_pos + (stage == ZK_FAIL_FCS ? b.regen : 0u);
+    }
+    atomicAdd(&a.counters->n_errors, 1u);
+}
+
+__global__ void __launch_bounds__(128) zk_plan_kernel(ZkDecodeArgs a) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (e >= a.n_entries || a.counters->overflow) return;
+    const ZkEntry ent = a.entries[e];
+    if (ent.status != 0) return;
+    ZkBlock* blocks = a.blocks + ent.first_block;
+    const unsigned long long cap64 = a.d_off[e + 1] - a.d_off[e];
+    const unsigned long long cap = cap64 > 0xFFFFFFFFull ? 0xFFFFFFFFull : cap64;
+    const unsigned long long need = a.d_need ? a.d_need[e] : 0xFFFFFFFFull;
+    // ---- forward: output positions, frame starts, where the walk stops
+    unsigned long long pos = 0, zs = 0, fail = ~0ull;
+    uint32_t run = ent.n_blocks;
+    bool stopped = false;
+    for (uint32_t t = 0; t < ent.n_blocks; t += 32) {
+        const uint32_t bi = t + (uint32_t)lane;
+        const bool in = bi < ent.n_blocks;
+        uint32_t regen = 0, flags = 0; int32_t st = 0; unsigned long long fcs = 0;
+        if (in) { const ZkBlock& b = blocks[bi]; regen = b.regen; flags = b.flags; st = b.status ? b.status : b.lit_status; fcs = b.fcs; }
+        unsigned long long end = regen, fs = in && (flags & ZKB_FIRST) ? 1ull + bi : 0ull;   // fs: 1 + index of the frame's first block
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const unsigned long long x = __shfl_up_sync(0xFFFFFFFFu, end, d), y = __shfl_up_sync(0xFFFFFFFFu, fs, d);
+            if (lane >= d) { end += x; fs = fs > y ? fs : y; }
+        }
+        end += pos;
+        const unsigned long long p = end - regen;
+        // the frame start is the position of that first block: p of its lane, or the carry from an earlier tile
+        const unsigned long long fsp = __shfl_sync(0xFFFFFFFFu, p, fs > t ? (int)(fs - 1 - t) : 0);
+        const unsigned long long z = fs > t ? fsp : zs;
+        uint32_t stage = 0, code = 0;
+        bool ev = false;
+        if (in) {
+            if (p >= need) ev = true;                                                    // the wanted prefix is complete
+            else if (st) { ev = true; stage = ZK_FAIL_STATUS; code = (uint32_t)-st; }
+            else if (end > cap) { ev = true; stage = ZK_FAIL_DST; code = ZKZ_DST_TOO_SMALL; }
+            else if ((flags & ZKB_LAST) && (flags & ZKB_HAS_FCS) && fcs != end - z) { ev = true; stage = ZK_FAIL_FCS; code = ZKZ_CORRUPTION; }
+        }
+        const uint32_t evm = __ballot_sync(0xFFFFFFFFu, ev);
+        const int first = evm ? __ffs((int)evm) - 1 : 32;
+        if (in && lane <= first) {
+            ZkBlock& b = blocks[bi];
+            b.out_pos = (uint32_t)p; b.frame_start = (uint32_t)z;
+            if ((flags & ZKB_LAST) && !ev) { b.hash_start = (uint32_t)z; b.hash_len = (uint32_t)(end - z); }
+        }
+        if (evm) {
+            if (lane == first) {
+                if (code) fail = ZK_FAIL_KEY(bi, stage, code);
+                else stopped = true;
+                run = stage == ZK_FAIL_FCS ? bi + 1 : bi;
+                pos = p;
+            }
+            fail = __shfl_sync(0xFFFFFFFFu, fail, first); stopped = __shfl_sync(0xFFFFFFFFu, (uint32_t)stopped, first) != 0;
+            run = __shfl_sync(0xFFFFFFFFu, run, first); pos = __shfl_sync(0xFFFFFFFFu, pos, first);
+            break;
+        }
+        pos = __shfl_sync(0xFFFFFFFFu, end, 31); zs = __shfl_sync(0xFFFFFFFFu, z, 31);
+    }
+    if (fail == ~0ull && !stopped && pos != cap64)                                      // tagged after the last block
+        fail = ZK_FAIL_KEY(ent.n_blocks, ZK_FAIL_STATUS, pos < cap64 ? ZKZ_SRC_SIZE_WRONG : ZKZ_DST_TOO_SMALL);
+    // ---- backward over the blocks that run: suffix minimum of the lowest position read, segment starts
+    long long low = 0x7FFFFFFFFFFFFFFFll;                                                // lowest position read by the blocks after this tile
+    uint32_t nseg = 0;
+    for (uint32_t t = run ? (run - 1) & ~31u : 0; run; t -= 32) {
+        const uint32_t bi = t + (uint32_t)lane;
+        const bool in = bi < run;
+        long long lo = 0x7FFFFFFFFFFFFFFFll;
+        uint32_t flags = 0, op = 0; bool conc = false;
+        if (in) {
+            const ZkBlock& b = blocks[bi];
+            flags = b.flags; op = b.out_pos;
+            lo = b.back == ZK_BACK_UNKNOWN ? -0x7FFFFFFFFFFFFFFFll : (long long)op - (long long)b.back;
+            conc = !((b.rep_out[0] | b.rep_out[1] | b.rep_out[2]) & ZK_SYM);
+        }
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const long long x = __shfl_down_sync(0xFFFFFFFFu, lo, d);
+            if (lane + d < 32 && x < lo) lo = x;
+        }
+        if (low < lo) lo = low;
+        const bool start = in && (bi == 0 || (lo >= (long long)op && ((flags & ZKB_FIRST) || conc)));
+        if (in) blocks[bi].flags = (uint8_t)(start ? flags | ZKB_SEG : flags & ~ZKB_SEG);
+        const uint32_t m = __ballot_sync(0xFFFFFFFFu, start);
+        if (m) {
+            uint32_t base = 0;
+            if (lane == 0) base = atomicAdd(&a.counters->n_segments, (uint32_t)__popc(m));
+            base = __shfl_sync(0xFFFFFFFFu, base, 0);
+            if (start) a.seg_list[base + __popc(m & ((1u << lane) - 1u))] = ent.first_block + bi;
+            nseg += __popc(m);
+        }
+        low = __shfl_sync(0xFFFFFFFFu, lo, 0);
+        if (t == 0) break;
+    }
+    if (lane == 0) {
+        ZkEntry& en = a.entries[e];
+        en.run_blocks = run; en.produced = (uint32_t)pos; en.fail = fail; en.segs_left = nseg;
+        if (nseg == 0) zk_entry_finish(a, e);
+    }
+}
+
+// =============================================================================================
 // K-D2: ordered sequence execution with a shared-memory window.
 //
 // One CTA per seek-table entry, W warps.  The entry's sequences are cut into chunks of 32 (one per
@@ -926,6 +1062,8 @@ struct ZkD2Smem {
     uint32_t done_pos, done_chunk;         // every byte below done_pos is final (readable from the ring); chunks [0, done_chunk) are done
     uint32_t flushed_pos, flushed_chunk;   // ... and below flushed_pos it is in HBM too
     int abort_code;
+    uint32_t abort_block;                  // the earliest block (entry-relative) at which a warp aborted
+    uint32_t seg;                          // the segment this CTA runs now (index into seg_list)
     // per-chunk descriptors, slot = chunk & (ZK_D2_META-1); a field is valid for chunk k iff its tag == k + 1
     uint32_t started[ZK_D2_META], start[ZK_D2_META], end[ZK_D2_META], done[ZK_D2_META], flushed[ZK_D2_META];
     // per-SEQUENCE completion inside a chunk (the dependency chain of a frame runs sequence to sequence, not chunk to chunk):
@@ -935,7 +1073,7 @@ struct ZkD2Smem {
 };
 #define ZK_VOL(x) (*(volatile uint32_t*)&(x))
 
-__device__ __forceinline__ void zk_d2_abort(ZkD2Smem& sm, int code) { atomicCAS(&sm.abort_code, 0, code); }
+__device__ __forceinline__ void zk_d2_abort(ZkD2Smem& sm, int code, uint32_t block) { atomicCAS(&sm.abort_code, 0, code); atomicMin(&sm.abort_block, block); }
 // warp-uniform view of the abort flag (every lane must take the same branch around collectives)
 __device__ __forceinline__ bool zk_d2_aborted(ZkD2Smem& sm) { return __any_sync(0xFFFFFFFFu, *(volatile int*)&sm.abort_code != 0); }
 
@@ -1206,39 +1344,36 @@ __device__ __forceinline__ bool zk_d2_wait_start(ZkD2Smem& sm, uint32_t c, uint3
     }
 }
 
-template <int VARIANT>
-__device__ __forceinline__ void zk_exec_body(ZkD2Smem& sm, const ZkDecodeArgs& a, uint32_t ring_bytes) {
+// One segment (K-D1p) of an entry: blocks [first block, next segment start or run_blocks), from the segment's output
+// position on.  The ring and the in-order state start at that position; a segment's first block either starts a zstd
+// frame or uses no repeat offset it did not set itself, so R0..R2 need no incoming state.  The checks that need only
+// block sizes were made by the plan kernel, which also stopped the walk where the serial one stopped.
+__device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs& a, uint32_t ring_bytes, uint32_t first_bidx) {
     ZK_DYN_SMEM(ring_mem);
-    const uint32_t e = blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, W = blockDim.x >> 5;
-    ZkEntry ent = a.entries[e];
-    if (ent.status != 0 || a.counters->overflow) return;
-    if (threadIdx.x == 0) { sm.done_pos = 0; sm.done_chunk = 0; sm.flushed_pos = 0; sm.flushed_chunk = 0; sm.abort_code = 0; }
+    const ZkBlock head = a.blocks[first_bidx];
+    const uint32_t e = head.entry;
+    const ZkEntry ent = a.entries[e];
+    const uint32_t pos0 = head.out_pos;
+    if (threadIdx.x == 0) { sm.done_pos = pos0; sm.done_chunk = 0; sm.flushed_pos = pos0; sm.flushed_chunk = 0; sm.abort_code = 0; sm.abort_block = 0xFFFFFFFFu; }
     for (uint32_t i = threadIdx.x; i < ZK_D2_META; i += blockDim.x) { sm.started[i] = 0; sm.done[i] = 0; sm.flushed[i] = 0; sm.litdone[i] = 0; }
     __syncthreads();
     uint8_t* out = a.dst + a.d_off[e];
-    const unsigned long long cap64 = a.d_off[e + 1] - a.d_off[e];
-    const uint32_t cap = cap64 > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)cap64;
     const uint8_t* ebase = a.comp + a.c_off[e];
     ZkRing rg; rg.ring = ring_mem; rg.mask = ring_bytes - 1; rg.mis = (uint32_t)((uintptr_t)out & 15); rg.out = out;
     const uint32_t half = ring_bytes >> 1;
 
-    uint32_t pos = 0, zstart = 0, chunk_base = 0;
+    uint32_t pos = pos0, zstart = head.frame_start, chunk_base = 0;
     uint32_t R0 = 1, R1 = 4, R2 = 8;
     uint32_t preannounced = 0xFFFFFFFFu;          // chunk id this warp has already announced ahead of time
-    // range reads: stop at the first block boundary at or after the wanted prefix (every warp takes the same decision)
-    const uint32_t need = a.d_need ? a.d_need[e] : 0xFFFFFFFFu;
-    bool stopped = false;
-    for (uint32_t bi = 0; bi < ent.n_blocks; bi++) {
+    for (uint32_t bi = first_bidx - ent.first_block; bi < ent.run_blocks; bi++) {
         if (zk_d2_aborted(sm)) break;
-        if (pos >= need) { stopped = true; break; }
         const uint32_t bidx = ent.first_block + bi;
         const ZkBlock blk = a.blocks[bidx];
+        if (bidx != first_bidx && (blk.flags & ZKB_SEG)) break;
         if (blk.flags & ZKB_FIRST) { R0 = 1; R1 = 4; R2 = 8; zstart = pos; }
-        if (blk.status != 0 || blk.lit_status != 0) { zk_d2_abort(sm, blk.status ? -blk.status : -blk.lit_status); break; }
         const bool has_seq = blk.type == 2 && blk.nseq > 0;
         const uint32_t nchunks = has_seq ? (blk.nseq + 31) / 32 + 1 : 1;
-        if ((unsigned long long)pos + blk.regen > cap) { zk_d2_abort(sm, ZKZ_DST_TOO_SMALL); break; }
         // first chunk index of this block that belongs to this warp
         uint32_t c = chunk_base + ((uint32_t)warp + W - (chunk_base % W)) % W;
         for (; c < chunk_base + nchunks; c += W) {
@@ -1252,7 +1387,7 @@ __device__ __forceinline__ void zk_exec_body(ZkD2Smem& sm, const ZkDecodeArgs& a
                 else if (blk.lit_kind == 1) zk_warp_fill(out + pos, blk.lit_byte, blk.lit_size, lane);
                 else zk_warp_copy(out + pos, blk.lit_kind == 0 ? ebase + blk.lit_src : a.lit + blk.lit_base, blk.lit_size, lane);
                 __syncwarp();
-                { uint32_t en = pos + blk.regen; zk_ring_reload(rg, en > half ? en - half : 0, en, lane, 32); }
+                { uint32_t en = pos + blk.regen; zk_ring_reload(rg, en - pos0 > half ? en - half : pos0, en, lane, 32); }   // (output before pos0 belongs to other CTAs)
                 zk_d2_mark_done(sm, c, lane);
                 zk_d2_mark_flushed(sm, c, lane);
                 continue;
@@ -1310,7 +1445,7 @@ __device__ __forceinline__ void zk_exec_body(ZkD2Smem& sm, const ZkDecodeArgs& a
                 }
                 if (off == 0 || off > md - zstart) bad = true;
             }
-            if (__any_sync(0xFFFFFFFFu, bad)) { zk_d2_abort(sm, ZKZ_CORRUPTION); break; }
+            if (__any_sync(0xFFFFFFFFu, bad)) { zk_d2_abort(sm, ZKZ_CORRUPTION, bi); break; }
             const uint32_t chunk_start = pos + __shfl_sync(0xFFFFFFFFu, oe_prev, 0);
             const uint32_t chunk_end = pos + __shfl_sync(0xFFFFFFFFu, oe, min(31u, blk.nseq - 1 - j * 32));
             const bool direct = chunk_end - chunk_start > half;
@@ -1525,18 +1660,28 @@ __device__ __forceinline__ void zk_exec_body(ZkD2Smem& sm, const ZkDecodeArgs& a
         }
         pos += blk.regen;
         chunk_base += nchunks;
-        if (blk.flags & ZKB_LAST) {
-            if ((blk.flags & ZKB_HAS_FCS) && blk.fcs != (unsigned long long)(pos - zstart)) { zk_d2_abort(sm, ZKZ_CORRUPTION); break; }
-            if (threadIdx.x == 0) { a.blocks[bidx].hash_start = zstart; a.blocks[bidx].hash_len = pos - zstart; }
-        }
     }
     __syncthreads();
     if (threadIdx.x == 0) {
-        int code = sm.abort_code;
-        if (!code && !stopped && (unsigned long long)pos != cap64) code = pos < cap64 ? ZKZ_SRC_SIZE_WRONG : ZKZ_DST_TOO_SMALL;
-        a.entries[e].status = code ? -code : 0;
-        a.entries[e].produced = pos;
-        if (code) atomicAdd(&a.counters->n_errors, 1u);
+        ZkEntry& en = a.entries[e];
+        if (sm.abort_code) atomicMin(&en.fail, ZK_FAIL_KEY(sm.abort_block, ZK_FAIL_EXEC, sm.abort_code));
+        __threadfence();
+        if (atomicSub(&en.segs_left, 1u) == 1u) { __threadfence(); zk_entry_finish(a, e); }   // the entry's last segment
+    }
+}
+
+// CTAs are persistent: each pulls segments from a work counter until none is left.  Segments never wait for each other,
+// so a CTA that is not resident holds nobody up.
+__device__ __forceinline__ void zk_exec_body(ZkD2Smem& sm, const ZkDecodeArgs& a, uint32_t ring_bytes) {
+    if (a.counters->overflow) return;
+    const uint32_t nseg = a.counters->n_segments;
+    for (;;) {
+        if (threadIdx.x == 0) sm.seg = atomicAdd(&a.work_counter[2], 1u);
+        __syncthreads();
+        const uint32_t s = sm.seg;
+        if (s >= nseg) break;
+        zk_exec_segment(sm, a, ring_bytes, a.seg_list[s]);
+        __syncthreads();                          // every warp is done with the segment before its state is reset
     }
 }
 
@@ -1932,11 +2077,11 @@ __global__ void __launch_bounds__(1024, 1) zk_exec2_kernel(ZkDecodeArgs a, uint3
 // stay resident and the warps per SM are what hides the latency.
 __global__ void __launch_bounds__(512, 1) zk_exec_kernel(ZkDecodeArgs a, uint32_t ring_bytes) {
     __shared__ ZkD2Smem sm;
-    zk_exec_body<0>(sm, a, ring_bytes);
+    zk_exec_body(sm, a, ring_bytes);
 }
 __global__ void __launch_bounds__(160, 4) zk_exec_kernel_w5(ZkDecodeArgs a, uint32_t ring_bytes) {
     __shared__ ZkD2Smem sm;
-    zk_exec_body<1>(sm, a, ring_bytes);
+    zk_exec_body(sm, a, ring_bytes);
 }
 
 // =============================================================================================
@@ -1987,7 +2132,7 @@ static int zk_grow(void** p, size_t* cap, size_t need, size_t elem) {
 
 void zk_decode_ws_free(ZkDecodeWs* ws) {
     void* ptrs[] = { ws->blocks, ws->entries, ws->counters, ws->lit, ws->seq_lit_end, ws->seq_out_end, ws->seq_off, ws->c_off, ws->d_off,
-                     ws->huf_list, ws->seq_list, ws->d_need };
+                     ws->huf_list, ws->seq_list, ws->seg_list, ws->d_need };
     for (void* p : ptrs) if (p) cudaFree(p);
     if (ws->h_need) cudaFreeHost(ws->h_need);
     if (ws->h_entries) cudaFreeHost(ws->h_entries);
@@ -2007,11 +2152,13 @@ static int zk_decode_ensure(ZkDecodeWs* ws, uint32_t n, size_t need_blocks, size
     int rc;
     size_t cap;
     if (ws->cap_blocks < need_blocks || !ws->blocks) {
-        size_t c1 = ws->cap_blocks, c2 = ws->cap_blocks, c3 = ws->cap_blocks;
+        size_t c1 = ws->cap_blocks, c2 = ws->cap_blocks, c3 = ws->cap_blocks, c4 = ws->cap_blocks;
         if ((rc = zk_grow((void**)&ws->blocks, &c1, need_blocks, sizeof(ZkBlock)))) return rc;
         if ((rc = zk_grow((void**)&ws->huf_list, &c2, need_blocks, 4))) return rc;
         if ((rc = zk_grow((void**)&ws->seq_list, &c3, need_blocks, 4))) return rc;
+        if ((rc = zk_grow((void**)&ws->seg_list, &c4, need_blocks, 4))) return rc;
         ws->cap_blocks = c1 < c2 ? (c1 < c3 ? c1 : c3) : (c2 < c3 ? c2 : c3);
+        if (c4 < ws->cap_blocks) ws->cap_blocks = c4;
     }
     cap = ws->cap_lit; if ((rc = zk_grow((void**)&ws->lit, &cap, need_lit + 64, 1))) return rc; ws->cap_lit = cap;
     if (ws->cap_seq < need_seq || !ws->seq_off) {
@@ -2078,9 +2225,9 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     ZkDecodeArgs a;
     a.comp = d_comp; a.c_off = (const unsigned long long*)ws->c_off; a.d_off = (const unsigned long long*)ws->d_off; a.dst = d_dst; a.n_entries = n;
     a.blocks = ws->blocks; a.entries = ws->entries; a.counters = ws->counters;
-    a.work_counter = (uint32_t*)((uint8_t*)ws->counters + sizeof(ZkCounters));   // two counters (seq, huf), zeroed with the struct
+    a.work_counter = (uint32_t*)((uint8_t*)ws->counters + sizeof(ZkCounters));   // three counters (seq, huf, exec), zeroed with the struct
     a.lit = ws->lit; a.seq_lit_end = ws->seq_lit_end; a.seq_out_end = ws->seq_out_end; a.seq_off = ws->seq_off;
-    a.huf_list = ws->huf_list; a.seq_list = ws->seq_list;
+    a.huf_list = ws->huf_list; a.seq_list = ws->seq_list; a.seg_list = ws->seg_list;
     a.cap_blocks = ws->cap_blocks; a.cap_lit = ws->cap_lit - 64; a.cap_seq = ws->cap_seq;
     a.trace = nullptr;
     a.d_need = nullptr;
@@ -2151,8 +2298,10 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     int per_sm = (int)(((unsigned long long)n * (unsigned)(ws->share > 0 ? ws->share : 1) + (uint32_t)sms - 1) / (uint32_t)sms);
     if (per_sm < 1) per_sm = 1;
     int W = exec_warps;
-    ws->prof.begin(3, stream);
-    if (ws->exec_v2 || a.prefix_len) {           // (prefix mode exists in the in-order kernel only)
+    const bool exec_v2 = ws->exec_v2 || a.prefix_len;
+    ws->prof.begin(3, stream);                   // (the exec slot includes the plan kernel)
+    if (!exec_v2) ZK_LAUNCH(zk_plan_kernel, (n + 3) / 4, 128, 0, stream, a);
+    if (exec_v2) {           // (prefix mode exists in the in-order kernel only)
         // second-generation kernel: <= 64 registers, so 32 warps per SM whatever the split; ring = what is left of the
         // SM's shared memory per resident entry
         if (per_sm > 8) per_sm = 8;
@@ -2165,7 +2314,8 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
         ZK_LAUNCH(zk_exec2_kernel, n, W * 32, ring, stream, a, ring);
     } else {
         // 126 registers/thread -> 16 warps per SM; from four entries per SM on, the 96-register build of the same body
-        // (20 warps per SM, <= 5 per entry) keeps every entry of the batch resident with one more warp each
+        // (20 warps per SM, <= 5 per entry) keeps every entry of the batch resident with one more warp each.  One CTA per
+        // entry; the CTAs then share the batch's segments (K-D1p).
         bool small_regs = false;
         if (W <= 0) {
             if (per_sm >= 4) { W = 20 / per_sm; if (W < 2) W = 2; small_regs = true; }
@@ -2183,7 +2333,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     if (ds != stream) { ZK_CUDA_OK(cudaEventRecord(ws->ev_done, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(ds, ws->ev_done, 0)); }
     ZK_CUDA_OK(cudaMemcpyAsync(ws->h_entries, ws->entries, (size_t)n * sizeof(ZkEntry), cudaMemcpyDeviceToHost, ds));
     ZK_CUDA_OK(cudaMemcpyAsync(ws->h_counters, ws->counters, sizeof(ZkCounters), cudaMemcpyDeviceToHost, ds));
-    ws->launches += 4 + (verify_checksum ? 1 : 0);
+    ws->launches += 4 + (exec_v2 ? 0 : 1) + (verify_checksum ? 1 : 0);
     ws->pending_n = n;
     return 0;
 }
@@ -2211,6 +2361,7 @@ int zk_decode_collect(ZkDecodeWs* ws, cudaStream_t stream, int32_t* status_out) 
         ws->want_blocks = (size_t)ws->h_counters->n_blocks; ws->want_lit = (size_t)ws->h_counters->n_lit; ws->want_seq = (size_t)ws->h_counters->n_seq;
         return ZK_ST_RETRY;
     }
+    ws->segments += ws->h_counters->n_segments;
     int worst = 0;
     for (uint32_t i = 0; i < n; i++) {
         int32_t st = ws->h_entries[i].status;

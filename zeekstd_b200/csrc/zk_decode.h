@@ -12,6 +12,7 @@ struct ZkDecodeArgs {                 // kernel parameter block (by value)
     ZkBlock* blocks; ZkEntry* entries; ZkCounters* counters; uint32_t* work_counter;
     uint8_t* lit; uint32_t* seq_lit_end; uint32_t* seq_out_end; uint32_t* seq_off;
     uint32_t* huf_list; uint32_t* seq_list;   // compacted indices of blocks with Huffman literals / with sequences
+    uint32_t* seg_list;                       // compacted indices of the first blocks of execution segments
     unsigned long long cap_blocks, cap_lit, cap_seq;
     unsigned long long* trace;        // debug: per-chunk clock64 stamps of entry 0 (env ZK_EXEC_TRACE), else nullptr
     const uint8_t* prefix; uint32_t prefix_len;   // raw-content prefix of every zstd frame (Decoder::decompress_with_prefix, decode.rs:211-214, 246-255); device pointer or nullptr
@@ -28,7 +29,7 @@ struct ZkDecodeWs {                   // HBM scratch owned by a zk_ctx, grown on
     const uint32_t* need = nullptr;   // host array for the NEXT enqueue (one-shot): leading bytes wanted per entry, see ZkDecodeArgs::d_need
     uint32_t* d_need = nullptr; uint32_t* h_need = nullptr;
     const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device pointer for the NEXT enqueue (one-shot, like `need`)
-    uint32_t* huf_list = nullptr; uint32_t* seq_list = nullptr;
+    uint32_t* huf_list = nullptr; uint32_t* seq_list = nullptr; uint32_t* seg_list = nullptr;
     bool attr_set = false; uint32_t ring_override = 0;
     bool seq_v1 = false, attr_set2 = false; uint32_t seq2_ctas = 6;   // ZK_SEQ_V1=1: the first-generation FSE kernel; persistent CTAs per SM of the second
     bool exec_v2 = false;             // ZK_EXEC_V2=1: the in-order exec kernel (zk_exec2_kernel) for every batch, not only in prefix mode
@@ -46,6 +47,7 @@ struct ZkDecodeWs {                   // HBM scratch owned by a zk_ctx, grown on
     uint32_t pending_n = 0;
     int sm_count = 0;
     unsigned long long launches = 0;  // kernels launched so far (bench.py's gpu_launches)
+    unsigned long long segments = 0;  // execution segments run so far (zk_ctx_decode_segments)
     ZkProf prof;
 };
 
