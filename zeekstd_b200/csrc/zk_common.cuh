@@ -139,7 +139,8 @@ struct ZkCounters {
     uint32_t overflow;
     uint32_t n_errors;
     uint32_t n_huf_blocks, n_seq_blocks;         // lengths of huf_list / seq_list
-    uint32_t n_segments;                         // length of seg_list: execution segments of the batch (plan kernel)
+    uint32_t n_long, n_short;                    // execution segments of the batch (plan kernel): seg_list[0, n_long) run on CTAs,
+                                                 // seg_list[cap_blocks - n_short, cap_blocks) on one warp each
 };
 
 // -------------------------------------------------------------------------------------------

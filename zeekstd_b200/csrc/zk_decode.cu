@@ -1001,6 +1001,8 @@ __global__ void __launch_bounds__(128) zk_plan_kernel(ZkDecodeArgs a) {
     // ---- backward over the blocks that run: suffix minimum of the lowest position read, segment starts
     long long low = 0x7FFFFFFFFFFFFFFFll;                                                // lowest position read by the blocks after this tile
     uint32_t nseg = 0;
+    __syncwarp();
+    uint32_t seg_end = run ? blocks[run - 1].out_pos + blocks[run - 1].regen : 0u;      // output end of the first segment after this tile
     for (uint32_t t = run ? (run - 1) & ~31u : 0; run; t -= 32) {
         const uint32_t bi = t + (uint32_t)lane;
         const bool in = bi < run;
@@ -1022,11 +1024,22 @@ __global__ void __launch_bounds__(128) zk_plan_kernel(ZkDecodeArgs a) {
         if (in) blocks[bi].flags = (uint8_t)(start ? flags | ZKB_SEG : flags & ~ZKB_SEG);
         const uint32_t m = __ballot_sync(0xFFFFFFFFu, start);
         if (m) {
-            uint32_t base = 0;
-            if (lane == 0) base = atomicAdd(&a.counters->n_segments, (uint32_t)__popc(m));
-            base = __shfl_sync(0xFFFFFFFFu, base, 0);
-            if (start) a.seg_list[base + __popc(m & ((1u << lane) - 1u))] = ent.first_block + bi;
+            // a segment ends where the next one starts (in this tile, else seg_end); short ones go to the single-warp list
+            const uint32_t later = m & (0xFFFFFFFEu << lane);
+            const uint32_t nxp = __shfl_sync(0xFFFFFFFFu, op, later ? __ffs((int)later) - 1 : 0);
+            const uint32_t end = later ? nxp : seg_end;
+            const uint32_t ms = __ballot_sync(0xFFFFFFFFu, start && a.exec_short && end - op <= a.exec_short), mlong = m & ~ms;
+            uint32_t base_l = 0, base_s = 0;
+            if (lane == 0) {
+                if (mlong) base_l = atomicAdd(&a.counters->n_long, (uint32_t)__popc(mlong));
+                if (ms) base_s = atomicAdd(&a.counters->n_short, (uint32_t)__popc(ms));
+            }
+            base_l = __shfl_sync(0xFFFFFFFFu, base_l, 0); base_s = __shfl_sync(0xFFFFFFFFu, base_s, 0);
+            const uint32_t below = (1u << lane) - 1u;
+            if ((ms >> lane) & 1u) a.seg_list[a.cap_blocks - 1 - (base_s + __popc(ms & below))] = ent.first_block + bi;
+            else if (start) a.seg_list[base_l + __popc(mlong & below)] = ent.first_block + bi;
             nseg += __popc(m);
+            seg_end = __shfl_sync(0xFFFFFFFFu, op, __ffs((int)m) - 1);
         }
         low = __shfl_sync(0xFFFFFFFFu, lo, 0);
         if (t == 0) break;
@@ -1674,7 +1687,7 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
 // so a CTA that is not resident holds nobody up.
 __device__ __forceinline__ void zk_exec_body(ZkD2Smem& sm, const ZkDecodeArgs& a, uint32_t ring_bytes) {
     if (a.counters->overflow) return;
-    const uint32_t nseg = a.counters->n_segments;
+    const uint32_t nseg = a.counters->n_long;
     for (;;) {
         if (threadIdx.x == 0) sm.seg = atomicAdd(&a.work_counter[2], 1u);
         __syncthreads();
@@ -1682,6 +1695,173 @@ __device__ __forceinline__ void zk_exec_body(ZkD2Smem& sm, const ZkDecodeArgs& a
         if (s >= nseg) break;
         zk_exec_segment(sm, a, ring_bytes, a.seg_list[s]);
         __syncthreads();                          // every warp is done with the segment before its state is reset
+    }
+}
+
+// =============================================================================================
+// K-D2w: short segments, one warp each.
+//
+// A segment is one serial chain that no other warp can shorten, so a warp runs it alone, strictly chunk after chunk:
+// when a chunk starts, everything before it is final, and none of the CTA kernel's cross-warp bookkeeping (descriptors,
+// completion masks, announcements, helping) is needed.  The warp keeps its last ZK_XW_WIN bytes of output in a private
+// shared-memory window with the CTA kernel's discipline: a chunk of at most half a window is built there and flushed to
+// HBM, so a source less than half a window before the chunk is still in the window ("near") and an older one is in HBM
+// ("far", flushed by this warp earlier: __syncwarp orders it).  Larger chunks, Raw / RLE and literal-only blocks are
+// copied HBM to HBM and the window is reloaded.  Inside a chunk, matches go in ballot rounds: a lane copies once every
+// earlier lane whose destination overlaps its source is done.  Every store lies inside the segment's output range, which no other warp or
+// CTA writes.  Repeat offsets, bounds and the failure key are those of zk_exec_segment.
+// =============================================================================================
+#define ZK_XW_WARPS 4u          // warps per CTA; __launch_bounds__ below asks for 8 CTAs (32 warps) per SM, i.e. <= 64 registers
+#define ZK_XW_WIN 4096u         // window bytes per warp (H100, bench mix: 2 KiB ran as fast, 8 KiB 9 % slower)
+
+__device__ __forceinline__ void zk_exec_warp_segment(const ZkDecodeArgs& a, uint8_t* win, uint32_t first_bidx, int lane) {
+    const ZkBlock& head = a.blocks[first_bidx];
+    const uint32_t e = head.entry, pos0 = head.out_pos;
+    const ZkEntry ent = a.entries[e];
+    uint8_t* out = a.dst + a.d_off[e];
+    const uint8_t* ebase = a.comp + a.c_off[e];
+    ZkRing rg; rg.ring = win; rg.mask = ZK_XW_WIN - 1; rg.mis = (uint32_t)((uintptr_t)out & 15); rg.out = out;
+    const uint32_t half = ZK_XW_WIN >> 1;
+    uint32_t pos = pos0, zstart = head.frame_start, R0 = 1, R1 = 4, R2 = 8;
+    uint32_t bad_block = 0xFFFFFFFFu;
+    for (uint32_t bi = first_bidx - ent.first_block; bi < ent.run_blocks && bad_block == 0xFFFFFFFFu; bi++) {
+        const uint32_t bidx = ent.first_block + bi;
+        const ZkBlock& blk = a.blocks[bidx];
+        const uint32_t flags = blk.flags, type = blk.type, nseq = blk.nseq, regen = blk.regen;
+        if (bidx != first_bidx && (flags & ZKB_SEG)) break;
+        if (flags & ZKB_FIRST) { R0 = 1; R1 = 4; R2 = 8; zstart = pos; }
+        const uint32_t lit_kind = blk.lit_kind, lit_byte = blk.lit_byte;
+        if (!(type == 2 && nseq > 0)) {
+            // ---------------- Raw block / RLE block / literals-only compressed block: HBM to HBM
+            if (type == 0) zk_warp_copy(out + pos, ebase + blk.src, blk.size, lane);
+            else if (type == 1) zk_warp_fill(out + pos, ebase[blk.src], blk.size, lane);
+            else if (lit_kind == 1) zk_warp_fill(out + pos, lit_byte, blk.lit_size, lane);
+            else zk_warp_copy(out + pos, lit_kind == 0 ? ebase + blk.lit_src : a.lit + blk.lit_base, blk.lit_size, lane);
+            pos += regen;
+            __syncwarp();
+            zk_ring_reload(rg, pos - pos0 > half ? pos - half : pos0, pos, lane, 32);   // (output before pos0 belongs to other warps)
+            __syncwarp();
+            continue;
+        }
+        const uint32_t seq_base = blk.seq_base;
+        const uint32_t* s_lit = a.seq_lit_end + seq_base;
+        const uint32_t* s_out = a.seq_out_end + seq_base;
+        const uint8_t* lit = lit_kind == 0 ? ebase + blk.lit_src : a.lit + blk.lit_base;
+        uint32_t le_last = 0, oe_last = 0;            // cumulative literal / output ends of the sequences before the chunk
+        for (uint32_t j = 0; j * 32 < nseq; j++) {
+            // ---------------- 32 sequences, one per lane
+            const uint32_t s = j * 32 + lane;
+            const bool valid = s < nseq;
+            const uint32_t sc = valid ? s : nseq - 1;     // lanes past the last sequence repeat its ends (zero-length runs)
+            const uint32_t le = s_lit[sc], oe = s_out[sc], offv = valid ? a.seq_off[seq_base + s] : 0u;
+            uint32_t le_prev = __shfl_up_sync(0xFFFFFFFFu, le, 1), oe_prev = __shfl_up_sync(0xFFFFFFFFu, oe, 1);
+            if (lane == 0) { le_prev = le_last; oe_prev = oe_last; }
+            const uint32_t ll = le - le_prev, ml = (oe - oe_prev) - ll;
+            const uint32_t o_lit = pos + oe_prev, md = o_lit + ll;
+            uint32_t off = offv;
+            bool bad = false;
+            if (valid) {
+                if (offv & ZK_SYM) {
+                    const uint32_t sl = ZK_SYM_SLOT(offv), dl = ZK_SYM_DELTA(offv);
+                    const uint32_t r = sl == 0 ? R0 : (sl == 1 ? R1 : R2);
+                    bad = r <= dl; off = r - dl;
+                }
+                if (off == 0 || off > md - zstart) bad = true;
+            }
+            if (__any_sync(0xFFFFFFFFu, bad)) { bad_block = bi; break; }
+            le_last = __shfl_sync(0xFFFFFFFFu, le, 31); oe_last = __shfl_sync(0xFFFFFFFFu, oe, 31);
+            const uint32_t chunk_start = pos + __shfl_sync(0xFFFFFFFFu, oe_prev, 0), chunk_end = pos + oe_last;
+            const bool direct = chunk_end - chunk_start > half;
+            const uint32_t src0 = md - off, need_end = src0 + (ml < off ? ml : off);
+            const bool near_src = !direct && src0 + half >= chunk_start;
+            if (direct) zk_chunk_literals<false>(rg, lit, lit_kind, lit_byte, le, le_prev, o_lit, lane);
+            else zk_chunk_literals<true>(rg, lit, lit_kind, lit_byte, le, le_prev, o_lit, lane);
+            __syncwarp();
+            uint32_t pending = __ballot_sync(0xFFFFFFFFu, valid && ml > 0);
+            while (pending) {
+                // everything below the first pending match's destination is final
+                const int first = __ffs((int)pending) - 1;
+                const uint32_t md_first = __shfl_sync(0xFFFFFFFFu, md, first);
+                const bool ready = ((pending >> lane) & 1u) && (need_end <= md_first || lane == first);
+                const uint32_t rmask = __ballot_sync(0xFFFFFFFFu, ready);
+                if (ready && ml < ZK_LONG) {
+                    if (direct) { uint8_t* d = out + md; const uint8_t* sp = d - off; for (uint32_t i = 0; i < ml; i++) d[i] = sp[i]; }
+                    else if (near_src) rg.copy_near(md, src0, ml);
+                    else {   // far source (HBM, never overlapping): 8 bytes per round trip
+                        const uint8_t* sp = out + src0;
+                        for (uint32_t i = 0; i < ml; i += 8) {
+                            unsigned long long v = zk_ld8_unaligned(sp + i);
+                            const uint32_t nb = ml - i < 8 ? ml - i : 8;
+                            rg.st8(md + i, (uint32_t)v, (uint32_t)(v >> 32), nb);
+                        }
+                    }
+                }
+                uint32_t longm = __ballot_sync(0xFFFFFFFFu, ready && ml >= ZK_LONG);
+                while (longm) {
+                    const int l = __ffs((int)longm) - 1; longm &= longm - 1;
+                    const uint32_t n = __shfl_sync(0xFFFFFFFFu, ml, l), d = __shfl_sync(0xFFFFFFFFu, md, l), o = __shfl_sync(0xFFFFFFFFu, off, l);
+                    const bool nr = __shfl_sync(0xFFFFFFFFu, (uint32_t)near_src, l) != 0;
+                    if (direct) zk_warp_match(out + d, o, n, lane);
+                    else if (!nr) { const uint8_t* sp = out + (d - o); for (uint32_t i = lane; i < n; i += 32) rg.at(d + i) = sp[i]; }
+                    else if (o >= n) { for (uint32_t i = lane; i < n; i += 32) rg.at(d + i) = rg.at(d - o + i); }
+                    else if (o >= 32) {           // overlapping, period >= 32: 32 bytes per step are already final
+                        for (uint32_t i0 = 0; i0 < n; i0 += 32) { const uint32_t i = i0 + lane; if (i < n) rg.at(d + i) = rg.at(d - o + i); __syncwarp(); }
+                    } else {                      // short period: replicate the pattern
+                        for (uint32_t i = lane; i < n; i += 32) rg.at(d + i) = rg.at(d - o + (i % o));
+                    }
+                }
+                __syncwarp();
+                pending &= ~rmask;
+            }
+            if (direct) zk_ring_reload(rg, chunk_end - half, chunk_end, lane, 32);
+            else zk_ring_flush(rg, chunk_start, chunk_end, lane);
+            __syncwarp();
+        }
+        if (bad_block != 0xFFFFFFFFu) break;
+        {   // ---------------- trailing literals of the block
+            const uint32_t n = blk.lit_size - le_last, st0 = pos + oe_last, en = pos + regen;
+            if (n > half) {
+                if (lit_kind == 1) zk_warp_fill(out + st0, lit_byte, n, lane);
+                else zk_warp_copy(out + st0, lit + le_last, n, lane);
+                __syncwarp();
+                zk_ring_reload(rg, en - half, en, lane, 32);
+            } else {
+                for (uint32_t i = lane; i < n; i += 32) rg.at(st0 + i) = lit_kind == 1 ? lit_byte : lit[le_last + i];
+                __syncwarp();
+                zk_ring_flush(rg, st0, en, lane);
+            }
+            __syncwarp();
+        }
+        uint32_t v[3] = { blk.rep_out[0], blk.rep_out[1], blk.rep_out[2] }, nr[3];
+        for (int q = 0; q < 3; q++) {
+            if (v[q] & ZK_SYM) { const uint32_t sl = ZK_SYM_SLOT(v[q]); const uint32_t r = sl == 0 ? R0 : (sl == 1 ? R1 : R2); nr[q] = r - ZK_SYM_DELTA(v[q]); }
+            else nr[q] = v[q];
+        }
+        R0 = nr[0]; R1 = nr[1]; R2 = nr[2];
+        pos += regen;
+    }
+    if (lane == 0) {
+        ZkEntry& en = a.entries[e];
+        if (bad_block != 0xFFFFFFFFu) atomicMin(&en.fail, ZK_FAIL_KEY(bad_block, ZK_FAIL_EXEC, ZKZ_CORRUPTION));
+        __threadfence();
+        if (atomicSub(&en.segs_left, 1u) == 1u) { __threadfence(); zk_entry_finish(a, e); }   // the entry's last segment
+    }
+    __syncwarp();
+}
+
+// Persistent: every warp pulls short segments from its own work counter until none is left.
+__global__ void __launch_bounds__(32 * ZK_XW_WARPS, 8) zk_exec_warp_kernel(ZkDecodeArgs a) {
+    ZK_DYN_SMEM(win_mem);
+    if (a.counters->overflow) return;
+    const int lane = threadIdx.x & 31;
+    uint8_t* win = win_mem + (threadIdx.x >> 5) * ZK_XW_WIN;
+    const uint32_t nshort = a.counters->n_short;
+    for (;;) {
+        uint32_t s = 0;
+        if (lane == 0) s = atomicAdd(&a.work_counter[3], 1u);
+        s = __shfl_sync(0xFFFFFFFFu, s, 0);
+        if (s >= nshort) break;
+        zk_exec_warp_segment(a, win, a.seg_list[a.cap_blocks - 1 - s], lane);
     }
 }
 
@@ -2225,7 +2405,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     ZkDecodeArgs a;
     a.comp = d_comp; a.c_off = (const unsigned long long*)ws->c_off; a.d_off = (const unsigned long long*)ws->d_off; a.dst = d_dst; a.n_entries = n;
     a.blocks = ws->blocks; a.entries = ws->entries; a.counters = ws->counters;
-    a.work_counter = (uint32_t*)((uint8_t*)ws->counters + sizeof(ZkCounters));   // three counters (seq, huf, exec), zeroed with the struct
+    a.work_counter = (uint32_t*)((uint8_t*)ws->counters + sizeof(ZkCounters));   // four counters (seq, huf, exec, single-warp exec), zeroed with the struct
     a.lit = ws->lit; a.seq_lit_end = ws->seq_lit_end; a.seq_out_end = ws->seq_out_end; a.seq_off = ws->seq_off;
     a.huf_list = ws->huf_list; a.seq_list = ws->seq_list; a.seg_list = ws->seg_list;
     a.cap_blocks = ws->cap_blocks; a.cap_lit = ws->cap_lit - 64; a.cap_seq = ws->cap_seq;
@@ -2299,6 +2479,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     if (per_sm < 1) per_sm = 1;
     int W = exec_warps;
     const bool exec_v2 = ws->exec_v2 || a.prefix_len;
+    a.exec_short = exec_v2 ? 0u : ws->exec_short;
     ws->prof.begin(3, stream);                   // (the exec slot includes the plan kernel)
     if (!exec_v2) ZK_LAUNCH(zk_plan_kernel, (n + 3) / 4, 128, 0, stream, a);
     if (exec_v2) {           // (prefix mode exists in the in-order kernel only)
@@ -2325,6 +2506,12 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
         uint32_t ring = 128 * 1024;
         while (ring > 8 * 1024 && (size_t)ring * (size_t)per_sm > 200 * 1024) ring >>= 1;
         if (ws->ring_override) ring = ws->ring_override;
+        if (a.exec_short) {      // short segments first, on single warps; the CTAs below then pull only long ones
+            uint32_t gw = (uint32_t)sms * 8u;
+            const size_t need_w = est_blocks / ZK_XW_WARPS + 1;
+            if (need_w < gw) gw = (uint32_t)need_w;
+            ZK_LAUNCH(zk_exec_warp_kernel, gw, 32 * ZK_XW_WARPS, ZK_XW_WARPS * ZK_XW_WIN, stream, a);
+        }
         if (small_regs) ZK_LAUNCH(zk_exec_kernel_w5, n, W * 32, ring, stream, a, ring);
         else ZK_LAUNCH(zk_exec_kernel, n, W * 32, ring, stream, a, ring);
     }
@@ -2333,7 +2520,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     if (ds != stream) { ZK_CUDA_OK(cudaEventRecord(ws->ev_done, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(ds, ws->ev_done, 0)); }
     ZK_CUDA_OK(cudaMemcpyAsync(ws->h_entries, ws->entries, (size_t)n * sizeof(ZkEntry), cudaMemcpyDeviceToHost, ds));
     ZK_CUDA_OK(cudaMemcpyAsync(ws->h_counters, ws->counters, sizeof(ZkCounters), cudaMemcpyDeviceToHost, ds));
-    ws->launches += 4 + (exec_v2 ? 0 : 1) + (verify_checksum ? 1 : 0);
+    ws->launches += 4 + (exec_v2 ? 0 : 1) + (a.exec_short ? 1 : 0) + (verify_checksum ? 1 : 0);
     ws->pending_n = n;
     return 0;
 }
@@ -2361,7 +2548,7 @@ int zk_decode_collect(ZkDecodeWs* ws, cudaStream_t stream, int32_t* status_out) 
         ws->want_blocks = (size_t)ws->h_counters->n_blocks; ws->want_lit = (size_t)ws->h_counters->n_lit; ws->want_seq = (size_t)ws->h_counters->n_seq;
         return ZK_ST_RETRY;
     }
-    ws->segments += ws->h_counters->n_segments;
+    ws->segments += ws->h_counters->n_long + ws->h_counters->n_short;
     int worst = 0;
     for (uint32_t i = 0; i < n; i++) {
         int32_t st = ws->h_entries[i].status;

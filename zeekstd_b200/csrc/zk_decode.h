@@ -12,7 +12,9 @@ struct ZkDecodeArgs {                 // kernel parameter block (by value)
     ZkBlock* blocks; ZkEntry* entries; ZkCounters* counters; uint32_t* work_counter;
     uint8_t* lit; uint32_t* seq_lit_end; uint32_t* seq_out_end; uint32_t* seq_off;
     uint32_t* huf_list; uint32_t* seq_list;   // compacted indices of blocks with Huffman literals / with sequences
-    uint32_t* seg_list;                       // compacted indices of the first blocks of execution segments
+    uint32_t* seg_list;                       // compacted indices of the first blocks of execution segments (long ones from the
+                                              // front, short ones from the back: together never more than cap_blocks)
+    uint32_t exec_short;                      // segments of at most this many output bytes run on one warp each; 0 = none
     unsigned long long cap_blocks, cap_lit, cap_seq;
     unsigned long long* trace;        // debug: per-chunk clock64 stamps of entry 0 (env ZK_EXEC_TRACE), else nullptr
     const uint8_t* prefix; uint32_t prefix_len;   // raw-content prefix of every zstd frame (Decoder::decompress_with_prefix, decode.rs:211-214, 246-255); device pointer or nullptr
@@ -33,6 +35,7 @@ struct ZkDecodeWs {                   // HBM scratch owned by a zk_ctx, grown on
     bool attr_set = false; uint32_t ring_override = 0;
     bool seq_v1 = false, attr_set2 = false; uint32_t seq2_ctas = 6;   // ZK_SEQ_V1=1: the first-generation FSE kernel; persistent CTAs per SM of the second
     bool exec_v2 = false;             // ZK_EXEC_V2=1: the in-order exec kernel (zk_exec2_kernel) for every batch, not only in prefix mode
+    uint32_t exec_short = 128 << 10;  // ZK_EXEC_SHORT: output bytes up to which a segment runs on one warp (zk_exec_warp_kernel); 0 = CTAs only
     uint32_t huf_pad = 0;             // extra dynamic smem per Huffman CTA: fewer resident CTAs -> more L1 for the streams (tuning)
     unsigned long long* trace = nullptr;
     int share = 1;                    // how many batches share the GPU concurrently (host pipeline depth)
