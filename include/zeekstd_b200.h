@@ -135,6 +135,24 @@ int32_t zk_decompress_frames_dev(zk_ctx* ctx, const void* d_comp, const uint64_t
                                  uint32_t n_frames, void* d_dst, int32_t verify_checksum, int32_t* status,
                                  void* cuda_stream);
 
+/*
+ * FrameSizePolicy::Compressed(target) over a whole buffer: frames close after the first 32 KiB block at which header + blocks >= target
+ * (or at 1 GiB of input).  "header + blocks" is the 10-byte frame header plus every block with its 3-byte block header; the 4-byte
+ * checksum does not count (encode.rs:537-544).  The cut depends only on the input, target, level, checksum flag and prefix.
+ * final == 0: only closed frames are written; *consumed = input bytes they cover, the rest must be passed again with more input (a
+ * frame that would end exactly at the end of the input stays open).  final != 0: the rest becomes the last frame; n == 0 gives one
+ * empty frame.  target == 0 behaves like 1.  dst_cap >= zk_compress_bound(n, 32768) and frames_cap >= n / 32768 + 2 always suffice;
+ * less returns -70 (dstSize_tooSmall).  HOST pointers.
+ */
+int32_t zk_compress_frames_csize(zk_ctx* ctx, const uint8_t* src, size_t n, uint32_t target, int32_t level, int32_t checksum,
+                                 const uint8_t* prefix, size_t prefix_len, int32_t final, uint8_t* dst, size_t dst_cap,
+                                 uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames,
+                                 size_t* dst_len, size_t* consumed);
+/* the same on device pointers (conventions of zk_compress_frames_dev; no prefix, like the other _dev entry points) */
+int32_t zk_compress_frames_csize_dev(zk_ctx* ctx, const void* d_src, size_t n, uint32_t target, int32_t level, int32_t checksum,
+                                     int32_t final, void* d_dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes,
+                                     uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len, size_t* consumed, void* cuda_stream);
+
 /* ------------------------------------------------------------------ SeekTable (lib/src/seek_table.rs) */
 typedef struct zk_seek_table zk_seek_table;
 typedef enum { ZK_FORMAT_HEAD = 0, ZK_FORMAT_FOOT = 1 } zk_format; /* seek_table.rs:228-241 */

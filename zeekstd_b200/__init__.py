@@ -146,6 +146,23 @@ class Context:
                                           byref(dl)), lib)
         return dst[: dl.value], cs[: nf.value].copy(), ds[: nf.value].copy()
 
+    def compress_frames_csize(self, data, target: int, level: int = 0, checksum: bool = False, prefix=None, final: bool = True):
+        """FrameSizePolicy::Compressed(target) on the batch path -> (compressed bytes (np.uint8), c_sizes, d_sizes, consumed).
+        A frame closes after the first 32 KiB block at which its header + blocks reach `target` (or at 1 GiB of input).
+        final=False: only closed frames are made and `consumed` input bytes are covered; pass the rest again with more input."""
+        addr, n, keep = _buf(data)
+        lib = self.lib
+        cap = lib.zk_compress_bound(n, 32768)
+        dst = np.empty(cap + 64, dtype=np.uint8)
+        nfmax = n // 32768 + 2
+        cs = np.zeros(nfmax, dtype=np.uint32); ds = np.zeros(nfmax, dtype=np.uint32)
+        nf = c_uint32(); dl = c_size_t(); used = c_size_t()
+        paddr, pn, pkeep = _buf(prefix) if prefix is not None else (None, 0, None)
+        _check(lib.zk_compress_frames_csize(self._h, addr, n, target, level, int(checksum), paddr, pn, int(final), dst.ctypes.data, cap,
+                                            cs.ctypes.data_as(_native.u32p), ds.ctypes.data_as(_native.u32p), nfmax, byref(nf), byref(dl),
+                                            byref(used)), lib)
+        return dst[: dl.value], cs[: nf.value].copy(), ds[: nf.value].copy(), int(used.value)
+
     def decompress_frames(self, comp, c_off, d_off, verify_checksum: bool = True, out: np.ndarray | None = None, need=None, prefix=None):
         """decode frames given N+1 cumulative offsets -> (np.uint8 output, per-frame status, rc).
         need (optional, one uint32 per frame): only that many leading bytes of each frame are wanted (range reads,

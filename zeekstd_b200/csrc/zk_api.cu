@@ -486,3 +486,101 @@ extern "C" int32_t zk_decompress_frames_prefix(zk_ctx* c, const uint8_t* comp, c
     c->cur_prefix_len = 0;
     return rc;
 }
+
+// ---------------------------------------------------------------------------------------------
+// FrameSizePolicy::Compressed(target) on the batch path (zk_encode_csize): passes over the input, each starting at the first byte
+// the previous one left in an open frame.  A pass starts at the encode sub-batch size and doubles while it closes no frame, up to
+// 1 GiB, where the frame-size cap forces a close.
+// ---------------------------------------------------------------------------------------------
+static int32_t zk_csize_passes(zk_ctx* c, bool host, const uint8_t* src, size_t n, uint32_t target, int32_t level, int32_t checksum,
+                               const uint8_t* d_prefix, uint32_t prefix_len, int32_t final_, uint8_t* dst, size_t dst_cap,
+                               uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len,
+                               size_t* consumed, cudaStream_t st, size_t first_pass) {
+    const size_t block = 32768, max_pass = ZK_SEEKABLE_MAX_FRAME_SIZE;
+    first_pass = first_pass / block * block;
+    if (first_pass < block) first_pass = block;
+    if (first_pass > max_pass) first_pass = max_pass;
+    ZkSlot& s = c->slot[0];
+    s.ews.no_side = false;
+    size_t pos = 0, out = 0, pass = first_pass;
+    uint32_t nf = 0;
+    while (pos < n) {
+        const size_t len = n - pos < pass ? n - pos : pass;
+        const int at_end = pos + len == n;
+        const uint8_t* d_in = src + pos; uint8_t* d_out = dst + out; size_t cap = dst_cap - out;
+        if (host) {
+            cap = zk_encode_bound(len, (uint32_t)block);
+            int rc = zk_slot_ensure(&s, len + 32, cap + 32);
+            if (rc) return rc;
+            ZK_RT_OK(cudaMemcpyAsync(s.d_in, src + pos, len, cudaMemcpyHostToDevice, st));
+            d_in = s.d_in; d_out = s.d_out;
+        }
+        ZkCsizeOut r;
+        int rc = zk_encode_csize(&s.ews, st, d_in, len, target, level, checksum, final_, at_end, d_prefix, prefix_len, d_out, cap, &r);
+        if (rc) return rc;
+        if (r.n_frames == 0) {
+            if (at_end) break;
+            pass = 2 * pass < max_pass ? 2 * pass : max_pass;
+            continue;
+        }
+        if (r.n_frames > frames_cap - nf) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
+        if (host) {
+            if (r.total > dst_cap - out) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
+            ZK_RT_OK(cudaMemcpy(dst + out, s.d_out, r.total, cudaMemcpyDeviceToHost));
+        }
+        for (uint32_t f = 0; f < r.n_frames; f++) {
+            const size_t lo = (size_t)r.starts[f] * block, hi = (size_t)r.starts[f + 1] * block < len ? (size_t)r.starts[f + 1] * block : len;
+            if (c_sizes) c_sizes[nf + f] = r.c_sizes[f];
+            if (d_sizes) d_sizes[nf + f] = (uint32_t)(hi - lo);
+        }
+        nf += r.n_frames; out += r.total; pos += r.consumed;
+        pass = first_pass;
+    }
+    if (n_frames) *n_frames = nf;
+    if (dst_len) *dst_len = out;
+    if (consumed) *consumed = pos;
+    return 0;
+}
+
+extern "C" int32_t zk_compress_frames_csize(zk_ctx* c, const uint8_t* src, size_t n, uint32_t target, int32_t level, int32_t checksum,
+                                            const uint8_t* prefix, size_t prefix_len, int32_t final_, uint8_t* dst, size_t dst_cap,
+                                            uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames,
+                                            size_t* dst_len, size_t* consumed) {
+    if (!c || !dst || (n && !src)) return ZK_ERR_INVALID_ARG;
+    if (consumed) *consumed = 0;
+    if (n == 0) {                                           // one empty frame, as zk_compress_frames makes of no input
+        if (final_) return zk_compress_frames_prefix(c, src, 0, 1, level, checksum, prefix, prefix_len, dst, dst_cap, c_sizes, d_sizes, frames_cap, n_frames, dst_len);
+        if (n_frames) *n_frames = 0;
+        if (dst_len) *dst_len = 0;
+        return 0;
+    }
+    ZK_RT_OK(cudaSetDevice(c->device));
+    int32_t rc = zk_ctx_set_prefix(c, prefix, prefix_len);
+    if (rc) return rc;
+    rc = zk_csize_passes(c, true, src, n, target, level, checksum, c->cur_prefix_len ? c->d_prefix : nullptr, c->cur_prefix_len, final_, dst, dst_cap,
+                         c_sizes, d_sizes, frames_cap, n_frames, dst_len, consumed, c->slot[0].stream, zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20));
+    c->cur_prefix_len = 0;
+    return rc;
+}
+
+extern "C" int32_t zk_compress_frames_csize_dev(zk_ctx* c, const void* d_src, size_t n, uint32_t target, int32_t level, int32_t checksum,
+                                                int32_t final_, void* d_dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes,
+                                                uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len, size_t* consumed, void* cuda_stream) {
+    if (!c || !d_dst || (n && !d_src)) return ZK_ERR_INVALID_ARG;
+    if (consumed) *consumed = 0;
+    if (n == 0) {
+        if (final_) return zk_compress_frames_dev(c, d_src, 0, 1, level, checksum, d_dst, dst_cap, c_sizes, d_sizes, frames_cap, n_frames, dst_len, cuda_stream);
+        if (n_frames) *n_frames = 0;
+        if (dst_len) *dst_len = 0;
+        return 0;
+    }
+    ZK_RT_OK(cudaSetDevice(c->device));
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : c->slot[0].stream;
+    cudaEventRecord(c->ev0, st);
+    const int32_t rc = zk_csize_passes(c, false, (const uint8_t*)d_src, n, target, level, checksum, nullptr, 0, final_, (uint8_t*)d_dst, dst_cap,
+                                       c_sizes, d_sizes, frames_cap, n_frames, dst_len, consumed, st, zk_env_size("ZK_DEV_SUB_BYTES", (size_t)1 << 30));
+    cudaEventRecord(c->ev1, st);
+    cudaEventSynchronize(c->ev1);
+    cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1);
+    return rc;
+}

@@ -50,6 +50,9 @@ struct ZkEncodeArgs {
     // ptail <= ZKC_BLOCK bytes of it are staged in front of a copy of each frame's first block, so that block's match finder sees
     // one contiguous history and needs no second pointer
     const uint8_t* prefix; uint32_t prefix_len, ptail; uint8_t* pstage;
+    // bytes of the frame before a block that K-C1 may search, on top of the tier's own limit: unlimited (~0) except in the size variants
+    // of the wide tier (zk_encode_csize), where variant d must match the block d blocks into its frame
+    size_t hist_cap;
 };
 #define ZKC_PSLOT (2u * ZKC_BLOCK + 64u)   // per-frame staging slot: [prefix tail | first block]
 
@@ -990,6 +993,196 @@ __global__ void __launch_bounds__(128) zk_frame_gather_kernel(ZkEncodeArgs a) {
 }
 
 // =============================================================================================
+// K-C3c: FrameSizePolicy::Compressed(target) over one pass of at most 1 GiB (zk_encode_csize).
+//
+// A block's compressed bytes depend only on its own input, on how many earlier blocks of its frame it may search (its history
+// depth: <= 1 below the wide tier, <= ZKC_WIDE_HIST in it) and on whether it opens its frame (prefix tail, repeat offsets
+// {1,4,8}).  So K-C1/K-C2 run once per depth d = 0 .. V-1 over the whole pass ("variant d"), and block i of a frame that starts
+// at block s is variant min(i - s, V-1) of block i.  Every frame's size is then known for every possible start, and the cut is
+// exact: a frame closes after the first block at which header + blocks >= target, or at 1 GiB of input.
+// =============================================================================================
+#define ZKC_CAP_BLOCKS (0x40000000u / ZKC_BLOCK)     // SEEKABLE_MAX_FRAME_SIZE in blocks
+#define ZKC_OPEN 0xFFFFFFFFu                         // next[i]: the frame starting at block i does not close inside this pass
+#define ZKC_RES_HDR 8u                               // u32 words before fcs[] in the result area
+
+struct ZkCsizeArgs {
+    const uint8_t* src; size_t n;                    // the pass
+    uint32_t nb, V, target, level, checksum;
+    uint32_t end_closes;                             // the pass ends the input and the caller is done with it: the rest is the last frame
+    uint32_t end_lazy;                               // the pass ends the input but more may follow: a frame that ends there stays open
+    const ZkcBlock* vblocks;                         // V x nb: variant d of block i at [d * nb + i]
+    const uint8_t* vstage;                           // V x nb staging slots, same order
+    unsigned long long* psum;                        // nb + 1: prefix sum of variant V-1's sizes
+    uint32_t* next;                                  // nb: first block after the frame that starts at block i, or ZKC_OPEN
+    uint32_t* boff; uint32_t* bframe;                // nb: offset of the block inside its frame, frame of the block
+    unsigned long long* foff; uint32_t* fhash;       // per frame (nb at most)
+    // [0] frames, [1] blocks consumed, [2] error, [4..5] total bytes (u64); then fcs[nb] (frame sizes), starts[nb + 1] (first blocks)
+    uint32_t* res;
+    uint8_t* dst; size_t dst_cap;
+};
+
+// prefix sum of variant V-1's block sizes (one CTA)
+__global__ void __launch_bounds__(1024) zk_csize_psum_kernel(ZkCsizeArgs c) {
+    __shared__ unsigned long long part[1024];
+    __shared__ unsigned long long carry;
+    const ZkcBlock* bl = c.vblocks + (size_t)(c.V - 1) * c.nb;
+    if (threadIdx.x == 0) { carry = 0; c.psum[0] = 0; }
+    __syncthreads();
+    for (uint32_t base = 0; base < c.nb; base += 1024) {
+        const uint32_t i = base + threadIdx.x;
+        part[threadIdx.x] = i < c.nb ? bl[i].csize : 0;
+        __syncthreads();
+        for (uint32_t d = 1; d < 1024; d <<= 1) {
+            const unsigned long long t = threadIdx.x >= d ? part[threadIdx.x - d] : 0;
+            __syncthreads();
+            part[threadIdx.x] += t;
+            __syncthreads();
+        }
+        if (i < c.nb) c.psum[i + 1] = carry + part[threadIdx.x];
+        __syncthreads();
+        if (threadIdx.x == 1023) carry += part[1023];
+        __syncthreads();
+    }
+}
+
+// next[i] for every block i: the first V-1 blocks of the frame from their own variants, the rest by binary search in psum
+__global__ void __launch_bounds__(256) zk_csize_next_kernel(ZkCsizeArgs c) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= c.nb) return;
+    const uint32_t lim = c.nb - i < ZKC_CAP_BLOCKS ? c.nb : i + ZKC_CAP_BLOCKS;       // exclusive: end of the pass or the 1 GiB cap
+    unsigned long long acc = ZKC_FRAME_HDR;
+    uint32_t end = 0;                                                              // 0: target not reached before lim
+    for (uint32_t t = 0; t + 1 < c.V && i + t < lim; t++) {
+        acc += c.vblocks[(size_t)t * c.nb + i + t].csize;
+        if (acc >= c.target) { end = i + t + 1; break; }
+    }
+    if (!end && i + c.V - 1 < lim) {
+        // smallest j in [i + V, lim] with acc + psum[j] - psum[i + V - 1] >= target
+        const unsigned long long need = c.target - acc + c.psum[i + c.V - 1];
+        uint32_t lo = i + c.V, hi = lim + 1;
+        while (lo < hi) { const uint32_t mid = lo + (hi - lo) / 2; if (c.psum[mid] >= need) hi = mid; else lo = mid + 1; }
+        if (lo <= lim) end = lo;
+    }
+    bool closed = true;
+    if (!end) { end = lim; closed = lim - i == ZKC_CAP_BLOCKS || c.end_closes; }
+    if (end == c.nb && c.end_lazy) closed = false;
+    c.next[i] = closed ? end : ZKC_OPEN;
+}
+
+// the chain of frame starts from block 0 (one CTA; next[] in shared memory: a 1 GiB pass is 128 KiB of it)
+__global__ void __launch_bounds__(1024) zk_csize_walk_kernel(ZkCsizeArgs c) {
+    ZK_DYN_SMEM(smem);
+    uint32_t* nx = (uint32_t*)smem;
+    for (uint32_t i = threadIdx.x; i < c.nb; i += blockDim.x) nx[i] = c.next[i];
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t* starts = c.res + ZKC_RES_HDR + c.nb;
+        uint32_t f = 0, p = 0;
+        while (p < c.nb && nx[p] != ZKC_OPEN) { starts[f++] = p; p = nx[p]; }
+        starts[f] = p;
+        c.res[0] = f; c.res[1] = p;
+    }
+}
+
+// one warp per frame: block offsets inside the frame (warp scan over the chosen variants), frame size, XXH64 of the frame's input
+__global__ void __launch_bounds__(128) zk_csize_frame_kernel(ZkCsizeArgs c) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t f = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (f >= c.res[0]) return;
+    const uint32_t* starts = c.res + ZKC_RES_HDR + c.nb;
+    const uint32_t s = starts[f], e = starts[f + 1];
+    uint32_t run = ZKC_FRAME_HDR;
+    for (uint32_t j = s; j < e; j += 32) {
+        const uint32_t i = j + (uint32_t)lane;
+        uint32_t cs = 0;
+        if (i < e) { const uint32_t v = min(i - s, c.V - 1); cs = c.vblocks[(size_t)v * c.nb + i].csize; }
+        uint32_t incl = cs;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += t; }
+        if (i < e) { c.boff[i] = run + incl - cs; c.bframe[i] = f; }
+        run += __shfl_sync(0xFFFFFFFFu, incl, 31);
+    }
+    if (lane == 0) c.res[ZKC_RES_HDR + f] = run + (c.checksum ? 4u : 0u);
+    if (c.checksum) {
+        const size_t lo = (size_t)s * ZKC_BLOCK, hi = (size_t)e * ZKC_BLOCK < c.n ? (size_t)e * ZKC_BLOCK : c.n;
+        const unsigned long long h = zk_warp_xxh64(c.src + lo, (uint32_t)(hi - lo), lane);
+        if (lane == 0) c.fhash[f] = (uint32_t)h;
+    }
+}
+
+// frame offsets (one CTA; the frame count is read on the device)
+__global__ void __launch_bounds__(1024) zk_csize_scan_kernel(ZkCsizeArgs c) {
+    __shared__ unsigned long long part[1024];
+    __shared__ unsigned long long carry;
+    const uint32_t nf = c.res[0];
+    const uint32_t* fcs = c.res + ZKC_RES_HDR;
+    if (threadIdx.x == 0) carry = 0;
+    __syncthreads();
+    for (uint32_t base = 0; base < nf; base += 1024) {
+        const uint32_t f = base + threadIdx.x;
+        const unsigned long long v = f < nf ? fcs[f] : 0;
+        part[threadIdx.x] = v;
+        __syncthreads();
+        for (uint32_t d = 1; d < 1024; d <<= 1) {
+            const unsigned long long t = threadIdx.x >= d ? part[threadIdx.x - d] : 0;
+            __syncthreads();
+            part[threadIdx.x] += t;
+            __syncthreads();
+        }
+        if (f < nf) c.foff[f] = carry + part[threadIdx.x] - v;
+        __syncthreads();
+        if (threadIdx.x == 1023) carry += part[1023];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        *(unsigned long long*)(c.res + 4) = carry;
+        if (carry > c.dst_cap) c.res[2] = ZKZ_DST_TOO_SMALL;
+    }
+}
+
+// one warp per consumed block: copy its chosen variant into place and set Last_Block; a frame's first block also writes the frame
+// header (FCS = the frame's input length) and the checksum
+__global__ void __launch_bounds__(128) zk_csize_gather_kernel(ZkCsizeArgs c) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= c.res[1] || c.res[2]) return;
+    const uint32_t f = c.bframe[i];
+    const uint32_t* starts = c.res + ZKC_RES_HDR + c.nb;
+    const uint32_t s = starts[f], e = starts[f + 1], v = min(i - s, c.V - 1);
+    const uint32_t n = c.vblocks[(size_t)v * c.nb + i].csize;
+    const uint8_t* src = c.vstage + ((size_t)v * c.nb + i) * ZKC_SLOT;
+    uint8_t* fo = c.dst + c.foff[f];
+    if (i == s && lane == 0) {
+        const size_t lo = (size_t)s * ZKC_BLOCK, hi = (size_t)e * ZKC_BLOCK < c.n ? (size_t)e * ZKC_BLOCK : c.n;
+        const uint32_t fcs = (uint32_t)(hi - lo);
+        fo[0] = 0x28; fo[1] = 0xB5; fo[2] = 0x2F; fo[3] = 0xFD;
+        fo[4] = (uint8_t)(0x80 | (c.checksum ? 0x04 : 0));
+        fo[5] = c.level >= ZKC_WIDE_LEVEL ? 0x40 : 0x38;           // window 256 KiB in the wide tier, else 128 KiB (as zk_frame_{gather,window}_kernel)
+        fo[6] = (uint8_t)fcs; fo[7] = (uint8_t)(fcs >> 8); fo[8] = (uint8_t)(fcs >> 16); fo[9] = (uint8_t)(fcs >> 24);
+        if (c.checksum) {
+            const uint32_t h = c.fhash[f]; uint8_t* q = fo + c.res[ZKC_RES_HDR + f] - 4;
+            q[0] = (uint8_t)h; q[1] = (uint8_t)(h >> 8); q[2] = (uint8_t)(h >> 16); q[3] = (uint8_t)(h >> 24);
+        }
+    }
+    uint8_t* d = fo + c.boff[i];
+    // staged slots are 16-byte aligned; destinations are arbitrary -> byte-granular head, 16-byte body
+    uint32_t head = (uint32_t)((16 - ((uintptr_t)d & 15)) & 15); if (head > n) head = n;
+    if (lane < (int)head) d[lane] = src[lane];
+    const uint8_t* s2 = src + head; uint8_t* d2 = d + head; const uint32_t n2 = n - head, nvec = n2 >> 4;
+    const uint32_t mis = (uint32_t)((uintptr_t)s2 & 3);
+    const uint32_t* sa = (const uint32_t*)(s2 - mis); const uint32_t sh = mis * 8;
+    for (uint32_t k = lane; k < nvec; k += 32) {
+        const uint32_t* q = sa + 4 * k;
+        const uint32_t w0 = q[0], w1 = q[1], w2 = q[2], w3 = q[3], w4 = mis ? q[4] : 0;
+        ((uint4*)d2)[k] = mis ? make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh), __funnelshift_r(w3, w4, sh))
+                              : make_uint4(w0, w1, w2, w3);
+    }
+    for (uint32_t k = (nvec << 4) + lane; k < n2; k += 32) d2[k] = s2[k];
+    __syncwarp();
+    if (lane == 0) d[0] = (uint8_t)((src[0] & 0xFEu) | (i + 1 == e ? 1u : 0u));    // Last_Block: the variant was staged with its own layout's flag
+}
+
+// =============================================================================================
 // host-side launcher
 // =============================================================================================
 #ifndef ZK_EMUL
@@ -1017,6 +1210,7 @@ void zk_encode_ws_free(ZkEncodeWs* ws) {
 }
 
 static size_t zkc_align(size_t v) { return (v + 255) & ~(size_t)255; }
+static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, const ZkEncodeArgs& a);
 
 int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t frame_size, int level,
                       int checksum, uint8_t* d_dst, size_t dst_cap, uint32_t n_frames) {
@@ -1067,6 +1261,7 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     a.frame_csize = (uint32_t*)(base + o_fcs); a.frame_off = (unsigned long long*)(base + o_foff); a.frame_hash = (uint32_t*)(base + o_fh);
     a.dst = d_dst; a.dst_cap = dst_cap; a.total = (unsigned long long*)(base + o_tot); a.error = (uint32_t*)(base + o_tot + 8);
     a.prefix = d_prefix; a.prefix_len = 0; a.ptail = 0; a.pstage = base + o_pst;
+    a.hist_cap = ~(size_t)0;
     if (d_prefix && prefix_len && n) {
         a.prefix_len = prefix_len; a.ptail = prefix_len < ZKC_BLOCK ? prefix_len : ZKC_BLOCK;
         ZK_LAUNCH(zk_prefix_stage_kernel, n_frames, 256, 0, stream, a);
@@ -1089,6 +1284,25 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
         ZKC_CUDA_OK(cudaEventRecord(ws->ev_c, stream)); ZKC_CUDA_OK(cudaStreamWaitEvent(ss, ws->ev_c, 0));     // after whatever produced the input
         ZK_LAUNCH(zk_frame_hash_kernel, (n_frames + 3) / 4, 128, 0, ss, a);
     }
+    int rc = zkc_run_blocks(ws, stream, ss, a);
+    if (rc) return rc;
+    ws->prof.begin(7, stream);
+    if (checksum && ss == stream) ZK_LAUNCH(zk_frame_hash_kernel, (n_frames + 3) / 4, 128, 0, stream, a);   // else: already done on the side stream (joined by ev_b)
+    ZK_LAUNCH(zk_frame_size_kernel, (n_frames + 255) / 256, 256, 0, stream, a);
+    ZK_LAUNCH(zk_frame_scan_kernel, 1, 1024, 0, stream, a);
+    ZK_LAUNCH(zk_frame_gather_kernel, (uint32_t)((n_blocks + 3) / 4), 128, 0, stream, a);
+    if (a.level >= ZKC_WIDE_LEVEL) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames); ws->launches++; }
+    ws->prof.end(7, stream);
+    ZKC_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, a.frame_csize, (size_t)n_frames * 4, cudaMemcpyDeviceToHost, stream));
+    ZKC_CUDA_OK(cudaMemcpyAsync(ws->h_sizes + ws->cap_frames, a.total, 16, cudaMemcpyDeviceToHost, stream));
+    ws->launches += 7 + (checksum ? 1 : 0);
+    ws->pending_frames = n_frames;
+    return 0;
+}
+
+// K-C1 and K-C2 over every block of `a` (match finding, then sequences on `ss` beside literals on `stream`, joined by the finish kernel)
+static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, const ZkEncodeArgs& a) {
+    const size_t n_blocks = a.n_blocks;
     ws->prof.begin(5, stream);
     // six tiers (EncodeOptions::compression_level, encode.rs:176): 1 = 2048-entry table, no history, no lazy step; 2-3 = 4096 entries,
     // previous-block history, one lazy step; 4-6 = double table (8-byte + 5-byte hashes, 4096 entries each), two warps per CTA; 7-9 = double
@@ -1116,17 +1330,6 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     if (ss != stream) ZKC_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_b, 0));
     ZK_LAUNCH(zk_block_finish_kernel, (uint32_t)((n_blocks + 3) / 4), 128, 0, stream, a);
     ws->prof.end(6, stream);
-    ws->prof.begin(7, stream);
-    if (checksum && ss == stream) ZK_LAUNCH(zk_frame_hash_kernel, (n_frames + 3) / 4, 128, 0, stream, a);   // else: already done on the side stream (joined by ev_b)
-    ZK_LAUNCH(zk_frame_size_kernel, (n_frames + 255) / 256, 256, 0, stream, a);
-    ZK_LAUNCH(zk_frame_scan_kernel, 1, 1024, 0, stream, a);
-    ZK_LAUNCH(zk_frame_gather_kernel, (uint32_t)((n_blocks + 3) / 4), 128, 0, stream, a);
-    if (a.level >= ZKC_WIDE_LEVEL) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames); ws->launches++; }
-    ws->prof.end(7, stream);
-    ZKC_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, a.frame_csize, (size_t)n_frames * 4, cudaMemcpyDeviceToHost, stream));
-    ZKC_CUDA_OK(cudaMemcpyAsync(ws->h_sizes + ws->cap_frames, a.total, 16, cudaMemcpyDeviceToHost, stream));
-    ws->launches += 7 + (checksum ? 1 : 0);
-    ws->pending_frames = n_frames;
     return 0;
 }
 
@@ -1153,4 +1356,121 @@ int zk_encode_batch(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     int rc = zk_encode_enqueue(ws, stream, d_src, n, frame_size, level, checksum, d_dst, dst_cap, n_frames);
     if (rc) return rc;
     return zk_encode_collect(ws, stream, c_sizes, dst_len);
+}
+
+// FrameSizePolicy::Compressed(target) over one pass of n <= 1 GiB bytes: V variant passes of K-C1/K-C2 (shared sequence, literal
+// and section scratch; a ZkcBlock[] and a staging area each), the cut (K-C3c), then the assembly of the frames it chose.
+// One D2H copy of the counts and sizes, then one synchronisation.
+int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t target, int level, int checksum,
+                    int final_, int at_end, const uint8_t* d_prefix, uint32_t prefix_len, uint8_t* d_dst, size_t dst_cap, ZkCsizeOut* out) {
+    *out = ZkCsizeOut();
+    if (n == 0) return 0;
+    if (n > 0x40000000u) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
+    const int lvl = level <= 0 ? 3 : level;
+    const uint32_t nb = (uint32_t)((n + ZKC_BLOCK - 1) / ZKC_BLOCK);
+    const uint32_t V = lvl >= ZKC_WIDE_LEVEL ? ZKC_WIDE_HIST + 1 : 2;
+    const bool pfx = d_prefix && prefix_len;
+    const size_t res_words = ZKC_RES_HDR + 2 * (size_t)nb + 1;
+    size_t off = 0;
+    const size_t o_blocks = off; off = zkc_align(off + (size_t)V * nb * sizeof(ZkcBlock));
+    const size_t o_ll = off; off = zkc_align(off + (size_t)nb * ZKC_MAXSEQ * 2);
+    const size_t o_ml = off; off = zkc_align(off + (size_t)nb * ZKC_MAXSEQ * 2);
+    const size_t o_off = off; off = zkc_align(off + (size_t)nb * ZKC_MAXSEQ * 4);
+    const size_t o_lits = off; off = zkc_align(off + (size_t)nb * ZKC_BLOCK);
+    const size_t o_stage = off; off = zkc_align(off + (size_t)V * nb * ZKC_SLOT + 64);
+    const size_t o_seqsec = off; off = zkc_align(off + (size_t)nb * ZKC_SEQSEC);
+    const size_t o_psum = off; off = zkc_align(off + ((size_t)nb + 1) * 8);
+    const size_t o_next = off; off = zkc_align(off + (size_t)nb * 4);
+    const size_t o_boff = off; off = zkc_align(off + (size_t)nb * 4);
+    const size_t o_bfr = off; off = zkc_align(off + (size_t)nb * 4);
+    const size_t o_foff = off; off = zkc_align(off + (size_t)nb * 8);
+    const size_t o_fh = off; off = zkc_align(off + (size_t)nb * 4);
+    const size_t o_res = off; off = zkc_align(off + res_words * 4);
+    const size_t o_pst = off; if (pfx) off = zkc_align(off + (size_t)nb * ZKC_PSLOT);
+    if (ws->cap < off) {
+        if (ws->buf) cudaFree(ws->buf);
+        ws->buf = nullptr; ws->cap = 0;
+        size_t want = off + off / 8;
+        if (cudaMalloc(&ws->buf, want) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
+        ws->cap = want;
+    }
+    if (ws->cap_frames < res_words) {
+        if (ws->h_sizes) cudaFreeHost(ws->h_sizes);
+        ws->h_sizes = nullptr; ws->cap_frames = 0;
+        size_t want = res_words + res_words / 8 + 16;
+        if (cudaMallocHost((void**)&ws->h_sizes, want * 4 + 32) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
+        ws->cap_frames = want;
+    }
+    uint8_t* base = (uint8_t*)ws->buf;
+    ZkCsizeArgs c;
+    c.src = d_src; c.n = n; c.nb = nb; c.V = V; c.target = target ? target : 1; c.level = (uint32_t)lvl; c.checksum = checksum ? 1 : 0;
+    c.end_closes = at_end && final_; c.end_lazy = at_end && !final_;
+    c.vblocks = (const ZkcBlock*)(base + o_blocks); c.vstage = base + o_stage;
+    c.psum = (unsigned long long*)(base + o_psum); c.next = (uint32_t*)(base + o_next);
+    c.boff = (uint32_t*)(base + o_boff); c.bframe = (uint32_t*)(base + o_bfr);
+    c.foff = (unsigned long long*)(base + o_foff); c.fhash = (uint32_t*)(base + o_fh);
+    c.res = (uint32_t*)(base + o_res); c.dst = d_dst; c.dst_cap = dst_cap;
+    ZKC_CUDA_OK(cudaMemsetAsync(c.res, 0, ZKC_RES_HDR * 4, stream));
+    cudaStream_t ss = stream;
+    if (!ws->no_side) {
+        if (!ws->side) {
+            ZKC_CUDA_OK(cudaStreamCreateWithPriority(&ws->side, cudaStreamNonBlocking, ws->prio));
+            ZKC_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_a, cudaEventDisableTiming));
+            ZKC_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_b, cudaEventDisableTiming));
+            ZKC_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_c, cudaEventDisableTiming));
+        }
+        ss = ws->side;
+    }
+    // variant passes.  d = 0: frames of one block, so every block opens its frame (prefix staging included); d >= 1: one frame
+    // over the pass, with the wide tier's history capped at d blocks below V - 1
+    for (uint32_t d = 0; d < V; d++) {
+        ZkEncodeArgs a;
+        a.src = d_src; a.n = n; a.n_blocks = nb;
+        a.frame_size = d == 0 ? ZKC_BLOCK : (uint32_t)n; a.n_frames = d == 0 ? nb : 1; a.blocks_per_frame = d == 0 ? 1 : nb;
+        a.level = lvl; a.checksum = c.checksum;
+        a.blocks = (ZkcBlock*)(base + o_blocks) + (size_t)d * nb;
+        a.seq_ll = (uint16_t*)(base + o_ll); a.seq_ml = (uint16_t*)(base + o_ml); a.seq_off = (uint32_t*)(base + o_off);
+        a.lits = base + o_lits; a.stage = base + o_stage + (size_t)d * nb * ZKC_SLOT; a.seqsec = base + o_seqsec;
+        a.frame_csize = nullptr; a.frame_off = nullptr; a.frame_hash = nullptr;
+        a.dst = d_dst; a.dst_cap = dst_cap; a.total = nullptr; a.error = nullptr;
+        a.prefix = d_prefix; a.prefix_len = 0; a.ptail = 0; a.pstage = base + o_pst;
+        a.hist_cap = d >= 1 && d + 1 < V ? (size_t)d * ZKC_BLOCK : ~(size_t)0;
+        if (d == 0 && pfx) {
+            a.prefix_len = prefix_len; a.ptail = prefix_len < ZKC_BLOCK ? prefix_len : ZKC_BLOCK;
+            ZK_LAUNCH(zk_prefix_stage_kernel, nb, 256, 0, stream, a);
+            ws->launches += 1;
+        }
+        int rc = zkc_run_blocks(ws, stream, ss, a);
+        if (rc) return rc;
+        ws->launches += 4;
+    }
+    ws->prof.begin(7, stream);
+    const uint32_t walk_smem = nb * 4;
+    if (!ws->attr_set_walk) {
+        ZKC_CUDA_OK(cudaFuncSetAttribute(zk_csize_walk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(ZKC_CAP_BLOCKS * 4)));
+        ws->attr_set_walk = true;
+    }
+    ZK_LAUNCH(zk_csize_psum_kernel, 1, 1024, 0, stream, c);
+    ZK_LAUNCH(zk_csize_next_kernel, (nb + 255) / 256, 256, 0, stream, c);
+    ZK_LAUNCH(zk_csize_walk_kernel, 1, 1024, walk_smem, stream, c);
+    ZK_LAUNCH(zk_csize_frame_kernel, (nb + 3) / 4, 128, 0, stream, c);
+    ZK_LAUNCH(zk_csize_scan_kernel, 1, 1024, 0, stream, c);
+    ZK_LAUNCH(zk_csize_gather_kernel, (nb + 3) / 4, 128, 0, stream, c);
+    ws->prof.end(7, stream);
+    ws->launches += 6;
+    ZKC_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, c.res, res_words * 4, cudaMemcpyDeviceToHost, stream));
+    ZKC_CUDA_OK(cudaStreamSynchronize(stream));
+#ifndef ZK_EMUL
+    { cudaError_t le__ = cudaGetLastError(); if (le__ != cudaSuccess) { zk_note_cuda_error("kernel launch / execution", (int)le__); return ZK_INT_CUDA; } }
+#endif
+    ws->prof.harvest();
+    const uint32_t* h = ws->h_sizes;
+    if (h[2]) return -(int)h[2];
+    out->n_frames = h[0];
+    out->consumed = (size_t)h[1] * ZKC_BLOCK < n ? (size_t)h[1] * ZKC_BLOCK : n;
+    unsigned long long total; memcpy(&total, h + 4, 8);
+    out->total = (size_t)total;
+    out->c_sizes = h + ZKC_RES_HDR;
+    out->starts = h + ZKC_RES_HDR + nb;
+    return 0;
 }

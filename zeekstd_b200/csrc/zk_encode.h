@@ -8,7 +8,7 @@ struct ZkEncodeWs {                    // HBM scratch owned by a zk_ctx slot, gr
     int sm_count = 0;
     unsigned long long launches = 0;
     uint32_t pending_frames = 0;
-    bool attr_set = false, attr_set_wide = false;
+    bool attr_set = false, attr_set_wide = false, attr_set_walk = false;
     const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device pointer: raw-content prefix for the NEXT enqueue (one-shot)
     int prio = 0;                     // CUDA stream priority of the side stream (matches the slot's stream)
     bool no_side = false;             // host pipelines: concurrency comes from the other sub-batches; every extra stream costs a hardware queue
@@ -25,3 +25,16 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
 int zk_encode_collect(ZkEncodeWs* ws, cudaStream_t stream, uint32_t* c_sizes, size_t* dst_len);
 void zk_encode_ws_free(ZkEncodeWs* ws);
 size_t zk_encode_bound(size_t n, uint32_t frame_size);
+
+// FrameSizePolicy::Compressed(target) over one pass of n <= 1 GiB bytes at d_src: frames close after the first 32 KiB block at which
+// header + blocks >= target, or at 1 GiB of input.  at_end: the pass ends the caller's input; final_: and no more input follows, so
+// the rest becomes the last frame (otherwise a frame that would end at the end of the input stays open).  Frames are written back to
+// back at d_dst.  The arrays in *out live in the workspace's pinned buffer until the next call.  Synchronous on `stream`.
+struct ZkCsizeOut {
+    uint32_t n_frames = 0;
+    size_t consumed = 0, total = 0;      // input bytes the frames cover; bytes written
+    const uint32_t* c_sizes = nullptr;   // n_frames compressed sizes
+    const uint32_t* starts = nullptr;    // n_frames + 1 first blocks (32 KiB units from d_src); the last one is the end of the last frame
+};
+int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t target, int level, int checksum,
+                    int final_, int at_end, const uint8_t* d_prefix, uint32_t prefix_len, uint8_t* d_dst, size_t dst_cap, ZkCsizeOut* out);

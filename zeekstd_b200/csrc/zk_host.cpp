@@ -364,9 +364,9 @@ extern "C" void zk_raw_encoder_reset_frame(zk_raw_encoder* e) { e->reset_frame()
 extern "C" void zk_raw_encoder_reset_seek_table(zk_raw_encoder* e) { e->seek_table = zk_seek_table(); }
 
 // ---- Encoder<W: Write> (encode.rs:568-800) -----------------------------------------------------------------
-// For FrameSizePolicy::Uncompressed whole frames are buffered and handed to the GPU in batches (the sink is owned by
-// the encoder, so delaying writes is invisible to the caller).  Compressed(n) goes frame by frame through the
-// RawEncoder logic above.
+// Input is buffered and handed to the GPU in batches (the sink is owned by the encoder, so delaying writes is invisible to
+// the caller).  Uncompressed(n) batches whole frames; Compressed(n) hands the buffer to zk_compress_frames_csize, which
+// closes frames by the rule of that entry point and leaves the open frame in the buffer.
 struct zk_encoder {
     zk_raw_encoder raw;
     zk_write_fn write; zk_flush_fn flush; void* user;
@@ -376,6 +376,7 @@ struct zk_encoder {
     size_t batch_frames = 8192;            // a GPU call takes the buffered complete frames once there are this many ...
     size_t batch_bytes = (size_t)128 << 20; // ... or this many bytes of them (64 frames of 2 MiB; thousands of small ones: one launch sequence serves them all)
     const uint8_t* prefix = nullptr; size_t prefix_len = 0;   // prefix of the frames in `batch` (compress_with_prefix)
+    size_t csize_at = (size_t)128 << 20;   // Compressed(n): buffered bytes at which the next cut runs (doubles while a cut closes no frame)
 
     int32_t sink(const uint8_t* p, size_t n) {
         if (!n) return 0;
@@ -401,6 +402,26 @@ struct zk_encoder {
         rc = sink(stage.data(), len);
         if (rc) return rc;
         batch.erase(batch.begin(), batch.begin() + (ptrdiff_t)count);
+        if (written) *written = len;
+        return 0;
+    }
+    // Compressed(n): every frame of `batch` that closes (all of them with final_), in one batch call
+    int32_t flush_csize(int32_t final_, size_t* written) {
+        const size_t count = batch.size();
+        size_t cap = zk_compress_bound(count, 32768);
+        stage.resize(cap);
+        uint32_t nfmax = (uint32_t)(count / 32768 + 2);
+        std::vector<uint32_t> cs(nfmax), ds(nfmax);
+        uint32_t nf = 0; size_t len = 0, used = 0;
+        static const uint8_t dummy = 0;
+        int32_t rc = zk_compress_frames_csize(raw.ctx, count ? batch.data() : &dummy, count, raw.size, raw.level, raw.checksum, prefix, prefix_len, final_,
+                                              stage.data(), cap, cs.data(), ds.data(), nfmax, &nf, &len, &used);
+        if (rc) return rc;
+        for (uint32_t i = 0; i < nf; i++) { rc = zk_seek_table_log_frame(&raw.seek_table, cs[i], ds[i]); if (rc) return rc; }
+        rc = sink(stage.data(), len);
+        if (rc) return rc;
+        batch.erase(batch.begin(), batch.begin() + (ptrdiff_t)used);
+        csize_at = nf || final_ ? batch_bytes : 2 * count;
         if (written) *written = len;
         return 0;
     }
@@ -439,19 +460,9 @@ extern "C" int32_t zk_encoder_compress_with_prefix(zk_encoder* e, const uint8_t*
         if (e->batch.empty()) { e->prefix = prefix; e->prefix_len = prefix_len; }
     }
     if (e->raw.kind == ZK_POLICY_COMPRESSED) {
-        // frame-at-a-time through the RawEncoder state machine, 128 KiB staging like the reference (:599)
-        std::vector<uint8_t>& st = e->stage; st.resize(131591);
-        size_t in_pos = 0;
-        while (in_pos < len) {
-            zk_compression_progress p{};
-            int32_t rc = zk_raw_encoder_compress_with_prefix(&e->raw, buf + in_pos, len - in_pos, st.data(), st.size(), prefix, prefix_len, &p);
-            if (rc) return rc;
-            if (p.in_progress == 0 && p.out_progress == 0) break;
-            rc = e->sink(st.data(), p.out_progress);
-            if (rc) return rc;
-            in_pos += p.in_progress;
-        }
-        if (consumed) *consumed = in_pos;
+        e->batch.insert(e->batch.end(), buf, buf + len);
+        if (e->batch.size() >= e->csize_at) { int32_t rc = e->flush_csize(0, nullptr); if (rc) return rc; }
+        if (consumed) *consumed = len;
         return 0;
     }
     const uint32_t fs = e->frame_limit();
@@ -467,21 +478,7 @@ extern "C" int32_t zk_encoder_compress_with_prefix(zk_encoder* e, const uint8_t*
 }
 
 extern "C" int32_t zk_encoder_end_frame(zk_encoder* e, size_t* written) {                                      // :704-717
-    if (e->raw.kind == ZK_POLICY_COMPRESSED) {
-        std::vector<uint8_t>& st = e->stage; st.resize(131591);
-        size_t total = 0;
-        for (;;) {
-            zk_epilogue_progress p{};
-            int32_t rc = zk_raw_encoder_end_frame(&e->raw, st.data(), st.size(), &p);
-            if (rc) return rc;
-            rc = e->sink(st.data(), p.out_progress);
-            if (rc) return rc;
-            total += p.out_progress;
-            if (p.data_left == 0) break;
-        }
-        if (written) *written = total;
-        return 0;
-    }
+    if (e->raw.kind == ZK_POLICY_COMPRESSED) return e->flush_csize(1, written);
     // everything buffered becomes frames; the last one may be short (or empty: end_frame on a fresh frame emits an
     // empty frame, exactly what the reference's finish() does on an empty stream)
     return e->flush_batch(e->batch.size(), written, true);

@@ -113,6 +113,23 @@ class DeviceCodec:
         k, cs, ds = self.compress_into(src, n, frame_size, level, checksum, dst)
         return dst[:k], cs, ds
 
+    def compress_csize(self, x: torch.Tensor, target: int, level: int, checksum: bool, final: bool = True):
+        """FrameSizePolicy::Compressed(target) (zk_compress_frames_csize_dev) -> (frames, c_sizes, d_sizes, consumed)"""
+        n = x.numel()
+        src = torch.cat([x, torch.zeros(self.PAD, dtype=torch.uint8, device=x.device)])
+        cap = self.compress_bound(n, 32768)
+        dst = self.empty(cap, x.device)
+        nfmax = n // 32768 + 2
+        cs = np.zeros(nfmax, dtype=np.uint32); ds = np.zeros(nfmax, dtype=np.uint32)
+        nf = ctypes.c_uint32(); dl = ctypes.c_size_t(); used = ctypes.c_size_t()
+        rc = self.lib.zk_compress_frames_csize_dev(self.ctx._h, src.data_ptr(), n, target, level, int(checksum), int(final), dst.data_ptr(), cap,
+                                                   cs.ctypes.data_as(_native.u32p), ds.ctypes.data_as(_native.u32p), nfmax, ctypes.byref(nf),
+                                                   ctypes.byref(dl), ctypes.byref(used), torch_stream_handle(x.device))
+        if rc:
+            raise RuntimeError(f"zk_compress_frames_csize_dev: {rc}")
+        self.device_ms += self.ctx.last_device_ms
+        return dst[: int(dl.value)], cs[: nf.value].astype(np.int64), ds[: nf.value].astype(np.int64), int(used.value)
+
     def decompress(self, comp: torch.Tensor, c_off, d_off, verify: bool):
         src = torch.cat([comp, torch.zeros(self.PAD, dtype=torch.uint8, device=comp.device)])
         out = self.empty(int(c_off[-1] * 0 + d_off[-1]), comp.device)
