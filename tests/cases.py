@@ -11,6 +11,7 @@ import numpy as np
 import zeekstd_b200 as zk
 from oracle import oracle as O
 from zeekstd_b200 import _native, corpus
+from framegen import BackBits as _BackBits, lit_header as _lit_header, nseq_bytes as _nseq_bytes
 from util import decode_frames, golden_bytes, golden_meta, offsets, split_frames
 
 INPUT = golden_bytes("dickens_96k.txt")[:12_345]       # plays the role of lib.rs's INPUT (the reference uses its own source text)
@@ -115,20 +116,6 @@ def check_corruption_is_detected(ctx, trials: int = 24):
     check_crafted_frames_rejected(ctx)
 
 
-class _BackBits:
-    """writer for zstd's backward bitstreams (RFC 8878 4.1): fields in the order they are WRITTEN, then the end mark"""
-
-    def __init__(self):
-        self.acc, self.n = 0, 0
-
-    def put(self, value: int, bits: int):
-        self.acc |= (value & ((1 << bits) - 1)) << self.n; self.n += bits
-
-    def finish(self) -> bytes:
-        self.put(1, 1)
-        return self.acc.to_bytes((self.n + 7) // 8, "little")
-
-
 def _frame(blocks) -> bytes:
     """magic, FHD 0 (no FCS, no checksum), window descriptor 0x50 (1 MiB), then (type, content[, regen]) blocks"""
     out = bytearray(b"\x28\xb5\x2f\xfd\x00\x50")
@@ -172,23 +159,6 @@ def crafted_frames():
 # --- hand-built VALID frames for the cells of the matrix libzstd's encoder does not reach on demand ------------------
 _LL_BITS = [0] * 16 + [1, 1, 1, 1, 2, 2, 3, 3, 4, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16]
 _ML_BITS = [0] * 32 + [1, 1, 1, 1, 2, 2, 3, 3, 4, 4, 5, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16]
-
-
-def _lit_header(kind: int, regen: int) -> bytes:
-    """Literals_Section_Header for Raw (0) / RLE (1) literals"""
-    if regen < 32:
-        return bytes([(regen << 3) | kind])
-    if regen < 4096:
-        return ((regen << 4) | (1 << 2) | kind).to_bytes(2, "little")
-    return ((regen << 4) | (3 << 2) | kind).to_bytes(3, "little")
-
-
-def _nseq_bytes(n: int) -> bytes:
-    if n < 128:
-        return bytes([n])
-    if n < 0x7F00:
-        return bytes([128 + (n >> 8), n & 0xFF])
-    return bytes([0xFF, (n - 0x7F00) & 0xFF, (n - 0x7F00) >> 8])
 
 
 def _rle_seq_block(lit_section: bytes, codes, seqs, repeat_tables: bool = False) -> bytes:
