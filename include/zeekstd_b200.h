@@ -44,6 +44,13 @@ extern "C" {
 #define ZK_SKIPPABLE_HEADER_SIZE 8u
 #define ZK_DEFAULT_FRAME_SIZE 0x200000u /* FrameSizePolicy::default(), encode.rs:33-39 */
 
+/* Compression levels (the `level` argument of every compress entry point and of zk_encode_options_compression_level), as in libzstd:
+ *   0                 the default, level 3;
+ *   1 .. 22           the ratio tiers of DESIGN.md 3 (from 13 on: a 256 KiB window);
+ *   -1 .. -131072     fast mode with acceleration -level: sparser match probing, literals stored without Huffman coding.
+ *                     Lower levels clamp to ZK_MIN_COMPRESSION_LEVEL, as in libzstd (ZSTD_minCLevel()). */
+#define ZK_MIN_COMPRESSION_LEVEL (-131072)
+
 /* ------------------------------------------------------------------ errors (lib/src/error.rs:101-113) */
 #define ZK_OK 0
 #define ZK_ERR_NUMBER_CONVERSION (-1001) /* Kind::NumberConversionFailed */

@@ -8,8 +8,9 @@ What each piece follows in the reference: argument set and value parsers cli/src
 path derivation, overwrite checks and the list tables cli/src/command.rs:33-473; the compress loop (Encoder fed from a
 reader, optional stand-alone Head-format seek table) cli/src/compress.rs:55-106; the decompress loop
 cli/src/decompress.rs:21-117.  The codec underneath is this package's Encoder / Decoder, i.e. the CUDA path: there is no
-CPU route.  The window-log / long-distance-matching parameters the reference sets for patch files have no counterpart
-here (the kernels take the prefix as it is); `--mmap-prefix` / `--no-mmap-prefix` choose between np.memmap and a read.
+CPU route.  Compression levels are 1..19 as in the reference CLI, plus zstd's negative fast levels (`-l -5` or
+`--compression-level=-5`; acceleration = -level, clamped at -131072).  The window-log / long-distance-matching parameters
+the reference sets for patch files have no counterpart here (the kernels take the prefix as it is); `--mmap-prefix` / `--no-mmap-prefix` choose between np.memmap and a read.
 """
 from __future__ import annotations
 
@@ -117,9 +118,10 @@ def _add_common(p):
 
 
 def _level(s: str) -> int:
+    """1..19, or a negative level: zstd's fast mode (the codec clamps levels below -131072 to it, as libzstd does)"""
     v = int(s)
-    if not 1 <= v <= 19:
-        raise argparse.ArgumentTypeError("compression level must be between 1 and 19")
+    if not (1 <= v <= 19 or -(1 << 31) <= v < 0):
+        raise argparse.ArgumentTypeError("compression level must be between 1 and 19, or negative for fast mode")
     return v
 
 
@@ -130,7 +132,9 @@ def build_parser() -> argparse.ArgumentParser:
 
     c = sub.add_parser("compress", aliases=["c"], help="Compress INPUT_FILE (default); reads from STDIN if INPUT_FILE is `-` or not provided")
     _add_flags(c, False); _add_common(c)
-    c.add_argument("-l", "--compression-level", type=_level, default=3)
+    c.add_argument("-l", "--compression-level", type=_level, default=3,
+                   help="Compression level: 1-19, or negative (-1 down to -131072) for fast mode: faster, lower ratio, literals stored without "
+                        "Huffman coding. Default 3.")
     c.add_argument("--no-checksum", action="store_true", help="Don't include frame checksums.")
     c.add_argument("-s", "--frame-size", type=byte_value, default=byte_value("2M"))
     c.add_argument("--frame-size-policy", choices=["compressed", "uncompressed"], default="uncompressed")

@@ -94,6 +94,48 @@ __device__ __forceinline__ uint32_t zkc_hash8(unsigned long long v) {
 // =============================================================================================
 #define ZKC_C1_WARPS 4
 
+// a match whose first ml = 8 bytes agree, extended cooperatively: lane k compares bytes [8 + 8k, 16 + 8k) of it, 256 bytes a round
+__device__ __forceinline__ void zkc_extend_fwd(const uint8_t* sb, uint32_t mpos, uint32_t off, uint32_t hi32, int lane, uint32_t& ml) {
+    for (;;) {
+        const uint32_t q = mpos + ml + (uint32_t)lane * 8u;
+        uint32_t eq = 8;
+        if (q + 8 <= hi32) { const unsigned long long x = zkc_ld8(sb + q) ^ zkc_ld8(sb + q - off); if (x) eq = (uint32_t)(__ffsll((long long)x) - 1) >> 3; }
+        else { eq = 0; for (uint32_t t = q; t < hi32 && sb[t] == sb[t - off]; t++) eq++; }
+        const uint32_t stop = __ballot_sync(0xFFFFFFFFu, eq < 8);
+        if (stop) { const int g = __ffs((int)stop) - 1; ml += 8 * g + __shfl_sync(0xFFFFFFFFu, eq, g); break; }
+        ml += 256;
+    }
+}
+
+// Offset_Value of a sequence (A.5) for the fast tier, updating the repeat-offset history r0..r2 as the decoder will: the rule of
+// zk_match_body.inc, which keeps its own inline copy (as a call it costs the level-1 kernel two registers)
+__device__ __forceinline__ uint32_t zkc_offset_value(uint32_t off, uint32_t ll, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& known) {
+    uint32_t ov = off + 3;
+    if (off != r0 && off != r1 && off != r2 && off + 1 != r0) {           // the common case: an explicit offset
+        r2 = r1; r1 = r0; r0 = off; known += known < 3;
+    } else {
+        bool hit0 = false, hit1 = false;
+        if (known == 3) {
+            const bool e0 = off == r0, e1 = off == r1, e2 = off == r2, em = r0 > 1 && off == r0 - 1;
+            if (ll != 0) { if (e0) { ov = 1; hit0 = true; } else if (e1) { ov = 2; hit1 = true; } else if (e2) ov = 3; }
+            else { if (e1) { ov = 1; hit1 = true; } else if (e2) ov = 2; else if (em) ov = 3; }
+        } else known++;
+        if (!hit0) { r2 = hit1 ? r2 : r1; r1 = r0; r0 = off; }
+    }
+    return ov;
+}
+
+// n bytes from s to d by one warp: 8 bytes per lane and round (the source is read as aligned words, never past the word holding s[n - 1])
+__device__ __forceinline__ void zkc_warp_copy(uint8_t* __restrict__ d, const uint8_t* __restrict__ s, uint32_t n, int lane) {
+    const uint32_t n8 = n & ~7u;
+    for (uint32_t i = 8u * (uint32_t)lane; i < n8; i += 256) {
+        const unsigned long long v = zkc_ld8(s + i);
+#pragma unroll
+        for (int q = 0; q < 8; q++) d[i + q] = (uint8_t)(v >> (8 * q));
+    }
+    if ((uint32_t)lane < n - n8) d[n8 + lane] = s[n8 + lane];
+}
+
 // prefix mode: [tail of the prefix | first block of frame f] -> pstage slot f (one CTA per frame)
 __global__ void __launch_bounds__(256) zk_prefix_stage_kernel(ZkEncodeArgs a) {
     const uint32_t f = blockIdx.x;
@@ -146,6 +188,120 @@ __global__ void __launch_bounds__(32) zk_match_wide_kernel(ZkEncodeArgs a) {
 #include "zk_match_body.inc"
 #undef ZKM_POS_T
 #undef ZKM_HIST_BYTES
+}
+
+// Fast tier (level < 0, zstd's negative levels; acceleration A = -level): level 1's table, warps and history, with sparse probing.  Lane i of
+// a window probes position ip + i * s, where s = A + 1 + (windows since the last match) / ZKC_FAST_GROW, so long stretches without a match
+// are crossed ever faster.  Lanes whose probe lies past the last position where 8 bytes can be read idle for that window; only probed positions
+// are inserted.  A hit is extended forward as in the other tiers and backward down to the end of the previous sequence, which recovers the
+// start a sparse probe missed.  Literals are copied from the input when a sequence (or the block) ends.
+#define ZKC_FAST_GROW 8
+#define ZKC_MIN_LEVEL (-131072)          // ZSTD_minCLevel(): lower levels clamp to it
+template <int HLOG, int NW>
+__global__ void __launch_bounds__(NW * 32) zk_match_fast_kernel(ZkEncodeArgs a) {
+    __shared__ uint16_t tables[NW][1 << HLOG];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t b = blockIdx.x * NW + warp;
+    if (b >= a.n_blocks) return;
+    uint16_t* table = tables[warp];
+    size_t lo, hi, fstart;
+    zkc_block_range(a, b, lo, hi, fstart);
+    const bool pfx = a.ptail != 0 && lo == fstart;
+    const size_t hist = a.hist_cap < ZKC_BLOCK ? a.hist_cap : ZKC_BLOCK;
+    const size_t base = lo - fstart >= hist ? lo - hist : fstart;
+    const uint8_t* sb = pfx ? a.pstage + (size_t)(b / a.blocks_per_frame) * ZKC_PSLOT : a.src + base;
+    const uint32_t lo32 = pfx ? a.ptail : (uint32_t)(lo - base), hi32 = lo32 + (uint32_t)(hi - lo);
+    for (int i = lane; i < (1 << HLOG); i += 32) table[i] = 0;
+    __syncwarp();
+    uint16_t* o_ll = a.seq_ll + (size_t)b * ZKC_MAXSEQ; uint16_t* o_ml = a.seq_ml + (size_t)b * ZKC_MAXSEQ;
+    uint32_t* o_off = a.seq_off + (size_t)b * ZKC_MAXSEQ;
+    uint8_t* o_lit = a.lits + (size_t)b * ZKC_BLOCK;
+    uint32_t nseq = 0, nlit = 0;
+    uint32_t anchor = lo32;                                 // end of the last sequence: every literal byte below it is in o_lit
+    if (hi32 - lo32 >= 16) {
+        const uint32_t mflimit = hi32 - 8;                  // last position where 8 bytes can be read
+        const uint32_t step0 = (uint32_t)(-a.level) + 1u;
+        if (pfx) {                                          // the prefix tail, as at level 1
+            for (uint32_t p0 = 0; p0 < lo32; p0 += 32) {
+                const uint32_t p = p0 + lane;
+                const uint32_t hh = p < lo32 ? zkc_hash5<HLOG>(zkc_ld8(sb + p)) : (0xFFFF0000u | (uint32_t)lane);
+                const uint32_t same = __match_any_sync(0xFFFFFFFFu, hh);
+                if (p < lo32 && lane == 31 - __clz((int)same)) table[hh] = (uint16_t)p;
+            }
+            __syncwarp();
+        }
+        uint32_t rep = 0, r0 = 1, r1 = 4, r2 = 8, known = lo == fstart ? 3u : 0u;
+        uint32_t misses = 0;                                // windows since the last match
+        uint32_t s_ll = 0, s_ml = 0, s_off = 0, flushed = 0; // staged sequences: slot nseq - flushed lives in that lane
+        for (uint32_t ip = lo32; ip <= mflimit;) {
+            const uint32_t s = step0 + misses / ZKC_FAST_GROW;
+            const uint32_t wb = ip, p = wb + (uint32_t)lane * s;      // no overflow: s <= 2^17 + 65 (a block is <= 512 windows)
+            const bool live = p <= mflimit;
+            const unsigned long long cur = live ? zkc_ld8(sb + p) : 0ull;
+            const uint32_t h = live ? zkc_hash5<HLOG>(cur) : (0xFFFF0000u | (uint32_t)lane);
+            const uint32_t cand = live ? table[h] : 0u;
+            __syncwarp();
+            // several lanes may hash to the same slot: the highest position wins, as sequential insertion would leave it
+            const uint32_t same = __match_any_sync(0xFFFFFFFFu, h);
+            if (live && lane == 31 - __clz((int)same)) table[h] = (uint16_t)p;
+            uint32_t moff = 0, mlen0 = 0;
+            if (live && cand < p) {
+                const unsigned long long x = zkc_ld8(sb + cand) ^ cur;
+                const uint32_t m = x ? (uint32_t)(__ffsll((long long)x) - 1) >> 3 : 8;
+                if (m >= ZKC_MINMATCH) { moff = p - cand; mlen0 = m; }
+            }
+            if (live && rep && p >= rep) {
+                const unsigned long long x = zkc_ld8(sb + p - rep) ^ cur;
+                const uint32_t m = x ? (uint32_t)(__ffsll((long long)x) - 1) >> 3 : 8;
+                if (m >= 4 && m + 1 >= mlen0) { moff = rep; mlen0 = m; }
+            }
+            const uint32_t found = __ballot_sync(0xFFFFFFFFu, mlen0 != 0);
+            ip = wb + 32u * s;
+            if (!found) { misses++; continue; }
+            misses = 0;
+            const uint32_t packed = (moff << 4) | mlen0;
+            // every hit at or after the end of the previous sequence, left to right
+            for (uint32_t m = found; m;) {
+                const int f = __ffs((int)m) - 1;
+                const uint32_t mo = __shfl_sync(0xFFFFFFFFu, packed, f);
+                const uint32_t off = mo >> 4;
+                uint32_t mpos = wb + (uint32_t)f * s;
+                uint32_t ml = mo & 15u;
+                if (ml == 8) zkc_extend_fwd(sb, mpos, off, hi32, lane, ml);
+                // backward, one byte per lane and round, down to the previous sequence (and the start of the history)
+                const uint32_t lim = anchor > off ? anchor : off;
+                for (;;) {
+                    const bool eq = (uint32_t)lane < mpos - lim && sb[mpos - 1 - lane] == sb[mpos - 1 - lane - off];
+                    const uint32_t ne = __ballot_sync(0xFFFFFFFFu, !eq);
+                    const uint32_t k = ne ? (uint32_t)__ffs((int)ne) - 1 : 32u;
+                    mpos -= k; ml += k;
+                    if (k < 32) break;
+                }
+                const uint32_t ll = mpos - anchor;
+                zkc_warp_copy(o_lit + nlit, sb + anchor, ll, lane);
+                nlit += ll;
+                const uint32_t ov = zkc_offset_value(off, ll, r0, r1, r2, known);
+                if (nseq - flushed == 32) {
+                    const uint32_t at = flushed + (uint32_t)lane; o_ll[at] = (uint16_t)s_ll; o_ml[at] = (uint16_t)s_ml; o_off[at] = s_off;
+                    flushed = nseq;
+                }
+                if (lane == (int)(nseq - flushed)) { s_ll = ll; s_ml = ml - 3; s_off = ov; }
+                nseq++;
+                anchor = mpos + ml; rep = off;
+                if (anchor >= ip) { ip = anchor; break; }
+                const uint32_t first = (anchor - wb + s - 1) / s;           // the first lane whose probe lies at or after anchor
+                if (first >= 32) break;
+                m = found & (0xFFFFFFFFu << first);
+            }
+        }
+        if ((uint32_t)lane < nseq - flushed) {
+            const uint32_t at = flushed + (uint32_t)lane;
+            o_ll[at] = (uint16_t)s_ll; o_ml[at] = (uint16_t)s_ml; o_off[at] = s_off;
+        }
+    }
+    zkc_warp_copy(o_lit + nlit, sb + anchor, hi32 - anchor, lane);
+    nlit += hi32 - anchor;
+    if (lane == 0) { a.blocks[b].nseq = nseq; a.blocks[b].nlit = nlit; }
 }
 
 // =============================================================================================
@@ -601,6 +757,19 @@ __device__ int zkc_huf_build(ZkcC2Smem& sm, int lane) {
     return (int)sm.scratch[2];
 }
 
+// are all n >= 2 literals the same byte?  4-byte words (the buffer is 32 KiB aligned); most blocks settle in the first round
+__device__ __forceinline__ bool zkc_lits_rle(const uint8_t* lits, uint32_t n, int lane) {
+    const uint32_t c4 = lits[0] * 0x01010101u, n4 = n & ~3u;
+    bool rle = n >= 2;
+    for (uint32_t i0 = 0; rle && i0 < n4; i0 += 128) {
+        const uint32_t i = i0 + 4u * (uint32_t)lane;
+        rle = __all_sync(0xFFFFFFFFu, i >= n4 || *(const uint32_t*)(lits + i) == c4);
+    }
+    return __all_sync(0xFFFFFFFFu, (uint32_t)lane >= n - n4 || lits[n4 + lane] == lits[0]) && rle;
+}
+
+// HUF = false (the fast tier): literals are only ever Raw or RLE, decided without a histogram
+template <bool HUF>
 __global__ void __launch_bounds__(32) zk_lit_enc_kernel(ZkEncodeArgs a) {
     __shared__ ZkcC2Smem sm;
     const int lane = threadIdx.x;
@@ -610,17 +779,10 @@ __global__ void __launch_bounds__(32) zk_lit_enc_kernel(ZkEncodeArgs a) {
     const uint32_t len = (uint32_t)(hi - lo);
     const uint32_t k_in_frame = b % a.blocks_per_frame;
     // blocks past the end of a short last frame carry nothing
-    {
-        uint32_t f = b / a.blocks_per_frame;
-        size_t fend = fstart + a.frame_size < a.n ? fstart + a.frame_size : a.n;
-        uint32_t nb_frame = (uint32_t)((fend - fstart + ZKC_BLOCK - 1) / ZKC_BLOCK); if (nb_frame == 0) nb_frame = 1;
-        (void)f;
-        if (k_in_frame >= nb_frame) { if (lane == 0) { a.blocks[b].csize = 0; a.blocks[b].lit_bytes = 0xFFFFFFFFu; } return; }
-        // Last_Block flag
-        sm.scratch[0] = (k_in_frame == nb_frame - 1) ? 1u : 0u;
-    }
-    __syncwarp();
-    const uint32_t last_flag = sm.scratch[0];
+    const size_t fend = fstart + a.frame_size < a.n ? fstart + a.frame_size : a.n;
+    uint32_t nb_frame = (uint32_t)((fend - fstart + ZKC_BLOCK - 1) / ZKC_BLOCK); if (nb_frame == 0) nb_frame = 1;
+    if (k_in_frame >= nb_frame) { if (lane == 0) { a.blocks[b].csize = 0; a.blocks[b].lit_bytes = 0xFFFFFFFFu; } return; }
+    const uint32_t last_flag = k_in_frame == nb_frame - 1 ? 1u : 0u;
     const uint32_t nseq = a.blocks[b].nseq, nlit = a.blocks[b].nlit;
     const uint8_t* lits = a.lits + (size_t)b * ZKC_BLOCK;
     uint8_t* out = a.stage + (size_t)b * ZKC_SLOT;
@@ -629,45 +791,48 @@ __global__ void __launch_bounds__(32) zk_lit_enc_kernel(ZkEncodeArgs a) {
 
     // ------------------------------------------------------------------ literals section (A.3)
     if (!raw_block) {
-        for (int i = lane; i < 256; i += 32) { sm.hist4[0][i] = 0; sm.hist4[1][i] = 0; sm.hlen[i] = 0; }
-        __syncwarp();
-        {   // four literals per lane and load (the buffer is 32 KiB aligned); the stream a literal belongs to follows from its index
-            const uint32_t seg = (nlit + 3) / 4, n4 = nlit & ~3u;
-            for (uint32_t i = 4u * (uint32_t)lane; i < n4; i += 128) {
-                const uint32_t w = *(const uint32_t*)(lits + i);
+        int maxlen = 0; uint32_t lit_mode = 0;           // 0 raw, 1 rle, 2 huffman
+        if (!HUF) lit_mode = zkc_lits_rle(lits, nlit, lane) ? 1u : 0u;
+        else {
+            for (int i = lane; i < 256; i += 32) { sm.hist4[0][i] = 0; sm.hist4[1][i] = 0; sm.hlen[i] = 0; }
+            __syncwarp();
+            {   // four literals per lane and load (the buffer is 32 KiB aligned); the stream a literal belongs to follows from its index
+                const uint32_t seg = (nlit + 3) / 4, n4 = nlit & ~3u;
+                for (uint32_t i = 4u * (uint32_t)lane; i < n4; i += 128) {
+                    const uint32_t w = *(const uint32_t*)(lits + i);
 #pragma unroll
-                for (int q = 0; q < 4; q++) {
-                    const uint32_t idx = i + q, st = (idx >= seg) + (idx >= 2 * seg) + (idx >= 3 * seg);
-                    atomicAdd(&sm.hist4[st >> 1][(w >> (8 * q)) & 255u], 1u << ((st & 1u) * 16u));
+                    for (int q = 0; q < 4; q++) {
+                        const uint32_t idx = i + q, st = (idx >= seg) + (idx >= 2 * seg) + (idx >= 3 * seg);
+                        atomicAdd(&sm.hist4[st >> 1][(w >> (8 * q)) & 255u], 1u << ((st & 1u) * 16u));
+                    }
+                }
+                if ((uint32_t)lane < nlit - n4) {
+                    const uint32_t idx = n4 + lane, st = (idx >= seg) + (idx >= 2 * seg) + (idx >= 3 * seg);
+                    atomicAdd(&sm.hist4[st >> 1][lits[idx]], 1u << ((st & 1u) * 16u));
                 }
             }
-            if ((uint32_t)lane < nlit - n4) {
-                const uint32_t idx = n4 + lane, st = (idx >= seg) + (idx >= 2 * seg) + (idx >= 3 * seg);
-                atomicAdd(&sm.hist4[st >> 1][lits[idx]], 1u << ((st & 1u) * 16u));
-            }
-        }
-        __syncwarp();
-        for (int i = lane; i < 256; i += 32) { const uint32_t a0 = sm.hist4[0][i], a1 = sm.hist4[1][i]; sm.hist[i] = (a0 & 0xFFFFu) + (a0 >> 16) + (a1 & 0xFFFFu) + (a1 >> 16); }
-        __syncwarp();
-        // decide: Raw / RLE / Huffman
-        int maxlen = 0; uint32_t lit_mode = 0;           // 0 raw, 1 rle, 2 huffman
-        uint32_t mx = 0;
-        for (int s = lane; s < 256; s += 32) mx = max(mx, sm.hist[s]);
-        for (int d = 16; d; d >>= 1) mx = max(mx, __shfl_xor_sync(0xFFFFFFFFu, mx, d));
-        if (nlit > 0 && mx == nlit && nlit >= 2) lit_mode = 1;
-        else if (nlit >= 64) {
-            maxlen = zkc_huf_build(sm, lane);
-            if (maxlen) {
-                uint32_t bits = 0;
-                for (int s = lane; s < 256; s += 32) bits += sm.hist[s] * sm.hlen[s];
-                for (int d = 16; d; d >>= 1) bits += __shfl_xor_sync(0xFFFFFFFFu, bits, d);
-                uint32_t est = (bits + 7) / 8 + 8 + 130;
-                if (est < nlit) lit_mode = 2;
+            __syncwarp();
+            for (int i = lane; i < 256; i += 32) { const uint32_t a0 = sm.hist4[0][i], a1 = sm.hist4[1][i]; sm.hist[i] = (a0 & 0xFFFFu) + (a0 >> 16) + (a1 & 0xFFFFu) + (a1 >> 16); }
+            __syncwarp();
+            // decide: Raw / RLE / Huffman
+            uint32_t mx = 0;
+            for (int s = lane; s < 256; s += 32) mx = max(mx, sm.hist[s]);
+            for (int d = 16; d; d >>= 1) mx = max(mx, __shfl_xor_sync(0xFFFFFFFFu, mx, d));
+            if (nlit > 0 && mx == nlit && nlit >= 2) lit_mode = 1;
+            else if (nlit >= 64) {
+                maxlen = zkc_huf_build(sm, lane);
+                if (maxlen) {
+                    uint32_t bits = 0;
+                    for (int s = lane; s < 256; s += 32) bits += sm.hist[s] * sm.hlen[s];
+                    for (int d = 16; d; d >>= 1) bits += __shfl_xor_sync(0xFFFFFFFFu, bits, d);
+                    uint32_t est = (bits + 7) / 8 + 8 + 130;
+                    if (est < nlit) lit_mode = 2;
+                }
             }
         }
 
         uint32_t tree_bytes = 0;
-        if (lit_mode == 2) {
+        if (HUF && lit_mode == 2) {
             // canonical codes exactly as the decoder lays out its table: weight ascending, symbol ascending (A.4)
             if (lane == 0) {
                 int last_sym = 255; while (last_sym > 0 && sm.hlen[last_sym] == 0) last_sym--;
@@ -723,7 +888,7 @@ __global__ void __launch_bounds__(32) zk_lit_enc_kernel(ZkEncodeArgs a) {
             if (!tree_bytes) lit_mode = 0;               // cannot describe the tree: raw literals
         }
 
-        if (lit_mode == 2) {
+        if (HUF && lit_mode == 2) {
             // stream sizes first (so the section header, which precedes the streams, can be sized)
             const uint32_t seg = (nlit + 3) / 4;
             uint32_t ssz[4];
@@ -846,7 +1011,7 @@ __global__ void __launch_bounds__(32) zk_lit_enc_kernel(ZkEncodeArgs a) {
             }
             opos += hsz;
             if (opos + nlit + 4 >= len + 3) raw_block = true;       // cannot win any more
-            else { for (uint32_t i = lane; i < nlit; i += 32) out[opos + i] = lits[i]; opos += nlit; }
+            else { zkc_warp_copy(out + opos, lits, nlit, lane); opos += nlit; }
         }
     }
 
@@ -1007,7 +1172,8 @@ __global__ void __launch_bounds__(128) zk_frame_gather_kernel(ZkEncodeArgs a) {
 
 struct ZkCsizeArgs {
     const uint8_t* src; size_t n;                    // the pass
-    uint32_t nb, V, target, level, checksum;
+    uint32_t nb, V, target, checksum;
+    int level;
     uint32_t end_closes;                             // the pass ends the input and the caller is done with it: the rest is the last frame
     uint32_t end_lazy;                               // the pass ends the input but more may follow: a frame that ends there stays open
     const ZkcBlock* vblocks;                         // V x nb: variant d of block i at [d * nb + i]
@@ -1210,6 +1376,8 @@ void zk_encode_ws_free(ZkEncodeWs* ws) {
 }
 
 static size_t zkc_align(size_t v) { return (v + 255) & ~(size_t)255; }
+// the level a caller asks for -> the one the kernels run: 0 is the default (3), levels below ZSTD_minCLevel() clamp to it
+static int zkc_level(int level) { return level == 0 ? 3 : (level < ZKC_MIN_LEVEL ? ZKC_MIN_LEVEL : level); }
 static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, const ZkEncodeArgs& a);
 
 int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t frame_size, int level,
@@ -1254,7 +1422,7 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     uint8_t* base = (uint8_t*)ws->buf;
     ZkEncodeArgs a;
     a.src = d_src; a.n = n; a.frame_size = frame_size; a.n_frames = n_frames; a.blocks_per_frame = bpf; a.n_blocks = (uint32_t)n_blocks;
-    a.level = level <= 0 ? 3 : level; a.checksum = checksum ? 1 : 0;
+    a.level = zkc_level(level); a.checksum = checksum ? 1 : 0;
     a.blocks = (ZkcBlock*)(base + o_blocks);
     a.seq_ll = (uint16_t*)(base + o_ll); a.seq_ml = (uint16_t*)(base + o_ml); a.seq_off = (uint32_t*)(base + o_off);
     a.lits = base + o_lits; a.stage = base + o_stage; a.seqsec = base + o_seqsec;
@@ -1307,8 +1475,10 @@ static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, 
     // six tiers (EncodeOptions::compression_level, encode.rs:176): 1 = 2048-entry table, no history, no lazy step; 2-3 = 4096 entries,
     // previous-block history, one lazy step; 4-6 = double table (8-byte + 5-byte hashes, 4096 entries each), two warps per CTA; 7-9 = double
     // table of 8192 entries each, one warp per CTA; 10-12 = one table of 16384 entries, one warp per CTA; >= 13 = 256 KiB history, 32768 x u32
-    // entries in dynamic shared memory.  Ratio on the reference's corpus: 2.12 / 2.24 / 2.28 / 2.38 / 2.40 / 2.50
-    if (a.level <= 1) ZK_LAUNCH((zk_match_kernel<ZKC_HLOG_FAST, ZKC_C1_WARPS, false>), (uint32_t)((n_blocks + ZKC_C1_WARPS - 1) / ZKC_C1_WARPS), ZKC_C1_WARPS * 32, 0, stream, a);
+    // entries in dynamic shared memory.  Ratio on the reference's corpus: 2.12 / 2.24 / 2.28 / 2.38 / 2.40 / 2.50.  Below them the fast tier
+    // (level < 0): level 1's table with sparse probing, literals without Huffman coding
+    if (a.level < 0) ZK_LAUNCH((zk_match_fast_kernel<ZKC_HLOG_FAST, ZKC_C1_WARPS>), (uint32_t)((n_blocks + ZKC_C1_WARPS - 1) / ZKC_C1_WARPS), ZKC_C1_WARPS * 32, 0, stream, a);
+    else if (a.level <= 1) ZK_LAUNCH((zk_match_kernel<ZKC_HLOG_FAST, ZKC_C1_WARPS, false>), (uint32_t)((n_blocks + ZKC_C1_WARPS - 1) / ZKC_C1_WARPS), ZKC_C1_WARPS * 32, 0, stream, a);
     else if (a.level <= 3) ZK_LAUNCH((zk_match_kernel<ZKC_HLOG, ZKC_C1_WARPS, false>), (uint32_t)((n_blocks + ZKC_C1_WARPS - 1) / ZKC_C1_WARPS), ZKC_C1_WARPS * 32, 0, stream, a);
     else if (a.level <= 6) ZK_LAUNCH((zk_match_kernel<ZKC_HLOG, 2, true>), (uint32_t)((n_blocks + 1) / 2), 64, 0, stream, a);
     else if (a.level <= 9) ZK_LAUNCH((zk_match_kernel<13, 1, true>), (uint32_t)n_blocks, 32, 0, stream, a);
@@ -1326,7 +1496,8 @@ static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, 
     if (ss != stream) { ZKC_CUDA_OK(cudaEventRecord(ws->ev_a, stream)); ZKC_CUDA_OK(cudaStreamWaitEvent(ss, ws->ev_a, 0)); }
     ZK_LAUNCH(zk_seq_enc_kernel, (uint32_t)((n_blocks + ZKC_SW - 1) / ZKC_SW), 32 * ZKC_SW, seq_smem, ss, a);
     if (ss != stream) ZKC_CUDA_OK(cudaEventRecord(ws->ev_b, ss));
-    ZK_LAUNCH(zk_lit_enc_kernel, (uint32_t)n_blocks, 32, 0, stream, a);
+    if (a.level < 0) ZK_LAUNCH(zk_lit_enc_kernel<false>, (uint32_t)n_blocks, 32, 0, stream, a);
+    else ZK_LAUNCH(zk_lit_enc_kernel<true>, (uint32_t)n_blocks, 32, 0, stream, a);
     if (ss != stream) ZKC_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_b, 0));
     ZK_LAUNCH(zk_block_finish_kernel, (uint32_t)((n_blocks + 3) / 4), 128, 0, stream, a);
     ws->prof.end(6, stream);
@@ -1366,7 +1537,7 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     *out = ZkCsizeOut();
     if (n == 0) return 0;
     if (n > 0x40000000u) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
-    const int lvl = level <= 0 ? 3 : level;
+    const int lvl = zkc_level(level);
     const uint32_t nb = (uint32_t)((n + ZKC_BLOCK - 1) / ZKC_BLOCK);
     const uint32_t V = lvl >= ZKC_WIDE_LEVEL ? ZKC_WIDE_HIST + 1 : 2;
     const bool pfx = d_prefix && prefix_len;
@@ -1403,7 +1574,7 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     }
     uint8_t* base = (uint8_t*)ws->buf;
     ZkCsizeArgs c;
-    c.src = d_src; c.n = n; c.nb = nb; c.V = V; c.target = target ? target : 1; c.level = (uint32_t)lvl; c.checksum = checksum ? 1 : 0;
+    c.src = d_src; c.n = n; c.nb = nb; c.V = V; c.target = target ? target : 1; c.level = lvl; c.checksum = checksum ? 1 : 0;
     c.end_closes = at_end && final_; c.end_lazy = at_end && !final_;
     c.vblocks = (const ZkcBlock*)(base + o_blocks); c.vstage = base + o_stage;
     c.psum = (unsigned long long*)(base + o_psum); c.next = (uint32_t*)(base + o_next);
