@@ -9,7 +9,7 @@
 //   K-C1 zk_match_kernel<HLOG> one warp / block : LZ77 match finding (hash table in shared memory), greedy parse resolved
 //                                               with ballots, repeat-offset codes, sequences + literals written per window
 //   K-C2s zk_seq_enc_kernel  one warp / block : FSE sequences (three lanes run the state chains, 32 lanes pack the bits)
-//   K-C2l zk_lit_enc_kernel  one warp / block : Huffman literals (tree build, FSE-coded weights, 4 streams packed by warp scan)
+//   K-C2l zk_lit_enc_kernel  one warp / block : Huffman literals (tree build, FSE-coded weights, 4 streams packed by warp scan), 4 warps / CTA
 //   K-C2f zk_block_finish_kernel              : joins the two sections of a block (coded on two streams), Raw fallback, header
 //   K-C3 zk_frame_{hash,size,scan,gather}_kernel : optional XXH64, frame sizes, offsets, frame headers + block gather
 //
@@ -381,10 +381,9 @@ __device__ void zkc_fse_normalize(ZkcFse& t, const CT* cnt, int nsym, uint32_t t
     t.log = (int8_t)log; t.nsym = (uint8_t)nsym;
 }
 
-// build the encoding tables from t.norm (mirror of A.6 table build)
-__device__ void zkc_fse_build(ZkcFse& t, uint8_t* symof /* >= 512 bytes scratch */) {
+// build the encoding tables from t.norm (mirror of A.6 table build); symof: 2^log bytes of scratch, cumul: nsym + 1 entries
+__device__ __forceinline__ void zkc_fse_build_in(ZkcFse& t, uint8_t* symof, uint16_t* cumul) {
     const int log = t.log, S = 1 << log, nsym = t.nsym;
-    uint16_t cumul[65];
     int high = S - 1;
     cumul[0] = 0;
     for (int s = 0; s < nsym; s++) {
@@ -408,6 +407,7 @@ __device__ void zkc_fse_build(ZkcFse& t, uint8_t* symof /* >= 512 bytes scratch 
         }
     }
 }
+__device__ void zkc_fse_build(ZkcFse& t, uint8_t* symof /* >= 512 bytes scratch */) { uint16_t cumul[65]; zkc_fse_build_in(t, symof, cumul); }
 
 // write the normalised-count header (A.6); returns bytes written (0 on overflow)
 __device__ uint32_t zkc_fse_write_ncount(const ZkcFse& t, uint8_t* out, uint32_t cap) {
@@ -677,84 +677,112 @@ __global__ void __launch_bounds__(32 * ZKC_SW) zk_seq_enc_kernel(ZkEncodeArgs a)
     if (lane == 0) { a.blocks[b].seq_hdr = hb; a.blocks[b].seq_bits = sb; }
 }
 
-#define ZKC_BITBUF 6144u                // shared-memory scratch: Huffman build arrays, then one Huffman stream (longer streams are packed in tiles)
+#define ZKC_LW 4                        // K-C2l warps per CTA, one block each
+#define ZKC_LWIN 48u                    // stream packing window in words: the carried partial word + one 128-symbol tile (<= 1408 bits) + 2
 
-// per-warp shared state of K-C2l.  The three phases (tree build, tree description, stream packing) never overlap, so
-// their scratch shares one union: 10 KiB per warp instead of 18 -- the kernel is latency-bound and shared memory was
-// what limited the warps per SM.
-struct ZkcC2Smem {
-    uint32_t hist[256];
-    uint32_t hist4[2][256];             // per-stream counts, two 16-bit fields per word (streams 0|1, 2|3): stream sizes without a second pass over the literals
-    uint16_t hcode[256]; uint8_t hlen[256];      // hcode: (length << 11) | code
+// per-warp shared state of K-C2l (4 KiB).  The phases (tree build + code lengths and codes, weight coding, stream packing)
+// never overlap, so their scratch shares one union; with four warps per CTA, registers rather than shared memory set the
+// warps per SM of this latency-bound kernel.
+struct ZkcLitWarp {
+    uint32_t hist4[2][256];             // per-stream counts, two 16-bit fields per word (streams 0|1, 2|3); a symbol's count is their sum
+    uint16_t hcode[256];                // (length << 11) | code; 0: symbol absent
     union {
-        uint8_t bitbuf[ZKC_BITBUF];
-        struct { ZkcFse fse; uint8_t symof[512]; uint8_t weights[256]; } w;    // FSE coding of the Huffman weights
+        struct { uint16_t node[511]; uint32_t num[33]; uint32_t cls[16]; } t;      // tree (weights -> parents -> depths), lengths, code cursors
+        struct { ZkcFse fse; uint8_t symof[64]; uint8_t weights[256]; uint32_t wc[16]; uint16_t cumul[16]; } w;    // FSE coding of the weights
+        uint32_t win[ZKC_LWIN];         // stream packing: [0] carries the partial word of the previous tile
     } u;
-    uint8_t hdr[256];                   // literal header + tree description
-    uint32_t scratch[16];
+    uint8_t hdr[128];                   // tree description
 };
 
-// Huffman code lengths limited to 11 bits.  Whole warp: the symbols are ranked by count with an all-pairs comparison
-// in shared memory (each lane ranks 8 symbols), then lane 0 runs the two-queue tree build on shared-memory arrays
-// (aliasing the bit buffer, which is not in use yet).  Returns max code length (0 = fewer than two symbols).
-__device__ int zkc_huf_build(ZkcC2Smem& sm, int lane) {
-    uint16_t* order = (uint16_t*)sm.u.bitbuf;                 // 256 x u16   symbols sorted by count ascending
-    uint32_t* weight = (uint32_t*)(sm.u.bitbuf + 512);        // 511 x u32
-    uint16_t* parent = (uint16_t*)(sm.u.bitbuf + 512 + 2048); // 511 x u16
-    uint8_t* depth = sm.u.bitbuf + 512 + 2048 + 1024;         // 511 x u8
+// Huffman code lengths limited to 11 bits, into sm.hcode (length << 11).  Whole warp: the present symbols are ranked by
+// (count, symbol) with a bitonic sort of the keys (count << 8) | symbol, eight per lane in registers; lane 0 runs the
+// two-queue tree build in one array (a consumed node's slot takes its parent, then the depths replace the parents in
+// place); the warp turns depths into limited lengths.  Returns max code length (0 = fewer than two symbols).
+__device__ int zkc_huf_build(ZkcLitWarp& sm, int lane) {
+    uint32_t key[8];
     int n = 0;
-    for (int s0 = 0; s0 < 256; s0 += 32) n += __popc(__ballot_sync(0xFFFFFFFFu, sm.hist[s0 + lane] != 0));
+#pragma unroll
+    for (int r = 0; r < 8; r++) {
+        const uint32_t s = 32u * r + (uint32_t)lane, a0 = sm.hist4[0][s], a1 = sm.hist4[1][s];
+        const uint32_t c = (a0 & 0xFFFFu) + (a0 >> 16) + (a1 & 0xFFFFu) + (a1 >> 16);
+        key[r] = (c << 8) | s;
+        n += __popc(__ballot_sync(0xFFFFFFFFu, c != 0));
+    }
     if (n < 2) return 0;
-    // compact the present symbols (ascending), then rank them among themselves: n^2 / 32 comparisons per lane instead of 256 * 8
-    uint32_t* pcnt = (uint32_t*)(sm.u.bitbuf + 4608);         // n x u32
-    uint8_t* psym = sm.u.bitbuf + 4608 + 1024;                // n x u8
-    {
-        int basep = 0;
-        for (int s0 = 0; s0 < 256; s0 += 32) {
-            const uint32_t c = sm.hist[s0 + lane];
-            const uint32_t m = __ballot_sync(0xFFFFFFFFu, c != 0);
-            if (c) { const int k = basep + __popc(m & ((1u << lane) - 1u)); pcnt[k] = c; psym[k] = (uint8_t)(s0 + lane); }
-            basep += __popc(m);
+    // ascending over e = 8 * lane + r: strides of 8 and more are lane shuffles, smaller ones stay in the lane
+#pragma unroll
+    for (int ks = 1; ks <= 8; ks++) {
+#pragma unroll
+        for (int js = ks - 1; js >= 0; js--) {
+            if (js >= 3) {
+                const int lj = 1 << (js - 3);
+                const bool upper = (lane & lj) != 0, desc = ((lane >> (ks - 3)) & 1) != 0;
+#pragma unroll
+                for (int r = 0; r < 8; r++) {
+                    const uint32_t o = __shfl_xor_sync(0xFFFFFFFFu, key[r], lj);
+                    key[r] = upper != desc ? max(key[r], o) : min(key[r], o);
+                }
+            } else {
+#pragma unroll
+                for (int r = 0; r < 8; r++) {
+                    if (r & (1 << js)) continue;
+                    const int p = r | (1 << js);
+                    const bool desc = (((8 * lane + r) >> ks) & 1) != 0;
+                    const uint32_t lo = min(key[r], key[p]), hi = max(key[r], key[p]);
+                    key[r] = desc ? hi : lo; key[p] = desc ? lo : hi;
+                }
+            }
         }
     }
-    __syncwarp();
-    for (int k = lane; k < n; k += 32) {
-        const uint32_t c = pcnt[k];
-        int rank = 0;
-        for (int j = 0; j < n; j++) { const uint32_t cj = pcnt[j]; rank += (cj < c || (cj == c && j < k)); }
-        order[rank] = (uint16_t)psym[k];
-    }
+    // the present symbols are the top n keys: rank k = e - (256 - n)
+    uint16_t* node = sm.u.t.node;                             // leaves 0..n-1 (sorted), internal nodes n..2n-2
+    uint32_t* num = sm.u.t.num;
+    const int off = 256 - n;
+#pragma unroll
+    for (int r = 0; r < 8; r++) { const int k = 8 * lane + r - off; if (k >= 0) node[k] = (uint16_t)(key[r] >> 8); }
+    for (int i = lane; i <= 32; i += 32) num[i] = 0;
     __syncwarp();
     if (lane == 0) {
-        for (int i = 0; i < n; i++) weight[i] = sm.hist[order[i]];
         int leaf = 0, inode = n, next = n;
-        for (int k = 0; k < n - 1; k++) {       // two-queue Huffman: leaves 0..n-1 (sorted), internal nodes n..2n-2
+        for (int k = 0; k < n - 1; k++) {       // weights fit 16 bits: they sum to at most ZKC_BLOCK
             int a, b;
-            if (leaf < n && (inode >= next || weight[leaf] <= weight[inode])) a = leaf++; else a = inode++;
-            if (leaf < n && (inode >= next || weight[leaf] <= weight[inode])) b = leaf++; else b = inode++;
-            weight[next] = weight[a] + weight[b]; parent[a] = (uint16_t)next; parent[b] = (uint16_t)next; next++;
+            if (leaf < n && (inode >= next || node[leaf] <= node[inode])) a = leaf++; else a = inode++;
+            if (leaf < n && (inode >= next || node[leaf] <= node[inode])) b = leaf++; else b = inode++;
+            const uint32_t w = (uint32_t)node[a] + node[b];
+            node[a] = (uint16_t)next; node[b] = (uint16_t)next; node[next] = (uint16_t)w; next++;
         }
-        depth[next - 1] = 0;
-        for (int i = next - 2; i >= 0; i--) depth[i] = (uint8_t)(depth[parent[i]] + 1);
-        // histogram of code lengths, limited to 11 (miniz-style redistribution keeps the code complete)
-        const int L = 11;
-        int num[33]; for (int i = 0; i <= 32; i++) num[i] = 0;
-        for (int i = 0; i < n; i++) num[depth[i] > 32 ? 32 : depth[i]]++;
-        for (int i = L + 1; i <= 32; i++) { num[L] += num[i]; num[i] = 0; }
+        node[next - 1] = 0;
+        for (int i = next - 2; i >= 0; i--) node[i] = (uint16_t)(node[node[i]] + 1);
+    }
+    __syncwarp();
+    // histogram of code lengths, limited to 11 (miniz-style redistribution keeps the code complete)
+    const int L = 11;
+    for (int i = lane; i < n; i += 32) { const uint32_t d = node[i]; atomicAdd(&num[d < (uint32_t)L ? d : (uint32_t)L], 1u); }
+    __syncwarp();
+    if (lane == 0) {
         unsigned total = 0;
-        for (int i = L; i > 0; i--) total += (unsigned)num[i] << (L - i);
+        for (int i = L; i > 0; i--) total += num[i] << (L - i);
         while (total != (1u << L)) {
             num[L]--;
             for (int i = L - 1; i > 0; i--) if (num[i]) { num[i]--; num[i + 1] += 2; break; }
             total--;
         }
-        // most frequent symbols (end of `order`) get the shortest codes
-        int idx = n - 1, maxlen = 0;
-        for (int l = 1; l <= L; l++) for (int k = 0; k < num[l]; k++) { sm.hlen[order[idx--]] = (uint8_t)l; maxlen = l; }
-        sm.scratch[2] = (uint32_t)maxlen;
     }
     __syncwarp();
-    return (int)sm.scratch[2];
+    // most frequent symbols (top ranks) get the shortest codes: rank k from the top takes the length whose class holds it
+    int maxlen = L; while (!num[maxlen]) maxlen--;
+#pragma unroll
+    for (int r = 0; r < 8; r++) {
+        const int k = 8 * lane + r - off;
+        if (k >= 0) {
+            const uint32_t p = (uint32_t)(n - 1 - k);
+            uint32_t l = 1, c = num[1];
+            while (p >= c) c += num[++l];
+            sm.hcode[key[r] & 255u] = (uint16_t)(l << 11);
+        }
+    }
+    __syncwarp();
+    return maxlen;
 }
 
 // are all n >= 2 literals the same byte?  4-byte words (the buffer is 32 KiB aligned); most blocks settle in the first round
@@ -768,12 +796,15 @@ __device__ __forceinline__ bool zkc_lits_rle(const uint8_t* lits, uint32_t n, in
     return __all_sync(0xFFFFFFFFu, (uint32_t)lane >= n - n4 || lits[n4 + lane] == lits[0]) && rle;
 }
 
-// HUF = false (the fast tier): literals are only ever Raw or RLE, decided without a histogram
-template <bool HUF>
-__global__ void __launch_bounds__(32) zk_lit_enc_kernel(ZkEncodeArgs a) {
-    __shared__ ZkcC2Smem sm;
-    const int lane = threadIdx.x;
-    const uint32_t b = blockIdx.x;
+// HUF = false (the fast tier): literals are only ever Raw or RLE, decided without a histogram or shared memory.
+// NW warps per CTA, one block per warp (64 registers at most with HUF, so that 32 warps fit an SM).
+template <bool HUF, int NW>
+__global__ void __launch_bounds__(32 * NW, HUF ? 32 / NW : 1) zk_lit_enc_kernel(ZkEncodeArgs a) {
+    __shared__ ZkcLitWarp sms[HUF ? NW : 1];
+    const int lane = threadIdx.x & 31;
+    const uint32_t b = blockIdx.x * NW + (threadIdx.x >> 5);
+    if (b >= a.n_blocks) return;
+    ZkcLitWarp& sm = sms[HUF ? threadIdx.x >> 5 : 0];
     size_t lo, hi, fstart;
     zkc_block_range(a, b, lo, hi, fstart);
     const uint32_t len = (uint32_t)(hi - lo);
@@ -783,7 +814,7 @@ __global__ void __launch_bounds__(32) zk_lit_enc_kernel(ZkEncodeArgs a) {
     uint32_t nb_frame = (uint32_t)((fend - fstart + ZKC_BLOCK - 1) / ZKC_BLOCK); if (nb_frame == 0) nb_frame = 1;
     if (k_in_frame >= nb_frame) { if (lane == 0) { a.blocks[b].csize = 0; a.blocks[b].lit_bytes = 0xFFFFFFFFu; } return; }
     const uint32_t last_flag = k_in_frame == nb_frame - 1 ? 1u : 0u;
-    const uint32_t nseq = a.blocks[b].nseq, nlit = a.blocks[b].nlit;
+    const uint32_t nlit = a.blocks[b].nlit;
     const uint8_t* lits = a.lits + (size_t)b * ZKC_BLOCK;
     uint8_t* out = a.stage + (size_t)b * ZKC_SLOT;
     uint32_t opos = 3;                                   // block header written last
@@ -794,7 +825,7 @@ __global__ void __launch_bounds__(32) zk_lit_enc_kernel(ZkEncodeArgs a) {
         int maxlen = 0; uint32_t lit_mode = 0;           // 0 raw, 1 rle, 2 huffman
         if (!HUF) lit_mode = zkc_lits_rle(lits, nlit, lane) ? 1u : 0u;
         else {
-            for (int i = lane; i < 256; i += 32) { sm.hist4[0][i] = 0; sm.hist4[1][i] = 0; sm.hlen[i] = 0; }
+            for (int i = lane; i < 256; i += 32) { sm.hist4[0][i] = 0; sm.hist4[1][i] = 0; sm.hcode[i] = 0; }
             __syncwarp();
             {   // four literals per lane and load (the buffer is 32 KiB aligned); the stream a literal belongs to follows from its index
                 const uint32_t seg = (nlit + 3) / 4, n4 = nlit & ~3u;
@@ -812,18 +843,22 @@ __global__ void __launch_bounds__(32) zk_lit_enc_kernel(ZkEncodeArgs a) {
                 }
             }
             __syncwarp();
-            for (int i = lane; i < 256; i += 32) { const uint32_t a0 = sm.hist4[0][i], a1 = sm.hist4[1][i]; sm.hist[i] = (a0 & 0xFFFFu) + (a0 >> 16) + (a1 & 0xFFFFu) + (a1 >> 16); }
-            __syncwarp();
             // decide: Raw / RLE / Huffman
             uint32_t mx = 0;
-            for (int s = lane; s < 256; s += 32) mx = max(mx, sm.hist[s]);
+            for (int s = lane; s < 256; s += 32) {
+                const uint32_t a0 = sm.hist4[0][s], a1 = sm.hist4[1][s];
+                mx = max(mx, (a0 & 0xFFFFu) + (a0 >> 16) + (a1 & 0xFFFFu) + (a1 >> 16));
+            }
             for (int d = 16; d; d >>= 1) mx = max(mx, __shfl_xor_sync(0xFFFFFFFFu, mx, d));
             if (nlit > 0 && mx == nlit && nlit >= 2) lit_mode = 1;
             else if (nlit >= 64) {
                 maxlen = zkc_huf_build(sm, lane);
                 if (maxlen) {
                     uint32_t bits = 0;
-                    for (int s = lane; s < 256; s += 32) bits += sm.hist[s] * sm.hlen[s];
+                    for (int s = lane; s < 256; s += 32) {
+                        const uint32_t a0 = sm.hist4[0][s], a1 = sm.hist4[1][s];
+                        bits += ((a0 & 0xFFFFu) + (a0 >> 16) + (a1 & 0xFFFFu) + (a1 >> 16)) * (uint32_t)(sm.hcode[s] >> 11);
+                    }
                     for (int d = 16; d; d >>= 1) bits += __shfl_xor_sync(0xFFFFFFFFu, bits, d);
                     uint32_t est = (bits + 7) / 8 + 8 + 130;
                     if (est < nlit) lit_mode = 2;
@@ -833,32 +868,54 @@ __global__ void __launch_bounds__(32) zk_lit_enc_kernel(ZkEncodeArgs a) {
 
         uint32_t tree_bytes = 0;
         if (HUF && lit_mode == 2) {
-            // canonical codes exactly as the decoder lays out its table: weight ascending, symbol ascending (A.4)
+            // canonical codes exactly as the decoder lays out its table: weight ascending, symbol ascending (A.4).  A symbol's
+            // code is its class's start cell (lane w scans the cells of the classes below w) plus its rank among the class's
+            // earlier symbols (a match over each 32 symbols, then the class cursor moves on)
+            int last_sym = 0;
+            for (int s0 = 224; s0 >= 0; s0 -= 32) {
+                const uint32_t m = __ballot_sync(0xFFFFFFFFu, sm.hcode[s0 + lane] != 0);
+                if (m) { last_sym = s0 + 31 - __clz((int)m); break; }
+            }
+            uint32_t* cls = sm.u.t.cls;
+            {
+                const bool in = lane >= 1 && lane <= maxlen;
+                const uint32_t v = in ? sm.u.t.num[maxlen + 1 - lane] << (lane - 1) : 0u;
+                uint32_t incl = v;
+                for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += t; }
+                if (in) cls[lane] = incl - v;
+            }
+            __syncwarp();
+            for (int s0 = 0; s0 <= last_sym; s0 += 32) {
+                const uint32_t l = sm.hcode[s0 + lane] >> 11;
+                const int w = l ? maxlen + 1 - (int)l : 0;
+                const uint32_t m = __match_any_sync(0xFFFFFFFFu, (uint32_t)w), below = m & ((1u << lane) - 1u);
+                if (l) sm.hcode[s0 + lane] = (uint16_t)(((cls[w] >> (w - 1)) + (uint32_t)__popc(below)) | (l << 11));
+                __syncwarp();
+                if (l && !below) cls[w] += (uint32_t)__popc(m) << (w - 1);
+                __syncwarp();
+            }
+            // tree description: weights of symbols 0..last_sym-1 (the last one is implied)
+            const int nw = last_sym;
+            if (lane < 16) sm.u.w.wc[lane] = 0;
+            __syncwarp();
+            int maxw = 0;
+            for (int s = lane; s < nw; s += 32) {
+                const int l = sm.hcode[s] >> 11, wt = l ? maxlen + 1 - l : 0;
+                sm.u.w.weights[s] = (uint8_t)wt; atomicAdd(&sm.u.w.wc[wt], 1u); maxw = max(maxw, wt);
+            }
+            for (int d = 16; d; d >>= 1) maxw = max(maxw, __shfl_xor_sync(0xFFFFFFFFu, maxw, d));
+            __syncwarp();
+            uint32_t tb = 0;
             if (lane == 0) {
-                int last_sym = 255; while (last_sym > 0 && sm.hlen[last_sym] == 0) last_sym--;
-                // start cell of every symbol in two linear passes: cells per weight class, then a running cursor per class
-                uint32_t cls[13];
-                for (int w = 0; w < 13; w++) cls[w] = 0;
-                for (int s = 0; s <= last_sym; s++) if (sm.hlen[s]) cls[maxlen + 1 - sm.hlen[s]] += 1;
-                { uint32_t acc = 0; for (int w = 1; w <= maxlen; w++) { uint32_t n = cls[w]; cls[w] = acc; acc += n << (w - 1); } }
-                for (int s = 0; s <= last_sym; s++)
-                    if (sm.hlen[s]) { const int w = maxlen + 1 - sm.hlen[s]; sm.hcode[s] = (uint16_t)((cls[w] >> (w - 1)) | ((uint32_t)sm.hlen[s] << 11)); cls[w] += 1u << (w - 1); }
-                // tree description: weights of symbols 0..last_sym-1 (the last one is implied)
-                int nw = last_sym;
-                for (int s = 0; s < nw; s++) sm.u.w.weights[s] = sm.hlen[s] ? (uint8_t)(maxlen + 1 - sm.hlen[s]) : 0;
-                uint32_t tb = 0;
                 // FSE-compressed weights (two interleaved states), A.4
                 if (nw > 1) {
-                    uint32_t wc[16]; for (int i = 0; i < 16; i++) wc[i] = 0;
-                    int maxw = 0;
-                    for (int s = 0; s < nw; s++) { wc[sm.u.w.weights[s]]++; if (sm.u.w.weights[s] > maxw) maxw = sm.u.w.weights[s]; }
-                    uint32_t distinct = 0; for (int i = 0; i <= maxw; i++) distinct += wc[i] != 0;
+                    uint32_t distinct = 0; for (int i = 0; i <= maxw; i++) distinct += sm.u.w.wc[i] != 0;
                     if (distinct > 1) {
                         ZkcFse& t = sm.u.w.fse;
                         int lg = 6; while (lg > 5 && (1 << lg) > nw) lg--;        // table log 5..6
-                        zkc_fse_normalize(t, wc, maxw + 1, (uint32_t)nw, lg);
+                        zkc_fse_normalize(t, sm.u.w.wc, maxw + 1, (uint32_t)nw, lg);
                         t.mode = 2;
-                        zkc_fse_build(t, sm.u.w.symof);
+                        zkc_fse_build_in(t, sm.u.w.symof, sm.u.w.cumul);
                         uint32_t hb = zkc_fse_write_ncount(t, sm.hdr + 1, 120);
                         if (hb) {
                             ZkcBitW w; w.init(sm.hdr + 1 + hb, 127 - hb);
@@ -881,10 +938,8 @@ __global__ void __launch_bounds__(32) zk_lit_enc_kernel(ZkEncodeArgs a) {
                         tb = 1 + (uint32_t)(nw + 1) / 2;
                     }
                 }
-                sm.scratch[3] = tb;
             }
-            __syncwarp();
-            tree_bytes = sm.scratch[3];
+            tree_bytes = __shfl_sync(0xFFFFFFFFu, tb, 0);
             if (!tree_bytes) lit_mode = 0;               // cannot describe the tree: raw literals
         }
 
@@ -895,7 +950,7 @@ __global__ void __launch_bounds__(32) zk_lit_enc_kernel(ZkEncodeArgs a) {
             {
                 uint32_t b0 = 0, b1 = 0, b2 = 0, b3 = 0;
                 for (int sy = lane; sy < 256; sy += 32) {
-                    const uint32_t l = sm.hlen[sy], a0 = sm.hist4[0][sy], a1 = sm.hist4[1][sy];
+                    const uint32_t l = sm.hcode[sy] >> 11, a0 = sm.hist4[0][sy], a1 = sm.hist4[1][sy];
                     b0 += (a0 & 0xFFFFu) * l; b1 += (a0 >> 16) * l; b2 += (a1 & 0xFFFFu) * l; b3 += (a1 >> 16) * l;
                 }
                 for (int d = 16; d; d >>= 1) {
@@ -922,18 +977,19 @@ __global__ void __launch_bounds__(32) zk_lit_enc_kernel(ZkEncodeArgs a) {
                                  out[opos + 4] = (uint8_t)ssz[2]; out[opos + 5] = (uint8_t)(ssz[2] >> 8); }
                 opos += 6;
                 // encode each stream: symbol i of the stream sits above all later symbols (the decoder reads backward),
-                // so its bit position is the sum of the code lengths of the symbols after it -> warp scan over reversed order
-                __syncwarp();                                         // the tree description has left the union
+                // so its bit position is the sum of the code lengths of the symbols after it -> warp scan over reversed order.
+                // Every stream goes through the window as whole words of the staging slot (the slot is 4-byte aligned), flushed
+                // after each 128 symbols; its first word starts with the bytes before the stream, read back from the slot.
+                // The last word may run up to 3 bytes past the stream: the next stream or K-C2f writes over them.
+                __syncwarp();                                         // the tree description has left the union; the bytes above are in the slot
+                uint32_t* const win = sm.u.win;
                 for (int st = 0; st < 4; st++) {
                     const uint32_t s0 = st * seg, s1 = st < 3 ? s0 + seg : nlit, m = s1 - s0;
-                    uint32_t* wbuf = (uint32_t*)sm.u.bitbuf;
-                    // a stream that fits the buffer is packed there and copied out once; a longer one goes through a 48-word
-                    // window whose full words are flushed after every 128 symbols
-                    const bool whole = ssz[st] + 8 <= ZKC_BITBUF;
-                    const uint32_t words = whole ? (ssz[st] + 3) / 4 : 64u;
-                    for (uint32_t i = lane; i < words; i += 32) wbuf[i] = 0;
+                    const uint32_t pre = opos & 3u;
+                    uint32_t* const gw = (uint32_t*)(out + (opos - pre));
+                    for (uint32_t i = lane; i < ZKC_LWIN; i += 32) win[i] = (i == 0 && pre) ? gw[0] & ((1u << (8u * pre)) - 1u) : 0u;
                     __syncwarp();
-                    uint32_t base = 0;                                // bits of the stream emitted so far
+                    uint32_t base = 8u * pre;                         // bit position in gw
                     for (uint32_t g = 0; g < m; g += 128) {
                         // four symbols per lane (reversed indices r .. r+3, r lowest in the stream): one scan and at most
                         // three atomics serve 128 symbols
@@ -956,37 +1012,26 @@ __global__ void __launch_bounds__(32) zk_lit_enc_kernel(ZkEncodeArgs a) {
                         }
                         uint32_t incl = l;
                         for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += t; }
-                        const uint32_t org = whole ? base : (base & 31u);     // bit position of the tile inside wbuf
+                        const uint32_t org = base & 31u;                  // bit position of the tile inside win
                         const uint32_t bitpos = org + incl - l;
                         if (l) {
                             const uint32_t sh = bitpos & 31u, w = bitpos >> 5;
                             const unsigned long long lo2 = v << sh;
-                            atomicOr(&wbuf[w], (uint32_t)lo2);
-                            if (lo2 >> 32) atomicOr(&wbuf[w + 1], (uint32_t)(lo2 >> 32));
-                            if (sh) { const uint32_t hi2 = (uint32_t)(v >> (64u - sh)); if (hi2) atomicOr(&wbuf[w + 2], hi2); }
+                            atomicOr(&win[w], (uint32_t)lo2);
+                            if (lo2 >> 32) atomicOr(&win[w + 1], (uint32_t)(lo2 >> 32));
+                            if (sh) { const uint32_t hi2 = (uint32_t)(v >> (64u - sh)); if (hi2) atomicOr(&win[w + 2], hi2); }
                         }
                         const uint32_t tile_bits = __shfl_sync(0xFFFFFFFFu, incl, 31);
-                        if (!whole) {
-                            __syncwarp();
-                            const uint32_t nwords = (org + tile_bits) >> 5, byte0 = (base >> 5) * 4u;
-                            for (uint32_t i = lane; i < nwords * 4u; i += 32) out[opos + byte0 + i] = sm.u.bitbuf[i];
-                            const uint32_t carry = wbuf[nwords];
-                            __syncwarp();
-                            for (uint32_t i = lane; i <= nwords + 2; i += 32) wbuf[i] = i == 0 ? carry : 0u;
-                            __syncwarp();
-                        }
+                        __syncwarp();
+                        const uint32_t nwords = (org + tile_bits) >> 5, word0 = base >> 5;
+                        for (uint32_t i = lane; i < nwords; i += 32) gw[word0 + i] = win[i];
+                        const uint32_t carry = win[nwords];
+                        __syncwarp();
+                        for (uint32_t i = lane; i <= nwords + 2; i += 32) win[i] = i == 0 ? carry : 0u;
+                        __syncwarp();
                         base += tile_bits;
                     }
-                    __syncwarp();
-                    if (whole) {
-                        if (lane == 0) atomicOr(&wbuf[base >> 5], 1u << (base & 31));   // end mark
-                        __syncwarp();
-                        for (uint32_t i = lane; i < ssz[st]; i += 32) out[opos + i] = sm.u.bitbuf[i];
-                    } else if (lane == 0) {
-                        const unsigned long long tail = (unsigned long long)wbuf[0] | (1ull << (base & 31u));
-                        const uint32_t byte0 = (base >> 5) * 4u;
-                        for (uint32_t i = 0; byte0 + i < ssz[st]; i++) out[opos + byte0 + i] = (uint8_t)(tail >> (8u * i));
-                    }
+                    if (lane == 0) gw[base >> 5] = win[0] | (1u << (base & 31u));   // the partial word and the end mark
                     opos += ssz[st];
                     __syncwarp();
                 }
@@ -1496,8 +1541,8 @@ static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, 
     if (ss != stream) { ZKC_CUDA_OK(cudaEventRecord(ws->ev_a, stream)); ZKC_CUDA_OK(cudaStreamWaitEvent(ss, ws->ev_a, 0)); }
     ZK_LAUNCH(zk_seq_enc_kernel, (uint32_t)((n_blocks + ZKC_SW - 1) / ZKC_SW), 32 * ZKC_SW, seq_smem, ss, a);
     if (ss != stream) ZKC_CUDA_OK(cudaEventRecord(ws->ev_b, ss));
-    if (a.level < 0) ZK_LAUNCH(zk_lit_enc_kernel<false>, (uint32_t)n_blocks, 32, 0, stream, a);
-    else ZK_LAUNCH(zk_lit_enc_kernel<true>, (uint32_t)n_blocks, 32, 0, stream, a);
+    if (a.level < 0) ZK_LAUNCH((zk_lit_enc_kernel<false, 1>), (uint32_t)n_blocks, 32, 0, stream, a);
+    else ZK_LAUNCH((zk_lit_enc_kernel<true, ZKC_LW>), (uint32_t)((n_blocks + ZKC_LW - 1) / ZKC_LW), 32 * ZKC_LW, 0, stream, a);
     if (ss != stream) ZKC_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_b, 0));
     ZK_LAUNCH(zk_block_finish_kernel, (uint32_t)((n_blocks + 3) / 4), 128, 0, stream, a);
     ws->prof.end(6, stream);
