@@ -705,32 +705,37 @@ __global__ void __launch_bounds__(32) zk_seq2_kernel(ZkDecodeArgs a) {
 // =============================================================================================
 // K-D1h: Huffman literal decode -- one LANE per Huffman stream (4 lanes per 4-stream block).
 // =============================================================================================
-#define ZK_HUF_SLOTS 8            // blocks per warp-CTA; 8 x 3.1 KiB -> 9 CTAs / SM
+#define ZK_HUF_SLOTS 8            // blocks per warp-CTA; 8 x 2 KiB of tables + 0.3 KiB of build scratch
 
 // Two-level decoding table.  Cells are laid out weight ascending (A.4), so the codes of the two longest lengths occupy
 // the first L <= 510 cells of the 2^maxBits index space, and everything above is replicated at least four times:
 //   idx < L  -> low[idx]        (full resolution)        idx >= L -> l1[idx >> 2]      (2^(maxBits-2) <= 512 entries)
-// 2 KiB instead of the flat 4 KiB table: the kernel is bound by memory latency with shared memory capping the streams
-// in flight, so the extra compare per symbol buys 1.7x the blocks per SM.
-struct ZkHufSlot {
-    uint16_t l1[512], low[512];                // (nbBits << 8) | symbol
-    uint32_t n_low;                            // L
-    uint8_t weights[256];
-    uint16_t hpos[256];
-    uint8_t wsym[64], wnb[64]; uint16_t wbase[64];   // FSE table for compressed weights (log <= 6)
-    int huf_bits, nw, st;
-    uint32_t tree_bytes;
+// 2 KiB instead of the flat 4 KiB table.  The kernel is bound by memory latency and runs beside K-D1s, so the shared
+// memory a block holds decides how many blocks and how many K-D1s chains fit on an SM: the table is all a block keeps
+// through its decode (L and maxBits live in registers).  Before the table is filled, the same memory holds the block's
+// weights, decoded by one lane per block with the eight blocks side by side.
+union ZkHufTab {
+    struct { uint16_t l1[512], low[512]; } t;  // (nbBits << 8) | symbol
+    struct {
+        uint8_t weights[256];                  // explicit weights, as the tree description gives them
+        uint8_t sym[64], nb[64]; uint16_t base[64];   // FSE table for compressed weights (log <= 6)
+    } w;
+};
+// Build scratch, one per warp: the warp ranks the weights and fills the tables one block after another.
+struct ZkHufScratch {
+    uint8_t sorted[256];                       // the symbols by (weight, symbol): the order of their cells
+    uint32_t cntw[16];                         // symbols per weight
 };
 
-// Huffman tree description -> sl.weights[0..nw) incl. the implied last weight (A.4).
-// Returns bytes consumed or 0 on corruption; sets sl.huf_bits / sl.nw.
-__device__ uint32_t zk_read_huf_weights(ZkHufSlot& sl, const uint8_t* p, uint32_t n) {
+// Huffman tree description -> hw.weights[0..*nw) without the implied last weight (A.4).  Serial (one lane per block).
+// Returns bytes consumed or 0 on corruption.
+__device__ uint32_t zk_read_huf_weights(ZkHufTab& hw, const uint8_t* p, uint32_t n, int* nw_out) {
     if (n < 1) return 0;
     uint32_t hb = p[0], used; int nw = 0;
     if (hb >= 128) {
         nw = (int)hb - 127; used = 1 + (uint32_t)(nw + 1) / 2;
         if (used > n) return 0;
-        for (int i = 0; i < nw; i++) { uint32_t b = p[1 + i / 2]; sl.weights[i] = (uint8_t)((i & 1) ? (b & 15) : (b >> 4)); }
+        for (int i = 0; i < nw; i++) { uint32_t b = p[1 + i / 2]; hw.w.weights[i] = (uint8_t)((i & 1) ? (b & 15) : (b >> 4)); }
     } else {
         used = 1 + hb;
         if (hb == 0 || used > n) return 0;
@@ -738,14 +743,14 @@ __device__ uint32_t zk_read_huf_weights(ZkHufSlot& sl, const uint8_t* p, uint32_
         uint32_t r = zk_fse_read_ncount(p + 1, hb, 6, 12, cnt, &ns, &lg);
         if (!r) return 0;
         int S = 1 << lg, high = S - 1; uint16_t nx[16];
-        for (int s = 0; s < ns; s++) { if (cnt[s] == -1) { sl.wsym[high--] = (uint8_t)s; nx[s] = 1; } else nx[s] = (uint16_t)cnt[s]; }
+        for (int s = 0; s < ns; s++) { if (cnt[s] == -1) { hw.w.sym[high--] = (uint8_t)s; nx[s] = 1; } else nx[s] = (uint16_t)cnt[s]; }
         int step = (S >> 1) + (S >> 3) + 3, pos = 0;
         for (int s = 0; s < ns; s++)
-            for (int q = 0; q < cnt[s]; q++) { sl.wsym[pos] = (uint8_t)s; do { pos = (pos + step) & (S - 1); } while (pos > high); }
+            for (int q = 0; q < cnt[s]; q++) { hw.w.sym[pos] = (uint8_t)s; do { pos = (pos + step) & (S - 1); } while (pos > high); }
         if (pos != 0) return 0;
         for (int u = 0; u < S; u++) {
-            int s = sl.wsym[u]; uint32_t x = nx[s]++; int nb = lg - zk_highbit(x);
-            sl.wnb[u] = (uint8_t)nb; sl.wbase[u] = (uint16_t)((x << nb) - S);
+            int s = hw.w.sym[u]; uint32_t x = nx[s]++; int nb = lg - zk_highbit(x);
+            hw.w.nb[u] = (uint8_t)nb; hw.w.base[u] = (uint16_t)((x << nb) - S);
         }
         ZkBackBits br;
         if (!br.init(p + 1 + r, hb - r)) return 0;
@@ -755,66 +760,121 @@ __device__ uint32_t zk_read_huf_weights(ZkHufSlot& sl, const uint8_t* p, uint32_
         for (;;) {   // two interleaved states, over-read terminates (A.4)
             if (nw >= 254) return 0;
             br.refill();
-            sl.weights[nw++] = sl.wsym[s1];
-            s1 = sl.wbase[s1] + br.read(sl.wnb[s1]);
-            if (br.bp < 0) { sl.weights[nw++] = sl.wsym[s2]; break; }
-            sl.weights[nw++] = sl.wsym[s2];
-            s2 = sl.wbase[s2] + br.read(sl.wnb[s2]);
-            if (br.bp < 0) { sl.weights[nw++] = sl.wsym[s1]; break; }
+            hw.w.weights[nw++] = hw.w.sym[s1];
+            s1 = hw.w.base[s1] + br.read(hw.w.nb[s1]);
+            if (br.bp < 0) { hw.w.weights[nw++] = hw.w.sym[s2]; break; }
+            hw.w.weights[nw++] = hw.w.sym[s2];
+            s2 = hw.w.base[s2] + br.read(hw.w.nb[s2]);
+            if (br.bp < 0) { hw.w.weights[nw++] = hw.w.sym[s1]; break; }
         }
         if (nw > 255) return 0;                    // at most 255 explicit weights (+ the implied one = 256 symbols)
     }
-    uint32_t total = 0, n_w1 = 0;
-    for (int i = 0; i < nw; i++) {
-        uint32_t w = sl.weights[i];
-        if (w > 11) return 0;
-        if (w) total += 1u << (w - 1);
-        n_w1 += (w == 1);
-    }
-    if (total == 0) return 0;
-    int max_bits = zk_highbit(total) + 1;
-    if (max_bits > 11) return 0;
-    uint32_t left = (1u << max_bits) - total;
-    if (left & (left - 1)) return 0;               // must be a power of two (left >= 1 by construction)
-    uint32_t lw = (uint32_t)zk_highbit(left) + 1;
-    sl.weights[nw++] = (uint8_t)lw;
-    n_w1 += (lw == 1);
-    if (n_w1 < 2 || (n_w1 & 1)) return 0;          // libzstd's HUF_readStats sanity rule
-    sl.huf_bits = max_bits; sl.nw = nw;
+    *nw_out = nw;
     return used;
 }
 
-// Decode `cnt` Huffman symbols of one stream into out (A.4).  Returns false on corruption.
-__device__ __forceinline__ uint32_t zk_huf_lookup(const ZkHufSlot& sl, uint32_t idx) {
-    return idx < sl.n_low ? sl.low[idx & 511u] : sl.l1[idx >> 2];
+// The nw explicit weights in hw -> decoding table in the same memory, built by the whole warp (warp-uniform arguments,
+// every lane returns the same).  Returns false on corruption; sets *n_low (L) and *bits (maxBits).  Symbol lane + 32k is
+// this lane's k-th symbol: its weight and its rank among the symbols of that weight stay in registers.
+__device__ bool zk_huf_build(ZkHufTab& hw, ZkHufScratch& sc, int nw, int lane, uint32_t* n_low, int* bits) {
+    const uint32_t full = 0xFFFFFFFFu, lt = (1u << lane) - 1u;
+    // 1. the implied last weight and libzstd's sanity rules (HUF_readStats)
+    uint32_t w[8], total = 0, n_w1 = 0; bool bad = false;
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+        const int s = lane + 32 * k;
+        w[k] = s < nw ? hw.w.weights[s] : 0u;
+        bad |= w[k] > 11;
+        total += w[k] ? 1u << (w[k] - 1) : 0u;
+        n_w1 += w[k] == 1;
+    }
+    if (__any_sync(full, bad)) return false;
+    total = __reduce_add_sync(full, total); n_w1 = __reduce_add_sync(full, n_w1);
+    if (total == 0) return false;
+    const int max_bits = zk_highbit(total) + 1;
+    if (max_bits > 11) return false;
+    const uint32_t left = (1u << max_bits) - total;
+    if (left & (left - 1)) return false;       // must be a power of two (left >= 1 by construction)
+    const uint32_t lw = (uint32_t)zk_highbit(left) + 1;
+#pragma unroll
+    for (int k = 0; k < 8; k++) if (lane + 32 * k == nw) w[k] = lw;
+    n_w1 += (lw == 1);
+    if (n_w1 < 2 || (n_w1 & 1)) return false;
+    // 2. symbols per weight, and each symbol's rank among those of its weight (natural order)
+    if (lane < 16) sc.cntw[lane] = 0;
+    __syncwarp();
+    uint32_t occ[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+        const uint32_t m = __match_any_sync(full, w[k]);
+        occ[k] = sc.cntw[w[k]] + (uint32_t)__popc(m & lt);
+        __syncwarp();
+        if (!(m & lt)) sc.cntw[w[k]] += (uint32_t)__popc(m);
+        __syncwarp();
+    }
+    // lane w (1 <= w <= maxBits): first cell and first sorted index of weight w, by exclusive scans over 16 lanes
+    const uint32_t cw = (lane >= 1 && lane <= max_bits) ? sc.cntw[lane] : 0u, own = lane >= 1 ? cw << (lane - 1) : 0u;
+    uint32_t cells = own, cs = cw;
+#pragma unroll
+    for (int d = 1; d < 16; d <<= 1) {
+        const uint32_t x = __shfl_up_sync(full, cells, d), y = __shfl_up_sync(full, cs, d);
+        if (lane >= d) { cells += x; cs += y; }
+    }
+    const uint32_t acc = __shfl_sync(full, cells, 15), rank_start = cells - own, cstart = cs - cw;
+    if (acc != (1u << max_bits)) return false;
+    const uint32_t nl = __shfl_sync(full, cw, 1) + 2u * __shfl_sync(full, cw, 2);   // cells of the two longest code lengths
+    if (nl > 512u) return false;
+    // 3. symbols in cell order
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+        const uint32_t at = __shfl_sync(full, cstart, (int)w[k]) + occ[k];
+        if (w[k]) sc.sorted[at] = (uint8_t)(lane + 32 * k);
+    }
+    __syncwarp();
+    // 4. fill (the weights are in registers now): weight w owns the cells [rank_start, + count << (w-1)); w <= 2 -> low,
+    //    one l1 entry per 4 cells above (L is a multiple of 4 whenever a weight >= 3 exists)
+    for (int wt = 1; wt <= max_bits; wt++) {
+        const uint32_t c = __shfl_sync(full, cw, wt), rs = __shfl_sync(full, rank_start, wt), c0 = __shfl_sync(full, cstart, wt);
+        const uint32_t hi = (uint32_t)(max_bits + 1 - wt) << 8;
+        if (wt <= 2) { for (uint32_t i = lane; i < (c << (wt - 1)); i += 32) hw.t.low[rs + i] = (uint16_t)(hi | sc.sorted[c0 + (i >> (wt - 1))]); }
+        else { for (uint32_t i = lane; i < (c << (wt - 3)); i += 32) hw.t.l1[(rs >> 2) + i] = (uint16_t)(hi | sc.sorted[c0 + (i >> (wt - 3))]); }
+    }
+    *n_low = nl; *bits = max_bits;
+    return true;
 }
-__device__ bool zk_huf_decode_stream(const ZkHufSlot& sl, int max_bits, const uint8_t* p, uint32_t n, uint8_t* out, uint32_t cnt) {
+
+// Decode `cnt` Huffman symbols of one stream into out (A.4).  Returns false on corruption.
+__device__ __forceinline__ uint32_t zk_huf_lookup(const ZkHufTab& t, uint32_t n_low, uint32_t idx) {
+    return idx < n_low ? t.t.low[idx & 511u] : t.t.l1[idx >> 2];
+}
+__device__ bool zk_huf_decode_stream(const ZkHufTab& t, uint32_t n_low, int max_bits, const uint8_t* p, uint32_t n, uint8_t* out, uint32_t cnt) {
     ZkBackBits br;
     if (!br.init(p, n)) return false;
     uint32_t i = 0;
     while (i < cnt && ((uintptr_t)(out + i) & 3)) {
         br.refill();
-        uint32_t e = zk_huf_lookup(sl, br.peek(max_bits)); br.skip((int)(e >> 8)); out[i++] = (uint8_t)e;
+        uint32_t e = zk_huf_lookup(t, n_low, br.peek(max_bits)); br.skip((int)(e >> 8)); out[i++] = (uint8_t)e;
     }
     for (; i + 4 <= cnt; i += 4) {
         br.refill();                                   // >= 33 bits: three codes of <= 11 bits
-        uint32_t e0 = zk_huf_lookup(sl, br.peek(max_bits)); br.skip((int)(e0 >> 8));
-        uint32_t e1 = zk_huf_lookup(sl, br.peek(max_bits)); br.skip((int)(e1 >> 8));
-        uint32_t e2 = zk_huf_lookup(sl, br.peek(max_bits)); br.skip((int)(e2 >> 8));
+        uint32_t e0 = zk_huf_lookup(t, n_low, br.peek(max_bits)); br.skip((int)(e0 >> 8));
+        uint32_t e1 = zk_huf_lookup(t, n_low, br.peek(max_bits)); br.skip((int)(e1 >> 8));
+        uint32_t e2 = zk_huf_lookup(t, n_low, br.peek(max_bits)); br.skip((int)(e2 >> 8));
         br.refill();
-        uint32_t e3 = zk_huf_lookup(sl, br.peek(max_bits)); br.skip((int)(e3 >> 8));
+        uint32_t e3 = zk_huf_lookup(t, n_low, br.peek(max_bits)); br.skip((int)(e3 >> 8));
         *(uint32_t*)(out + i) = (e0 & 0xFF) | ((e1 & 0xFF) << 8) | ((e2 & 0xFF) << 16) | ((e3 & 0xFF) << 24);
     }
     for (; i < cnt; i++) {
         br.refill();
-        uint32_t e = zk_huf_lookup(sl, br.peek(max_bits)); br.skip((int)(e >> 8)); out[i] = (uint8_t)e;
+        uint32_t e = zk_huf_lookup(t, n_low, br.peek(max_bits)); br.skip((int)(e >> 8)); out[i] = (uint8_t)e;
     }
     return br.bp == 0;
 }
 
 __global__ void __launch_bounds__(32) zk_huf_kernel(ZkDecodeArgs a) {
     ZK_DYN_SMEM(smem);
-    ZkHufSlot* slots = (ZkHufSlot*)smem;
+    ZkHufTab* tabs = (ZkHufTab*)smem;
+    ZkHufScratch& sc = *(ZkHufScratch*)(smem + sizeof(ZkHufTab) * ZK_HUF_SLOTS);
     const int lane = threadIdx.x, si = lane >> 2, stream = lane & 3;
     if (a.counters->overflow) return;
     const uint32_t n = a.counters->n_huf_blocks;
@@ -826,8 +886,8 @@ __global__ void __launch_bounds__(32) zk_huf_kernel(ZkDecodeArgs a) {
         if (first >= n) break;
         const uint32_t my = first + si;
         const bool active = my < n;
-        ZkHufSlot& sl = slots[si];
         uint32_t bidx = 0; ZkBlock blk; ZkLitHdr lh; const uint8_t* ebase = nullptr;
+        const uint8_t* tree = nullptr; uint32_t tree_n = 0;
         bool live = false;
         if (active) {
             bidx = a.huf_list[my];
@@ -838,53 +898,40 @@ __global__ void __launch_bounds__(32) zk_huf_kernel(ZkDecodeArgs a) {
             if (live) {
                 ebase = a.comp + a.c_off[blk.entry];
                 zk_parse_lit_hdr(ebase + blk.src, blk.size, lh);  // validated by the scan kernel
+                if (lh.type == 2) { tree = ebase + blk.src + lh.hdr; tree_n = lh.comp; }
+                else {                                              // Treeless: the tree of the block it refers to
+                    const ZkBlock& rb = a.blocks[blk.huf_ref];
+                    ZkLitHdr rh; zk_parse_lit_hdr(ebase + rb.src, rb.size, rh);
+                    tree = ebase + rb.src + rh.hdr; tree_n = rh.comp;
+                }
             }
         }
-        // 1. tree description (own block, or the block a Treeless block refers to) -- one lane per block
+        // 1. tables: weights by one lane per block, the eight blocks side by side; ranks and cells by the whole warp, one
+        //    block after another in the shared scratch
+        int st = 0, huf_bits = 0, nw = 0; uint32_t n_low = 0, tree_bytes = 0;
         if (live && stream == 0) {
-            int st = 0; uint32_t tb = 0;
-            if (lh.type == 2) { tb = zk_read_huf_weights(sl, ebase + blk.src + lh.hdr, lh.comp); if (!tb) st = ZKZ_CORRUPTION; }
-            else {
-                const ZkBlock& rb = a.blocks[blk.huf_ref];
-                ZkLitHdr rh; zk_parse_lit_hdr(ebase + rb.src, rb.size, rh);
-                if (!zk_read_huf_weights(sl, ebase + rb.src + rh.hdr, rh.comp)) st = ZKZ_CORRUPTION;
-            }
-            if (!st) {   // start cell of every symbol: weight ascending, symbols in natural order
-                uint32_t rank_start[13], cntw[13];
-                for (int w = 0; w < 13; w++) cntw[w] = 0;
-                for (int s = 0; s < sl.nw; s++) cntw[sl.weights[s]]++;
-                uint32_t acc = 0;
-                for (int w = 1; w <= sl.huf_bits; w++) { rank_start[w] = acc; acc += cntw[w] << (w - 1); }
-                for (int s = 0; s < sl.nw; s++) { int w = sl.weights[s]; if (w) { sl.hpos[s] = (uint16_t)rank_start[w]; rank_start[w] += 1u << (w - 1); } }
-                if (acc != (1u << sl.huf_bits)) st = ZKZ_CORRUPTION;
-                sl.n_low = cntw[1] + 2u * cntw[2];                 // cells of the two longest code lengths (<= 512)
-                if (sl.n_low > 512u) st = ZKZ_CORRUPTION;
-            }
-            sl.st = st; sl.tree_bytes = tb;
+            const uint32_t used = zk_read_huf_weights(tabs[si], tree, tree_n, &nw);
+            if (!used) st = ZKZ_CORRUPTION;
+            tree_bytes = lh.type == 2 ? used : 0u;
         }
         __syncwarp();
-        // 2. fill the decoding table -- the block's four lanes share the symbols
-        const bool good = live && sl.st == 0;
-        if (good) {
-            const int max_bits = sl.huf_bits;
-            for (int s = stream; s < sl.nw; s += 4) {
-                int w = sl.weights[s];
-                if (!w) continue;
-                uint32_t len = 1u << (w - 1), pos = sl.hpos[s];
-                uint16_t e = (uint16_t)(((max_bits + 1 - w) << 8) | s);
-                if (w <= 2) for (uint32_t i = 0; i < len; i++) sl.low[pos + i] = e;
-                else for (uint32_t i = 0; i < (len >> 2); i++) sl.l1[(pos >> 2) + i] = e;
-            }
+        st = __shfl_sync(0xFFFFFFFFu, st, lane & ~3); tree_bytes = __shfl_sync(0xFFFFFFFFu, tree_bytes, lane & ~3);   // to the block's four lanes
+        for (int b = 0; b < ZK_HUF_SLOTS; b++) {
+            if (!__shfl_sync(0xFFFFFFFFu, (int)live && st == 0, 4 * b)) continue;
+            uint32_t nl = 0; int bits = 0;
+            const bool built = zk_huf_build(tabs[b], sc, __shfl_sync(0xFFFFFFFFu, nw, 4 * b), lane, &nl, &bits);
+            __syncwarp();
+            if (si == b) { st = built ? 0 : ZKZ_CORRUPTION; n_low = nl; huf_bits = bits; }
         }
-        __syncwarp();
-        // 3. decode: one lane per stream
+        // 2. decode: one lane per stream
+        const ZkHufTab& tb = tabs[si];
         bool ok = true;
-        if (good) {
-            const uint8_t* q = ebase + blk.src + lh.hdr + sl.tree_bytes;
-            uint32_t qn = lh.comp - sl.tree_bytes;
+        if (live && st == 0) {
+            const uint8_t* q = ebase + blk.src + lh.hdr + tree_bytes;
+            uint32_t qn = lh.comp - tree_bytes;
             uint8_t* out = a.lit + blk.lit_base;
             if (lh.streams == 1) {
-                if (stream == 0) ok = zk_huf_decode_stream(sl, sl.huf_bits, q, qn, out, lh.regen);
+                if (stream == 0) ok = zk_huf_decode_stream(tb, n_low, huf_bits, q, qn, out, lh.regen);
             } else {
                 uint32_t seg = (lh.regen + 3) / 4;
                 if (qn < 10 || lh.regen < 6 || seg * 3 > lh.regen) ok = false;   // jump table + 4 non-empty streams; libzstd rejects regen < 6
@@ -896,14 +943,13 @@ __global__ void __launch_bounds__(32) zk_huf_kernel(ZkDecodeArgs a) {
                         uint32_t off = stream == 0 ? 0 : (stream == 1 ? s1 : (stream == 2 ? s1 + s2 : s1 + s2 + s3));
                         uint32_t len = stream == 0 ? s1 : (stream == 1 ? s2 : (stream == 2 ? s3 : s4));
                         uint32_t cnt = stream < 3 ? seg : lh.regen - 3 * seg;
-                        ok = zk_huf_decode_stream(sl, sl.huf_bits, q + 6 + off, len, out + stream * seg, cnt);
+                        ok = zk_huf_decode_stream(tb, n_low, huf_bits, q + 6 + off, len, out + stream * seg, cnt);
                     }
                 }
             }
         }
         uint32_t bad = __ballot_sync(0xFFFFFFFFu, !ok);
         if (live && stream == 0) {
-            int st = sl.st;
             if (!st && ((bad >> (si * 4)) & 0xFu)) st = ZKZ_CORRUPTION;
             a.blocks[bidx].lit_status = st ? -st : 0;
         }
@@ -2430,7 +2476,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     ws->prof.end(0, stream);
     // entropy stage: persistent warp-CTAs pulling groups of blocks from a work counter
     size_t est_blocks = (size_t)(total_d / ZK_BLOCK_MAX) + n;
-    const size_t seq_smem = ((sizeof(ZkSeqTabs) + 15) & ~(size_t)15) + sizeof(ZkSeqSlot) * ZK_SEQ_LANES, huf_smem = sizeof(ZkHufSlot) * ZK_HUF_SLOTS;
+    const size_t seq_smem = ((sizeof(ZkSeqTabs) + 15) & ~(size_t)15) + sizeof(ZkSeqSlot) * ZK_SEQ_LANES, huf_smem = sizeof(ZkHufTab) * ZK_HUF_SLOTS + sizeof(ZkHufScratch);
     if (!ws->attr_set) {
         ZK_CUDA_OK(cudaFuncSetAttribute(zk_seq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)seq_smem));
         ZK_CUDA_OK(cudaFuncSetAttribute(zk_huf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)huf_smem + 65536));
@@ -2439,7 +2485,19 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
         ZK_CUDA_OK(cudaFuncSetAttribute(zk_exec2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
         ws->attr_set = true;
     }
-    uint32_t gs = (uint32_t)sms * ws->seq_ctas, gh = (uint32_t)sms * ws->huf_ctas;          // persistent CTAs: as many as fit (shared memory: 4 x 51 KiB, 5 x 41 KiB)
+    if (!ws->huf_fit) {                          // K-D1h CTAs that fit on an SM by their shared memory (+ the tuning pad)
+#ifndef ZK_EMUL
+        int fit = 0;
+        ZK_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fit, zk_huf_kernel, 32, huf_smem + ws->huf_pad));
+        ws->huf_fit = fit > 0 ? (uint32_t)fit : 1u;
+#else
+        ws->huf_fit = 16;                        // (no SM to fill)
+#endif
+    }
+    // Half of them: K-D1s runs beside K-D1h, and the two only overlap when both fit on the SM (DESIGN §6).  Two K-D1h CTAs are
+    // resident beside K-D1s's five, the rest start as K-D1s's CTAs finish.
+    const uint32_t huf_ctas = ws->huf_ctas ? ws->huf_ctas : (ws->huf_fit > 1 ? ws->huf_fit / 2 : 1u);
+    uint32_t gs = (uint32_t)sms * ws->seq_ctas, gh = (uint32_t)sms * huf_ctas;              // persistent CTAs (K-D1s v1: 4 x 51 KiB, 5 x 41 KiB)
     size_t need_s = est_blocks / ZK_SEQ_LANES + 1, need_h = est_blocks / ZK_HUF_SLOTS + 1;
     if (need_s < gs) gs = (uint32_t)need_s;
     if (need_h < gh) gh = (uint32_t)need_h;
