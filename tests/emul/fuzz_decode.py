@@ -1,7 +1,8 @@
 """TEST INFRASTRUCTURE: mutation fuzzing of the DECODE kernels on the sanitized CPU emulation build (see asan_check.py for the
 environment).  Seeds are libzstd-written frames of every corpus class at several levels; each case mutates one (bit flips, byte
-stores, truncation, splices, length-field edits) and decodes it three ways -- default kernels, ZK_EXEC_V2=1 / ZK_SEQ_V1=1
-contexts, prefix mode -- beside libzstd:
+stores, truncation, splices, length-field edits) and decodes it under three contexts -- default routing of segments,
+CTAs only (ZK_EXEC_SHORT=0), single warps only (ZK_EXEC_SHORT=2^30) -- beside libzstd; seeds with a prefix decode in
+prefix mode under all three:
   * libzstd restores the mutated frame  -> our output must be identical (checksum verification off on both sides when the
     mutation may have hit the checksum itself);
   * libzstd rejects it                  -> we must reject it too, with a zstd error code;
@@ -23,8 +24,8 @@ rng = np.random.default_rng(int(sys.argv[2]) if len(sys.argv) > 2 else 1)
 # ZK_FUZZ_LIB=product: the nvcc build on a real GPU (optionally under compute-sanitizer) instead of the emulation build
 lib = N.load() if os.environ.get("ZK_FUZZ_LIB") == "product" else N.load(build_emul(sanitize=os.environ.get("ZK_FUZZ_SANITIZE", "1") == "1"))
 ctxs = {"default": zk.Context(0, lib)}
-for name, env in (("exec_v2", "ZK_EXEC_V2"), ("seq_v1", "ZK_SEQ_V1")):
-    os.environ[env] = "1"; ctxs[name] = zk.Context(0, lib); del os.environ[env]
+for name, short in (("cta", "0"), ("warp_all", str(1 << 30))):
+    os.environ["ZK_EXEC_SHORT"] = short; ctxs[name] = zk.Context(0, lib); del os.environ["ZK_EXEC_SHORT"]
 
 kinds = ["text", "structured", "lowent", "random", "runs"]
 seeds = []
@@ -68,8 +69,7 @@ while time.time() - t0 < secs:
     cap = dlen
     ref_out, ref_sizes = O.ref_decompress_frames(np.frombuffer(bad, dtype=np.uint8) if bad else np.zeros(0, np.uint8), [0, len(bad)], [0, cap], prefix=pfx)
     ref_ok = ref_sizes[0] >= 0
-    which = list(ctxs) if pfx is None else ["default"]
-    for name in which:
+    for name in ctxs:
         ctx = ctxs[name]
         comp = np.frombuffer(bad, dtype=np.uint8)
         out, st, rc = ctx.decompress_frames(comp, np.array([0, len(bad)], dtype=np.uint64), np.array([0, cap], dtype=np.uint64), True, prefix=pfx)

@@ -436,10 +436,11 @@ def execute(frames, prefix: bytes = b"") -> bytes:
 
 
 # ------------------------------------------------------------------------------------------------ segment rule (DESIGN §3.2)
-def block_facts(frames, back_known: bool = True):
+def block_facts(frames):
     """per block of the entry: (output position, starts a zstd frame, back or None (unknown), outgoing repeat offsets concrete).
     The repeat history entering every block is symbolic (slot k, delta d) -- blocks are entropy-decoded independently --
-    and explicit offsets only shift it, as in the sequence kernel."""
+    and explicit offsets only shift it, as in the sequence kernel.  back is measured from the block's first byte, so a read
+    into the prefix (prefix mode) counts as a read before the block."""
     facts, pos = [], 0
     for fr in frames:
         for bi, blk in enumerate(fr.blocks):
@@ -465,15 +466,15 @@ def block_facts(frames, back_known: bool = True):
                     back = max(back, off[1] - op)
                 op += ml
             conc = all(r[0] == "c" for r in reps)
-            facts.append((pos, bi == 0, None if (sym or not back_known) else back, conc))
+            facts.append((pos, bi == 0, None if sym else back, conc))
             pos += blk.regen()
     return facts
 
 
-def segment_starts(frames, back_known: bool = True) -> list:
+def segment_starts(frames) -> list:
     """indices of the blocks that start a segment: the entry's first block, or a block b such that every block from b on
     reads nothing before b's first byte, and b starts a zstd frame or leaves concrete repeat offsets"""
-    facts = block_facts(frames, back_known)
+    facts = block_facts(frames)
     starts, low = [], None
     for b in range(len(facts) - 1, -1, -1):
         op, first, back, conc = facts[b]

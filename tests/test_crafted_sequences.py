@@ -1,9 +1,10 @@
 """Crafted frames on the decode kernels' own boundaries.  Every frame is written by tests/framegen.py, so each case sits
 exactly where a kernel changes path: the single-warp executor's 4 KiB window (near / far split and reloads at 2 KiB), the
-CTA executor's ring (R/2), the long-copy paths at 48 bytes, the prefix of the in-order executor, the plan kernel's segment
+CTA executor's ring (R/2), the long-copy paths at 48 bytes, matches into the prefix (prefix mode), the plan kernel's segment
 starts, the sequence-stream forms and the two-level Huffman table.  Every valid entry is checked three ways before the
 codec sees it (executor == libzstd == the restatement) and must then decode to the executor's bytes under every context
-listed for its family; invalid entries must get libzstd's status while good entries in the same batch decode intact.
+listed for its family; invalid entries must get libzstd's status (and the serial walk's, util.serial_status) while good
+entries in the same batch decode intact.
 Every case runs on the emulation build (`-m "not gpu"`) and on the H100 (`-m gpu`)."""
 import os
 
@@ -14,7 +15,7 @@ import zeekstd_b200 as zk
 import framegen as G
 from framegen import Block, Frame
 from oracle import oracle as O
-from util import offsets
+from util import offsets, serial_status
 
 
 @pytest.fixture(scope="module", params=["emul", pytest.param("gpu", marks=pytest.mark.gpu)])
@@ -41,11 +42,12 @@ CTX_ENV = {
     "default": {},
     "warp_all": {"ZK_EXEC_SHORT": str(1 << 30)},
     "cta": {"ZK_EXEC_SHORT": "0"},
-    "serial": {"ZK_EXEC_V2": "1"},
-    "seq_v1": {"ZK_SEQ_V1": "1"},
     **{f"cta_r{r}_w{w}": {"ZK_EXEC_SHORT": "0", "ZK_RING_BYTES": str(r), "ZK_EXEC_WARPS": str(w)} for r in (1024, 4096) for w in (2, 5, 16)},
 }
 PIN_ENTRIES = 140
+# prefix mode on both executors: single warps and CTAs as the defaults route them, all on single warps, all on CTAs, and
+# CTAs pinned to a small ring
+PREFIX_CTXS = ("default", "warp_all", "cta", "cta_r1024_w5")
 
 
 @pytest.fixture(scope="module")
@@ -222,8 +224,11 @@ def test_b_cta_ring(ctxs, ring):
         expect(ctxs(f"cta_r{ring}_w{w}"), b)
 
 
-# ------------------------------------------------------------------------------------------------ C: prefix, in-order executor
+# ------------------------------------------------------------------------------------------------ C: prefix mode
 def test_c_prefix_and_in_order(ctxs):
+    """matches into the raw-content prefix before every zstd frame, in both segment executors: whole, straddling the frame
+    start, through repeat offsets, in every frame of an entry; a block reading into the prefix starts no segment unless it
+    is the entry's first"""
     rng = np.random.default_rng(4)
     prefix = rng.integers(0, 256, 3000, dtype=np.uint8).tobytes()
     P = len(prefix)
@@ -235,9 +240,11 @@ def test_c_prefix_and_in_order(ctxs):
                                      FB(rng, fcs_width=4).seqs([(0, P, 30), (2, 8, 8)]).frame(),
                                      FB(rng).raw(500).seqs([(0, 500 + P, 16)]).frame()]),
     ]
-    b = batch([(n, f, 0, prefix) for n, f in cases])
-    expect(ctxs("default"), b, prefix=prefix)
-    expect(ctxs("serial"), b, prefix=prefix)
+    b = batch([(n, f, 0, prefix) for n, f in cases], PIN_ENTRIES)
+    ref = sum(len(G.segment_starts(f)) for f in b[4])
+    for name in PREFIX_CTXS:
+        segs = expect(ctxs(name), b, prefix=prefix)
+        assert segs == ref, (name, segs, ref)
     # one byte past the prefix start: corruption (-20), the good entries intact
     bad = [FB(rng).seqs([(5, 6 + P, 20)]).frame()]
     blob = G.entry_bytes(bad)
@@ -246,8 +253,12 @@ def test_c_prefix_and_in_order(ctxs):
     assert e.value.code == 20
     _, sizes = O.ref_decompress_frames(np.frombuffer(blob, np.uint8), [0, len(blob)], [0, 25], prefix=np.frombuffer(prefix, np.uint8))
     assert sizes == [-20]
-    b = batch([(n, f, 0, prefix) for n, f in cases] + [("past_prefix", bad, 20, prefix)])
-    expect(ctxs("default"), b, {len(b[0]) - 1: -20}, prefix=prefix)
+    b = batch([(n, f, 0, prefix) for n, f in cases] + [("past_prefix", bad, 20, prefix)], PIN_ENTRIES)
+    i_bad = b[3].index("past_prefix")
+    want = {i: st for i, st in enumerate(serial_status(e, n, True, np.frombuffer(prefix, np.uint8)) for e, n in zip(b[0], b[1])) if st}
+    assert want == {i_bad: -20}
+    for name in PREFIX_CTXS:
+        expect(ctxs(name), b, want, prefix=prefix)
 
 
 # ------------------------------------------------------------------------------------------------ D: segment starts
@@ -273,12 +284,12 @@ def segment_cases(seed: int):
     return cases
 
 
-@pytest.mark.parametrize("name", ["default", "warp_all", "cta", "seq_v1"])
+@pytest.mark.parametrize("name", ["default", "warp_all", "cta"])
 def test_d_segments(ctxs, name):
     cases = segment_cases(5)
     b = batch(cases)
     segs = expect(ctxs(name), b)
-    ref = sum(len(G.segment_starts(f, back_known=name != "seq_v1")) for f in b[4])
+    ref = sum(len(G.segment_starts(f)) for f in b[4])
     assert segs == ref, (segs, ref)
 
 
@@ -320,8 +331,7 @@ def test_e_sequence_stream(ctxs, lib):
     for n in range(40, 72):
         add(f"stream{n}", FB(rng).raw(128).seqs(short_seqs(rng, n, reach=100)))
     b = batch(cases)
-    for name in ("default", "seq_v1"):
-        expect(ctxs(name), b)
+    expect(ctxs("default"), b)
 
 
 def test_e_large_nseq(ctxs):
@@ -442,7 +452,8 @@ def test_g_errors(ctxs):
     code = {e[0]: -e[2] for e in errs}
     want = {i: code[n] for i, n in enumerate(b[3]) if n in code}
     assert len(want) == len(errs)
-    for name in ("default", "warp_all", "cta", "serial", "seq_v1"):
+    assert {i: st for i, st in enumerate(serial_status(e, n) for e, n in zip(b[0], b[1])) if st} == want
+    for name in ("default", "warp_all", "cta"):
         expect(ctxs(name), b, want)
 
 

@@ -1,14 +1,11 @@
 """Execution segments (K-D1p / K-D2): a seek-table entry is run as several independent runs of blocks when its sequences
 allow it.  Every case runs on the emulation build (`-m "not gpu"`) and on the H100 (`-m gpu`); `ctx.decode_segments`
 counts the segments the decoder ran, so splitting is asserted, not hoped for."""
-import os
-
 import numpy as np
 import pytest
 
-import zeekstd_b200 as zk
 from oracle import oracle as O
-from util import decode_frames, make_ctx, offsets, split_frames
+from util import decode_frames, make_ctx, offsets, serial_status, split_frames
 from zeekstd_b200 import _native, corpus
 
 # A level-1 archive of the bench generator (64 KiB class pieces, 256 KiB frames).  This seed's archive has blocks whose
@@ -21,18 +18,6 @@ MIX_SEED, MIX_BYTES, MIX_FRAME = 20260924, 1 << 20, 256 << 10
 def ctx(request):
     lib = request.getfixturevalue("emul_lib" if request.param == "emul" else "gpu_lib")
     c = make_ctx(lib)
-    yield c
-    c.close()
-
-
-@pytest.fixture(scope="module")
-def ctx_serial(ctx):
-    """the same build with the in-order exec kernel, which walks every entry serially as one unit"""
-    os.environ["ZK_EXEC_V2"] = "1"
-    try:
-        c = zk.Context(0, ctx.lib)
-    finally:
-        del os.environ["ZK_EXEC_V2"]
     yield c
     c.close()
 
@@ -104,9 +89,9 @@ def test_range_read_inside_split_entry(ctx, mix):
             assert out[a0:a0 + want].tobytes() == mix[a0:a0 + want].tobytes()
 
 
-def test_failures_keep_serial_order(ctx, ctx_serial, mix):
+def test_failures_keep_serial_order(ctx, mix):
     """corruption in a later segment of an entry, alone or while an earlier segment fails too (and with the entry's
-    output size also wrong): the same per-entry status as the serial walk"""
+    output size also wrong): the same per-entry status as the serial walk (util.serial_status)"""
     comp, cs, ds = ctx.compress_frames(mix, MIX_FRAME, 1, False)
     frames = split_frames(comp.tobytes(), cs)
     rng = np.random.default_rng(7)
@@ -125,7 +110,7 @@ def test_failures_keep_serial_order(ctx, ctx_serial, mix):
         if trial % 3 == 0:
             sizes[e] += 1                                                             # the final size check fails as well
         _, st, _, _ = _decode(ctx, fr, sizes, False)
-        _, st_ref, _, _ = _decode(ctx_serial, fr, sizes, False)
+        st_ref = [serial_status(x, s, False) for x, s in zip(fr, sizes)]
         assert list(st) == list(st_ref), (trial, list(st), list(st_ref))
         checked += st[e] != 0
     assert checked > 12

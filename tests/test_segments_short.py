@@ -1,7 +1,7 @@
 """Short execution segments run on one warp each (zk_exec_warp_kernel), long ones on CTAs (zk_exec_kernel); ZK_EXEC_SHORT
 is the output size up to which a segment counts as short.  Under a threshold that splits the batch between both kernels,
 under 0 (CTAs only) and under one that makes every segment short, the output, the per-entry status and the number of
-segments must be those of the serial walk (the in-order kernel, ZK_EXEC_V2=1) and of each other.  Every case runs on the
+segments must be those of the serial walk (util.serial_status) and of each other.  Every case runs on the
 emulation build (`-m "not gpu"`) and on the H100 (`-m gpu`)."""
 import os
 
@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 import zeekstd_b200 as zk
-from util import decode_frames, split_frames
+from util import decode_frames, serial_status, split_frames
 from zeekstd_b200 import corpus
 
 MIX_SEED, MIX_BYTES, MIX_FRAME = 20260924, 1 << 20, 256 << 10
@@ -38,7 +38,6 @@ def _context(lib, env: dict):
 @pytest.fixture(scope="module")
 def ctxs(lib):
     c = {name: _context(lib, {"ZK_EXEC_SHORT": str(v)}) for name, v in SETTINGS.items()}
-    c["serial"] = _context(lib, {"ZK_EXEC_V2": "1"})
     yield c
     for x in c.values():
         x.close()
@@ -47,7 +46,7 @@ def ctxs(lib):
 @pytest.fixture(scope="module")
 def archive(ctxs):
     mix = corpus.as_numpy(corpus.make_mix(MIX_BYTES, seed=MIX_SEED, segment=64 << 10))
-    comp, cs, ds = ctxs["serial"].compress_frames(mix, MIX_FRAME, 1, False)
+    comp, cs, ds = ctxs["both"].compress_frames(mix, MIX_FRAME, 1, False)
     return mix, split_frames(comp.tobytes(), cs), [int(d) for d in ds]
 
 
@@ -84,7 +83,7 @@ def test_failures_keep_serial_order_under_every_threshold(ctxs, archive):
         sizes = list(ds)
         if trial % 3 == 0:
             sizes[e] += 1
-        _, st_ref, _, _ = _decode(ctxs["serial"], fr, sizes, False)
+        st_ref = [serial_status(x, s, False) for x, s in zip(fr, sizes)]
         for name in SETTINGS:
             _, st, _, _ = _decode(ctxs[name], fr, sizes, False)
             assert st == st_ref, (name, trial, st, st_ref)

@@ -38,6 +38,17 @@ def decode_frames(ctx, frames, d_sizes, verify=True):
     return out.tobytes(), st, rc
 
 
+def serial_status(entry: bytes, size: int, verify: bool = True, prefix=None) -> int:
+    """the status of one seek-table entry as the serial walk defines it: the C restatement decoding it into exactly `size`
+    bytes -> 0, -(zstd code), or -72 (srcSize_wrong) when it ends short of `size`"""
+    from oracle import oracle as O
+    try:
+        out, _ = O.oracle_decompress_ex(np.frombuffer(entry, np.uint8), size, prefix=prefix, verify_checksum=verify)
+    except O.ZstdError as e:
+        return -e.code
+    return 0 if len(out) == size else -72
+
+
 def split_frames(comp: bytes, c_sizes):
     out, pos = [], 0
     for c in c_sizes:

@@ -20,7 +20,7 @@ for l in sass.split("\n"):
 dem = lambda n: subprocess.run(["c++filt", n], capture_output=True, text=True).stdout.strip().split("(")[0]
 print("# SASS summary of zeekstd_b200/libzeekstd_b200.so (cuobjdump -sass, sm_90a) -- tools/sass_summary.py")
 print("# UBLKCP = cp.async.bulk (TMA bulk copy global -> shared; K-D1s stages sequence bitstreams with it), SYNCS = mbarrier operations")
-print("# (arrive / expect_tx / try_wait: the tile barriers of K-D1s and the event waits of zk_exec2_kernel), REDUX = redux.sync, MATCH = match.any")
+print("# (arrive / expect_tx / try_wait: the tile barriers of K-D1s), REDUX = redux.sync, MATCH = match.any")
 print("kernel | SASS instructions | registers | static smem | UBLKCP | SYNCS | REDUX | MATCH | LDS | STS | LDG | STG | ATOM/RED | BAR")
 for k, c in cnt.items():
     if "zk_" not in k: continue

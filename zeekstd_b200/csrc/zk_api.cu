@@ -112,10 +112,9 @@ extern "C" int32_t zk_ctx_create(int32_t device_ordinal, uint32_t flags, zk_ctx*
         c->slot[i].dws.sm_count = c->sm_count;
         c->slot[i].dws.ring_override = (uint32_t)zk_env_size("ZK_RING_BYTES", 0);   // tuning / tests: power of two >= 1024
         c->slot[i].dws.huf_pad = (uint32_t)zk_env_size("ZK_HUF_PAD", 0);
-        c->slot[i].dws.exec_v2 = zk_env_size("ZK_EXEC_V2", 0) != 0;
         c->slot[i].dws.exec_short = (uint32_t)zk_env_size("ZK_EXEC_SHORT", 128 << 10);
-        c->slot[i].dws.seq_v1 = zk_env_size("ZK_SEQ_V1", 0) != 0; c->slot[i].dws.seq2_ctas = (uint32_t)zk_env_size("ZK_SEQ2_CTAS", 5);
-        c->slot[i].dws.seq_ctas = (uint32_t)zk_env_size("ZK_SEQ_CTAS", 4); c->slot[i].dws.huf_ctas = (uint32_t)zk_env_size("ZK_HUF_CTAS", 0);
+        c->slot[i].dws.seq2_ctas = (uint32_t)zk_env_size("ZK_SEQ2_CTAS", 5);
+        c->slot[i].dws.huf_ctas = (uint32_t)zk_env_size("ZK_HUF_CTAS", 0);
         c->slot[i].ews.sm_count = c->sm_count;
     }
     cudaEventCreate(&c->ev0); cudaEventCreate(&c->ev1);

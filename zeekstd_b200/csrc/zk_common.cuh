@@ -281,40 +281,12 @@ __device__ inline uint32_t zk_fse_read_ncount(const uint8_t* p, uint32_t n, int 
 }
 
 // -------------------------------------------------------------------------------------------
-// Event = an mbarrier with an arrival count of one: every arrive completes a phase, so "something changed" wakes
-// whoever sleeps in try_wait on it (hardware sleep: a waiting warp issues nothing, and wakes ~60 cycles after the
-// arrive -- PTX ISA, mbarrier).  A waiter re-checks its own condition after every wake-up; it first learns the
-// parity of the running phase (test_wait), THEN checks the condition, then sleeps on that parity, so a change between the
-// check and the sleep ends the sleep at once.  Two changes in that window would be missed; the time hint bounds that.
-// -------------------------------------------------------------------------------------------
-#ifndef ZK_EMUL
-__device__ __forceinline__ uint32_t zk_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void zk_event_init(unsigned long long* bar) { asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(zk_smem_u32(bar)) : "memory"); }
-__device__ __forceinline__ void zk_event_signal(unsigned long long* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(zk_smem_u32(bar)) : "memory"); }
-__device__ __forceinline__ uint32_t zk_event_parity(unsigned long long* bar) {      // parity of the phase that is running now
-    uint32_t done0;
-    asm volatile("{ .reg .pred p; mbarrier.test_wait.parity.shared::cta.b64 p, [%1], 0; selp.u32 %0, 1, 0, p; }" : "=r"(done0) : "r"(zk_smem_u32(bar)) : "memory");
-    return done0;                                                                     // phase of parity 0 complete <=> parity 1 is running
-}
-__device__ __forceinline__ bool zk_event_sleep(unsigned long long* bar, uint32_t parity, uint32_t hint_ns) {   // true: that phase has completed
-    uint32_t ok;
-    asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3; selp.u32 %0, 1, 0, p; }"
-                 : "=r"(ok) : "r"(zk_smem_u32(bar)), "r"(parity), "r"(hint_ns) : "memory");
-    return ok != 0;
-}
-#else
-__device__ __forceinline__ void zk_event_init(unsigned long long* bar) { *bar = 0; }
-__device__ __forceinline__ void zk_event_signal(unsigned long long* bar) { *(volatile unsigned long long*)bar = *bar + 1; }
-__device__ __forceinline__ uint32_t zk_event_parity(unsigned long long* bar) { return (uint32_t)(*(volatile unsigned long long*)bar & 1); }
-__device__ __forceinline__ bool zk_event_sleep(unsigned long long* bar, uint32_t parity, uint32_t) { emu::yield(); return (uint32_t)(*(volatile unsigned long long*)bar & 1) != parity; }
-#endif
-
-// -------------------------------------------------------------------------------------------
 // TMA bulk copy global -> shared (cp.async.bulk, SASS UBLKCP) completing on an mbarrier: one thread arms the barrier with
 // the byte count and issues the copy; the data lands without passing through registers and whoever needs it waits on the
 // barrier's phase.  Addresses and sizes are multiples of 16 bytes.
 // -------------------------------------------------------------------------------------------
 #ifndef ZK_EMUL
+__device__ __forceinline__ uint32_t zk_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void zk_mbar_init(unsigned long long* bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(zk_smem_u32(bar)), "r"(count) : "memory"); }
 __device__ __forceinline__ void zk_bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, unsigned long long* bar) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(zk_smem_u32(bar)), "r"(bytes) : "memory");

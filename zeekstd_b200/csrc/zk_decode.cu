@@ -2,15 +2,18 @@
 //
 // Replaces the reference's only decompression call into libzstd,
 //   lib/src/decode.rs:243-245   self.dctx.decompress_stream(&mut out_buffer, &mut in_buffer)
-// with four kernels over a whole batch of independent seek-table entries ("frames" of the
+// with these kernels over a whole batch of independent seek-table entries ("frames" of the
 // seekable format, seekable_format.md:23-29):
 //
-//   K-D0 zk_scan_kernel     one thread / entry : walk frame + block headers, carve scratch
-//   K-D1s zk_seq_kernel     one LANE  / block  : FSE sequence decode (4-byte cells + state machine in smem)
-//   K-D1h zk_huf_kernel     one LANE  / stream : Huffman literal decode (4 lanes per 4-stream block, two-level table)
-//   K-D1p zk_plan_kernel    one warp / entry   : output positions, the serial walk's checks, execution segments
-//   K-D2 zk_exec_kernel[_w5] one CTA  / segment : ordered sequence execution through a shared-memory window
-//   K-D3 zk_xxh64_kernel    one warp  / entry  : content checksum (only if requested & present)
+//   K-D0 zk_scan_kernel        one thread / entry   : walk frame + block headers, carve scratch
+//   K-D1s zk_seq2_kernel       one chain / block    : FSE sequence decode (4 chains per warp, TMA-staged bitstreams)
+//   K-D1h zk_huf_kernel        one LANE  / stream   : Huffman literal decode (4 lanes per 4-stream block, two-level table)
+//   K-D1p zk_plan_kernel       one warp / entry     : output positions, the serial walk's checks, execution segments
+//   K-D2w zk_exec_warp_kernel  one warp / segment   : short segments, strictly in order through a per-warp window
+//   K-D2 zk_exec_kernel[_w5]   one CTA  / segment   : long segments, sequence execution through a shared-memory ring
+//   K-D3 zk_xxh64_kernel       one warp  / entry    : content checksum (only if requested & present)
+// Both executors come in a prefix-mode build (template PREFIX): matches may reach into a raw-content prefix before
+// every zstd frame.
 //
 // Format rules: RFC 8878 as restated in SURVEY.md Appendix A (the arithmetic is not in the
 // reference tree).  All integer/byte work; no tensor cores.
@@ -239,17 +242,11 @@ __global__ void __launch_bounds__(128) zk_scan_kernel(ZkDecodeArgs a) {
 }
 
 // =============================================================================================
-// K-D1s: FSE sequence decode -- one LANE per zstd block.
+// K-D1s: FSE sequence decode tables.
 //
 // A sequence bitstream is one serial dependency chain (three interleaved FSE states sharing one
-// backward bit cursor, A.5), so the only parallelism is across blocks.  Profiling the first version
-// (one block per CTA, one active lane per warp) showed the SMs issue-bound at 1/32 SIMT efficiency;
-// here every lane of a warp runs the identical decode loop over ITS OWN block with ITS OWN tables
-// in shared memory, so one issued instruction advances up to ZK_SEQ_LANES chains.
+// backward bit cursor, A.5), so the only parallelism is across blocks.
 // =============================================================================================
-#define ZK_SEQ_LPW 3              // chains per warp
-#define ZK_SEQ_WARPS 3            // warps per CTA: 9 x 5.6 KiB of tables per CTA (4 CTAs / SM) spread over more warps --
-#define ZK_SEQ_LANES (ZK_SEQ_LPW * ZK_SEQ_WARPS)   // each chain is ALU-latency bound, so more warps per SM hide more of it
 
 // Thin decoding cell: one 32-bit shared-memory load yields everything on the dependency chain of a sequence (bits to
 // skip, bits of the next state, next-state baseline); the value baselines come from small per-CTA tables by symbol code,
@@ -344,100 +341,6 @@ __device__ int zk_build_seq_table(ZkSeqSlot& sl, int t, uint16_t* nxt_scratch = 
         cell[u] = ZK_CELL(sy, add, nb, (x << nb) - (uint32_t)S);
     }
     return 0;
-}
-
-// Decode all sequences of one block (lane-local).  Returns 0 or a zstd code.
-__device__ int zk_decode_block_sequences(ZkSeqSlot& sl, const ZkSeqTabs& tb, const ZkDecodeArgs& a, const ZkBlock& blk, uint32_t bidx, const uint8_t* ebase) {
-    const uint8_t* b = ebase + blk.src;
-    uint32_t bits_off = 0;
-    int st = zk_locate_seq_tables(sl, b, blk.size, blk.ll_ref < 0, blk.of_ref < 0, blk.ml_ref < 0, &bits_off);
-    if (st) return st;
-    if (blk.ll_ref >= 0) { const ZkBlock& rb = a.blocks[blk.ll_ref]; uint32_t d; if ((st = zk_locate_seq_tables(sl, ebase + rb.src, rb.size, true, false, false, &d))) return st; }
-    if (blk.of_ref >= 0) { const ZkBlock& rb = a.blocks[blk.of_ref]; uint32_t d; if ((st = zk_locate_seq_tables(sl, ebase + rb.src, rb.size, false, true, false, &d))) return st; }
-    if (blk.ml_ref >= 0) { const ZkBlock& rb = a.blocks[blk.ml_ref]; uint32_t d; if ((st = zk_locate_seq_tables(sl, ebase + rb.src, rb.size, false, false, true, &d))) return st; }
-    for (int t = 0; t < 3; t++) if ((st = zk_build_seq_table(sl, t))) return st;
-
-    ZkBackBits br;
-    if (!br.init(b + bits_off, blk.size - bits_off)) return ZKZ_CORRUPTION;
-    const int ll_log = sl.tbl_log[0], of_log = sl.tbl_log[1], ml_log = sl.tbl_log[2];
-    br.refill();
-    uint32_t s_l = br.read(ll_log), s_o = br.read(of_log), s_m = br.read(ml_log);
-    uint32_t r0 = ZK_SYM_MAKE(0, 0), r1 = ZK_SYM_MAKE(1, 0), r2 = ZK_SYM_MAKE(2, 0);
-    uint32_t lit_end = 0, out_end = 0;
-    uint32_t* o_lit = a.seq_lit_end + blk.seq_base;
-    uint32_t* o_out = a.seq_out_end + blk.seq_base;
-    uint32_t* o_off = a.seq_off + blk.seq_base;
-    const uint32_t nseq = blk.nseq;
-    for (uint32_t i = 0; i < nseq; i++) {
-        const uint32_t cl = sl.ll[s_l], co = sl.of[s_o], cm = sl.ml[s_m];
-        br.refill();                                                  // <= 31 bits follow
-        const uint32_t ofc = ZK_CELL_CODE(co);
-        uint32_t ofv = (1u << ofc) + br.read((int)ofc);
-        br.refill();                                                  // <= 16 + 16 bits follow
-        uint32_t mlv = tb.ml_base[ZK_CELL_CODE(cm)] + br.read((int)ZK_CELL_ADD(cm));
-        uint32_t llv = tb.ll_base[ZK_CELL_CODE(cl)] + br.read((int)ZK_CELL_ADD(cl));
-        br.refill();                                                  // <= 9 + 9 + 8 bits follow
-        if (i + 1 < nseq) {
-            s_l = ZK_CELL_BASE(cl) + br.read((int)ZK_CELL_NB(cl));
-            s_m = ZK_CELL_BASE(cm) + br.read((int)ZK_CELL_NB(cm));
-            s_o = ZK_CELL_BASE(co) + br.read((int)ZK_CELL_NB(co));
-        }
-        // repeat-offset history, kept symbolic w.r.t. the (unknown) state entering this block
-        uint32_t off;
-        if (ofv > 3) { off = ofv - 3; r2 = r1; r1 = r0; r0 = off; }
-        else {
-            uint32_t idx = ofv - 1 + (llv == 0);
-            if (idx == 0) off = r0;
-            else {
-                if (idx == 3) {
-                    if (r0 & ZK_SYM) off = r0 + 1;                    // delta + 1
-                    else { off = r0 - 1; if (off == 0) st = ZKZ_CORRUPTION; }
-                } else off = idx == 1 ? r1 : r2;
-                if (idx != 1) r2 = r1;
-                r1 = r0; r0 = off;
-            }
-        }
-        lit_end += llv; out_end += llv + mlv;
-        // bounded after EVERY sequence (one step adds < 2^18, so neither sum can wrap past 2^32 unnoticed): the exec
-        // kernel uses the intermediate sums as literal-source and output positions
-        if (lit_end > blk.lit_size || out_end > ZK_BLOCK_MAX) { st = ZKZ_CORRUPTION; break; }
-        o_lit[i] = lit_end; o_out[i] = out_end; o_off[i] = off;
-    }
-    if (!st && br.bp != 0) st = ZKZ_CORRUPTION;
-    if (!st && out_end + (blk.lit_size - lit_end) > blk.bmax) st = ZKZ_CORRUPTION;
-    a.blocks[bidx].rep_out[0] = r0; a.blocks[bidx].rep_out[1] = r1; a.blocks[bidx].rep_out[2] = r2;
-    a.blocks[bidx].regen = out_end + (blk.lit_size - lit_end);
-    return st;
-}
-
-__global__ void __launch_bounds__(32 * ZK_SEQ_WARPS) zk_seq_kernel(ZkDecodeArgs a) {
-    ZK_DYN_SMEM(smem);
-    ZkSeqTabs* tb = (ZkSeqTabs*)smem;
-    ZkSeqSlot* slots = (ZkSeqSlot*)(smem + ((sizeof(ZkSeqTabs) + 15) & ~(size_t)15));
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int i = threadIdx.x; i < 36; i += 32 * ZK_SEQ_WARPS) tb->ll_base[i] = ZK_LL_BASE[i];
-    for (int i = threadIdx.x; i < 53; i += 32 * ZK_SEQ_WARPS) tb->ml_base[i] = ZK_ML_BASE[i];
-    __syncthreads();
-    if (a.counters->overflow) return;
-    const uint32_t n = a.counters->n_seq_blocks;
-    for (;;) {                                  // every warp pulls its own groups of ZK_SEQ_LPW blocks
-        uint32_t g = 0;
-        if (lane == 0) g = atomicAdd(&a.work_counter[0], 1u);
-        g = __shfl_sync(0xFFFFFFFFu, g, 0);
-        uint32_t first = g * ZK_SEQ_LPW;
-        if (first >= n) break;
-        uint32_t my = first + lane;
-        if (lane < ZK_SEQ_LPW && my < n) {
-            uint32_t bidx = a.seq_list[my];
-            ZkBlock blk; blk.entry = 0xFFFFFFFFu;
-            if (bidx < a.cap_blocks) blk = a.blocks[bidx];          // always: every reserved slot is written by the scan kernel
-            if (blk.entry < a.n_entries && a.entries[blk.entry].status == 0) {
-                int st = zk_decode_block_sequences(slots[warp * ZK_SEQ_LPW + lane], *tb, a, blk, bidx, a.comp + a.c_off[blk.entry]);
-                a.blocks[bidx].status = st ? -st : 0;
-            }
-        }
-        __syncwarp();
-    }
 }
 
 // =============================================================================================
@@ -1342,6 +1245,21 @@ __device__ __forceinline__ void zk_chunk_literals(const ZkRing& rg, const uint8_
     }
 }
 
+// Prefix mode: the part of a match that lies before its frame's first byte (zstart) comes from the raw-content prefix that
+// precedes every zstd frame.  That part is constant data with no dependency, copied at once by its lane; what is left of the
+// match, if anything, starts at the frame's first byte with the same offset and is an ordinary match.  TO_RING: destination
+// is the ring, else HBM directly.
+template <bool TO_RING>
+__device__ __forceinline__ void zk_prefix_part(const ZkRing& rg, const ZkDecodeArgs& a, bool valid, uint32_t zstart, uint32_t off,
+                                               uint32_t& md, uint32_t& ml) {
+    if (valid && ml > 0 && off > md - zstart) {
+        const uint32_t back = off - (md - zstart), la = ml < back ? ml : back;
+        const uint8_t* ps = a.prefix + (a.prefix_len - back);
+        for (uint32_t i = 0; i < la; i++) { if (TO_RING) rg.at(md + i) = ps[i]; else rg.out[md + i] = ps[i]; }
+        md += la; ml -= la;
+    }
+}
+
 // chunk c's bytes are final in the ring: dependants may read them
 __device__ __forceinline__ void zk_d2_mark_done(ZkD2Smem& sm, uint32_t c, int lane) {
     __threadfence_block();
@@ -1407,6 +1325,7 @@ __device__ __forceinline__ bool zk_d2_wait_start(ZkD2Smem& sm, uint32_t c, uint3
 // position on.  The ring and the in-order state start at that position; a segment's first block either starts a zstd
 // frame or uses no repeat offset it did not set itself, so R0..R2 need no incoming state.  The checks that need only
 // block sizes were made by the plan kernel, which also stopped the walk where the serial one stopped.
+template <bool PREFIX>
 __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs& a, uint32_t ring_bytes, uint32_t first_bidx) {
     ZK_DYN_SMEM(ring_mem);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, W = blockDim.x >> 5;
@@ -1492,8 +1411,8 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
             }
             uint32_t le_prev = __shfl_up_sync(0xFFFFFFFFu, le, 1), oe_prev = __shfl_up_sync(0xFFFFFFFFu, oe, 1);
             if (lane == 0) { le_prev = s ? s_lit[s - 1] : 0; oe_prev = s ? s_out[s - 1] : 0; }
-            const uint32_t ll = le - le_prev, ml = (oe - oe_prev) - ll;
-            const uint32_t o_lit = pos + oe_prev, md = o_lit + ll;          // entry-relative positions
+            const uint32_t ll = le - le_prev; uint32_t ml = (oe - oe_prev) - ll;
+            const uint32_t o_lit = pos + oe_prev; uint32_t md = o_lit + ll;   // entry-relative positions (PREFIX: md / ml shrink to the in-frame part)
             uint32_t off = offv;
             bool bad = false;
             if (valid) {
@@ -1502,7 +1421,7 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
                     uint32_t r = sl == 0 ? R0 : (sl == 1 ? R1 : R2);
                     bad = r <= dl; off = r - dl;
                 }
-                if (off == 0 || off > md - zstart) bad = true;
+                if (off == 0 || off > md - zstart + (PREFIX ? a.prefix_len : 0u)) bad = true;
             }
             if (__any_sync(0xFFFFFFFFu, bad)) { zk_d2_abort(sm, ZKZ_CORRUPTION, bi); break; }
             const uint32_t chunk_start = pos + __shfl_sync(0xFFFFFFFFu, oe_prev, 0);
@@ -1552,6 +1471,7 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
                         }
                     }
                 }
+                if (PREFIX) zk_prefix_part<false>(rg, a, valid, zstart, off, md, ml);
                 __syncwarp();
                 const uint32_t need_end = md - off + (ml < off ? ml : off);
                 uint32_t pending = __ballot_sync(0xFFFFFFFFu, valid && ml > 0);
@@ -1583,6 +1503,7 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
             // ======== normal chunk: build the output in the ring, then flush
             // literal runs: no dependencies (HBM scratch -> ring)
             zk_chunk_literals<true>(rg, lit, blk.lit_kind, blk.lit_byte, le, le_prev, o_lit, lane);
+            if (PREFIX) zk_prefix_part<true>(rg, a, valid, zstart, off, md, ml);
             {   // all literal runs are in place: sequences without a match (and the lanes past the last one) are complete
                 const uint32_t withm = __ballot_sync(0xFFFFFFFFu, valid && ml > 0);
                 zk_d2_progress(sm, c, ~withm, lane);
@@ -1731,6 +1652,7 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
 
 // CTAs are persistent: each pulls segments from a work counter until none is left.  Segments never wait for each other,
 // so a CTA that is not resident holds nobody up.
+template <bool PREFIX>
 __device__ __forceinline__ void zk_exec_body(ZkD2Smem& sm, const ZkDecodeArgs& a, uint32_t ring_bytes) {
     if (a.counters->overflow) return;
     const uint32_t nseg = a.counters->n_long;
@@ -1739,7 +1661,7 @@ __device__ __forceinline__ void zk_exec_body(ZkD2Smem& sm, const ZkDecodeArgs& a
         __syncthreads();
         const uint32_t s = sm.seg;
         if (s >= nseg) break;
-        zk_exec_segment(sm, a, ring_bytes, a.seg_list[s]);
+        zk_exec_segment<PREFIX>(sm, a, ring_bytes, a.seg_list[s]);
         __syncthreads();                          // every warp is done with the segment before its state is reset
     }
 }
@@ -1760,6 +1682,7 @@ __device__ __forceinline__ void zk_exec_body(ZkD2Smem& sm, const ZkDecodeArgs& a
 #define ZK_XW_WARPS 4u          // warps per CTA; __launch_bounds__ below asks for 8 CTAs (32 warps) per SM, i.e. <= 64 registers
 #define ZK_XW_WIN 4096u         // window bytes per warp (H100, bench mix: 2 KiB ran as fast, 8 KiB 9 % slower)
 
+template <bool PREFIX>
 __device__ __forceinline__ void zk_exec_warp_segment(const ZkDecodeArgs& a, uint8_t* win, uint32_t first_bidx, int lane) {
     const ZkBlock& head = a.blocks[first_bidx];
     const uint32_t e = head.entry, pos0 = head.out_pos;
@@ -1802,8 +1725,8 @@ __device__ __forceinline__ void zk_exec_warp_segment(const ZkDecodeArgs& a, uint
             const uint32_t le = s_lit[sc], oe = s_out[sc], offv = valid ? a.seq_off[seq_base + s] : 0u;
             uint32_t le_prev = __shfl_up_sync(0xFFFFFFFFu, le, 1), oe_prev = __shfl_up_sync(0xFFFFFFFFu, oe, 1);
             if (lane == 0) { le_prev = le_last; oe_prev = oe_last; }
-            const uint32_t ll = le - le_prev, ml = (oe - oe_prev) - ll;
-            const uint32_t o_lit = pos + oe_prev, md = o_lit + ll;
+            const uint32_t ll = le - le_prev; uint32_t ml = (oe - oe_prev) - ll;
+            const uint32_t o_lit = pos + oe_prev; uint32_t md = o_lit + ll;   // (PREFIX: md / ml shrink to the in-frame part)
             uint32_t off = offv;
             bool bad = false;
             if (valid) {
@@ -1812,12 +1735,16 @@ __device__ __forceinline__ void zk_exec_warp_segment(const ZkDecodeArgs& a, uint
                     const uint32_t r = sl == 0 ? R0 : (sl == 1 ? R1 : R2);
                     bad = r <= dl; off = r - dl;
                 }
-                if (off == 0 || off > md - zstart) bad = true;
+                if (off == 0 || off > md - zstart + (PREFIX ? a.prefix_len : 0u)) bad = true;
             }
             if (__any_sync(0xFFFFFFFFu, bad)) { bad_block = bi; break; }
             le_last = __shfl_sync(0xFFFFFFFFu, le, 31); oe_last = __shfl_sync(0xFFFFFFFFu, oe, 31);
             const uint32_t chunk_start = pos + __shfl_sync(0xFFFFFFFFu, oe_prev, 0), chunk_end = pos + oe_last;
             const bool direct = chunk_end - chunk_start > half;
+            if (PREFIX) {
+                if (direct) zk_prefix_part<false>(rg, a, valid, zstart, off, md, ml);
+                else zk_prefix_part<true>(rg, a, valid, zstart, off, md, ml);
+            }
             const uint32_t src0 = md - off, need_end = src0 + (ml < off ? ml : off);
             const bool near_src = !direct && src0 + half >= chunk_start;
             if (direct) zk_chunk_literals<false>(rg, lit, lit_kind, lit_byte, le, le_prev, o_lit, lane);
@@ -1896,6 +1823,7 @@ __device__ __forceinline__ void zk_exec_warp_segment(const ZkDecodeArgs& a, uint
 }
 
 // Persistent: every warp pulls short segments from its own work counter until none is left.
+template <bool PREFIX>
 __global__ void __launch_bounds__(32 * ZK_XW_WARPS, 8) zk_exec_warp_kernel(ZkDecodeArgs a) {
     ZK_DYN_SMEM(win_mem);
     if (a.counters->overflow) return;
@@ -1907,407 +1835,22 @@ __global__ void __launch_bounds__(32 * ZK_XW_WARPS, 8) zk_exec_warp_kernel(ZkDec
         if (lane == 0) s = atomicAdd(&a.work_counter[3], 1u);
         s = __shfl_sync(0xFFFFFFFFu, s, 0);
         if (s >= nshort) break;
-        zk_exec_warp_segment(a, win, a.seg_list[a.cap_blocks - 1 - s], lane);
+        zk_exec_warp_segment<PREFIX>(a, win, a.seg_list[a.cap_blocks - 1 - s], lane);
     }
-}
-
-// =============================================================================================
-// K-D2 (second generation): the same job with in-order bookkeeping only.
-//
-// Profiling the dataflow kernel above showed about 3 500 warp instructions per
-// 32-sequence chunk at 15 warps per SM: it was bound by instruction issue, not by the dependency chain of a frame (a
-// frame whose every chunk waits for its predecessor would still finish in ~2 ms at ~1 000 cycles per chunk).  This
-// version keeps the shared-memory ring, the 32-sequence chunks dealt round-robin to the W warps of the CTA and the ring
-// discipline (start rule, near / far sources, direct path for oversized chunks), and replaces the per-sequence dataflow
-// (descriptor search, completion masks, pre-announcement) by ONE monotone counter:
-//   done_pos     every byte below it is final in the ring (or in HBM, for the direct path);  a match may go as soon as
-//                the part of its source that lies before its own chunk is below done_pos and the part inside its chunk
-//                is below the chunk's own frontier (the destination of its first pending match);
-//   the OLDEST unfinished chunk publishes its frontier after every round, so dependants in the next chunk start while it
-//   is still running; finished chunks are published in order by whoever polls (per-chunk flags, "helping").
-// About a fifth of the instructions per chunk, <= 64 registers, so 32 warps per SM stay resident.
-// =============================================================================================
-#define ZK_X2_META 64u
-#define ZK_X2_G 1u                       // items per group (one warp runs a group's items back to back: only group boundaries cost a cross-warp hand-off)
-struct ZkX2Smem {
-    unsigned long long ev_done, ev_flush;  // events (mbarriers): done_pos / done_chunk moved; flushed_pos / flushed_chunk moved
-    uint32_t done_pos, done_chunk;         // every byte below done_pos is final and readable; chunks [0, done_chunk) are done
-    uint32_t flushed_pos, flushed_chunk;   // ... and below flushed_pos it is in HBM too (ring slots may be reused)
-    int abort_code;
-    uint32_t end[ZK_X2_META], done[ZK_X2_META], flushed[ZK_X2_META];   // slot = chunk & 63; valid for chunk k iff tag == k + 1 (end: written before done)
-};
-#define ZK_X2_HINT_NS 20000u               // upper bound of one sleep (a missed wake-up costs at most this)
-
-__device__ __forceinline__ void zk_x2_abort(ZkX2Smem& sm, int code) {
-    // exactly ONE thread of the CTA ever signals the abort: an event has an arrival count of one, and a warp-wide arrive
-    // (32 arrivals in one instruction) would underflow it
-    if (atomicCAS(&sm.abort_code, 0, code) == 0) {
-        __threadfence_block();
-        zk_event_signal(&sm.ev_done); zk_event_signal(&sm.ev_flush);
-    }
-}
-__device__ __forceinline__ bool zk_x2_aborted(ZkX2Smem& sm) { return __any_sync(0xFFFFFFFFu, *(volatile int*)&sm.abort_code != 0); }
-
-// advance the in-order prefixes as far as the per-chunk flags allow and wake the sleepers (called by whoever just set a flag)
-__device__ __noinline__ void zk_x2_advance_done(ZkX2Smem& sm) {
-    uint32_t dc = ZK_VOL(sm.done_chunk), dc0 = dc, dp = 0;
-    while (ZK_VOL(sm.done[dc & (ZK_X2_META - 1)]) == dc + 1) { dp = ZK_VOL(sm.end[dc & (ZK_X2_META - 1)]); dc++; }
-    if (dc != dc0) { atomicMax(&sm.done_pos, dp); __threadfence_block(); atomicMax(&sm.done_chunk, dc); __threadfence_block(); zk_event_signal(&sm.ev_done); }
-}
-__device__ __noinline__ void zk_x2_advance_flushed(ZkX2Smem& sm) {
-    uint32_t fc = ZK_VOL(sm.flushed_chunk), fc0 = fc, fp = 0;
-    while (ZK_VOL(sm.flushed[fc & (ZK_X2_META - 1)]) == fc + 1) { fp = ZK_VOL(sm.end[fc & (ZK_X2_META - 1)]); fc++; }
-    if (fc != fc0) { atomicMax(&sm.flushed_pos, fp); __threadfence_block(); atomicMax(&sm.flushed_chunk, fc); __threadfence_block(); zk_event_signal(&sm.ev_flush); }
-}
-
-// warp-uniform wait until an item of group g (ending at end_pos) may start; false if the CTA aborted.
-// exclusive: every earlier group is done and flushed (the item then runs alone, HBM to HBM; earlier items of the same group
-// were flushed by this very warp).
-__device__ __forceinline__ bool zk_x2_wait_start(ZkX2Smem& sm, uint32_t g, uint32_t end_pos, uint32_t window, bool exclusive, int lane) {
-    uint32_t ok = 0;
-    if (lane == 0) {
-        uint32_t ph = 2;                                                     // parity not known yet
-        for (;;) {
-            const uint32_t fg = ZK_VOL(sm.flushed_chunk), fp = ZK_VOL(sm.flushed_pos);
-            if (exclusive ? (fg == g) : (fg == g || (end_pos - fp <= window && g - fg < ZK_X2_META - 2))) { ok = 1; break; }
-            if (*(volatile int*)&sm.abort_code != 0) break;
-            if (ph == 2) { ph = zk_event_parity(&sm.ev_flush); continue; }   // learn the phase, then look again before sleeping
-            if (zk_event_sleep(&sm.ev_flush, ph, ZK_X2_HINT_NS)) ph ^= 1;
-        }
-    }
-    return __shfl_sync(0xFFFFFFFFu, ok, 0) != 0;
-}
-// lane 0: sleep until done_pos >= want (returns the value seen) or the CTA aborts (returns 0xFFFFFFFF)
-__device__ __forceinline__ uint32_t zk_x2_wait_done_pos(ZkX2Smem& sm, uint32_t want) {
-    uint32_t ph = 2;
-    for (;;) {
-        const uint32_t dp = ZK_VOL(sm.done_pos);
-        if (dp >= want) return dp;
-        if (*(volatile int*)&sm.abort_code != 0) return 0xFFFFFFFFu;
-        if (ph == 2) { ph = zk_event_parity(&sm.ev_done); continue; }
-        if (zk_event_sleep(&sm.ev_done, ph, ZK_X2_HINT_NS)) ph ^= 1;
-    }
-}
-// an item of group g, ending at end_pos, is final in the ring (or in HBM).  The last item of a group publishes the group;
-// before that, the OLDEST group publishes its progress item by item (dependants need not wait for the whole group).
-__device__ __forceinline__ void zk_x2_item_done(ZkX2Smem& sm, uint32_t g, uint32_t end_pos, bool last, int lane) {
-    __threadfence_block();
-    __syncwarp();
-    if (lane == 0) {
-        if (last) { ZK_VOL(sm.end[g & (ZK_X2_META - 1)]) = end_pos; __threadfence_block(); ZK_VOL(sm.done[g & (ZK_X2_META - 1)]) = g + 1; __threadfence_block(); zk_x2_advance_done(sm); }
-        else if (ZK_VOL(sm.done_chunk) == g && end_pos > ZK_VOL(sm.done_pos)) { atomicMax(&sm.done_pos, end_pos); __threadfence_block(); zk_event_signal(&sm.ev_done); }
-    }
-}
-__device__ __forceinline__ void zk_x2_item_flushed(ZkX2Smem& sm, uint32_t g, uint32_t end_pos, bool last, int lane) {
-    __threadfence_block();
-    __syncwarp();
-    if (lane == 0) {
-        if (last) { ZK_VOL(sm.flushed[g & (ZK_X2_META - 1)]) = g + 1; __threadfence_block(); zk_x2_advance_flushed(sm); }
-        else if (ZK_VOL(sm.flushed_chunk) == g && end_pos > ZK_VOL(sm.flushed_pos)) { atomicMax(&sm.flushed_pos, end_pos); __threadfence_block(); zk_event_signal(&sm.ev_flush); }
-    }
-    __syncwarp();
-}
-
-__device__ __forceinline__ void zk_exec2_body(ZkX2Smem& sm, const ZkDecodeArgs& a, uint32_t ring_bytes) {
-    ZK_DYN_SMEM(ring_mem);
-    const uint32_t e = blockIdx.x;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, W = blockDim.x >> 5;
-    ZkEntry ent = a.entries[e];
-    if (ent.status != 0 || a.counters->overflow) return;
-    if (threadIdx.x == 0) { sm.done_pos = 0; sm.done_chunk = 0; sm.flushed_pos = 0; sm.flushed_chunk = 0; sm.abort_code = 0; zk_event_init(&sm.ev_done); zk_event_init(&sm.ev_flush); }
-    for (uint32_t i = threadIdx.x; i < ZK_X2_META; i += blockDim.x) { sm.done[i] = 0; sm.flushed[i] = 0; sm.end[i] = 0; }
-    __syncthreads();
-    uint8_t* out = a.dst + a.d_off[e];
-    const unsigned long long cap64 = a.d_off[e + 1] - a.d_off[e];
-    const uint32_t cap = cap64 > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)cap64;
-    const uint8_t* ebase = a.comp + a.c_off[e];
-    ZkRing rg; rg.ring = ring_mem; rg.mask = ring_bytes - 1; rg.mis = (uint32_t)((uintptr_t)out & 15); rg.out = out;
-    const uint32_t half = ring_bytes >> 1;
-
-    uint32_t pos = 0, zstart = 0, chunk_base = 0, gstart = 0;
-    uint32_t R0 = 1, R1 = 4, R2 = 8;
-    const uint32_t need = a.d_need ? a.d_need[e] : 0xFFFFFFFFu;      // range reads: stop at the first block boundary at or after the wanted prefix
-    bool stopped = false;
-    for (uint32_t bi = 0; bi < ent.n_blocks; bi++) {
-        if (zk_x2_aborted(sm)) break;
-        if (pos >= need) { stopped = true; break; }
-        const uint32_t bidx = ent.first_block + bi;
-        const ZkBlock blk = a.blocks[bidx];
-        if (blk.flags & ZKB_FIRST) { R0 = 1; R1 = 4; R2 = 8; zstart = pos; }
-        if (blk.status != 0 || blk.lit_status != 0) { zk_x2_abort(sm, blk.status ? -blk.status : -blk.lit_status); break; }
-        const bool has_seq = blk.type == 2 && blk.nseq > 0;
-        const uint32_t nchunks = has_seq ? (blk.nseq + 31) / 32 + 1 : 1;
-        if ((unsigned long long)pos + blk.regen > cap) { zk_x2_abort(sm, ZKZ_DST_TOO_SMALL); break; }
-        // items (32-sequence chunks, trailing literals, whole non-sequence blocks) are numbered through the entry; ZK_X2_G
-        // consecutive items form a group, group g belongs to warp g % W, which runs its items one after the other
-        const uint32_t g_lo = chunk_base / ZK_X2_G;
-        for (uint32_t g = g_lo + ((uint32_t)warp + (uint32_t)W - g_lo % (uint32_t)W) % (uint32_t)W; g * ZK_X2_G < chunk_base + nchunks; g += (uint32_t)W)
-        for (uint32_t c = g * ZK_X2_G > chunk_base ? g * ZK_X2_G : chunk_base; c < (g + 1) * ZK_X2_G && c < chunk_base + nchunks; c++) {
-            const uint32_t j = c - chunk_base;
-            const bool glast = (c + 1) % ZK_X2_G == 0;                       // (the entry's last, incomplete group is closed after the loop)
-            if (!has_seq) {
-                // ---------------- Raw block / RLE block / literals-only compressed block: direct path, runs alone
-                if (c % ZK_X2_G == 0) gstart = pos;
-                if (!zk_x2_wait_start(sm, g, pos + blk.regen, 0, true, lane)) break;
-                if (blk.type == 0) zk_warp_copy(out + pos, ebase + blk.src, blk.size, lane);
-                else if (blk.type == 1) zk_warp_fill(out + pos, ebase[blk.src], blk.size, lane);
-                else if (blk.lit_kind == 1) zk_warp_fill(out + pos, blk.lit_byte, blk.lit_size, lane);
-                else zk_warp_copy(out + pos, blk.lit_kind == 0 ? ebase + blk.lit_src : a.lit + blk.lit_base, blk.lit_size, lane);
-                __syncwarp();
-                { uint32_t en = pos + blk.regen; zk_ring_reload(rg, en > half ? en - half : 0, en, lane, 32); }
-                zk_x2_item_done(sm, g, pos + blk.regen, glast, lane);
-                zk_x2_item_flushed(sm, g, pos + blk.regen, glast, lane);
-                continue;
-            }
-            const uint32_t* s_lit = a.seq_lit_end + blk.seq_base;
-            const uint32_t* s_out = a.seq_out_end + blk.seq_base;
-            const uint8_t* lit = blk.lit_kind == 0 ? ebase + blk.lit_src : a.lit + blk.lit_base;
-            if (j == nchunks - 1) {
-                // ---------------- trailing literals of the block
-                const uint32_t le = s_lit[blk.nseq - 1], oe = s_out[blk.nseq - 1];
-                const uint32_t n = blk.lit_size - le, st0 = pos + oe, en = pos + blk.regen;
-                const bool direct = n > half;
-                if (c % ZK_X2_G == 0) gstart = st0;
-                if (!zk_x2_wait_start(sm, g, en, half, direct, lane)) break;
-                if (direct) {
-                    if (blk.lit_kind == 1) zk_warp_fill(out + st0, blk.lit_byte, n, lane);
-                    else zk_warp_copy(out + st0, lit + le, n, lane);
-                    __syncwarp();
-                    zk_ring_reload(rg, en - half, en, lane, 32);
-                    zk_x2_item_done(sm, g, en, glast, lane);
-                } else {
-                    for (uint32_t i = lane; i < n; i += 32) rg.at(st0 + i) = blk.lit_kind == 1 ? blk.lit_byte : lit[le + i];
-                    zk_x2_item_done(sm, g, en, glast, lane);
-                    __syncwarp();
-                    zk_ring_flush(rg, st0, en, lane);
-                }
-                zk_x2_item_flushed(sm, g, en, glast, lane);
-                continue;
-            }
-            // ---------------- 32 sequences, one per lane (all loads issued before the first use)
-            const uint32_t s = j * 32 + lane;
-            const bool valid = s < blk.nseq;
-            const uint32_t sc = valid ? s : blk.nseq - 1;      // lanes past the last sequence repeat its cumulative ends (zero-length runs)
-            const uint32_t le = s_lit[sc], oe = s_out[sc];
-            const uint32_t offv = valid ? a.seq_off[blk.seq_base + s] : 0u;
-            uint32_t le_first = 0, oe_first = 0;
-            if (lane == 0 && s) { le_first = s_lit[s - 1]; oe_first = s_out[s - 1]; }
-            uint32_t le_prev = __shfl_up_sync(0xFFFFFFFFu, le, 1), oe_prev = __shfl_up_sync(0xFFFFFFFFu, oe, 1);
-            if (lane == 0) { le_prev = le_first; oe_prev = oe_first; }
-            const uint32_t ll = le - le_prev; uint32_t ml = (oe - oe_prev) - ll;
-            const uint32_t o_lit = pos + oe_prev; uint32_t md = o_lit + ll;  // entry-relative positions (md / ml shrink to the in-frame part of a prefix match below)
-            uint32_t off = offv;
-            bool bad = false;
-            if (valid) {
-                if (offv & ZK_SYM) {
-                    const uint32_t sl = ZK_SYM_SLOT(offv), dl = ZK_SYM_DELTA(offv);
-                    const uint32_t r = sl == 0 ? R0 : (sl == 1 ? R1 : R2);
-                    bad = r <= dl; off = r - dl;
-                }
-                if (off == 0 || off > md - zstart + a.prefix_len) bad = true;
-            }
-            if (__any_sync(0xFFFFFFFFu, bad)) { zk_x2_abort(sm, ZKZ_CORRUPTION); break; }
-            const uint32_t chunk_start = pos + __shfl_sync(0xFFFFFFFFu, oe_prev, 0);
-            const uint32_t chunk_end = pos + __shfl_sync(0xFFFFFFFFu, oe, 31);
-            const bool direct = chunk_end - chunk_start > half;
-            if (c % ZK_X2_G == 0) gstart = chunk_start;
-            if (!glast && j + 2 < nchunks) {      // the next item is this warp's too: pull its sequences and the start of its literals towards L1
-                const uint32_t le_last = __shfl_sync(0xFFFFFFFFu, le, 31);
-                if (lane == 0) { zk_prefetch_l1(s_lit + s + 32); zk_prefetch_l1(s_out + s + 32); zk_prefetch_l1(a.seq_off + blk.seq_base + s + 32); }
-                if (lane >= 4 && lane < 8 && blk.lit_kind != 1) zk_prefetch_l1(lit + le_last + (uint32_t)(lane - 4) * 64u);
-            }
-            if (!zk_x2_wait_start(sm, g, chunk_end, half, direct, lane)) break;
-
-            if (direct) {
-                // ======== huge chunk: HBM -> HBM, alone in flight (it is the oldest chunk and everything before it is flushed)
-                {
-                    uint32_t longlit = __ballot_sync(0xFFFFFFFFu, valid && ll >= 256);
-                    if (!longlit) zk_chunk_literals<false>(rg, lit, blk.lit_kind, blk.lit_byte, le, le_prev, o_lit, lane);
-                    else {
-                        if (valid && ll < 256) {
-                            uint8_t* d = out + o_lit;
-                            if (blk.lit_kind == 1) for (uint32_t i = 0; i < ll; i++) d[i] = blk.lit_byte;
-                            else { const uint8_t* sp = lit + le_prev; for (uint32_t i = 0; i < ll; i++) d[i] = sp[i]; }
-                        }
-                        while (longlit) {
-                            const int l = __ffs((int)longlit) - 1; longlit &= longlit - 1;
-                            const uint32_t n = __shfl_sync(0xFFFFFFFFu, ll, l), d = __shfl_sync(0xFFFFFFFFu, o_lit, l), sp = __shfl_sync(0xFFFFFFFFu, le_prev, l);
-                            if (blk.lit_kind == 1) zk_warp_fill(out + d, blk.lit_byte, n, lane);
-                            else zk_warp_copy(out + d, lit + sp, n, lane);
-                        }
-                    }
-                }
-                if (valid && ml > 0 && off > md - zstart) {          // the match starts in the prefix
-                    const uint32_t back = off - (md - zstart), la = ml < back ? ml : back;
-                    const uint8_t* ps = a.prefix + (a.prefix_len - back);
-                    for (uint32_t i = 0; i < la; i++) out[md + i] = ps[i];
-                    md += la; ml -= la;
-                }
-                __threadfence_block();
-                __syncwarp();
-                const uint32_t need_end = md - off + (ml < off ? ml : off);
-                uint32_t pending = __ballot_sync(0xFFFFFFFFu, valid && ml > 0);
-                while (pending) {
-                    const int first = __ffs((int)pending) - 1;
-                    const uint32_t frontier = __shfl_sync(0xFFFFFFFFu, md, first);
-                    const bool mine = (pending >> lane) & 1;
-                    const bool ready = mine && (need_end <= frontier || lane == first);
-                    const uint32_t rmask = __ballot_sync(0xFFFFFFFFu, ready);
-                    if (ready && ml < ZK_LONG) {
-                        uint8_t* d = out + md; const uint8_t* sp = d - off;
-                        for (uint32_t i = 0; i < ml; i++) d[i] = sp[i];
-                    }
-                    uint32_t longm = __ballot_sync(0xFFFFFFFFu, ready && ml >= ZK_LONG);
-                    while (longm) {
-                        const int l = __ffs((int)longm) - 1; longm &= longm - 1;
-                        const uint32_t n = __shfl_sync(0xFFFFFFFFu, ml, l), d = __shfl_sync(0xFFFFFFFFu, md, l), o = __shfl_sync(0xFFFFFFFFu, off, l);
-                        zk_warp_match(out + d, o, n, lane);
-                    }
-                    __threadfence_block();
-                    __syncwarp();
-                    pending &= ~rmask;
-                }
-                zk_ring_reload(rg, chunk_end - half, chunk_end, lane, 32);
-                zk_x2_item_done(sm, g, chunk_end, glast, lane);
-                zk_x2_item_flushed(sm, g, chunk_end, glast, lane);
-                continue;
-            }
-
-            // ======== normal chunk: build the output in the ring, then flush
-            zk_chunk_literals<true>(rg, lit, blk.lit_kind, blk.lit_byte, le, le_prev, o_lit, lane);      // no dependencies
-            if (a.prefix_len && valid && ml > 0 && off > md - zstart) {
-                // the match starts in the raw-content prefix that precedes every zstd frame: that part is constant data, copied now;
-                // what is left of the match (if anything) starts at the frame's first byte and is an ordinary match
-                const uint32_t back = off - (md - zstart), la = ml < back ? ml : back;
-                const uint8_t* ps = a.prefix + (a.prefix_len - back);
-                for (uint32_t i = 0; i < la; i++) rg.at(md + i) = ps[i];
-                md += la; ml -= la;
-            }
-            // matches.  near: the source is still resident in the ring (distance < R/2 from the chunk start); far: it is in HBM
-            // (flushed, by the start rule) and has no dependency on anything in flight.
-            const uint32_t src0 = md - off;
-            const bool has_m = valid && ml > 0;
-            const bool near_src = src0 + half >= chunk_start;
-            const uint32_t need_end = src0 + (ml < off ? ml : off);
-            const bool ext_dep = near_src && src0 < gstart;                            // part of the source was produced by OTHER warps' groups
-            const uint32_t ext_need = need_end < gstart ? need_end : gstart;           // (earlier items of this group are final: program order)
-            bool aborted = false;
-            // ---- far matches first: nothing to wait for.  Short ones lane by lane with all the loads of up to 16 bytes in flight at
-            // once (one round trip for most matches), long ones by the whole warp.
-            {
-                const bool far_m = has_m && !near_src;
-                if (far_m && ml < ZK_LONG) {
-                    const uint8_t* sp = out + src0;
-                    for (uint32_t i = 0; i < ml; i += 16) {
-                        const unsigned long long v0 = zk_ld8_unaligned(sp + i), v1 = ml - i > 8 ? zk_ld8_unaligned(sp + i + 8) : 0ull;
-                        rg.st8(md + i, (uint32_t)v0, (uint32_t)(v0 >> 32), ml - i);
-                        if (ml - i > 8) rg.st8(md + i + 8, (uint32_t)v1, (uint32_t)(v1 >> 32), ml - i - 8);
-                    }
-                }
-                uint32_t longf = __ballot_sync(0xFFFFFFFFu, far_m && ml >= ZK_LONG);
-                while (longf) {
-                    const int l = __ffs((int)longf) - 1; longf &= longf - 1;
-                    const uint32_t n = __shfl_sync(0xFFFFFFFFu, ml, l), d = __shfl_sync(0xFFFFFFFFu, md, l), o = __shfl_sync(0xFFFFFFFFu, off, l);
-                    const uint8_t* sp = out + (d - o);
-                    for (uint32_t i = lane; i < n; i += 32) rg.at(d + i) = sp[i];
-                }
-            }
-            uint32_t pending = __ballot_sync(0xFFFFFFFFu, has_m && near_src);
-            __threadfence_block();
-            __syncwarp();                                                              // literals and far matches are visible to every lane
-            uint32_t dp = __shfl_sync(0xFFFFFFFFu, ZK_VOL(sm.done_pos), 0);          // one reading for the whole warp (the branches below must be uniform)
-            while (pending) {
-                const int first = __ffs((int)pending) - 1;
-                const uint32_t frontier = __shfl_sync(0xFFFFFFFFu, md, first);       // inside this chunk everything below it is final
-                const bool mine = (pending >> lane) & 1;
-                const bool int_ok = mine && need_end <= frontier;                      // (always true for the first pending lane)
-                // the smallest done_pos that lets some lane go; sleep until it is reached (one lane sleeps, the warp issues nothing)
-                const uint32_t want = __reduce_min_sync(0xFFFFFFFFu, int_ok ? (ext_dep ? ext_need : 0u) : 0xFFFFFFFFu);
-                if (want > dp) {
-                    uint32_t v = 0;
-                    if (lane == 0) v = zk_x2_wait_done_pos(sm, want);
-                    dp = __shfl_sync(0xFFFFFFFFu, v, 0);
-                    if (dp == 0xFFFFFFFFu) { aborted = true; break; }
-                    __threadfence_block();         // acquire: done_pos was read before the data is
-                }
-                const bool ready = int_ok && (!ext_dep || ext_need <= dp);
-                const uint32_t rmask = __ballot_sync(0xFFFFFFFFu, ready);
-                if (ready && ml < ZK_LONG) rg.copy_near(md, src0, ml);
-                uint32_t longm = __ballot_sync(0xFFFFFFFFu, ready && ml >= ZK_LONG);
-                while (longm) {
-                    const int l = __ffs((int)longm) - 1; longm &= longm - 1;
-                    const uint32_t n = __shfl_sync(0xFFFFFFFFu, ml, l), d = __shfl_sync(0xFFFFFFFFu, md, l), o = __shfl_sync(0xFFFFFFFFu, off, l);
-                    if (o >= n) { for (uint32_t i = lane; i < n; i += 32) rg.at(d + i) = rg.at(d - o + i); }
-                    else if (o >= 32) {           // overlapping, period >= 32: 32 bytes per step are already final
-                        for (uint32_t i0 = 0; i0 < n; i0 += 32) { const uint32_t i = i0 + lane; if (i < n) rg.at(d + i) = rg.at(d - o + i); __syncwarp(); }
-                    } else {                      // short period: replicate the pattern
-                        for (uint32_t i = lane; i < n; i += 32) rg.at(d + i) = rg.at(d - o + (i % o));
-                    }
-                }
-                pending &= ~rmask;
-                __threadfence_block();
-                __syncwarp();
-                // the oldest unfinished chunk publishes its frontier: dependants in later chunks need not wait for the whole chunk
-                if (pending) {
-                    const uint32_t nf = __shfl_sync(0xFFFFFFFFu, md, __ffs((int)pending) - 1);
-                    if (lane == 0 && ZK_VOL(sm.done_chunk) == g && nf > ZK_VOL(sm.done_pos)) {
-                        atomicMax(&sm.done_pos, nf); __threadfence_block(); zk_event_signal(&sm.ev_done);
-                    }
-                }
-            }
-            if (aborted) break;
-            zk_x2_item_done(sm, g, chunk_end, glast, lane);        // dependants can read the ring now ...
-            __syncwarp();
-            zk_ring_flush(rg, chunk_start, chunk_end, lane);       // ... while the HBM flush happens off the critical chain
-            zk_x2_item_flushed(sm, g, chunk_end, glast, lane);
-        }
-        // advance to the next block
-        if (has_seq) {
-            uint32_t v[3] = { blk.rep_out[0], blk.rep_out[1], blk.rep_out[2] }, n[3];
-            for (int q = 0; q < 3; q++) {
-                if (v[q] & ZK_SYM) { const uint32_t sl = ZK_SYM_SLOT(v[q]); const uint32_t r = sl == 0 ? R0 : (sl == 1 ? R1 : R2); n[q] = r - ZK_SYM_DELTA(v[q]); }
-                else n[q] = v[q];
-            }
-            R0 = n[0]; R1 = n[1]; R2 = n[2];
-        }
-        pos += blk.regen;
-        chunk_base += nchunks;
-        if (blk.flags & ZKB_LAST) {
-            if ((blk.flags & ZKB_HAS_FCS) && blk.fcs != (unsigned long long)(pos - zstart)) { zk_x2_abort(sm, ZKZ_CORRUPTION); break; }
-            if (threadIdx.x == 0) { a.blocks[bidx].hash_start = zstart; a.blocks[bidx].hash_len = pos - zstart; }
-        }
-    }
-    if (chunk_base % ZK_X2_G && (chunk_base / ZK_X2_G) % (uint32_t)W == (uint32_t)warp && !zk_x2_aborted(sm)) {
-        // the entry's last group has fewer than ZK_X2_G items: its owner closes it (nobody waits on it any more, but the
-        // in-order prefixes stay exact)
-        zk_x2_item_done(sm, chunk_base / ZK_X2_G, pos, true, lane);
-        zk_x2_item_flushed(sm, chunk_base / ZK_X2_G, pos, true, lane);
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        int code = sm.abort_code;
-        if (!code && !stopped && (unsigned long long)pos != cap64) code = pos < cap64 ? ZKZ_SRC_SIZE_WRONG : ZKZ_DST_TOO_SMALL;
-        a.entries[e].status = code ? -code : 0;
-        a.entries[e].produced = pos;
-        if (code) atomicAdd(&a.counters->n_errors, 1u);
-    }
-}
-
-__global__ void __launch_bounds__(1024, 1) zk_exec2_kernel(ZkDecodeArgs a, uint32_t ring_bytes) {
-    __shared__ ZkX2Smem sm;
-    zk_exec2_body(sm, a, ring_bytes);
 }
 
 // Two register budgets for the same body: up to 16 warps per entry (<= 128 registers, few entries per SM), and a
 // 5-warp variant compiled for 4 CTAs per SM (<= 102 registers) for large batches, where every entry of the batch should
 // stay resident and the warps per SM are what hides the latency.
+template <bool PREFIX>
 __global__ void __launch_bounds__(512, 1) zk_exec_kernel(ZkDecodeArgs a, uint32_t ring_bytes) {
     __shared__ ZkD2Smem sm;
-    zk_exec_body(sm, a, ring_bytes);
+    zk_exec_body<PREFIX>(sm, a, ring_bytes);
 }
+template <bool PREFIX>
 __global__ void __launch_bounds__(160, 4) zk_exec_kernel_w5(ZkDecodeArgs a, uint32_t ring_bytes) {
     __shared__ ZkD2Smem sm;
-    zk_exec_body(sm, a, ring_bytes);
+    zk_exec_body<PREFIX>(sm, a, ring_bytes);
 }
 
 // =============================================================================================
@@ -2476,13 +2019,15 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     ws->prof.end(0, stream);
     // entropy stage: persistent warp-CTAs pulling groups of blocks from a work counter
     size_t est_blocks = (size_t)(total_d / ZK_BLOCK_MAX) + n;
-    const size_t seq_smem = ((sizeof(ZkSeqTabs) + 15) & ~(size_t)15) + sizeof(ZkSeqSlot) * ZK_SEQ_LANES, huf_smem = sizeof(ZkHufTab) * ZK_HUF_SLOTS + sizeof(ZkHufScratch);
+    const size_t huf_smem = sizeof(ZkHufTab) * ZK_HUF_SLOTS + sizeof(ZkHufScratch);
+    const size_t seq2_smem = ((sizeof(ZkSeqTabs) + 127) & ~(size_t)127) + sizeof(ZkSeq2Chain) * ZK_S2_NCH;
     if (!ws->attr_set) {
-        ZK_CUDA_OK(cudaFuncSetAttribute(zk_seq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)seq_smem));
+        ZK_CUDA_OK(cudaFuncSetAttribute(zk_seq2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)seq2_smem));
         ZK_CUDA_OK(cudaFuncSetAttribute(zk_huf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)huf_smem + 65536));
-        ZK_CUDA_OK(cudaFuncSetAttribute(zk_exec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
-        ZK_CUDA_OK(cudaFuncSetAttribute(zk_exec_kernel_w5, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
-        ZK_CUDA_OK(cudaFuncSetAttribute(zk_exec2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
+        ZK_CUDA_OK(cudaFuncSetAttribute(zk_exec_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
+        ZK_CUDA_OK(cudaFuncSetAttribute(zk_exec_kernel_w5<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
+        ZK_CUDA_OK(cudaFuncSetAttribute(zk_exec_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
+        ZK_CUDA_OK(cudaFuncSetAttribute(zk_exec_kernel_w5<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
         ws->attr_set = true;
     }
     if (!ws->huf_fit) {                          // K-D1h CTAs that fit on an SM by their shared memory (+ the tuning pad)
@@ -2497,9 +2042,8 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     // Half of them: K-D1s runs beside K-D1h, and the two only overlap when both fit on the SM (DESIGN §6).  Two K-D1h CTAs are
     // resident beside K-D1s's five, the rest start as K-D1s's CTAs finish.
     const uint32_t huf_ctas = ws->huf_ctas ? ws->huf_ctas : (ws->huf_fit > 1 ? ws->huf_fit / 2 : 1u);
-    uint32_t gs = (uint32_t)sms * ws->seq_ctas, gh = (uint32_t)sms * huf_ctas;              // persistent CTAs (K-D1s v1: 4 x 51 KiB, 5 x 41 KiB)
-    size_t need_s = est_blocks / ZK_SEQ_LANES + 1, need_h = est_blocks / ZK_HUF_SLOTS + 1;
-    if (need_s < gs) gs = (uint32_t)need_s;
+    uint32_t gh = (uint32_t)sms * huf_ctas;      // persistent CTAs
+    const size_t need_h = est_blocks / ZK_HUF_SLOTS + 1;
     if (need_h < gh) gh = (uint32_t)need_h;
     // the two entropy kernels are independent: run the Huffman one on a side stream
     cudaStream_t hs = stream;
@@ -2518,10 +2062,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     ws->prof.end(2, hs);
     if (hs != stream) ZK_CUDA_OK(cudaEventRecord(ws->ev_huf, hs));
     ws->prof.begin(1, stream);
-    if (ws->seq_v1) ZK_LAUNCH(zk_seq_kernel, gs, 32 * ZK_SEQ_WARPS, seq_smem, stream, a);
-    else {
-        const size_t seq2_smem = ((sizeof(ZkSeqTabs) + 127) & ~(size_t)127) + sizeof(ZkSeq2Chain) * ZK_S2_NCH;
-        if (!ws->attr_set2) { ZK_CUDA_OK(cudaFuncSetAttribute(zk_seq2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)seq2_smem)); ws->attr_set2 = true; }
+    {
         uint32_t g2 = (uint32_t)sms * ws->seq2_ctas;
         const size_t need2 = est_blocks / ZK_S2_NCH + 1;
         if (need2 < g2) g2 = (uint32_t)need2;
@@ -2536,49 +2077,39 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     int per_sm = (int)(((unsigned long long)n * (unsigned)(ws->share > 0 ? ws->share : 1) + (uint32_t)sms - 1) / (uint32_t)sms);
     if (per_sm < 1) per_sm = 1;
     int W = exec_warps;
-    const bool exec_v2 = ws->exec_v2 || a.prefix_len;
-    a.exec_short = exec_v2 ? 0u : ws->exec_short;
+    a.exec_short = ws->exec_short;
     ws->prof.begin(3, stream);                   // (the exec slot includes the plan kernel)
-    if (!exec_v2) ZK_LAUNCH(zk_plan_kernel, (n + 3) / 4, 128, 0, stream, a);
-    if (exec_v2) {           // (prefix mode exists in the in-order kernel only)
-        // second-generation kernel: <= 64 registers, so 32 warps per SM whatever the split; ring = what is left of the
-        // SM's shared memory per resident entry
-        if (per_sm > 8) per_sm = 8;
-        if (W <= 0) W = 16 / per_sm;        // more warps per frame than this made the in-order chain SLOWER when this kernel was tuned
-        if (W > 32) W = 32;
-        if (W < 2) W = 2;
-        uint32_t ring = 128 * 1024;
-        while (ring > 8 * 1024 && ((size_t)ring + 2048) * (size_t)per_sm > 220 * 1024) ring >>= 1;
-        if (ws->ring_override) ring = ws->ring_override;
-        ZK_LAUNCH(zk_exec2_kernel, n, W * 32, ring, stream, a, ring);
-    } else {
-        // 126 registers/thread -> 16 warps per SM; from four entries per SM on, the 96-register build of the same body
-        // (20 warps per SM, <= 5 per entry) keeps every entry of the batch resident with one more warp each.  One CTA per
-        // entry; the CTAs then share the batch's segments (K-D1p).
-        bool small_regs = false;
-        if (W <= 0) {
-            if (per_sm >= 4) { W = 20 / per_sm; if (W < 2) W = 2; small_regs = true; }
-            else W = 16 / per_sm;
-        } else small_regs = W <= 5 && per_sm >= 4;
-        if (W > 16) W = 16;
-        uint32_t ring = 128 * 1024;
-        while (ring > 8 * 1024 && (size_t)ring * (size_t)per_sm > 200 * 1024) ring >>= 1;
-        if (ws->ring_override) ring = ws->ring_override;
-        if (a.exec_short) {      // short segments first, on single warps; the CTAs below then pull only long ones
-            uint32_t gw = (uint32_t)sms * 8u;
-            const size_t need_w = est_blocks / ZK_XW_WARPS + 1;
-            if (need_w < gw) gw = (uint32_t)need_w;
-            ZK_LAUNCH(zk_exec_warp_kernel, gw, 32 * ZK_XW_WARPS, ZK_XW_WARPS * ZK_XW_WIN, stream, a);
-        }
-        if (small_regs) ZK_LAUNCH(zk_exec_kernel_w5, n, W * 32, ring, stream, a, ring);
-        else ZK_LAUNCH(zk_exec_kernel, n, W * 32, ring, stream, a, ring);
+    ZK_LAUNCH(zk_plan_kernel, (n + 3) / 4, 128, 0, stream, a);
+    // 126 registers/thread -> 16 warps per SM; from four entries per SM on, the 96-register build of the same body
+    // (20 warps per SM, <= 5 per entry) keeps every entry of the batch resident with one more warp each.  One CTA per
+    // entry; the CTAs then share the batch's segments (K-D1p).
+    bool small_regs = false;
+    if (W <= 0) {
+        if (per_sm >= 4) { W = 20 / per_sm; if (W < 2) W = 2; small_regs = true; }
+        else W = 16 / per_sm;
+    } else small_regs = W <= 5 && per_sm >= 4;
+    if (W > 16) W = 16;
+    uint32_t ring = 128 * 1024;
+    while (ring > 8 * 1024 && (size_t)ring * (size_t)per_sm > 200 * 1024) ring >>= 1;
+    if (ws->ring_override) ring = ws->ring_override;
+    // prefix mode: the same executors, built with the prefix split
+    const bool prefix = a.prefix_len != 0;
+    if (a.exec_short) {          // short segments first, on single warps; the CTAs below then pull only long ones
+        uint32_t gw = (uint32_t)sms * 8u;
+        const size_t need_w = est_blocks / ZK_XW_WARPS + 1;
+        if (need_w < gw) gw = (uint32_t)need_w;
+        void (*warp_kernel)(ZkDecodeArgs) = prefix ? zk_exec_warp_kernel<true> : zk_exec_warp_kernel<false>;
+        ZK_LAUNCH(warp_kernel, gw, 32 * ZK_XW_WARPS, ZK_XW_WARPS * ZK_XW_WIN, stream, a);
     }
+    void (*cta_kernel)(ZkDecodeArgs, uint32_t) = small_regs ? (prefix ? zk_exec_kernel_w5<true> : zk_exec_kernel_w5<false>)
+                                                            : (prefix ? zk_exec_kernel<true> : zk_exec_kernel<false>);
+    ZK_LAUNCH(cta_kernel, n, W * 32, ring, stream, a, ring);
     ws->prof.end(3, stream);
     if (verify_checksum) { ws->prof.begin(4, stream); ZK_LAUNCH(zk_xxh64_kernel, (n + 3) / 4, 128, 0, stream, a); ws->prof.end(4, stream); }
     if (ds != stream) { ZK_CUDA_OK(cudaEventRecord(ws->ev_done, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(ds, ws->ev_done, 0)); }
     ZK_CUDA_OK(cudaMemcpyAsync(ws->h_entries, ws->entries, (size_t)n * sizeof(ZkEntry), cudaMemcpyDeviceToHost, ds));
     ZK_CUDA_OK(cudaMemcpyAsync(ws->h_counters, ws->counters, sizeof(ZkCounters), cudaMemcpyDeviceToHost, ds));
-    ws->launches += 4 + (exec_v2 ? 0 : 1) + (a.exec_short ? 1 : 0) + (verify_checksum ? 1 : 0);
+    ws->launches += 5 + (a.exec_short ? 1 : 0) + (verify_checksum ? 1 : 0);
     ws->pending_n = n;
     return 0;
 }

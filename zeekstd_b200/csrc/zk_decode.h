@@ -33,15 +33,14 @@ struct ZkDecodeWs {                   // HBM scratch owned by a zk_ctx, grown on
     const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device pointer for the NEXT enqueue (one-shot, like `need`)
     uint32_t* huf_list = nullptr; uint32_t* seq_list = nullptr; uint32_t* seg_list = nullptr;
     bool attr_set = false; uint32_t ring_override = 0;
-    bool seq_v1 = false, attr_set2 = false; uint32_t seq2_ctas = 5;   // ZK_SEQ_V1=1: the first-generation FSE kernel; persistent CTAs per SM of the second
-                                      // (5 x 35.4 KiB leave room for two K-D1h CTAs beside them; 6 leave none: DESIGN §6)
-    bool exec_v2 = false;             // ZK_EXEC_V2=1: the in-order exec kernel (zk_exec2_kernel) for every batch, not only in prefix mode
+    uint32_t seq2_ctas = 5;           // ZK_SEQ2_CTAS: persistent K-D1s CTAs per SM (5 x 35.4 KiB leave room for two K-D1h CTAs
+                                      // beside them; 6 leave none: DESIGN §6)
     uint32_t exec_short = 128 << 10;  // ZK_EXEC_SHORT: output bytes up to which a segment runs on one warp (zk_exec_warp_kernel); 0 = CTAs only
     uint32_t huf_pad = 0;             // extra dynamic smem per Huffman CTA: fewer resident CTAs -> more L1 for the streams (tuning)
     unsigned long long* trace = nullptr;
     int share = 1;                    // how many batches share the GPU concurrently (host pipeline depth)
     int prio = 0;                     // CUDA stream priority of the side stream (matches the slot's stream)
-    uint32_t seq_ctas = 4, huf_ctas = 0;   // persistent CTAs per SM of the two entropy kernels (tuning: ZK_SEQ_CTAS / ZK_HUF_CTAS); 0: half of huf_fit
+    uint32_t huf_ctas = 0;            // persistent K-D1h CTAs per SM (tuning: ZK_HUF_CTAS); 0: half of huf_fit
     uint32_t huf_fit = 0;             // K-D1h CTAs that fit on an SM (occupancy query at the first launch; 0 = not asked yet)
     bool no_side = false;             // host pipelines: concurrency comes from the other sub-batches; every extra stream costs a hardware queue
     cudaStream_t up = nullptr, down = nullptr;      // host pipelines: dedicated upload / download streams (not owned); nullptr = everything on `stream`
