@@ -111,6 +111,7 @@ extern "C" int32_t zk_ctx_create(int32_t device_ordinal, uint32_t flags, zk_ctx*
         c->slot[i].dws.prio = c->slot[i].ews.prio = prio;
         c->slot[i].dws.sm_count = c->sm_count;
         c->slot[i].dws.ring_override = (uint32_t)zk_env_size("ZK_RING_BYTES", 0);   // tuning / tests: power of two >= 1024
+        c->slot[i].dws.exec_warps = (uint32_t)zk_env_size("ZK_EXEC_WARPS", 0);
         c->slot[i].dws.huf_pad = (uint32_t)zk_env_size("ZK_HUF_PAD", 0);
         c->slot[i].dws.exec_short = (uint32_t)zk_env_size("ZK_EXEC_SHORT", 128 << 10);
         c->slot[i].dws.seq2_ctas = (uint32_t)zk_env_size("ZK_SEQ2_CTAS", 5);
@@ -195,7 +196,7 @@ extern "C" int32_t zk_decompress_frames_dev(zk_ctx* c, const void* d_comp, const
     for (uint32_t first = 0; first < n;) {
         uint32_t end = zk_next_sub(d_off, first, n, sub_bytes, 1u << 20);
         int rc = zk_decode_batch(ws, st, (const uint8_t*)d_comp, c_off + first, d_off + first, end - first, (uint8_t*)d_dst,
-                                 verify, status ? status + first : nullptr, (int)zk_env_size("ZK_EXEC_WARPS", 0));
+                                 verify, status ? status + first : nullptr);
         if (rc && !worst) worst = rc;
         if (rc == ZK_INT_CUDA || rc == -(int)ZKZ_MEMORY_ALLOCATION) return rc;
         first = end;
@@ -251,8 +252,7 @@ static int zk_dec_sub_enqueue(zk_ctx* c, int si, ZkSubDec& sb, const uint8_t* co
     s.dws.share = (int)zk_env_size("ZK_HOST_SHARE", 3);
     s.dws.need = need ? need + f : nullptr;
     s.dws.prefix = c->cur_prefix_len ? c->d_prefix : nullptr; s.dws.prefix_len = c->cur_prefix_len;
-    rc = zk_decode_enqueue(&s.dws, s.stream, s.d_in, sb.c_rel.data(), sb.d_rel.data(), cnt, s.d_out, verify,
-                           (int)zk_env_size("ZK_EXEC_WARPS", 0));
+    rc = zk_decode_enqueue(&s.dws, s.stream, s.d_in, sb.c_rel.data(), sb.d_rel.data(), cnt, s.d_out, verify);
     if (rc) return rc;
     if (tr) tr->mark(s.stream, k, 2);
     if (obytes) ZK_RT_OK(cudaMemcpyAsync(dst + d_off[f], s.d_out, obytes, cudaMemcpyDeviceToHost, ds));

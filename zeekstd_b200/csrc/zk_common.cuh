@@ -109,7 +109,7 @@ struct ZkBlock {                 // one zstd block of one seek-table entry
 #define ZKB_HAS_CSUM 4u          // 4-byte content checksum follows the last block
 #define ZKB_HAS_FCS 8u
 #define ZKB_SEG 16u              // first block of an execution segment   [plan kernel]
-#define ZK_BACK_UNKNOWN 0xFFFFFFFFu   // a symbolic offset, or sequences that were not (successfully) decoded by the second-generation FSE kernel
+#define ZK_BACK_UNKNOWN 0xFFFFFFFFu   // a symbolic offset, or sequences that were not (successfully) decoded
 
 // symbolic repeat offset: "incoming repeat slot s (0..2) minus delta" (delta in 0..2^20)
 #define ZK_SYM 0x80000000u

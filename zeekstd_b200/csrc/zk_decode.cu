@@ -1049,22 +1049,6 @@ __device__ __noinline__ void zk_d2_help(ZkD2Smem& sm) {
     if (fc != fc0) { atomicMax(&sm.flushed_pos, fp); __threadfence_block(); atomicMax(&sm.flushed_chunk, fc); }
 }
 
-// Are all bytes of [src0, need_end) that lie BEFORE this chunk final?  (lane-level; scans the descriptors of the chunks in flight)
-__device__ __forceinline__ bool zk_d2_ext_ready(ZkD2Smem& sm, uint32_t c, uint32_t src0, uint32_t need_end, uint32_t chunk_start) {
-    if (src0 >= chunk_start) return true;                               // purely intra-chunk
-    const uint32_t ne = need_end < chunk_start ? need_end : chunk_start;
-    if (ne <= ZK_VOL(sm.done_pos)) return true;
-    const uint32_t dc = ZK_VOL(sm.done_chunk);
-    for (uint32_t k = c; k-- > dc;) {
-        const uint32_t e = k & (ZK_D2_META - 1);
-        if (ZK_VOL(sm.started[e]) != k + 1) return false;               // its range is not known yet
-        const uint32_t sk = ZK_VOL(sm.start[e]), ek = ZK_VOL(sm.end[e]);
-        if (sk < ne && ek > src0 && ZK_VOL(sm.done[e]) != k + 1) return false;
-        if (sk <= src0) return true;                                    // older chunks end at or before src0
-    }
-    return true;                                                         // reached the done prefix
-}
-
 // warp-cooperative copy of n bytes HBM -> HBM, non-overlapping (or src entirely before dst with distance >= n)
 __device__ __noinline__ void zk_warp_copy(uint8_t* dst, const uint8_t* src, uint32_t n, int lane) {
     uint32_t head = (uint32_t)((16 - ((uintptr_t)dst & 15)) & 15);
@@ -1260,6 +1244,180 @@ __device__ __forceinline__ void zk_prefix_part(const ZkRing& rg, const ZkDecodeA
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// The work both segment executors (zk_exec_segment, zk_exec_warp_segment) share: repeat offsets, loading and checking the
+// sequences of a chunk, blocks without sequences, trailing literals, direct chunks, match copies into the ring and the end
+// of a segment.  A bound check that reached one executor only would accept a corrupt frame on some segment lengths only.
+// ---------------------------------------------------------------------------------------------
+
+// R0..R2 while a segment's blocks execute in order
+struct ZkRepOffsets {
+    uint32_t r0 = 1, r1 = 4, r2 = 8;
+    __device__ __forceinline__ void reset() { r0 = 1; r1 = 4; r2 = 8; }        // a zstd frame starts
+    // the incoming slot a symbolic value (ZK_SYM) names; the value is that minus its ZK_SYM_DELTA
+    __device__ __forceinline__ uint32_t slot(uint32_t v) const { const uint32_t sl = ZK_SYM_SLOT(v); return sl == 0 ? r0 : (sl == 1 ? r1 : r2); }
+    // the state after a block with sequences: its rep_out, symbolic values resolved against the state before it
+    __device__ __forceinline__ void advance(const ZkBlock& blk) {
+        uint32_t n[3];
+        for (int q = 0; q < 3; q++) { const uint32_t v = blk.rep_out[q]; n[q] = (v & ZK_SYM) ? slot(v) - ZK_SYM_DELTA(v) : v; }
+        r0 = n[0]; r1 = n[1]; r2 = n[2];
+    }
+};
+
+// One lane's sequence of a chunk of 32: the literal run lit[le_prev, le) goes to [o_lit, md), then a match of ml bytes at md
+// from md - off (entry-relative positions; PREFIX: md / ml shrink to the in-frame part).  le / oe are the cumulative literal
+// / output ends of the block's sequences; lanes past the block's last sequence repeat its ends (zero-length runs; keeps `le`
+// monotone across the lanes).
+struct ZkLaneSeq {
+    bool valid;
+    uint32_t le, oe, le_prev, oe_prev, ll, ml, o_lit, md, off;
+};
+
+// Load lane `lane`'s sequence of chunk j of a block (sequences seq_base + [32j, 32j + 32) of nseq); le0 / oe0 are lane 0's
+// predecessor ends (those of sequence 32j - 1, 0 for the first chunk).  Resolves a symbolic offset and checks the offset
+// against the output of the frame before it (and the prefix).  Returns, on every lane, whether some lane's offset is bad.
+template <bool PREFIX>
+__device__ __forceinline__ bool zk_lane_seq(ZkLaneSeq& q, const ZkDecodeArgs& a, uint32_t seq_base, uint32_t nseq, const ZkRepOffsets& rep,
+                                            uint32_t j, uint32_t pos, uint32_t zstart, uint32_t le0, uint32_t oe0, int lane) {
+    const uint32_t s = j * 32 + lane;
+    q.valid = s < nseq;
+    const uint32_t sc = q.valid ? s : nseq - 1;
+    q.le = a.seq_lit_end[seq_base + sc]; q.oe = a.seq_out_end[seq_base + sc];
+    const uint32_t offv = q.valid ? a.seq_off[seq_base + s] : 0u;
+    q.le_prev = __shfl_up_sync(0xFFFFFFFFu, q.le, 1); q.oe_prev = __shfl_up_sync(0xFFFFFFFFu, q.oe, 1);
+    if (lane == 0) { q.le_prev = le0; q.oe_prev = oe0; }
+    q.ll = q.le - q.le_prev; q.ml = (q.oe - q.oe_prev) - q.ll;
+    q.o_lit = pos + q.oe_prev; q.md = q.o_lit + q.ll;
+    q.off = offv;
+    bool bad = false;
+    if (q.valid) {
+        if (offv & ZK_SYM) {
+            const uint32_t r = rep.slot(offv), dl = ZK_SYM_DELTA(offv);
+            bad = r <= dl; q.off = r - dl;
+        }
+        if (q.off == 0 || q.off > q.md - zstart + (PREFIX ? a.prefix_len : 0u)) bad = true;
+    }
+    return __any_sync(0xFFFFFFFFu, bad);
+}
+
+__device__ __forceinline__ const uint8_t* zk_block_lit(const ZkDecodeArgs& a, const ZkBlock& blk, const uint8_t* ebase) {
+    return blk.lit_kind == 0 ? ebase + blk.lit_src : a.lit + blk.lit_base;
+}
+
+// A Raw block, an RLE block or a compressed block without sequences: HBM to HBM at [pos, pos + regen), then the ring is
+// reloaded with the last half ring of it (nothing before pos0: that output belongs to another warp or CTA).
+__device__ __forceinline__ void zk_direct_block(const ZkRing& rg, const ZkDecodeArgs& a, const ZkBlock& blk, const uint8_t* ebase,
+                                                uint32_t pos, uint32_t pos0, uint32_t half, int lane) {
+    uint8_t* d = rg.out + pos;
+    const uint32_t en = pos + blk.regen;
+    if (blk.type == 0) zk_warp_copy(d, ebase + blk.src, blk.size, lane);
+    else if (blk.type == 1) zk_warp_fill(d, ebase[blk.src], blk.size, lane);
+    else if (blk.lit_kind == 1) zk_warp_fill(d, blk.lit_byte, blk.lit_size, lane);
+    else zk_warp_copy(d, zk_block_lit(a, blk, ebase), blk.lit_size, lane);
+    __syncwarp();
+    zk_ring_reload(rg, en - pos0 > half ? en - half : pos0, en, lane, 32);
+}
+
+// The literals after a block's last sequence, lit[le, le + n) to [st0, en): more than half a ring HBM to HBM, then the ring is
+// reloaded (the caller runs them alone); else into the ring, and the caller flushes [st0, en).
+__device__ __forceinline__ void zk_trailing_literals(const ZkRing& rg, uint32_t lit_kind, uint32_t lit_byte, const uint8_t* lit, uint32_t le, uint32_t n,
+                                                     uint32_t st0, uint32_t en, uint32_t half, int lane) {
+    if (n > half) {
+        if (lit_kind == 1) zk_warp_fill(rg.out + st0, lit_byte, n, lane);
+        else zk_warp_copy(rg.out + st0, lit + le, n, lane);
+        __syncwarp();
+        zk_ring_reload(rg, en - half, en, lane, 32);
+    } else {
+        for (uint32_t i = lane; i < n; i += 32) rg.at(st0 + i) = lit_kind == 1 ? lit_byte : lit[le + i];
+    }
+}
+
+// A chunk larger than half a ring: built HBM to HBM while everything before it is final (the CTA kernel runs it alone), then
+// the ring is reloaded with its last half ring.  Literal runs of 256 bytes or more are copied by the whole warp, shorter ones
+// byte-parallel; within the chunk, a match goes once every earlier match that its source overlaps is written.
+template <bool PREFIX>
+__device__ __forceinline__ void zk_direct_chunk(const ZkRing& rg, const ZkDecodeArgs& a, uint32_t lit_kind, uint32_t lit_byte, const uint8_t* lit, ZkLaneSeq& q,
+                                                uint32_t zstart, uint32_t chunk_end, uint32_t half, int lane) {
+    uint8_t* out = rg.out;
+    uint32_t longlit = __ballot_sync(0xFFFFFFFFu, q.valid && q.ll >= 256);
+    if (!longlit) zk_chunk_literals<false>(rg, lit, lit_kind, lit_byte, q.le, q.le_prev, q.o_lit, lane);
+    else {
+        if (q.valid && q.ll < 256) {
+            uint8_t* d = out + q.o_lit;
+            if (lit_kind == 1) for (uint32_t i = 0; i < q.ll; i++) d[i] = lit_byte;
+            else { const uint8_t* sp = lit + q.le_prev; for (uint32_t i = 0; i < q.ll; i++) d[i] = sp[i]; }
+        }
+        while (longlit) {
+            int l = __ffs((int)longlit) - 1; longlit &= longlit - 1;
+            uint32_t n = __shfl_sync(0xFFFFFFFFu, q.ll, l), d = __shfl_sync(0xFFFFFFFFu, q.o_lit, l), sp = __shfl_sync(0xFFFFFFFFu, q.le_prev, l);
+            if (lit_kind == 1) zk_warp_fill(out + d, lit_byte, n, lane);
+            else zk_warp_copy(out + d, lit + sp, n, lane);
+        }
+    }
+    if (PREFIX) zk_prefix_part<false>(rg, a, q.valid, zstart, q.off, q.md, q.ml);
+    __syncwarp();
+    const uint32_t need_end = q.md - q.off + (q.ml < q.off ? q.ml : q.off);
+    uint32_t pending = __ballot_sync(0xFFFFFFFFu, q.valid && q.ml > 0);
+    while (pending) {
+        const int first = __ffs((int)pending) - 1;
+        const uint32_t frontier = __shfl_sync(0xFFFFFFFFu, q.md, first);
+        const bool mine = (pending >> lane) & 1;
+        const bool ready = mine && (need_end <= frontier || lane == first);
+        const uint32_t rmask = __ballot_sync(0xFFFFFFFFu, ready);
+        if (ready && q.ml < ZK_LONG) {
+            uint8_t* d = out + q.md; const uint8_t* sp = d - q.off;
+            for (uint32_t i = 0; i < q.ml; i++) d[i] = sp[i];
+        }
+        uint32_t longm = __ballot_sync(0xFFFFFFFFu, ready && q.ml >= ZK_LONG);
+        while (longm) {
+            int l = __ffs((int)longm) - 1; longm &= longm - 1;
+            uint32_t n = __shfl_sync(0xFFFFFFFFu, q.ml, l), d = __shfl_sync(0xFFFFFFFFu, q.md, l), o = __shfl_sync(0xFFFFFFFFu, q.off, l);
+            zk_warp_match(out + d, o, n, lane);
+        }
+        __syncwarp();
+        pending &= ~rmask;
+    }
+    zk_ring_reload(rg, chunk_end - half, chunk_end, lane, 32);
+}
+
+// The matches of the `ready` lanes, built in the ring.  A short one is copied by its lane: from the ring if its source is near
+// (less than half a ring before the chunk start, so all of it is resident), else from HBM, where it is final and never
+// overlaps, 8 bytes per round trip.  A long one (>= ZK_LONG) is copied by the whole warp.
+__device__ __forceinline__ void zk_ring_matches(const ZkRing& rg, bool ready, bool near_src, uint32_t md, uint32_t off, uint32_t ml, int lane) {
+    if (ready && ml < ZK_LONG) {
+        if (near_src) rg.copy_near(md, md - off, ml);
+        else {
+            const uint8_t* sp = rg.out + (md - off);
+            for (uint32_t i = 0; i < ml; i += 8) {
+                const unsigned long long v = zk_ld8_unaligned(sp + i);
+                rg.st8(md + i, (uint32_t)v, (uint32_t)(v >> 32), ml - i < 8 ? ml - i : 8);
+            }
+        }
+    }
+    uint32_t longm = __ballot_sync(0xFFFFFFFFu, ready && ml >= ZK_LONG);
+    while (longm) {
+        const int l = __ffs((int)longm) - 1; longm &= longm - 1;
+        const uint32_t n = __shfl_sync(0xFFFFFFFFu, ml, l), d = __shfl_sync(0xFFFFFFFFu, md, l), o = __shfl_sync(0xFFFFFFFFu, off, l);
+        const bool nr = __shfl_sync(0xFFFFFFFFu, (uint32_t)near_src, l) != 0;
+        if (!nr) { const uint8_t* sp = rg.out + (d - o); for (uint32_t i = lane; i < n; i += 32) rg.at(d + i) = sp[i]; }
+        else if (o >= n) { for (uint32_t i = lane; i < n; i += 32) rg.at(d + i) = rg.at(d - o + i); }
+        else if (o >= 32) {           // overlapping, period >= 32: 32 bytes per step are already final
+            for (uint32_t i0 = 0; i0 < n; i0 += 32) { const uint32_t i = i0 + lane; if (i < n) rg.at(d + i) = rg.at(d - o + i); __syncwarp(); }
+        } else {                      // short period: replicate the pattern
+            for (uint32_t i = lane; i < n; i += 32) rg.at(d + i) = rg.at(d - o + (i % o));
+        }
+    }
+}
+
+// One thread, once a segment is done: record its failure (a bad offset at entry-relative block fail_block; code 0 = none)
+// and, if it was the entry's last segment, write the entry's status.
+__device__ __forceinline__ void zk_segment_end(const ZkDecodeArgs& a, uint32_t e, uint32_t fail_block, int code) {
+    ZkEntry& en = a.entries[e];
+    if (code) atomicMin(&en.fail, ZK_FAIL_KEY(fail_block, ZK_FAIL_EXEC, code));
+    __threadfence();
+    if (atomicSub(&en.segs_left, 1u) == 1u) { __threadfence(); zk_entry_finish(a, e); }   // the entry's last segment
+}
+
 // chunk c's bytes are final in the ring: dependants may read them
 __device__ __forceinline__ void zk_d2_mark_done(ZkD2Smem& sm, uint32_t c, int lane) {
     __threadfence_block();
@@ -1342,14 +1500,14 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
     const uint32_t half = ring_bytes >> 1;
 
     uint32_t pos = pos0, zstart = head.frame_start, chunk_base = 0;
-    uint32_t R0 = 1, R1 = 4, R2 = 8;
+    ZkRepOffsets rep;
     uint32_t preannounced = 0xFFFFFFFFu;          // chunk id this warp has already announced ahead of time
     for (uint32_t bi = first_bidx - ent.first_block; bi < ent.run_blocks; bi++) {
         if (zk_d2_aborted(sm)) break;
         const uint32_t bidx = ent.first_block + bi;
         const ZkBlock blk = a.blocks[bidx];
         if (bidx != first_bidx && (blk.flags & ZKB_SEG)) break;
-        if (blk.flags & ZKB_FIRST) { R0 = 1; R1 = 4; R2 = 8; zstart = pos; }
+        if (blk.flags & ZKB_FIRST) { rep.reset(); zstart = pos; }
         const bool has_seq = blk.type == 2 && blk.nseq > 0;
         const uint32_t nchunks = has_seq ? (blk.nseq + 31) / 32 + 1 : 1;
         // first chunk index of this block that belongs to this warp
@@ -1360,19 +1518,14 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
                 // ---------------- Raw block / RLE block / literals-only compressed block: direct path, runs alone
                 if (!zk_d2_wait_start(sm, c, pos, pos + blk.regen, 0, true, lane)) break;
                 zk_d2_announce(sm, c, pos, pos + blk.regen, pos + blk.regen, 0u, lane);
-                if (blk.type == 0) zk_warp_copy(out + pos, ebase + blk.src, blk.size, lane);
-                else if (blk.type == 1) zk_warp_fill(out + pos, ebase[blk.src], blk.size, lane);
-                else if (blk.lit_kind == 1) zk_warp_fill(out + pos, blk.lit_byte, blk.lit_size, lane);
-                else zk_warp_copy(out + pos, blk.lit_kind == 0 ? ebase + blk.lit_src : a.lit + blk.lit_base, blk.lit_size, lane);
-                __syncwarp();
-                { uint32_t en = pos + blk.regen; zk_ring_reload(rg, en - pos0 > half ? en - half : pos0, en, lane, 32); }   // (output before pos0 belongs to other CTAs)
+                zk_direct_block(rg, a, blk, ebase, pos, pos0, half, lane);
                 zk_d2_mark_done(sm, c, lane);
                 zk_d2_mark_flushed(sm, c, lane);
                 continue;
             }
             const uint32_t* s_lit = a.seq_lit_end + blk.seq_base;
             const uint32_t* s_out = a.seq_out_end + blk.seq_base;
-            const uint8_t* lit = blk.lit_kind == 0 ? ebase + blk.lit_src : a.lit + blk.lit_base;
+            const uint8_t* lit = zk_block_lit(a, blk, ebase);
             if (j == nchunks - 1) {
                 // ---------------- trailing literals of the block
                 const uint32_t le = s_lit[blk.nseq - 1], oe = s_out[blk.nseq - 1];
@@ -1380,56 +1533,22 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
                 const bool direct = n > half;
                 if (!zk_d2_wait_start(sm, c, st0, en, half, direct, lane)) break;
                 zk_d2_announce(sm, c, st0, en, en, 0u, lane);
-                if (direct) {
-                    if (blk.lit_kind == 1) zk_warp_fill(out + st0, blk.lit_byte, n, lane);
-                    else zk_warp_copy(out + st0, lit + le, n, lane);
-                    __syncwarp();
-                    zk_ring_reload(rg, en - half, en, lane, 32);
-                    zk_d2_mark_done(sm, c, lane);
-                } else {
-                    for (uint32_t i = lane; i < n; i += 32) rg.at(st0 + i) = blk.lit_kind == 1 ? blk.lit_byte : lit[le + i];
-                    zk_d2_mark_done(sm, c, lane);
-                    zk_ring_flush(rg, st0, en, lane);
-                }
+                zk_trailing_literals(rg, blk.lit_kind, blk.lit_byte, lit, le, n, st0, en, half, lane);
+                zk_d2_mark_done(sm, c, lane);
+                if (!direct) zk_ring_flush(rg, st0, en, lane);
                 zk_d2_mark_flushed(sm, c, lane);
                 continue;
             }
             // ---------------- 32 sequences, one per lane
-#if !defined(ZK_EMUL) && defined(ZK_EXEC_TRACE_BUILD)       // per-chunk clock64 stamps of entry 0 (tools/exec_trace.py): a debug build only --
-#define ZK_STAMP(k) do { if (a.trace && e == 0 && c < 1024 && lane == 0) a.trace[c * 8 + (k)] = clock64(); } while (0)   // the checks were 3 % of the kernel's instructions
-#else
-#define ZK_STAMP(k) do { } while (0)
-#endif
-            ZK_STAMP(0);
-            const uint32_t s = j * 32 + lane;
-            const bool valid = s < blk.nseq;
-            uint32_t le = 0, oe = 0, offv = 0;
-            {   // lanes past the last sequence of the block repeat its cumulative ends (zero-length runs; keeps `le` monotone)
-                const uint32_t sc = valid ? s : blk.nseq - 1;
-                le = s_lit[sc]; oe = s_out[sc];
-                if (valid) offv = a.seq_off[blk.seq_base + s];
-            }
-            uint32_t le_prev = __shfl_up_sync(0xFFFFFFFFu, le, 1), oe_prev = __shfl_up_sync(0xFFFFFFFFu, oe, 1);
-            if (lane == 0) { le_prev = s ? s_lit[s - 1] : 0; oe_prev = s ? s_out[s - 1] : 0; }
-            const uint32_t ll = le - le_prev; uint32_t ml = (oe - oe_prev) - ll;
-            const uint32_t o_lit = pos + oe_prev; uint32_t md = o_lit + ll;   // entry-relative positions (PREFIX: md / ml shrink to the in-frame part)
-            uint32_t off = offv;
-            bool bad = false;
-            if (valid) {
-                if (offv & ZK_SYM) {
-                    uint32_t sl = ZK_SYM_SLOT(offv), dl = ZK_SYM_DELTA(offv);
-                    uint32_t r = sl == 0 ? R0 : (sl == 1 ? R1 : R2);
-                    bad = r <= dl; off = r - dl;
-                }
-                if (off == 0 || off > md - zstart + (PREFIX ? a.prefix_len : 0u)) bad = true;
-            }
-            if (__any_sync(0xFFFFFFFFu, bad)) { zk_d2_abort(sm, ZKZ_CORRUPTION, bi); break; }
-            const uint32_t chunk_start = pos + __shfl_sync(0xFFFFFFFFu, oe_prev, 0);
-            const uint32_t chunk_end = pos + __shfl_sync(0xFFFFFFFFu, oe, min(31u, blk.nseq - 1 - j * 32));
+            uint32_t le0 = 0, oe0 = 0;
+            if (lane == 0 && j) { le0 = s_lit[j * 32 - 1]; oe0 = s_out[j * 32 - 1]; }
+            ZkLaneSeq q;
+            if (zk_lane_seq<PREFIX>(q, a, blk.seq_base, blk.nseq, rep, j, pos, zstart, le0, oe0, lane)) { zk_d2_abort(sm, ZKZ_CORRUPTION, bi); break; }
+            const uint32_t chunk_start = pos + __shfl_sync(0xFFFFFFFFu, q.oe_prev, 0);
+            const uint32_t chunk_end = pos + __shfl_sync(0xFFFFFFFFu, q.oe, min(31u, blk.nseq - 1 - j * 32));
             const bool direct = chunk_end - chunk_start > half;
-            ZK_STAMP(1);
             if (!zk_d2_wait_start(sm, c, chunk_start, chunk_end, half, direct, lane)) break;
-            if (preannounced != c) zk_d2_announce(sm, c, chunk_start, chunk_end, pos + oe, 0u, lane);
+            if (preannounced != c) zk_d2_announce(sm, c, chunk_start, chunk_end, pos + q.oe, 0u, lane);
             // Announce this warp's NEXT chunk of the block right away (its sequence ends are one coalesced load away): chunks of
             // other warps that depend on it can then resolve their producers without waiting for this warp to get there.
             {
@@ -1449,52 +1568,10 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
                     }
                 }
             }
-            ZK_STAMP(2);
 
             if (direct) {
                 // ======== huge chunk: HBM -> HBM, alone in flight (it is the oldest chunk)
-                {
-                    // short runs byte-parallel; long runs with the vectorised warp copy
-                    uint32_t longlit = __ballot_sync(0xFFFFFFFFu, valid && ll >= 256);
-                    if (!longlit) zk_chunk_literals<false>(rg, lit, blk.lit_kind, blk.lit_byte, le, le_prev, o_lit, lane);
-                    else {
-                        if (valid && ll < 256) {
-                            uint8_t* d = out + o_lit;
-                            if (blk.lit_kind == 1) for (uint32_t i = 0; i < ll; i++) d[i] = blk.lit_byte;
-                            else { const uint8_t* sp = lit + le_prev; for (uint32_t i = 0; i < ll; i++) d[i] = sp[i]; }
-                        }
-                        while (longlit) {
-                            int l = __ffs((int)longlit) - 1; longlit &= longlit - 1;
-                            uint32_t n = __shfl_sync(0xFFFFFFFFu, ll, l), d = __shfl_sync(0xFFFFFFFFu, o_lit, l), sp = __shfl_sync(0xFFFFFFFFu, le_prev, l);
-                            if (blk.lit_kind == 1) zk_warp_fill(out + d, blk.lit_byte, n, lane);
-                            else zk_warp_copy(out + d, lit + sp, n, lane);
-                        }
-                    }
-                }
-                if (PREFIX) zk_prefix_part<false>(rg, a, valid, zstart, off, md, ml);
-                __syncwarp();
-                const uint32_t need_end = md - off + (ml < off ? ml : off);
-                uint32_t pending = __ballot_sync(0xFFFFFFFFu, valid && ml > 0);
-                while (pending) {
-                    const int first = __ffs((int)pending) - 1;
-                    const uint32_t frontier = __shfl_sync(0xFFFFFFFFu, md, first);
-                    const bool mine = (pending >> lane) & 1;
-                    const bool ready = mine && (need_end <= frontier || lane == first);
-                    const uint32_t rmask = __ballot_sync(0xFFFFFFFFu, ready);
-                    if (ready && ml < ZK_LONG) {
-                        uint8_t* d = out + md; const uint8_t* sp = d - off;
-                        for (uint32_t i = 0; i < ml; i++) d[i] = sp[i];
-                    }
-                    uint32_t longm = __ballot_sync(0xFFFFFFFFu, ready && ml >= ZK_LONG);
-                    while (longm) {
-                        int l = __ffs((int)longm) - 1; longm &= longm - 1;
-                        uint32_t n = __shfl_sync(0xFFFFFFFFu, ml, l), d = __shfl_sync(0xFFFFFFFFu, md, l), o = __shfl_sync(0xFFFFFFFFu, off, l);
-                        zk_warp_match(out + d, o, n, lane);
-                    }
-                    __syncwarp();
-                    pending &= ~rmask;
-                }
-                zk_ring_reload(rg, chunk_end - half, chunk_end, lane, 32);
+                zk_direct_chunk<PREFIX>(rg, a, blk.lit_kind, blk.lit_byte, lit, q, zstart, chunk_end, half, lane);
                 zk_d2_mark_done(sm, c, lane);
                 zk_d2_mark_flushed(sm, c, lane);
                 continue;
@@ -1502,22 +1579,21 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
 
             // ======== normal chunk: build the output in the ring, then flush
             // literal runs: no dependencies (HBM scratch -> ring)
-            zk_chunk_literals<true>(rg, lit, blk.lit_kind, blk.lit_byte, le, le_prev, o_lit, lane);
-            if (PREFIX) zk_prefix_part<true>(rg, a, valid, zstart, off, md, ml);
+            zk_chunk_literals<true>(rg, lit, blk.lit_kind, blk.lit_byte, q.le, q.le_prev, q.o_lit, lane);
+            if (PREFIX) zk_prefix_part<true>(rg, a, q.valid, zstart, q.off, q.md, q.ml);
             {   // all literal runs are in place: sequences without a match (and the lanes past the last one) are complete
-                const uint32_t withm = __ballot_sync(0xFFFFFFFFu, valid && ml > 0);
+                const uint32_t withm = __ballot_sync(0xFFFFFFFFu, q.valid && q.ml > 0);
                 zk_d2_progress(sm, c, ~withm, lane);
                 if (lane == 0) ZK_VOL(sm.litdone[c & (ZK_D2_META - 1)]) = c + 1;
             }
             __syncwarp();
-            ZK_STAMP(3);
 
             // matches.  near: the whole source is still resident in the ring (distance < R/2 from the chunk start);
             // far: it is read from HBM and must be published (done_pos).  A lane may go once its source is final.
-            const uint32_t src0 = md - off;
+            const uint32_t src0 = q.md - q.off;
             const bool near_src = src0 + half >= chunk_start;          // src0 >= chunk_start - R/2
-            const uint32_t need_end = src0 + (ml < off ? ml : off);
-            uint32_t pending = __ballot_sync(0xFFFFFFFFu, valid && ml > 0);
+            const uint32_t need_end = src0 + (q.ml < q.off ? q.ml : q.off);
+            uint32_t pending = __ballot_sync(0xFFFFFFFFu, q.valid && q.ml > 0);
             bool aborted = false;
             // dataflow readiness: a match may go as soon as the bytes of its source are final -- the part that lies before this
             // chunk is tracked per chunk (descriptors in shared memory), the part inside this chunk by lane order.  Sources older
@@ -1527,7 +1603,7 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
             uint32_t klo = 1, khi = 0;                                  // empty range: nothing to wait for outside this chunk
             uint32_t mask_lo = 0, mask_hi = 0;                          // which sequences of chunk klo / khi produce my source
             {
-                bool resolved = !(valid && ml > 0) || !near_src || src0 >= chunk_start;
+                bool resolved = !(q.valid && q.ml > 0) || !near_src || src0 >= chunk_start;
                 const uint32_t ne = need_end < chunk_start ? need_end : chunk_start;
                 for (;;) {
                     if (!resolved) {
@@ -1572,8 +1648,6 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
                     ZK_SPIN();
                 }
             }
-            ZK_STAMP(4);
-            bool stamped5 = false;
             while (pending && !aborted) {
                 const bool mine = (pending >> lane) & 1;
                 bool ext_ok = true;
@@ -1588,66 +1662,28 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
                     if (ext_ok) khi = 0, klo = 1;                       // sticky
                 }
                 const int first = __ffs((int)pending) - 1;
-                const uint32_t md_first = __shfl_sync(0xFFFFFFFFu, md, first);   // inside this chunk everything below it is final
+                const uint32_t md_first = __shfl_sync(0xFFFFFFFFu, q.md, first);   // inside this chunk everything below it is final
                 const bool ready = mine && ext_ok && (need_end <= md_first || lane == first);
                 const uint32_t rmask = __ballot_sync(0xFFFFFFFFu, ready);
                 if (!rmask) { if (zk_d2_aborted(sm)) { aborted = true; break; } ZK_SPIN(); continue; }
                 __threadfence_block();             // acquire: the flags were read before the data is
-                if (!stamped5) { ZK_STAMP(5); stamped5 = true; }
-                if (ready && ml < ZK_LONG) {
-                    if (near_src) rg.copy_near(md, src0, ml);
-                    else {   // far source (HBM, never overlapping): 8 bytes per round trip
-                        const uint8_t* sp = out + src0;
-                        for (uint32_t i = 0; i < ml; i += 8) {
-                            unsigned long long v = zk_ld8_unaligned(sp + i);
-                            const uint32_t nb = ml - i < 8 ? ml - i : 8;
-                            for (uint32_t q = 0; q < nb; q++) { rg.at(md + i + q) = (uint8_t)v; v >>= 8; }
-                        }
-                    }
-                }
-                uint32_t longm = __ballot_sync(0xFFFFFFFFu, ready && ml >= ZK_LONG);
-                while (longm) {
-                    int l = __ffs((int)longm) - 1; longm &= longm - 1;
-                    const uint32_t n = __shfl_sync(0xFFFFFFFFu, ml, l), d = __shfl_sync(0xFFFFFFFFu, md, l), o = __shfl_sync(0xFFFFFFFFu, off, l);
-                    const bool nr = __shfl_sync(0xFFFFFFFFu, (uint32_t)near_src, l) != 0;
-                    if (!nr) { const uint8_t* sp = out + (d - o); for (uint32_t i = lane; i < n; i += 32) rg.at(d + i) = sp[i]; }
-                    else if (o >= n) { for (uint32_t i = lane; i < n; i += 32) rg.at(d + i) = rg.at(d - o + i); }
-                    else if (o >= 32) {           // overlapping, period >= 32: 32 bytes per step are already final
-                        for (uint32_t i0 = 0; i0 < n; i0 += 32) { uint32_t i = i0 + lane; if (i < n) rg.at(d + i) = rg.at(d - o + i); __syncwarp(); }
-                    } else {                      // short period: replicate the pattern
-                        for (uint32_t i = lane; i < n; i += 32) rg.at(d + i) = rg.at(d - o + (i % o));
-                    }
-                }
+                zk_ring_matches(rg, ready, near_src, q.md, q.off, q.ml, lane);
                 zk_d2_progress(sm, c, rmask, lane);    // dependants of these sequences may go now (not only when the whole chunk is done)
                 __syncwarp();
                 pending &= ~rmask;
             }
             if (aborted) break;
-            ZK_STAMP(6);
             zk_d2_mark_done(sm, c, lane);                          // dependants can read the ring now ...
-            ZK_STAMP(7);
             zk_ring_flush(rg, chunk_start, chunk_end, lane);       // ... while the HBM flush happens off the critical chain
             zk_d2_mark_flushed(sm, c, lane);
         }
         // advance to the next block
-        if (has_seq) {
-            uint32_t v[3] = { blk.rep_out[0], blk.rep_out[1], blk.rep_out[2] }, n[3];
-            for (int q = 0; q < 3; q++) {
-                if (v[q] & ZK_SYM) { uint32_t sl = ZK_SYM_SLOT(v[q]); uint32_t r = sl == 0 ? R0 : (sl == 1 ? R1 : R2); n[q] = r - ZK_SYM_DELTA(v[q]); }
-                else n[q] = v[q];
-            }
-            R0 = n[0]; R1 = n[1]; R2 = n[2];
-        }
+        if (has_seq) rep.advance(blk);
         pos += blk.regen;
         chunk_base += nchunks;
     }
     __syncthreads();
-    if (threadIdx.x == 0) {
-        ZkEntry& en = a.entries[e];
-        if (sm.abort_code) atomicMin(&en.fail, ZK_FAIL_KEY(sm.abort_block, ZK_FAIL_EXEC, sm.abort_code));
-        __threadfence();
-        if (atomicSub(&en.segs_left, 1u) == 1u) { __threadfence(); zk_entry_finish(a, e); }   // the entry's last segment
-    }
+    if (threadIdx.x == 0) zk_segment_end(a, e, sm.abort_block, sm.abort_code);
 }
 
 // CTAs are persistent: each pulls segments from a work counter until none is left.  Segments never wait for each other,
@@ -1677,7 +1713,7 @@ __device__ __forceinline__ void zk_exec_body(ZkD2Smem& sm, const ZkDecodeArgs& a
 // ("far", flushed by this warp earlier: __syncwarp orders it).  Larger chunks, Raw / RLE and literal-only blocks are
 // copied HBM to HBM and the window is reloaded.  Inside a chunk, matches go in ballot rounds: a lane copies once every
 // earlier lane whose destination overlaps its source is done.  Every store lies inside the segment's output range, which no other warp or
-// CTA writes.  Repeat offsets, bounds and the failure key are those of zk_exec_segment.
+// CTA writes.  Repeat offsets, the offset check, direct chunks, copies and the failure key are the helpers zk_exec_segment calls.
 // =============================================================================================
 #define ZK_XW_WARPS 4u          // warps per CTA; __launch_bounds__ below asks for 8 CTAs (32 warps) per SM, i.e. <= 64 registers
 #define ZK_XW_WIN 4096u         // window bytes per warp (H100, bench mix: 2 KiB ran as fast, 8 KiB 9 % slower)
@@ -1691,134 +1727,67 @@ __device__ __forceinline__ void zk_exec_warp_segment(const ZkDecodeArgs& a, uint
     const uint8_t* ebase = a.comp + a.c_off[e];
     ZkRing rg; rg.ring = win; rg.mask = ZK_XW_WIN - 1; rg.mis = (uint32_t)((uintptr_t)out & 15); rg.out = out;
     const uint32_t half = ZK_XW_WIN >> 1;
-    uint32_t pos = pos0, zstart = head.frame_start, R0 = 1, R1 = 4, R2 = 8;
+    uint32_t pos = pos0, zstart = head.frame_start;
+    ZkRepOffsets rep;
     uint32_t bad_block = 0xFFFFFFFFu;
     for (uint32_t bi = first_bidx - ent.first_block; bi < ent.run_blocks && bad_block == 0xFFFFFFFFu; bi++) {
         const uint32_t bidx = ent.first_block + bi;
         const ZkBlock& blk = a.blocks[bidx];
-        const uint32_t flags = blk.flags, type = blk.type, nseq = blk.nseq, regen = blk.regen;
+        const uint32_t flags = blk.flags, nseq = blk.nseq, regen = blk.regen;
         if (bidx != first_bidx && (flags & ZKB_SEG)) break;
-        if (flags & ZKB_FIRST) { R0 = 1; R1 = 4; R2 = 8; zstart = pos; }
-        const uint32_t lit_kind = blk.lit_kind, lit_byte = blk.lit_byte;
-        if (!(type == 2 && nseq > 0)) {
+        if (flags & ZKB_FIRST) { rep.reset(); zstart = pos; }
+        if (!(blk.type == 2 && nseq > 0)) {
             // ---------------- Raw block / RLE block / literals-only compressed block: HBM to HBM
-            if (type == 0) zk_warp_copy(out + pos, ebase + blk.src, blk.size, lane);
-            else if (type == 1) zk_warp_fill(out + pos, ebase[blk.src], blk.size, lane);
-            else if (lit_kind == 1) zk_warp_fill(out + pos, lit_byte, blk.lit_size, lane);
-            else zk_warp_copy(out + pos, lit_kind == 0 ? ebase + blk.lit_src : a.lit + blk.lit_base, blk.lit_size, lane);
+            zk_direct_block(rg, a, blk, ebase, pos, pos0, half, lane);
             pos += regen;
-            __syncwarp();
-            zk_ring_reload(rg, pos - pos0 > half ? pos - half : pos0, pos, lane, 32);   // (output before pos0 belongs to other warps)
             __syncwarp();
             continue;
         }
-        const uint32_t seq_base = blk.seq_base;
-        const uint32_t* s_lit = a.seq_lit_end + seq_base;
-        const uint32_t* s_out = a.seq_out_end + seq_base;
-        const uint8_t* lit = lit_kind == 0 ? ebase + blk.lit_src : a.lit + blk.lit_base;
+        const uint32_t seq_base = blk.seq_base, lit_kind = blk.lit_kind, lit_byte = blk.lit_byte;
+        const uint8_t* lit = zk_block_lit(a, blk, ebase);
         uint32_t le_last = 0, oe_last = 0;            // cumulative literal / output ends of the sequences before the chunk
         for (uint32_t j = 0; j * 32 < nseq; j++) {
             // ---------------- 32 sequences, one per lane
-            const uint32_t s = j * 32 + lane;
-            const bool valid = s < nseq;
-            const uint32_t sc = valid ? s : nseq - 1;     // lanes past the last sequence repeat its ends (zero-length runs)
-            const uint32_t le = s_lit[sc], oe = s_out[sc], offv = valid ? a.seq_off[seq_base + s] : 0u;
-            uint32_t le_prev = __shfl_up_sync(0xFFFFFFFFu, le, 1), oe_prev = __shfl_up_sync(0xFFFFFFFFu, oe, 1);
-            if (lane == 0) { le_prev = le_last; oe_prev = oe_last; }
-            const uint32_t ll = le - le_prev; uint32_t ml = (oe - oe_prev) - ll;
-            const uint32_t o_lit = pos + oe_prev; uint32_t md = o_lit + ll;   // (PREFIX: md / ml shrink to the in-frame part)
-            uint32_t off = offv;
-            bool bad = false;
-            if (valid) {
-                if (offv & ZK_SYM) {
-                    const uint32_t sl = ZK_SYM_SLOT(offv), dl = ZK_SYM_DELTA(offv);
-                    const uint32_t r = sl == 0 ? R0 : (sl == 1 ? R1 : R2);
-                    bad = r <= dl; off = r - dl;
-                }
-                if (off == 0 || off > md - zstart + (PREFIX ? a.prefix_len : 0u)) bad = true;
+            ZkLaneSeq q;
+            if (zk_lane_seq<PREFIX>(q, a, seq_base, nseq, rep, j, pos, zstart, le_last, oe_last, lane)) { bad_block = bi; break; }
+            le_last = __shfl_sync(0xFFFFFFFFu, q.le, 31); oe_last = __shfl_sync(0xFFFFFFFFu, q.oe, 31);
+            const uint32_t chunk_start = pos + __shfl_sync(0xFFFFFFFFu, q.oe_prev, 0), chunk_end = pos + oe_last;
+            if (chunk_end - chunk_start > half) {
+                zk_direct_chunk<PREFIX>(rg, a, lit_kind, lit_byte, lit, q, zstart, chunk_end, half, lane);
+                __syncwarp();
+                continue;
             }
-            if (__any_sync(0xFFFFFFFFu, bad)) { bad_block = bi; break; }
-            le_last = __shfl_sync(0xFFFFFFFFu, le, 31); oe_last = __shfl_sync(0xFFFFFFFFu, oe, 31);
-            const uint32_t chunk_start = pos + __shfl_sync(0xFFFFFFFFu, oe_prev, 0), chunk_end = pos + oe_last;
-            const bool direct = chunk_end - chunk_start > half;
-            if (PREFIX) {
-                if (direct) zk_prefix_part<false>(rg, a, valid, zstart, off, md, ml);
-                else zk_prefix_part<true>(rg, a, valid, zstart, off, md, ml);
-            }
-            const uint32_t src0 = md - off, need_end = src0 + (ml < off ? ml : off);
-            const bool near_src = !direct && src0 + half >= chunk_start;
-            if (direct) zk_chunk_literals<false>(rg, lit, lit_kind, lit_byte, le, le_prev, o_lit, lane);
-            else zk_chunk_literals<true>(rg, lit, lit_kind, lit_byte, le, le_prev, o_lit, lane);
+            if (PREFIX) zk_prefix_part<true>(rg, a, q.valid, zstart, q.off, q.md, q.ml);
+            const uint32_t src0 = q.md - q.off, need_end = src0 + (q.ml < q.off ? q.ml : q.off);
+            const bool near_src = src0 + half >= chunk_start;
+            zk_chunk_literals<true>(rg, lit, lit_kind, lit_byte, q.le, q.le_prev, q.o_lit, lane);
             __syncwarp();
-            uint32_t pending = __ballot_sync(0xFFFFFFFFu, valid && ml > 0);
+            uint32_t pending = __ballot_sync(0xFFFFFFFFu, q.valid && q.ml > 0);
             while (pending) {
                 // everything below the first pending match's destination is final
                 const int first = __ffs((int)pending) - 1;
-                const uint32_t md_first = __shfl_sync(0xFFFFFFFFu, md, first);
+                const uint32_t md_first = __shfl_sync(0xFFFFFFFFu, q.md, first);
                 const bool ready = ((pending >> lane) & 1u) && (need_end <= md_first || lane == first);
                 const uint32_t rmask = __ballot_sync(0xFFFFFFFFu, ready);
-                if (ready && ml < ZK_LONG) {
-                    if (direct) { uint8_t* d = out + md; const uint8_t* sp = d - off; for (uint32_t i = 0; i < ml; i++) d[i] = sp[i]; }
-                    else if (near_src) rg.copy_near(md, src0, ml);
-                    else {   // far source (HBM, never overlapping): 8 bytes per round trip
-                        const uint8_t* sp = out + src0;
-                        for (uint32_t i = 0; i < ml; i += 8) {
-                            unsigned long long v = zk_ld8_unaligned(sp + i);
-                            const uint32_t nb = ml - i < 8 ? ml - i : 8;
-                            rg.st8(md + i, (uint32_t)v, (uint32_t)(v >> 32), nb);
-                        }
-                    }
-                }
-                uint32_t longm = __ballot_sync(0xFFFFFFFFu, ready && ml >= ZK_LONG);
-                while (longm) {
-                    const int l = __ffs((int)longm) - 1; longm &= longm - 1;
-                    const uint32_t n = __shfl_sync(0xFFFFFFFFu, ml, l), d = __shfl_sync(0xFFFFFFFFu, md, l), o = __shfl_sync(0xFFFFFFFFu, off, l);
-                    const bool nr = __shfl_sync(0xFFFFFFFFu, (uint32_t)near_src, l) != 0;
-                    if (direct) zk_warp_match(out + d, o, n, lane);
-                    else if (!nr) { const uint8_t* sp = out + (d - o); for (uint32_t i = lane; i < n; i += 32) rg.at(d + i) = sp[i]; }
-                    else if (o >= n) { for (uint32_t i = lane; i < n; i += 32) rg.at(d + i) = rg.at(d - o + i); }
-                    else if (o >= 32) {           // overlapping, period >= 32: 32 bytes per step are already final
-                        for (uint32_t i0 = 0; i0 < n; i0 += 32) { const uint32_t i = i0 + lane; if (i < n) rg.at(d + i) = rg.at(d - o + i); __syncwarp(); }
-                    } else {                      // short period: replicate the pattern
-                        for (uint32_t i = lane; i < n; i += 32) rg.at(d + i) = rg.at(d - o + (i % o));
-                    }
-                }
+                zk_ring_matches(rg, ready, near_src, q.md, q.off, q.ml, lane);
                 __syncwarp();
                 pending &= ~rmask;
             }
-            if (direct) zk_ring_reload(rg, chunk_end - half, chunk_end, lane, 32);
-            else zk_ring_flush(rg, chunk_start, chunk_end, lane);
+            zk_ring_flush(rg, chunk_start, chunk_end, lane);
             __syncwarp();
         }
         if (bad_block != 0xFFFFFFFFu) break;
         {   // ---------------- trailing literals of the block
             const uint32_t n = blk.lit_size - le_last, st0 = pos + oe_last, en = pos + regen;
-            if (n > half) {
-                if (lit_kind == 1) zk_warp_fill(out + st0, lit_byte, n, lane);
-                else zk_warp_copy(out + st0, lit + le_last, n, lane);
-                __syncwarp();
-                zk_ring_reload(rg, en - half, en, lane, 32);
-            } else {
-                for (uint32_t i = lane; i < n; i += 32) rg.at(st0 + i) = lit_kind == 1 ? lit_byte : lit[le_last + i];
-                __syncwarp();
-                zk_ring_flush(rg, st0, en, lane);
-            }
+            zk_trailing_literals(rg, lit_kind, lit_byte, lit, le_last, n, st0, en, half, lane);
+            __syncwarp();
+            if (n <= half) zk_ring_flush(rg, st0, en, lane);
             __syncwarp();
         }
-        uint32_t v[3] = { blk.rep_out[0], blk.rep_out[1], blk.rep_out[2] }, nr[3];
-        for (int q = 0; q < 3; q++) {
-            if (v[q] & ZK_SYM) { const uint32_t sl = ZK_SYM_SLOT(v[q]); const uint32_t r = sl == 0 ? R0 : (sl == 1 ? R1 : R2); nr[q] = r - ZK_SYM_DELTA(v[q]); }
-            else nr[q] = v[q];
-        }
-        R0 = nr[0]; R1 = nr[1]; R2 = nr[2];
+        rep.advance(blk);
         pos += regen;
     }
-    if (lane == 0) {
-        ZkEntry& en = a.entries[e];
-        if (bad_block != 0xFFFFFFFFu) atomicMin(&en.fail, ZK_FAIL_KEY(bad_block, ZK_FAIL_EXEC, ZKZ_CORRUPTION));
-        __threadfence();
-        if (atomicSub(&en.segs_left, 1u) == 1u) { __threadfence(); zk_entry_finish(a, e); }   // the entry's last segment
-    }
+    if (lane == 0) zk_segment_end(a, e, bad_block, bad_block != 0xFFFFFFFFu ? ZKZ_CORRUPTION : 0);
     __syncwarp();
 }
 
@@ -1964,7 +1933,7 @@ static int zk_decode_ensure(ZkDecodeWs* ws, uint32_t n, size_t need_blocks, size
 
 // Enqueue one batch on `stream` (scan, entropy, exec[, checksum], status read-back).  No host sync.
 int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp, const uint64_t* c_off, const uint64_t* d_off,
-                      uint32_t n, uint8_t* d_dst, int verify_checksum, int exec_warps) {
+                      uint32_t n, uint8_t* d_dst, int verify_checksum) {
     ws->pending_n = 0;
     if (n == 0) return 0;
     unsigned long long total_d = d_off[n] - d_off[0];
@@ -1998,7 +1967,6 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     a.lit = ws->lit; a.seq_lit_end = ws->seq_lit_end; a.seq_out_end = ws->seq_out_end; a.seq_off = ws->seq_off;
     a.huf_list = ws->huf_list; a.seq_list = ws->seq_list; a.seg_list = ws->seg_list;
     a.cap_blocks = ws->cap_blocks; a.cap_lit = ws->cap_lit - 64; a.cap_seq = ws->cap_seq;
-    a.trace = nullptr;
     a.d_need = nullptr;
     a.prefix = ws->prefix; a.prefix_len = ws->prefix ? ws->prefix_len : 0; ws->prefix = nullptr; ws->prefix_len = 0;
     if (ws->need) {
@@ -2006,13 +1974,6 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
         ZK_CUDA_OK(cudaMemcpyAsync(ws->d_need, ws->h_need, (size_t)n * 4, cudaMemcpyHostToDevice, us));
         a.d_need = ws->d_need; ws->need = nullptr;
     }
-#ifndef ZK_EMUL
-    if (getenv("ZK_EXEC_TRACE")) {
-        if (!ws->trace) cudaMalloc((void**)&ws->trace, 1024 * 8 * 8);
-        cudaMemsetAsync(ws->trace, 0, 1024 * 8 * 8, stream);
-        a.trace = ws->trace;
-    }
-#endif
     if (us != stream) { ZK_CUDA_OK(cudaEventRecord(ws->ev_up, us)); ZK_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_up, 0)); }   // also orders the caller's upload of the compressed bytes
     ws->prof.begin(0, stream);
     ZK_LAUNCH(zk_scan_kernel, (n + 127) / 128, 128, 0, stream, a);
@@ -2076,7 +2037,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     // (`share` > 1: that many sub-batches of a host pipeline run concurrently on different streams)
     int per_sm = (int)(((unsigned long long)n * (unsigned)(ws->share > 0 ? ws->share : 1) + (uint32_t)sms - 1) / (uint32_t)sms);
     if (per_sm < 1) per_sm = 1;
-    int W = exec_warps;
+    int W = (int)ws->exec_warps;
     a.exec_short = ws->exec_short;
     ws->prof.begin(3, stream);                   // (the exec slot includes the plan kernel)
     ZK_LAUNCH(zk_plan_kernel, (n + 3) / 4, 128, 0, stream, a);
@@ -2125,13 +2086,6 @@ int zk_decode_collect(ZkDecodeWs* ws, cudaStream_t stream, int32_t* status_out) 
     { cudaError_t le__ = cudaGetLastError(); if (le__ != cudaSuccess) { zk_note_cuda_error("kernel launch / execution", (int)le__); return ZK_INT_CUDA; } }
 #endif
     ws->pending_n = 0;
-#ifndef ZK_EMUL
-    if (ws->trace && getenv("ZK_EXEC_TRACE")) {
-        static unsigned long long host[1024 * 8];
-        cudaMemcpy(host, ws->trace, sizeof host, cudaMemcpyDeviceToHost);
-        FILE* f = fopen(getenv("ZK_EXEC_TRACE"), "wb"); if (f) { fwrite(host, 1, sizeof host, f); fclose(f); }
-    }
-#endif
     ws->prof.harvest();
     if (ws->h_counters->overflow) {
         ws->want_blocks = (size_t)ws->h_counters->n_blocks; ws->want_lit = (size_t)ws->h_counters->n_lit; ws->want_seq = (size_t)ws->h_counters->n_seq;
@@ -2149,9 +2103,9 @@ int zk_decode_collect(ZkDecodeWs* ws, cudaStream_t stream, int32_t* status_out) 
 }
 
 int zk_decode_batch(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp, const uint64_t* c_off, const uint64_t* d_off,
-                    uint32_t n, uint8_t* d_dst, int verify_checksum, int32_t* status_out, int exec_warps) {
+                    uint32_t n, uint8_t* d_dst, int verify_checksum, int32_t* status_out) {
     for (int attempt = 0; attempt < 2; attempt++) {
-        int rc = zk_decode_enqueue(ws, stream, d_comp, c_off, d_off, n, d_dst, verify_checksum, exec_warps);
+        int rc = zk_decode_enqueue(ws, stream, d_comp, c_off, d_off, n, d_dst, verify_checksum);
         if (rc) return rc;
         rc = zk_decode_collect(ws, stream, status_out);
         if (rc != ZK_ST_RETRY) return rc;

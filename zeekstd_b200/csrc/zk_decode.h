@@ -16,7 +16,6 @@ struct ZkDecodeArgs {                 // kernel parameter block (by value)
                                               // front, short ones from the back: together never more than cap_blocks)
     uint32_t exec_short;                      // segments of at most this many output bytes run on one warp each; 0 = none
     unsigned long long cap_blocks, cap_lit, cap_seq;
-    unsigned long long* trace;        // debug: per-chunk clock64 stamps of entry 0 (env ZK_EXEC_TRACE), else nullptr
     const uint8_t* prefix; uint32_t prefix_len;   // raw-content prefix of every zstd frame (Decoder::decompress_with_prefix, decode.rs:211-214, 246-255); device pointer or nullptr
     const uint32_t* d_need;           // per entry: only this many leading bytes are wanted (range reads); nullptr = everything
 };
@@ -33,11 +32,11 @@ struct ZkDecodeWs {                   // HBM scratch owned by a zk_ctx, grown on
     const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device pointer for the NEXT enqueue (one-shot, like `need`)
     uint32_t* huf_list = nullptr; uint32_t* seq_list = nullptr; uint32_t* seg_list = nullptr;
     bool attr_set = false; uint32_t ring_override = 0;
+    uint32_t exec_warps = 0;          // ZK_EXEC_WARPS: warps per K-D2 CTA (at most 16); 0 = chosen from the entries per SM
     uint32_t seq2_ctas = 5;           // ZK_SEQ2_CTAS: persistent K-D1s CTAs per SM (5 x 35.4 KiB leave room for two K-D1h CTAs
                                       // beside them; 6 leave none: DESIGN §6)
     uint32_t exec_short = 128 << 10;  // ZK_EXEC_SHORT: output bytes up to which a segment runs on one warp (zk_exec_warp_kernel); 0 = CTAs only
     uint32_t huf_pad = 0;             // extra dynamic smem per Huffman CTA: fewer resident CTAs -> more L1 for the streams (tuning)
-    unsigned long long* trace = nullptr;
     int share = 1;                    // how many batches share the GPU concurrently (host pipeline depth)
     int prio = 0;                     // CUDA stream priority of the side stream (matches the slot's stream)
     uint32_t huf_ctas = 0;            // persistent K-D1h CTAs per SM (tuning: ZK_HUF_CTAS); 0: half of huf_fit
@@ -61,8 +60,8 @@ struct ZkDecodeWs {                   // HBM scratch owned by a zk_ctx, grown on
 // Returns 0, or the first non-zero entry status, or -(code) for a launch/allocation failure.
 // Synchronous with respect to `stream` on return.
 int zk_decode_batch(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp, const uint64_t* c_off, const uint64_t* d_off,
-                    uint32_t n, uint8_t* d_dst, int verify_checksum, int32_t* status_out, int exec_warps);
+                    uint32_t n, uint8_t* d_dst, int verify_checksum, int32_t* status_out);
 int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp, const uint64_t* c_off, const uint64_t* d_off,
-                      uint32_t n, uint8_t* d_dst, int verify_checksum, int exec_warps);
+                      uint32_t n, uint8_t* d_dst, int verify_checksum);
 int zk_decode_collect(ZkDecodeWs* ws, cudaStream_t stream, int32_t* status_out);
 void zk_decode_ws_free(ZkDecodeWs* ws);
