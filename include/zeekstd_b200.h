@@ -46,7 +46,8 @@ extern "C" {
 
 /* Compression levels (the `level` argument of every compress entry point and of zk_encode_options_compression_level), as in libzstd:
  *   0                 the default, level 3;
- *   1 .. 22           the ratio tiers of DESIGN.md 3 (from 13 on: a 256 KiB window);
+ *   1 .. 22           the ratio tiers of DESIGN.md 3 (13 .. 15: a 256 KiB window; from 16 on: hash chains over a 2 MiB window of
+ *                     the frame and a price-based parse; higher levels run that tier too);
  *   -1 .. -131072     fast mode with acceleration -level: sparser match probing, literals stored without Huffman coding.
  *                     Lower levels clamp to ZK_MIN_COMPRESSION_LEVEL, as in libzstd (ZSTD_minCLevel()). */
 #define ZK_MIN_COMPRESSION_LEVEL (-131072)

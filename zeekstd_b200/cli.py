@@ -8,8 +8,9 @@ What each piece follows in the reference: argument set and value parsers cli/src
 path derivation, overwrite checks and the list tables cli/src/command.rs:33-473; the compress loop (Encoder fed from a
 reader, optional stand-alone Head-format seek table) cli/src/compress.rs:55-106; the decompress loop
 cli/src/decompress.rs:21-117.  The codec underneath is this package's Encoder / Decoder, i.e. the CUDA path: there is no
-CPU route.  Compression levels are 1..19 as in the reference CLI, plus zstd's negative fast levels (`-l -5` or
-`--compression-level=-5`; acceleration = -level, clamped at -131072).  The window-log / long-distance-matching parameters
+CPU route.  Compression levels are 1..19 as in the reference CLI (16..19 run the high-level tier: a 2 MiB window and a
+price-based parse), plus zstd's negative fast levels (`-l -5` or `--compression-level=-5`; acceleration = -level, clamped
+at -131072).  The window-log / long-distance-matching parameters
 the reference sets for patch files have no counterpart here (the kernels take the prefix as it is); `--mmap-prefix` / `--no-mmap-prefix` choose between np.memmap and a read.
 """
 from __future__ import annotations
@@ -133,8 +134,8 @@ def build_parser() -> argparse.ArgumentParser:
     c = sub.add_parser("compress", aliases=["c"], help="Compress INPUT_FILE (default); reads from STDIN if INPUT_FILE is `-` or not provided")
     _add_flags(c, False); _add_common(c)
     c.add_argument("-l", "--compression-level", type=_level, default=3,
-                   help="Compression level: 1-19, or negative (-1 down to -131072) for fast mode: faster, lower ratio, literals stored without "
-                        "Huffman coding. Default 3.")
+                   help="Compression level: 1-19 (16-19: 2 MiB window, price-based parse, the smallest archives), or negative (-1 down to "
+                        "-131072) for fast mode: faster, lower ratio, literals stored without Huffman coding. Default 3.")
     c.add_argument("--no-checksum", action="store_true", help="Don't include frame checksums.")
     c.add_argument("-s", "--frame-size", type=byte_value, default=byte_value("2M"))
     c.add_argument("--frame-size-policy", choices=["compressed", "uncompressed"], default="uncompressed")

@@ -53,6 +53,7 @@ struct ZkEncodeArgs {
     // bytes of the frame before a block that K-C1 may search, on top of the tier's own limit: unlimited (~0) except in the size variants
     // of the wide tier (zk_encode_csize), where variant d must match the block d blocks into its frame
     size_t hist_cap;
+    uint8_t* hc;                         // scratch of the high-level tier (zk_hc.inc), carved for its largest internal pass
 };
 #define ZKC_PSLOT (2u * ZKC_BLOCK + 64u)   // per-frame staging slot: [prefix tail | first block]
 
@@ -1155,12 +1156,19 @@ __global__ void __launch_bounds__(1024) zk_frame_scan_kernel(ZkEncodeArgs a) {
     if (threadIdx.x == 0) { *a.total = carry; if (carry > a.dst_cap) *a.error = ZKZ_DST_TOO_SMALL; }
 }
 
-// wide-history tier only: the frame headers written by zk_frame_gather_kernel announce a 128 KiB window; offsets of this tier reach
-// (ZKC_WIDE_HIST + 1) blocks back, so the Window_Descriptor becomes 256 KiB (exponent 8, mantissa 0)
-__global__ void __launch_bounds__(128) zk_frame_window_kernel(ZkEncodeArgs a, uint32_t n_frames) {
+// tiers above level 12 only: the frame headers written by zk_frame_gather_kernel announce a 128 KiB window.  This rewrites the
+// Window_Descriptor to the smallest one >= max(wmin, min(frame content + prefix tail, wmax)): the wide tier's offsets reach
+// (ZKC_WIDE_HIST + 1) blocks back (wmin = wmax = 256 KiB), the high-level tier's ZKC_HC_WINDOW bytes within the frame and its prefix tail
+__global__ void __launch_bounds__(128) zk_frame_window_kernel(ZkEncodeArgs a, uint32_t n_frames, uint32_t wmin, uint32_t wmax) {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= n_frames || *a.error) return;
-    a.dst[a.frame_off[f] + 5] = 0x40;
+    const size_t fstart = (size_t)f * a.frame_size;
+    const size_t fcs = (fstart + a.frame_size < a.n ? fstart + a.frame_size : a.n) - fstart;
+    size_t want = fcs + a.ptail < wmax ? fcs + a.ptail : wmax;
+    if (want < wmin) want = wmin;
+    uint32_t e = 0, m = 0;                                    // Window_Size = 2^(10 + e) * (1 + m / 8)
+    while (((size_t)8 + m) << (7 + e) < want) { if (++m == 8) { m = 0; e++; } }
+    a.dst[a.frame_off[f] + 5] = (uint8_t)((e << 3) | m);
 }
 
 // gather: one warp per block copies its staged bytes to the final position; block 0 of a frame also writes the
@@ -1425,6 +1433,8 @@ static size_t zkc_align(size_t v) { return (v + 255) & ~(size_t)255; }
 static int zkc_level(int level) { return level == 0 ? 3 : (level < ZKC_MIN_LEVEL ? ZKC_MIN_LEVEL : level); }
 static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, const ZkEncodeArgs& a);
 
+#include "zk_hc.inc"
+
 int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t frame_size, int level,
                       int checksum, uint8_t* d_dst, size_t dst_cap, uint32_t n_frames) {
     const uint8_t* d_prefix = ws->prefix; const uint32_t prefix_len = ws->prefix_len;     // one-shot (set by the caller for THIS batch)
@@ -1450,6 +1460,12 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     const size_t o_fh = off; off = zkc_align(off + (size_t)n_frames * 4);
     const size_t o_tot = off; off = zkc_align(off + 16);
     const size_t o_pst = off; if (d_prefix && prefix_len && n) off = zkc_align(off + (size_t)n_frames * ZKC_PSLOT);
+    const int lvl = zkc_level(level);
+    const size_t o_hc = off;
+    if (lvl >= ZKC_HC_LEVEL) {
+        const uint32_t pt = d_prefix && prefix_len && n ? (prefix_len < ZKC_BLOCK ? prefix_len : ZKC_BLOCK) : 0u;
+        off = zkc_align(off + zkc_hc_layout(zkc_hc_span(n, frame_size, bpf, (uint32_t)n_blocks, pt), nullptr, nullptr));
+    }
     if (ws->cap < off) {
         if (ws->buf) cudaFree(ws->buf);
         ws->buf = nullptr; ws->cap = 0;
@@ -1467,7 +1483,7 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     uint8_t* base = (uint8_t*)ws->buf;
     ZkEncodeArgs a;
     a.src = d_src; a.n = n; a.frame_size = frame_size; a.n_frames = n_frames; a.blocks_per_frame = bpf; a.n_blocks = (uint32_t)n_blocks;
-    a.level = zkc_level(level); a.checksum = checksum ? 1 : 0;
+    a.level = lvl; a.checksum = checksum ? 1 : 0;
     a.blocks = (ZkcBlock*)(base + o_blocks);
     a.seq_ll = (uint16_t*)(base + o_ll); a.seq_ml = (uint16_t*)(base + o_ml); a.seq_off = (uint32_t*)(base + o_off);
     a.lits = base + o_lits; a.stage = base + o_stage; a.seqsec = base + o_seqsec;
@@ -1475,6 +1491,7 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     a.dst = d_dst; a.dst_cap = dst_cap; a.total = (unsigned long long*)(base + o_tot); a.error = (uint32_t*)(base + o_tot + 8);
     a.prefix = d_prefix; a.prefix_len = 0; a.ptail = 0; a.pstage = base + o_pst;
     a.hist_cap = ~(size_t)0;
+    a.hc = base + o_hc;
     if (d_prefix && prefix_len && n) {
         a.prefix_len = prefix_len; a.ptail = prefix_len < ZKC_BLOCK ? prefix_len : ZKC_BLOCK;
         ZK_LAUNCH(zk_prefix_stage_kernel, n_frames, 256, 0, stream, a);
@@ -1504,7 +1521,8 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     ZK_LAUNCH(zk_frame_size_kernel, (n_frames + 255) / 256, 256, 0, stream, a);
     ZK_LAUNCH(zk_frame_scan_kernel, 1, 1024, 0, stream, a);
     ZK_LAUNCH(zk_frame_gather_kernel, (uint32_t)((n_blocks + 3) / 4), 128, 0, stream, a);
-    if (a.level >= ZKC_WIDE_LEVEL) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames); ws->launches++; }
+    if (a.level >= ZKC_HC_LEVEL) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 128u << 10, ZKC_HC_WINDOW); ws->launches++; }
+    else if (a.level >= ZKC_WIDE_LEVEL) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 256u << 10, 256u << 10); ws->launches++; }
     ws->prof.end(7, stream);
     ZKC_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, a.frame_csize, (size_t)n_frames * 4, cudaMemcpyDeviceToHost, stream));
     ZKC_CUDA_OK(cudaMemcpyAsync(ws->h_sizes + ws->cap_frames, a.total, 16, cudaMemcpyDeviceToHost, stream));
@@ -1521,8 +1539,10 @@ static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, 
     // previous-block history, one lazy step; 4-6 = double table (8-byte + 5-byte hashes, 4096 entries each), two warps per CTA; 7-9 = double
     // table of 8192 entries each, one warp per CTA; 10-12 = one table of 16384 entries, one warp per CTA; >= 13 = 256 KiB history, 32768 x u32
     // entries in dynamic shared memory.  Ratio on the reference's corpus: 2.12 / 2.24 / 2.28 / 2.38 / 2.40 / 2.50.  Below them the fast tier
-    // (level < 0): level 1's table with sparse probing, literals without Huffman coding
-    if (a.level < 0) ZK_LAUNCH((zk_match_fast_kernel<ZKC_HLOG_FAST, ZKC_C1_WARPS>), (uint32_t)((n_blocks + ZKC_C1_WARPS - 1) / ZKC_C1_WARPS), ZKC_C1_WARPS * 32, 0, stream, a);
+    // (level < 0): level 1's table with sparse probing, literals without Huffman coding.  From ZKC_HC_LEVEL on, K-C1h (zk_hc.inc): hash chains
+    // over 2 MiB of the frame and a price-based parse
+    if (a.level >= ZKC_HC_LEVEL) { const int rc = zkc_run_hc(ws, stream, a); if (rc) return rc; }
+    else if (a.level < 0) ZK_LAUNCH((zk_match_fast_kernel<ZKC_HLOG_FAST, ZKC_C1_WARPS>), (uint32_t)((n_blocks + ZKC_C1_WARPS - 1) / ZKC_C1_WARPS), ZKC_C1_WARPS * 32, 0, stream, a);
     else if (a.level <= 1) ZK_LAUNCH((zk_match_kernel<ZKC_HLOG_FAST, ZKC_C1_WARPS, false>), (uint32_t)((n_blocks + ZKC_C1_WARPS - 1) / ZKC_C1_WARPS), ZKC_C1_WARPS * 32, 0, stream, a);
     else if (a.level <= 3) ZK_LAUNCH((zk_match_kernel<ZKC_HLOG, ZKC_C1_WARPS, false>), (uint32_t)((n_blocks + ZKC_C1_WARPS - 1) / ZKC_C1_WARPS), ZKC_C1_WARPS * 32, 0, stream, a);
     else if (a.level <= 6) ZK_LAUNCH((zk_match_kernel<ZKC_HLOG, 2, true>), (uint32_t)((n_blocks + 1) / 2), 64, 0, stream, a);
@@ -1582,7 +1602,9 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     *out = ZkCsizeOut();
     if (n == 0) return 0;
     if (n > 0x40000000u) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
-    const int lvl = zkc_level(level);
+    // the exact cut needs a bounded history per block (the V variants); the high-level tier's frame-wide chains have none, so its levels
+    // run the wide tier here
+    const int lvl = zkc_level(level) >= ZKC_HC_LEVEL ? ZKC_WIDE_LEVEL : zkc_level(level);
     const uint32_t nb = (uint32_t)((n + ZKC_BLOCK - 1) / ZKC_BLOCK);
     const uint32_t V = lvl >= ZKC_WIDE_LEVEL ? ZKC_WIDE_HIST + 1 : 2;
     const bool pfx = d_prefix && prefix_len;
@@ -1651,6 +1673,7 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
         a.dst = d_dst; a.dst_cap = dst_cap; a.total = nullptr; a.error = nullptr;
         a.prefix = d_prefix; a.prefix_len = 0; a.ptail = 0; a.pstage = base + o_pst;
         a.hist_cap = d >= 1 && d + 1 < V ? (size_t)d * ZKC_BLOCK : ~(size_t)0;
+        a.hc = nullptr;
         if (d == 0 && pfx) {
             a.prefix_len = prefix_len; a.ptail = prefix_len < ZKC_BLOCK ? prefix_len : ZKC_BLOCK;
             ZK_LAUNCH(zk_prefix_stage_kernel, nb, 256, 0, stream, a);

@@ -8,7 +8,7 @@ struct ZkEncodeWs {                    // HBM scratch owned by a zk_ctx slot, gr
     int sm_count = 0;
     unsigned long long launches = 0;
     uint32_t pending_frames = 0;
-    bool attr_set = false, attr_set_wide = false, attr_set_walk = false;
+    bool attr_set = false, attr_set_wide = false, attr_set_walk = false, attr_set_hc = false;
     const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device pointer: raw-content prefix for the NEXT enqueue (one-shot)
     int prio = 0;                     // CUDA stream priority of the side stream (matches the slot's stream)
     bool no_side = false;             // host pipelines: concurrency comes from the other sub-batches; every extra stream costs a hardware queue
