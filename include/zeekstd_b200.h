@@ -161,6 +161,25 @@ int32_t zk_compress_frames_csize_dev(zk_ctx* ctx, const void* d_src, size_t n, u
                                      int32_t final, void* d_dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes,
                                      uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len, size_t* consumed, void* cuda_stream);
 
+/*
+ * Frames of caller-chosen sizes in one batch (a frame boundary at any byte, as Encoder::end_frame, encode.rs:438-472): frame f covers the
+ * next frame_sizes[f] bytes of src, whose length is the sum of the sizes.  Frame f's bytes are exactly what zk_compress_frames_prefix
+ * writes for those bytes alone with frame_size = max(frame_sizes[f], 1): a size of 0 gives the empty frame of n == 0, and every level,
+ * the checksum and the prefix behave as there.  The frames are written back to back into dst; c_sizes (n_frames entries) receives their
+ * compressed sizes (the d_sizes are frame_sizes).  n_frames == 0 writes nothing.  A size above 1 GiB returns -42 (parameter_outOfBound),
+ * more than ZK_SEEKABLE_MAX_FRAMES frames ZK_ERR_FRAME_INDEX_TOO_LARGE, and a dst_cap below what the frames need -70 (dstSize_tooSmall);
+ * dst_cap >= zk_compress_bound_sized(frame_sizes, n_frames) always suffices.  HOST pointers.
+ */
+int32_t zk_compress_frames_sized(zk_ctx* ctx, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                 int32_t checksum, const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap,
+                                 uint32_t* c_sizes, size_t* dst_len);
+/* the same on device src / dst (frame_sizes and c_sizes stay on the host; no prefix, like the other _dev entry points) */
+int32_t zk_compress_frames_sized_dev(zk_ctx* ctx, const void* d_src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                     int32_t checksum, void* d_dst, size_t dst_cap, uint32_t* c_sizes, size_t* dst_len,
+                                     void* cuda_stream);
+/* Upper bound of the compressed size of frames of these sizes (excl. seek table). */
+size_t zk_compress_bound_sized(const uint32_t* frame_sizes, uint32_t n_frames);
+
 /* ------------------------------------------------------------------ SeekTable (lib/src/seek_table.rs) */
 typedef struct zk_seek_table zk_seek_table;
 typedef enum { ZK_FORMAT_HEAD = 0, ZK_FORMAT_FOOT = 1 } zk_format; /* seek_table.rs:228-241 */

@@ -146,6 +146,24 @@ class Context:
                                           byref(dl)), lib)
         return dst[: dl.value], cs[: nf.value].copy(), ds[: nf.value].copy()
 
+    def compress_frames_sized(self, data, frame_sizes, level: int = 0, checksum: bool = False, prefix=None):
+        """frames of caller-chosen sizes in one batch: frame f covers the next frame_sizes[f] bytes of data (their sum is its length)
+        -> (compressed bytes (np.uint8), c_sizes, d_sizes).  Each frame is what compress_frames makes of its bytes alone."""
+        addr, n, keep = _buf(data)
+        ds = np.ascontiguousarray(frame_sizes, dtype=np.uint32).reshape(-1)
+        if int(np.sum(ds, dtype=np.uint64)) != n:
+            raise ValueError(f"frame sizes add up to {int(np.sum(ds, dtype=np.uint64))} bytes, the input has {n}")
+        lib = self.lib
+        dsp = ds.ctypes.data_as(_native.u32p)
+        cap = lib.zk_compress_bound_sized(dsp, ds.size)
+        dst = np.empty(cap + 64, dtype=np.uint8)
+        cs = np.zeros(ds.size, dtype=np.uint32)
+        dl = c_size_t()
+        paddr, pn, pkeep = _buf(prefix) if prefix is not None else (None, 0, None)
+        _check(lib.zk_compress_frames_sized(self._h, addr, dsp, ds.size, level, int(checksum), paddr, pn, dst.ctypes.data, cap,
+                                            cs.ctypes.data_as(_native.u32p), byref(dl)), lib)
+        return dst[: dl.value], cs, ds.copy()
+
     def compress_frames_csize(self, data, target: int, level: int = 0, checksum: bool = False, prefix=None, final: bool = True):
         """FrameSizePolicy::Compressed(target) on the batch path -> (compressed bytes (np.uint8), c_sizes, d_sizes, consumed).
         A frame closes after the first 32 KiB block at which its header + blocks reach `target` (or at 1 GiB of input).

@@ -66,6 +66,11 @@ _SIGS = {
                                            c_size_t, u32p, u32p, c_uint32, u32p, POINTER(c_size_t), POINTER(c_size_t)]),
     "zk_compress_frames_csize_dev": (c_int32, [c_void_p, c_void_p, c_size_t, c_uint32, c_int32, c_int32, c_int32, c_void_p, c_size_t,
                                                u32p, u32p, c_uint32, u32p, POINTER(c_size_t), POINTER(c_size_t), c_void_p]),
+    "zk_compress_frames_sized": (c_int32, [c_void_p, c_void_p, u32p, c_uint32, c_int32, c_int32, c_void_p, c_size_t, c_void_p, c_size_t,
+                                           u32p, POINTER(c_size_t)]),
+    "zk_compress_frames_sized_dev": (c_int32, [c_void_p, c_void_p, u32p, c_uint32, c_int32, c_int32, c_void_p, c_size_t, u32p,
+                                               POINTER(c_size_t), c_void_p]),
+    "zk_compress_bound_sized": (c_size_t, [u32p, c_uint32]),
     # seek table
     "zk_seek_table_new": (c_void_p, []),
     "zk_seek_table_free": (None, [c_void_p]),

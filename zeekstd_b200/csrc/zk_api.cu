@@ -324,61 +324,90 @@ static uint32_t zk_frames_of(size_t n, uint32_t frame_size) {
     return (uint32_t)((n + frame_size - 1) / frame_size);
 }
 
+// The frames of one compress call: the caller's sizes, or the uniform layout (frame_size bytes each, the last frame shorter, one empty
+// frame of no input).  Both pipelines below cut it into sub-batches of whole consecutive frames.
+struct ZkFrameList {
+    const uint32_t* sizes;                                  // nullptr: uniform
+    size_t n; uint32_t frame_size, count;
+    uint32_t size(uint32_t f) const {
+        if (sizes) return sizes[f];
+        const size_t lo = (size_t)f * frame_size;
+        return (uint32_t)(n - lo < frame_size ? n - lo : frame_size);
+    }
+    // the sub-batch from frame f0: as many frames as fit max_bytes of input, at least one -> its end frame; *bytes: its input
+    uint32_t next_sub(uint32_t f0, size_t max_bytes, size_t* bytes) const {
+        size_t b = size(f0); uint32_t e = f0 + 1;
+        if (!sizes) {                                       // frames before the last are full: the same rule in closed form
+            const uint32_t per = frame_size <= max_bytes ? (uint32_t)(max_bytes / frame_size) : 1u;
+            e = count - f0 < per ? count : f0 + per;
+            b = (e == count ? n : (size_t)e * frame_size) - (size_t)f0 * frame_size;
+            if (e < count && b + size(e) <= max_bytes) { b += size(e); e++; }   // a short last frame that still fits
+        } else while (e < count && b + sizes[e] <= max_bytes) b += sizes[e++];
+        *bytes = b;
+        return e;
+    }
+    size_t bound(uint32_t f0, uint32_t cnt, size_t bytes) const {
+        return sizes ? zk_encode_bound_sized(sizes + f0, cnt) : zk_encode_bound(bytes, frame_size);
+    }
+    int enqueue(ZkEncodeWs* ws, cudaStream_t st, const uint8_t* d_in, uint32_t f0, uint32_t cnt, size_t bytes, int32_t level, int32_t checksum,
+                uint8_t* d_out, size_t cap) const {
+        return sizes ? zk_encode_enqueue_sized(ws, st, d_in, sizes + f0, cnt, level, checksum, d_out, cap)
+                     : zk_encode_enqueue(ws, st, d_in, bytes, frame_size, level, checksum, d_out, cap, cnt);
+    }
+};
+
+// device-resident input and output: sub-batches (which bound the scratch, about 4x the sub-batch input) one after the other on st
+static int32_t zk_compress_dev_run(zk_ctx* c, const ZkFrameList& fl, const uint8_t* d_src, int32_t level, int32_t checksum, uint8_t* d_dst,
+                                   size_t dst_cap, uint32_t* c_sizes, size_t* dst_len, cudaStream_t st) {
+    const size_t sub_bytes = zk_env_size("ZK_DEV_SUB_BYTES", (size_t)1 << 30);
+    cudaEventRecord(c->ev0, st);
+    size_t out_pos = 0, in_off = 0;
+    for (uint32_t f0 = 0; f0 < fl.count;) {
+        size_t in_len = 0;
+        const uint32_t end = fl.next_sub(f0, sub_bytes, &in_len);
+        size_t produced = 0;
+        c->slot[0].ews.no_side = false;
+        int rc = fl.enqueue(&c->slot[0].ews, st, d_src + in_off, f0, end - f0, in_len, level, checksum, d_dst + out_pos, dst_cap - out_pos);
+        if (!rc) rc = zk_encode_collect(&c->slot[0].ews, st, c_sizes ? c_sizes + f0 : nullptr, &produced);
+        if (rc) return rc;
+        out_pos += produced; in_off += in_len; f0 = end;
+    }
+    cudaEventRecord(c->ev1, st);
+    cudaEventSynchronize(c->ev1);
+    cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1);
+    if (dst_len) *dst_len = out_pos;
+    return 0;
+}
+
 extern "C" int32_t zk_compress_frames_dev(zk_ctx* c, const void* d_src, size_t n, uint32_t frame_size, int32_t level, int32_t checksum,
                                           void* d_dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap,
                                           uint32_t* n_frames, size_t* dst_len, void* cuda_stream) {
     if (!c || !d_dst || (n && !d_src) || frame_size == 0) return ZK_ERR_INVALID_ARG;
     if (frame_size > ZK_SEEKABLE_MAX_FRAME_SIZE) frame_size = ZK_SEEKABLE_MAX_FRAME_SIZE;       // encode.rs:531-534
     if ((n + frame_size - 1) / frame_size > ZK_SEEKABLE_MAX_FRAMES) return ZK_ERR_FRAME_INDEX_TOO_LARGE;
-    const uint32_t nf = zk_frames_of(n, frame_size);
-    if (nf > frames_cap) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
+    const ZkFrameList fl = {nullptr, n, frame_size, zk_frames_of(n, frame_size)};
+    if (fl.count > frames_cap) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
     ZK_RT_OK(cudaSetDevice(c->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : c->slot[0].stream;
-    // sub-batches bound the scratch (about 4x the sub-batch input)
-    const size_t sub_bytes = zk_env_size("ZK_DEV_SUB_BYTES", (size_t)1 << 30);
-    uint32_t per = (uint32_t)(sub_bytes / frame_size); if (per == 0) per = 1;
-    cudaEventRecord(c->ev0, st);
-    size_t out_pos = 0;
-    for (uint32_t f0 = 0; f0 < nf; f0 += per) {
-        const uint32_t cnt = nf - f0 < per ? nf - f0 : per;
-        const size_t in_off = (size_t)f0 * frame_size;
-        const size_t in_len = n - in_off < (size_t)cnt * frame_size ? n - in_off : (size_t)cnt * frame_size;
-        size_t produced = 0;
-        c->slot[0].ews.no_side = false;
-        int rc = zk_encode_batch(&c->slot[0].ews, st, (const uint8_t*)d_src + in_off, in_len, frame_size, level, checksum,
-                                 (uint8_t*)d_dst + out_pos, dst_cap - out_pos, c_sizes ? c_sizes + f0 : nullptr, cnt, &produced);
-        if (rc) return rc;
-        out_pos += produced;
-    }
-    cudaEventRecord(c->ev1, st);
-    cudaEventSynchronize(c->ev1);
-    cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1);
-    if (d_sizes) for (uint32_t f = 0; f < nf; f++) {
-        size_t lo = (size_t)f * frame_size; d_sizes[f] = (uint32_t)(n - lo < frame_size ? n - lo : frame_size);
-    }
-    if (n_frames) *n_frames = nf;
-    if (dst_len) *dst_len = out_pos;
+    const int32_t rc = zk_compress_dev_run(c, fl, (const uint8_t*)d_src, level, checksum, (uint8_t*)d_dst, dst_cap, c_sizes, dst_len, st);
+    if (rc) return rc;
+    if (d_sizes) for (uint32_t f = 0; f < fl.count; f++) d_sizes[f] = fl.size(f);
+    if (n_frames) *n_frames = fl.count;
     return 0;
 }
 
 struct ZkSubEnc { uint32_t f0 = 0, cnt = 0; size_t in_off = 0, in_len = 0, out_pos = 0; bool busy = false; };
 
-extern "C" int32_t zk_compress_frames(zk_ctx* c, const uint8_t* src, size_t n, uint32_t frame_size, int32_t level, int32_t checksum,
-                                      uint8_t* dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap,
-                                      uint32_t* n_frames, size_t* dst_len) {
-    if (!c || !dst || (n && !src) || frame_size == 0) return ZK_ERR_INVALID_ARG;
-    if (frame_size > ZK_SEEKABLE_MAX_FRAME_SIZE) frame_size = ZK_SEEKABLE_MAX_FRAME_SIZE;
-    if ((n + frame_size - 1) / frame_size > ZK_SEEKABLE_MAX_FRAMES) return ZK_ERR_FRAME_INDEX_TOO_LARGE;
-    const uint32_t nf = zk_frames_of(n, frame_size);
-    if (nf > frames_cap) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
+// host input and output (prefix: the context's current one): sub-batches on up to ZK_HOST_SLOTS_ENC slots, output placed in order
+static int32_t zk_compress_host_run(zk_ctx* c, const ZkFrameList& fl, const uint8_t* src, int32_t level, int32_t checksum, uint8_t* dst,
+                                    size_t dst_cap, uint32_t* c_sizes, size_t* dst_len) {
     ZK_RT_OK(cudaSetDevice(c->device));
     const size_t sub_bytes = zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20);    // tuning knob (tools/knobs_round.sh sweeps it)
-    uint32_t per = (uint32_t)(sub_bytes / frame_size); if (per == 0) per = 1;
     // The compressed size of a sub-batch is only known when it completes, so output positions are assigned in
     // order at completion time: H2D and kernels of later sub-batches overlap the D2H of earlier ones.
     ZkSubEnc sub[ZK_SLOTS];
-    size_t out_pos = 0; int32_t err = 0;
-    std::vector<uint32_t> tmp_sizes(per);
+    size_t out_pos = 0, in_off = 0; int32_t err = 0;
+    std::vector<uint32_t> tmp_sizes(c_sizes ? 0 : fl.count);
     ZkTrace tr; tr.begin(c->slot[0].stream);
     int sub_k[ZK_SLOTS] = {0};
     auto finish = [&](int si) -> int {
@@ -386,7 +415,7 @@ extern "C" int32_t zk_compress_frames(zk_ctx* c, const uint8_t* src, size_t n, u
         if (!sb.busy) return 0;
         sb.busy = false;
         size_t produced = 0;
-        int rc = zk_encode_collect(&s.ews, s.stream, c_sizes ? c_sizes + sb.f0 : tmp_sizes.data(), &produced);
+        int rc = zk_encode_collect(&s.ews, s.stream, (c_sizes ? c_sizes : tmp_sizes.data()) + sb.f0, &produced);
         if (rc) return rc;
         if (out_pos + produced > dst_cap) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
         tr.mark(s.stream, sub_k[si], 3);
@@ -397,8 +426,8 @@ extern "C" int32_t zk_compress_frames(zk_ctx* c, const uint8_t* src, size_t n, u
     };
     uint32_t k = 0;
     const int NS = zk_host_slots(true);
-    int order[ZK_SLOTS]; int n_inflight = 0;              // completion must follow submission order
-    for (uint32_t f0 = 0; f0 < nf && !err; f0 += per, k++) {
+    int n_inflight = 0;                                     // completion must follow submission order
+    for (uint32_t f0 = 0; f0 < fl.count && !err; k++) {
         const int si = (int)(k % NS);
         if (n_inflight == NS) {                             // oldest in flight is exactly slot si
             err = finish(si); n_inflight--;
@@ -406,10 +435,9 @@ extern "C" int32_t zk_compress_frames(zk_ctx* c, const uint8_t* src, size_t n, u
         }
         ZkSlot& s = c->slot[si]; ZkSubEnc& sb = sub[si];
         if (cudaStreamSynchronize(s.stream) != cudaSuccess) { err = ZK_ERR_CUDA; break; }   // its previous D2H must be done before d_out is reused
-        sb.f0 = f0; sb.cnt = nf - f0 < per ? nf - f0 : per;
-        sb.in_off = (size_t)f0 * frame_size;
-        sb.in_len = n - sb.in_off < (size_t)sb.cnt * frame_size ? n - sb.in_off : (size_t)sb.cnt * frame_size;
-        const size_t bound = zk_encode_bound(sb.in_len, frame_size);
+        const uint32_t end = fl.next_sub(f0, sub_bytes, &sb.in_len);
+        sb.f0 = f0; sb.cnt = end - f0; sb.in_off = in_off;
+        const size_t bound = fl.bound(f0, sb.cnt, sb.in_len);
         int rc = zk_slot_ensure(&s, sb.in_len + 32, bound + 32);
         if (rc) { err = rc; break; }
         sub_k[si] = (int)k; tr.mark(s.stream, (int)k, 0);
@@ -417,10 +445,11 @@ extern "C" int32_t zk_compress_frames(zk_ctx* c, const uint8_t* src, size_t n, u
         tr.mark(s.stream, (int)k, 1);
         s.ews.no_side = zk_env_size("ZK_HOST_SIDE", 1) == 0;
         s.ews.prefix = c->cur_prefix_len ? c->d_prefix : nullptr; s.ews.prefix_len = c->cur_prefix_len;
-        rc = zk_encode_enqueue(&s.ews, s.stream, s.d_in, sb.in_len, frame_size, level, checksum, s.d_out, bound, sb.cnt);
+        rc = fl.enqueue(&s.ews, s.stream, s.d_in, f0, sb.cnt, sb.in_len, level, checksum, s.d_out, bound);
         if (rc) { err = rc; break; }
         tr.mark(s.stream, (int)k, 2);
-        sb.busy = true; order[n_inflight++ % ZK_SLOTS] = si;
+        sb.busy = true; n_inflight++;
+        f0 = end; in_off += sb.in_len;
     }
     // drain in submission order
     for (uint32_t j = 0; j < (uint32_t)NS && !err; j++) {
@@ -430,14 +459,39 @@ extern "C" int32_t zk_compress_frames(zk_ctx* c, const uint8_t* src, size_t n, u
     }
     for (int si = 0; si < ZK_SLOTS; si++) cudaStreamSynchronize(c->slot[si].stream);
     tr.end("enc");
-    (void)order;
     if (err) return err;
-    if (d_sizes) for (uint32_t f = 0; f < nf; f++) {
-        size_t lo = (size_t)f * frame_size; d_sizes[f] = (uint32_t)(n - lo < frame_size ? n - lo : frame_size);
-    }
-    if (n_frames) *n_frames = nf;
     if (dst_len) *dst_len = out_pos;
     return 0;
+}
+
+extern "C" int32_t zk_compress_frames(zk_ctx* c, const uint8_t* src, size_t n, uint32_t frame_size, int32_t level, int32_t checksum,
+                                      uint8_t* dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap,
+                                      uint32_t* n_frames, size_t* dst_len) {
+    if (!c || !dst || (n && !src) || frame_size == 0) return ZK_ERR_INVALID_ARG;
+    if (frame_size > ZK_SEEKABLE_MAX_FRAME_SIZE) frame_size = ZK_SEEKABLE_MAX_FRAME_SIZE;
+    if ((n + frame_size - 1) / frame_size > ZK_SEEKABLE_MAX_FRAMES) return ZK_ERR_FRAME_INDEX_TOO_LARGE;
+    const ZkFrameList fl = {nullptr, n, frame_size, zk_frames_of(n, frame_size)};
+    if (fl.count > frames_cap) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
+    const int32_t rc = zk_compress_host_run(c, fl, src, level, checksum, dst, dst_cap, c_sizes, dst_len);
+    if (rc) return rc;
+    if (d_sizes) for (uint32_t f = 0; f < fl.count; f++) d_sizes[f] = fl.size(f);
+    if (n_frames) *n_frames = fl.count;
+    return 0;
+}
+
+// caller-chosen frame sizes: the checks of the header's contract -> the input length, or an error code
+static int32_t zk_sized_check(const uint32_t* frame_sizes, uint32_t n_frames, size_t* n) {
+    if (n_frames > ZK_SEEKABLE_MAX_FRAMES) return ZK_ERR_FRAME_INDEX_TOO_LARGE;
+    *n = 0;
+    for (uint32_t f = 0; f < n_frames; f++) {
+        if (frame_sizes[f] > ZK_SEEKABLE_MAX_FRAME_SIZE) return ZK_ERR_ZSTD(ZKZ_PARAM_OUT_OF_BOUND);
+        *n += frame_sizes[f];
+    }
+    return 0;
+}
+
+extern "C" size_t zk_compress_bound_sized(const uint32_t* frame_sizes, uint32_t n_frames) {
+    return frame_sizes || n_frames == 0 ? zk_encode_bound_sized(frame_sizes, n_frames) : 0;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -484,6 +538,44 @@ extern "C" int32_t zk_decompress_frames_prefix(zk_ctx* c, const uint8_t* comp, c
     rc = zk_decompress_frames_upto(c, comp, c_off, d_off, n, dst, d_need, verify, status);
     c->cur_prefix_len = 0;
     return rc;
+}
+
+// ---------------------------------------------------------------------------------------------
+// caller-chosen frame sizes (Encoder::end_frame at any byte, encode.rs:438-472, as one batch): frame f is what
+// zk_compress_frames_prefix writes for its bytes alone with frame_size = max(size, 1)
+// ---------------------------------------------------------------------------------------------
+extern "C" int32_t zk_compress_frames_sized(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                            int32_t checksum, const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap,
+                                            uint32_t* c_sizes, size_t* dst_len) {
+    if (!c || (n_frames && (!frame_sizes || !dst))) return ZK_ERR_INVALID_ARG;
+    size_t n = 0;
+    int32_t rc = zk_sized_check(frame_sizes, n_frames, &n);
+    if (rc) return rc;
+    if (n && !src) return ZK_ERR_INVALID_ARG;
+    if (dst_len) *dst_len = 0;
+    if (n_frames == 0) return 0;
+    rc = zk_ctx_set_prefix(c, prefix, prefix_len);
+    if (rc) return rc;
+    const ZkFrameList fl = {frame_sizes, n, 0, n_frames};
+    rc = zk_compress_host_run(c, fl, src, level, checksum, dst, dst_cap, c_sizes, dst_len);
+    c->cur_prefix_len = 0;
+    return rc;
+}
+
+extern "C" int32_t zk_compress_frames_sized_dev(zk_ctx* c, const void* d_src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                                int32_t checksum, void* d_dst, size_t dst_cap, uint32_t* c_sizes, size_t* dst_len,
+                                                void* cuda_stream) {
+    if (!c || (n_frames && (!frame_sizes || !d_dst))) return ZK_ERR_INVALID_ARG;
+    size_t n = 0;
+    const int32_t rc = zk_sized_check(frame_sizes, n_frames, &n);
+    if (rc) return rc;
+    if (n && !d_src) return ZK_ERR_INVALID_ARG;
+    if (dst_len) *dst_len = 0;
+    if (n_frames == 0) return 0;
+    ZK_RT_OK(cudaSetDevice(c->device));
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : c->slot[0].stream;
+    const ZkFrameList fl = {frame_sizes, n, 0, n_frames};
+    return zk_compress_dev_run(c, fl, (const uint8_t*)d_src, level, checksum, (uint8_t*)d_dst, dst_cap, c_sizes, dst_len, st);
 }
 
 // ---------------------------------------------------------------------------------------------

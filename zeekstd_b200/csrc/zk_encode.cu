@@ -17,6 +17,7 @@
 // by libzstd; the compressed bytes are NOT meant to equal libzstd's.
 #include "zk_encode.h"
 #include <string.h>
+#include <vector>
 
 #define ZKC_BLOCK 32768u                 // zstd block size used by this encoder (<= Block_Maximum_Size)
 #define ZKC_HLOG_FAST 11                 // hash table per warp: 2048 x u16 at level 1 (40 warps / SM hide the two dependent loads per window),
@@ -36,8 +37,23 @@ struct ZkcBlock {                        // per-block record in HBM
 #define ZKC_SEQSEC 16384u                // per-block scratch for the sequence section: [0,256) header, [256,..) bitstream
 #define ZKC_SEQHDR 256u
 
+// The block geometry of a batch (DESIGN §2), built on the device by zk_geo_*_kernel from per-frame sizes (the caller's, or those of
+// the uniform layout): every kernel reads a block's input range and its place in its frame, and a frame's range and blocks, from
+// these two tables and nowhere else.  A frame of d bytes has max(1, ceil(d / ZKC_BLOCK)) blocks, cut from its first byte.
+struct ZkcGeo {                          // per block, 24 bytes
+    size_t lo;                           // first input byte; the frame starts at lo - k * ZKC_BLOCK
+    uint32_t len;                        // input bytes (0 only in the one block of an empty frame)
+    uint32_t frame, k;                   // frame index, block index inside the frame
+    uint32_t last;                       // 1: the last block of its frame
+};
+struct ZkcFrame {                        // per frame, 24 bytes
+    size_t start;                        // first input byte
+    uint32_t size, first_block, n_blocks, pad;
+};
+
 struct ZkEncodeArgs {
-    const uint8_t* src; size_t n; uint32_t frame_size; uint32_t n_frames; uint32_t blocks_per_frame; uint32_t n_blocks;
+    const uint8_t* src; size_t n; uint32_t n_frames; uint32_t n_blocks;
+    const ZkcGeo* geo; const ZkcFrame* frames;
     int level, checksum;
     ZkcBlock* blocks;
     uint16_t* seq_ll; uint16_t* seq_ml; uint32_t* seq_off;      // ZKC_MAXSEQ per block
@@ -57,12 +73,78 @@ struct ZkEncodeArgs {
 };
 #define ZKC_PSLOT (2u * ZKC_BLOCK + 64u)   // per-frame staging slot: [prefix tail | first block]
 
-__device__ __forceinline__ void zkc_block_range(const ZkEncodeArgs& a, uint32_t b, size_t& lo, size_t& hi, size_t& fstart) {
-    uint32_t f = b / a.blocks_per_frame, k = b % a.blocks_per_frame;
-    fstart = (size_t)f * a.frame_size;
-    size_t fend = fstart + a.frame_size < a.n ? fstart + a.frame_size : a.n;
-    lo = fstart + (size_t)k * ZKC_BLOCK; if (lo > fend) lo = fend;
-    hi = lo + ZKC_BLOCK < fend ? lo + ZKC_BLOCK : fend;
+__device__ __forceinline__ ZkcGeo zkc_block_range(const ZkEncodeArgs& a, uint32_t b, size_t& lo, size_t& hi, size_t& fstart) {
+    const ZkcGeo g = a.geo[b];
+    lo = g.lo; hi = g.lo + g.len; fstart = g.lo - (size_t)g.k * ZKC_BLOCK;
+    return g;
+}
+
+// uniform layout: frames of frame_size bytes, the last one shorter (n_frames = 1 and one empty frame when n == 0).  Every frame but the
+// last is full, so frame f starts at block f * ceil(frame_size / ZKC_BLOCK)
+__global__ void __launch_bounds__(256) zk_geo_uniform_kernel(ZkcFrame* fr, uint32_t n_frames, size_t n, uint32_t frame_size) {
+    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n_frames) return;
+    const uint32_t bpf = (uint32_t)(((size_t)frame_size + ZKC_BLOCK - 1) / ZKC_BLOCK);
+    const size_t start = (size_t)f * frame_size;
+    const uint32_t size = (uint32_t)(n - start < frame_size ? n - start : frame_size);
+    ZkcFrame r;
+    r.start = start; r.size = size; r.first_block = f * bpf; r.n_blocks = size ? (size + ZKC_BLOCK - 1) / ZKC_BLOCK : 1u; r.pad = 0;
+    fr[f] = r;
+}
+
+// caller-chosen sizes: frame starts and first blocks by one scan (one CTA, 1024 frames a round)
+__global__ void __launch_bounds__(1024) zk_geo_sized_kernel(ZkcFrame* fr, const uint32_t* sizes, uint32_t n_frames) {
+    __shared__ unsigned long long wb[32], cb;
+    __shared__ uint32_t wk[32], ck;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) { cb = 0; ck = 0; }
+    __syncthreads();
+    for (uint32_t base = 0; base < n_frames; base += 1024) {
+        const uint32_t f = base + threadIdx.x;
+        const uint32_t d = f < n_frames ? sizes[f] : 0u;
+        const uint32_t nb = f < n_frames ? (d ? (d + ZKC_BLOCK - 1) / ZKC_BLOCK : 1u) : 0u;
+        unsigned long long xb = d; uint32_t xk = nb;
+#pragma unroll
+        for (int s = 1; s < 32; s <<= 1) {
+            const unsigned long long tb = __shfl_up_sync(0xFFFFFFFFu, xb, s); const uint32_t tk = __shfl_up_sync(0xFFFFFFFFu, xk, s);
+            if (lane >= s) { xb += tb; xk += tk; }
+        }
+        if (lane == 31) { wb[warp] = xb; wk[warp] = xk; }
+        __syncthreads();
+        if (warp == 0) {
+            unsigned long long yb = wb[lane]; uint32_t yk = wk[lane];
+#pragma unroll
+            for (int s = 1; s < 32; s <<= 1) {
+                const unsigned long long tb = __shfl_up_sync(0xFFFFFFFFu, yb, s); const uint32_t tk = __shfl_up_sync(0xFFFFFFFFu, yk, s);
+                if (lane >= s) { yb += tb; yk += tk; }
+            }
+            wb[lane] = yb; wk[lane] = yk;
+        }
+        __syncthreads();
+        if (f < n_frames) {
+            ZkcFrame r;
+            r.start = cb + (warp ? wb[warp - 1] : 0ull) + xb - d; r.size = d;
+            r.first_block = ck + (warp ? wk[warp - 1] : 0u) + xk - nb; r.n_blocks = nb; r.pad = 0;
+            fr[f] = r;
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) { cb += wb[31]; ck += wk[31]; }
+        __syncthreads();
+    }
+}
+
+// one thread per block: its frame is the last one whose first block is <= b (every frame has a block, so first blocks increase)
+__global__ void __launch_bounds__(256) zk_geo_block_kernel(ZkcGeo* geo, const ZkcFrame* fr, uint32_t n_frames, uint32_t n_blocks) {
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= n_blocks) return;
+    uint32_t lo = 0, hi = n_frames - 1;
+    while (lo < hi) { const uint32_t mid = lo + (hi - lo + 1) / 2; if (fr[mid].first_block <= b) lo = mid; else hi = mid - 1; }
+    const ZkcFrame F = fr[lo];
+    const uint32_t k = b - F.first_block, off = k * ZKC_BLOCK;
+    ZkcGeo g;
+    g.lo = F.start + off; g.len = F.size - off < ZKC_BLOCK ? F.size - off : ZKC_BLOCK;
+    g.frame = lo; g.k = k; g.last = k + 1 == F.n_blocks ? 1u : 0u;
+    geo[b] = g;
 }
 
 // unaligned 8-byte little-endian load from global memory
@@ -140,9 +222,8 @@ __device__ __forceinline__ void zkc_warp_copy(uint8_t* __restrict__ d, const uin
 // prefix mode: [tail of the prefix | first block of frame f] -> pstage slot f (one CTA per frame)
 __global__ void __launch_bounds__(256) zk_prefix_stage_kernel(ZkEncodeArgs a) {
     const uint32_t f = blockIdx.x;
-    const size_t fstart = (size_t)f * a.frame_size;
-    const size_t fend = fstart + a.frame_size < a.n ? fstart + a.frame_size : a.n;
-    const uint32_t len = (uint32_t)(fend - fstart < ZKC_BLOCK ? fend - fstart : ZKC_BLOCK);
+    const size_t fstart = a.frames[f].start;
+    const uint32_t len = a.geo[a.frames[f].first_block].len;
     uint8_t* d = a.pstage + (size_t)f * ZKC_PSLOT;
     const uint8_t* pt = a.prefix + (a.prefix_len - a.ptail);
     for (uint32_t i = threadIdx.x; i < a.ptail; i += blockDim.x) d[i] = pt[i];
@@ -206,11 +287,11 @@ __global__ void __launch_bounds__(NW * 32) zk_match_fast_kernel(ZkEncodeArgs a) 
     if (b >= a.n_blocks) return;
     uint16_t* table = tables[warp];
     size_t lo, hi, fstart;
-    zkc_block_range(a, b, lo, hi, fstart);
+    const ZkcGeo g = zkc_block_range(a, b, lo, hi, fstart);
     const bool pfx = a.ptail != 0 && lo == fstart;
     const size_t hist = a.hist_cap < ZKC_BLOCK ? a.hist_cap : ZKC_BLOCK;
     const size_t base = lo - fstart >= hist ? lo - hist : fstart;
-    const uint8_t* sb = pfx ? a.pstage + (size_t)(b / a.blocks_per_frame) * ZKC_PSLOT : a.src + base;
+    const uint8_t* sb = pfx ? a.pstage + (size_t)g.frame * ZKC_PSLOT : a.src + base;
     const uint32_t lo32 = pfx ? a.ptail : (uint32_t)(lo - base), hi32 = lo32 + (uint32_t)(hi - lo);
     for (int i = lane; i < (1 << HLOG); i += 32) table[i] = 0;
     __syncwarp();
@@ -806,15 +887,9 @@ __global__ void __launch_bounds__(32 * NW, HUF ? 32 / NW : 1) zk_lit_enc_kernel(
     const uint32_t b = blockIdx.x * NW + (threadIdx.x >> 5);
     if (b >= a.n_blocks) return;
     ZkcLitWarp& sm = sms[HUF ? threadIdx.x >> 5 : 0];
-    size_t lo, hi, fstart;
-    zkc_block_range(a, b, lo, hi, fstart);
-    const uint32_t len = (uint32_t)(hi - lo);
-    const uint32_t k_in_frame = b % a.blocks_per_frame;
-    // blocks past the end of a short last frame carry nothing
-    const size_t fend = fstart + a.frame_size < a.n ? fstart + a.frame_size : a.n;
-    uint32_t nb_frame = (uint32_t)((fend - fstart + ZKC_BLOCK - 1) / ZKC_BLOCK); if (nb_frame == 0) nb_frame = 1;
-    if (k_in_frame >= nb_frame) { if (lane == 0) { a.blocks[b].csize = 0; a.blocks[b].lit_bytes = 0xFFFFFFFFu; } return; }
-    const uint32_t last_flag = k_in_frame == nb_frame - 1 ? 1u : 0u;
+    const ZkcGeo g = a.geo[b];
+    const uint32_t len = g.len;
+    const uint32_t last_flag = g.last;
     const uint32_t nlit = a.blocks[b].nlit;
     const uint8_t* lits = a.lits + (size_t)b * ZKC_BLOCK;
     uint8_t* out = a.stage + (size_t)b * ZKC_SLOT;
@@ -1071,10 +1146,9 @@ __global__ void __launch_bounds__(128) zk_block_finish_kernel(ZkEncodeArgs a) {
     const uint32_t b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (b >= a.n_blocks) return;
     const ZkcBlock bl = a.blocks[b];
-    if (bl.csize == 0 && bl.lit_bytes == 0xFFFFFFFFu) return;           // slot beyond the end of a short frame
-    size_t lo, hi, fstart;
-    zkc_block_range(a, b, lo, hi, fstart);
-    const uint32_t len = (uint32_t)(hi - lo);
+    const ZkcGeo g = a.geo[b];
+    const size_t lo = g.lo;
+    const uint32_t len = g.len;
     uint8_t* out = a.stage + (size_t)b * ZKC_SLOT;
     uint32_t opos = bl.lit_bytes;
     bool raw_block = opos == 0;
@@ -1112,9 +1186,7 @@ __global__ void __launch_bounds__(128) zk_frame_hash_kernel(ZkEncodeArgs a) {
     const int lane = threadIdx.x & 31;
     const uint32_t f = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (f >= a.n_frames) return;
-    const size_t fstart = (size_t)f * a.frame_size;
-    const size_t fend = fstart + a.frame_size < a.n ? fstart + a.frame_size : a.n;
-    const uint8_t* p = a.src + fstart; const uint32_t len = (uint32_t)(fend - fstart);
+    const uint8_t* p = a.src + a.frames[f].start; const uint32_t len = a.frames[f].size;
     const unsigned long long h = zk_warp_xxh64(p, len, lane);
     if (lane == 0) a.frame_hash[f] = (uint32_t)h;
 }
@@ -1124,8 +1196,9 @@ __global__ void __launch_bounds__(256) zk_frame_size_kernel(ZkEncodeArgs a) {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= a.n_frames) return;
     uint32_t off = ZKC_FRAME_HDR;
-    for (uint32_t k = 0; k < a.blocks_per_frame; k++) {
-        ZkcBlock& bl = a.blocks[(size_t)f * a.blocks_per_frame + k];
+    const uint32_t b0 = a.frames[f].first_block, b1 = b0 + a.frames[f].n_blocks;
+    for (uint32_t b = b0; b < b1; b++) {
+        ZkcBlock& bl = a.blocks[b];
         bl.out_off = off; off += bl.csize;
     }
     if (a.checksum) off += 4;
@@ -1162,8 +1235,7 @@ __global__ void __launch_bounds__(1024) zk_frame_scan_kernel(ZkEncodeArgs a) {
 __global__ void __launch_bounds__(128) zk_frame_window_kernel(ZkEncodeArgs a, uint32_t n_frames, uint32_t wmin, uint32_t wmax) {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= n_frames || *a.error) return;
-    const size_t fstart = (size_t)f * a.frame_size;
-    const size_t fcs = (fstart + a.frame_size < a.n ? fstart + a.frame_size : a.n) - fstart;
+    const size_t fcs = a.frames[f].size;
     size_t want = fcs + a.ptail < wmax ? fcs + a.ptail : wmax;
     if (want < wmin) want = wmin;
     uint32_t e = 0, m = 0;                                    // Window_Size = 2^(10 + e) * (1 + m / 8)
@@ -1177,13 +1249,12 @@ __global__ void __launch_bounds__(128) zk_frame_gather_kernel(ZkEncodeArgs a) {
     const int lane = threadIdx.x & 31;
     const uint32_t b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (b >= a.n_blocks || *a.error) return;
-    const uint32_t f = b / a.blocks_per_frame, k = b % a.blocks_per_frame;
+    const ZkcGeo g = a.geo[b];
+    const uint32_t f = g.frame;
     const ZkcBlock bl = a.blocks[b];
     uint8_t* fo = a.dst + a.frame_off[f];
-    if (k == 0 && lane == 0) {
-        const size_t fstart = (size_t)f * a.frame_size;
-        const size_t fend = fstart + a.frame_size < a.n ? fstart + a.frame_size : a.n;
-        const uint32_t fcs = (uint32_t)(fend - fstart);
+    if (g.k == 0 && lane == 0) {
+        const uint32_t fcs = a.frames[f].size;
         fo[0] = 0x28; fo[1] = 0xB5; fo[2] = 0x2F; fo[3] = 0xFD;
         fo[4] = (uint8_t)(0x80 | (a.checksum ? 0x04 : 0));       // FCS 4 bytes, no single segment, no dict
         fo[5] = 0x38;                                             // window 128 KiB (log 17): offsets stay below 64 KiB
@@ -1417,6 +1488,15 @@ size_t zk_encode_bound(size_t n, uint32_t frame_size) {
     return n + frames * (ZKC_FRAME_HDR + 4) + blocks * 3 + 64;
 }
 
+// blocks of a frame of d bytes
+static inline uint32_t zkc_frame_blocks(size_t d) { return d ? (uint32_t)((d + ZKC_BLOCK - 1) / ZKC_BLOCK) : 1u; }
+
+size_t zk_encode_bound_sized(const uint32_t* sizes, uint32_t n_frames) {
+    size_t b = 64;
+    for (uint32_t f = 0; f < n_frames; f++) b += (size_t)sizes[f] + ZKC_FRAME_HDR + 4 + 3 * (size_t)zkc_frame_blocks(sizes[f]);
+    return b;
+}
+
 void zk_encode_ws_free(ZkEncodeWs* ws) {
     if (ws->buf) cudaFree(ws->buf);
     if (ws->h_sizes) cudaFreeHost(ws->h_sizes);
@@ -1431,23 +1511,51 @@ void zk_encode_ws_free(ZkEncodeWs* ws) {
 static size_t zkc_align(size_t v) { return (v + 255) & ~(size_t)255; }
 // the level a caller asks for -> the one the kernels run: 0 is the default (3), levels below ZSTD_minCLevel() clamp to it
 static int zkc_level(int level) { return level == 0 ? 3 : (level < ZKC_MIN_LEVEL ? ZKC_MIN_LEVEL : level); }
-static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, const ZkEncodeArgs& a);
+struct ZkcHcPass;
+static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, const ZkEncodeArgs& a, const std::vector<ZkcHcPass>* hc_plan);
+
+// the frame and block tables of a batch, on `stream`: h_sizes == nullptr: the uniform layout of (n, frame_size), generated on the device;
+// otherwise the caller's sizes, uploaded to d_sizes and scanned there
+static int zkc_build_geometry(ZkEncodeWs* ws, cudaStream_t stream, ZkcGeo* geo, ZkcFrame* fr, uint32_t n_frames, uint32_t n_blocks,
+                              size_t n, uint32_t frame_size, const uint32_t* h_sizes, uint32_t* d_sizes) {
+    if (h_sizes) {
+        ZKC_CUDA_OK(cudaMemcpyAsync(d_sizes, h_sizes, (size_t)n_frames * 4, cudaMemcpyHostToDevice, stream));
+        ZK_LAUNCH(zk_geo_sized_kernel, 1, 1024, 0, stream, fr, (const uint32_t*)d_sizes, n_frames);
+    } else ZK_LAUNCH(zk_geo_uniform_kernel, (n_frames + 255) / 256, 256, 0, stream, fr, n_frames, n, frame_size);
+    ZK_LAUNCH(zk_geo_block_kernel, (n_blocks + 255) / 256, 256, 0, stream, geo, (const ZkcFrame*)fr, n_frames, n_blocks);
+    ws->launches += 2;
+    return 0;
+}
 
 #include "zk_hc.inc"
 
-int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t frame_size, int level,
-                      int checksum, uint8_t* d_dst, size_t dst_cap, uint32_t n_frames) {
+// one batch of n_frames frames: of frame_size bytes (the last one shorter) when h_sizes is null, else of h_sizes[f] bytes (n = their sum)
+static int zkc_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t frame_size, const uint32_t* h_sizes,
+                       uint32_t n_frames, int level, int checksum, uint8_t* d_dst, size_t dst_cap) {
     const uint8_t* d_prefix = ws->prefix; const uint32_t prefix_len = ws->prefix_len;     // one-shot (set by the caller for THIS batch)
     ws->prefix = nullptr; ws->prefix_len = 0;
     ws->pending_frames = 0;
     if (n_frames == 0) return 0;
-    if (frame_size == 0 || frame_size > 0x40000000u) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
-    const size_t eff = n < frame_size ? n : frame_size;          // a lone short frame needs fewer block slots
-    uint32_t bpf = (uint32_t)((eff + ZKC_BLOCK - 1) / ZKC_BLOCK); if (bpf == 0) bpf = 1;
-    const size_t n_blocks = (size_t)n_frames * bpf;
+    size_t n_blocks = 0;
+    if (h_sizes) {
+        for (uint32_t f = 0; f < n_frames; f++) {
+            if (h_sizes[f] > 0x40000000u) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
+            n_blocks += zkc_frame_blocks(h_sizes[f]);
+        }
+    } else {
+        if (frame_size == 0 || frame_size > 0x40000000u) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
+        n_blocks = (size_t)(n_frames - 1) * zkc_frame_blocks(frame_size) + zkc_frame_blocks(n - (size_t)(n_frames - 1) * frame_size);
+    }
     if (n_blocks > 0x7FFFFFFFull) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
+    const int lvl = zkc_level(level);
+    const uint32_t pt = d_prefix && prefix_len && n ? (prefix_len < ZKC_BLOCK ? prefix_len : ZKC_BLOCK) : 0u;
+    std::vector<ZkcHcPass> hc_plan;
+    const uint32_t hc_span = lvl >= ZKC_HC_LEVEL ? zkc_hc_plan(n, frame_size, h_sizes, n_frames, (uint32_t)n_blocks, pt, hc_plan) : 0u;
     // carve the workspace
     size_t off = 0;
+    const size_t o_geo = off; off = zkc_align(off + n_blocks * sizeof(ZkcGeo));
+    const size_t o_fr = off; off = zkc_align(off + (size_t)n_frames * sizeof(ZkcFrame));
+    const size_t o_fsz = off; if (h_sizes) off = zkc_align(off + (size_t)n_frames * 4);
     const size_t o_blocks = off; off = zkc_align(off + n_blocks * sizeof(ZkcBlock));
     const size_t o_ll = off; off = zkc_align(off + n_blocks * ZKC_MAXSEQ * 2);
     const size_t o_ml = off; off = zkc_align(off + n_blocks * ZKC_MAXSEQ * 2);
@@ -1459,13 +1567,9 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     const size_t o_foff = off; off = zkc_align(off + (size_t)n_frames * 8);
     const size_t o_fh = off; off = zkc_align(off + (size_t)n_frames * 4);
     const size_t o_tot = off; off = zkc_align(off + 16);
-    const size_t o_pst = off; if (d_prefix && prefix_len && n) off = zkc_align(off + (size_t)n_frames * ZKC_PSLOT);
-    const int lvl = zkc_level(level);
+    const size_t o_pst = off; if (pt) off = zkc_align(off + (size_t)n_frames * ZKC_PSLOT);
     const size_t o_hc = off;
-    if (lvl >= ZKC_HC_LEVEL) {
-        const uint32_t pt = d_prefix && prefix_len && n ? (prefix_len < ZKC_BLOCK ? prefix_len : ZKC_BLOCK) : 0u;
-        off = zkc_align(off + zkc_hc_layout(zkc_hc_span(n, frame_size, bpf, (uint32_t)n_blocks, pt), nullptr, nullptr));
-    }
+    if (lvl >= ZKC_HC_LEVEL) off = zkc_align(off + zkc_hc_layout(hc_span, nullptr, nullptr));
     if (ws->cap < off) {
         if (ws->buf) cudaFree(ws->buf);
         ws->buf = nullptr; ws->cap = 0;
@@ -1482,7 +1586,8 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     }
     uint8_t* base = (uint8_t*)ws->buf;
     ZkEncodeArgs a;
-    a.src = d_src; a.n = n; a.frame_size = frame_size; a.n_frames = n_frames; a.blocks_per_frame = bpf; a.n_blocks = (uint32_t)n_blocks;
+    a.src = d_src; a.n = n; a.n_frames = n_frames; a.n_blocks = (uint32_t)n_blocks;
+    a.geo = (const ZkcGeo*)(base + o_geo); a.frames = (const ZkcFrame*)(base + o_fr);
     a.level = lvl; a.checksum = checksum ? 1 : 0;
     a.blocks = (ZkcBlock*)(base + o_blocks);
     a.seq_ll = (uint16_t*)(base + o_ll); a.seq_ml = (uint16_t*)(base + o_ml); a.seq_off = (uint32_t*)(base + o_off);
@@ -1492,8 +1597,11 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     a.prefix = d_prefix; a.prefix_len = 0; a.ptail = 0; a.pstage = base + o_pst;
     a.hist_cap = ~(size_t)0;
     a.hc = base + o_hc;
-    if (d_prefix && prefix_len && n) {
-        a.prefix_len = prefix_len; a.ptail = prefix_len < ZKC_BLOCK ? prefix_len : ZKC_BLOCK;
+    int rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo), (ZkcFrame*)(base + o_fr), n_frames, (uint32_t)n_blocks, n, frame_size,
+                                h_sizes, (uint32_t*)(base + o_fsz));
+    if (rc) return rc;
+    if (pt) {
+        a.prefix_len = prefix_len; a.ptail = pt;
         ZK_LAUNCH(zk_prefix_stage_kernel, n_frames, 256, 0, stream, a);
         ws->launches += 1;
     }
@@ -1514,7 +1622,7 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
         ZKC_CUDA_OK(cudaEventRecord(ws->ev_c, stream)); ZKC_CUDA_OK(cudaStreamWaitEvent(ss, ws->ev_c, 0));     // after whatever produced the input
         ZK_LAUNCH(zk_frame_hash_kernel, (n_frames + 3) / 4, 128, 0, ss, a);
     }
-    int rc = zkc_run_blocks(ws, stream, ss, a);
+    rc = zkc_run_blocks(ws, stream, ss, a, &hc_plan);
     if (rc) return rc;
     ws->prof.begin(7, stream);
     if (checksum && ss == stream) ZK_LAUNCH(zk_frame_hash_kernel, (n_frames + 3) / 4, 128, 0, stream, a);   // else: already done on the side stream (joined by ev_b)
@@ -1531,8 +1639,21 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     return 0;
 }
 
-// K-C1 and K-C2 over every block of `a` (match finding, then sequences on `ss` beside literals on `stream`, joined by the finish kernel)
-static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, const ZkEncodeArgs& a) {
+int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t frame_size, int level,
+                      int checksum, uint8_t* d_dst, size_t dst_cap, uint32_t n_frames) {
+    return zkc_enqueue(ws, stream, d_src, n, frame_size, nullptr, n_frames, level, checksum, d_dst, dst_cap);
+}
+
+int zk_encode_enqueue_sized(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, const uint32_t* frame_sizes, uint32_t n_frames,
+                            int level, int checksum, uint8_t* d_dst, size_t dst_cap) {
+    size_t n = 0;
+    for (uint32_t f = 0; f < n_frames; f++) n += frame_sizes[f];
+    return zkc_enqueue(ws, stream, d_src, n, 0, frame_sizes, n_frames, level, checksum, d_dst, dst_cap);
+}
+
+// K-C1 and K-C2 over every block of `a` (match finding, then sequences on `ss` beside literals on `stream`, joined by the finish kernel);
+// hc_plan: the internal passes of the high-level tier (zkc_hc_plan)
+static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, const ZkEncodeArgs& a, const std::vector<ZkcHcPass>* hc_plan) {
     const size_t n_blocks = a.n_blocks;
     ws->prof.begin(5, stream);
     // six tiers (EncodeOptions::compression_level, encode.rs:176): 1 = 2048-entry table, no history, no lazy step; 2-3 = 4096 entries,
@@ -1541,7 +1662,7 @@ static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, 
     // entries in dynamic shared memory.  Ratio on the reference's corpus: 2.12 / 2.24 / 2.28 / 2.38 / 2.40 / 2.50.  Below them the fast tier
     // (level < 0): level 1's table with sparse probing, literals without Huffman coding.  From ZKC_HC_LEVEL on, K-C1h (zk_hc.inc): hash chains
     // over 2 MiB of the frame and a price-based parse
-    if (a.level >= ZKC_HC_LEVEL) { const int rc = zkc_run_hc(ws, stream, a); if (rc) return rc; }
+    if (a.level >= ZKC_HC_LEVEL) { const int rc = zkc_run_hc(ws, stream, a, *hc_plan); if (rc) return rc; }
     else if (a.level < 0) ZK_LAUNCH((zk_match_fast_kernel<ZKC_HLOG_FAST, ZKC_C1_WARPS>), (uint32_t)((n_blocks + ZKC_C1_WARPS - 1) / ZKC_C1_WARPS), ZKC_C1_WARPS * 32, 0, stream, a);
     else if (a.level <= 1) ZK_LAUNCH((zk_match_kernel<ZKC_HLOG_FAST, ZKC_C1_WARPS, false>), (uint32_t)((n_blocks + ZKC_C1_WARPS - 1) / ZKC_C1_WARPS), ZKC_C1_WARPS * 32, 0, stream, a);
     else if (a.level <= 3) ZK_LAUNCH((zk_match_kernel<ZKC_HLOG, ZKC_C1_WARPS, false>), (uint32_t)((n_blocks + ZKC_C1_WARPS - 1) / ZKC_C1_WARPS), ZKC_C1_WARPS * 32, 0, stream, a);
@@ -1625,6 +1746,11 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     const size_t o_fh = off; off = zkc_align(off + (size_t)nb * 4);
     const size_t o_res = off; off = zkc_align(off + res_words * 4);
     const size_t o_pst = off; if (pfx) off = zkc_align(off + (size_t)nb * ZKC_PSLOT);
+    // the two layouts of the variants: frames of one block (d = 0), one frame over the pass (d >= 1)
+    const size_t o_geo0 = off; off = zkc_align(off + (size_t)nb * sizeof(ZkcGeo));
+    const size_t o_fr0 = off; off = zkc_align(off + (size_t)nb * sizeof(ZkcFrame));
+    const size_t o_geo1 = off; off = zkc_align(off + (size_t)nb * sizeof(ZkcGeo));
+    const size_t o_fr1 = off; off = zkc_align(off + sizeof(ZkcFrame));
     if (ws->cap < off) {
         if (ws->buf) cudaFree(ws->buf);
         ws->buf = nullptr; ws->cap = 0;
@@ -1659,12 +1785,15 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
         }
         ss = ws->side;
     }
+    int rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo0), (ZkcFrame*)(base + o_fr0), nb, nb, n, ZKC_BLOCK, nullptr, nullptr);
+    if (!rc) rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo1), (ZkcFrame*)(base + o_fr1), 1, nb, n, (uint32_t)n, nullptr, nullptr);
+    if (rc) return rc;
     // variant passes.  d = 0: frames of one block, so every block opens its frame (prefix staging included); d >= 1: one frame
     // over the pass, with the wide tier's history capped at d blocks below V - 1
     for (uint32_t d = 0; d < V; d++) {
         ZkEncodeArgs a;
-        a.src = d_src; a.n = n; a.n_blocks = nb;
-        a.frame_size = d == 0 ? ZKC_BLOCK : (uint32_t)n; a.n_frames = d == 0 ? nb : 1; a.blocks_per_frame = d == 0 ? 1 : nb;
+        a.src = d_src; a.n = n; a.n_blocks = nb; a.n_frames = d == 0 ? nb : 1;
+        a.geo = (const ZkcGeo*)(base + (d == 0 ? o_geo0 : o_geo1)); a.frames = (const ZkcFrame*)(base + (d == 0 ? o_fr0 : o_fr1));
         a.level = lvl; a.checksum = c.checksum;
         a.blocks = (ZkcBlock*)(base + o_blocks) + (size_t)d * nb;
         a.seq_ll = (uint16_t*)(base + o_ll); a.seq_ml = (uint16_t*)(base + o_ml); a.seq_off = (uint32_t*)(base + o_off);
@@ -1679,7 +1808,7 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
             ZK_LAUNCH(zk_prefix_stage_kernel, nb, 256, 0, stream, a);
             ws->launches += 1;
         }
-        int rc = zkc_run_blocks(ws, stream, ss, a);
+        rc = zkc_run_blocks(ws, stream, ss, a, nullptr);
         if (rc) return rc;
         ws->launches += 4;
     }

@@ -22,9 +22,13 @@ int zk_encode_batch(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
                     int checksum, uint8_t* d_dst, size_t dst_cap, uint32_t* c_sizes, uint32_t n_frames, size_t* dst_len);
 int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t frame_size, int level,
                       int checksum, uint8_t* d_dst, size_t dst_cap, uint32_t n_frames);
+// The same with caller-chosen frame sizes: frame f covers frame_sizes[f] bytes (each <= 1 GiB; 0: an empty frame) of d_src, back to back
+int zk_encode_enqueue_sized(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, const uint32_t* frame_sizes, uint32_t n_frames,
+                            int level, int checksum, uint8_t* d_dst, size_t dst_cap);
 int zk_encode_collect(ZkEncodeWs* ws, cudaStream_t stream, uint32_t* c_sizes, size_t* dst_len);
 void zk_encode_ws_free(ZkEncodeWs* ws);
 size_t zk_encode_bound(size_t n, uint32_t frame_size);
+size_t zk_encode_bound_sized(const uint32_t* frame_sizes, uint32_t n_frames);
 
 // FrameSizePolicy::Compressed(target) over one pass of n <= 1 GiB bytes at d_src: frames close after the first 32 KiB block at which
 // header + blocks >= target, or at 1 GiB of input.  at_end: the pass ends the caller's input; final_: and no more input follows, so
