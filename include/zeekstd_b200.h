@@ -180,6 +180,25 @@ int32_t zk_compress_frames_sized_dev(zk_ctx* ctx, const void* d_src, const uint3
 /* Upper bound of the compressed size of frames of these sizes (excl. seek table). */
 size_t zk_compress_bound_sized(const uint32_t* frame_sizes, uint32_t n_frames);
 
+/*
+ * Long-distance matching (patch mode): zk_compress_frames_prefix / zk_compress_frames_sized with every frame matched against the WHOLE
+ * prefix, not only its last 32 KiB -- what the reference CLI asks of libzstd for `--patch-from` (WindowLog and
+ * EnableLongDistanceMatching on the CCtx it hands to EncodeOptions::with_cctx, cli/src/compress.rs:31-37).  A frame that repeats the
+ * prefix with a few edits shrinks to the edits.  A non-empty frame announces a Window_Size of min(frame content + prefix_len, 2^27) (at
+ * least what the prefix calls announce), which a default libzstd DCtx and zk_decompress_frames_prefix accept; no offset exceeds it, so with a
+ * prefix above 128 MiB only its last 128 MiB are matched, and the far end of the prefix is out of reach late in a large frame.
+ * Long-distance matching is part of the high-level tier: every `level`, negative ones included, writes what level 16 writes here.
+ * prefix == NULL or prefix_len == 0: exactly the plain call at `level`.  The index of the prefix is rebuilt on every call (and for
+ * every 96 MiB of input within one).  zk_compress_frames_csize has no such variant: its exact cut needs a bounded history per block.
+ * HOST pointers.
+ */
+int32_t zk_compress_frames_ldm(zk_ctx* ctx, const uint8_t* src, size_t n, uint32_t frame_size, int32_t level,
+                               int32_t checksum, const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap,
+                               uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len);
+int32_t zk_compress_frames_sized_ldm(zk_ctx* ctx, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                     int32_t checksum, const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap,
+                                     uint32_t* c_sizes, size_t* dst_len);
+
 /* ------------------------------------------------------------------ SeekTable (lib/src/seek_table.rs) */
 typedef struct zk_seek_table zk_seek_table;
 typedef enum { ZK_FORMAT_HEAD = 0, ZK_FORMAT_FOOT = 1 } zk_format; /* seek_table.rs:228-241 */
@@ -230,6 +249,11 @@ void zk_encode_options_free(zk_encode_options* o);
 void zk_encode_options_frame_size_policy(zk_encode_options* o, zk_frame_size_policy kind, uint32_t size); /* :158 */
 void zk_encode_options_checksum_flag(zk_encode_options* o, int32_t flag);               /* :166 */
 void zk_encode_options_compression_level(zk_encode_options* o, int32_t level);          /* :176 */
+/* flag != 0: frames given a prefix (the *_compress_with_prefix calls) are matched against the whole of it, as by zk_compress_frames_ldm
+ * (the counterpart of the CCtx the reference CLI prepares for with_cctx); every level then runs as level 16.  RawEncoder honours it
+ * under both policies (its trial compressions included), Encoder under Uncompressed(n): with Compressed(n)
+ * zk_encode_options_into_encoder returns ZK_ERR_INVALID_ARG and does not consume the options */
+void zk_encode_options_long_distance_matching(zk_encode_options* o, int32_t flag);
 /* consume the options (like `self`) */
 int32_t zk_encode_options_into_raw_encoder(zk_encode_options* o, zk_raw_encoder** out); /* :188 */
 int32_t zk_encode_options_into_encoder(zk_encode_options* o, zk_write_fn write, zk_flush_fn flush, void* user,

@@ -127,8 +127,10 @@ class Context:
     def last_device_ms(self) -> float: return float(self.lib.zk_ctx_last_device_ms(self._h))
 
     # ---- batch codec (the hot path) ------------------------------------------------------------
-    def compress_frames(self, data, frame_size: int = 0x200000, level: int = 0, checksum: bool = False, prefix=None):
-        """-> (compressed bytes (np.uint8), c_sizes, d_sizes).  Host buffers.  prefix: raw-content prefix of every frame."""
+    def compress_frames(self, data, frame_size: int = 0x200000, level: int = 0, checksum: bool = False, prefix=None, long_distance: bool = False):
+        """-> (compressed bytes (np.uint8), c_sizes, d_sizes).  Host buffers.  prefix: raw-content prefix of every frame.
+        long_distance: match every frame against the whole prefix (its last 128 MiB), not only its last 32 KiB: patch mode.  Every level
+        then writes what level 16 writes; without a prefix the flag changes nothing."""
         addr, n, keep = _buf(data)
         lib = self.lib
         cap = lib.zk_compress_bound(n, frame_size)
@@ -138,7 +140,8 @@ class Context:
         nf = c_uint32(); dl = c_size_t()
         if prefix is not None:
             paddr, pn, pkeep = _buf(prefix)
-            _check(lib.zk_compress_frames_prefix(self._h, addr, n, frame_size, level, int(checksum), paddr, pn, dst.ctypes.data, cap,
+            fn = lib.zk_compress_frames_ldm if long_distance else lib.zk_compress_frames_prefix
+            _check(fn(self._h, addr, n, frame_size, level, int(checksum), paddr, pn, dst.ctypes.data, cap,
                                                  cs.ctypes.data_as(_native.u32p), ds.ctypes.data_as(_native.u32p), nfmax, byref(nf), byref(dl)), lib)
         else:
             _check(lib.zk_compress_frames(self._h, addr, n, frame_size, level, int(checksum), dst.ctypes.data, cap,
@@ -146,9 +149,10 @@ class Context:
                                           byref(dl)), lib)
         return dst[: dl.value], cs[: nf.value].copy(), ds[: nf.value].copy()
 
-    def compress_frames_sized(self, data, frame_sizes, level: int = 0, checksum: bool = False, prefix=None):
+    def compress_frames_sized(self, data, frame_sizes, level: int = 0, checksum: bool = False, prefix=None, long_distance: bool = False):
         """frames of caller-chosen sizes in one batch: frame f covers the next frame_sizes[f] bytes of data (their sum is its length)
-        -> (compressed bytes (np.uint8), c_sizes, d_sizes).  Each frame is what compress_frames makes of its bytes alone."""
+        -> (compressed bytes (np.uint8), c_sizes, d_sizes).  Each frame is what compress_frames makes of its bytes alone
+        (long_distance as there)."""
         addr, n, keep = _buf(data)
         ds = np.ascontiguousarray(frame_sizes, dtype=np.uint32).reshape(-1)
         if int(np.sum(ds, dtype=np.uint64)) != n:
@@ -160,7 +164,8 @@ class Context:
         cs = np.zeros(ds.size, dtype=np.uint32)
         dl = c_size_t()
         paddr, pn, pkeep = _buf(prefix) if prefix is not None else (None, 0, None)
-        _check(lib.zk_compress_frames_sized(self._h, addr, dsp, ds.size, level, int(checksum), paddr, pn, dst.ctypes.data, cap,
+        fn = lib.zk_compress_frames_sized_ldm if long_distance else lib.zk_compress_frames_sized
+        _check(fn(self._h, addr, dsp, ds.size, level, int(checksum), paddr, pn, dst.ctypes.data, cap,
                                             cs.ctypes.data_as(_native.u32p), byref(dl)), lib)
         return dst[: dl.value], cs, ds.copy()
 
@@ -329,10 +334,16 @@ class EncodeOptions:
         self._policy = FrameSizePolicy.default()
         self._checksum = False
         self._level = 0
+        self._ldm = False
 
     def frame_size_policy(self, policy: FrameSizePolicy): self._policy = policy; return self
     def checksum_flag(self, flag: bool): self._checksum = bool(flag); return self
     def compression_level(self, level: int): self._level = int(level); return self
+
+    def long_distance_matching(self, flag: bool):
+        """match the frames of compress_with_prefix against the whole prefix (what the reference CLI sets on the CCtx it passes to
+        with_cctx for patch files).  Every level then runs as level 16; into_encoder refuses it with FrameSizePolicy.Compressed"""
+        self._ldm = bool(flag); return self
 
     def _native_opts(self):
         lib = self.ctx.lib
@@ -340,6 +351,7 @@ class EncodeOptions:
         lib.zk_encode_options_frame_size_policy(o, self._policy.kind, self._policy.size)
         lib.zk_encode_options_checksum_flag(o, int(self._checksum))
         lib.zk_encode_options_compression_level(o, self._level)
+        lib.zk_encode_options_long_distance_matching(o, int(self._ldm))
         return o
 
     def into_raw_encoder(self): return RawEncoder(self)
@@ -432,7 +444,12 @@ class Encoder(io.RawIOBase):
         self._wcb = _native.WRITE_FN(_write)
         self._fcb = _native.FLUSH_FN(_flush)
         h = c_void_p()
-        _check(self.lib.zk_encode_options_into_encoder(opts._native_opts(), self._wcb, self._fcb, None, byref(h)), self.lib)
+        self._h = None
+        o = opts._native_opts()
+        rc = self.lib.zk_encode_options_into_encoder(o, self._wcb, self._fcb, None, byref(h))
+        if rc:                                              # refused options are not consumed
+            self.lib.zk_encode_options_free(o)
+        _check(rc, self.lib)
         self._h = h
 
     def __del__(self):

@@ -1,6 +1,6 @@
 """Command-line front end with the reference CLI's arguments and behaviour (SURVEY.md 8f.4), over the GPU codec.
 
-    python -m zeekstd_b200 [compress] [-l N] [-s 2M] [--frame-size-policy ..] [--patch-from F] [INPUT] [-o OUT]
+    python -m zeekstd_b200 [compress] [-l N] [-s 2M] [--frame-size-policy ..] [--patch-from F [--long]] [INPUT] [-o OUT]
     python -m zeekstd_b200 decompress [--from N | --from-frame I] [--to N|end | --to-frame I|end] [--patch-apply F] INPUT [-o OUT]
     python -m zeekstd_b200 list [--from-frame I] [--to-frame I|end | --num-frames N] [-d] [--seek-table-format head|foot] INPUT
 
@@ -10,8 +10,11 @@ reader, optional stand-alone Head-format seek table) cli/src/compress.rs:55-106;
 cli/src/decompress.rs:21-117.  The codec underneath is this package's Encoder / Decoder, i.e. the CUDA path: there is no
 CPU route.  Compression levels are 1..19 as in the reference CLI (16..19 run the high-level tier: a 2 MiB window and a
 price-based parse), plus zstd's negative fast levels (`-l -5` or `--compression-level=-5`; acceleration = -level, clamped
-at -131072).  The window-log / long-distance-matching parameters
-the reference sets for patch files have no counterpart here (the kernels take the prefix as it is); `--mmap-prefix` / `--no-mmap-prefix` choose between np.memmap and a read.
+at -131072).  `--patch-from F` alone matches every frame against the last 32 KiB of F.  With `--long` (zstd's name for it) the
+window-log / long-distance-matching parameters the reference sets for patch files take effect: every frame is matched against
+the whole of F (its last 128 MiB when it is larger), which is what makes the archive a patch.  Long-distance matching is part
+of the high-level tier, so with `--long` every compression level writes what level 16 writes, and the frame size policy must be
+`uncompressed`.  `--mmap-prefix` / `--no-mmap-prefix` choose between np.memmap and a read.
 """
 from __future__ import annotations
 
@@ -140,6 +143,9 @@ def build_parser() -> argparse.ArgumentParser:
     c.add_argument("-s", "--frame-size", type=byte_value, default=byte_value("2M"))
     c.add_argument("--frame-size-policy", choices=["compressed", "uncompressed"], default="uncompressed")
     c.add_argument("--patch-from", default=None, help="Provide a reference point for Zstandard's diff engine.")
+    c.add_argument("--long", action="store_true",
+                   help="With --patch-from: long-distance matching against the whole reference file (its last 128 MiB), so that the archive "
+                        "is a patch. Every compression level then runs as level 16; needs --frame-size-policy uncompressed.")
     c.add_argument("input_file", nargs="?", default="-")
     c.add_argument("-o", "--output-file", default=None)
 
@@ -308,6 +314,10 @@ def _run_compress(zk, ns, fmt_bytes) -> int:
         reader = sys.stdin.buffer
     if ns.frame_size >= 1 << 32:
         raise CliError("Frame size too big")
+    if ns.long and not ns.patch_from:
+        raise CliError("--long needs --patch-from: long-distance matching runs against the reference file")
+    if ns.long and ns.frame_size_policy == "compressed":
+        raise CliError("--long needs --frame-size-policy uncompressed")
     prefix_len = os.path.getsize(ns.patch_from) if ns.patch_from and os.path.exists(ns.patch_from) else None
     st_file = None
     if ns.seek_table_file is not None:
@@ -321,7 +331,7 @@ def _run_compress(zk, ns, fmt_bytes) -> int:
 
     policy = (zk.FrameSizePolicy.Compressed if ns.frame_size_policy == "compressed" else zk.FrameSizePolicy.Uncompressed)(ns.frame_size)
     enc = (zk.EncodeOptions().frame_size_policy(policy).checksum_flag(not ns.no_checksum)
-           .compression_level(ns.compression_level).into_encoder(writer))
+           .compression_level(ns.compression_level).long_distance_matching(ns.long).into_encoder(writer))
     prefix = _load_prefix(ns.patch_from, _use_mmap(ns, prefix_len))
 
     read = 0

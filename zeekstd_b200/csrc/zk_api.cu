@@ -445,6 +445,7 @@ static int32_t zk_compress_host_run(zk_ctx* c, const ZkFrameList& fl, const uint
         tr.mark(s.stream, (int)k, 1);
         s.ews.no_side = zk_env_size("ZK_HOST_SIDE", 1) == 0;
         s.ews.prefix = c->cur_prefix_len ? c->d_prefix : nullptr; s.ews.prefix_len = c->cur_prefix_len;
+        s.ews.ldm = c->cur_ldm;
         rc = fl.enqueue(&s.ews, s.stream, s.d_in, f0, sb.cnt, sb.in_len, level, checksum, s.d_out, bound);
         if (rc) { err = rc; break; }
         tr.mark(s.stream, (int)k, 2);
@@ -559,6 +560,31 @@ extern "C" int32_t zk_compress_frames_sized(zk_ctx* c, const uint8_t* src, const
     const ZkFrameList fl = {frame_sizes, n, 0, n_frames};
     rc = zk_compress_host_run(c, fl, src, level, checksum, dst, dst_cap, c_sizes, dst_len);
     c->cur_prefix_len = 0;
+    return rc;
+}
+
+// ---------------------------------------------------------------------------------------------
+// long-distance matching (the reference CLI's patch mode: WindowLog + EnableLongDistanceMatching on the CCtx it hands to with_cctx,
+// cli/src/compress.rs:31-37): the prefix calls with K-C1h matching every frame against the whole prefix (zk_ldm.inc)
+// ---------------------------------------------------------------------------------------------
+extern "C" int32_t zk_compress_frames_ldm(zk_ctx* c, const uint8_t* src, size_t n, uint32_t frame_size, int32_t level, int32_t checksum,
+                                          const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap, uint32_t* c_sizes,
+                                          uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len) {
+    if (!c) return ZK_ERR_INVALID_ARG;
+    c->cur_ldm = true;
+    const int32_t rc = zk_compress_frames_prefix(c, src, n, frame_size, level, checksum, prefix, prefix_len, dst, dst_cap, c_sizes, d_sizes, frames_cap,
+                                                 n_frames, dst_len);
+    c->cur_ldm = false;
+    return rc;
+}
+
+extern "C" int32_t zk_compress_frames_sized_ldm(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                                int32_t checksum, const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap,
+                                                uint32_t* c_sizes, size_t* dst_len) {
+    if (!c) return ZK_ERR_INVALID_ARG;
+    c->cur_ldm = true;
+    const int32_t rc = zk_compress_frames_sized(c, src, frame_sizes, n_frames, level, checksum, prefix, prefix_len, dst, dst_cap, c_sizes, dst_len);
+    c->cur_ldm = false;
     return rc;
 }
 

@@ -1231,12 +1231,15 @@ __global__ void __launch_bounds__(1024) zk_frame_scan_kernel(ZkEncodeArgs a) {
 
 // tiers above level 12 only: the frame headers written by zk_frame_gather_kernel announce a 128 KiB window.  This rewrites the
 // Window_Descriptor to the smallest one >= max(wmin, min(frame content + prefix tail, wmax)): the wide tier's offsets reach
-// (ZKC_WIDE_HIST + 1) blocks back (wmin = wmax = 256 KiB), the high-level tier's ZKC_HC_WINDOW bytes within the frame and its prefix tail
-__global__ void __launch_bounds__(128) zk_frame_window_kernel(ZkEncodeArgs a, uint32_t n_frames, uint32_t wmin, uint32_t wmax) {
+// (ZKC_WIDE_HIST + 1) blocks back (wmin = wmax = 256 KiB), the high-level tier's ZKC_HC_WINDOW bytes within the frame and its prefix tail.
+// hist: the bytes of the prefix a frame can reach: its tail, or with long-distance matching all of it (wmax = 2^27 then, the largest
+// window a default libzstd decoder and this one accept; zkc_ldm_window keeps every offset within it)
+__global__ void __launch_bounds__(128) zk_frame_window_kernel(ZkEncodeArgs a, uint32_t n_frames, uint32_t wmin, uint32_t wmax, uint32_t hist) {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= n_frames || *a.error) return;
     const size_t fcs = a.frames[f].size;
-    size_t want = fcs + a.ptail < wmax ? fcs + a.ptail : wmax;
+    const size_t reach = fcs ? hist : 0;                      // an empty frame holds no match: the minimum, whatever the prefix
+    size_t want = fcs + reach < wmax ? fcs + reach : wmax;
     if (want < wmin) want = wmin;
     uint32_t e = 0, m = 0;                                    // Window_Size = 2^(10 + e) * (1 + m / 8)
     while (((size_t)8 + m) << (7 + e) < want) { if (++m == 8) { m = 0; e++; } }
@@ -1512,7 +1515,8 @@ static size_t zkc_align(size_t v) { return (v + 255) & ~(size_t)255; }
 // the level a caller asks for -> the one the kernels run: 0 is the default (3), levels below ZSTD_minCLevel() clamp to it
 static int zkc_level(int level) { return level == 0 ? 3 : (level < ZKC_MIN_LEVEL ? ZKC_MIN_LEVEL : level); }
 struct ZkcHcPass;
-static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, const ZkEncodeArgs& a, const std::vector<ZkcHcPass>* hc_plan);
+struct ZkcHcRun;
+static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, const ZkEncodeArgs& a, const ZkcHcRun* hc);
 
 // the frame and block tables of a batch, on `stream`: h_sizes == nullptr: the uniform layout of (n, frame_size), generated on the device;
 // otherwise the caller's sizes, uploaded to d_sizes and scanned there
@@ -1547,10 +1551,14 @@ static int zkc_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src
         n_blocks = (size_t)(n_frames - 1) * zkc_frame_blocks(frame_size) + zkc_frame_blocks(n - (size_t)(n_frames - 1) * frame_size);
     }
     if (n_blocks > 0x7FFFFFFFull) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
-    const int lvl = zkc_level(level);
     const uint32_t pt = d_prefix && prefix_len && n ? (prefix_len < ZKC_BLOCK ? prefix_len : ZKC_BLOCK) : 0u;
-    std::vector<ZkcHcPass> hc_plan;
-    const uint32_t hc_span = lvl >= ZKC_HC_LEVEL ? zkc_hc_plan(n, frame_size, h_sizes, n_frames, (uint32_t)n_blocks, pt, hc_plan) : 0u;
+    // long-distance matching is a part of K-C1h: with it every level runs that tier
+    const bool ldm = ws->ldm && pt;
+    ws->ldm = false;
+    const int lvl = ldm ? ZKC_HC_LEVEL : zkc_level(level);
+    ZkcHcRun hc;
+    const uint32_t hc_span = lvl >= ZKC_HC_LEVEL ? zkc_hc_plan(n, frame_size, h_sizes, n_frames, (uint32_t)n_blocks, pt, hc.plan) : 0u;
+    if (ldm) hc.reach = prefix_len < ZKC_LDM_REACH ? prefix_len : ZKC_LDM_REACH;
     // carve the workspace
     size_t off = 0;
     const size_t o_geo = off; off = zkc_align(off + n_blocks * sizeof(ZkcGeo));
@@ -1570,6 +1578,8 @@ static int zkc_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src
     const size_t o_pst = off; if (pt) off = zkc_align(off + (size_t)n_frames * ZKC_PSLOT);
     const size_t o_hc = off;
     if (lvl >= ZKC_HC_LEVEL) off = zkc_align(off + zkc_hc_layout(hc_span, nullptr, nullptr));
+    const size_t o_ldm = off;
+    if (ldm) off = zkc_align(off + zkc_ldm_layout(hc.reach, n_blocks, nullptr, nullptr, nullptr));
     if (ws->cap < off) {
         if (ws->buf) cudaFree(ws->buf);
         ws->buf = nullptr; ws->cap = 0;
@@ -1597,6 +1607,7 @@ static int zkc_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src
     a.prefix = d_prefix; a.prefix_len = 0; a.ptail = 0; a.pstage = base + o_pst;
     a.hist_cap = ~(size_t)0;
     a.hc = base + o_hc;
+    if (ldm) hc.ldm = base + o_ldm;
     int rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo), (ZkcFrame*)(base + o_fr), n_frames, (uint32_t)n_blocks, n, frame_size,
                                 h_sizes, (uint32_t*)(base + o_fsz));
     if (rc) return rc;
@@ -1622,15 +1633,16 @@ static int zkc_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src
         ZKC_CUDA_OK(cudaEventRecord(ws->ev_c, stream)); ZKC_CUDA_OK(cudaStreamWaitEvent(ss, ws->ev_c, 0));     // after whatever produced the input
         ZK_LAUNCH(zk_frame_hash_kernel, (n_frames + 3) / 4, 128, 0, ss, a);
     }
-    rc = zkc_run_blocks(ws, stream, ss, a, &hc_plan);
+    rc = zkc_run_blocks(ws, stream, ss, a, &hc);
     if (rc) return rc;
     ws->prof.begin(7, stream);
     if (checksum && ss == stream) ZK_LAUNCH(zk_frame_hash_kernel, (n_frames + 3) / 4, 128, 0, stream, a);   // else: already done on the side stream (joined by ev_b)
     ZK_LAUNCH(zk_frame_size_kernel, (n_frames + 255) / 256, 256, 0, stream, a);
     ZK_LAUNCH(zk_frame_scan_kernel, 1, 1024, 0, stream, a);
     ZK_LAUNCH(zk_frame_gather_kernel, (uint32_t)((n_blocks + 3) / 4), 128, 0, stream, a);
-    if (a.level >= ZKC_HC_LEVEL) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 128u << 10, ZKC_HC_WINDOW); ws->launches++; }
-    else if (a.level >= ZKC_WIDE_LEVEL) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 256u << 10, 256u << 10); ws->launches++; }
+    if (ldm) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 128u << 10, 1u << 27, prefix_len); ws->launches++; }
+    else if (a.level >= ZKC_HC_LEVEL) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 128u << 10, ZKC_HC_WINDOW, pt); ws->launches++; }
+    else if (a.level >= ZKC_WIDE_LEVEL) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 256u << 10, 256u << 10, pt); ws->launches++; }
     ws->prof.end(7, stream);
     ZKC_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, a.frame_csize, (size_t)n_frames * 4, cudaMemcpyDeviceToHost, stream));
     ZKC_CUDA_OK(cudaMemcpyAsync(ws->h_sizes + ws->cap_frames, a.total, 16, cudaMemcpyDeviceToHost, stream));
@@ -1652,8 +1664,8 @@ int zk_encode_enqueue_sized(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* 
 }
 
 // K-C1 and K-C2 over every block of `a` (match finding, then sequences on `ss` beside literals on `stream`, joined by the finish kernel);
-// hc_plan: the internal passes of the high-level tier (zkc_hc_plan)
-static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, const ZkEncodeArgs& a, const std::vector<ZkcHcPass>* hc_plan) {
+// hc: what the high-level tier needs beside `a` (its levels only)
+static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, const ZkEncodeArgs& a, const ZkcHcRun* hc) {
     const size_t n_blocks = a.n_blocks;
     ws->prof.begin(5, stream);
     // six tiers (EncodeOptions::compression_level, encode.rs:176): 1 = 2048-entry table, no history, no lazy step; 2-3 = 4096 entries,
@@ -1662,7 +1674,7 @@ static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, 
     // entries in dynamic shared memory.  Ratio on the reference's corpus: 2.12 / 2.24 / 2.28 / 2.38 / 2.40 / 2.50.  Below them the fast tier
     // (level < 0): level 1's table with sparse probing, literals without Huffman coding.  From ZKC_HC_LEVEL on, K-C1h (zk_hc.inc): hash chains
     // over 2 MiB of the frame and a price-based parse
-    if (a.level >= ZKC_HC_LEVEL) { const int rc = zkc_run_hc(ws, stream, a, *hc_plan); if (rc) return rc; }
+    if (a.level >= ZKC_HC_LEVEL) { const int rc = zkc_run_hc(ws, stream, a, *hc); if (rc) return rc; }
     else if (a.level < 0) ZK_LAUNCH((zk_match_fast_kernel<ZKC_HLOG_FAST, ZKC_C1_WARPS>), (uint32_t)((n_blocks + ZKC_C1_WARPS - 1) / ZKC_C1_WARPS), ZKC_C1_WARPS * 32, 0, stream, a);
     else if (a.level <= 1) ZK_LAUNCH((zk_match_kernel<ZKC_HLOG_FAST, ZKC_C1_WARPS, false>), (uint32_t)((n_blocks + ZKC_C1_WARPS - 1) / ZKC_C1_WARPS), ZKC_C1_WARPS * 32, 0, stream, a);
     else if (a.level <= 3) ZK_LAUNCH((zk_match_kernel<ZKC_HLOG, ZKC_C1_WARPS, false>), (uint32_t)((n_blocks + ZKC_C1_WARPS - 1) / ZKC_C1_WARPS), ZKC_C1_WARPS * 32, 0, stream, a);

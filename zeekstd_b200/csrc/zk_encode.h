@@ -10,6 +10,7 @@ struct ZkEncodeWs {                    // HBM scratch owned by a zk_ctx slot, gr
     uint32_t pending_frames = 0;
     bool attr_set = false, attr_set_wide = false, attr_set_walk = false, attr_set_hc = false;
     const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device pointer: raw-content prefix for the NEXT enqueue (one-shot)
+    bool ldm = false;                 // long-distance matching against that prefix for the NEXT enqueue (one-shot; nothing without a prefix)
     int prio = 0;                     // CUDA stream priority of the side stream (matches the slot's stream)
     bool no_side = false;             // host pipelines: concurrency comes from the other sub-batches; every extra stream costs a hardware queue
     cudaStream_t side = nullptr; cudaEvent_t ev_a = nullptr, ev_b = nullptr, ev_c = nullptr;   // K-C2s runs beside K-C2l
