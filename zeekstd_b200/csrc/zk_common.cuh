@@ -141,6 +141,7 @@ struct ZkCounters {
     uint32_t n_huf_blocks, n_seq_blocks;         // lengths of huf_list / seq_list
     uint32_t n_long, n_short;                    // execution segments of the batch (plan kernel): seg_list[0, n_long) run on CTAs,
                                                  // seg_list[cap_blocks - n_short, cap_blocks) on one warp each
+    uint32_t n_seq_full;                         // blocks zk_seq2_kernel passed to zk_seq2_full_kernel: seq_list[cap_blocks, + n_seq_full)
 };
 
 // -------------------------------------------------------------------------------------------

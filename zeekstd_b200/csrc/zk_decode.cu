@@ -6,7 +6,8 @@
 // seekable format, seekable_format.md:23-29):
 //
 //   K-D0 zk_scan_kernel        one thread / entry   : walk frame + block headers, carve scratch
-//   K-D1s zk_seq2_kernel       one chain / block    : FSE sequence decode (4 chains per warp, TMA-staged bitstreams)
+//   K-D1s zk_seq2_kernel       one chain / block    : FSE sequence decode (4 chains per warp, TMA-staged bitstreams);
+//         zk_seq2_full_kernel                       the same for blocks whose tables need more cells than zk_seq2_kernel holds
 //   K-D1h zk_huf_kernel        one LANE  / stream   : Huffman literal decode (4 lanes per 4-stream block, two-level table)
 //   K-D1p zk_plan_kernel       one warp / entry     : output positions, the serial walk's checks, execution segments
 //   K-D2w zk_exec_warp_kernel  one warp / segment   : short segments, strictly in order through a per-warp window
@@ -258,13 +259,18 @@ __global__ void __launch_bounds__(128) zk_scan_kernel(ZkDecodeArgs a) {
 #define ZK_CELL_ADD(c) (((c) >> 13) & 31u)
 #define ZK_CELL_CODE(c) (((c) >> 18) & 63u)
 
-struct ZkSeqSlot {
-    uint32_t ll[512], ml[512], of[256];        // 5 KiB
+struct ZkSeqSlot {                            // what a block's three table descriptions parse to, and the build scratch
     int16_t cnt[3][64];
     uint16_t nxt[64];
     int tbl_log[3], tbl_nsym[3], tbl_mode[3];  // mode: 0 = counts in cnt[t], 1 = RLE (cnt[t][0] = symbol)
 };
 struct ZkSeqTabs { uint32_t ll_base[36], ml_base[53]; };
+
+// A block's LL, OF and ML cells lie back to back in one array, each table as large as its log asks for.  The format allows
+// up to 512 + 256 + 512 cells; this codec's encoder never writes a table above log 8, so its blocks need at most 768.
+#define ZK_SEQ_CELLS_FULL 1280u
+#define ZK_SEQ_CELLS_COMPACT 768u
+__device__ __forceinline__ uint32_t zk_seq_cells(const ZkSeqSlot& sl, int t) { return sl.tbl_mode[t] == 1 ? 1u : 1u << sl.tbl_log[t]; }
 
 // Locate the three table descriptions of a block (A.5) and parse those that are wanted into sl.cnt[t]
 // (t: 0 LL, 1 OF, 2 ML).  Returns 0 or a zstd code.  *bits_off = start of the sequence bitstream.
@@ -310,10 +316,9 @@ __device__ int zk_locate_seq_tables(ZkSeqSlot& sl, const uint8_t* b, uint32_t bs
     return 0;
 }
 
-// Build one sequence decoding table from sl.cnt[t] (A.6).  The symbol spread is written into the cell array itself and
-// converted to cells in place.
-__device__ int zk_build_seq_table(ZkSeqSlot& sl, int t, uint16_t* nxt_scratch = nullptr) {
-    uint32_t* cell = t == 0 ? sl.ll : (t == 1 ? sl.of : sl.ml);
+// Build one sequence decoding table from sl.cnt[t] (A.6) into cell[0, zk_seq_cells(sl, t)).  The symbol spread is written
+// into the cell array itself and converted to cells in place.
+__device__ int zk_build_seq_table(ZkSeqSlot& sl, int t, uint32_t* cell, uint16_t* nxt_scratch = nullptr) {
     if (sl.tbl_mode[t] == 1) {
         const uint32_t sy = (uint32_t)sl.cnt[t][0];
         const uint32_t add = t == 0 ? ZK_LL_BITS[sy] : (t == 1 ? sy : ZK_ML_BITS[sy]);
@@ -350,7 +355,7 @@ __device__ int zk_build_seq_table(ZkSeqSlot& sl, int t, uint16_t* nxt_scratch = 
 // states' cells.  The first kernel ran the whole per-sequence work (~110 dependent instructions: extra-bit reads, value
 // arithmetic, repeat-offset history, three stores, refills from global memory) on that chain -- about 1 000 cycles per
 // sequence.  Here
-//   * the bitstream is staged in shared memory by TMA bulk copies (cp.async.bulk + mbarrier, four 512-byte tiles per
+//   * the bitstream is staged in shared memory by TMA bulk copies (cp.async.bulk + mbarrier, four 256-byte tiles per
 //     chain, refilled ahead of the cursor), so a bit field anywhere near the cursor is two shared-memory loads and a
 //     funnel shift -- no bit buffer, no refill branches, no global latency on the chain;
 //   * a CHAIN LANE only walks the states: three cell loads, the sum of the extra-bit counts, one 32-bit window for the
@@ -359,13 +364,21 @@ __device__ int zk_build_seq_table(ZkSeqSlot& sl, int t, uint16_t* nxt_scratch = 
 //     the cumulative ends, bounds checks, coalesced stores; the repeat-offset history -- a serial state machine -- is run
 //     warp-uniformly over the FEW sequences that use a repeat code (explicit offsets just shift it).
 // Four chains per warp (lanes 0, 8, 16, 24) share every issued instruction of the chain phase.
+//
+// Shared memory per chain decides how many chains an SM holds beside K-D1h, so the kernel comes in two layouts of the
+// cell array: zk_seq2_kernel (768 cells, every block of this codec's encoder) and zk_seq2_full_kernel (1280, the format's
+// largest tables).  The first kernel passes a block whose parsed tables need more cells than it has to the second, which
+// runs after it on the same stream.
 // =============================================================================================
 #define ZK_S2_NCH 4
-#define ZK_S2_TILE 512u
-#define ZK_S2_RING_BYTES 2048u            // four tiles: the cursor's tile, the two below it, one being refilled
+#define ZK_S2_TILE 256u
+#define ZK_S2_RING_BYTES 1024u            // four tiles: the cursor's tile, the two below it (>= 512 bytes below the cursor,
+                                          // more than a phase's 356), one being refilled
+template <uint32_t NCELLS>
 struct ZkSeq2Chain {
-    ZkSeqSlot t;                           // thin cells + build scratch (zk_locate_seq_tables / zk_build_seq_table)
-    alignas(128) uint32_t ring[ZK_S2_RING_BYTES / 4];   // staged bitstream (bulk copies want 16-byte aligned shared addresses): byte at offset o from gbase lives at ring byte o & 2047
+    uint32_t cells[NCELLS];                // thin cells: LL, OF, ML back to back (zk_seq_cells)
+    ZkSeqSlot t;                           // build scratch (zk_locate_seq_tables / zk_build_seq_table)
+    alignas(128) uint32_t ring[ZK_S2_RING_BYTES / 4];   // staged bitstream (bulk copies want 16-byte aligned shared addresses): byte at offset o from gbase lives at ring byte o & 1023
     uint4 rec[32];                         // per step: {LL cell, OF cell, ML cell, bit cursor before the extra bits}
     uint16_t nxt2[2][64];                  // build scratch of the OF / ML tables (LL uses t.nxt): the three tables are built side by side
     alignas(8) unsigned long long bar[4];  // one mbarrier per tile slot
@@ -383,10 +396,12 @@ __device__ __forceinline__ uint32_t zk_s2_bits(const uint32_t* ring, uint32_t cu
     return __funnelshift_l(zk_s2_window(ring, cur), 0u, n);
 }
 
-__global__ void __launch_bounds__(32) zk_seq2_kernel(ZkDecodeArgs a) {
+template <uint32_t NCELLS>
+__device__ __forceinline__ void zk_seq2_body(const ZkDecodeArgs& a) {
+    constexpr bool full = NCELLS == ZK_SEQ_CELLS_FULL;                 // decodes the blocks the compact layout passed on
     ZK_DYN_SMEM(smem);
     ZkSeqTabs* tb = (ZkSeqTabs*)smem;
-    ZkSeq2Chain* chains = (ZkSeq2Chain*)(smem + ((sizeof(ZkSeqTabs) + 127) & ~(size_t)127));
+    ZkSeq2Chain<NCELLS>* chains = (ZkSeq2Chain<NCELLS>*)(smem + ((sizeof(ZkSeqTabs) + 127) & ~(size_t)127));
     const int lane = threadIdx.x & 31;
     const int myc = lane >> 3;                                     // the chain this lane belongs to ...
     const bool chain_lane = (lane & 7) == 0;                       // ... and whether it walks it
@@ -398,17 +413,18 @@ __global__ void __launch_bounds__(32) zk_seq2_kernel(ZkDecodeArgs a) {
 #endif
     __syncwarp();
     if (a.counters->overflow) return;
-    const uint32_t n = a.counters->n_seq_blocks;
+    const uint32_t n = full ? a.counters->n_seq_full : a.counters->n_seq_blocks;
+    const uint32_t* list = full ? a.seq_list + a.cap_blocks : a.seq_list;
     uint32_t tile_uses = 0;                                        // tiles this chain lane has issued so far (slot = use & 3, parity = (use >> 2) & 1)
     for (;;) {
         uint32_t g = 0;
-        if (lane == 0) g = atomicAdd(&a.work_counter[0], 1u);
+        if (lane == 0) g = atomicAdd(&a.work_counter[full ? 4 : 0], 1u);
         g = __shfl_sync(0xFFFFFFFFu, g, 0);
         const uint32_t first = g * ZK_S2_NCH;
         if (first >= n) break;
-        ZkSeq2Chain& ch = chains[myc];
+        ZkSeq2Chain<NCELLS>& ch = chains[myc];
         // ---------------- per chain: tables, stream geometry, first tiles, initial states (chain lanes, side by side)
-        uint32_t bidx = 0, remaining = 0, done = 0, cur = 0, sb_bit = 0, s_l = 0, s_o = 0, s_m = 0, seq_base = 0, lit_size = 0;
+        uint32_t bidx = 0, remaining = 0, done = 0, cur = 0, sb_bit = 0, s_l = 0, s_o = 0, s_m = 0, seq_base = 0, lit_size = 0, o_of = 0, o_ml = 0;
         const uint8_t* gbase = nullptr;
         int next_issue = -1, next_wait = -1, top_tile = 0; uint32_t stream_end_off = 0, use0 = 0;
         bool live = false, parsed = false;
@@ -416,7 +432,7 @@ __global__ void __launch_bounds__(32) zk_seq2_kernel(ZkDecodeArgs a) {
             ch.st = 0; ch.lit_end = 0; ch.out_end = 0; ch.back = 0; ch.r0 = ZK_SYM_MAKE(0, 0); ch.r1 = ZK_SYM_MAKE(1, 0); ch.r2 = ZK_SYM_MAKE(2, 0);
             const uint32_t my = first + (uint32_t)myc;
             if (my < n) {
-                bidx = a.seq_list[my];
+                bidx = list[my];
                 ZkBlock blk; blk.entry = 0xFFFFFFFFu;
                 if (bidx < a.cap_blocks) blk = a.blocks[bidx];
                 if (blk.entry < a.n_entries && a.entries[blk.entry].status == 0) {
@@ -428,21 +444,27 @@ __global__ void __launch_bounds__(32) zk_seq2_kernel(ZkDecodeArgs a) {
                     if (!st && blk.ll_ref >= 0) { const ZkBlock& rb = a.blocks[blk.ll_ref]; uint32_t d; st = zk_locate_seq_tables(ch.t, ebase + rb.src, rb.size, true, false, false, &d); }
                     if (!st && blk.of_ref >= 0) { const ZkBlock& rb = a.blocks[blk.of_ref]; uint32_t d; st = zk_locate_seq_tables(ch.t, ebase + rb.src, rb.size, false, true, false, &d); }
                     if (!st && blk.ml_ref >= 0) { const ZkBlock& rb = a.blocks[blk.ml_ref]; uint32_t d; st = zk_locate_seq_tables(ch.t, ebase + rb.src, rb.size, false, false, true, &d); }
-                    ch.st = st; parsed = !st;
-                    const uint8_t* sp = b + bits_off; const uint32_t sn = blk.size - bits_off;
-                    if (!st && (sn == 0 || sp[sn - 1] == 0)) st = ZKZ_CORRUPTION;
-                    if (!st) {
-                        gbase = (const uint8_t*)((uintptr_t)sp & ~(uintptr_t)15);
-                        sb_bit = (uint32_t)(sp - gbase) * 8u;
-                        stream_end_off = (uint32_t)(sp - gbase) + sn;                       // byte offset of the end of the stream from gbase
-                        cur = sb_bit + (sn - 1) * 8u + (uint32_t)zk_highbit(sp[sn - 1]);     // the end mark itself is not data
-                        // tiles are staged from the CURSOR's tile downwards: when the end mark is the first byte of a tile, that tile holds
-                        // no data (the mark was read above), and counting it would put five tiles in flight on four slots
-                        top_tile = (int)(((cur ? cur - 1u : 0u) >> 3) / ZK_S2_TILE);
-                        next_issue = top_tile; next_wait = top_tile; use0 = tile_uses;
-                        remaining = blk.nseq; seq_base = blk.seq_base; lit_size = blk.lit_size;
+                    if (!st) { o_of = zk_seq_cells(ch.t, 0); o_ml = o_of + zk_seq_cells(ch.t, 1); }
+                    if (!full && !st && o_ml + zk_seq_cells(ch.t, 2) > NCELLS) {
+                        a.seq_list[a.cap_blocks + atomicAdd(&a.counters->n_seq_full, 1u)] = bidx;          // tables too large for these cells: the
+                        live = false;                                                        // full layout decodes the block
+                    } else {
+                        ch.st = st; parsed = !st;
+                        const uint8_t* sp = b + bits_off; const uint32_t sn = blk.size - bits_off;
+                        if (!st && (sn == 0 || sp[sn - 1] == 0)) st = ZKZ_CORRUPTION;
+                        if (!st) {
+                            gbase = (const uint8_t*)((uintptr_t)sp & ~(uintptr_t)15);
+                            sb_bit = (uint32_t)(sp - gbase) * 8u;
+                            stream_end_off = (uint32_t)(sp - gbase) + sn;                       // byte offset of the end of the stream from gbase
+                            cur = sb_bit + (sn - 1) * 8u + (uint32_t)zk_highbit(sp[sn - 1]);     // the end mark itself is not data
+                            // tiles are staged from the CURSOR's tile downwards: when the end mark is the first byte of a tile, that tile holds
+                            // no data (the mark was read above), and counting it would put five tiles in flight on four slots
+                            top_tile = (int)(((cur ? cur - 1u : 0u) >> 3) / ZK_S2_TILE);
+                            next_issue = top_tile; next_wait = top_tile; use0 = tile_uses;
+                            remaining = blk.nseq; seq_base = blk.seq_base; lit_size = blk.lit_size;
+                        }
+                        ch.st = st;
                     }
-                    ch.st = st;
                 }
             }
         }
@@ -452,7 +474,10 @@ __global__ void __launch_bounds__(32) zk_seq2_kernel(ZkDecodeArgs a) {
             const bool go = __shfl_sync(0xFFFFFFFFu, (uint32_t)(parsed && ch.st == 0), myc * 8) != 0;
             const int t = lane & 7;
             int bst = 0;
-            if (go && t < 3) bst = zk_build_seq_table(ch.t, t, t == 0 ? nullptr : ch.nxt2[t - 1]);
+            if (go && t < 3) {
+                const uint32_t off = t == 0 ? 0u : (t == 1 ? zk_seq_cells(ch.t, 0) : zk_seq_cells(ch.t, 0) + zk_seq_cells(ch.t, 1));
+                bst = zk_build_seq_table(ch.t, t, ch.cells + off, t == 0 ? nullptr : ch.nxt2[t - 1]);
+            }
             const uint32_t failed = __ballot_sync(0xFFFFFFFFu, bst != 0);
             if (chain_lane && ((failed >> (myc * 8)) & 7u) && ch.st == 0) ch.st = ZKZ_CORRUPTION;
         }
@@ -491,8 +516,9 @@ __global__ void __launch_bounds__(32) zk_seq2_kernel(ZkDecodeArgs a) {
                     cnt = remaining < 32u ? remaining : 32u;
                     const bool last_tile = cnt == remaining;
                     bool over = false;
+                    const uint32_t* cof = ch.cells + o_of; const uint32_t* cml = ch.cells + o_ml;
                     for (uint32_t k = 0; k < cnt; k++) {
-                        const uint32_t cl = ch.t.ll[s_l], co = ch.t.of[s_o], cm = ch.t.ml[s_m];
+                        const uint32_t cl = ch.cells[s_l], co = cof[s_o], cm = cml[s_m];
                         ch.rec[k] = make_uint4(cl, co, cm, cur);
                         const uint32_t eb = ZK_CELL_CODE(co) + ZK_CELL_ADD(cm) + ZK_CELL_ADD(cl);
                         const uint32_t nl = ZK_CELL_NB(cl), nm = ZK_CELL_NB(cm), no = ZK_CELL_NB(co);
@@ -521,7 +547,7 @@ __global__ void __launch_bounds__(32) zk_seq2_kernel(ZkDecodeArgs a) {
                 const uint32_t ncc = __shfl_sync(0xFFFFFFFFu, cnt, cc * 8);
                 if (ncc == 0) continue;
                 any = 1;
-                ZkSeq2Chain& hc = chains[cc];
+                ZkSeq2Chain<NCELLS>& hc = chains[cc];
                 const uint32_t sbase = __shfl_sync(0xFFFFFFFFu, seq_base, cc * 8), sdone = __shfl_sync(0xFFFFFFFFu, done, cc * 8);
                 const uint32_t lsz = __shfl_sync(0xFFFFFFFFu, lit_size, cc * 8);
                 const bool act = (uint32_t)lane < ncc;
@@ -604,6 +630,10 @@ __global__ void __launch_bounds__(32) zk_seq2_kernel(ZkDecodeArgs a) {
         __syncwarp();
     }
 }
+static_assert(ZK_SEQ_CELLS_FULL == 512 + 256 + 512, "the full layout holds the largest tables the format allows (LL, ML log 9; OF log 8)");
+
+__global__ void __launch_bounds__(32) zk_seq2_kernel(ZkDecodeArgs a) { zk_seq2_body<ZK_SEQ_CELLS_COMPACT>(a); }
+__global__ void __launch_bounds__(32) zk_seq2_full_kernel(ZkDecodeArgs a) { zk_seq2_body<ZK_SEQ_CELLS_FULL>(a); }
 
 // =============================================================================================
 // K-D1h: Huffman literal decode -- one LANE per Huffman stream (4 lanes per 4-stream block).
@@ -1857,6 +1887,8 @@ __global__ void __launch_bounds__(128) zk_xxh64_kernel(ZkDecodeArgs a) {
 #define ZK_CUDA_OK(x) do { (void)(x); } while (0)
 #endif
 
+#define ZK_WORK_COUNTERS 5
+
 static int zk_grow(void** p, size_t* cap, size_t need, size_t elem) {
     if (*cap >= need && *p) return 0;
     if (*p) cudaFree(*p);
@@ -1893,7 +1925,8 @@ static int zk_decode_ensure(ZkDecodeWs* ws, uint32_t n, size_t need_blocks, size
         size_t c1 = ws->cap_blocks, c2 = ws->cap_blocks, c3 = ws->cap_blocks, c4 = ws->cap_blocks;
         if ((rc = zk_grow((void**)&ws->blocks, &c1, need_blocks, sizeof(ZkBlock)))) return rc;
         if ((rc = zk_grow((void**)&ws->huf_list, &c2, need_blocks, 4))) return rc;
-        if ((rc = zk_grow((void**)&ws->seq_list, &c3, need_blocks, 4))) return rc;
+        if ((rc = zk_grow((void**)&ws->seq_list, &c3, 2 * need_blocks, 4))) return rc;   // two lists (ZkDecodeArgs::seq_list)
+        c3 /= 2;
         if ((rc = zk_grow((void**)&ws->seg_list, &c4, need_blocks, 4))) return rc;
         ws->cap_blocks = c1 < c2 ? (c1 < c3 ? c1 : c3) : (c2 < c3 ? c2 : c3);
         if (c4 < ws->cap_blocks) ws->cap_blocks = c4;
@@ -1925,8 +1958,8 @@ static int zk_decode_ensure(ZkDecodeWs* ws, uint32_t n, size_t need_blocks, size
         ws->cap_entries = c;
     }
     if (!ws->counters) {
-        if (cudaMalloc((void**)&ws->counters, sizeof(ZkCounters) + 16) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
-        if (cudaMallocHost((void**)&ws->h_counters, sizeof(ZkCounters) + 16) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
+        if (cudaMalloc((void**)&ws->counters, sizeof(ZkCounters) + ZK_WORK_COUNTERS * 4) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
+        if (cudaMallocHost((void**)&ws->h_counters, sizeof(ZkCounters) + ZK_WORK_COUNTERS * 4) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
     }
     return 0;
 }
@@ -1959,11 +1992,11 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     }
     ZK_CUDA_OK(cudaMemcpyAsync(ws->c_off, ws->h_off, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, us));
     ZK_CUDA_OK(cudaMemcpyAsync(ws->d_off, ws->h_off + (n + 1), (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, us));
-    ZK_CUDA_OK(cudaMemsetAsync(ws->counters, 0, sizeof(ZkCounters) + 16, stream));
+    ZK_CUDA_OK(cudaMemsetAsync(ws->counters, 0, sizeof(ZkCounters) + ZK_WORK_COUNTERS * 4, stream));
     ZkDecodeArgs a;
     a.comp = d_comp; a.c_off = (const unsigned long long*)ws->c_off; a.d_off = (const unsigned long long*)ws->d_off; a.dst = d_dst; a.n_entries = n;
     a.blocks = ws->blocks; a.entries = ws->entries; a.counters = ws->counters;
-    a.work_counter = (uint32_t*)((uint8_t*)ws->counters + sizeof(ZkCounters));   // four counters (seq, huf, exec, single-warp exec), zeroed with the struct
+    a.work_counter = (uint32_t*)((uint8_t*)ws->counters + sizeof(ZkCounters));   // seq, huf, exec, single-warp exec, full-layout seq; zeroed with the struct
     a.lit = ws->lit; a.seq_lit_end = ws->seq_lit_end; a.seq_out_end = ws->seq_out_end; a.seq_off = ws->seq_off;
     a.huf_list = ws->huf_list; a.seq_list = ws->seq_list; a.seg_list = ws->seg_list;
     a.cap_blocks = ws->cap_blocks; a.cap_lit = ws->cap_lit - 64; a.cap_seq = ws->cap_seq;
@@ -1981,9 +2014,11 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     // entropy stage: persistent warp-CTAs pulling groups of blocks from a work counter
     size_t est_blocks = (size_t)(total_d / ZK_BLOCK_MAX) + n;
     const size_t huf_smem = sizeof(ZkHufTab) * ZK_HUF_SLOTS + sizeof(ZkHufScratch);
-    const size_t seq2_smem = ((sizeof(ZkSeqTabs) + 127) & ~(size_t)127) + sizeof(ZkSeq2Chain) * ZK_S2_NCH;
+    const size_t seq2_smem = ((sizeof(ZkSeqTabs) + 127) & ~(size_t)127) + sizeof(ZkSeq2Chain<ZK_SEQ_CELLS_COMPACT>) * ZK_S2_NCH;
+    const size_t seq2f_smem = ((sizeof(ZkSeqTabs) + 127) & ~(size_t)127) + sizeof(ZkSeq2Chain<ZK_SEQ_CELLS_FULL>) * ZK_S2_NCH;
     if (!ws->attr_set) {
         ZK_CUDA_OK(cudaFuncSetAttribute(zk_seq2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)seq2_smem));
+        ZK_CUDA_OK(cudaFuncSetAttribute(zk_seq2_full_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)seq2f_smem));
         ZK_CUDA_OK(cudaFuncSetAttribute(zk_huf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)huf_smem + 65536));
         ZK_CUDA_OK(cudaFuncSetAttribute(zk_exec_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
         ZK_CUDA_OK(cudaFuncSetAttribute(zk_exec_kernel_w5<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
@@ -2000,9 +2035,23 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
         ws->huf_fit = 16;                        // (no SM to fill)
 #endif
     }
-    // Half of them: K-D1s runs beside K-D1h, and the two only overlap when both fit on the SM (DESIGN §6).  Two K-D1h CTAs are
-    // resident beside K-D1s's five, the rest start as K-D1s's CTAs finish.
+    // Half of them: K-D1s runs beside K-D1h, and the two only overlap when both fit on the SM (DESIGN §6).  K-D1s gets the CTAs
+    // that fit in three quarters of an SM's shared memory (7 on H100: the best of 5-8 measured beside K-D1h's grid), at most
+    // what the occupancy query allows; the CTAs of either kernel that do not fit beside the other's start as those finish.
     const uint32_t huf_ctas = ws->huf_ctas ? ws->huf_ctas : (ws->huf_fit > 1 ? ws->huf_fit / 2 : 1u);
+    if (!ws->seq2_fit) {
+#ifndef ZK_EMUL
+        int dev = 0, fit = 0, sm_smem = 0, reserved = 0;
+        ZK_CUDA_OK(cudaGetDevice(&dev));
+        ZK_CUDA_OK(cudaDeviceGetAttribute(&sm_smem, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
+        ZK_CUDA_OK(cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev));
+        ZK_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fit, zk_seq2_kernel, 32, seq2_smem));
+        const int share = (int)((size_t)sm_smem * 3 / 4 / (seq2_smem + (size_t)reserved));
+        ws->seq2_fit = share < 1 ? 1u : (uint32_t)(share < fit ? share : fit);
+#else
+        ws->seq2_fit = 4;                        // (no SM to fill)
+#endif
+    }
     uint32_t gh = (uint32_t)sms * huf_ctas;      // persistent CTAs
     const size_t need_h = est_blocks / ZK_HUF_SLOTS + 1;
     if (need_h < gh) gh = (uint32_t)need_h;
@@ -2024,10 +2073,12 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     if (hs != stream) ZK_CUDA_OK(cudaEventRecord(ws->ev_huf, hs));
     ws->prof.begin(1, stream);
     {
-        uint32_t g2 = (uint32_t)sms * ws->seq2_ctas;
+        uint32_t g2 = (uint32_t)sms * (ws->seq2_ctas ? ws->seq2_ctas : ws->seq2_fit);
         const size_t need2 = est_blocks / ZK_S2_NCH + 1;
         if (need2 < g2) g2 = (uint32_t)need2;
         ZK_LAUNCH(zk_seq2_kernel, g2, 32, seq2_smem, stream, a);
+        // the blocks it passed on (none in this codec's own archives: the CTAs exit at their first work-counter read)
+        ZK_LAUNCH(zk_seq2_full_kernel, (uint32_t)sms, 32, seq2f_smem, stream, a);
     }
     ws->prof.end(1, stream);
     if (hs != stream) ZK_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_huf, 0));
@@ -2070,7 +2121,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     if (ds != stream) { ZK_CUDA_OK(cudaEventRecord(ws->ev_done, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(ds, ws->ev_done, 0)); }
     ZK_CUDA_OK(cudaMemcpyAsync(ws->h_entries, ws->entries, (size_t)n * sizeof(ZkEntry), cudaMemcpyDeviceToHost, ds));
     ZK_CUDA_OK(cudaMemcpyAsync(ws->h_counters, ws->counters, sizeof(ZkCounters), cudaMemcpyDeviceToHost, ds));
-    ws->launches += 5 + (a.exec_short ? 1 : 0) + (verify_checksum ? 1 : 0);
+    ws->launches += 6 + (a.exec_short ? 1 : 0) + (verify_checksum ? 1 : 0);
     ws->pending_n = n;
     return 0;
 }

@@ -11,7 +11,9 @@ struct ZkDecodeArgs {                 // kernel parameter block (by value)
     uint32_t n_entries;
     ZkBlock* blocks; ZkEntry* entries; ZkCounters* counters; uint32_t* work_counter;
     uint8_t* lit; uint32_t* seq_lit_end; uint32_t* seq_out_end; uint32_t* seq_off;
-    uint32_t* huf_list; uint32_t* seq_list;   // compacted indices of blocks with Huffman literals / with sequences
+    uint32_t* huf_list; uint32_t* seq_list;   // compacted indices of blocks with Huffman literals / with sequences; seq_list has
+                                              // 2 x cap_blocks entries: the second half lists the blocks zk_seq2_kernel passes to
+                                              // zk_seq2_full_kernel
     uint32_t* seg_list;                       // compacted indices of the first blocks of execution segments (long ones from the
                                               // front, short ones from the back: together never more than cap_blocks)
     uint32_t exec_short;                      // segments of at most this many output bytes run on one warp each; 0 = none
@@ -33,8 +35,8 @@ struct ZkDecodeWs {                   // HBM scratch owned by a zk_ctx, grown on
     uint32_t* huf_list = nullptr; uint32_t* seq_list = nullptr; uint32_t* seg_list = nullptr;
     bool attr_set = false; uint32_t ring_override = 0;
     uint32_t exec_warps = 0;          // ZK_EXEC_WARPS: warps per K-D2 CTA (at most 16); 0 = chosen from the entries per SM
-    uint32_t seq2_ctas = 5;           // ZK_SEQ2_CTAS: persistent K-D1s CTAs per SM (5 x 35.4 KiB leave room for two K-D1h CTAs
-                                      // beside them; 6 leave none: DESIGN §6)
+    uint32_t seq2_ctas = 0;           // ZK_SEQ2_CTAS: persistent K-D1s CTAs per SM; 0 = seq2_fit
+    uint32_t seq2_fit = 0;            // K-D1s CTAs in three quarters of an SM's shared memory (queried at the first launch; DESIGN §6)
     uint32_t exec_short = 128 << 10;  // ZK_EXEC_SHORT: output bytes up to which a segment runs on one warp (zk_exec_warp_kernel); 0 = CTAs only
     uint32_t huf_pad = 0;             // extra dynamic smem per Huffman CTA: fewer resident CTAs -> more L1 for the streams (tuning)
     int share = 1;                    // how many batches share the GPU concurrently (host pipeline depth)
