@@ -162,6 +162,29 @@ int32_t zk_compress_frames_csize_dev(zk_ctx* ctx, const void* d_src, size_t n, u
                                      uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len, size_t* consumed, void* cuda_stream);
 
 /*
+ * FrameSizePolicy::ContentDefined(size) over a whole buffer: frame boundaries chosen by the content, so that an edit changes only the frames
+ * around it and later frames keep their bytes.  size (the target mean frame size) is clamped to [4096, 2^30]; mn = size / 4,
+ * mx = min(4 size, 2^30), T = floor((2^64 - 1) / (size - mn)).  Position p is a candidate when h_p >= 2^64 - T, where
+ * h_p = sum over j = max(0, p - 63) .. p of gear(src[j]) * 2^(p - j) mod 2^64 and gear(b) is splitmix64 of b + 1 (the sampling hash of
+ * zk_compress_frames_ldm).  A frame that starts at byte b ends at the first candidate e with b + mn - 1 <= e <= b + mx - 1 (e - b + 1
+ * bytes), else after mx bytes.  The cut depends on the input bytes and size only: not on level, checksum, prefix, or how the input is
+ * split into calls.  A run of one byte value never holds a candidate, so it is cut every mx bytes.  Frame f's bytes are what
+ * zk_compress_frames_sized writes for the same sizes, at every level.
+ * final == 0: only closed frames are written; *consumed = input bytes they cover, the rest must be passed again with more input (a frame
+ * that would end exactly at the end of the input stays open).  final != 0: the rest becomes the last frame; n == 0 gives one empty frame.
+ * Every frame but the last has at least 1024 bytes, so dst_cap >= zk_compress_bound(n, 1024) and frames_cap >= n / 1024 + 1 always
+ * suffice; less than a call needs returns -70 (dstSize_tooSmall).  HOST pointers.
+ */
+int32_t zk_compress_frames_cdc(zk_ctx* ctx, const uint8_t* src, size_t n, uint32_t size, int32_t level, int32_t checksum,
+                               const uint8_t* prefix, size_t prefix_len, int32_t final, uint8_t* dst, size_t dst_cap,
+                               uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames,
+                               size_t* dst_len, size_t* consumed);
+/* the same on device pointers (conventions of zk_compress_frames_dev; no prefix, like the other _dev entry points) */
+int32_t zk_compress_frames_cdc_dev(zk_ctx* ctx, const void* d_src, size_t n, uint32_t size, int32_t level, int32_t checksum,
+                                   int32_t final, void* d_dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes,
+                                   uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len, size_t* consumed, void* cuda_stream);
+
+/*
  * Frames of caller-chosen sizes in one batch (a frame boundary at any byte, as Encoder::end_frame, encode.rs:438-472): frame f covers the
  * next frame_sizes[f] bytes of src, whose length is the sum of the sizes.  Frame f's bytes are exactly what zk_compress_frames_prefix
  * writes for those bytes alone with frame_size = max(frame_sizes[f], 1): a size of 0 gives the empty frame of n == 0, and every level,
@@ -237,7 +260,8 @@ size_t zk_serializer_encoded_len(const zk_serializer* s);                       
 typedef struct zk_encode_options zk_encode_options;
 typedef struct zk_raw_encoder zk_raw_encoder;
 typedef struct zk_encoder zk_encoder;
-typedef enum { ZK_POLICY_COMPRESSED = 0, ZK_POLICY_UNCOMPRESSED = 1 } zk_frame_size_policy; /* encode.rs:21-31 */
+/* encode.rs:21-31; ZK_POLICY_CONTENT: content-defined frames (zk_compress_frames_cdc), an extension of this codec */
+typedef enum { ZK_POLICY_COMPRESSED = 0, ZK_POLICY_UNCOMPRESSED = 1, ZK_POLICY_CONTENT = 2 } zk_frame_size_policy;
 typedef struct { size_t in_progress, out_progress; } zk_compression_progress;           /* encode.rs:43-65 */
 typedef struct { size_t out_progress, data_left; } zk_epilogue_progress;                /* encode.rs:69-92 */
 /* Write sink (W: std::io::Write, encode.rs:570): must consume all len bytes; return 0 on success */
@@ -251,10 +275,12 @@ void zk_encode_options_checksum_flag(zk_encode_options* o, int32_t flag);       
 void zk_encode_options_compression_level(zk_encode_options* o, int32_t level);          /* :176 */
 /* flag != 0: frames given a prefix (the *_compress_with_prefix calls) are matched against the whole of it, as by zk_compress_frames_ldm
  * (the counterpart of the CCtx the reference CLI prepares for with_cctx); every level then runs as level 16.  RawEncoder honours it
- * under both policies (its trial compressions included), Encoder under Uncompressed(n): with Compressed(n)
+ * under both policies (its trial compressions included), Encoder under Uncompressed(n): with Compressed(n) or ContentDefined(n)
  * zk_encode_options_into_encoder returns ZK_ERR_INVALID_ARG and does not consume the options */
 void zk_encode_options_long_distance_matching(zk_encode_options* o, int32_t flag);
-/* consume the options (like `self`) */
+/* consume the options (like `self`).  ZK_POLICY_CONTENT: Encoder only (it buffers and cuts like Compressed(n), through
+ * zk_compress_frames_cdc); zk_encode_options_into_raw_encoder returns ZK_ERR_INVALID_ARG for it, since a RawEncoder reports each call's
+ * progress before the frame's end is known, and does not consume the options */
 int32_t zk_encode_options_into_raw_encoder(zk_encode_options* o, zk_raw_encoder** out); /* :188 */
 int32_t zk_encode_options_into_encoder(zk_encode_options* o, zk_write_fn write, zk_flush_fn flush, void* user,
                                        zk_encoder** out);                               /* :204 */

@@ -81,6 +81,7 @@ class FrameSizePolicy:
     """encode.rs:21-39"""
     COMPRESSED = 0
     UNCOMPRESSED = 1
+    CONTENT = 2
 
     def __init__(self, kind: int, size: int):
         self.kind, self.size = kind, size
@@ -90,6 +91,13 @@ class FrameSizePolicy:
 
     @classmethod
     def Uncompressed(cls, size: int): return cls(cls.UNCOMPRESSED, size)
+
+    @classmethod
+    def ContentDefined(cls, size: int):
+        """frames end where a rolling hash of the input says so, about `size` bytes apart on average (between size/4 and 4*size), so that
+        an edit changes only the frames around it.  An extension of this codec: Encoder only (not RawEncoder, not with long-distance
+        matching); Context.compress_frames_cdc is the batch form"""
+        return cls(cls.CONTENT, size)
 
     @classmethod
     def default(cls): return cls.Uncompressed(0x200000)
@@ -184,6 +192,24 @@ class Context:
         _check(lib.zk_compress_frames_csize(self._h, addr, n, target, level, int(checksum), paddr, pn, int(final), dst.ctypes.data, cap,
                                             cs.ctypes.data_as(_native.u32p), ds.ctypes.data_as(_native.u32p), nfmax, byref(nf), byref(dl),
                                             byref(used)), lib)
+        return dst[: dl.value], cs[: nf.value].copy(), ds[: nf.value].copy(), int(used.value)
+
+    def compress_frames_cdc(self, data, size: int, level: int = 0, checksum: bool = False, prefix=None, final: bool = True):
+        """FrameSizePolicy::ContentDefined(size) on the batch path -> (compressed bytes (np.uint8), c_sizes, d_sizes, consumed).
+        Frame boundaries depend on the input bytes and `size` only (the rule: include/zeekstd_b200.h, zk_compress_frames_cdc); frame f's
+        bytes are what compress_frames_sized writes for the same sizes.  final=False: only closed frames are made and `consumed` input
+        bytes are covered; pass the rest again with more input."""
+        addr, n, keep = _buf(data)
+        lib = self.lib
+        cap = lib.zk_compress_bound(n, 1024)
+        dst = np.empty(cap + 64, dtype=np.uint8)
+        nfmax = n // 1024 + 1
+        cs = np.zeros(nfmax, dtype=np.uint32); ds = np.zeros(nfmax, dtype=np.uint32)
+        nf = c_uint32(); dl = c_size_t(); used = c_size_t()
+        paddr, pn, pkeep = _buf(prefix) if prefix is not None else (None, 0, None)
+        _check(lib.zk_compress_frames_cdc(self._h, addr, n, size, level, int(checksum), paddr, pn, int(final), dst.ctypes.data, cap,
+                                          cs.ctypes.data_as(_native.u32p), ds.ctypes.data_as(_native.u32p), nfmax, byref(nf), byref(dl),
+                                          byref(used)), lib)
         return dst[: dl.value], cs[: nf.value].copy(), ds[: nf.value].copy(), int(used.value)
 
     def decompress_frames(self, comp, c_off, d_off, verify_checksum: bool = True, out: np.ndarray | None = None, need=None, prefix=None):
@@ -342,7 +368,8 @@ class EncodeOptions:
 
     def long_distance_matching(self, flag: bool):
         """match the frames of compress_with_prefix against the whole prefix (what the reference CLI sets on the CCtx it passes to
-        with_cctx for patch files).  Every level then runs as level 16; into_encoder refuses it with FrameSizePolicy.Compressed"""
+        with_cctx for patch files).  Every level then runs as level 16; into_encoder refuses it with FrameSizePolicy.Compressed and
+        FrameSizePolicy.ContentDefined"""
         self._ldm = bool(flag); return self
 
     def _native_opts(self):
@@ -365,7 +392,12 @@ class RawEncoder:
         opts = opts or EncodeOptions()
         self.ctx, self.lib = opts.ctx, opts.ctx.lib
         h = c_void_p()
-        _check(self.lib.zk_encode_options_into_raw_encoder(opts._native_opts(), byref(h)), self.lib)
+        self._h = None
+        o = opts._native_opts()
+        rc = self.lib.zk_encode_options_into_raw_encoder(o, byref(h))
+        if rc:                                              # refused options (FrameSizePolicy.ContentDefined) are not consumed
+            self.lib.zk_encode_options_free(o)
+        _check(rc, self.lib)
         self._h = h
 
     def __del__(self):

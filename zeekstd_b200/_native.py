@@ -66,6 +66,10 @@ _SIGS = {
                                            c_size_t, u32p, u32p, c_uint32, u32p, POINTER(c_size_t), POINTER(c_size_t)]),
     "zk_compress_frames_csize_dev": (c_int32, [c_void_p, c_void_p, c_size_t, c_uint32, c_int32, c_int32, c_int32, c_void_p, c_size_t,
                                                u32p, u32p, c_uint32, u32p, POINTER(c_size_t), POINTER(c_size_t), c_void_p]),
+    "zk_compress_frames_cdc": (c_int32, [c_void_p, c_void_p, c_size_t, c_uint32, c_int32, c_int32, c_void_p, c_size_t, c_int32, c_void_p,
+                                         c_size_t, u32p, u32p, c_uint32, u32p, POINTER(c_size_t), POINTER(c_size_t)]),
+    "zk_compress_frames_cdc_dev": (c_int32, [c_void_p, c_void_p, c_size_t, c_uint32, c_int32, c_int32, c_int32, c_void_p, c_size_t,
+                                             u32p, u32p, c_uint32, u32p, POINTER(c_size_t), POINTER(c_size_t), c_void_p]),
     "zk_compress_frames_sized": (c_int32, [c_void_p, c_void_p, u32p, c_uint32, c_int32, c_int32, c_void_p, c_size_t, c_void_p, c_size_t,
                                            u32p, POINTER(c_size_t)]),
     "zk_compress_frames_sized_dev": (c_int32, [c_void_p, c_void_p, u32p, c_uint32, c_int32, c_int32, c_void_p, c_size_t, u32p,

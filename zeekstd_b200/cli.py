@@ -14,7 +14,9 @@ at -131072).  `--patch-from F` alone matches every frame against the last 32 KiB
 window-log / long-distance-matching parameters the reference sets for patch files take effect: every frame is matched against
 the whole of F (its last 128 MiB when it is larger), which is what makes the archive a patch.  Long-distance matching is part
 of the high-level tier, so with `--long` every compression level writes what level 16 writes, and the frame size policy must be
-`uncompressed`.  `--mmap-prefix` / `--no-mmap-prefix` choose between np.memmap and a read.
+`uncompressed`.  `--mmap-prefix` / `--no-mmap-prefix` choose between np.memmap and a read.  `--frame-size-policy content` (an
+extension of this codec) ends frames where a rolling hash of the data says so, about `-s` bytes apart on average, so that an edit
+of the input changes only the frames around it and rsync, dedup stores and range-fetching clients can reuse the rest.
 """
 from __future__ import annotations
 
@@ -141,7 +143,9 @@ def build_parser() -> argparse.ArgumentParser:
                         "-131072) for fast mode: faster, lower ratio, literals stored without Huffman coding. Default 3.")
     c.add_argument("--no-checksum", action="store_true", help="Don't include frame checksums.")
     c.add_argument("-s", "--frame-size", type=byte_value, default=byte_value("2M"))
-    c.add_argument("--frame-size-policy", choices=["compressed", "uncompressed"], default="uncompressed")
+    c.add_argument("--frame-size-policy", choices=["compressed", "uncompressed", "content"], default="uncompressed",
+                   help="content: content-defined frames of about --frame-size bytes on average (between a quarter and four times it), "
+                        "so that an edit changes only the frames around it.")
     c.add_argument("--patch-from", default=None, help="Provide a reference point for Zstandard's diff engine.")
     c.add_argument("--long", action="store_true",
                    help="With --patch-from: long-distance matching against the whole reference file (its last 128 MiB), so that the archive "
@@ -316,7 +320,7 @@ def _run_compress(zk, ns, fmt_bytes) -> int:
         raise CliError("Frame size too big")
     if ns.long and not ns.patch_from:
         raise CliError("--long needs --patch-from: long-distance matching runs against the reference file")
-    if ns.long and ns.frame_size_policy == "compressed":
+    if ns.long and ns.frame_size_policy in ("compressed", "content"):
         raise CliError("--long needs --frame-size-policy uncompressed")
     prefix_len = os.path.getsize(ns.patch_from) if ns.patch_from and os.path.exists(ns.patch_from) else None
     st_file = None
@@ -329,7 +333,8 @@ def _run_compress(zk, ns, fmt_bytes) -> int:
     bar = _Progress(in_len, fmt_bytes, not ns.quiet and not ns.no_progress)
     writer = _new_writer(out_path, in_path, ns.quiet, ns.force)
 
-    policy = (zk.FrameSizePolicy.Compressed if ns.frame_size_policy == "compressed" else zk.FrameSizePolicy.Uncompressed)(ns.frame_size)
+    policy = {"compressed": zk.FrameSizePolicy.Compressed, "uncompressed": zk.FrameSizePolicy.Uncompressed,
+              "content": zk.FrameSizePolicy.ContentDefined}[ns.frame_size_policy](ns.frame_size)
     enc = (zk.EncodeOptions().frame_size_policy(policy).checksum_flag(not ns.no_checksum)
            .compression_level(ns.compression_level).long_distance_matching(ns.long).into_encoder(writer))
     prefix = _load_prefix(ns.patch_from, _use_mmap(ns, prefix_len))

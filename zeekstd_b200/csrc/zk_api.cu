@@ -6,6 +6,7 @@
 #include <stdio.h>
 #include <time.h>
 #include <stdlib.h>
+#include <string.h>
 #include <vector>
 
 static thread_local char zk_tls_cuda_msg[256] = "";
@@ -356,22 +357,34 @@ struct ZkFrameList {
     }
 };
 
-// device-resident input and output: sub-batches (which bound the scratch, about 4x the sub-batch input) one after the other on st
-static int32_t zk_compress_dev_run(zk_ctx* c, const ZkFrameList& fl, const uint8_t* d_src, int32_t level, int32_t checksum, uint8_t* d_dst,
-                                   size_t dst_cap, uint32_t* c_sizes, size_t* dst_len, cudaStream_t st) {
-    const size_t sub_bytes = zk_env_size("ZK_DEV_SUB_BYTES", (size_t)1 << 30);
-    cudaEventRecord(c->ev0, st);
+// device-resident input and output: sub-batches of at most sub_bytes input (which bound the scratch, about 4x that) one after the other on
+// st, every frame with the prefix d_prefix (device memory; nullptr: none) -> *dst_len
+static int32_t zk_compress_dev_subs(zk_ctx* c, const ZkFrameList& fl, const uint8_t* d_src, const uint8_t* d_prefix, uint32_t prefix_len,
+                                    int32_t level, int32_t checksum, uint8_t* d_dst, size_t dst_cap, uint32_t* c_sizes, size_t* dst_len,
+                                    cudaStream_t st, size_t sub_bytes) {
     size_t out_pos = 0, in_off = 0;
     for (uint32_t f0 = 0; f0 < fl.count;) {
         size_t in_len = 0;
         const uint32_t end = fl.next_sub(f0, sub_bytes, &in_len);
         size_t produced = 0;
         c->slot[0].ews.no_side = false;
+        c->slot[0].ews.prefix = d_prefix; c->slot[0].ews.prefix_len = prefix_len;
         int rc = fl.enqueue(&c->slot[0].ews, st, d_src + in_off, f0, end - f0, in_len, level, checksum, d_dst + out_pos, dst_cap - out_pos);
         if (!rc) rc = zk_encode_collect(&c->slot[0].ews, st, c_sizes ? c_sizes + f0 : nullptr, &produced);
         if (rc) return rc;
         out_pos += produced; in_off += in_len; f0 = end;
     }
+    *dst_len = out_pos;
+    return 0;
+}
+
+static int32_t zk_compress_dev_run(zk_ctx* c, const ZkFrameList& fl, const uint8_t* d_src, int32_t level, int32_t checksum, uint8_t* d_dst,
+                                   size_t dst_cap, uint32_t* c_sizes, size_t* dst_len, cudaStream_t st) {
+    const size_t sub_bytes = zk_env_size("ZK_DEV_SUB_BYTES", (size_t)1 << 30);
+    cudaEventRecord(c->ev0, st);
+    size_t out_pos = 0;
+    const int32_t rc = zk_compress_dev_subs(c, fl, d_src, nullptr, 0, level, checksum, d_dst, dst_cap, c_sizes, &out_pos, st, sub_bytes);
+    if (rc) return rc;
     cudaEventRecord(c->ev1, st);
     cudaEventSynchronize(c->ev1);
     cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1);
@@ -605,14 +618,21 @@ extern "C" int32_t zk_compress_frames_sized_dev(zk_ctx* c, const void* d_src, co
 }
 
 // ---------------------------------------------------------------------------------------------
-// FrameSizePolicy::Compressed(target) on the batch path (zk_encode_csize): passes over the input, each starting at the first byte
-// the previous one left in an open frame.  A pass starts at the encode sub-batch size and doubles while it closes no frame, up to
-// 1 GiB, where the frame-size cap forces a close.
+// Frame sizes decided on the GPU (FrameSizePolicy::Compressed and ::ContentDefined): passes over the input, each starting at the first
+// byte the previous one left in an open frame.  A pass starts at the encode sub-batch size and doubles while it closes no frame, up to
+// grow_to, a pass length at which the policy always closes one.  step(d_in, len, at_end, d_out, cap, &r) cuts one pass and compresses the
+// frames it closes to d_out.  min_frame: the fewest bytes of any frame but the last, which bounds a pass's output.
 // ---------------------------------------------------------------------------------------------
-static int32_t zk_csize_passes(zk_ctx* c, bool host, const uint8_t* src, size_t n, uint32_t target, int32_t level, int32_t checksum,
-                               const uint8_t* d_prefix, uint32_t prefix_len, int32_t final_, uint8_t* dst, size_t dst_cap,
-                               uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len,
-                               size_t* consumed, cudaStream_t st, size_t first_pass) {
+struct ZkPassOut {
+    uint32_t n_frames = 0;
+    size_t consumed = 0, total = 0;                         // input bytes the frames cover; bytes written
+    const uint32_t* c_sizes = nullptr; const uint32_t* d_sizes = nullptr;
+};
+
+template <class Step>
+static int32_t zk_frame_passes(zk_ctx* c, bool host, const uint8_t* src, size_t n, uint8_t* dst, size_t dst_cap, uint32_t* c_sizes,
+                               uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len, size_t* consumed, cudaStream_t st,
+                               size_t first_pass, size_t grow_to, uint32_t min_frame, const Step& step) {
     const size_t block = 32768, max_pass = ZK_SEEKABLE_MAX_FRAME_SIZE;
     first_pass = first_pass / block * block;
     if (first_pass < block) first_pass = block;
@@ -626,18 +646,18 @@ static int32_t zk_csize_passes(zk_ctx* c, bool host, const uint8_t* src, size_t 
         const int at_end = pos + len == n;
         const uint8_t* d_in = src + pos; uint8_t* d_out = dst + out; size_t cap = dst_cap - out;
         if (host) {
-            cap = zk_encode_bound(len, (uint32_t)block);
+            cap = zk_encode_bound(len, min_frame);
             int rc = zk_slot_ensure(&s, len + 32, cap + 32);
             if (rc) return rc;
             ZK_RT_OK(cudaMemcpyAsync(s.d_in, src + pos, len, cudaMemcpyHostToDevice, st));
             d_in = s.d_in; d_out = s.d_out;
         }
-        ZkCsizeOut r;
-        int rc = zk_encode_csize(&s.ews, st, d_in, len, target, level, checksum, final_, at_end, d_prefix, prefix_len, d_out, cap, &r);
+        ZkPassOut r;
+        int rc = step(d_in, len, at_end, d_out, cap, &r);
         if (rc) return rc;
         if (r.n_frames == 0) {
             if (at_end) break;
-            pass = 2 * pass < max_pass ? 2 * pass : max_pass;
+            pass = 2 * pass < grow_to ? 2 * pass : grow_to;
             continue;
         }
         if (r.n_frames > frames_cap - nf) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
@@ -645,11 +665,8 @@ static int32_t zk_csize_passes(zk_ctx* c, bool host, const uint8_t* src, size_t 
             if (r.total > dst_cap - out) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
             ZK_RT_OK(cudaMemcpy(dst + out, s.d_out, r.total, cudaMemcpyDeviceToHost));
         }
-        for (uint32_t f = 0; f < r.n_frames; f++) {
-            const size_t lo = (size_t)r.starts[f] * block, hi = (size_t)r.starts[f + 1] * block < len ? (size_t)r.starts[f + 1] * block : len;
-            if (c_sizes) c_sizes[nf + f] = r.c_sizes[f];
-            if (d_sizes) d_sizes[nf + f] = (uint32_t)(hi - lo);
-        }
+        if (c_sizes) memcpy(c_sizes + nf, r.c_sizes, (size_t)r.n_frames * 4);
+        if (d_sizes) memcpy(d_sizes + nf, r.d_sizes, (size_t)r.n_frames * 4);
         nf += r.n_frames; out += r.total; pos += r.consumed;
         pass = first_pass;
     }
@@ -657,6 +674,29 @@ static int32_t zk_csize_passes(zk_ctx* c, bool host, const uint8_t* src, size_t 
     if (dst_len) *dst_len = out;
     if (consumed) *consumed = pos;
     return 0;
+}
+
+// Compressed(target) (zk_encode_csize): the cut and the frames in one step; frames start at 32 KiB blocks
+static int32_t zk_csize_passes(zk_ctx* c, bool host, const uint8_t* src, size_t n, uint32_t target, int32_t level, int32_t checksum,
+                               const uint8_t* d_prefix, uint32_t prefix_len, int32_t final_, uint8_t* dst, size_t dst_cap,
+                               uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len,
+                               size_t* consumed, cudaStream_t st, size_t first_pass) {
+    const size_t block = 32768;
+    std::vector<uint32_t> ds;
+    auto step = [&](const uint8_t* d_in, size_t len, int at_end, uint8_t* d_out, size_t cap, ZkPassOut* o) -> int32_t {
+        ZkCsizeOut r;
+        const int rc = zk_encode_csize(&c->slot[0].ews, st, d_in, len, target, level, checksum, final_, at_end, d_prefix, prefix_len, d_out, cap, &r);
+        if (rc) return rc;
+        ds.resize(r.n_frames);
+        for (uint32_t f = 0; f < r.n_frames; f++) {
+            const size_t lo = (size_t)r.starts[f] * block, hi = (size_t)r.starts[f + 1] * block < len ? (size_t)r.starts[f + 1] * block : len;
+            ds[f] = (uint32_t)(hi - lo);
+        }
+        o->n_frames = r.n_frames; o->consumed = r.consumed; o->total = r.total; o->c_sizes = r.c_sizes; o->d_sizes = ds.data();
+        return 0;
+    };
+    return zk_frame_passes(c, host, src, n, dst, dst_cap, c_sizes, d_sizes, frames_cap, n_frames, dst_len, consumed, st, first_pass,
+                           ZK_SEEKABLE_MAX_FRAME_SIZE, (uint32_t)block, step);
 }
 
 extern "C" int32_t zk_compress_frames_csize(zk_ctx* c, const uint8_t* src, size_t n, uint32_t target, int32_t level, int32_t checksum,
@@ -696,6 +736,77 @@ extern "C" int32_t zk_compress_frames_csize_dev(zk_ctx* c, const void* d_src, si
     cudaEventRecord(c->ev0, st);
     const int32_t rc = zk_csize_passes(c, false, (const uint8_t*)d_src, n, target, level, checksum, nullptr, 0, final_, (uint8_t*)d_dst, dst_cap,
                                        c_sizes, d_sizes, frames_cap, n_frames, dst_len, consumed, st, zk_env_size("ZK_DEV_SUB_BYTES", (size_t)1 << 30));
+    cudaEventRecord(c->ev1, st);
+    cudaEventSynchronize(c->ev1);
+    cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1);
+    return rc;
+}
+
+// ---------------------------------------------------------------------------------------------
+// FrameSizePolicy::ContentDefined(size): each pass is cut on the GPU (zk_encode_cdc), then its closed frames are compressed from the same
+// device memory by the sized path, in sub-batches of at most the first pass's length.  A pass of mx bytes always closes a frame.
+// ZK_CDC_CAP (tests): candidate positions kept per pass (default pass / 64 + 1); fewer only makes a pass cover less.
+// ---------------------------------------------------------------------------------------------
+static int32_t zk_cdc_passes(zk_ctx* c, bool host, const uint8_t* src, size_t n, uint32_t size, int32_t level, int32_t checksum,
+                             const uint8_t* d_prefix, uint32_t prefix_len, int32_t final_, uint8_t* dst, size_t dst_cap,
+                             uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len,
+                             size_t* consumed, cudaStream_t st, size_t first_pass) {
+    const ZkCdcRule rule = zk_cdc_rule(size);
+    const uint32_t cand_cap = (uint32_t)zk_env_size("ZK_CDC_CAP", 0);
+    std::vector<uint32_t> ds, cs;
+    auto step = [&](const uint8_t* d_in, size_t len, int at_end, uint8_t* d_out, size_t cap, ZkPassOut* o) -> int32_t {
+        ZkCdcOut r;
+        int32_t rc = zk_encode_cdc(&c->slot[0].ews, st, d_in, len, size, final_, at_end, cand_cap, &r);
+        if (rc || r.n_frames == 0) return rc;
+        ds.assign(r.sizes, r.sizes + r.n_frames);
+        cs.resize(r.n_frames);
+        const ZkFrameList fl = {ds.data(), r.consumed, 0, r.n_frames};
+        rc = zk_compress_dev_subs(c, fl, d_in, d_prefix, prefix_len, level, checksum, d_out, cap, cs.data(), &o->total, st, first_pass);
+        if (rc) return rc;
+        o->n_frames = r.n_frames; o->consumed = r.consumed; o->c_sizes = cs.data(); o->d_sizes = ds.data();
+        return 0;
+    };
+    return zk_frame_passes(c, host, src, n, dst, dst_cap, c_sizes, d_sizes, frames_cap, n_frames, dst_len, consumed, st, first_pass, rule.mx,
+                           rule.mn, step);
+}
+
+extern "C" int32_t zk_compress_frames_cdc(zk_ctx* c, const uint8_t* src, size_t n, uint32_t size, int32_t level, int32_t checksum,
+                                          const uint8_t* prefix, size_t prefix_len, int32_t final_, uint8_t* dst, size_t dst_cap,
+                                          uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames,
+                                          size_t* dst_len, size_t* consumed) {
+    if (!c || !dst || (n && !src)) return ZK_ERR_INVALID_ARG;
+    if (consumed) *consumed = 0;
+    if (n == 0) {                                           // one empty frame, as zk_compress_frames makes of no input
+        if (final_) return zk_compress_frames_prefix(c, src, 0, 1, level, checksum, prefix, prefix_len, dst, dst_cap, c_sizes, d_sizes, frames_cap, n_frames, dst_len);
+        if (n_frames) *n_frames = 0;
+        if (dst_len) *dst_len = 0;
+        return 0;
+    }
+    ZK_RT_OK(cudaSetDevice(c->device));
+    int32_t rc = zk_ctx_set_prefix(c, prefix, prefix_len);
+    if (rc) return rc;
+    rc = zk_cdc_passes(c, true, src, n, size, level, checksum, c->cur_prefix_len ? c->d_prefix : nullptr, c->cur_prefix_len, final_, dst, dst_cap,
+                       c_sizes, d_sizes, frames_cap, n_frames, dst_len, consumed, c->slot[0].stream, zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20));
+    c->cur_prefix_len = 0;
+    return rc;
+}
+
+extern "C" int32_t zk_compress_frames_cdc_dev(zk_ctx* c, const void* d_src, size_t n, uint32_t size, int32_t level, int32_t checksum,
+                                              int32_t final_, void* d_dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes,
+                                              uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len, size_t* consumed, void* cuda_stream) {
+    if (!c || !d_dst || (n && !d_src)) return ZK_ERR_INVALID_ARG;
+    if (consumed) *consumed = 0;
+    if (n == 0) {
+        if (final_) return zk_compress_frames_dev(c, d_src, 0, 1, level, checksum, d_dst, dst_cap, c_sizes, d_sizes, frames_cap, n_frames, dst_len, cuda_stream);
+        if (n_frames) *n_frames = 0;
+        if (dst_len) *dst_len = 0;
+        return 0;
+    }
+    ZK_RT_OK(cudaSetDevice(c->device));
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : c->slot[0].stream;
+    cudaEventRecord(c->ev0, st);
+    const int32_t rc = zk_cdc_passes(c, false, (const uint8_t*)d_src, n, size, level, checksum, nullptr, 0, final_, (uint8_t*)d_dst, dst_cap,
+                                     c_sizes, d_sizes, frames_cap, n_frames, dst_len, consumed, st, zk_env_size("ZK_DEV_SUB_BYTES", (size_t)1 << 30));
     cudaEventRecord(c->ev1, st);
     cudaEventSynchronize(c->ev1);
     cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1);

@@ -1502,6 +1502,7 @@ size_t zk_encode_bound_sized(const uint32_t* sizes, uint32_t n_frames) {
 
 void zk_encode_ws_free(ZkEncodeWs* ws) {
     if (ws->buf) cudaFree(ws->buf);
+    if (ws->cut) cudaFree(ws->cut);
     if (ws->h_sizes) cudaFreeHost(ws->h_sizes);
     if (ws->side) cudaStreamDestroy(ws->side);
     if (ws->ev_a) cudaEventDestroy(ws->ev_a);
@@ -1532,6 +1533,7 @@ static int zkc_build_geometry(ZkEncodeWs* ws, cudaStream_t stream, ZkcGeo* geo, 
 }
 
 #include "zk_hc.inc"
+#include "zk_cdc.inc"
 
 // one batch of n_frames frames: of frame_size bytes (the last one shorter) when h_sizes is null, else of h_sizes[f] bytes (n = their sum)
 static int zkc_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t frame_size, const uint32_t* h_sizes,
@@ -1852,5 +1854,79 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     out->total = (size_t)total;
     out->c_sizes = h + ZKC_RES_HDR;
     out->starts = h + ZKC_RES_HDR + nb;
+    return 0;
+}
+
+ZkCdcRule zk_cdc_rule(uint32_t size) {
+    const uint32_t s = size < 4096u ? 4096u : (size > 0x40000000u ? 0x40000000u : size);
+    ZkCdcRule r;
+    r.mn = s / 4;
+    r.mx = (uint32_t)((uint64_t)s * 4 < 0x40000000ull ? (uint64_t)s * 4 : 0x40000000ull);
+    r.thr = 0ull - ~0ull / (s - r.mn);
+    return r;
+}
+
+// FrameSizePolicy::ContentDefined(size) over one pass of n <= 1 GiB bytes at d_src, which starts a frame: the cut of zk_cdc.inc, then one
+// D2H copy of the counts and sizes and one synchronisation.  cap: candidates kept (0: n / 64 + 1).
+int zk_encode_cdc(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t size, int final_, int at_end, uint32_t cap,
+                  ZkCdcOut* out) {
+    *out = ZkCdcOut();
+    if (n == 0) return 0;
+    if (n > 0x40000000u) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
+    const ZkCdcRule rule = zk_cdc_rule(size);
+    ZkCdcArgs a;
+    a.src = d_src; a.n = (uint32_t)n; a.mn = rule.mn; a.mx = rule.mx; a.thr = rule.thr;
+    a.runs = (uint32_t)((n + ZKC_CDC_RUN - 1) / ZKC_CDC_RUN);
+    a.cap = cap ? cap : (uint32_t)(n / 64 + 1);
+    a.end_closes = at_end && final_; a.end_lazy = at_end && !final_;
+    const size_t nc = (size_t)a.runs + 1, nchunks = (nc + ZKC_HC_SCAN - 1) / ZKC_HC_SCAN;
+    const size_t res_words = ZKC_CDC_RES_HDR + n / rule.mn + 2;       // every frame but the last has at least mn bytes
+    size_t off = 0;
+    const size_t o_cnt = off; off = zkc_align(off + nc * 4);
+    const size_t o_sum = off; off = zkc_align(off + (nchunks + 1) * 4);
+    const size_t o_cand = off; off = zkc_align(off + (size_t)a.cap * 4);
+    const size_t o_nxt = off; off = zkc_align(off + (size_t)a.cap * 8);
+    const size_t o_res = off; off = zkc_align(off + res_words * 4);
+    if (ws->cut_cap < off) {
+        if (ws->cut) cudaFree(ws->cut);
+        ws->cut = nullptr; ws->cut_cap = 0;
+        const size_t want = off + off / 8;
+        if (cudaMalloc(&ws->cut, want) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
+        ws->cut_cap = want;
+    }
+    if (ws->cap_frames < res_words) {
+        if (ws->h_sizes) cudaFreeHost(ws->h_sizes);
+        ws->h_sizes = nullptr; ws->cap_frames = 0;
+        const size_t want = res_words + res_words / 8 + 16;
+        if (cudaMallocHost((void**)&ws->h_sizes, want * 4 + 32) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
+        ws->cap_frames = want;
+    }
+    uint8_t* base = (uint8_t*)ws->cut;
+    a.counts = (uint32_t*)(base + o_cnt); a.cand = (uint32_t*)(base + o_cand); a.nxt = (uint2*)(base + o_nxt); a.res = (uint32_t*)(base + o_res);
+    uint32_t* sums = (uint32_t*)(base + o_sum);
+    if (!ws->attr_set_cdc) {
+        ZKC_CUDA_OK(cudaFuncSetAttribute(zk_cdc_walk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(ZKC_CDC_STAGE * 8)));
+        ws->attr_set_cdc = true;
+    }
+    const uint32_t grid = (a.runs + 255) / 256;
+    ws->prof.begin(0, stream);
+    ZK_LAUNCH(zk_cdc_count_kernel, grid, 256, 0, stream, a);
+    ZK_LAUNCH(zk_hc_scan_kernel, (uint32_t)nchunks, 1024, 0, stream, a.counts, nc, sums);
+    ZK_LAUNCH(zk_hc_scan_top_kernel, 1, 1024, 0, stream, sums, (uint32_t)nchunks);
+    ZK_LAUNCH(zk_hc_scan_add_kernel, (uint32_t)((nc + 255) / 256), 256, 0, stream, a.counts, nc, (const uint32_t*)sums);
+    ZK_LAUNCH(zk_cdc_emit_kernel, grid, 256, 0, stream, a);
+    ZK_LAUNCH(zk_cdc_next_kernel, (a.cap + 255) / 256, 256, 0, stream, a);
+    ZK_LAUNCH(zk_cdc_walk_kernel, 1, 1024, (a.cap < ZKC_CDC_STAGE ? a.cap : ZKC_CDC_STAGE) * 8, stream, a);
+    ws->prof.end(0, stream);
+    ws->launches += 7;
+    ZKC_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, a.res, res_words * 4, cudaMemcpyDeviceToHost, stream));
+    ZKC_CUDA_OK(cudaStreamSynchronize(stream));
+#ifndef ZK_EMUL
+    { cudaError_t le__ = cudaGetLastError(); if (le__ != cudaSuccess) { zk_note_cuda_error("kernel launch / execution", (int)le__); return ZK_INT_CUDA; } }
+#endif
+    ws->prof.harvest();
+    out->n_frames = ws->h_sizes[0];
+    out->consumed = ws->h_sizes[1];
+    out->sizes = ws->h_sizes + ZKC_CDC_RES_HDR;
     return 0;
 }

@@ -4,11 +4,12 @@
 
 struct ZkEncodeWs {                    // HBM scratch owned by a zk_ctx slot, grown on demand
     void* buf = nullptr; size_t cap = 0;
+    void* cut = nullptr; size_t cut_cap = 0;              // content-defined cut (zk_encode_cdc): kept apart from buf, which the frames of a cut then use
     uint32_t* h_sizes = nullptr; size_t cap_frames = 0;   // pinned: per-frame compressed sizes
     int sm_count = 0;
     unsigned long long launches = 0;
     uint32_t pending_frames = 0;
-    bool attr_set = false, attr_set_wide = false, attr_set_walk = false, attr_set_hc = false;
+    bool attr_set = false, attr_set_wide = false, attr_set_walk = false, attr_set_hc = false, attr_set_cdc = false;
     const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device pointer: raw-content prefix for the NEXT enqueue (one-shot)
     bool ldm = false;                 // long-distance matching against that prefix for the NEXT enqueue (one-shot; nothing without a prefix)
     int prio = 0;                     // CUDA stream priority of the side stream (matches the slot's stream)
@@ -43,3 +44,18 @@ struct ZkCsizeOut {
 };
 int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t target, int level, int checksum,
                     int final_, int at_end, const uint8_t* d_prefix, uint32_t prefix_len, uint8_t* d_dst, size_t dst_cap, ZkCsizeOut* out);
+
+// FrameSizePolicy::ContentDefined(size): size clamped to [4096, 2^30]; frames of mn .. mx bytes end at the first position whose 64-byte gear
+// hash is >= thr (zk_cdc.inc states the rule)
+struct ZkCdcRule { uint32_t mn, mx; unsigned long long thr; };
+ZkCdcRule zk_cdc_rule(uint32_t size);
+// The cut only, over one pass of n <= 1 GiB bytes at d_src that starts a frame (at_end / final_ as for zk_encode_csize).  cap: candidate
+// positions kept (0: n / 64 + 1); fewer only shortens what one pass covers.  *out->sizes lives in the workspace's pinned buffer until the
+// next call.  Synchronous on `stream`.
+struct ZkCdcOut {
+    uint32_t n_frames = 0;
+    size_t consumed = 0;                 // input bytes the frames cover
+    const uint32_t* sizes = nullptr;     // n_frames frame sizes
+};
+int zk_encode_cdc(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t size, int final_, int at_end, uint32_t cap,
+                  ZkCdcOut* out);

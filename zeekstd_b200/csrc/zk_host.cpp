@@ -290,6 +290,9 @@ struct zk_raw_encoder {                    // encode.rs:266-545
 
 extern "C" int32_t zk_encode_options_into_raw_encoder(zk_encode_options* o, zk_raw_encoder** out) {
     if (!o || !out) return ZK_ERR_INVALID_ARG;
+    // content-defined frames end where a hash of later bytes says so, and there is no CPU path to hash on: a RawEncoder could not report
+    // its progress before the end is known
+    if (o->kind == ZK_POLICY_CONTENT) return ZK_ERR_INVALID_ARG;
     zk_raw_encoder* e = new (std::nothrow) zk_raw_encoder();
     if (!e) return ZK_ERR_ZSTD(64);
     e->ctx = o->ctx; e->kind = o->kind; e->size = o->size; e->checksum = o->checksum; e->level = o->level; e->ldm = o->ldm;
@@ -367,8 +370,8 @@ extern "C" void zk_raw_encoder_reset_seek_table(zk_raw_encoder* e) { e->seek_tab
 
 // ---- Encoder<W: Write> (encode.rs:568-800) -----------------------------------------------------------------
 // Input is buffered and handed to the GPU in batches (the sink is owned by the encoder, so delaying writes is invisible to
-// the caller).  Uncompressed(n) batches whole frames; Compressed(n) hands the buffer to zk_compress_frames_csize, which
-// closes frames by the rule of that entry point and leaves the open frame in the buffer.
+// the caller).  Uncompressed(n) batches whole frames; Compressed(n) and ContentDefined(n) hand the buffer to zk_compress_frames_csize /
+// zk_compress_frames_cdc, which close frames by the rule of that entry point and leave the open frame in the buffer.
 struct zk_encoder {
     zk_raw_encoder raw;
     zk_write_fn write; zk_flush_fn flush; void* user;
@@ -378,7 +381,7 @@ struct zk_encoder {
     size_t batch_frames = 8192;            // a GPU call takes the buffered complete frames once there are this many ...
     size_t batch_bytes = (size_t)128 << 20; // ... or this many bytes of them (64 frames of 2 MiB; thousands of small ones: one launch sequence serves them all)
     const uint8_t* prefix = nullptr; size_t prefix_len = 0;   // prefix of the frames in `batch` (compress_with_prefix)
-    size_t csize_at = (size_t)128 << 20;   // Compressed(n): buffered bytes at which the next cut runs (doubles while a cut closes no frame)
+    size_t csize_at = (size_t)128 << 20;   // Compressed(n), ContentDefined(n): buffered bytes at which the next cut runs (doubles while a cut closes no frame)
 
     int32_t sink(const uint8_t* p, size_t n) {
         if (!n) return 0;
@@ -407,16 +410,19 @@ struct zk_encoder {
         if (written) *written = len;
         return 0;
     }
-    // Compressed(n): every frame of `batch` that closes (all of them with final_), in one batch call
+    bool cuts_on_gpu() const { return raw.kind == ZK_POLICY_COMPRESSED || raw.kind == ZK_POLICY_CONTENT; }
+    // Compressed(n), ContentDefined(n): every frame of `batch` that closes (all of them with final_), in one batch call.  Every frame but
+    // the last has at least min_frame bytes.
     int32_t flush_csize(int32_t final_, size_t* written) {
-        const size_t count = batch.size();
-        size_t cap = zk_compress_bound(count, 32768);
+        const bool cdc = raw.kind == ZK_POLICY_CONTENT;
+        const size_t count = batch.size(), min_frame = cdc ? 1024 : 32768;
+        size_t cap = zk_compress_bound(count, (uint32_t)min_frame);
         stage.resize(cap);
-        uint32_t nfmax = (uint32_t)(count / 32768 + 2);
+        uint32_t nfmax = (uint32_t)(count / min_frame + 2);
         std::vector<uint32_t> cs(nfmax), ds(nfmax);
         uint32_t nf = 0; size_t len = 0, used = 0;
         static const uint8_t dummy = 0;
-        int32_t rc = zk_compress_frames_csize(raw.ctx, count ? batch.data() : &dummy, count, raw.size, raw.level, raw.checksum, prefix, prefix_len, final_,
+        int32_t rc = (cdc ? zk_compress_frames_cdc : zk_compress_frames_csize)(raw.ctx, count ? batch.data() : &dummy, count, raw.size, raw.level, raw.checksum, prefix, prefix_len, final_,
                                               stage.data(), cap, cs.data(), ds.data(), nfmax, &nf, &len, &used);
         if (rc) return rc;
         for (uint32_t i = 0; i < nf; i++) { rc = zk_seek_table_log_frame(&raw.seek_table, cs[i], ds[i]); if (rc) return rc; }
@@ -431,8 +437,9 @@ struct zk_encoder {
 
 extern "C" int32_t zk_encode_options_into_encoder(zk_encode_options* o, zk_write_fn write, zk_flush_fn flush, void* user, zk_encoder** out) {
     if (!o || !out || !write) return ZK_ERR_INVALID_ARG;
-    // the exact cut of Compressed(n) needs a bounded history per block, which the tier that matches over long distances does not have
-    if (o->kind == ZK_POLICY_COMPRESSED && o->ldm) return ZK_ERR_INVALID_ARG;
+    // the exact cut of Compressed(n) needs a bounded history per block, which the tier that matches over long distances does not have;
+    // content-defined frames are meant to stand alone
+    if ((o->kind == ZK_POLICY_COMPRESSED || o->kind == ZK_POLICY_CONTENT) && o->ldm) return ZK_ERR_INVALID_ARG;
     zk_encoder* e = new (std::nothrow) zk_encoder();
     if (!e) return ZK_ERR_ZSTD(64);
     e->raw.ctx = o->ctx; e->raw.kind = o->kind; e->raw.size = o->size; e->raw.checksum = o->checksum; e->raw.level = o->level; e->raw.ldm = o->ldm;
@@ -456,14 +463,14 @@ extern "C" int32_t zk_encoder_compress_with_prefix(zk_encoder* e, const uint8_t*
     if (prefix != e->prefix || prefix_len != e->prefix_len) {
         // the batch buffer holds frames of ONE prefix: close what was buffered under the previous one first (whole frames only;
         // a partial frame keeps the prefix it started with, as in the reference)
-        if (e->raw.kind != ZK_POLICY_COMPRESSED && !e->batch.empty()) {
+        if (!e->cuts_on_gpu() && !e->batch.empty()) {
             const uint32_t fs0 = e->frame_limit();
             const size_t whole = fs0 ? (e->batch.size() / fs0) * fs0 : 0;
             if (whole && whole == e->batch.size()) { int32_t rc = e->flush_batch(whole, nullptr, false); if (rc) return rc; }
         }
         if (e->batch.empty()) { e->prefix = prefix; e->prefix_len = prefix_len; }
     }
-    if (e->raw.kind == ZK_POLICY_COMPRESSED) {
+    if (e->cuts_on_gpu()) {
         e->batch.insert(e->batch.end(), buf, buf + len);
         if (e->batch.size() >= e->csize_at) { int32_t rc = e->flush_csize(0, nullptr); if (rc) return rc; }
         if (consumed) *consumed = len;
@@ -482,7 +489,7 @@ extern "C" int32_t zk_encoder_compress_with_prefix(zk_encoder* e, const uint8_t*
 }
 
 extern "C" int32_t zk_encoder_end_frame(zk_encoder* e, size_t* written) {                                      // :704-717
-    if (e->raw.kind == ZK_POLICY_COMPRESSED) return e->flush_csize(1, written);
+    if (e->cuts_on_gpu()) return e->flush_csize(1, written);
     // everything buffered becomes frames; the last one may be short (or empty: end_frame on a fresh frame emits an
     // empty frame, exactly what the reference's finish() does on an empty stream)
     return e->flush_batch(e->batch.size(), written, true);

@@ -130,6 +130,23 @@ class DeviceCodec:
         self.device_ms += self.ctx.last_device_ms
         return dst[: int(dl.value)], cs[: nf.value].astype(np.int64), ds[: nf.value].astype(np.int64), int(used.value)
 
+    def compress_cdc(self, x: torch.Tensor, size: int, level: int, checksum: bool, final: bool = True):
+        """FrameSizePolicy::ContentDefined(size) (zk_compress_frames_cdc_dev) -> (frames, c_sizes, d_sizes, consumed)"""
+        n = x.numel()
+        src = torch.cat([x, torch.zeros(self.PAD, dtype=torch.uint8, device=x.device)])
+        cap = self.compress_bound(n, 1024)
+        dst = self.empty(cap, x.device)
+        nfmax = n // 1024 + 1
+        cs = np.zeros(nfmax, dtype=np.uint32); ds = np.zeros(nfmax, dtype=np.uint32)
+        nf = ctypes.c_uint32(); dl = ctypes.c_size_t(); used = ctypes.c_size_t()
+        rc = self.lib.zk_compress_frames_cdc_dev(self.ctx._h, src.data_ptr(), n, size, level, int(checksum), int(final), dst.data_ptr(), cap,
+                                                 cs.ctypes.data_as(_native.u32p), ds.ctypes.data_as(_native.u32p), nfmax, ctypes.byref(nf),
+                                                 ctypes.byref(dl), ctypes.byref(used), torch_stream_handle(x.device))
+        if rc:
+            raise RuntimeError(f"zk_compress_frames_cdc_dev: {rc}")
+        self.device_ms += self.ctx.last_device_ms
+        return dst[: int(dl.value)], cs[: nf.value].astype(np.int64), ds[: nf.value].astype(np.int64), int(used.value)
+
     def decompress(self, comp: torch.Tensor, c_off, d_off, verify: bool):
         src = torch.cat([comp, torch.zeros(self.PAD, dtype=torch.uint8, device=comp.device)])
         out = self.empty(int(c_off[-1] * 0 + d_off[-1]), comp.device)
