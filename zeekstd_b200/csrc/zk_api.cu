@@ -14,11 +14,6 @@ void zk_note_cuda_error(const char* what, int code) {
     snprintf(zk_tls_cuda_msg, sizeof zk_tls_cuda_msg, "%s: %s", what, cudaGetErrorString((cudaError_t)code));
 }
 extern "C" const char* zk_last_cuda_error(void) { return zk_tls_cuda_msg; }
-#ifndef ZK_EMUL
-#define ZK_RT_OK(x) do { cudaError_t e__ = (x); if (e__ != cudaSuccess) { zk_note_cuda_error(#x, (int)e__); (void)cudaGetLastError(); return ZK_ERR_CUDA; } } while (0)
-#else
-#define ZK_RT_OK(x) do { (void)(x); } while (0)
-#endif
 
 static int zk_host_slots(bool enc);
 static size_t zk_env_size(const char* name, size_t dflt) {
@@ -71,21 +66,8 @@ extern "C" const char* zk_error_name(int32_t rc) {
 }
 
 int zk_slot_ensure(ZkSlot* s, size_t need_in, size_t need_out) {
-    if (s->cap_in < need_in) {
-        if (s->d_in) cudaFree(s->d_in);
-        s->d_in = nullptr; s->cap_in = 0;
-        size_t want = need_in + need_in / 8 + 256;
-        if (cudaMalloc((void**)&s->d_in, want) != cudaSuccess) return ZK_ERR_ZSTD(ZKZ_MEMORY_ALLOCATION);
-        s->cap_in = want;
-    }
-    if (s->cap_out < need_out) {
-        if (s->d_out) cudaFree(s->d_out);
-        s->d_out = nullptr; s->cap_out = 0;
-        size_t want = need_out + need_out / 8 + 256;
-        if (cudaMalloc((void**)&s->d_out, want) != cudaSuccess) return ZK_ERR_ZSTD(ZKZ_MEMORY_ALLOCATION);
-        s->cap_out = want;
-    }
-    return 0;
+    const int rc = zk_grow((void**)&s->d_in, &s->cap_in, need_in, 1);
+    return rc ? rc : zk_grow((void**)&s->d_out, &s->cap_out, need_out, 1);
 }
 
 extern "C" int32_t zk_ctx_create(int32_t device_ordinal, uint32_t flags, zk_ctx** out) {
@@ -95,9 +77,9 @@ extern "C" int32_t zk_ctx_create(int32_t device_ordinal, uint32_t flags, zk_ctx*
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { (void)cudaGetLastError(); return ZK_ERR_NO_DEVICE; }
     if (device_ordinal < 0 || device_ordinal >= ndev) return ZK_ERR_INVALID_ARG;
-    ZK_RT_OK(cudaSetDevice(device_ordinal));
+    ZK_CUDA_OK(cudaSetDevice(device_ordinal));
     cudaDeviceProp prop;
-    ZK_RT_OK(cudaGetDeviceProperties(&prop, device_ordinal));
+    ZK_CUDA_OK(cudaGetDeviceProperties(&prop, device_ordinal));
     zk_ctx* c = new zk_ctx();
     c->device = device_ordinal;
     c->sm_count = prop.multiProcessorCount > 0 ? prop.multiProcessorCount : 132;
@@ -172,6 +154,28 @@ extern "C" void zk_ctx_profile_read(const zk_ctx* c, float* ms, uint32_t* launch
     }
 }
 
+
+// ---------------------------------------------------------------------------------------------
+// prefix / patch mode (SURVEY.md 8f.3): every frame is coded against the same raw-content prefix
+//   RawEncoder::compress_with_prefix   encode.rs:311-338  (cctx.ref_prefix at the start of every frame)
+//   Decoder::decompress_with_prefix    decode.rs:201-214, 246-255  (dctx.ref_prefix before the first frame and after every frame end)
+// The prefix is uploaded once per call and stays resident; K-C1 searches its tail from the first block of every frame, K-D2
+// resolves offsets that reach before a frame's first byte into it.
+// ---------------------------------------------------------------------------------------------
+// the prefix of one call (host memory; nullptr or len 0: none) -> its device copy *d_prefix, *d_len (nullptr, 0: none)
+static int32_t zk_upload_prefix(zk_ctx* c, const uint8_t* prefix, size_t len, const uint8_t** d_prefix, uint32_t* d_len) {
+    *d_prefix = nullptr; *d_len = 0;
+    if (!prefix || len == 0) return 0;
+    if (len > 0x7FFFFFFFull) return ZK_ERR_INVALID_ARG;
+    ZK_CUDA_OK(cudaSetDevice(c->device));
+    const int32_t rc = zk_grow(&c->d_prefix, &c->cap_prefix, len + 64, 1);
+    if (rc) return rc;
+    for (int i = 0; i < ZK_SLOTS; i++) if (c->slot[i].stream) cudaStreamSynchronize(c->slot[i].stream);    // nobody reads the old prefix any more
+    ZK_CUDA_OK(cudaMemcpy(c->d_prefix, prefix, len, cudaMemcpyHostToDevice));
+    *d_prefix = (const uint8_t*)c->d_prefix; *d_len = (uint32_t)len;
+    return 0;
+}
+
 // ---------------------------------------------------------------------------------------------
 // decompress
 // ---------------------------------------------------------------------------------------------
@@ -186,18 +190,17 @@ extern "C" int32_t zk_decompress_frames_dev(zk_ctx* c, const void* d_comp, const
                                             uint32_t n, void* d_dst, int32_t verify, int32_t* status, void* cuda_stream) {
     if (!c || (n && (!d_comp || !c_off || !d_off || !d_dst))) return ZK_ERR_INVALID_ARG;
     if (n == 0) return 0;
-    ZK_RT_OK(cudaSetDevice(c->device));
+    ZK_CUDA_OK(cudaSetDevice(c->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : c->slot[0].stream;
     const size_t sub_bytes = zk_env_size("ZK_DEV_SUB_BYTES", (size_t)1 << 30);
-    ZkDecodeWs* ws = &c->slot[0].dws;
-    ws->share = 1; ws->no_side = zk_env_size("ZK_DEV_SIDE", 1) == 0;
-    ws->up = ws->down = nullptr;                           // device-resident data: nothing to copy but offsets and statuses
+    ZkDecodeParams p;                                       // device-resident data: nothing to copy but offsets and statuses
+    p.side = zk_env_size("ZK_DEV_SIDE", 1) != 0;
     cudaEventRecord(c->ev0, st);
     int32_t worst = 0;
     for (uint32_t first = 0; first < n;) {
         uint32_t end = zk_next_sub(d_off, first, n, sub_bytes, 1u << 20);
-        int rc = zk_decode_batch(ws, st, (const uint8_t*)d_comp, c_off + first, d_off + first, end - first, (uint8_t*)d_dst,
-                                 verify, status ? status + first : nullptr);
+        int rc = zk_decode_batch(&c->slot[0].dws, st, (const uint8_t*)d_comp, c_off + first, d_off + first, end - first, (uint8_t*)d_dst,
+                                 verify, p, status ? status + first : nullptr);
         if (rc && !worst) worst = rc;
         if (rc == ZK_INT_CUDA || rc == -(int)ZKZ_MEMORY_ALLOCATION) return rc;
         first = end;
@@ -233,45 +236,47 @@ struct ZkTrace {
     }
 };
 
+// one host-pointer decompress call
+struct ZkDecCall {
+    const uint8_t* comp; const uint64_t* c_off; const uint64_t* d_off; uint8_t* dst; int verify; int32_t* status;
+    ZkDecodeParams p;                                       // p.need: the whole call's
+};
 struct ZkSubDec { uint32_t first = 0, count = 0; std::vector<uint64_t> c_rel, d_rel; bool busy = false; };
 
-static int zk_dec_sub_enqueue(zk_ctx* c, int si, ZkSubDec& sb, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off,
-                              uint8_t* dst, int verify, ZkTrace* tr = nullptr, int k = 0, const uint32_t* need = nullptr) {
+static int zk_dec_sub_enqueue(zk_ctx* c, int si, ZkSubDec& sb, const ZkDecCall& q, ZkTrace* tr = nullptr, int k = 0) {
     ZkSlot& s = c->slot[si];
     uint32_t f = sb.first, cnt = sb.count;
+    const uint64_t* c_off = q.c_off; const uint64_t* d_off = q.d_off;
     size_t cbytes = (size_t)(c_off[f + cnt] - c_off[f]), obytes = (size_t)(d_off[f + cnt] - d_off[f]);
     int rc = zk_slot_ensure(&s, cbytes + 32, obytes + 32);
     if (rc) return rc;
     sb.c_rel.resize(cnt + 1); sb.d_rel.resize(cnt + 1);
     for (uint32_t j = 0; j <= cnt; j++) { sb.c_rel[j] = c_off[f + j] - c_off[f]; sb.d_rel[j] = d_off[f + j] - d_off[f]; }
-    cudaStream_t us = c->up ? c->up : s.stream, ds = c->down ? c->down : s.stream;
-    s.dws.up = c->up; s.dws.down = c->down;
+    cudaStream_t us = q.p.up ? q.p.up : s.stream, ds = q.p.down ? q.p.down : s.stream;
     if (tr) tr->mark(us, k, 0);
-    ZK_RT_OK(cudaMemcpyAsync(s.d_in, comp + c_off[f], cbytes, cudaMemcpyHostToDevice, us));
+    ZK_CUDA_OK(cudaMemcpyAsync(s.d_in, q.comp + c_off[f], cbytes, cudaMemcpyHostToDevice, us));
     if (tr) tr->mark(us, k, 1);
-    s.dws.no_side = zk_env_size("ZK_HOST_SIDE", 1) == 0;
-    s.dws.share = (int)zk_env_size("ZK_HOST_SHARE", 3);
-    s.dws.need = need ? need + f : nullptr;
-    s.dws.prefix = c->cur_prefix_len ? c->d_prefix : nullptr; s.dws.prefix_len = c->cur_prefix_len;
-    rc = zk_decode_enqueue(&s.dws, s.stream, s.d_in, sb.c_rel.data(), sb.d_rel.data(), cnt, s.d_out, verify);
+    ZkDecodeParams p = q.p;
+    if (p.need) p.need += f;
+    rc = zk_decode_enqueue(&s.dws, s.stream, s.d_in, sb.c_rel.data(), sb.d_rel.data(), cnt, s.d_out, q.verify, p);
     if (rc) return rc;
     if (tr) tr->mark(s.stream, k, 2);
-    if (obytes) ZK_RT_OK(cudaMemcpyAsync(dst + d_off[f], s.d_out, obytes, cudaMemcpyDeviceToHost, ds));
-    if (ds != s.stream) ZK_RT_OK(cudaEventRecord(s.dws.ev_down, ds));        // what zk_decode_collect waits for
+    if (obytes) ZK_CUDA_OK(cudaMemcpyAsync(q.dst + d_off[f], s.d_out, obytes, cudaMemcpyDeviceToHost, ds));
+    if (ds != s.stream) ZK_CUDA_OK(cudaEventRecord(s.dws.ev_down, ds));        // what zk_decode_collect waits for
     if (tr) tr->mark(ds, k, 4);
     sb.busy = true;
     return 0;
 }
 
-static int zk_dec_sub_finish(zk_ctx* c, int si, ZkSubDec& sb, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off,
-                             uint8_t* dst, int verify, int32_t* status, const uint32_t* need = nullptr) {
+static int zk_dec_sub_finish(zk_ctx* c, int si, ZkSubDec& sb, const ZkDecCall& q) {
     ZkSlot& s = c->slot[si];
     if (!sb.busy) return 0;
-    int rc = zk_decode_collect(&s.dws, s.stream, status ? status + sb.first : nullptr);
+    int32_t* status = q.status ? q.status + sb.first : nullptr;
+    int rc = zk_decode_collect(&s.dws, s.stream, q.p, status);
     if (rc == ZK_ST_RETRY) {            // scratch was too small for this sub-batch: exact needs are known now
-        rc = zk_dec_sub_enqueue(c, si, sb, comp, c_off, d_off, dst, verify, nullptr, 0, need);
+        rc = zk_dec_sub_enqueue(c, si, sb, q);
         if (rc) { sb.busy = false; return rc; }
-        rc = zk_decode_collect(&s.dws, s.stream, status ? status + sb.first : nullptr);
+        rc = zk_decode_collect(&s.dws, s.stream, q.p, status);
         if (rc == ZK_ST_RETRY) rc = ZK_ERR_ZSTD(ZKZ_MEMORY_ALLOCATION);
     }
     sb.busy = false;
@@ -285,10 +290,24 @@ extern "C" int32_t zk_decompress_frames(zk_ctx* c, const uint8_t* comp, const ui
 
 extern "C" int32_t zk_decompress_frames_upto(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off,
                                              uint32_t n, uint8_t* dst, const uint32_t* d_need, int32_t verify, int32_t* status) {
-    if (!c || (n && (!comp || !c_off || !d_off || !dst))) return ZK_ERR_INVALID_ARG;
+    return zk_decompress_frames_prefix(c, comp, c_off, d_off, n, dst, d_need, verify, status, nullptr, 0);
+}
+
+extern "C" int32_t zk_decompress_frames_prefix(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n,
+                                               uint8_t* dst, const uint32_t* d_need, int32_t verify, int32_t* status,
+                                               const uint8_t* prefix, size_t prefix_len) {
+    if (!c) return ZK_ERR_INVALID_ARG;
+    ZkDecCall q = {comp, c_off, d_off, dst, verify, status, ZkDecodeParams()};
+    int32_t rc = zk_upload_prefix(c, prefix, prefix_len, &q.p.prefix, &q.p.prefix_len);
+    if (rc) return rc;
+    if (n && (!comp || !c_off || !d_off || !dst)) return ZK_ERR_INVALID_ARG;
     if (n == 0) return 0;
-    ZK_RT_OK(cudaSetDevice(c->device));
+    ZK_CUDA_OK(cudaSetDevice(c->device));
     const size_t sub_bytes = zk_env_size("ZK_HOST_SUB_BYTES", (size_t)128 << 20);     // tuning knob (tools/e2e_sweep2.sh sweeps it)
+    q.p.need = d_need;
+    q.p.share = (int)zk_env_size("ZK_HOST_SHARE", 3);
+    q.p.side = zk_env_size("ZK_HOST_SIDE", 1) != 0;
+    q.p.up = c->up; q.p.down = c->down;
     ZkSubDec sub[ZK_SLOTS];
     const int NS = zk_host_slots(false);
     const uint32_t ramp = (uint32_t)zk_env_size("ZK_HOST_RAMP", 0);            // the first `ramp` sub-batches are 1/2^ramp ... 1/2 of the full size
@@ -297,7 +316,7 @@ extern "C" int32_t zk_decompress_frames_upto(zk_ctx* c, const uint8_t* comp, con
     ZkTrace tr; tr.begin(c->slot[0].stream);
     for (uint32_t first = 0; first < n; k++) {
         int si = (int)(k % NS);
-        int rc = zk_dec_sub_finish(c, si, sub[si], comp, c_off, d_off, dst, verify, status, d_need);
+        rc = zk_dec_sub_finish(c, si, sub[si], q);
         if (rc && !worst) worst = rc;
         // ZK_HOST_RAMP=r (default 0): the first r sub-batches are 1/2^r ... 1/2 of the full size, so that the output copy could start
         // earlier.  It gave no gain when it was tried: a sub-batch of any size spends about one frame latency in
@@ -305,12 +324,12 @@ extern "C" int32_t zk_decompress_frames_upto(zk_ctx* c, const uint8_t* comp, con
         const size_t this_sub = k < ramp ? sub_bytes >> (ramp - k) : sub_bytes;
         uint32_t end = zk_next_sub(d_off, first, n, this_sub, 1u << 20);
         sub[si].first = first; sub[si].count = end - first;
-        rc = zk_dec_sub_enqueue(c, si, sub[si], comp, c_off, d_off, dst, verify, &tr, (int)k, d_need);
+        rc = zk_dec_sub_enqueue(c, si, sub[si], q, &tr, (int)k);
         if (rc) { if (!worst) worst = rc; break; }
         first = end;
     }
     for (int si = 0; si < ZK_SLOTS; si++) {
-        int rc = zk_dec_sub_finish(c, si, sub[si], comp, c_off, d_off, dst, verify, status, d_need);
+        rc = zk_dec_sub_finish(c, si, sub[si], q);
         if (rc && !worst) worst = rc;
     }
     tr.end("dec");
@@ -318,58 +337,34 @@ extern "C" int32_t zk_decompress_frames_upto(zk_ctx* c, const uint8_t* comp, con
 }
 
 // ---------------------------------------------------------------------------------------------
-// compress
+// compress: every entry point describes its call as a ZkCompressReq, and zk_compress runs it
 // ---------------------------------------------------------------------------------------------
-static uint32_t zk_frames_of(size_t n, uint32_t frame_size) {
-    if (n == 0) return 1;                                   // Encoder::finish() always closes one frame (encode.rs:755-756)
-    return (uint32_t)((n + frame_size - 1) / frame_size);
-}
+enum ZkPolicy { ZK_FRAMES_UNIFORM, ZK_FRAMES_SIZED, ZK_FRAMES_COMPRESSED, ZK_FRAMES_CONTENT };
 
-// The frames of one compress call: the caller's sizes, or the uniform layout (frame_size bytes each, the last frame shorter, one empty
-// frame of no input).  Both pipelines below cut it into sub-batches of whole consecutive frames.
-struct ZkFrameList {
-    const uint32_t* sizes;                                  // nullptr: uniform
-    size_t n; uint32_t frame_size, count;
-    uint32_t size(uint32_t f) const {
-        if (sizes) return sizes[f];
-        const size_t lo = (size_t)f * frame_size;
-        return (uint32_t)(n - lo < frame_size ? n - lo : frame_size);
-    }
-    // the sub-batch from frame f0: as many frames as fit max_bytes of input, at least one -> its end frame; *bytes: its input
-    uint32_t next_sub(uint32_t f0, size_t max_bytes, size_t* bytes) const {
-        size_t b = size(f0); uint32_t e = f0 + 1;
-        if (!sizes) {                                       // frames before the last are full: the same rule in closed form
-            const uint32_t per = frame_size <= max_bytes ? (uint32_t)(max_bytes / frame_size) : 1u;
-            e = count - f0 < per ? count : f0 + per;
-            b = (e == count ? n : (size_t)e * frame_size) - (size_t)f0 * frame_size;
-            if (e < count && b + size(e) <= max_bytes) { b += size(e); e++; }   // a short last frame that still fits
-        } else while (e < count && b + sizes[e] <= max_bytes) b += sizes[e++];
-        *bytes = b;
-        return e;
-    }
-    size_t bound(uint32_t f0, uint32_t cnt, size_t bytes) const {
-        return sizes ? zk_encode_bound_sized(sizes + f0, cnt) : zk_encode_bound(bytes, frame_size);
-    }
-    int enqueue(ZkEncodeWs* ws, cudaStream_t st, const uint8_t* d_in, uint32_t f0, uint32_t cnt, size_t bytes, int32_t level, int32_t checksum,
-                uint8_t* d_out, size_t cap) const {
-        return sizes ? zk_encode_enqueue_sized(ws, st, d_in, sizes + f0, cnt, level, checksum, d_out, cap)
-                     : zk_encode_enqueue(ws, st, d_in, bytes, frame_size, level, checksum, d_out, cap, cnt);
-    }
+struct ZkCompressReq {
+    ZkPolicy policy = ZK_FRAMES_UNIFORM;
+    uint32_t size = 0;                                      // uniform: the frame size; Compressed: the target; ContentDefined: the size
+    const uint32_t* sizes = nullptr; uint32_t count = 0;    // sized: the caller's frame sizes
+    const uint8_t* src = nullptr; size_t n = 0;
+    bool host = true;                                       // src and dst in host memory; else device memory, worked on `stream`
+    cudaStream_t stream = nullptr;                          // nullptr: slot 0's
+    const uint8_t* prefix = nullptr; size_t prefix_len = 0; // host memory
+    ZkEncodeParams params;                                  // its prefix: the device copy of `prefix`
+    int32_t final_ = 1;                                     // Compressed / ContentDefined: no more input follows this call's
+    uint8_t* dst = nullptr; size_t dst_cap = 0;
+    uint32_t* c_sizes = nullptr; uint32_t* d_sizes = nullptr; uint32_t frames_cap = 0; uint32_t* n_frames = nullptr;
+    size_t* dst_len = nullptr; size_t* consumed = nullptr;
 };
 
-// device-resident input and output: sub-batches of at most sub_bytes input (which bound the scratch, about 4x that) one after the other on
-// st, every frame with the prefix d_prefix (device memory; nullptr: none) -> *dst_len
-static int32_t zk_compress_dev_subs(zk_ctx* c, const ZkFrameList& fl, const uint8_t* d_src, const uint8_t* d_prefix, uint32_t prefix_len,
-                                    int32_t level, int32_t checksum, uint8_t* d_dst, size_t dst_cap, uint32_t* c_sizes, size_t* dst_len,
-                                    cudaStream_t st, size_t sub_bytes) {
+// device-resident input and output: sub-batches of at most sub_bytes input (which bound the scratch, about 4x that) one after the other on st
+static int32_t zk_compress_dev_subs(zk_ctx* c, const ZkFrames& fr, const uint8_t* d_src, const ZkEncodeParams& p, uint8_t* d_dst,
+                                    size_t dst_cap, uint32_t* c_sizes, size_t* dst_len, cudaStream_t st, size_t sub_bytes) {
     size_t out_pos = 0, in_off = 0;
-    for (uint32_t f0 = 0; f0 < fl.count;) {
+    for (uint32_t f0 = 0; f0 < fr.count;) {
         size_t in_len = 0;
-        const uint32_t end = fl.next_sub(f0, sub_bytes, &in_len);
+        const uint32_t end = fr.next_sub(f0, sub_bytes, &in_len);
         size_t produced = 0;
-        c->slot[0].ews.no_side = false;
-        c->slot[0].ews.prefix = d_prefix; c->slot[0].ews.prefix_len = prefix_len;
-        int rc = fl.enqueue(&c->slot[0].ews, st, d_src + in_off, f0, end - f0, in_len, level, checksum, d_dst + out_pos, dst_cap - out_pos);
+        int rc = zk_encode_enqueue(&c->slot[0].ews, st, d_src + in_off, fr.sub(f0, end - f0, in_len), p, d_dst + out_pos, dst_cap - out_pos);
         if (!rc) rc = zk_encode_collect(&c->slot[0].ews, st, c_sizes ? c_sizes + f0 : nullptr, &produced);
         if (rc) return rc;
         out_pos += produced; in_off += in_len; f0 = end;
@@ -378,49 +373,17 @@ static int32_t zk_compress_dev_subs(zk_ctx* c, const ZkFrameList& fl, const uint
     return 0;
 }
 
-static int32_t zk_compress_dev_run(zk_ctx* c, const ZkFrameList& fl, const uint8_t* d_src, int32_t level, int32_t checksum, uint8_t* d_dst,
-                                   size_t dst_cap, uint32_t* c_sizes, size_t* dst_len, cudaStream_t st) {
-    const size_t sub_bytes = zk_env_size("ZK_DEV_SUB_BYTES", (size_t)1 << 30);
-    cudaEventRecord(c->ev0, st);
-    size_t out_pos = 0;
-    const int32_t rc = zk_compress_dev_subs(c, fl, d_src, nullptr, 0, level, checksum, d_dst, dst_cap, c_sizes, &out_pos, st, sub_bytes);
-    if (rc) return rc;
-    cudaEventRecord(c->ev1, st);
-    cudaEventSynchronize(c->ev1);
-    cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1);
-    if (dst_len) *dst_len = out_pos;
-    return 0;
-}
-
-extern "C" int32_t zk_compress_frames_dev(zk_ctx* c, const void* d_src, size_t n, uint32_t frame_size, int32_t level, int32_t checksum,
-                                          void* d_dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap,
-                                          uint32_t* n_frames, size_t* dst_len, void* cuda_stream) {
-    if (!c || !d_dst || (n && !d_src) || frame_size == 0) return ZK_ERR_INVALID_ARG;
-    if (frame_size > ZK_SEEKABLE_MAX_FRAME_SIZE) frame_size = ZK_SEEKABLE_MAX_FRAME_SIZE;       // encode.rs:531-534
-    if ((n + frame_size - 1) / frame_size > ZK_SEEKABLE_MAX_FRAMES) return ZK_ERR_FRAME_INDEX_TOO_LARGE;
-    const ZkFrameList fl = {nullptr, n, frame_size, zk_frames_of(n, frame_size)};
-    if (fl.count > frames_cap) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
-    ZK_RT_OK(cudaSetDevice(c->device));
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : c->slot[0].stream;
-    const int32_t rc = zk_compress_dev_run(c, fl, (const uint8_t*)d_src, level, checksum, (uint8_t*)d_dst, dst_cap, c_sizes, dst_len, st);
-    if (rc) return rc;
-    if (d_sizes) for (uint32_t f = 0; f < fl.count; f++) d_sizes[f] = fl.size(f);
-    if (n_frames) *n_frames = fl.count;
-    return 0;
-}
-
 struct ZkSubEnc { uint32_t f0 = 0, cnt = 0; size_t in_off = 0, in_len = 0, out_pos = 0; bool busy = false; };
 
-// host input and output (prefix: the context's current one): sub-batches on up to ZK_HOST_SLOTS_ENC slots, output placed in order
-static int32_t zk_compress_host_run(zk_ctx* c, const ZkFrameList& fl, const uint8_t* src, int32_t level, int32_t checksum, uint8_t* dst,
-                                    size_t dst_cap, uint32_t* c_sizes, size_t* dst_len) {
-    ZK_RT_OK(cudaSetDevice(c->device));
-    const size_t sub_bytes = zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20);    // tuning knob (tools/knobs_round.sh sweeps it)
+// host input and output: sub-batches on up to ZK_HOST_SLOTS_ENC slots, output placed in order
+static int32_t zk_compress_host_run(zk_ctx* c, const ZkFrames& fr, const ZkCompressReq& q, size_t sub_bytes, size_t* dst_len) {
+    ZkEncodeParams p = q.params;
+    p.side = zk_env_size("ZK_HOST_SIDE", 1) != 0;
     // The compressed size of a sub-batch is only known when it completes, so output positions are assigned in
     // order at completion time: H2D and kernels of later sub-batches overlap the D2H of earlier ones.
     ZkSubEnc sub[ZK_SLOTS];
     size_t out_pos = 0, in_off = 0; int32_t err = 0;
-    std::vector<uint32_t> tmp_sizes(c_sizes ? 0 : fl.count);
+    std::vector<uint32_t> tmp_sizes(q.c_sizes ? 0 : fr.count);
     ZkTrace tr; tr.begin(c->slot[0].stream);
     int sub_k[ZK_SLOTS] = {0};
     auto finish = [&](int si) -> int {
@@ -428,11 +391,11 @@ static int32_t zk_compress_host_run(zk_ctx* c, const ZkFrameList& fl, const uint
         if (!sb.busy) return 0;
         sb.busy = false;
         size_t produced = 0;
-        int rc = zk_encode_collect(&s.ews, s.stream, (c_sizes ? c_sizes : tmp_sizes.data()) + sb.f0, &produced);
+        int rc = zk_encode_collect(&s.ews, s.stream, (q.c_sizes ? q.c_sizes : tmp_sizes.data()) + sb.f0, &produced);
         if (rc) return rc;
-        if (out_pos + produced > dst_cap) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
+        if (out_pos + produced > q.dst_cap) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
         tr.mark(s.stream, sub_k[si], 3);
-        if (cudaMemcpyAsync(dst + out_pos, s.d_out, produced, cudaMemcpyDeviceToHost, s.stream) != cudaSuccess) return ZK_ERR_CUDA;
+        if (cudaMemcpyAsync(q.dst + out_pos, s.d_out, produced, cudaMemcpyDeviceToHost, s.stream) != cudaSuccess) return ZK_ERR_CUDA;
         tr.mark(s.stream, sub_k[si], 4);
         out_pos += produced;
         return 0;
@@ -440,7 +403,7 @@ static int32_t zk_compress_host_run(zk_ctx* c, const ZkFrameList& fl, const uint
     uint32_t k = 0;
     const int NS = zk_host_slots(true);
     int n_inflight = 0;                                     // completion must follow submission order
-    for (uint32_t f0 = 0; f0 < fl.count && !err; k++) {
+    for (uint32_t f0 = 0; f0 < fr.count && !err; k++) {
         const int si = (int)(k % NS);
         if (n_inflight == NS) {                             // oldest in flight is exactly slot si
             err = finish(si); n_inflight--;
@@ -448,18 +411,16 @@ static int32_t zk_compress_host_run(zk_ctx* c, const ZkFrameList& fl, const uint
         }
         ZkSlot& s = c->slot[si]; ZkSubEnc& sb = sub[si];
         if (cudaStreamSynchronize(s.stream) != cudaSuccess) { err = ZK_ERR_CUDA; break; }   // its previous D2H must be done before d_out is reused
-        const uint32_t end = fl.next_sub(f0, sub_bytes, &sb.in_len);
+        const uint32_t end = fr.next_sub(f0, sub_bytes, &sb.in_len);
         sb.f0 = f0; sb.cnt = end - f0; sb.in_off = in_off;
-        const size_t bound = fl.bound(f0, sb.cnt, sb.in_len);
+        const ZkFrames sf = fr.sub(f0, sb.cnt, sb.in_len);
+        const size_t bound = sf.bound();
         int rc = zk_slot_ensure(&s, sb.in_len + 32, bound + 32);
         if (rc) { err = rc; break; }
         sub_k[si] = (int)k; tr.mark(s.stream, (int)k, 0);
-        if (sb.in_len && cudaMemcpyAsync(s.d_in, src + sb.in_off, sb.in_len, cudaMemcpyHostToDevice, s.stream) != cudaSuccess) { err = ZK_ERR_CUDA; break; }
+        if (sb.in_len && cudaMemcpyAsync(s.d_in, q.src + sb.in_off, sb.in_len, cudaMemcpyHostToDevice, s.stream) != cudaSuccess) { err = ZK_ERR_CUDA; break; }
         tr.mark(s.stream, (int)k, 1);
-        s.ews.no_side = zk_env_size("ZK_HOST_SIDE", 1) == 0;
-        s.ews.prefix = c->cur_prefix_len ? c->d_prefix : nullptr; s.ews.prefix_len = c->cur_prefix_len;
-        s.ews.ldm = c->cur_ldm;
-        rc = fl.enqueue(&s.ews, s.stream, s.d_in, f0, sb.cnt, sb.in_len, level, checksum, s.d_out, bound);
+        rc = zk_encode_enqueue(&s.ews, s.stream, s.d_in, sf, p, s.d_out, bound);
         if (rc) { err = rc; break; }
         tr.mark(s.stream, (int)k, 2);
         sb.busy = true; n_inflight++;
@@ -474,154 +435,16 @@ static int32_t zk_compress_host_run(zk_ctx* c, const ZkFrameList& fl, const uint
     for (int si = 0; si < ZK_SLOTS; si++) cudaStreamSynchronize(c->slot[si].stream);
     tr.end("enc");
     if (err) return err;
-    if (dst_len) *dst_len = out_pos;
+    *dst_len = out_pos;
     return 0;
-}
-
-extern "C" int32_t zk_compress_frames(zk_ctx* c, const uint8_t* src, size_t n, uint32_t frame_size, int32_t level, int32_t checksum,
-                                      uint8_t* dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap,
-                                      uint32_t* n_frames, size_t* dst_len) {
-    if (!c || !dst || (n && !src) || frame_size == 0) return ZK_ERR_INVALID_ARG;
-    if (frame_size > ZK_SEEKABLE_MAX_FRAME_SIZE) frame_size = ZK_SEEKABLE_MAX_FRAME_SIZE;
-    if ((n + frame_size - 1) / frame_size > ZK_SEEKABLE_MAX_FRAMES) return ZK_ERR_FRAME_INDEX_TOO_LARGE;
-    const ZkFrameList fl = {nullptr, n, frame_size, zk_frames_of(n, frame_size)};
-    if (fl.count > frames_cap) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
-    const int32_t rc = zk_compress_host_run(c, fl, src, level, checksum, dst, dst_cap, c_sizes, dst_len);
-    if (rc) return rc;
-    if (d_sizes) for (uint32_t f = 0; f < fl.count; f++) d_sizes[f] = fl.size(f);
-    if (n_frames) *n_frames = fl.count;
-    return 0;
-}
-
-// caller-chosen frame sizes: the checks of the header's contract -> the input length, or an error code
-static int32_t zk_sized_check(const uint32_t* frame_sizes, uint32_t n_frames, size_t* n) {
-    if (n_frames > ZK_SEEKABLE_MAX_FRAMES) return ZK_ERR_FRAME_INDEX_TOO_LARGE;
-    *n = 0;
-    for (uint32_t f = 0; f < n_frames; f++) {
-        if (frame_sizes[f] > ZK_SEEKABLE_MAX_FRAME_SIZE) return ZK_ERR_ZSTD(ZKZ_PARAM_OUT_OF_BOUND);
-        *n += frame_sizes[f];
-    }
-    return 0;
-}
-
-extern "C" size_t zk_compress_bound_sized(const uint32_t* frame_sizes, uint32_t n_frames) {
-    return frame_sizes || n_frames == 0 ? zk_encode_bound_sized(frame_sizes, n_frames) : 0;
-}
-
-// ---------------------------------------------------------------------------------------------
-// prefix / patch mode (SURVEY.md 8f.3): every frame is coded against the same raw-content prefix
-//   RawEncoder::compress_with_prefix   encode.rs:311-338  (cctx.ref_prefix at the start of every frame)
-//   Decoder::decompress_with_prefix    decode.rs:201-214, 246-255  (dctx.ref_prefix before the first frame and after every frame end)
-// The prefix is uploaded once per call and stays resident; K-C1 searches its tail from the first block of every frame, K-D2
-// resolves offsets that reach before a frame's first byte into it.
-// ---------------------------------------------------------------------------------------------
-static int32_t zk_ctx_set_prefix(zk_ctx* c, const uint8_t* prefix, size_t len) {
-    c->cur_prefix_len = 0;
-    if (!prefix || len == 0) return 0;
-    if (len > 0x7FFFFFFFull) return ZK_ERR_INVALID_ARG;
-    ZK_RT_OK(cudaSetDevice(c->device));
-    if (c->cap_prefix < len + 64) {
-        if (c->d_prefix) cudaFree(c->d_prefix);
-        c->d_prefix = nullptr; c->cap_prefix = 0;
-        if (cudaMalloc((void**)&c->d_prefix, len + len / 8 + 256) != cudaSuccess) return ZK_ERR_ZSTD(ZKZ_MEMORY_ALLOCATION);
-        c->cap_prefix = len + len / 8 + 256;
-    }
-    for (int i = 0; i < ZK_SLOTS; i++) if (c->slot[i].stream) cudaStreamSynchronize(c->slot[i].stream);    // nobody reads the old prefix any more
-    ZK_RT_OK(cudaMemcpy(c->d_prefix, prefix, len, cudaMemcpyHostToDevice));
-    c->cur_prefix_len = (uint32_t)len;
-    return 0;
-}
-
-extern "C" int32_t zk_compress_frames_prefix(zk_ctx* c, const uint8_t* src, size_t n, uint32_t frame_size, int32_t level, int32_t checksum,
-                                             const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap, uint32_t* c_sizes,
-                                             uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len) {
-    if (!c) return ZK_ERR_INVALID_ARG;
-    int32_t rc = zk_ctx_set_prefix(c, prefix, prefix_len);
-    if (rc) return rc;
-    rc = zk_compress_frames(c, src, n, frame_size, level, checksum, dst, dst_cap, c_sizes, d_sizes, frames_cap, n_frames, dst_len);
-    c->cur_prefix_len = 0;
-    return rc;
-}
-
-extern "C" int32_t zk_decompress_frames_prefix(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n,
-                                               uint8_t* dst, const uint32_t* d_need, int32_t verify, int32_t* status,
-                                               const uint8_t* prefix, size_t prefix_len) {
-    if (!c) return ZK_ERR_INVALID_ARG;
-    int32_t rc = zk_ctx_set_prefix(c, prefix, prefix_len);
-    if (rc) return rc;
-    rc = zk_decompress_frames_upto(c, comp, c_off, d_off, n, dst, d_need, verify, status);
-    c->cur_prefix_len = 0;
-    return rc;
-}
-
-// ---------------------------------------------------------------------------------------------
-// caller-chosen frame sizes (Encoder::end_frame at any byte, encode.rs:438-472, as one batch): frame f is what
-// zk_compress_frames_prefix writes for its bytes alone with frame_size = max(size, 1)
-// ---------------------------------------------------------------------------------------------
-extern "C" int32_t zk_compress_frames_sized(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
-                                            int32_t checksum, const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap,
-                                            uint32_t* c_sizes, size_t* dst_len) {
-    if (!c || (n_frames && (!frame_sizes || !dst))) return ZK_ERR_INVALID_ARG;
-    size_t n = 0;
-    int32_t rc = zk_sized_check(frame_sizes, n_frames, &n);
-    if (rc) return rc;
-    if (n && !src) return ZK_ERR_INVALID_ARG;
-    if (dst_len) *dst_len = 0;
-    if (n_frames == 0) return 0;
-    rc = zk_ctx_set_prefix(c, prefix, prefix_len);
-    if (rc) return rc;
-    const ZkFrameList fl = {frame_sizes, n, 0, n_frames};
-    rc = zk_compress_host_run(c, fl, src, level, checksum, dst, dst_cap, c_sizes, dst_len);
-    c->cur_prefix_len = 0;
-    return rc;
-}
-
-// ---------------------------------------------------------------------------------------------
-// long-distance matching (the reference CLI's patch mode: WindowLog + EnableLongDistanceMatching on the CCtx it hands to with_cctx,
-// cli/src/compress.rs:31-37): the prefix calls with K-C1h matching every frame against the whole prefix (zk_ldm.inc)
-// ---------------------------------------------------------------------------------------------
-extern "C" int32_t zk_compress_frames_ldm(zk_ctx* c, const uint8_t* src, size_t n, uint32_t frame_size, int32_t level, int32_t checksum,
-                                          const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap, uint32_t* c_sizes,
-                                          uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len) {
-    if (!c) return ZK_ERR_INVALID_ARG;
-    c->cur_ldm = true;
-    const int32_t rc = zk_compress_frames_prefix(c, src, n, frame_size, level, checksum, prefix, prefix_len, dst, dst_cap, c_sizes, d_sizes, frames_cap,
-                                                 n_frames, dst_len);
-    c->cur_ldm = false;
-    return rc;
-}
-
-extern "C" int32_t zk_compress_frames_sized_ldm(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
-                                                int32_t checksum, const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap,
-                                                uint32_t* c_sizes, size_t* dst_len) {
-    if (!c) return ZK_ERR_INVALID_ARG;
-    c->cur_ldm = true;
-    const int32_t rc = zk_compress_frames_sized(c, src, frame_sizes, n_frames, level, checksum, prefix, prefix_len, dst, dst_cap, c_sizes, dst_len);
-    c->cur_ldm = false;
-    return rc;
-}
-
-extern "C" int32_t zk_compress_frames_sized_dev(zk_ctx* c, const void* d_src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
-                                                int32_t checksum, void* d_dst, size_t dst_cap, uint32_t* c_sizes, size_t* dst_len,
-                                                void* cuda_stream) {
-    if (!c || (n_frames && (!frame_sizes || !d_dst))) return ZK_ERR_INVALID_ARG;
-    size_t n = 0;
-    const int32_t rc = zk_sized_check(frame_sizes, n_frames, &n);
-    if (rc) return rc;
-    if (n && !d_src) return ZK_ERR_INVALID_ARG;
-    if (dst_len) *dst_len = 0;
-    if (n_frames == 0) return 0;
-    ZK_RT_OK(cudaSetDevice(c->device));
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : c->slot[0].stream;
-    const ZkFrameList fl = {frame_sizes, n, 0, n_frames};
-    return zk_compress_dev_run(c, fl, (const uint8_t*)d_src, level, checksum, (uint8_t*)d_dst, dst_cap, c_sizes, dst_len, st);
 }
 
 // ---------------------------------------------------------------------------------------------
 // Frame sizes decided on the GPU (FrameSizePolicy::Compressed and ::ContentDefined): passes over the input, each starting at the first
 // byte the previous one left in an open frame.  A pass starts at the encode sub-batch size and doubles while it closes no frame, up to
 // grow_to, a pass length at which the policy always closes one.  step(d_in, len, at_end, d_out, cap, &r) cuts one pass and compresses the
-// frames it closes to d_out.  min_frame: the fewest bytes of any frame but the last, which bounds a pass's output.
+// frames it closes to d_out.  min_frame: the fewest bytes of any frame but the last, which bounds a pass's output.  The host paths run
+// unpipelined on slot 0.
 // ---------------------------------------------------------------------------------------------
 struct ZkPassOut {
     uint32_t n_frames = 0;
@@ -630,26 +453,24 @@ struct ZkPassOut {
 };
 
 template <class Step>
-static int32_t zk_frame_passes(zk_ctx* c, bool host, const uint8_t* src, size_t n, uint8_t* dst, size_t dst_cap, uint32_t* c_sizes,
-                               uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len, size_t* consumed, cudaStream_t st,
-                               size_t first_pass, size_t grow_to, uint32_t min_frame, const Step& step) {
+static int32_t zk_frame_passes(zk_ctx* c, const ZkCompressReq& q, cudaStream_t st, size_t first_pass, size_t grow_to, uint32_t min_frame,
+                               const Step& step) {
     const size_t block = 32768, max_pass = ZK_SEEKABLE_MAX_FRAME_SIZE;
     first_pass = first_pass / block * block;
     if (first_pass < block) first_pass = block;
     if (first_pass > max_pass) first_pass = max_pass;
     ZkSlot& s = c->slot[0];
-    s.ews.no_side = false;
     size_t pos = 0, out = 0, pass = first_pass;
     uint32_t nf = 0;
-    while (pos < n) {
-        const size_t len = n - pos < pass ? n - pos : pass;
-        const int at_end = pos + len == n;
-        const uint8_t* d_in = src + pos; uint8_t* d_out = dst + out; size_t cap = dst_cap - out;
-        if (host) {
+    while (pos < q.n) {
+        const size_t len = q.n - pos < pass ? q.n - pos : pass;
+        const int at_end = pos + len == q.n;
+        const uint8_t* d_in = q.src + pos; uint8_t* d_out = q.dst + out; size_t cap = q.dst_cap - out;
+        if (q.host) {
             cap = zk_encode_bound(len, min_frame);
             int rc = zk_slot_ensure(&s, len + 32, cap + 32);
             if (rc) return rc;
-            ZK_RT_OK(cudaMemcpyAsync(s.d_in, src + pos, len, cudaMemcpyHostToDevice, st));
+            ZK_CUDA_OK(cudaMemcpyAsync(s.d_in, q.src + pos, len, cudaMemcpyHostToDevice, st));
             d_in = s.d_in; d_out = s.d_out;
         }
         ZkPassOut r;
@@ -660,32 +481,29 @@ static int32_t zk_frame_passes(zk_ctx* c, bool host, const uint8_t* src, size_t 
             pass = 2 * pass < grow_to ? 2 * pass : grow_to;
             continue;
         }
-        if (r.n_frames > frames_cap - nf) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
-        if (host) {
-            if (r.total > dst_cap - out) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
-            ZK_RT_OK(cudaMemcpy(dst + out, s.d_out, r.total, cudaMemcpyDeviceToHost));
+        if (r.n_frames > q.frames_cap - nf) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
+        if (q.host) {
+            if (r.total > q.dst_cap - out) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
+            ZK_CUDA_OK(cudaMemcpy(q.dst + out, s.d_out, r.total, cudaMemcpyDeviceToHost));
         }
-        if (c_sizes) memcpy(c_sizes + nf, r.c_sizes, (size_t)r.n_frames * 4);
-        if (d_sizes) memcpy(d_sizes + nf, r.d_sizes, (size_t)r.n_frames * 4);
+        if (q.c_sizes) memcpy(q.c_sizes + nf, r.c_sizes, (size_t)r.n_frames * 4);
+        if (q.d_sizes) memcpy(q.d_sizes + nf, r.d_sizes, (size_t)r.n_frames * 4);
         nf += r.n_frames; out += r.total; pos += r.consumed;
         pass = first_pass;
     }
-    if (n_frames) *n_frames = nf;
-    if (dst_len) *dst_len = out;
-    if (consumed) *consumed = pos;
+    if (q.n_frames) *q.n_frames = nf;
+    if (q.dst_len) *q.dst_len = out;
+    if (q.consumed) *q.consumed = pos;
     return 0;
 }
 
 // Compressed(target) (zk_encode_csize): the cut and the frames in one step; frames start at 32 KiB blocks
-static int32_t zk_csize_passes(zk_ctx* c, bool host, const uint8_t* src, size_t n, uint32_t target, int32_t level, int32_t checksum,
-                               const uint8_t* d_prefix, uint32_t prefix_len, int32_t final_, uint8_t* dst, size_t dst_cap,
-                               uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len,
-                               size_t* consumed, cudaStream_t st, size_t first_pass) {
+static int32_t zk_csize_passes(zk_ctx* c, const ZkCompressReq& q, cudaStream_t st, size_t first_pass) {
     const size_t block = 32768;
     std::vector<uint32_t> ds;
     auto step = [&](const uint8_t* d_in, size_t len, int at_end, uint8_t* d_out, size_t cap, ZkPassOut* o) -> int32_t {
         ZkCsizeOut r;
-        const int rc = zk_encode_csize(&c->slot[0].ews, st, d_in, len, target, level, checksum, final_, at_end, d_prefix, prefix_len, d_out, cap, &r);
+        const int rc = zk_encode_csize(&c->slot[0].ews, st, d_in, len, q.size, q.params, q.final_, at_end, d_out, cap, &r);
         if (rc) return rc;
         ds.resize(r.n_frames);
         for (uint32_t f = 0; f < r.n_frames; f++) {
@@ -695,120 +513,214 @@ static int32_t zk_csize_passes(zk_ctx* c, bool host, const uint8_t* src, size_t 
         o->n_frames = r.n_frames; o->consumed = r.consumed; o->total = r.total; o->c_sizes = r.c_sizes; o->d_sizes = ds.data();
         return 0;
     };
-    return zk_frame_passes(c, host, src, n, dst, dst_cap, c_sizes, d_sizes, frames_cap, n_frames, dst_len, consumed, st, first_pass,
-                           ZK_SEEKABLE_MAX_FRAME_SIZE, (uint32_t)block, step);
+    return zk_frame_passes(c, q, st, first_pass, ZK_SEEKABLE_MAX_FRAME_SIZE, (uint32_t)block, step);
 }
 
+// ContentDefined(size): each pass is cut on the GPU (zk_encode_cdc), then its closed frames are compressed from the same device memory by
+// the sized path, in sub-batches of at most the first pass's length.  A pass of mx bytes always closes a frame.
+// ZK_CDC_CAP (tests): candidate positions kept per pass (default pass / 64 + 1); fewer only makes a pass cover less.
+static int32_t zk_cdc_passes(zk_ctx* c, const ZkCompressReq& q, cudaStream_t st, size_t first_pass) {
+    const ZkCdcRule rule = zk_cdc_rule(q.size);
+    const uint32_t cand_cap = (uint32_t)zk_env_size("ZK_CDC_CAP", 0);
+    std::vector<uint32_t> ds, cs;
+    auto step = [&](const uint8_t* d_in, size_t len, int at_end, uint8_t* d_out, size_t cap, ZkPassOut* o) -> int32_t {
+        ZkCdcOut r;
+        int32_t rc = zk_encode_cdc(&c->slot[0].ews, st, d_in, len, q.size, q.final_, at_end, cand_cap, &r);
+        if (rc || r.n_frames == 0) return rc;
+        ds.assign(r.sizes, r.sizes + r.n_frames);
+        cs.resize(r.n_frames);
+        const ZkFrames fr = {ds.data(), r.consumed, 0, r.n_frames};
+        rc = zk_compress_dev_subs(c, fr, d_in, q.params, d_out, cap, cs.data(), &o->total, st, first_pass);
+        if (rc) return rc;
+        o->n_frames = r.n_frames; o->consumed = r.consumed; o->c_sizes = cs.data(); o->d_sizes = ds.data();
+        return 0;
+    };
+    return zk_frame_passes(c, q, st, first_pass, rule.mx, rule.mn, step);
+}
+
+// One compress call: the argument checks of its policy, the prefix upload, then the pipeline of its policy and memory.  The order of the
+// checks decides which error a call with several faults reports, so each policy keeps its own.
+static int32_t zk_compress(zk_ctx* c, ZkCompressReq q) {
+    ZkFrames fr = {};
+    int32_t rc = 0;
+    if (q.policy == ZK_FRAMES_UNIFORM) {
+        if (!c) return ZK_ERR_INVALID_ARG;
+        if ((rc = zk_upload_prefix(c, q.prefix, q.prefix_len, &q.params.prefix, &q.params.prefix_len))) return rc;
+        if (!q.dst || (q.n && !q.src) || q.size == 0) return ZK_ERR_INVALID_ARG;
+        if (q.size > ZK_SEEKABLE_MAX_FRAME_SIZE) q.size = ZK_SEEKABLE_MAX_FRAME_SIZE;       // encode.rs:531-534
+        if ((q.n + q.size - 1) / q.size > ZK_SEEKABLE_MAX_FRAMES) return ZK_ERR_FRAME_INDEX_TOO_LARGE;
+        // no input: one empty frame, as Encoder::finish() always closes one (encode.rs:755-756)
+        fr = {nullptr, q.n, q.size, q.n ? (uint32_t)((q.n + q.size - 1) / q.size) : 1u};
+        if (fr.count > q.frames_cap) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
+    } else if (q.policy == ZK_FRAMES_SIZED) {
+        if (!c || (q.count && (!q.sizes || !q.dst))) return ZK_ERR_INVALID_ARG;
+        if (q.count > ZK_SEEKABLE_MAX_FRAMES) return ZK_ERR_FRAME_INDEX_TOO_LARGE;
+        for (uint32_t f = 0; f < q.count; f++) {
+            if (q.sizes[f] > ZK_SEEKABLE_MAX_FRAME_SIZE) return ZK_ERR_ZSTD(ZKZ_PARAM_OUT_OF_BOUND);
+            q.n += q.sizes[f];
+        }
+        if (q.n && !q.src) return ZK_ERR_INVALID_ARG;
+        if (q.dst_len) *q.dst_len = 0;
+        if (q.count == 0) return 0;                         // (no frame, unlike the uniform layout of no input)
+        if ((rc = zk_upload_prefix(c, q.prefix, q.prefix_len, &q.params.prefix, &q.params.prefix_len))) return rc;
+        fr = {q.sizes, q.n, 0, q.count};
+    } else {
+        if (!c || !q.dst || (q.n && !q.src)) return ZK_ERR_INVALID_ARG;
+        if (q.consumed) *q.consumed = 0;
+        if (q.n == 0) {                                     // one empty frame, as the uniform layout makes of no input
+            if (!q.final_) { if (q.n_frames) *q.n_frames = 0; if (q.dst_len) *q.dst_len = 0; return 0; }
+            q.policy = ZK_FRAMES_UNIFORM; q.size = 1;
+            return zk_compress(c, q);
+        }
+        if ((rc = zk_upload_prefix(c, q.prefix, q.prefix_len, &q.params.prefix, &q.params.prefix_len))) return rc;
+    }
+    ZK_CUDA_OK(cudaSetDevice(c->device));
+    const cudaStream_t st = q.stream ? q.stream : c->slot[0].stream;
+    // tuning knobs: input bytes per sub-batch, and the first pass of the cut policies (tools/knobs_round.sh sweeps the host one)
+    const size_t sub_bytes = q.host ? zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20) : zk_env_size("ZK_DEV_SUB_BYTES", (size_t)1 << 30);
+    if (!q.host) cudaEventRecord(c->ev0, st);
+    size_t out_len = 0;
+    if (q.policy == ZK_FRAMES_COMPRESSED) rc = zk_csize_passes(c, q, st, sub_bytes);
+    else if (q.policy == ZK_FRAMES_CONTENT) rc = zk_cdc_passes(c, q, st, sub_bytes);
+    else if (q.host) rc = zk_compress_host_run(c, fr, q, sub_bytes, &out_len);
+    else rc = zk_compress_dev_subs(c, fr, q.src, q.params, q.dst, q.dst_cap, q.c_sizes, &out_len, st, sub_bytes);
+    if (rc) return rc;
+    if (!q.host) {                                          // zk_ctx_last_device_ms: the device paths only
+        cudaEventRecord(c->ev1, st);
+        cudaEventSynchronize(c->ev1);
+        cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1);
+    }
+    if (q.policy == ZK_FRAMES_UNIFORM || q.policy == ZK_FRAMES_SIZED) { if (q.dst_len) *q.dst_len = out_len; }
+    if (q.policy == ZK_FRAMES_UNIFORM) {
+        if (q.d_sizes) for (uint32_t f = 0; f < fr.count; f++) q.d_sizes[f] = fr.size(f);
+        if (q.n_frames) *q.n_frames = fr.count;
+    }
+    return 0;
+}
+
+extern "C" int32_t zk_compress_frames(zk_ctx* c, const uint8_t* src, size_t n, uint32_t frame_size, int32_t level, int32_t checksum,
+                                      uint8_t* dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap,
+                                      uint32_t* n_frames, size_t* dst_len) {
+    return zk_compress_frames_prefix(c, src, n, frame_size, level, checksum, nullptr, 0, dst, dst_cap, c_sizes, d_sizes, frames_cap, n_frames,
+                                     dst_len);
+}
+
+extern "C" int32_t zk_compress_frames_prefix(zk_ctx* c, const uint8_t* src, size_t n, uint32_t frame_size, int32_t level, int32_t checksum,
+                                             const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap, uint32_t* c_sizes,
+                                             uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len) {
+    ZkCompressReq q;
+    q.size = frame_size; q.src = src; q.n = n; q.prefix = prefix; q.prefix_len = prefix_len;
+    q.params.level = level; q.params.checksum = checksum;
+    q.dst = dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.d_sizes = d_sizes; q.frames_cap = frames_cap; q.n_frames = n_frames; q.dst_len = dst_len;
+    return zk_compress(c, q);
+}
+
+extern "C" int32_t zk_compress_frames_dev(zk_ctx* c, const void* d_src, size_t n, uint32_t frame_size, int32_t level, int32_t checksum,
+                                          void* d_dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap,
+                                          uint32_t* n_frames, size_t* dst_len, void* cuda_stream) {
+    ZkCompressReq q;
+    q.size = frame_size; q.src = (const uint8_t*)d_src; q.n = n; q.host = false; q.stream = (cudaStream_t)cuda_stream;
+    q.params.level = level; q.params.checksum = checksum;
+    q.dst = (uint8_t*)d_dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.d_sizes = d_sizes; q.frames_cap = frames_cap; q.n_frames = n_frames;
+    q.dst_len = dst_len;
+    return zk_compress(c, q);
+}
+
+extern "C" size_t zk_compress_bound_sized(const uint32_t* frame_sizes, uint32_t n_frames) {
+    return frame_sizes || n_frames == 0 ? zk_encode_bound_sized(frame_sizes, n_frames) : 0;
+}
+
+// caller-chosen frame sizes (Encoder::end_frame at any byte, encode.rs:438-472, as one batch): frame f is what zk_compress_frames_prefix
+// writes for its bytes alone with frame_size = max(size, 1)
+extern "C" int32_t zk_compress_frames_sized(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                            int32_t checksum, const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap,
+                                            uint32_t* c_sizes, size_t* dst_len) {
+    ZkCompressReq q;
+    q.policy = ZK_FRAMES_SIZED; q.sizes = frame_sizes; q.count = n_frames; q.src = src; q.prefix = prefix; q.prefix_len = prefix_len;
+    q.params.level = level; q.params.checksum = checksum;
+    q.dst = dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.dst_len = dst_len;
+    return zk_compress(c, q);
+}
+
+extern "C" int32_t zk_compress_frames_sized_dev(zk_ctx* c, const void* d_src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                                int32_t checksum, void* d_dst, size_t dst_cap, uint32_t* c_sizes, size_t* dst_len,
+                                                void* cuda_stream) {
+    ZkCompressReq q;
+    q.policy = ZK_FRAMES_SIZED; q.sizes = frame_sizes; q.count = n_frames; q.src = (const uint8_t*)d_src; q.host = false;
+    q.stream = (cudaStream_t)cuda_stream; q.params.level = level; q.params.checksum = checksum;
+    q.dst = (uint8_t*)d_dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.dst_len = dst_len;
+    return zk_compress(c, q);
+}
+
+// ---------------------------------------------------------------------------------------------
+// long-distance matching (the reference CLI's patch mode: WindowLog + EnableLongDistanceMatching on the CCtx it hands to with_cctx,
+// cli/src/compress.rs:31-37): the prefix calls with K-C1h matching every frame against the whole prefix (zk_ldm.inc)
+// ---------------------------------------------------------------------------------------------
+extern "C" int32_t zk_compress_frames_ldm(zk_ctx* c, const uint8_t* src, size_t n, uint32_t frame_size, int32_t level, int32_t checksum,
+                                          const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap, uint32_t* c_sizes,
+                                          uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len) {
+    ZkCompressReq q;
+    q.size = frame_size; q.src = src; q.n = n; q.prefix = prefix; q.prefix_len = prefix_len;
+    q.params.level = level; q.params.checksum = checksum; q.params.ldm = true;
+    q.dst = dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.d_sizes = d_sizes; q.frames_cap = frames_cap; q.n_frames = n_frames; q.dst_len = dst_len;
+    return zk_compress(c, q);
+}
+
+extern "C" int32_t zk_compress_frames_sized_ldm(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                                int32_t checksum, const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap,
+                                                uint32_t* c_sizes, size_t* dst_len) {
+    ZkCompressReq q;
+    q.policy = ZK_FRAMES_SIZED; q.sizes = frame_sizes; q.count = n_frames; q.src = src; q.prefix = prefix; q.prefix_len = prefix_len;
+    q.params.level = level; q.params.checksum = checksum; q.params.ldm = true;
+    q.dst = dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.dst_len = dst_len;
+    return zk_compress(c, q);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Frame sizes decided on the GPU: FrameSizePolicy::Compressed(target) and ::ContentDefined(size)
+// ---------------------------------------------------------------------------------------------
 extern "C" int32_t zk_compress_frames_csize(zk_ctx* c, const uint8_t* src, size_t n, uint32_t target, int32_t level, int32_t checksum,
                                             const uint8_t* prefix, size_t prefix_len, int32_t final_, uint8_t* dst, size_t dst_cap,
                                             uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames,
                                             size_t* dst_len, size_t* consumed) {
-    if (!c || !dst || (n && !src)) return ZK_ERR_INVALID_ARG;
-    if (consumed) *consumed = 0;
-    if (n == 0) {                                           // one empty frame, as zk_compress_frames makes of no input
-        if (final_) return zk_compress_frames_prefix(c, src, 0, 1, level, checksum, prefix, prefix_len, dst, dst_cap, c_sizes, d_sizes, frames_cap, n_frames, dst_len);
-        if (n_frames) *n_frames = 0;
-        if (dst_len) *dst_len = 0;
-        return 0;
-    }
-    ZK_RT_OK(cudaSetDevice(c->device));
-    int32_t rc = zk_ctx_set_prefix(c, prefix, prefix_len);
-    if (rc) return rc;
-    rc = zk_csize_passes(c, true, src, n, target, level, checksum, c->cur_prefix_len ? c->d_prefix : nullptr, c->cur_prefix_len, final_, dst, dst_cap,
-                         c_sizes, d_sizes, frames_cap, n_frames, dst_len, consumed, c->slot[0].stream, zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20));
-    c->cur_prefix_len = 0;
-    return rc;
+    ZkCompressReq q;
+    q.policy = ZK_FRAMES_COMPRESSED; q.size = target; q.src = src; q.n = n; q.prefix = prefix; q.prefix_len = prefix_len;
+    q.params.level = level; q.params.checksum = checksum; q.final_ = final_;
+    q.dst = dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.d_sizes = d_sizes; q.frames_cap = frames_cap; q.n_frames = n_frames;
+    q.dst_len = dst_len; q.consumed = consumed;
+    return zk_compress(c, q);
 }
 
 extern "C" int32_t zk_compress_frames_csize_dev(zk_ctx* c, const void* d_src, size_t n, uint32_t target, int32_t level, int32_t checksum,
                                                 int32_t final_, void* d_dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes,
                                                 uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len, size_t* consumed, void* cuda_stream) {
-    if (!c || !d_dst || (n && !d_src)) return ZK_ERR_INVALID_ARG;
-    if (consumed) *consumed = 0;
-    if (n == 0) {
-        if (final_) return zk_compress_frames_dev(c, d_src, 0, 1, level, checksum, d_dst, dst_cap, c_sizes, d_sizes, frames_cap, n_frames, dst_len, cuda_stream);
-        if (n_frames) *n_frames = 0;
-        if (dst_len) *dst_len = 0;
-        return 0;
-    }
-    ZK_RT_OK(cudaSetDevice(c->device));
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : c->slot[0].stream;
-    cudaEventRecord(c->ev0, st);
-    const int32_t rc = zk_csize_passes(c, false, (const uint8_t*)d_src, n, target, level, checksum, nullptr, 0, final_, (uint8_t*)d_dst, dst_cap,
-                                       c_sizes, d_sizes, frames_cap, n_frames, dst_len, consumed, st, zk_env_size("ZK_DEV_SUB_BYTES", (size_t)1 << 30));
-    cudaEventRecord(c->ev1, st);
-    cudaEventSynchronize(c->ev1);
-    cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1);
-    return rc;
-}
-
-// ---------------------------------------------------------------------------------------------
-// FrameSizePolicy::ContentDefined(size): each pass is cut on the GPU (zk_encode_cdc), then its closed frames are compressed from the same
-// device memory by the sized path, in sub-batches of at most the first pass's length.  A pass of mx bytes always closes a frame.
-// ZK_CDC_CAP (tests): candidate positions kept per pass (default pass / 64 + 1); fewer only makes a pass cover less.
-// ---------------------------------------------------------------------------------------------
-static int32_t zk_cdc_passes(zk_ctx* c, bool host, const uint8_t* src, size_t n, uint32_t size, int32_t level, int32_t checksum,
-                             const uint8_t* d_prefix, uint32_t prefix_len, int32_t final_, uint8_t* dst, size_t dst_cap,
-                             uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len,
-                             size_t* consumed, cudaStream_t st, size_t first_pass) {
-    const ZkCdcRule rule = zk_cdc_rule(size);
-    const uint32_t cand_cap = (uint32_t)zk_env_size("ZK_CDC_CAP", 0);
-    std::vector<uint32_t> ds, cs;
-    auto step = [&](const uint8_t* d_in, size_t len, int at_end, uint8_t* d_out, size_t cap, ZkPassOut* o) -> int32_t {
-        ZkCdcOut r;
-        int32_t rc = zk_encode_cdc(&c->slot[0].ews, st, d_in, len, size, final_, at_end, cand_cap, &r);
-        if (rc || r.n_frames == 0) return rc;
-        ds.assign(r.sizes, r.sizes + r.n_frames);
-        cs.resize(r.n_frames);
-        const ZkFrameList fl = {ds.data(), r.consumed, 0, r.n_frames};
-        rc = zk_compress_dev_subs(c, fl, d_in, d_prefix, prefix_len, level, checksum, d_out, cap, cs.data(), &o->total, st, first_pass);
-        if (rc) return rc;
-        o->n_frames = r.n_frames; o->consumed = r.consumed; o->c_sizes = cs.data(); o->d_sizes = ds.data();
-        return 0;
-    };
-    return zk_frame_passes(c, host, src, n, dst, dst_cap, c_sizes, d_sizes, frames_cap, n_frames, dst_len, consumed, st, first_pass, rule.mx,
-                           rule.mn, step);
+    ZkCompressReq q;
+    q.policy = ZK_FRAMES_COMPRESSED; q.size = target; q.src = (const uint8_t*)d_src; q.n = n; q.host = false;
+    q.stream = (cudaStream_t)cuda_stream; q.params.level = level; q.params.checksum = checksum; q.final_ = final_;
+    q.dst = (uint8_t*)d_dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.d_sizes = d_sizes; q.frames_cap = frames_cap; q.n_frames = n_frames;
+    q.dst_len = dst_len; q.consumed = consumed;
+    return zk_compress(c, q);
 }
 
 extern "C" int32_t zk_compress_frames_cdc(zk_ctx* c, const uint8_t* src, size_t n, uint32_t size, int32_t level, int32_t checksum,
                                           const uint8_t* prefix, size_t prefix_len, int32_t final_, uint8_t* dst, size_t dst_cap,
                                           uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames,
                                           size_t* dst_len, size_t* consumed) {
-    if (!c || !dst || (n && !src)) return ZK_ERR_INVALID_ARG;
-    if (consumed) *consumed = 0;
-    if (n == 0) {                                           // one empty frame, as zk_compress_frames makes of no input
-        if (final_) return zk_compress_frames_prefix(c, src, 0, 1, level, checksum, prefix, prefix_len, dst, dst_cap, c_sizes, d_sizes, frames_cap, n_frames, dst_len);
-        if (n_frames) *n_frames = 0;
-        if (dst_len) *dst_len = 0;
-        return 0;
-    }
-    ZK_RT_OK(cudaSetDevice(c->device));
-    int32_t rc = zk_ctx_set_prefix(c, prefix, prefix_len);
-    if (rc) return rc;
-    rc = zk_cdc_passes(c, true, src, n, size, level, checksum, c->cur_prefix_len ? c->d_prefix : nullptr, c->cur_prefix_len, final_, dst, dst_cap,
-                       c_sizes, d_sizes, frames_cap, n_frames, dst_len, consumed, c->slot[0].stream, zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20));
-    c->cur_prefix_len = 0;
-    return rc;
+    ZkCompressReq q;
+    q.policy = ZK_FRAMES_CONTENT; q.size = size; q.src = src; q.n = n; q.prefix = prefix; q.prefix_len = prefix_len;
+    q.params.level = level; q.params.checksum = checksum; q.final_ = final_;
+    q.dst = dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.d_sizes = d_sizes; q.frames_cap = frames_cap; q.n_frames = n_frames;
+    q.dst_len = dst_len; q.consumed = consumed;
+    return zk_compress(c, q);
 }
 
 extern "C" int32_t zk_compress_frames_cdc_dev(zk_ctx* c, const void* d_src, size_t n, uint32_t size, int32_t level, int32_t checksum,
                                               int32_t final_, void* d_dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes,
                                               uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len, size_t* consumed, void* cuda_stream) {
-    if (!c || !d_dst || (n && !d_src)) return ZK_ERR_INVALID_ARG;
-    if (consumed) *consumed = 0;
-    if (n == 0) {
-        if (final_) return zk_compress_frames_dev(c, d_src, 0, 1, level, checksum, d_dst, dst_cap, c_sizes, d_sizes, frames_cap, n_frames, dst_len, cuda_stream);
-        if (n_frames) *n_frames = 0;
-        if (dst_len) *dst_len = 0;
-        return 0;
-    }
-    ZK_RT_OK(cudaSetDevice(c->device));
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : c->slot[0].stream;
-    cudaEventRecord(c->ev0, st);
-    const int32_t rc = zk_cdc_passes(c, false, (const uint8_t*)d_src, n, size, level, checksum, nullptr, 0, final_, (uint8_t*)d_dst, dst_cap,
-                                     c_sizes, d_sizes, frames_cap, n_frames, dst_len, consumed, st, zk_env_size("ZK_DEV_SUB_BYTES", (size_t)1 << 30));
-    cudaEventRecord(c->ev1, st);
-    cudaEventSynchronize(c->ev1);
-    cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1);
-    return rc;
+    ZkCompressReq q;
+    q.policy = ZK_FRAMES_CONTENT; q.size = size; q.src = (const uint8_t*)d_src; q.n = n; q.host = false;
+    q.stream = (cudaStream_t)cuda_stream; q.params.level = level; q.params.checksum = checksum; q.final_ = final_;
+    q.dst = (uint8_t*)d_dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.d_sizes = d_sizes; q.frames_cap = frames_cap; q.n_frames = n_frames;
+    q.dst_len = dst_len; q.consumed = consumed;
+    return zk_compress(c, q);
 }

@@ -20,10 +20,17 @@
 
 #include <stdint.h>
 #include <stddef.h>
+#include <stdio.h>
 
 // internal status of a failed CUDA runtime call / kernel (the C ABI's ZK_ERR_CUDA); the text is kept per thread
 #define ZK_INT_CUDA (-1007)
 void zk_note_cuda_error(const char* what, int code);
+// host code: a failed CUDA runtime call returns ZK_INT_CUDA from the calling function, its text kept (nothing to check in the emulation build)
+#ifndef ZK_EMUL
+#define ZK_CUDA_OK(x) do { cudaError_t e__ = (x); if (e__ != cudaSuccess) { zk_note_cuda_error(#x, (int)e__); (void)cudaGetLastError(); return ZK_INT_CUDA; } } while (0)
+#else
+#define ZK_CUDA_OK(x) do { (void)(x); } while (0)
+#endif
 
 // Optional per-kernel timing with CUDA events on the launching stream (bench.py's roofline numbers).
 // slots: 0 scan, 1 seq, 2 huf, 3 exec, 4 xxh64(dec), 5 match, 6 entropy-enc, 7 frame assembly
@@ -68,6 +75,33 @@ enum ZkZstdCode : int {
     ZKZ_DST_TOO_SMALL = 70,
     ZKZ_SRC_SIZE_WRONG = 72,
 };
+
+// host code: wait for `ev` (nullptr: for all of `stream`), then report a failed launch or kernel -> 0 or ZK_INT_CUDA
+static inline int zk_sync_check(cudaStream_t stream, cudaEvent_t ev = nullptr) {
+    ZK_CUDA_OK(ev ? cudaEventSynchronize(ev) : cudaStreamSynchronize(stream));
+#ifndef ZK_EMUL
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { zk_note_cuda_error("kernel launch / execution", (int)e); return ZK_INT_CUDA; }
+#endif
+    return 0;
+}
+
+// host code: a device (or pinned host) buffer of at least `need` elements of `elem` bytes; the old contents are not kept.  It grows by an
+// eighth more than it needs, so that a slowly growing need does not reallocate on every call.
+static inline int zk_grow(void** p, size_t* cap, size_t need, size_t elem, bool pinned = false) {
+    if (*cap >= need && *p) return 0;
+    if (*p) { if (pinned) cudaFreeHost(*p); else cudaFree(*p); }
+    *p = nullptr; *cap = 0;
+    const size_t want = need + need / 8 + 64;
+    const cudaError_t ce = pinned ? cudaMallocHost(p, want * elem) : cudaMalloc(p, want * elem);
+    if (ce != cudaSuccess) {
+        fprintf(stderr, "zeekstd_b200: %s(%zu bytes) failed: %s\n", pinned ? "cudaMallocHost" : "cudaMalloc", want * elem, cudaGetErrorString(ce));
+        (void)cudaGetLastError(); *p = nullptr;
+        return -(int)ZKZ_MEMORY_ALLOCATION;
+    }
+    *cap = want;
+    return 0;
+}
 
 #define ZK_BLOCK_MAX (1u << 17)          // Block_Maximum_Size, A.2
 #define ZK_MAGIC 0xFD2FB528u

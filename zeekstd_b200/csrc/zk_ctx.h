@@ -21,9 +21,7 @@ struct zk_ctx {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaStream_t up = nullptr, down = nullptr;            // dedicated copy streams of the host-pointer decompress pipeline
     float last_ms = 0.f;
-    uint8_t* d_prefix = nullptr; size_t cap_prefix = 0;   // device copy of the raw-content prefix of the *_prefix entry points
-    uint32_t cur_prefix_len = 0;                          // != 0 while such a call is running: every sub-batch gets the prefix
-    bool cur_ldm = false;                                 // set while a *_ldm call is running: every sub-batch matches against the whole prefix
+    void* d_prefix = nullptr; size_t cap_prefix = 0;      // device copy of the raw-content prefix of the calls that take one
     unsigned long long launches() const {
         unsigned long long n = 0;
         for (int i = 0; i < ZK_SLOTS; i++) n += slot[i].dws.launches + slot[i].ews.launches;

@@ -1881,24 +1881,7 @@ __global__ void __launch_bounds__(128) zk_xxh64_kernel(ZkDecodeArgs a) {
 // =============================================================================================
 // host-side launcher
 // =============================================================================================
-#ifndef ZK_EMUL
-#define ZK_CUDA_OK(x) do { cudaError_t err__ = (x); if (err__ != cudaSuccess) { zk_note_cuda_error(#x, (int)err__); return ZK_INT_CUDA; } } while (0)
-#else
-#define ZK_CUDA_OK(x) do { (void)(x); } while (0)
-#endif
-
 #define ZK_WORK_COUNTERS 5
-
-static int zk_grow(void** p, size_t* cap, size_t need, size_t elem) {
-    if (*cap >= need && *p) return 0;
-    if (*p) cudaFree(*p);
-    *p = nullptr; *cap = 0;
-    size_t want = need + need / 8 + 64;
-    cudaError_t ce = cudaMalloc(p, want * elem);
-    if (ce != cudaSuccess) { fprintf(stderr, "zeekstd_b200: cudaMalloc(%zu bytes) failed in the decode workspace: %s\n", want * elem, cudaGetErrorString(ce)); (void)cudaGetLastError(); *p = nullptr; return -(int)ZKZ_MEMORY_ALLOCATION; }
-    *cap = want;
-    return 0;
-}
 
 void zk_decode_ws_free(ZkDecodeWs* ws) {
     void* ptrs[] = { ws->blocks, ws->entries, ws->counters, ws->lit, ws->seq_lit_end, ws->seq_out_end, ws->seq_off, ws->c_off, ws->d_off,
@@ -1966,7 +1949,7 @@ static int zk_decode_ensure(ZkDecodeWs* ws, uint32_t n, size_t need_blocks, size
 
 // Enqueue one batch on `stream` (scan, entropy, exec[, checksum], status read-back).  No host sync.
 int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp, const uint64_t* c_off, const uint64_t* d_off,
-                      uint32_t n, uint8_t* d_dst, int verify_checksum) {
+                      uint32_t n, uint8_t* d_dst, int verify_checksum, const ZkDecodeParams& p) {
     ws->pending_n = 0;
     if (n == 0) return 0;
     unsigned long long total_d = d_off[n] - d_off[0];
@@ -1982,10 +1965,10 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     if (rc) return rc;
     memcpy(ws->h_off, c_off, (size_t)(n + 1) * 8);
     memcpy(ws->h_off + (n + 1), d_off, (size_t)(n + 1) * 8);
-    // Host pipelines hand in dedicated copy streams (ws->up / ws->down): copies of different compute streams otherwise share
+    // Host pipelines hand in dedicated copy streams (p.up / p.down): copies of different compute streams otherwise share
     // copy-engine channels, where the upload of one sub-batch queues behind the status read-back of another that is still
     // waiting for its kernels (measured: sub-batch k + 4 started its upload when sub-batch k had finished its download).
-    cudaStream_t us = ws->up ? ws->up : stream, ds = ws->down ? ws->down : stream;
+    cudaStream_t us = p.up ? p.up : stream, ds = p.down ? p.down : stream;
     if (us != stream && !ws->ev_up) {
         ZK_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_up, cudaEventDisableTiming)); ZK_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_done, cudaEventDisableTiming));
         ZK_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_down, cudaEventDisableTiming));
@@ -2001,11 +1984,11 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     a.huf_list = ws->huf_list; a.seq_list = ws->seq_list; a.seg_list = ws->seg_list;
     a.cap_blocks = ws->cap_blocks; a.cap_lit = ws->cap_lit - 64; a.cap_seq = ws->cap_seq;
     a.d_need = nullptr;
-    a.prefix = ws->prefix; a.prefix_len = ws->prefix ? ws->prefix_len : 0; ws->prefix = nullptr; ws->prefix_len = 0;
-    if (ws->need) {
-        memcpy(ws->h_need, ws->need, (size_t)n * 4);
+    a.prefix = p.prefix; a.prefix_len = p.prefix ? p.prefix_len : 0;
+    if (p.need) {
+        memcpy(ws->h_need, p.need, (size_t)n * 4);
         ZK_CUDA_OK(cudaMemcpyAsync(ws->d_need, ws->h_need, (size_t)n * 4, cudaMemcpyHostToDevice, us));
-        a.d_need = ws->d_need; ws->need = nullptr;
+        a.d_need = ws->d_need;
     }
     if (us != stream) { ZK_CUDA_OK(cudaEventRecord(ws->ev_up, us)); ZK_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_up, 0)); }   // also orders the caller's upload of the compressed bytes
     ws->prof.begin(0, stream);
@@ -2057,7 +2040,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     if (need_h < gh) gh = (uint32_t)need_h;
     // the two entropy kernels are independent: run the Huffman one on a side stream
     cudaStream_t hs = stream;
-    if (!ws->no_side) {
+    if (p.side) {
         if (!ws->side) {
             ZK_CUDA_OK(cudaStreamCreateWithPriority(&ws->side, cudaStreamNonBlocking, ws->prio));
             ZK_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_scan, cudaEventDisableTiming));
@@ -2086,7 +2069,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     // Each entry is one serial dependency chain, so throughput comes from entries in flight: pick warps per
     // CTA and ring size such that (if possible) every entry of the batch is resident at once.
     // (`share` > 1: that many sub-batches of a host pipeline run concurrently on different streams)
-    int per_sm = (int)(((unsigned long long)n * (unsigned)(ws->share > 0 ? ws->share : 1) + (uint32_t)sms - 1) / (uint32_t)sms);
+    int per_sm = (int)(((unsigned long long)n * (unsigned)(p.share > 0 ? p.share : 1) + (uint32_t)sms - 1) / (uint32_t)sms);
     if (per_sm < 1) per_sm = 1;
     int W = (int)ws->exec_warps;
     a.exec_short = ws->exec_short;
@@ -2128,14 +2111,11 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
 
 // Wait for the batch enqueued last on `stream`; returns 0, the first failing entry status, or ZK_ST_RETRY when the
 // scratch was too small (ws->want_* then hold the exact needs: the caller re-enqueues the same batch).
-int zk_decode_collect(ZkDecodeWs* ws, cudaStream_t stream, int32_t* status_out) {
+int zk_decode_collect(ZkDecodeWs* ws, cudaStream_t stream, const ZkDecodeParams& p, int32_t* status_out) {
     uint32_t n = ws->pending_n;
     if (n == 0) return 0;
-    if (ws->down && ws->ev_down) ZK_CUDA_OK(cudaEventSynchronize(ws->ev_down));     // recorded by the caller after the output copy on the download stream
-    else ZK_CUDA_OK(cudaStreamSynchronize(stream));
-#ifndef ZK_EMUL
-    { cudaError_t le__ = cudaGetLastError(); if (le__ != cudaSuccess) { zk_note_cuda_error("kernel launch / execution", (int)le__); return ZK_INT_CUDA; } }
-#endif
+    // with a download stream: ev_down, recorded by the caller after the output copy on it
+    if (const int rc = zk_sync_check(stream, p.down ? ws->ev_down : nullptr)) return rc;
     ws->pending_n = 0;
     ws->prof.harvest();
     if (ws->h_counters->overflow) {
@@ -2154,11 +2134,11 @@ int zk_decode_collect(ZkDecodeWs* ws, cudaStream_t stream, int32_t* status_out) 
 }
 
 int zk_decode_batch(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp, const uint64_t* c_off, const uint64_t* d_off,
-                    uint32_t n, uint8_t* d_dst, int verify_checksum, int32_t* status_out) {
+                    uint32_t n, uint8_t* d_dst, int verify_checksum, const ZkDecodeParams& p, int32_t* status_out) {
     for (int attempt = 0; attempt < 2; attempt++) {
-        int rc = zk_decode_enqueue(ws, stream, d_comp, c_off, d_off, n, d_dst, verify_checksum);
+        int rc = zk_decode_enqueue(ws, stream, d_comp, c_off, d_off, n, d_dst, verify_checksum, p);
         if (rc) return rc;
-        rc = zk_decode_collect(ws, stream, status_out);
+        rc = zk_decode_collect(ws, stream, p, status_out);
         if (rc != ZK_ST_RETRY) return rc;
     }
     fprintf(stderr, "zeekstd_b200: decode scratch still too small after growing to the exact needs (blocks %zu lit %zu seq %zu; caps %zu %zu %zu)\n",

@@ -29,9 +29,7 @@ struct ZkDecodeWs {                   // HBM scratch owned by a zk_ctx, grown on
     uint8_t* lit = nullptr; size_t cap_lit = 0;
     uint32_t* seq_lit_end = nullptr; uint32_t* seq_out_end = nullptr; uint32_t* seq_off = nullptr; size_t cap_seq = 0;
     uint64_t* c_off = nullptr; uint64_t* d_off = nullptr;
-    const uint32_t* need = nullptr;   // host array for the NEXT enqueue (one-shot): leading bytes wanted per entry, see ZkDecodeArgs::d_need
     uint32_t* d_need = nullptr; uint32_t* h_need = nullptr;
-    const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device pointer for the NEXT enqueue (one-shot, like `need`)
     uint32_t* huf_list = nullptr; uint32_t* seq_list = nullptr; uint32_t* seg_list = nullptr;
     bool attr_set = false; uint32_t ring_override = 0;
     uint32_t exec_warps = 0;          // ZK_EXEC_WARPS: warps per K-D2 CTA (at most 16); 0 = chosen from the entries per SM
@@ -39,12 +37,9 @@ struct ZkDecodeWs {                   // HBM scratch owned by a zk_ctx, grown on
     uint32_t seq2_fit = 0;            // K-D1s CTAs in three quarters of an SM's shared memory (queried at the first launch; DESIGN §6)
     uint32_t exec_short = 128 << 10;  // ZK_EXEC_SHORT: output bytes up to which a segment runs on one warp (zk_exec_warp_kernel); 0 = CTAs only
     uint32_t huf_pad = 0;             // extra dynamic smem per Huffman CTA: fewer resident CTAs -> more L1 for the streams (tuning)
-    int share = 1;                    // how many batches share the GPU concurrently (host pipeline depth)
     int prio = 0;                     // CUDA stream priority of the side stream (matches the slot's stream)
     uint32_t huf_ctas = 0;            // persistent K-D1h CTAs per SM (tuning: ZK_HUF_CTAS); 0: half of huf_fit
     uint32_t huf_fit = 0;             // K-D1h CTAs that fit on an SM (occupancy query at the first launch; 0 = not asked yet)
-    bool no_side = false;             // host pipelines: concurrency comes from the other sub-batches; every extra stream costs a hardware queue
-    cudaStream_t up = nullptr, down = nullptr;      // host pipelines: dedicated upload / download streams (not owned); nullptr = everything on `stream`
     cudaEvent_t ev_up = nullptr, ev_done = nullptr, ev_down = nullptr;
     cudaStream_t side = nullptr; cudaEvent_t ev_scan = nullptr, ev_huf = nullptr;   // Huffman kernel runs beside the FSE kernel
     ZkEntry* h_entries = nullptr; ZkCounters* h_counters = nullptr; uint64_t* h_off = nullptr;   // pinned
@@ -56,14 +51,24 @@ struct ZkDecodeWs {                   // HBM scratch owned by a zk_ctx, grown on
     ZkProf prof;
 };
 
+// What a call asks of every batch it enqueues
+struct ZkDecodeParams {
+    const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device memory: the raw-content prefix of every zstd frame (nullptr: none)
+    const uint32_t* need = nullptr;   // host, one per entry: leading bytes wanted (ZkDecodeArgs::d_need); nullptr = everything
+    int share = 1;                    // how many batches share the GPU concurrently (host pipeline depth)
+    bool side = true;                 // K-D1h on the side stream; host pipelines get their concurrency from the other sub-batches instead,
+                                      // and every extra stream costs a hardware queue
+    cudaStream_t up = nullptr, down = nullptr;      // host pipelines: dedicated upload / download streams (not owned); nullptr = everything on `stream`
+};
+
 // Decode n seek-table entries.  d_comp / d_dst are device pointers (16-byte aligned, 16 readable bytes of
 // padding after the last byte); c_off / d_off are HOST arrays of n+1 cumulative offsets relative to those
 // pointers (seek_table.rs:97-101).  status_out[n] (host, optional) receives 0 or -(zstd code) per entry.
 // Returns 0, or the first non-zero entry status, or -(code) for a launch/allocation failure.
 // Synchronous with respect to `stream` on return.
 int zk_decode_batch(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp, const uint64_t* c_off, const uint64_t* d_off,
-                    uint32_t n, uint8_t* d_dst, int verify_checksum, int32_t* status_out);
+                    uint32_t n, uint8_t* d_dst, int verify_checksum, const ZkDecodeParams& p, int32_t* status_out);
 int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp, const uint64_t* c_off, const uint64_t* d_off,
-                      uint32_t n, uint8_t* d_dst, int verify_checksum);
-int zk_decode_collect(ZkDecodeWs* ws, cudaStream_t stream, int32_t* status_out);
+                      uint32_t n, uint8_t* d_dst, int verify_checksum, const ZkDecodeParams& p);
+int zk_decode_collect(ZkDecodeWs* ws, cudaStream_t stream, const ZkDecodeParams& p, int32_t* status_out);
 void zk_decode_ws_free(ZkDecodeWs* ws);

@@ -1478,12 +1478,6 @@ __global__ void __launch_bounds__(128) zk_csize_gather_kernel(ZkCsizeArgs c) {
 // =============================================================================================
 // host-side launcher
 // =============================================================================================
-#ifndef ZK_EMUL
-#define ZKC_CUDA_OK(x) do { cudaError_t err__ = (x); if (err__ != cudaSuccess) { zk_note_cuda_error(#x, (int)err__); return ZK_INT_CUDA; } } while (0)
-#else
-#define ZKC_CUDA_OK(x) do { (void)(x); } while (0)
-#endif
-
 size_t zk_encode_bound(size_t n, uint32_t frame_size) {
     if (frame_size == 0) frame_size = 1;
     size_t frames = n / frame_size + 1;
@@ -1499,6 +1493,8 @@ size_t zk_encode_bound_sized(const uint32_t* sizes, uint32_t n_frames) {
     for (uint32_t f = 0; f < n_frames; f++) b += (size_t)sizes[f] + ZKC_FRAME_HDR + 4 + 3 * (size_t)zkc_frame_blocks(sizes[f]);
     return b;
 }
+
+size_t ZkFrames::bound() const { return sizes ? zk_encode_bound_sized(sizes, count) : zk_encode_bound(n, frame_size); }
 
 void zk_encode_ws_free(ZkEncodeWs* ws) {
     if (ws->buf) cudaFree(ws->buf);
@@ -1519,53 +1515,65 @@ struct ZkcHcPass;
 struct ZkcHcRun;
 static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, const ZkEncodeArgs& a, const ZkcHcRun* hc);
 
-// the frame and block tables of a batch, on `stream`: h_sizes == nullptr: the uniform layout of (n, frame_size), generated on the device;
-// otherwise the caller's sizes, uploaded to d_sizes and scanned there
-static int zkc_build_geometry(ZkEncodeWs* ws, cudaStream_t stream, ZkcGeo* geo, ZkcFrame* fr, uint32_t n_frames, uint32_t n_blocks,
-                              size_t n, uint32_t frame_size, const uint32_t* h_sizes, uint32_t* d_sizes) {
-    if (h_sizes) {
-        ZKC_CUDA_OK(cudaMemcpyAsync(d_sizes, h_sizes, (size_t)n_frames * 4, cudaMemcpyHostToDevice, stream));
+// the frame and block tables of a batch, on `stream`: the uniform layout is generated on the device, the caller's sizes are uploaded to
+// d_sizes and scanned there
+static int zkc_build_geometry(ZkEncodeWs* ws, cudaStream_t stream, ZkcGeo* geo, ZkcFrame* fr, const ZkFrames& frames, uint32_t n_blocks,
+                              uint32_t* d_sizes) {
+    const uint32_t n_frames = frames.count;
+    if (frames.sizes) {
+        ZK_CUDA_OK(cudaMemcpyAsync(d_sizes, frames.sizes, (size_t)n_frames * 4, cudaMemcpyHostToDevice, stream));
         ZK_LAUNCH(zk_geo_sized_kernel, 1, 1024, 0, stream, fr, (const uint32_t*)d_sizes, n_frames);
-    } else ZK_LAUNCH(zk_geo_uniform_kernel, (n_frames + 255) / 256, 256, 0, stream, fr, n_frames, n, frame_size);
+    } else ZK_LAUNCH(zk_geo_uniform_kernel, (n_frames + 255) / 256, 256, 0, stream, fr, n_frames, frames.n, frames.frame_size);
     ZK_LAUNCH(zk_geo_block_kernel, (n_blocks + 255) / 256, 256, 0, stream, geo, (const ZkcFrame*)fr, n_frames, n_blocks);
     ws->launches += 2;
+    return 0;
+}
+
+// the stream K-C2s and the checksum run on: the workspace's side stream (created at its first use), or `stream` itself without one
+static int zkc_side_stream(ZkEncodeWs* ws, cudaStream_t stream, bool side, cudaStream_t* ss) {
+    *ss = stream;
+    if (!side) return 0;
+    if (!ws->side) {
+        ZK_CUDA_OK(cudaStreamCreateWithPriority(&ws->side, cudaStreamNonBlocking, ws->prio));
+        ZK_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_a, cudaEventDisableTiming));
+        ZK_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_b, cudaEventDisableTiming));
+        ZK_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_c, cudaEventDisableTiming));
+    }
+    *ss = ws->side;
     return 0;
 }
 
 #include "zk_hc.inc"
 #include "zk_cdc.inc"
 
-// one batch of n_frames frames: of frame_size bytes (the last one shorter) when h_sizes is null, else of h_sizes[f] bytes (n = their sum)
-static int zkc_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t frame_size, const uint32_t* h_sizes,
-                       uint32_t n_frames, int level, int checksum, uint8_t* d_dst, size_t dst_cap) {
-    const uint8_t* d_prefix = ws->prefix; const uint32_t prefix_len = ws->prefix_len;     // one-shot (set by the caller for THIS batch)
-    ws->prefix = nullptr; ws->prefix_len = 0;
+int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, const ZkFrames& fr, const ZkEncodeParams& p, uint8_t* d_dst,
+                      size_t dst_cap) {
+    const size_t n = fr.n; const uint32_t n_frames = fr.count;
     ws->pending_frames = 0;
     if (n_frames == 0) return 0;
     size_t n_blocks = 0;
-    if (h_sizes) {
+    if (fr.sizes) {
         for (uint32_t f = 0; f < n_frames; f++) {
-            if (h_sizes[f] > 0x40000000u) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
-            n_blocks += zkc_frame_blocks(h_sizes[f]);
+            if (fr.sizes[f] > 0x40000000u) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
+            n_blocks += zkc_frame_blocks(fr.sizes[f]);
         }
     } else {
-        if (frame_size == 0 || frame_size > 0x40000000u) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
-        n_blocks = (size_t)(n_frames - 1) * zkc_frame_blocks(frame_size) + zkc_frame_blocks(n - (size_t)(n_frames - 1) * frame_size);
+        if (fr.frame_size == 0 || fr.frame_size > 0x40000000u) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
+        n_blocks = (size_t)(n_frames - 1) * zkc_frame_blocks(fr.frame_size) + zkc_frame_blocks(n - (size_t)(n_frames - 1) * fr.frame_size);
     }
     if (n_blocks > 0x7FFFFFFFull) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
-    const uint32_t pt = d_prefix && prefix_len && n ? (prefix_len < ZKC_BLOCK ? prefix_len : ZKC_BLOCK) : 0u;
+    const uint32_t pt = p.prefix && p.prefix_len && n ? (p.prefix_len < ZKC_BLOCK ? p.prefix_len : ZKC_BLOCK) : 0u;
     // long-distance matching is a part of K-C1h: with it every level runs that tier
-    const bool ldm = ws->ldm && pt;
-    ws->ldm = false;
-    const int lvl = ldm ? ZKC_HC_LEVEL : zkc_level(level);
+    const bool ldm = p.ldm && pt;
+    const int lvl = ldm ? ZKC_HC_LEVEL : zkc_level(p.level);
     ZkcHcRun hc;
-    const uint32_t hc_span = lvl >= ZKC_HC_LEVEL ? zkc_hc_plan(n, frame_size, h_sizes, n_frames, (uint32_t)n_blocks, pt, hc.plan) : 0u;
-    if (ldm) hc.reach = prefix_len < ZKC_LDM_REACH ? prefix_len : ZKC_LDM_REACH;
+    const uint32_t hc_span = lvl >= ZKC_HC_LEVEL ? zkc_hc_plan(fr, (uint32_t)n_blocks, pt, hc.plan) : 0u;
+    if (ldm) hc.reach = p.prefix_len < ZKC_LDM_REACH ? p.prefix_len : ZKC_LDM_REACH;
     // carve the workspace
     size_t off = 0;
     const size_t o_geo = off; off = zkc_align(off + n_blocks * sizeof(ZkcGeo));
     const size_t o_fr = off; off = zkc_align(off + (size_t)n_frames * sizeof(ZkcFrame));
-    const size_t o_fsz = off; if (h_sizes) off = zkc_align(off + (size_t)n_frames * 4);
+    const size_t o_fsz = off; if (fr.sizes) off = zkc_align(off + (size_t)n_frames * 4);
     const size_t o_blocks = off; off = zkc_align(off + n_blocks * sizeof(ZkcBlock));
     const size_t o_ll = off; off = zkc_align(off + n_blocks * ZKC_MAXSEQ * 2);
     const size_t o_ml = off; off = zkc_align(off + n_blocks * ZKC_MAXSEQ * 2);
@@ -1582,87 +1590,55 @@ static int zkc_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src
     if (lvl >= ZKC_HC_LEVEL) off = zkc_align(off + zkc_hc_layout(hc_span, nullptr, nullptr));
     const size_t o_ldm = off;
     if (ldm) off = zkc_align(off + zkc_ldm_layout(hc.reach, n_blocks, nullptr, nullptr, nullptr));
-    if (ws->cap < off) {
-        if (ws->buf) cudaFree(ws->buf);
-        ws->buf = nullptr; ws->cap = 0;
-        size_t want = off + off / 8;
-        if (cudaMalloc(&ws->buf, want) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
-        ws->cap = want;
-    }
-    if (ws->cap_frames < n_frames) {
-        if (ws->h_sizes) cudaFreeHost(ws->h_sizes);
-        ws->h_sizes = nullptr;
-        size_t want = (size_t)n_frames + n_frames / 8 + 16;
-        if (cudaMallocHost((void**)&ws->h_sizes, want * 4 + 32) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
-        ws->cap_frames = want;
-    }
+    int rc = zk_grow(&ws->buf, &ws->cap, off, 1);
+    if (!rc) rc = zk_grow((void**)&ws->h_sizes, &ws->cap_frames, (size_t)n_frames + 4, 4, true);     // the sizes, then the total and the error
+    if (rc) return rc;
     uint8_t* base = (uint8_t*)ws->buf;
     ZkEncodeArgs a;
     a.src = d_src; a.n = n; a.n_frames = n_frames; a.n_blocks = (uint32_t)n_blocks;
     a.geo = (const ZkcGeo*)(base + o_geo); a.frames = (const ZkcFrame*)(base + o_fr);
-    a.level = lvl; a.checksum = checksum ? 1 : 0;
+    a.level = lvl; a.checksum = p.checksum ? 1 : 0;
     a.blocks = (ZkcBlock*)(base + o_blocks);
     a.seq_ll = (uint16_t*)(base + o_ll); a.seq_ml = (uint16_t*)(base + o_ml); a.seq_off = (uint32_t*)(base + o_off);
     a.lits = base + o_lits; a.stage = base + o_stage; a.seqsec = base + o_seqsec;
     a.frame_csize = (uint32_t*)(base + o_fcs); a.frame_off = (unsigned long long*)(base + o_foff); a.frame_hash = (uint32_t*)(base + o_fh);
     a.dst = d_dst; a.dst_cap = dst_cap; a.total = (unsigned long long*)(base + o_tot); a.error = (uint32_t*)(base + o_tot + 8);
-    a.prefix = d_prefix; a.prefix_len = 0; a.ptail = 0; a.pstage = base + o_pst;
+    a.prefix = p.prefix; a.prefix_len = 0; a.ptail = 0; a.pstage = base + o_pst;
     a.hist_cap = ~(size_t)0;
     a.hc = base + o_hc;
     if (ldm) hc.ldm = base + o_ldm;
-    int rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo), (ZkcFrame*)(base + o_fr), n_frames, (uint32_t)n_blocks, n, frame_size,
-                                h_sizes, (uint32_t*)(base + o_fsz));
+    rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo), (ZkcFrame*)(base + o_fr), fr, (uint32_t)n_blocks, (uint32_t*)(base + o_fsz));
     if (rc) return rc;
     if (pt) {
-        a.prefix_len = prefix_len; a.ptail = pt;
+        a.prefix_len = p.prefix_len; a.ptail = pt;
         ZK_LAUNCH(zk_prefix_stage_kernel, n_frames, 256, 0, stream, a);
         ws->launches += 1;
     }
-    ZKC_CUDA_OK(cudaMemsetAsync(base + o_tot, 0, 16, stream));
+    ZK_CUDA_OK(cudaMemsetAsync(base + o_tot, 0, 16, stream));
     // the content checksum only needs the input: it runs beside the match finder on the side stream (one warp per frame, bound
     // by the latency of its four serial chains, so it leaves the machine to K-C1)
-    cudaStream_t ss = stream;
-    if (!ws->no_side) {
-        if (!ws->side) {
-            ZKC_CUDA_OK(cudaStreamCreateWithPriority(&ws->side, cudaStreamNonBlocking, ws->prio));
-            ZKC_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_a, cudaEventDisableTiming));
-            ZKC_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_b, cudaEventDisableTiming));
-            ZKC_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_c, cudaEventDisableTiming));
-        }
-        ss = ws->side;
-    }
-    if (checksum && ss != stream) {
-        ZKC_CUDA_OK(cudaEventRecord(ws->ev_c, stream)); ZKC_CUDA_OK(cudaStreamWaitEvent(ss, ws->ev_c, 0));     // after whatever produced the input
+    cudaStream_t ss;
+    if ((rc = zkc_side_stream(ws, stream, p.side, &ss))) return rc;
+    if (p.checksum && ss != stream) {
+        ZK_CUDA_OK(cudaEventRecord(ws->ev_c, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(ss, ws->ev_c, 0));     // after whatever produced the input
         ZK_LAUNCH(zk_frame_hash_kernel, (n_frames + 3) / 4, 128, 0, ss, a);
     }
     rc = zkc_run_blocks(ws, stream, ss, a, &hc);
     if (rc) return rc;
     ws->prof.begin(7, stream);
-    if (checksum && ss == stream) ZK_LAUNCH(zk_frame_hash_kernel, (n_frames + 3) / 4, 128, 0, stream, a);   // else: already done on the side stream (joined by ev_b)
+    if (p.checksum && ss == stream) ZK_LAUNCH(zk_frame_hash_kernel, (n_frames + 3) / 4, 128, 0, stream, a);   // else: already done on the side stream (joined by ev_b)
     ZK_LAUNCH(zk_frame_size_kernel, (n_frames + 255) / 256, 256, 0, stream, a);
     ZK_LAUNCH(zk_frame_scan_kernel, 1, 1024, 0, stream, a);
     ZK_LAUNCH(zk_frame_gather_kernel, (uint32_t)((n_blocks + 3) / 4), 128, 0, stream, a);
-    if (ldm) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 128u << 10, 1u << 27, prefix_len); ws->launches++; }
+    if (ldm) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 128u << 10, 1u << 27, p.prefix_len); ws->launches++; }
     else if (a.level >= ZKC_HC_LEVEL) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 128u << 10, ZKC_HC_WINDOW, pt); ws->launches++; }
     else if (a.level >= ZKC_WIDE_LEVEL) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 256u << 10, 256u << 10, pt); ws->launches++; }
     ws->prof.end(7, stream);
-    ZKC_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, a.frame_csize, (size_t)n_frames * 4, cudaMemcpyDeviceToHost, stream));
-    ZKC_CUDA_OK(cudaMemcpyAsync(ws->h_sizes + ws->cap_frames, a.total, 16, cudaMemcpyDeviceToHost, stream));
-    ws->launches += 7 + (checksum ? 1 : 0);
+    ZK_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, a.frame_csize, (size_t)n_frames * 4, cudaMemcpyDeviceToHost, stream));
+    ZK_CUDA_OK(cudaMemcpyAsync(ws->h_sizes + n_frames, a.total, 16, cudaMemcpyDeviceToHost, stream));
+    ws->launches += 7 + (p.checksum ? 1 : 0);
     ws->pending_frames = n_frames;
     return 0;
-}
-
-int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t frame_size, int level,
-                      int checksum, uint8_t* d_dst, size_t dst_cap, uint32_t n_frames) {
-    return zkc_enqueue(ws, stream, d_src, n, frame_size, nullptr, n_frames, level, checksum, d_dst, dst_cap);
-}
-
-int zk_encode_enqueue_sized(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, const uint32_t* frame_sizes, uint32_t n_frames,
-                            int level, int checksum, uint8_t* d_dst, size_t dst_cap) {
-    size_t n = 0;
-    for (uint32_t f = 0; f < n_frames; f++) n += frame_sizes[f];
-    return zkc_enqueue(ws, stream, d_src, n, 0, frame_sizes, n_frames, level, checksum, d_dst, dst_cap);
 }
 
 // K-C1 and K-C2 over every block of `a` (match finding, then sequences on `ss` beside literals on `stream`, joined by the finish kernel);
@@ -1685,20 +1661,20 @@ static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, 
     else if (a.level < ZKC_WIDE_LEVEL) ZK_LAUNCH((zk_match_kernel<14, 1, false>), (uint32_t)n_blocks, 32, 0, stream, a);
     else {
         const int wide_smem = (int)sizeof(uint32_t) << ZKC_WIDE_HLOG;
-        if (!ws->attr_set_wide) { ZKC_CUDA_OK(cudaFuncSetAttribute(zk_match_wide_kernel<ZKC_WIDE_HLOG>, cudaFuncAttributeMaxDynamicSharedMemorySize, wide_smem)); ws->attr_set_wide = true; }
+        if (!ws->attr_set_wide) { ZK_CUDA_OK(cudaFuncSetAttribute(zk_match_wide_kernel<ZKC_WIDE_HLOG>, cudaFuncAttributeMaxDynamicSharedMemorySize, wide_smem)); ws->attr_set_wide = true; }
         ZK_LAUNCH((zk_match_wide_kernel<ZKC_WIDE_HLOG>), (uint32_t)n_blocks, 32, wide_smem, stream, a);
     }
     ws->prof.end(5, stream);
     const size_t seq_smem = ((sizeof(ZkcTabs) + 15) & ~(size_t)15) + sizeof(ZkcSeqWarp) * ZKC_SW;
-    if (!ws->attr_set) { ZKC_CUDA_OK(cudaFuncSetAttribute(zk_seq_enc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)seq_smem)); ws->attr_set = true; }
+    if (!ws->attr_set) { ZK_CUDA_OK(cudaFuncSetAttribute(zk_seq_enc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)seq_smem)); ws->attr_set = true; }
     // the two entropy kernels are independent and both latency-bound: run them side by side, join in zk_block_finish_kernel
     ws->prof.begin(6, stream);
-    if (ss != stream) { ZKC_CUDA_OK(cudaEventRecord(ws->ev_a, stream)); ZKC_CUDA_OK(cudaStreamWaitEvent(ss, ws->ev_a, 0)); }
+    if (ss != stream) { ZK_CUDA_OK(cudaEventRecord(ws->ev_a, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(ss, ws->ev_a, 0)); }
     ZK_LAUNCH(zk_seq_enc_kernel, (uint32_t)((n_blocks + ZKC_SW - 1) / ZKC_SW), 32 * ZKC_SW, seq_smem, ss, a);
-    if (ss != stream) ZKC_CUDA_OK(cudaEventRecord(ws->ev_b, ss));
+    if (ss != stream) ZK_CUDA_OK(cudaEventRecord(ws->ev_b, ss));
     if (a.level < 0) ZK_LAUNCH((zk_lit_enc_kernel<false, 1>), (uint32_t)n_blocks, 32, 0, stream, a);
     else ZK_LAUNCH((zk_lit_enc_kernel<true, ZKC_LW>), (uint32_t)((n_blocks + ZKC_LW - 1) / ZKC_LW), 32 * ZKC_LW, 0, stream, a);
-    if (ss != stream) ZKC_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_b, 0));
+    if (ss != stream) ZK_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_b, 0));
     ZK_LAUNCH(zk_block_finish_kernel, (uint32_t)((n_blocks + 3) / 4), 128, 0, stream, a);
     ws->prof.end(6, stream);
     return 0;
@@ -1707,41 +1683,32 @@ static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, 
 int zk_encode_collect(ZkEncodeWs* ws, cudaStream_t stream, uint32_t* c_sizes, size_t* dst_len) {
     const uint32_t nf = ws->pending_frames;
     if (nf == 0) { if (dst_len) *dst_len = 0; return 0; }
-    ZKC_CUDA_OK(cudaStreamSynchronize(stream));
-#ifndef ZK_EMUL
-    { cudaError_t le__ = cudaGetLastError(); if (le__ != cudaSuccess) { zk_note_cuda_error("kernel launch / execution", (int)le__); return ZK_INT_CUDA; } }
-#endif
+    if (const int rc = zk_sync_check(stream)) return rc;
     ws->pending_frames = 0;
     ws->prof.harvest();
     unsigned long long total; uint32_t err;
-    memcpy(&total, ws->h_sizes + ws->cap_frames, 8);
-    memcpy(&err, (uint8_t*)(ws->h_sizes + ws->cap_frames) + 8, 4);
+    memcpy(&total, ws->h_sizes + nf, 8);
+    memcpy(&err, (uint8_t*)(ws->h_sizes + nf) + 8, 4);
     if (err) return -(int)err;
     if (c_sizes) memcpy(c_sizes, ws->h_sizes, (size_t)nf * 4);
     if (dst_len) *dst_len = (size_t)total;
     return 0;
 }
 
-int zk_encode_batch(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t frame_size, int level,
-                    int checksum, uint8_t* d_dst, size_t dst_cap, uint32_t* c_sizes, uint32_t n_frames, size_t* dst_len) {
-    int rc = zk_encode_enqueue(ws, stream, d_src, n, frame_size, level, checksum, d_dst, dst_cap, n_frames);
-    if (rc) return rc;
-    return zk_encode_collect(ws, stream, c_sizes, dst_len);
-}
-
 // FrameSizePolicy::Compressed(target) over one pass of n <= 1 GiB bytes: V variant passes of K-C1/K-C2 (shared sequence, literal
 // and section scratch; a ZkcBlock[] and a staging area each), the cut (K-C3c), then the assembly of the frames it chose.
 // One D2H copy of the counts and sizes, then one synchronisation.
-int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t target, int level, int checksum,
-                    int final_, int at_end, const uint8_t* d_prefix, uint32_t prefix_len, uint8_t* d_dst, size_t dst_cap, ZkCsizeOut* out) {
+int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t target, const ZkEncodeParams& p, int final_,
+                    int at_end, uint8_t* d_dst, size_t dst_cap, ZkCsizeOut* out) {
     *out = ZkCsizeOut();
     if (n == 0) return 0;
     if (n > 0x40000000u) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
     // the exact cut needs a bounded history per block (the V variants); the high-level tier's frame-wide chains have none, so its levels
     // run the wide tier here
-    const int lvl = zkc_level(level) >= ZKC_HC_LEVEL ? ZKC_WIDE_LEVEL : zkc_level(level);
+    const int lvl = zkc_level(p.level) >= ZKC_HC_LEVEL ? ZKC_WIDE_LEVEL : zkc_level(p.level);
     const uint32_t nb = (uint32_t)((n + ZKC_BLOCK - 1) / ZKC_BLOCK);
     const uint32_t V = lvl >= ZKC_WIDE_LEVEL ? ZKC_WIDE_HIST + 1 : 2;
+    const uint8_t* d_prefix = p.prefix; const uint32_t prefix_len = p.prefix_len;
     const bool pfx = d_prefix && prefix_len;
     const size_t res_words = ZKC_RES_HDR + 2 * (size_t)nb + 1;
     size_t off = 0;
@@ -1765,42 +1732,23 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     const size_t o_fr0 = off; off = zkc_align(off + (size_t)nb * sizeof(ZkcFrame));
     const size_t o_geo1 = off; off = zkc_align(off + (size_t)nb * sizeof(ZkcGeo));
     const size_t o_fr1 = off; off = zkc_align(off + sizeof(ZkcFrame));
-    if (ws->cap < off) {
-        if (ws->buf) cudaFree(ws->buf);
-        ws->buf = nullptr; ws->cap = 0;
-        size_t want = off + off / 8;
-        if (cudaMalloc(&ws->buf, want) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
-        ws->cap = want;
-    }
-    if (ws->cap_frames < res_words) {
-        if (ws->h_sizes) cudaFreeHost(ws->h_sizes);
-        ws->h_sizes = nullptr; ws->cap_frames = 0;
-        size_t want = res_words + res_words / 8 + 16;
-        if (cudaMallocHost((void**)&ws->h_sizes, want * 4 + 32) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
-        ws->cap_frames = want;
-    }
+    int rc = zk_grow(&ws->buf, &ws->cap, off, 1);
+    if (!rc) rc = zk_grow((void**)&ws->h_sizes, &ws->cap_frames, res_words, 4, true);
+    if (rc) return rc;
     uint8_t* base = (uint8_t*)ws->buf;
     ZkCsizeArgs c;
-    c.src = d_src; c.n = n; c.nb = nb; c.V = V; c.target = target ? target : 1; c.level = lvl; c.checksum = checksum ? 1 : 0;
+    c.src = d_src; c.n = n; c.nb = nb; c.V = V; c.target = target ? target : 1; c.level = lvl; c.checksum = p.checksum ? 1 : 0;
     c.end_closes = at_end && final_; c.end_lazy = at_end && !final_;
     c.vblocks = (const ZkcBlock*)(base + o_blocks); c.vstage = base + o_stage;
     c.psum = (unsigned long long*)(base + o_psum); c.next = (uint32_t*)(base + o_next);
     c.boff = (uint32_t*)(base + o_boff); c.bframe = (uint32_t*)(base + o_bfr);
     c.foff = (unsigned long long*)(base + o_foff); c.fhash = (uint32_t*)(base + o_fh);
     c.res = (uint32_t*)(base + o_res); c.dst = d_dst; c.dst_cap = dst_cap;
-    ZKC_CUDA_OK(cudaMemsetAsync(c.res, 0, ZKC_RES_HDR * 4, stream));
-    cudaStream_t ss = stream;
-    if (!ws->no_side) {
-        if (!ws->side) {
-            ZKC_CUDA_OK(cudaStreamCreateWithPriority(&ws->side, cudaStreamNonBlocking, ws->prio));
-            ZKC_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_a, cudaEventDisableTiming));
-            ZKC_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_b, cudaEventDisableTiming));
-            ZKC_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_c, cudaEventDisableTiming));
-        }
-        ss = ws->side;
-    }
-    int rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo0), (ZkcFrame*)(base + o_fr0), nb, nb, n, ZKC_BLOCK, nullptr, nullptr);
-    if (!rc) rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo1), (ZkcFrame*)(base + o_fr1), 1, nb, n, (uint32_t)n, nullptr, nullptr);
+    ZK_CUDA_OK(cudaMemsetAsync(c.res, 0, ZKC_RES_HDR * 4, stream));
+    cudaStream_t ss;
+    if ((rc = zkc_side_stream(ws, stream, p.side, &ss))) return rc;
+    rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo0), (ZkcFrame*)(base + o_fr0), {nullptr, n, ZKC_BLOCK, nb}, nb, nullptr);
+    if (!rc) rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo1), (ZkcFrame*)(base + o_fr1), {nullptr, n, (uint32_t)n, 1}, nb, nullptr);
     if (rc) return rc;
     // variant passes.  d = 0: frames of one block, so every block opens its frame (prefix staging included); d >= 1: one frame
     // over the pass, with the wide tier's history capped at d blocks below V - 1
@@ -1829,7 +1777,7 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     ws->prof.begin(7, stream);
     const uint32_t walk_smem = nb * 4;
     if (!ws->attr_set_walk) {
-        ZKC_CUDA_OK(cudaFuncSetAttribute(zk_csize_walk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(ZKC_CAP_BLOCKS * 4)));
+        ZK_CUDA_OK(cudaFuncSetAttribute(zk_csize_walk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(ZKC_CAP_BLOCKS * 4)));
         ws->attr_set_walk = true;
     }
     ZK_LAUNCH(zk_csize_psum_kernel, 1, 1024, 0, stream, c);
@@ -1840,11 +1788,8 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     ZK_LAUNCH(zk_csize_gather_kernel, (nb + 3) / 4, 128, 0, stream, c);
     ws->prof.end(7, stream);
     ws->launches += 6;
-    ZKC_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, c.res, res_words * 4, cudaMemcpyDeviceToHost, stream));
-    ZKC_CUDA_OK(cudaStreamSynchronize(stream));
-#ifndef ZK_EMUL
-    { cudaError_t le__ = cudaGetLastError(); if (le__ != cudaSuccess) { zk_note_cuda_error("kernel launch / execution", (int)le__); return ZK_INT_CUDA; } }
-#endif
+    ZK_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, c.res, res_words * 4, cudaMemcpyDeviceToHost, stream));
+    if ((rc = zk_sync_check(stream))) return rc;
     ws->prof.harvest();
     const uint32_t* h = ws->h_sizes;
     if (h[2]) return -(int)h[2];
@@ -1887,25 +1832,14 @@ int zk_encode_cdc(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, siz
     const size_t o_cand = off; off = zkc_align(off + (size_t)a.cap * 4);
     const size_t o_nxt = off; off = zkc_align(off + (size_t)a.cap * 8);
     const size_t o_res = off; off = zkc_align(off + res_words * 4);
-    if (ws->cut_cap < off) {
-        if (ws->cut) cudaFree(ws->cut);
-        ws->cut = nullptr; ws->cut_cap = 0;
-        const size_t want = off + off / 8;
-        if (cudaMalloc(&ws->cut, want) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
-        ws->cut_cap = want;
-    }
-    if (ws->cap_frames < res_words) {
-        if (ws->h_sizes) cudaFreeHost(ws->h_sizes);
-        ws->h_sizes = nullptr; ws->cap_frames = 0;
-        const size_t want = res_words + res_words / 8 + 16;
-        if (cudaMallocHost((void**)&ws->h_sizes, want * 4 + 32) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
-        ws->cap_frames = want;
-    }
+    int rc = zk_grow(&ws->cut, &ws->cut_cap, off, 1);
+    if (!rc) rc = zk_grow((void**)&ws->h_sizes, &ws->cap_frames, res_words, 4, true);
+    if (rc) return rc;
     uint8_t* base = (uint8_t*)ws->cut;
     a.counts = (uint32_t*)(base + o_cnt); a.cand = (uint32_t*)(base + o_cand); a.nxt = (uint2*)(base + o_nxt); a.res = (uint32_t*)(base + o_res);
     uint32_t* sums = (uint32_t*)(base + o_sum);
     if (!ws->attr_set_cdc) {
-        ZKC_CUDA_OK(cudaFuncSetAttribute(zk_cdc_walk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(ZKC_CDC_STAGE * 8)));
+        ZK_CUDA_OK(cudaFuncSetAttribute(zk_cdc_walk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(ZKC_CDC_STAGE * 8)));
         ws->attr_set_cdc = true;
     }
     const uint32_t grid = (a.runs + 255) / 256;
@@ -1919,11 +1853,8 @@ int zk_encode_cdc(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, siz
     ZK_LAUNCH(zk_cdc_walk_kernel, 1, 1024, (a.cap < ZKC_CDC_STAGE ? a.cap : ZKC_CDC_STAGE) * 8, stream, a);
     ws->prof.end(0, stream);
     ws->launches += 7;
-    ZKC_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, a.res, res_words * 4, cudaMemcpyDeviceToHost, stream));
-    ZKC_CUDA_OK(cudaStreamSynchronize(stream));
-#ifndef ZK_EMUL
-    { cudaError_t le__ = cudaGetLastError(); if (le__ != cudaSuccess) { zk_note_cuda_error("kernel launch / execution", (int)le__); return ZK_INT_CUDA; } }
-#endif
+    ZK_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, a.res, res_words * 4, cudaMemcpyDeviceToHost, stream));
+    if ((rc = zk_sync_check(stream))) return rc;
     ws->prof.harvest();
     out->n_frames = ws->h_sizes[0];
     out->consumed = ws->h_sizes[1];

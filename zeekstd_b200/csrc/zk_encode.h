@@ -10,23 +10,51 @@ struct ZkEncodeWs {                    // HBM scratch owned by a zk_ctx slot, gr
     unsigned long long launches = 0;
     uint32_t pending_frames = 0;
     bool attr_set = false, attr_set_wide = false, attr_set_walk = false, attr_set_hc = false, attr_set_cdc = false;
-    const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device pointer: raw-content prefix for the NEXT enqueue (one-shot)
-    bool ldm = false;                 // long-distance matching against that prefix for the NEXT enqueue (one-shot; nothing without a prefix)
     int prio = 0;                     // CUDA stream priority of the side stream (matches the slot's stream)
-    bool no_side = false;             // host pipelines: concurrency comes from the other sub-batches; every extra stream costs a hardware queue
     cudaStream_t side = nullptr; cudaEvent_t ev_a = nullptr, ev_b = nullptr, ev_c = nullptr;   // K-C2s runs beside K-C2l
     ZkProf prof;
 };
 
-// Compress n bytes at d_src into ceil(n/frame_size) frames written back to back at d_dst.
-// c_sizes (host, n_frames entries) receives each frame's compressed size.  Synchronous on `stream`.
-int zk_encode_batch(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t frame_size, int level,
-                    int checksum, uint8_t* d_dst, size_t dst_cap, uint32_t* c_sizes, uint32_t n_frames, size_t* dst_len);
-int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t frame_size, int level,
-                      int checksum, uint8_t* d_dst, size_t dst_cap, uint32_t n_frames);
-// The same with caller-chosen frame sizes: frame f covers frame_sizes[f] bytes (each <= 1 GiB; 0: an empty frame) of d_src, back to back
-int zk_encode_enqueue_sized(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, const uint32_t* frame_sizes, uint32_t n_frames,
-                            int level, int checksum, uint8_t* d_dst, size_t dst_cap);
+// What a call asks of every batch it enqueues
+struct ZkEncodeParams {
+    int level = 0, checksum = 0;
+    const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device memory: the raw-content prefix of every frame (nullptr: none)
+    bool ldm = false;                 // long-distance matching against the whole prefix (nothing without one)
+    bool side = true;                 // K-C2s and the checksum on the side stream; host pipelines get their concurrency from the other
+                                      // sub-batches instead, and every extra stream costs a hardware queue
+};
+
+// The frames of a batch: the caller's sizes (each <= 1 GiB; 0: an empty frame), or the uniform layout of n bytes (frame_size bytes each, the
+// last frame shorter, one empty frame of no input).  n is the bytes they cover.
+struct ZkFrames {
+    const uint32_t* sizes;            // nullptr: uniform
+    size_t n; uint32_t frame_size, count;
+    uint32_t size(uint32_t f) const {
+        if (sizes) return sizes[f];
+        const size_t lo = (size_t)f * frame_size;
+        return (uint32_t)(n - lo < frame_size ? n - lo : frame_size);
+    }
+    // the sub-batch from frame f0: as many frames as fit max_bytes of input, at least one -> its end frame; *bytes: its input
+    uint32_t next_sub(uint32_t f0, size_t max_bytes, size_t* bytes) const {
+        size_t b = size(f0); uint32_t e = f0 + 1;
+        if (!sizes) {                 // frames before the last are full: the same rule in closed form
+            const uint32_t per = frame_size <= max_bytes ? (uint32_t)(max_bytes / frame_size) : 1u;
+            e = count - f0 < per ? count : f0 + per;
+            b = (e == count ? n : (size_t)e * frame_size) - (size_t)f0 * frame_size;
+            if (e < count && b + size(e) <= max_bytes) { b += size(e); e++; }   // a short last frame that still fits
+        } else while (e < count && b + sizes[e] <= max_bytes) b += sizes[e++];
+        *bytes = b;
+        return e;
+    }
+    // frames [f0, f0 + cnt), which cover `bytes`
+    ZkFrames sub(uint32_t f0, uint32_t cnt, size_t bytes) const { return {sizes ? sizes + f0 : nullptr, bytes, frame_size, cnt}; }
+    size_t bound() const;             // the most bytes they compress to
+};
+
+// Enqueue the compression of `fr`, read back to back from d_src, into frames written back to back at d_dst.  zk_encode_collect then waits
+// for it: c_sizes (host, one entry per frame) receives each frame's compressed size, *dst_len the bytes written.
+int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, const ZkFrames& fr, const ZkEncodeParams& p, uint8_t* d_dst,
+                      size_t dst_cap);
 int zk_encode_collect(ZkEncodeWs* ws, cudaStream_t stream, uint32_t* c_sizes, size_t* dst_len);
 void zk_encode_ws_free(ZkEncodeWs* ws);
 size_t zk_encode_bound(size_t n, uint32_t frame_size);
@@ -42,8 +70,8 @@ struct ZkCsizeOut {
     const uint32_t* c_sizes = nullptr;   // n_frames compressed sizes
     const uint32_t* starts = nullptr;    // n_frames + 1 first blocks (32 KiB units from d_src); the last one is the end of the last frame
 };
-int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t target, int level, int checksum,
-                    int final_, int at_end, const uint8_t* d_prefix, uint32_t prefix_len, uint8_t* d_dst, size_t dst_cap, ZkCsizeOut* out);
+int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t target, const ZkEncodeParams& p, int final_,
+                    int at_end, uint8_t* d_dst, size_t dst_cap, ZkCsizeOut* out);
 
 // FrameSizePolicy::ContentDefined(size): size clamped to [4096, 2^30]; frames of mn .. mx bytes end at the first position whose 64-byte gear
 // hash is >= thr (zk_cdc.inc states the rule)
