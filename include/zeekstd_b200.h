@@ -222,6 +222,33 @@ int32_t zk_compress_frames_sized_ldm(zk_ctx* ctx, const uint8_t* src, const uint
                                      int32_t checksum, const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap,
                                      uint32_t* c_sizes, size_t* dst_len);
 
+/*
+ * Long mode (what `zstd --long` does within a frame): zk_compress_frames_prefix / zk_compress_frames_sized with every frame also matched
+ * against ITS OWN earlier bytes up to the window back, not only the last 2 MiB that level 16 searches.  A frame of many MiB that repeats
+ * itself far apart (a disk image, a tar of similar trees, a log rotated twice) shrinks to what differs.  Frames stay independent: a
+ * frame's bytes depend only on its own bytes, the checksum flag and the prefix, never on its neighbours in the batch, the sub-batch size,
+ * host vs device memory or where the encoder's internal passes cut the batch, so the sized call equals one call per frame.  A non-empty
+ * frame announces a Window_Size of min(max(frame content + prefix_len, 128 KiB), 2^27), as with zk_compress_frames_ldm, and no offset
+ * exceeds it.  With a prefix, every frame
+ * is also matched against the whole prefix exactly as by zk_compress_frames_ldm, so long mode is a superset of that switch; without one it
+ * needs none.  Long matches are at least 64 bytes.  Part of the high-level tier: every `level` writes what level 16 writes here.  The
+ * index of the input costs about 1 byte of device scratch per input byte and is rebuilt on every call.  zk_compress_frames_csize and
+ * zk_compress_frames_cdc have no such variant.  HOST pointers; the _dev pair takes device src / dst (sizes on the host) and no prefix, like
+ * every _dev entry point.
+ */
+int32_t zk_compress_frames_long(zk_ctx* ctx, const uint8_t* src, size_t n, uint32_t frame_size, int32_t level,
+                                int32_t checksum, const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap,
+                                uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len);
+int32_t zk_compress_frames_sized_long(zk_ctx* ctx, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                      int32_t checksum, const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap,
+                                      uint32_t* c_sizes, size_t* dst_len);
+int32_t zk_compress_frames_long_dev(zk_ctx* ctx, const void* d_src, size_t n, uint32_t frame_size, int32_t level, int32_t checksum,
+                                    void* d_dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap,
+                                    uint32_t* n_frames, size_t* dst_len, void* cuda_stream);
+int32_t zk_compress_frames_sized_long_dev(zk_ctx* ctx, const void* d_src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                          int32_t checksum, void* d_dst, size_t dst_cap, uint32_t* c_sizes, size_t* dst_len,
+                                          void* cuda_stream);
+
 /* ------------------------------------------------------------------ SeekTable (lib/src/seek_table.rs) */
 typedef struct zk_seek_table zk_seek_table;
 typedef enum { ZK_FORMAT_HEAD = 0, ZK_FORMAT_FOOT = 1 } zk_format; /* seek_table.rs:228-241 */
@@ -278,6 +305,11 @@ void zk_encode_options_compression_level(zk_encode_options* o, int32_t level);  
  * under both policies (its trial compressions included), Encoder under Uncompressed(n): with Compressed(n) or ContentDefined(n)
  * zk_encode_options_into_encoder returns ZK_ERR_INVALID_ARG and does not consume the options */
 void zk_encode_options_long_distance_matching(zk_encode_options* o, int32_t flag);
+/* flag != 0: long mode (zk_compress_frames_long): every frame is also matched against its own bytes up to 2^27 back, and frames given a
+ * prefix against the whole of it; every level then runs as level 16.  Independent of the long-distance switch above, and a superset of
+ * it.  RawEncoder honours it under both policies, Encoder under Uncompressed(n): with Compressed(n) or ContentDefined(n)
+ * zk_encode_options_into_encoder returns ZK_ERR_INVALID_ARG and does not consume the options */
+void zk_encode_options_long_mode(zk_encode_options* o, int32_t flag);
 /* consume the options (like `self`).  ZK_POLICY_CONTENT: Encoder only (it buffers and cuts like Compressed(n), through
  * zk_compress_frames_cdc); zk_encode_options_into_raw_encoder returns ZK_ERR_INVALID_ARG for it, since a RawEncoder reports each call's
  * progress before the frame's end is known, and does not consume the options */

@@ -135,10 +135,13 @@ class Context:
     def last_device_ms(self) -> float: return float(self.lib.zk_ctx_last_device_ms(self._h))
 
     # ---- batch codec (the hot path) ------------------------------------------------------------
-    def compress_frames(self, data, frame_size: int = 0x200000, level: int = 0, checksum: bool = False, prefix=None, long_distance: bool = False):
+    def compress_frames(self, data, frame_size: int = 0x200000, level: int = 0, checksum: bool = False, prefix=None, long_distance: bool = False,
+                        long_mode: bool = False):
         """-> (compressed bytes (np.uint8), c_sizes, d_sizes).  Host buffers.  prefix: raw-content prefix of every frame.
         long_distance: match every frame against the whole prefix (its last 128 MiB), not only its last 32 KiB: patch mode.  Every level
-        then writes what level 16 writes; without a prefix the flag changes nothing."""
+        then writes what level 16 writes; without a prefix the flag changes nothing.
+        long_mode: match every frame also against its own bytes up to 2^27 back (zstd --long), and against the whole prefix as
+        long_distance does; every level writes what level 16 writes."""
         addr, n, keep = _buf(data)
         lib = self.lib
         cap = lib.zk_compress_bound(n, frame_size)
@@ -146,9 +149,9 @@ class Context:
         nfmax = n // max(frame_size, 1) + 2
         cs = np.zeros(nfmax, dtype=np.uint32); ds = np.zeros(nfmax, dtype=np.uint32)
         nf = c_uint32(); dl = c_size_t()
-        if prefix is not None:
-            paddr, pn, pkeep = _buf(prefix)
-            fn = lib.zk_compress_frames_ldm if long_distance else lib.zk_compress_frames_prefix
+        if prefix is not None or long_mode:
+            paddr, pn, pkeep = _buf(prefix) if prefix is not None else (None, 0, None)
+            fn = lib.zk_compress_frames_long if long_mode else lib.zk_compress_frames_ldm if long_distance else lib.zk_compress_frames_prefix
             _check(fn(self._h, addr, n, frame_size, level, int(checksum), paddr, pn, dst.ctypes.data, cap,
                                                  cs.ctypes.data_as(_native.u32p), ds.ctypes.data_as(_native.u32p), nfmax, byref(nf), byref(dl)), lib)
         else:
@@ -157,10 +160,11 @@ class Context:
                                           byref(dl)), lib)
         return dst[: dl.value], cs[: nf.value].copy(), ds[: nf.value].copy()
 
-    def compress_frames_sized(self, data, frame_sizes, level: int = 0, checksum: bool = False, prefix=None, long_distance: bool = False):
+    def compress_frames_sized(self, data, frame_sizes, level: int = 0, checksum: bool = False, prefix=None, long_distance: bool = False,
+                              long_mode: bool = False):
         """frames of caller-chosen sizes in one batch: frame f covers the next frame_sizes[f] bytes of data (their sum is its length)
         -> (compressed bytes (np.uint8), c_sizes, d_sizes).  Each frame is what compress_frames makes of its bytes alone
-        (long_distance as there)."""
+        (long_distance and long_mode as there)."""
         addr, n, keep = _buf(data)
         ds = np.ascontiguousarray(frame_sizes, dtype=np.uint32).reshape(-1)
         if int(np.sum(ds, dtype=np.uint64)) != n:
@@ -172,7 +176,7 @@ class Context:
         cs = np.zeros(ds.size, dtype=np.uint32)
         dl = c_size_t()
         paddr, pn, pkeep = _buf(prefix) if prefix is not None else (None, 0, None)
-        fn = lib.zk_compress_frames_sized_ldm if long_distance else lib.zk_compress_frames_sized
+        fn = lib.zk_compress_frames_sized_long if long_mode else lib.zk_compress_frames_sized_ldm if long_distance else lib.zk_compress_frames_sized
         _check(fn(self._h, addr, dsp, ds.size, level, int(checksum), paddr, pn, dst.ctypes.data, cap,
                                             cs.ctypes.data_as(_native.u32p), byref(dl)), lib)
         return dst[: dl.value], cs, ds.copy()
@@ -361,6 +365,7 @@ class EncodeOptions:
         self._checksum = False
         self._level = 0
         self._ldm = False
+        self._long = False
 
     def frame_size_policy(self, policy: FrameSizePolicy): self._policy = policy; return self
     def checksum_flag(self, flag: bool): self._checksum = bool(flag); return self
@@ -372,6 +377,12 @@ class EncodeOptions:
         FrameSizePolicy.ContentDefined"""
         self._ldm = bool(flag); return self
 
+    def long_mode(self, flag: bool):
+        """match every frame also against its own bytes up to 2^27 back (zstd --long), and the frames of compress_with_prefix against
+        the whole prefix as long_distance_matching does.  Every level then runs as level 16; into_encoder refuses it with
+        FrameSizePolicy.Compressed and FrameSizePolicy.ContentDefined"""
+        self._long = bool(flag); return self
+
     def _native_opts(self):
         lib = self.ctx.lib
         o = c_void_p(lib.zk_encode_options_new(self.ctx._h))
@@ -379,6 +390,7 @@ class EncodeOptions:
         lib.zk_encode_options_checksum_flag(o, int(self._checksum))
         lib.zk_encode_options_compression_level(o, self._level)
         lib.zk_encode_options_long_distance_matching(o, int(self._ldm))
+        lib.zk_encode_options_long_mode(o, int(self._long))
         return o
 
     def into_raw_encoder(self): return RawEncoder(self)

@@ -79,6 +79,14 @@ _SIGS = {
                                          u32p, u32p, c_uint32, u32p, POINTER(c_size_t)]),
     "zk_compress_frames_sized_ldm": (c_int32, [c_void_p, c_void_p, u32p, c_uint32, c_int32, c_int32, c_void_p, c_size_t, c_void_p, c_size_t,
                                                u32p, POINTER(c_size_t)]),
+    "zk_compress_frames_long": (c_int32, [c_void_p, c_void_p, c_size_t, c_uint32, c_int32, c_int32, c_void_p, c_size_t, c_void_p, c_size_t,
+                                          u32p, u32p, c_uint32, u32p, POINTER(c_size_t)]),
+    "zk_compress_frames_sized_long": (c_int32, [c_void_p, c_void_p, u32p, c_uint32, c_int32, c_int32, c_void_p, c_size_t, c_void_p, c_size_t,
+                                                u32p, POINTER(c_size_t)]),
+    "zk_compress_frames_long_dev": (c_int32, [c_void_p, c_void_p, c_size_t, c_uint32, c_int32, c_int32, c_void_p, c_size_t,
+                                              u32p, u32p, c_uint32, u32p, POINTER(c_size_t), c_void_p]),
+    "zk_compress_frames_sized_long_dev": (c_int32, [c_void_p, c_void_p, u32p, c_uint32, c_int32, c_int32, c_void_p, c_size_t, u32p,
+                                                    POINTER(c_size_t), c_void_p]),
     # seek table
     "zk_seek_table_new": (c_void_p, []),
     "zk_seek_table_free": (None, [c_void_p]),
@@ -111,6 +119,7 @@ _SIGS = {
     "zk_encode_options_checksum_flag": (None, [c_void_p, c_int32]),
     "zk_encode_options_compression_level": (None, [c_void_p, c_int32]),
     "zk_encode_options_long_distance_matching": (None, [c_void_p, c_int32]),
+    "zk_encode_options_long_mode": (None, [c_void_p, c_int32]),
     "zk_encode_options_into_raw_encoder": (c_int32, [c_void_p, POINTER(c_void_p)]),
     "zk_encode_options_into_encoder": (c_int32, [c_void_p, WRITE_FN, FLUSH_FN, c_void_p, POINTER(c_void_p)]),
     "zk_raw_encoder_free": (None, [c_void_p]),

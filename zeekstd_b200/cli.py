@@ -1,6 +1,6 @@
 """Command-line front end with the reference CLI's arguments and behaviour (SURVEY.md 8f.4), over the GPU codec.
 
-    python -m zeekstd_b200 [compress] [-l N] [-s 2M] [--frame-size-policy ..] [--patch-from F [--long]] [INPUT] [-o OUT]
+    python -m zeekstd_b200 [compress] [-l N] [-s 2M] [--frame-size-policy ..] [--patch-from F [--long]] [--long-mode] [INPUT] [-o OUT]
     python -m zeekstd_b200 decompress [--from N | --from-frame I] [--to N|end | --to-frame I|end] [--patch-apply F] INPUT [-o OUT]
     python -m zeekstd_b200 list [--from-frame I] [--to-frame I|end | --num-frames N] [-d] [--seek-table-format head|foot] INPUT
 
@@ -14,7 +14,10 @@ at -131072).  `--patch-from F` alone matches every frame against the last 32 KiB
 window-log / long-distance-matching parameters the reference sets for patch files take effect: every frame is matched against
 the whole of F (its last 128 MiB when it is larger), which is what makes the archive a patch.  Long-distance matching is part
 of the high-level tier, so with `--long` every compression level writes what level 16 writes, and the frame size policy must be
-`uncompressed`.  `--mmap-prefix` / `--no-mmap-prefix` choose between np.memmap and a read.  `--frame-size-policy content` (an
+`uncompressed`.  `--long-mode` is a different switch, with or without `--patch-from`: every frame is also matched against its own
+bytes up to 128 MiB back (what `zstd --long` does), so large frames (`-s 64M`) find repeats that lie beyond level 16's 2 MiB
+window; with `--patch-from` it also matches the whole of F as `--long` does.  It too runs every level as level 16 and needs
+`--frame-size-policy uncompressed`.  `--mmap-prefix` / `--no-mmap-prefix` choose between np.memmap and a read.  `--frame-size-policy content` (an
 extension of this codec) ends frames where a rolling hash of the data says so, about `-s` bytes apart on average, so that an edit
 of the input changes only the frames around it and rsync, dedup stores and range-fetching clients can reuse the rest.
 """
@@ -150,6 +153,10 @@ def build_parser() -> argparse.ArgumentParser:
     c.add_argument("--long", action="store_true",
                    help="With --patch-from: long-distance matching against the whole reference file (its last 128 MiB), so that the archive "
                         "is a patch. Every compression level then runs as level 16; needs --frame-size-policy uncompressed.")
+    c.add_argument("--long-mode", action="store_true",
+                   help="Match every frame also against its own bytes up to 128 MiB back (zstd --long), and with --patch-from against the "
+                        "whole reference file as --long does: large frames find far repeats. Every compression level then runs as level 16; "
+                        "needs --frame-size-policy uncompressed.")
     c.add_argument("input_file", nargs="?", default="-")
     c.add_argument("-o", "--output-file", default=None)
 
@@ -322,6 +329,8 @@ def _run_compress(zk, ns, fmt_bytes) -> int:
         raise CliError("--long needs --patch-from: long-distance matching runs against the reference file")
     if ns.long and ns.frame_size_policy in ("compressed", "content"):
         raise CliError("--long needs --frame-size-policy uncompressed")
+    if ns.long_mode and ns.frame_size_policy in ("compressed", "content"):
+        raise CliError("--long-mode needs --frame-size-policy uncompressed")
     prefix_len = os.path.getsize(ns.patch_from) if ns.patch_from and os.path.exists(ns.patch_from) else None
     st_file = None
     if ns.seek_table_file is not None:
@@ -336,7 +345,8 @@ def _run_compress(zk, ns, fmt_bytes) -> int:
     policy = {"compressed": zk.FrameSizePolicy.Compressed, "uncompressed": zk.FrameSizePolicy.Uncompressed,
               "content": zk.FrameSizePolicy.ContentDefined}[ns.frame_size_policy](ns.frame_size)
     enc = (zk.EncodeOptions().frame_size_policy(policy).checksum_flag(not ns.no_checksum)
-           .compression_level(ns.compression_level).long_distance_matching(ns.long).into_encoder(writer))
+           .compression_level(ns.compression_level).long_distance_matching(ns.long).long_mode(ns.long_mode)
+           .into_encoder(writer))
     prefix = _load_prefix(ns.patch_from, _use_mmap(ns, prefix_len))
 
     read = 0

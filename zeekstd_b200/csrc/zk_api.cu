@@ -677,6 +677,51 @@ extern "C" int32_t zk_compress_frames_sized_ldm(zk_ctx* c, const uint8_t* src, c
 }
 
 // ---------------------------------------------------------------------------------------------
+// long mode (zstd --long): the calls above with K-C1h also matching every frame against its own bytes up to 2^27 back (zk_ldm.inc),
+// and against the whole prefix as the _ldm calls do
+// ---------------------------------------------------------------------------------------------
+extern "C" int32_t zk_compress_frames_long(zk_ctx* c, const uint8_t* src, size_t n, uint32_t frame_size, int32_t level, int32_t checksum,
+                                           const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap, uint32_t* c_sizes,
+                                           uint32_t* d_sizes, uint32_t frames_cap, uint32_t* n_frames, size_t* dst_len) {
+    ZkCompressReq q;
+    q.size = frame_size; q.src = src; q.n = n; q.prefix = prefix; q.prefix_len = prefix_len;
+    q.params.level = level; q.params.checksum = checksum; q.params.long_mode = true;
+    q.dst = dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.d_sizes = d_sizes; q.frames_cap = frames_cap; q.n_frames = n_frames; q.dst_len = dst_len;
+    return zk_compress(c, q);
+}
+
+extern "C" int32_t zk_compress_frames_sized_long(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                                 int32_t checksum, const uint8_t* prefix, size_t prefix_len, uint8_t* dst, size_t dst_cap,
+                                                 uint32_t* c_sizes, size_t* dst_len) {
+    ZkCompressReq q;
+    q.policy = ZK_FRAMES_SIZED; q.sizes = frame_sizes; q.count = n_frames; q.src = src; q.prefix = prefix; q.prefix_len = prefix_len;
+    q.params.level = level; q.params.checksum = checksum; q.params.long_mode = true;
+    q.dst = dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.dst_len = dst_len;
+    return zk_compress(c, q);
+}
+
+extern "C" int32_t zk_compress_frames_long_dev(zk_ctx* c, const void* d_src, size_t n, uint32_t frame_size, int32_t level, int32_t checksum,
+                                               void* d_dst, size_t dst_cap, uint32_t* c_sizes, uint32_t* d_sizes, uint32_t frames_cap,
+                                               uint32_t* n_frames, size_t* dst_len, void* cuda_stream) {
+    ZkCompressReq q;
+    q.size = frame_size; q.src = (const uint8_t*)d_src; q.n = n; q.host = false; q.stream = (cudaStream_t)cuda_stream;
+    q.params.level = level; q.params.checksum = checksum; q.params.long_mode = true;
+    q.dst = (uint8_t*)d_dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.d_sizes = d_sizes; q.frames_cap = frames_cap; q.n_frames = n_frames;
+    q.dst_len = dst_len;
+    return zk_compress(c, q);
+}
+
+extern "C" int32_t zk_compress_frames_sized_long_dev(zk_ctx* c, const void* d_src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                                     int32_t checksum, void* d_dst, size_t dst_cap, uint32_t* c_sizes, size_t* dst_len,
+                                                     void* cuda_stream) {
+    ZkCompressReq q;
+    q.policy = ZK_FRAMES_SIZED; q.sizes = frame_sizes; q.count = n_frames; q.src = (const uint8_t*)d_src; q.host = false;
+    q.stream = (cudaStream_t)cuda_stream; q.params.level = level; q.params.checksum = checksum; q.params.long_mode = true;
+    q.dst = (uint8_t*)d_dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.dst_len = dst_len;
+    return zk_compress(c, q);
+}
+
+// ---------------------------------------------------------------------------------------------
 // Frame sizes decided on the GPU: FrameSizePolicy::Compressed(target) and ::ContentDefined(size)
 // ---------------------------------------------------------------------------------------------
 extern "C" int32_t zk_compress_frames_csize(zk_ctx* c, const uint8_t* src, size_t n, uint32_t target, int32_t level, int32_t checksum,

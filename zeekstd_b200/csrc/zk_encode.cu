@@ -1563,12 +1563,15 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     }
     if (n_blocks > 0x7FFFFFFFull) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
     const uint32_t pt = p.prefix && p.prefix_len && n ? (p.prefix_len < ZKC_BLOCK ? p.prefix_len : ZKC_BLOCK) : 0u;
-    // long-distance matching is a part of K-C1h: with it every level runs that tier
-    const bool ldm = p.ldm && pt;
-    const int lvl = ldm ? ZKC_HC_LEVEL : zkc_level(p.level);
+    // long-distance matching is a part of K-C1h: with it every level runs that tier.  Long mode indexes the input too (positions are u32)
+    // and matches the prefix as the long-distance switch does
+    if (p.long_mode && n > 0xFFFFFFFFull) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
+    const bool ldm = (p.ldm || p.long_mode) && pt, lin = p.long_mode && n;
+    const int lvl = ldm || p.long_mode ? ZKC_HC_LEVEL : zkc_level(p.level);
     ZkcHcRun hc;
     const uint32_t hc_span = lvl >= ZKC_HC_LEVEL ? zkc_hc_plan(fr, (uint32_t)n_blocks, pt, hc.plan) : 0u;
     if (ldm) hc.reach = p.prefix_len < ZKC_LDM_REACH ? p.prefix_len : ZKC_LDM_REACH;
+    hc.input = lin;
     // carve the workspace
     size_t off = 0;
     const size_t o_geo = off; off = zkc_align(off + n_blocks * sizeof(ZkcGeo));
@@ -1589,7 +1592,7 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     const size_t o_hc = off;
     if (lvl >= ZKC_HC_LEVEL) off = zkc_align(off + zkc_hc_layout(hc_span, nullptr, nullptr));
     const size_t o_ldm = off;
-    if (ldm) off = zkc_align(off + zkc_ldm_layout(hc.reach, n_blocks, nullptr, nullptr, nullptr));
+    if (ldm || lin) off = zkc_align(off + zkc_ldm_layout(hc.reach, lin ? (uint32_t)n_blocks * ZKC_LDM_BSLOTS : 0u, n_blocks, nullptr, nullptr, nullptr, nullptr));
     int rc = zk_grow(&ws->buf, &ws->cap, off, 1);
     if (!rc) rc = zk_grow((void**)&ws->h_sizes, &ws->cap_frames, (size_t)n_frames + 4, 4, true);     // the sizes, then the total and the error
     if (rc) return rc;
@@ -1606,7 +1609,7 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     a.prefix = p.prefix; a.prefix_len = 0; a.ptail = 0; a.pstage = base + o_pst;
     a.hist_cap = ~(size_t)0;
     a.hc = base + o_hc;
-    if (ldm) hc.ldm = base + o_ldm;
+    if (ldm || lin) hc.ldm = base + o_ldm;
     rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo), (ZkcFrame*)(base + o_fr), fr, (uint32_t)n_blocks, (uint32_t*)(base + o_fsz));
     if (rc) return rc;
     if (pt) {
@@ -1630,7 +1633,7 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     ZK_LAUNCH(zk_frame_size_kernel, (n_frames + 255) / 256, 256, 0, stream, a);
     ZK_LAUNCH(zk_frame_scan_kernel, 1, 1024, 0, stream, a);
     ZK_LAUNCH(zk_frame_gather_kernel, (uint32_t)((n_blocks + 3) / 4), 128, 0, stream, a);
-    if (ldm) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 128u << 10, 1u << 27, p.prefix_len); ws->launches++; }
+    if (ldm || p.long_mode) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 128u << 10, 1u << 27, ldm ? p.prefix_len : 0u); ws->launches++; }
     else if (a.level >= ZKC_HC_LEVEL) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 128u << 10, ZKC_HC_WINDOW, pt); ws->launches++; }
     else if (a.level >= ZKC_WIDE_LEVEL) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 256u << 10, 256u << 10, pt); ws->launches++; }
     ws->prof.end(7, stream);

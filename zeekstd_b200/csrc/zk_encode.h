@@ -20,6 +20,7 @@ struct ZkEncodeParams {
     int level = 0, checksum = 0;
     const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device memory: the raw-content prefix of every frame (nullptr: none)
     bool ldm = false;                 // long-distance matching against the whole prefix (nothing without one)
+    bool long_mode = false;           // long mode: every frame also matches its own bytes up to 2^27 back (and the prefix as ldm does)
     bool side = true;                 // K-C2s and the checksum on the side stream; host pipelines get their concurrency from the other
                                       // sub-batches instead, and every extra stream costs a hardware queue
 };

@@ -242,6 +242,7 @@ struct zk_encode_options {                 // encode.rs:110-207
     zk_ctx* ctx; zk_frame_size_policy kind = ZK_POLICY_UNCOMPRESSED; uint32_t size = ZK_DEFAULT_FRAME_SIZE;
     int32_t checksum = 0; int32_t level = 0;           // CompressionLevel::default() == 0 -> codec default
     int32_t ldm = 0;                                   // long-distance matching against the prefix of compress_with_prefix
+    int32_t lmode = 0;                                 // long mode: frames also match their own bytes up to 2^27 back (zk_compress_frames_long)
 };
 extern "C" zk_encode_options* zk_encode_options_new(zk_ctx* ctx) {
     if (!ctx) return nullptr;
@@ -252,9 +253,10 @@ extern "C" void zk_encode_options_frame_size_policy(zk_encode_options* o, zk_fra
 extern "C" void zk_encode_options_checksum_flag(zk_encode_options* o, int32_t flag) { o->checksum = flag ? 1 : 0; }
 extern "C" void zk_encode_options_compression_level(zk_encode_options* o, int32_t level) { o->level = level; }
 extern "C" void zk_encode_options_long_distance_matching(zk_encode_options* o, int32_t flag) { o->ldm = flag ? 1 : 0; }
+extern "C" void zk_encode_options_long_mode(zk_encode_options* o, int32_t flag) { o->lmode = flag ? 1 : 0; }
 
 struct zk_raw_encoder {                    // encode.rs:266-545
-    zk_ctx* ctx; zk_frame_size_policy kind; uint32_t size; int32_t checksum, level, ldm = 0;
+    zk_ctx* ctx; zk_frame_size_policy kind; uint32_t size; int32_t checksum, level, ldm = 0, lmode = 0;
     uint32_t frame_c_size = 0, frame_d_size = 0;
     zk_seek_table seek_table;
     std::vector<uint8_t> in_buf;           // uncompressed bytes of the frame being built (whole frames go to the GPU)
@@ -279,7 +281,7 @@ struct zk_raw_encoder {                    // encode.rs:266-545
         out_buf.resize(cap);
         uint32_t cs = 0, ds = 0, nf = 0; size_t len = 0;
         static const uint8_t dummy = 0;
-        int32_t rc = (ldm ? zk_compress_frames_ldm : zk_compress_frames_prefix)(ctx, in_buf.empty() ? &dummy : in_buf.data(), in_buf.size(),
+        int32_t rc = (lmode ? zk_compress_frames_long : ldm ? zk_compress_frames_ldm : zk_compress_frames_prefix)(ctx, in_buf.empty() ? &dummy : in_buf.data(), in_buf.size(),
                                                (uint32_t)std::max<size_t>(in_buf.size(), 1), level, checksum, prefix, prefix_len, out_buf.data(), cap, &cs, &ds, 1, &nf, &len);
         if (rc) return rc;
         out_buf.resize(len);
@@ -295,7 +297,7 @@ extern "C" int32_t zk_encode_options_into_raw_encoder(zk_encode_options* o, zk_r
     if (o->kind == ZK_POLICY_CONTENT) return ZK_ERR_INVALID_ARG;
     zk_raw_encoder* e = new (std::nothrow) zk_raw_encoder();
     if (!e) return ZK_ERR_ZSTD(64);
-    e->ctx = o->ctx; e->kind = o->kind; e->size = o->size; e->checksum = o->checksum; e->level = o->level; e->ldm = o->ldm;
+    e->ctx = o->ctx; e->kind = o->kind; e->size = o->size; e->checksum = o->checksum; e->level = o->level; e->ldm = o->ldm; e->lmode = o->lmode;
     delete o;
     *out = e;
     return 0;
@@ -400,7 +402,7 @@ struct zk_encoder {
         std::vector<uint32_t> cs(nfmax), ds(nfmax);
         uint32_t nf = 0; size_t len = 0;
         static const uint8_t dummy = 0;
-        int32_t rc = (raw.ldm ? zk_compress_frames_ldm : zk_compress_frames_prefix)(raw.ctx, count ? batch.data() : &dummy, count, fs, raw.level, raw.checksum,
+        int32_t rc = (raw.lmode ? zk_compress_frames_long : raw.ldm ? zk_compress_frames_ldm : zk_compress_frames_prefix)(raw.ctx, count ? batch.data() : &dummy, count, fs, raw.level, raw.checksum,
                                                prefix, prefix_len, stage.data(), cap, cs.data(), ds.data(), nfmax, &nf, &len);
         if (rc) return rc;
         for (uint32_t i = 0; i < nf; i++) { rc = zk_seek_table_log_frame(&raw.seek_table, cs[i], ds[i]); if (rc) return rc; }
@@ -439,10 +441,10 @@ extern "C" int32_t zk_encode_options_into_encoder(zk_encode_options* o, zk_write
     if (!o || !out || !write) return ZK_ERR_INVALID_ARG;
     // the exact cut of Compressed(n) needs a bounded history per block, which the tier that matches over long distances does not have;
     // content-defined frames are meant to stand alone
-    if ((o->kind == ZK_POLICY_COMPRESSED || o->kind == ZK_POLICY_CONTENT) && o->ldm) return ZK_ERR_INVALID_ARG;
+    if ((o->kind == ZK_POLICY_COMPRESSED || o->kind == ZK_POLICY_CONTENT) && (o->ldm || o->lmode)) return ZK_ERR_INVALID_ARG;
     zk_encoder* e = new (std::nothrow) zk_encoder();
     if (!e) return ZK_ERR_ZSTD(64);
-    e->raw.ctx = o->ctx; e->raw.kind = o->kind; e->raw.size = o->size; e->raw.checksum = o->checksum; e->raw.level = o->level; e->raw.ldm = o->ldm;
+    e->raw.ctx = o->ctx; e->raw.kind = o->kind; e->raw.size = o->size; e->raw.checksum = o->checksum; e->raw.level = o->level; e->raw.ldm = o->ldm; e->raw.lmode = o->lmode;
     e->write = write; e->flush = flush; e->user = user;
     const char* bf = getenv("ZK_ENCODER_BATCH_FRAMES");
     if (bf && atoi(bf) > 0) e->batch_frames = (size_t)atoi(bf);

@@ -71,8 +71,10 @@ class DeviceCodec:
     def compress_bound(self, n: int, frame_size: int) -> int:
         return int(self.lib.zk_compress_bound(n, frame_size))
 
-    def compress_into(self, src: torch.Tensor, n: int, frame_size: int, level: int, checksum: bool, dst: torch.Tensor):
+    def compress_into(self, src: torch.Tensor, n: int, frame_size: int, level: int, checksum: bool, dst: torch.Tensor,
+                      long_mode: bool = False):
         """src[:n] -> frames written from dst[0]; src and dst are views with PAD readable / writable bytes behind them.
+        long_mode: every frame also matches its own bytes up to 2^27 back (zk_compress_frames_long_dev).
         -> (bytes written, c_sizes, d_sizes)"""
         if src.data_ptr() % 16:
             src = torch.cat([src[:n], torch.zeros(self.PAD, dtype=torch.uint8, device=src.device)])
@@ -80,11 +82,12 @@ class DeviceCodec:
         cs = np.zeros(nfmax, dtype=np.uint32); ds = np.zeros(nfmax, dtype=np.uint32)
         nf = ctypes.c_uint32(); dl = ctypes.c_size_t()
         cap = min(self.compress_bound(n, frame_size), dst.numel())
-        rc = self.lib.zk_compress_frames_dev(self.ctx._h, src.data_ptr(), n, frame_size, level, int(checksum), dst.data_ptr(), cap,
-                                             cs.ctypes.data_as(_native.u32p), ds.ctypes.data_as(_native.u32p), nfmax, ctypes.byref(nf),
-                                             ctypes.byref(dl), torch_stream_handle(src.device))
+        name = "zk_compress_frames_long_dev" if long_mode else "zk_compress_frames_dev"
+        rc = getattr(self.lib, name)(self.ctx._h, src.data_ptr(), n, frame_size, level, int(checksum), dst.data_ptr(), cap,
+                cs.ctypes.data_as(_native.u32p), ds.ctypes.data_as(_native.u32p), nfmax, ctypes.byref(nf),
+                ctypes.byref(dl), torch_stream_handle(src.device))
         if rc:
-            raise RuntimeError(f"zk_compress_frames_dev: {rc}")
+            raise RuntimeError(f"{name}: {rc}")
         self.device_ms += self.ctx.last_device_ms
         return int(dl.value), cs[: nf.value].astype(np.int64), ds[: nf.value].astype(np.int64)
 
@@ -106,11 +109,11 @@ class DeviceCodec:
             dst[: int(do[-1])] = tmp[: int(do[-1])]
 
     # whole-buffer conveniences (tools, tests)
-    def compress(self, x: torch.Tensor, frame_size: int, level: int, checksum: bool):
+    def compress(self, x: torch.Tensor, frame_size: int, level: int, checksum: bool, long_mode: bool = False):
         n = x.numel()
         src = torch.cat([x, torch.zeros(self.PAD, dtype=torch.uint8, device=x.device)])
         dst = self.empty(self.compress_bound(n, frame_size), x.device)
-        k, cs, ds = self.compress_into(src, n, frame_size, level, checksum, dst)
+        k, cs, ds = self.compress_into(src, n, frame_size, level, checksum, dst, long_mode)
         return dst[:k], cs, ds
 
     def compress_csize(self, x: torch.Tensor, target: int, level: int, checksum: bool, final: bool = True):
