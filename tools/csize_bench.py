@@ -43,7 +43,7 @@ def timed(fn, runs: int):
 
 PHASES = (("variants", ("zk_match", "zk_seq_enc", "zk_lit_enc", "zk_block_finish", "zk_prefix_stage")),
           ("cut", ("zk_csize_psum", "zk_csize_next", "zk_csize_walk")),
-          ("assembly", ("zk_csize_frame", "zk_csize_scan", "zk_csize_gather")))
+          ("assembly", ("zk_geo_starts", "zk_geo_block", "zk_frame_")))
 
 
 def kernel_split(fn) -> dict:

@@ -499,21 +499,14 @@ static int32_t zk_frame_passes(zk_ctx* c, const ZkCompressReq& q, cudaStream_t s
 
 // Compressed(target) (zk_encode_csize): the cut and the frames in one step; frames start at 32 KiB blocks
 static int32_t zk_csize_passes(zk_ctx* c, const ZkCompressReq& q, cudaStream_t st, size_t first_pass) {
-    const size_t block = 32768;
-    std::vector<uint32_t> ds;
     auto step = [&](const uint8_t* d_in, size_t len, int at_end, uint8_t* d_out, size_t cap, ZkPassOut* o) -> int32_t {
         ZkCsizeOut r;
         const int rc = zk_encode_csize(&c->slot[0].ews, st, d_in, len, q.size, q.params, q.final_, at_end, d_out, cap, &r);
         if (rc) return rc;
-        ds.resize(r.n_frames);
-        for (uint32_t f = 0; f < r.n_frames; f++) {
-            const size_t lo = (size_t)r.starts[f] * block, hi = (size_t)r.starts[f + 1] * block < len ? (size_t)r.starts[f + 1] * block : len;
-            ds[f] = (uint32_t)(hi - lo);
-        }
-        o->n_frames = r.n_frames; o->consumed = r.consumed; o->total = r.total; o->c_sizes = r.c_sizes; o->d_sizes = ds.data();
+        o->n_frames = r.n_frames; o->consumed = r.consumed; o->total = r.total; o->c_sizes = r.c_sizes; o->d_sizes = r.d_sizes;
         return 0;
     };
-    return zk_frame_passes(c, q, st, first_pass, ZK_SEEKABLE_MAX_FRAME_SIZE, (uint32_t)block, step);
+    return zk_frame_passes(c, q, st, first_pass, ZK_SEEKABLE_MAX_FRAME_SIZE, 32768u, step);
 }
 
 // ContentDefined(size): each pass is cut on the GPU (zk_encode_cdc), then its closed frames are compressed from the same device memory by

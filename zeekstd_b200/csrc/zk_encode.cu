@@ -11,7 +11,8 @@
 //   K-C2s zk_seq_enc_kernel  one warp / block : FSE sequences (three lanes run the state chains, 32 lanes pack the bits)
 //   K-C2l zk_lit_enc_kernel  one warp / block : Huffman literals (tree build, FSE-coded weights, 4 streams packed by warp scan), 4 warps / CTA
 //   K-C2f zk_block_finish_kernel              : joins the two sections of a block (coded on two streams), Raw fallback, header
-//   K-C3 zk_frame_{hash,size,scan,gather}_kernel : optional XXH64, frame sizes, offsets, frame headers + block gather
+//   K-C3 zk_frame_{hash,size,scan,gather}_kernel : optional XXH64, frame sizes, offsets, frame headers + block gather, over the
+//                                               frame and block tables (zk_geo_*_kernel, or the cut of K-C3c zk_csize_*_kernel)
 //
 // Output is a standard Zstandard frame per seek-table entry (RFC 8878; SURVEY.md Appendix A), decodable
 // by libzstd; the compressed bytes are NOT meant to equal libzstd's.
@@ -60,8 +61,11 @@ struct ZkEncodeArgs {
     uint8_t* lits;                                              // ZKC_BLOCK per block
     uint8_t* stage;                                             // ZKC_SLOT per block
     uint8_t* seqsec;                                            // ZKC_SEQSEC per block
-    uint32_t* frame_csize; unsigned long long* frame_off; uint32_t* frame_hash;
-    uint8_t* dst; size_t dst_cap; unsigned long long* total; uint32_t* error;
+    // K-C3 (the frame assembly).  res: the result area of the batch (ZKC_RES_HDR).  V: variants of every block (zk_encode_csize; 1
+    // elsewhere): block b of the tables is variant v = min(geo[b].k, V - 1), its record at blocks[v * n_blocks + b] and its staged bytes
+    // in slot v * n_blocks + b.  wmin, wmax, whist: the window the frames announce (zkc_carve)
+    uint32_t* res; unsigned long long* frame_off; uint32_t* frame_hash;
+    uint8_t* dst; size_t dst_cap; uint32_t V, wmin, wmax, whist;
     // raw-content prefix (RawEncoder::compress_with_prefix, encode.rs:311-338: re-applied at the start of EVERY frame): the last
     // ptail <= ZKC_BLOCK bytes of it are staged in front of a copy of each frame's first block, so that block's match finder sees
     // one contiguous history and needs no second pointer
@@ -71,6 +75,10 @@ struct ZkEncodeArgs {
     size_t hist_cap;
     uint8_t* hc;                         // scratch of the high-level tier (zk_hc.inc), carved for its largest internal pass
 };
+// The result area of a batch, read back by one copy: [0] frames and [1] blocks K-C3 assembles, written on the device by whatever built
+// the tables (n_frames / n_blocks bound them), [2] error, [4..5] the bytes written (u64); then the frames' compressed sizes and, where
+// the frames were cut on the device, their input sizes
+#define ZKC_RES_HDR 8u
 #define ZKC_PSLOT (2u * ZKC_BLOCK + 64u)   // per-frame staging slot: [prefix tail | first block]
 
 __device__ __forceinline__ ZkcGeo zkc_block_range(const ZkEncodeArgs& a, uint32_t b, size_t& lo, size_t& hi, size_t& fstart) {
@@ -80,8 +88,8 @@ __device__ __forceinline__ ZkcGeo zkc_block_range(const ZkEncodeArgs& a, uint32_
 }
 
 // uniform layout: frames of frame_size bytes, the last one shorter (n_frames = 1 and one empty frame when n == 0).  Every frame but the
-// last is full, so frame f starts at block f * ceil(frame_size / ZKC_BLOCK)
-__global__ void __launch_bounds__(256) zk_geo_uniform_kernel(ZkcFrame* fr, uint32_t n_frames, size_t n, uint32_t frame_size) {
+// last is full, so frame f starts at block f * ceil(frame_size / ZKC_BLOCK).  count: the frames and the blocks they cover
+__global__ void __launch_bounds__(256) zk_geo_uniform_kernel(ZkcFrame* fr, uint32_t* count, uint32_t n_frames, size_t n, uint32_t frame_size) {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= n_frames) return;
     const uint32_t bpf = (uint32_t)(((size_t)frame_size + ZKC_BLOCK - 1) / ZKC_BLOCK);
@@ -90,10 +98,11 @@ __global__ void __launch_bounds__(256) zk_geo_uniform_kernel(ZkcFrame* fr, uint3
     ZkcFrame r;
     r.start = start; r.size = size; r.first_block = f * bpf; r.n_blocks = size ? (size + ZKC_BLOCK - 1) / ZKC_BLOCK : 1u; r.pad = 0;
     fr[f] = r;
+    if (f + 1 == n_frames) { count[0] = n_frames; count[1] = r.first_block + r.n_blocks; }
 }
 
-// caller-chosen sizes: frame starts and first blocks by one scan (one CTA, 1024 frames a round)
-__global__ void __launch_bounds__(1024) zk_geo_sized_kernel(ZkcFrame* fr, const uint32_t* sizes, uint32_t n_frames) {
+// caller-chosen sizes: frame starts and first blocks by one scan (one CTA, 1024 frames a round); count as zk_geo_uniform_kernel
+__global__ void __launch_bounds__(1024) zk_geo_sized_kernel(ZkcFrame* fr, uint32_t* count, const uint32_t* sizes, uint32_t n_frames) {
     __shared__ unsigned long long wb[32], cb;
     __shared__ uint32_t wk[32], ck;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -126,6 +135,7 @@ __global__ void __launch_bounds__(1024) zk_geo_sized_kernel(ZkcFrame* fr, const 
             r.start = cb + (warp ? wb[warp - 1] : 0ull) + xb - d; r.size = d;
             r.first_block = ck + (warp ? wk[warp - 1] : 0u) + xk - nb; r.n_blocks = nb; r.pad = 0;
             fr[f] = r;
+            if (f + 1 == n_frames) { count[0] = n_frames; count[1] = r.first_block + nb; }
         }
         __syncthreads();
         if (threadIdx.x == 0) { cb += wb[31]; ck += wk[31]; }
@@ -133,11 +143,12 @@ __global__ void __launch_bounds__(1024) zk_geo_sized_kernel(ZkcFrame* fr, const 
     }
 }
 
-// one thread per block: its frame is the last one whose first block is <= b (every frame has a block, so first blocks increase)
-__global__ void __launch_bounds__(256) zk_geo_block_kernel(ZkcGeo* geo, const ZkcFrame* fr, uint32_t n_frames, uint32_t n_blocks) {
+// one thread per block of the count[1] the frame table covers: its frame is the last one whose first block is <= b (every frame has a
+// block, so first blocks increase)
+__global__ void __launch_bounds__(256) zk_geo_block_kernel(ZkcGeo* geo, const ZkcFrame* fr, const uint32_t* count) {
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= n_blocks) return;
-    uint32_t lo = 0, hi = n_frames - 1;
+    if (b >= count[1]) return;
+    uint32_t lo = 0, hi = count[0] - 1;
     while (lo < hi) { const uint32_t mid = lo + (hi - lo + 1) / 2; if (fr[mid].first_block <= b) lo = mid; else hi = mid - 1; }
     const ZkcFrame F = fr[lo];
     const uint32_t k = b - F.first_block, off = k * ZKC_BLOCK;
@@ -249,7 +260,7 @@ __global__ void __launch_bounds__(NW * 32) zk_match_kernel(ZkEncodeArgs a) {
 }
 
 // Wide-history tier (level >= ZKC_WIDE_LEVEL): the same body with a history of ZKC_WIDE_HIST blocks of the frame instead of one -- the frame
-// header then announces a 256 KiB window (zk_frame_window_kernel) --, 32-bit positions, and one table of 2^HLOG entries in DYNAMIC shared memory
+// header then announces a 256 KiB window (zk_frame_gather_kernel) --, 32-bit positions, and one table of 2^HLOG entries in DYNAMIC shared memory
 // (128 KiB at HLOG 15: one warp-CTA per SM).  Every block still finds its matches alone and pre-inserts its whole history first, so a block costs
 // several times a level-3 block: a tier for ratio (2.50 on the reference's corpus against 2.40 in a 64 KiB window), not for speed.
 #define ZKC_WIDE_LEVEL 13
@@ -1179,95 +1190,106 @@ __global__ void __launch_bounds__(128) zk_block_finish_kernel(ZkEncodeArgs a) {
 }
 
 // =============================================================================================
-// K-C3: frame layout + gather
+// K-C3: frame layout + gather, over the a.res[0] frames and a.res[1] blocks of the tables
 // =============================================================================================
 // XXH64 (A.8) of each frame's input, one warp per frame (zk_warp_xxh64: coalesced loads, products off the chain)
 __global__ void __launch_bounds__(128) zk_frame_hash_kernel(ZkEncodeArgs a) {
     const int lane = threadIdx.x & 31;
     const uint32_t f = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (f >= a.n_frames) return;
+    if (f >= a.res[0]) return;
     const uint8_t* p = a.src + a.frames[f].start; const uint32_t len = a.frames[f].size;
     const unsigned long long h = zk_warp_xxh64(p, len, lane);
     if (lane == 0) a.frame_hash[f] = (uint32_t)h;
 }
 
-// per-frame sizes and per-block offsets (one thread per frame), then a single-CTA scan for the frame offsets
-__global__ void __launch_bounds__(256) zk_frame_size_kernel(ZkEncodeArgs a) {
-    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
-    if (f >= a.n_frames) return;
-    uint32_t off = ZKC_FRAME_HDR;
-    const uint32_t b0 = a.frames[f].first_block, b1 = b0 + a.frames[f].n_blocks;
-    for (uint32_t b = b0; b < b1; b++) {
-        ZkcBlock& bl = a.blocks[b];
-        bl.out_off = off; off += bl.csize;
-    }
-    if (a.checksum) off += 4;
-    a.frame_csize[f] = off;
+// record and staging slot of block b, block k of its frame: those of its variant min(k, V - 1)
+__device__ __forceinline__ size_t zkc_variant_slot(const ZkEncodeArgs& a, uint32_t b, uint32_t k) {
+    return (size_t)min(k, a.V - 1) * a.n_blocks + b;
 }
 
-__global__ void __launch_bounds__(1024) zk_frame_scan_kernel(ZkEncodeArgs a) {
+// one warp per frame: block offsets inside the frame (warp scan over its blocks), frame size
+__global__ void __launch_bounds__(128) zk_frame_size_kernel(ZkEncodeArgs a) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t f = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (f >= a.res[0]) return;
+    const uint32_t s = a.frames[f].first_block, e = s + a.frames[f].n_blocks;
+    uint32_t run = ZKC_FRAME_HDR;
+    for (uint32_t j = s; j < e; j += 32) {
+        const uint32_t b = j + (uint32_t)lane;
+        ZkcBlock* bl = b < e ? a.blocks + zkc_variant_slot(a, b, b - s) : nullptr;
+        const uint32_t cs = bl ? bl->csize : 0u;
+        uint32_t incl = cs;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += t; }
+        if (bl) bl->out_off = run + incl - cs;
+        run += __shfl_sync(0xFFFFFFFFu, incl, 31);
+    }
+    if (lane == 0) a.res[ZKC_RES_HDR + f] = run + (a.checksum ? 4u : 0u);
+}
+
+// exclusive prefix sum of x(i), i < n, by one CTA of 1024 threads: put(i, x(0) + .. + x(i - 1)); returns the sum of all to every thread
+template <class X, class Put>
+__device__ __forceinline__ unsigned long long zkc_cta_scan(uint32_t n, X x, Put put) {
     __shared__ unsigned long long part[1024];
     __shared__ unsigned long long carry;
     if (threadIdx.x == 0) carry = 0;
     __syncthreads();
-    for (uint32_t base = 0; base < a.n_frames; base += 1024) {
-        const uint32_t f = base + threadIdx.x;
-        unsigned long long v = f < a.n_frames ? a.frame_csize[f] : 0;
+    for (uint32_t base = 0; base < n; base += 1024) {
+        const uint32_t i = base + threadIdx.x;
+        const unsigned long long v = i < n ? x(i) : 0;
         part[threadIdx.x] = v;
         __syncthreads();
         for (uint32_t d = 1; d < 1024; d <<= 1) {
-            unsigned long long t = threadIdx.x >= d ? part[threadIdx.x - d] : 0;
+            const unsigned long long t = threadIdx.x >= d ? part[threadIdx.x - d] : 0;
             __syncthreads();
             part[threadIdx.x] += t;
             __syncthreads();
         }
-        if (f < a.n_frames) a.frame_off[f] = carry + part[threadIdx.x] - v;
+        if (i < n) put(i, carry + part[threadIdx.x] - v);
         __syncthreads();
         if (threadIdx.x == 1023) carry += part[1023];
         __syncthreads();
     }
-    if (threadIdx.x == 0) { *a.total = carry; if (carry > a.dst_cap) *a.error = ZKZ_DST_TOO_SMALL; }
+    return carry;
 }
 
-// tiers above level 12 only: the frame headers written by zk_frame_gather_kernel announce a 128 KiB window.  This rewrites the
-// Window_Descriptor to the smallest one >= max(wmin, min(frame content + prefix tail, wmax)): the wide tier's offsets reach
-// (ZKC_WIDE_HIST + 1) blocks back (wmin = wmax = 256 KiB), the high-level tier's ZKC_HC_WINDOW bytes within the frame and its prefix tail.
-// hist: the bytes of the prefix a frame can reach: its tail, or with long-distance matching all of it (wmax = 2^27 then, the largest
-// window a default libzstd decoder and this one accept; zkc_ldm_window keeps every offset within it)
-__global__ void __launch_bounds__(128) zk_frame_window_kernel(ZkEncodeArgs a, uint32_t n_frames, uint32_t wmin, uint32_t wmax, uint32_t hist) {
-    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
-    if (f >= n_frames || *a.error) return;
-    const size_t fcs = a.frames[f].size;
-    const size_t reach = fcs ? hist : 0;                      // an empty frame holds no match: the minimum, whatever the prefix
-    size_t want = fcs + reach < wmax ? fcs + reach : wmax;
-    if (want < wmin) want = wmin;
-    uint32_t e = 0, m = 0;                                    // Window_Size = 2^(10 + e) * (1 + m / 8)
-    while (((size_t)8 + m) << (7 + e) < want) { if (++m == 8) { m = 0; e++; } }
-    a.dst[a.frame_off[f] + 5] = (uint8_t)((e << 3) | m);
+// frame offsets and the total (one CTA)
+__global__ void __launch_bounds__(1024) zk_frame_scan_kernel(ZkEncodeArgs a) {
+    const unsigned long long total = zkc_cta_scan(a.res[0], [&](uint32_t f) { return (unsigned long long)a.res[ZKC_RES_HDR + f]; },
+                                                  [&](uint32_t f, unsigned long long o) { a.frame_off[f] = o; });
+    if (threadIdx.x == 0) { *(unsigned long long*)(a.res + 4) = total; if (total > a.dst_cap) a.res[2] = ZKZ_DST_TOO_SMALL; }
 }
 
-// gather: one warp per block copies its staged bytes to the final position; block 0 of a frame also writes the
-// frame header, the last block the checksum
+// gather: one warp per block copies its staged bytes to the final position and sets Last_Block (a variant was staged with its own
+// layout's flag); block 0 of a frame also writes the frame header, the last block the checksum
 __global__ void __launch_bounds__(128) zk_frame_gather_kernel(ZkEncodeArgs a) {
     const int lane = threadIdx.x & 31;
     const uint32_t b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (b >= a.n_blocks || *a.error) return;
+    if (b >= a.res[1] || a.res[2]) return;
     const ZkcGeo g = a.geo[b];
     const uint32_t f = g.frame;
-    const ZkcBlock bl = a.blocks[b];
+    const size_t slot = zkc_variant_slot(a, b, g.k);
+    const ZkcBlock bl = a.blocks[slot];
     uint8_t* fo = a.dst + a.frame_off[f];
     if (g.k == 0 && lane == 0) {
         const uint32_t fcs = a.frames[f].size;
+        // the smallest Window_Size = 2^(10 + e) * (1 + m / 8) >= max(wmin, min(fcs + whist, wmax)); an empty frame holds no match, so
+        // it takes the minimum whatever the prefix
+        const size_t reach = fcs ? a.whist : 0;
+        size_t want = fcs + reach < a.wmax ? fcs + reach : a.wmax;
+        if (want < a.wmin) want = a.wmin;
+        uint32_t e = 0, m = 0;
+        while (((size_t)8 + m) << (7 + e) < want) { if (++m == 8) { m = 0; e++; } }
         fo[0] = 0x28; fo[1] = 0xB5; fo[2] = 0x2F; fo[3] = 0xFD;
         fo[4] = (uint8_t)(0x80 | (a.checksum ? 0x04 : 0));       // FCS 4 bytes, no single segment, no dict
-        fo[5] = 0x38;                                             // window 128 KiB (log 17): offsets stay below 64 KiB
+        fo[5] = (uint8_t)((e << 3) | m);
         fo[6] = (uint8_t)fcs; fo[7] = (uint8_t)(fcs >> 8); fo[8] = (uint8_t)(fcs >> 16); fo[9] = (uint8_t)(fcs >> 24);
         if (a.checksum) {
-            const uint32_t h = a.frame_hash[f]; uint8_t* c = fo + a.frame_csize[f] - 4;
+            const uint32_t h = a.frame_hash[f]; uint8_t* c = fo + a.res[ZKC_RES_HDR + f] - 4;
             c[0] = (uint8_t)h; c[1] = (uint8_t)(h >> 8); c[2] = (uint8_t)(h >> 16); c[3] = (uint8_t)(h >> 24);
         }
     }
-    const uint8_t* s = a.stage + (size_t)b * ZKC_SLOT; uint8_t* d = fo + bl.out_off;
+    const uint8_t* s = a.stage + slot * ZKC_SLOT; uint8_t* d = fo + bl.out_off;
     const uint32_t n = bl.csize;
     // staged slots are 16-byte aligned; destinations are arbitrary -> byte-granular head, 16-byte body when co-aligned
     uint32_t head = (uint32_t)((16 - ((uintptr_t)d & 15)) & 15); if (head > n) head = n;
@@ -1282,6 +1304,8 @@ __global__ void __launch_bounds__(128) zk_frame_gather_kernel(ZkEncodeArgs a) {
                               : make_uint4(w0, w1, w2, w3);
     }
     for (uint32_t i = (nvec << 4) + lane; i < n2; i += 32) d2[i] = s2[i];
+    __syncwarp();
+    if (lane == 0) d[0] = (uint8_t)((s[0] & 0xFEu) | g.last);
 }
 
 // =============================================================================================
@@ -1291,51 +1315,31 @@ __global__ void __launch_bounds__(128) zk_frame_gather_kernel(ZkEncodeArgs a) {
 // depth: <= 1 below the wide tier, <= ZKC_WIDE_HIST in it) and on whether it opens its frame (prefix tail, repeat offsets
 // {1,4,8}).  So K-C1/K-C2 run once per depth d = 0 .. V-1 over the whole pass ("variant d"), and block i of a frame that starts
 // at block s is variant min(i - s, V-1) of block i.  Every frame's size is then known for every possible start, and the cut is
-// exact: a frame closes after the first block at which header + blocks >= target, or at 1 GiB of input.
+// exact: a frame closes after the first block at which header + blocks >= target, or at 1 GiB of input.  The cut writes the
+// frame table of the frames it closes; K-C3 assembles them.
 // =============================================================================================
 #define ZKC_CAP_BLOCKS (0x40000000u / ZKC_BLOCK)     // SEEKABLE_MAX_FRAME_SIZE in blocks
 #define ZKC_OPEN 0xFFFFFFFFu                         // next[i]: the frame starting at block i does not close inside this pass
-#define ZKC_RES_HDR 8u                               // u32 words before fcs[] in the result area
 
 struct ZkCsizeArgs {
-    const uint8_t* src; size_t n;                    // the pass
-    uint32_t nb, V, target, checksum;
-    int level;
+    size_t n;                                        // the pass
+    uint32_t nb, V, target;
     uint32_t end_closes;                             // the pass ends the input and the caller is done with it: the rest is the last frame
     uint32_t end_lazy;                               // the pass ends the input but more may follow: a frame that ends there stays open
     const ZkcBlock* vblocks;                         // V x nb: variant d of block i at [d * nb + i]
-    const uint8_t* vstage;                           // V x nb staging slots, same order
     unsigned long long* psum;                        // nb + 1: prefix sum of variant V-1's sizes
     uint32_t* next;                                  // nb: first block after the frame that starts at block i, or ZKC_OPEN
-    uint32_t* boff; uint32_t* bframe;                // nb: offset of the block inside its frame, frame of the block
-    unsigned long long* foff; uint32_t* fhash;       // per frame (nb at most)
-    // [0] frames, [1] blocks consumed, [2] error, [4..5] total bytes (u64); then fcs[nb] (frame sizes), starts[nb + 1] (first blocks)
-    uint32_t* res;
-    uint8_t* dst; size_t dst_cap;
+    uint32_t* starts;                                // nb + 1: first blocks of the frames the walk closes, then the end of the last
+    ZkcFrame* frames;                                // their frame table
+    uint32_t* res;                                   // the result area of the chosen frames (ZKC_RES_HDR)
 };
 
 // prefix sum of variant V-1's block sizes (one CTA)
 __global__ void __launch_bounds__(1024) zk_csize_psum_kernel(ZkCsizeArgs c) {
-    __shared__ unsigned long long part[1024];
-    __shared__ unsigned long long carry;
     const ZkcBlock* bl = c.vblocks + (size_t)(c.V - 1) * c.nb;
-    if (threadIdx.x == 0) { carry = 0; c.psum[0] = 0; }
-    __syncthreads();
-    for (uint32_t base = 0; base < c.nb; base += 1024) {
-        const uint32_t i = base + threadIdx.x;
-        part[threadIdx.x] = i < c.nb ? bl[i].csize : 0;
-        __syncthreads();
-        for (uint32_t d = 1; d < 1024; d <<= 1) {
-            const unsigned long long t = threadIdx.x >= d ? part[threadIdx.x - d] : 0;
-            __syncthreads();
-            part[threadIdx.x] += t;
-            __syncthreads();
-        }
-        if (i < c.nb) c.psum[i + 1] = carry + part[threadIdx.x];
-        __syncthreads();
-        if (threadIdx.x == 1023) carry += part[1023];
-        __syncthreads();
-    }
+    const unsigned long long total = zkc_cta_scan(c.nb, [&](uint32_t i) { return (unsigned long long)bl[i].csize; },
+                                                  [&](uint32_t i, unsigned long long s) { c.psum[i] = s; });
+    if (threadIdx.x == 0) c.psum[c.nb] = total;
 }
 
 // next[i] for every block i: the first V-1 blocks of the frame from their own variants, the rest by binary search in psum
@@ -1369,110 +1373,22 @@ __global__ void __launch_bounds__(1024) zk_csize_walk_kernel(ZkCsizeArgs c) {
     for (uint32_t i = threadIdx.x; i < c.nb; i += blockDim.x) nx[i] = c.next[i];
     __syncthreads();
     if (threadIdx.x == 0) {
-        uint32_t* starts = c.res + ZKC_RES_HDR + c.nb;
         uint32_t f = 0, p = 0;
-        while (p < c.nb && nx[p] != ZKC_OPEN) { starts[f++] = p; p = nx[p]; }
-        starts[f] = p;
+        while (p < c.nb && nx[p] != ZKC_OPEN) { c.starts[f++] = p; p = nx[p]; }
+        c.starts[f] = p;
         c.res[0] = f; c.res[1] = p;
     }
 }
 
-// one warp per frame: block offsets inside the frame (warp scan over the chosen variants), frame size, XXH64 of the frame's input
-__global__ void __launch_bounds__(128) zk_csize_frame_kernel(ZkCsizeArgs c) {
-    const int lane = threadIdx.x & 31;
-    const uint32_t f = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+// the frame table of the frames the walk closed and their input sizes, one thread per frame
+__global__ void __launch_bounds__(256) zk_geo_starts_kernel(ZkCsizeArgs c) {
+    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= c.res[0]) return;
-    const uint32_t* starts = c.res + ZKC_RES_HDR + c.nb;
-    const uint32_t s = starts[f], e = starts[f + 1];
-    uint32_t run = ZKC_FRAME_HDR;
-    for (uint32_t j = s; j < e; j += 32) {
-        const uint32_t i = j + (uint32_t)lane;
-        uint32_t cs = 0;
-        if (i < e) { const uint32_t v = min(i - s, c.V - 1); cs = c.vblocks[(size_t)v * c.nb + i].csize; }
-        uint32_t incl = cs;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += t; }
-        if (i < e) { c.boff[i] = run + incl - cs; c.bframe[i] = f; }
-        run += __shfl_sync(0xFFFFFFFFu, incl, 31);
-    }
-    if (lane == 0) c.res[ZKC_RES_HDR + f] = run + (c.checksum ? 4u : 0u);
-    if (c.checksum) {
-        const size_t lo = (size_t)s * ZKC_BLOCK, hi = (size_t)e * ZKC_BLOCK < c.n ? (size_t)e * ZKC_BLOCK : c.n;
-        const unsigned long long h = zk_warp_xxh64(c.src + lo, (uint32_t)(hi - lo), lane);
-        if (lane == 0) c.fhash[f] = (uint32_t)h;
-    }
-}
-
-// frame offsets (one CTA; the frame count is read on the device)
-__global__ void __launch_bounds__(1024) zk_csize_scan_kernel(ZkCsizeArgs c) {
-    __shared__ unsigned long long part[1024];
-    __shared__ unsigned long long carry;
-    const uint32_t nf = c.res[0];
-    const uint32_t* fcs = c.res + ZKC_RES_HDR;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (uint32_t base = 0; base < nf; base += 1024) {
-        const uint32_t f = base + threadIdx.x;
-        const unsigned long long v = f < nf ? fcs[f] : 0;
-        part[threadIdx.x] = v;
-        __syncthreads();
-        for (uint32_t d = 1; d < 1024; d <<= 1) {
-            const unsigned long long t = threadIdx.x >= d ? part[threadIdx.x - d] : 0;
-            __syncthreads();
-            part[threadIdx.x] += t;
-            __syncthreads();
-        }
-        if (f < nf) c.foff[f] = carry + part[threadIdx.x] - v;
-        __syncthreads();
-        if (threadIdx.x == 1023) carry += part[1023];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) {
-        *(unsigned long long*)(c.res + 4) = carry;
-        if (carry > c.dst_cap) c.res[2] = ZKZ_DST_TOO_SMALL;
-    }
-}
-
-// one warp per consumed block: copy its chosen variant into place and set Last_Block; a frame's first block also writes the frame
-// header (FCS = the frame's input length) and the checksum
-__global__ void __launch_bounds__(128) zk_csize_gather_kernel(ZkCsizeArgs c) {
-    const int lane = threadIdx.x & 31;
-    const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (i >= c.res[1] || c.res[2]) return;
-    const uint32_t f = c.bframe[i];
-    const uint32_t* starts = c.res + ZKC_RES_HDR + c.nb;
-    const uint32_t s = starts[f], e = starts[f + 1], v = min(i - s, c.V - 1);
-    const uint32_t n = c.vblocks[(size_t)v * c.nb + i].csize;
-    const uint8_t* src = c.vstage + ((size_t)v * c.nb + i) * ZKC_SLOT;
-    uint8_t* fo = c.dst + c.foff[f];
-    if (i == s && lane == 0) {
-        const size_t lo = (size_t)s * ZKC_BLOCK, hi = (size_t)e * ZKC_BLOCK < c.n ? (size_t)e * ZKC_BLOCK : c.n;
-        const uint32_t fcs = (uint32_t)(hi - lo);
-        fo[0] = 0x28; fo[1] = 0xB5; fo[2] = 0x2F; fo[3] = 0xFD;
-        fo[4] = (uint8_t)(0x80 | (c.checksum ? 0x04 : 0));
-        fo[5] = c.level >= ZKC_WIDE_LEVEL ? 0x40 : 0x38;           // window 256 KiB in the wide tier, else 128 KiB (as zk_frame_{gather,window}_kernel)
-        fo[6] = (uint8_t)fcs; fo[7] = (uint8_t)(fcs >> 8); fo[8] = (uint8_t)(fcs >> 16); fo[9] = (uint8_t)(fcs >> 24);
-        if (c.checksum) {
-            const uint32_t h = c.fhash[f]; uint8_t* q = fo + c.res[ZKC_RES_HDR + f] - 4;
-            q[0] = (uint8_t)h; q[1] = (uint8_t)(h >> 8); q[2] = (uint8_t)(h >> 16); q[3] = (uint8_t)(h >> 24);
-        }
-    }
-    uint8_t* d = fo + c.boff[i];
-    // staged slots are 16-byte aligned; destinations are arbitrary -> byte-granular head, 16-byte body
-    uint32_t head = (uint32_t)((16 - ((uintptr_t)d & 15)) & 15); if (head > n) head = n;
-    if (lane < (int)head) d[lane] = src[lane];
-    const uint8_t* s2 = src + head; uint8_t* d2 = d + head; const uint32_t n2 = n - head, nvec = n2 >> 4;
-    const uint32_t mis = (uint32_t)((uintptr_t)s2 & 3);
-    const uint32_t* sa = (const uint32_t*)(s2 - mis); const uint32_t sh = mis * 8;
-    for (uint32_t k = lane; k < nvec; k += 32) {
-        const uint32_t* q = sa + 4 * k;
-        const uint32_t w0 = q[0], w1 = q[1], w2 = q[2], w3 = q[3], w4 = mis ? q[4] : 0;
-        ((uint4*)d2)[k] = mis ? make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh), __funnelshift_r(w3, w4, sh))
-                              : make_uint4(w0, w1, w2, w3);
-    }
-    for (uint32_t k = (nvec << 4) + lane; k < n2; k += 32) d2[k] = s2[k];
-    __syncwarp();
-    if (lane == 0) d[0] = (uint8_t)((src[0] & 0xFEu) | (i + 1 == e ? 1u : 0u));    // Last_Block: the variant was staged with its own layout's flag
+    const uint32_t s = c.starts[f], e = c.starts[f + 1];
+    const size_t hi = (size_t)e * ZKC_BLOCK < c.n ? (size_t)e * ZKC_BLOCK : c.n;
+    ZkcFrame r;
+    r.start = (size_t)s * ZKC_BLOCK; r.size = (uint32_t)(hi - r.start); r.first_block = s; r.n_blocks = e - s; r.pad = 0;
+    c.frames[f] = r; c.res[ZKC_RES_HDR + c.nb + f] = r.size;
 }
 
 // =============================================================================================
@@ -1515,16 +1431,16 @@ struct ZkcHcPass;
 struct ZkcHcRun;
 static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, const ZkEncodeArgs& a, const ZkcHcRun* hc);
 
-// the frame and block tables of a batch, on `stream`: the uniform layout is generated on the device, the caller's sizes are uploaded to
-// d_sizes and scanned there
-static int zkc_build_geometry(ZkEncodeWs* ws, cudaStream_t stream, ZkcGeo* geo, ZkcFrame* fr, const ZkFrames& frames, uint32_t n_blocks,
-                              uint32_t* d_sizes) {
+// the frame and block tables of a batch and their counts, on `stream`: the uniform layout is generated on the device, the caller's sizes
+// are uploaded to d_sizes and scanned there
+static int zkc_build_geometry(ZkEncodeWs* ws, cudaStream_t stream, ZkcGeo* geo, ZkcFrame* fr, uint32_t* count, const ZkFrames& frames,
+                              uint32_t n_blocks, uint32_t* d_sizes) {
     const uint32_t n_frames = frames.count;
     if (frames.sizes) {
         ZK_CUDA_OK(cudaMemcpyAsync(d_sizes, frames.sizes, (size_t)n_frames * 4, cudaMemcpyHostToDevice, stream));
-        ZK_LAUNCH(zk_geo_sized_kernel, 1, 1024, 0, stream, fr, (const uint32_t*)d_sizes, n_frames);
-    } else ZK_LAUNCH(zk_geo_uniform_kernel, (n_frames + 255) / 256, 256, 0, stream, fr, n_frames, frames.n, frames.frame_size);
-    ZK_LAUNCH(zk_geo_block_kernel, (n_blocks + 255) / 256, 256, 0, stream, geo, (const ZkcFrame*)fr, n_frames, n_blocks);
+        ZK_LAUNCH(zk_geo_sized_kernel, 1, 1024, 0, stream, fr, count, (const uint32_t*)d_sizes, n_frames);
+    } else ZK_LAUNCH(zk_geo_uniform_kernel, (n_frames + 255) / 256, 256, 0, stream, fr, count, n_frames, frames.n, frames.frame_size);
+    ZK_LAUNCH(zk_geo_block_kernel, (n_blocks + 255) / 256, 256, 0, stream, geo, (const ZkcFrame*)fr, (const uint32_t*)count);
     ws->launches += 2;
     return 0;
 }
@@ -1545,6 +1461,37 @@ static int zkc_side_stream(ZkEncodeWs* ws, cudaStream_t stream, bool side, cudaS
 
 #include "zk_hc.inc"
 #include "zk_cdc.inc"
+
+// The workspace of a batch of n_frames frames over n_blocks blocks, with V variants of every block's record and staged bytes (1 except in
+// zk_encode_csize) and, with a prefix tail of pt bytes, the frames' prefix staging slots: a's scratch pointers into it from `base`
+// (nullptr: only counts its bytes; the caller's own regions follow), and the fields every batch of tier `lvl` sets alike.  far: the tier
+// matches up to 2^27 bytes back (long-distance matching, long mode).  Returns the bytes it takes.
+static size_t zkc_carve(ZkEncodeArgs& a, uint8_t* base, uint32_t n_frames, size_t n_blocks, uint32_t V, int lvl, bool far, uint32_t pt,
+                        const ZkEncodeParams& p) {
+    size_t off = 0;
+    auto at = [&](size_t bytes) { const size_t o = off; off = zkc_align(off + bytes); return (uint8_t*)((uintptr_t)base + o); };
+    a.n_frames = n_frames; a.n_blocks = (uint32_t)n_blocks; a.V = V;
+    a.geo = (const ZkcGeo*)at(n_blocks * sizeof(ZkcGeo)); a.frames = (const ZkcFrame*)at((size_t)n_frames * sizeof(ZkcFrame));
+    a.blocks = (ZkcBlock*)at(V * n_blocks * sizeof(ZkcBlock));
+    a.seq_ll = (uint16_t*)at(n_blocks * ZKC_MAXSEQ * 2); a.seq_ml = (uint16_t*)at(n_blocks * ZKC_MAXSEQ * 2);
+    a.seq_off = (uint32_t*)at(n_blocks * ZKC_MAXSEQ * 4);
+    a.lits = at(n_blocks * ZKC_BLOCK); a.stage = at(V * n_blocks * ZKC_SLOT + 64); a.seqsec = at(n_blocks * ZKC_SEQSEC);
+    a.res = (uint32_t*)at((ZKC_RES_HDR + 2 * (size_t)n_frames) * 4);
+    a.frame_off = (unsigned long long*)at((size_t)n_frames * 8); a.frame_hash = (uint32_t*)at((size_t)n_frames * 4);
+    a.pstage = at(pt ? (size_t)n_frames * ZKC_PSLOT : 0);
+    a.level = lvl; a.checksum = p.checksum ? 1 : 0;
+    a.prefix = p.prefix; a.prefix_len = pt ? p.prefix_len : 0; a.ptail = pt;
+    a.hist_cap = ~(size_t)0; a.hc = nullptr;
+    // the window every frame announces (zk_frame_gather_kernel): 128 KiB below the wide tier, whose offsets stay below 64 KiB; the wide
+    // tier's offsets reach (ZKC_WIDE_HIST + 1) blocks back, the high-level tier's ZKC_HC_WINDOW bytes within the frame and its prefix tail.
+    // Up to 2^27 bytes back, the largest window a default libzstd decoder and this one accept (zkc_ldm_window keeps every offset within
+    // it), all of the prefix is in reach
+    a.wmin = a.wmax = 128u << 10; a.whist = pt;
+    if (far) { a.wmax = 1u << 27; a.whist = a.prefix_len; }
+    else if (lvl >= ZKC_HC_LEVEL) a.wmax = ZKC_HC_WINDOW;
+    else if (lvl >= ZKC_WIDE_LEVEL) a.wmin = a.wmax = 256u << 10;
+    return off;
+}
 
 int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, const ZkFrames& fr, const ZkEncodeParams& p, uint8_t* d_dst,
                       size_t dst_cap) {
@@ -1572,52 +1519,28 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     const uint32_t hc_span = lvl >= ZKC_HC_LEVEL ? zkc_hc_plan(fr, (uint32_t)n_blocks, pt, hc.plan) : 0u;
     if (ldm) hc.reach = p.prefix_len < ZKC_LDM_REACH ? p.prefix_len : ZKC_LDM_REACH;
     hc.input = lin;
-    // carve the workspace
-    size_t off = 0;
-    const size_t o_geo = off; off = zkc_align(off + n_blocks * sizeof(ZkcGeo));
-    const size_t o_fr = off; off = zkc_align(off + (size_t)n_frames * sizeof(ZkcFrame));
+    ZkEncodeArgs a;
+    size_t off = zkc_carve(a, nullptr, n_frames, n_blocks, 1, lvl, ldm || p.long_mode, pt, p);
     const size_t o_fsz = off; if (fr.sizes) off = zkc_align(off + (size_t)n_frames * 4);
-    const size_t o_blocks = off; off = zkc_align(off + n_blocks * sizeof(ZkcBlock));
-    const size_t o_ll = off; off = zkc_align(off + n_blocks * ZKC_MAXSEQ * 2);
-    const size_t o_ml = off; off = zkc_align(off + n_blocks * ZKC_MAXSEQ * 2);
-    const size_t o_off = off; off = zkc_align(off + n_blocks * ZKC_MAXSEQ * 4);
-    const size_t o_lits = off; off = zkc_align(off + n_blocks * ZKC_BLOCK);
-    const size_t o_stage = off; off = zkc_align(off + n_blocks * ZKC_SLOT + 64);
-    const size_t o_seqsec = off; off = zkc_align(off + n_blocks * ZKC_SEQSEC);
-    const size_t o_fcs = off; off = zkc_align(off + (size_t)n_frames * 4);
-    const size_t o_foff = off; off = zkc_align(off + (size_t)n_frames * 8);
-    const size_t o_fh = off; off = zkc_align(off + (size_t)n_frames * 4);
-    const size_t o_tot = off; off = zkc_align(off + 16);
-    const size_t o_pst = off; if (pt) off = zkc_align(off + (size_t)n_frames * ZKC_PSLOT);
     const size_t o_hc = off;
     if (lvl >= ZKC_HC_LEVEL) off = zkc_align(off + zkc_hc_layout(hc_span, nullptr, nullptr));
     const size_t o_ldm = off;
     if (ldm || lin) off = zkc_align(off + zkc_ldm_layout(hc.reach, lin ? (uint32_t)n_blocks * ZKC_LDM_BSLOTS : 0u, n_blocks, nullptr, nullptr, nullptr, nullptr));
     int rc = zk_grow(&ws->buf, &ws->cap, off, 1);
-    if (!rc) rc = zk_grow((void**)&ws->h_sizes, &ws->cap_frames, (size_t)n_frames + 4, 4, true);     // the sizes, then the total and the error
+    if (!rc) rc = zk_grow((void**)&ws->h_sizes, &ws->cap_frames, ZKC_RES_HDR + (size_t)n_frames, 4, true);
     if (rc) return rc;
     uint8_t* base = (uint8_t*)ws->buf;
-    ZkEncodeArgs a;
-    a.src = d_src; a.n = n; a.n_frames = n_frames; a.n_blocks = (uint32_t)n_blocks;
-    a.geo = (const ZkcGeo*)(base + o_geo); a.frames = (const ZkcFrame*)(base + o_fr);
-    a.level = lvl; a.checksum = p.checksum ? 1 : 0;
-    a.blocks = (ZkcBlock*)(base + o_blocks);
-    a.seq_ll = (uint16_t*)(base + o_ll); a.seq_ml = (uint16_t*)(base + o_ml); a.seq_off = (uint32_t*)(base + o_off);
-    a.lits = base + o_lits; a.stage = base + o_stage; a.seqsec = base + o_seqsec;
-    a.frame_csize = (uint32_t*)(base + o_fcs); a.frame_off = (unsigned long long*)(base + o_foff); a.frame_hash = (uint32_t*)(base + o_fh);
-    a.dst = d_dst; a.dst_cap = dst_cap; a.total = (unsigned long long*)(base + o_tot); a.error = (uint32_t*)(base + o_tot + 8);
-    a.prefix = p.prefix; a.prefix_len = 0; a.ptail = 0; a.pstage = base + o_pst;
-    a.hist_cap = ~(size_t)0;
+    zkc_carve(a, base, n_frames, n_blocks, 1, lvl, ldm || p.long_mode, pt, p);
+    a.src = d_src; a.n = n; a.dst = d_dst; a.dst_cap = dst_cap;
     a.hc = base + o_hc;
     if (ldm || lin) hc.ldm = base + o_ldm;
-    rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo), (ZkcFrame*)(base + o_fr), fr, (uint32_t)n_blocks, (uint32_t*)(base + o_fsz));
+    ZK_CUDA_OK(cudaMemsetAsync(a.res, 0, ZKC_RES_HDR * 4, stream));
+    rc = zkc_build_geometry(ws, stream, (ZkcGeo*)a.geo, (ZkcFrame*)a.frames, a.res, fr, (uint32_t)n_blocks, (uint32_t*)(base + o_fsz));
     if (rc) return rc;
     if (pt) {
-        a.prefix_len = p.prefix_len; a.ptail = pt;
         ZK_LAUNCH(zk_prefix_stage_kernel, n_frames, 256, 0, stream, a);
         ws->launches += 1;
     }
-    ZK_CUDA_OK(cudaMemsetAsync(base + o_tot, 0, 16, stream));
     // the content checksum only needs the input: it runs beside the match finder on the side stream (one warp per frame, bound
     // by the latency of its four serial chains, so it leaves the machine to K-C1)
     cudaStream_t ss;
@@ -1630,15 +1553,11 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     if (rc) return rc;
     ws->prof.begin(7, stream);
     if (p.checksum && ss == stream) ZK_LAUNCH(zk_frame_hash_kernel, (n_frames + 3) / 4, 128, 0, stream, a);   // else: already done on the side stream (joined by ev_b)
-    ZK_LAUNCH(zk_frame_size_kernel, (n_frames + 255) / 256, 256, 0, stream, a);
+    ZK_LAUNCH(zk_frame_size_kernel, (n_frames + 3) / 4, 128, 0, stream, a);
     ZK_LAUNCH(zk_frame_scan_kernel, 1, 1024, 0, stream, a);
     ZK_LAUNCH(zk_frame_gather_kernel, (uint32_t)((n_blocks + 3) / 4), 128, 0, stream, a);
-    if (ldm || p.long_mode) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 128u << 10, 1u << 27, ldm ? p.prefix_len : 0u); ws->launches++; }
-    else if (a.level >= ZKC_HC_LEVEL) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 128u << 10, ZKC_HC_WINDOW, pt); ws->launches++; }
-    else if (a.level >= ZKC_WIDE_LEVEL) { ZK_LAUNCH(zk_frame_window_kernel, (n_frames + 127) / 128, 128, 0, stream, a, n_frames, 256u << 10, 256u << 10, pt); ws->launches++; }
     ws->prof.end(7, stream);
-    ZK_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, a.frame_csize, (size_t)n_frames * 4, cudaMemcpyDeviceToHost, stream));
-    ZK_CUDA_OK(cudaMemcpyAsync(ws->h_sizes + n_frames, a.total, 16, cudaMemcpyDeviceToHost, stream));
+    ZK_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, a.res, (ZKC_RES_HDR + (size_t)n_frames) * 4, cudaMemcpyDeviceToHost, stream));
     ws->launches += 7 + (p.checksum ? 1 : 0);
     ws->pending_frames = n_frames;
     return 0;
@@ -1689,17 +1608,16 @@ int zk_encode_collect(ZkEncodeWs* ws, cudaStream_t stream, uint32_t* c_sizes, si
     if (const int rc = zk_sync_check(stream)) return rc;
     ws->pending_frames = 0;
     ws->prof.harvest();
-    unsigned long long total; uint32_t err;
-    memcpy(&total, ws->h_sizes + nf, 8);
-    memcpy(&err, (uint8_t*)(ws->h_sizes + nf) + 8, 4);
-    if (err) return -(int)err;
-    if (c_sizes) memcpy(c_sizes, ws->h_sizes, (size_t)nf * 4);
+    const uint32_t* h = ws->h_sizes;
+    if (h[2]) return -(int)h[2];
+    unsigned long long total; memcpy(&total, h + 4, 8);
+    if (c_sizes) memcpy(c_sizes, h + ZKC_RES_HDR, (size_t)nf * 4);
     if (dst_len) *dst_len = (size_t)total;
     return 0;
 }
 
 // FrameSizePolicy::Compressed(target) over one pass of n <= 1 GiB bytes: V variant passes of K-C1/K-C2 (shared sequence, literal
-// and section scratch; a ZkcBlock[] and a staging area each), the cut (K-C3c), then the assembly of the frames it chose.
+// and section scratch; a ZkcBlock[] and a staging area each), the cut (K-C3c), then K-C3 over the frames it chose.
 // One D2H copy of the counts and sizes, then one synchronisation.
 int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t target, const ZkEncodeParams& p, int final_,
                     int at_end, uint8_t* d_dst, size_t dst_cap, ZkCsizeOut* out) {
@@ -1711,69 +1629,51 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     const int lvl = zkc_level(p.level) >= ZKC_HC_LEVEL ? ZKC_WIDE_LEVEL : zkc_level(p.level);
     const uint32_t nb = (uint32_t)((n + ZKC_BLOCK - 1) / ZKC_BLOCK);
     const uint32_t V = lvl >= ZKC_WIDE_LEVEL ? ZKC_WIDE_HIST + 1 : 2;
-    const uint8_t* d_prefix = p.prefix; const uint32_t prefix_len = p.prefix_len;
-    const bool pfx = d_prefix && prefix_len;
-    const size_t res_words = ZKC_RES_HDR + 2 * (size_t)nb + 1;
-    size_t off = 0;
-    const size_t o_blocks = off; off = zkc_align(off + (size_t)V * nb * sizeof(ZkcBlock));
-    const size_t o_ll = off; off = zkc_align(off + (size_t)nb * ZKC_MAXSEQ * 2);
-    const size_t o_ml = off; off = zkc_align(off + (size_t)nb * ZKC_MAXSEQ * 2);
-    const size_t o_off = off; off = zkc_align(off + (size_t)nb * ZKC_MAXSEQ * 4);
-    const size_t o_lits = off; off = zkc_align(off + (size_t)nb * ZKC_BLOCK);
-    const size_t o_stage = off; off = zkc_align(off + (size_t)V * nb * ZKC_SLOT + 64);
-    const size_t o_seqsec = off; off = zkc_align(off + (size_t)nb * ZKC_SEQSEC);
+    const uint32_t pt = p.prefix && p.prefix_len ? (p.prefix_len < ZKC_BLOCK ? p.prefix_len : ZKC_BLOCK) : 0u;
+    // the batch of the chosen frames (nb at most; the cut writes their tables and result area), the cut's arrays, and the two layouts
+    // of the variants with their counts: frames of one block (d = 0), one frame over the pass (d >= 1)
+    ZkEncodeArgs a;
+    size_t off = zkc_carve(a, nullptr, nb, nb, V, lvl, false, pt, p);
     const size_t o_psum = off; off = zkc_align(off + ((size_t)nb + 1) * 8);
     const size_t o_next = off; off = zkc_align(off + (size_t)nb * 4);
-    const size_t o_boff = off; off = zkc_align(off + (size_t)nb * 4);
-    const size_t o_bfr = off; off = zkc_align(off + (size_t)nb * 4);
-    const size_t o_foff = off; off = zkc_align(off + (size_t)nb * 8);
-    const size_t o_fh = off; off = zkc_align(off + (size_t)nb * 4);
-    const size_t o_res = off; off = zkc_align(off + res_words * 4);
-    const size_t o_pst = off; if (pfx) off = zkc_align(off + (size_t)nb * ZKC_PSLOT);
-    // the two layouts of the variants: frames of one block (d = 0), one frame over the pass (d >= 1)
+    const size_t o_starts = off; off = zkc_align(off + ((size_t)nb + 1) * 4);
     const size_t o_geo0 = off; off = zkc_align(off + (size_t)nb * sizeof(ZkcGeo));
     const size_t o_fr0 = off; off = zkc_align(off + (size_t)nb * sizeof(ZkcFrame));
     const size_t o_geo1 = off; off = zkc_align(off + (size_t)nb * sizeof(ZkcGeo));
     const size_t o_fr1 = off; off = zkc_align(off + sizeof(ZkcFrame));
+    const size_t o_cnt = off; off = zkc_align(off + 16);
     int rc = zk_grow(&ws->buf, &ws->cap, off, 1);
-    if (!rc) rc = zk_grow((void**)&ws->h_sizes, &ws->cap_frames, res_words, 4, true);
+    if (!rc) rc = zk_grow((void**)&ws->h_sizes, &ws->cap_frames, ZKC_RES_HDR + 2 * (size_t)nb, 4, true);
     if (rc) return rc;
     uint8_t* base = (uint8_t*)ws->buf;
+    zkc_carve(a, base, nb, nb, V, lvl, false, pt, p);
+    a.src = d_src; a.n = n; a.dst = d_dst; a.dst_cap = dst_cap;
     ZkCsizeArgs c;
-    c.src = d_src; c.n = n; c.nb = nb; c.V = V; c.target = target ? target : 1; c.level = lvl; c.checksum = p.checksum ? 1 : 0;
+    c.n = n; c.nb = nb; c.V = V; c.target = target ? target : 1;
     c.end_closes = at_end && final_; c.end_lazy = at_end && !final_;
-    c.vblocks = (const ZkcBlock*)(base + o_blocks); c.vstage = base + o_stage;
-    c.psum = (unsigned long long*)(base + o_psum); c.next = (uint32_t*)(base + o_next);
-    c.boff = (uint32_t*)(base + o_boff); c.bframe = (uint32_t*)(base + o_bfr);
-    c.foff = (unsigned long long*)(base + o_foff); c.fhash = (uint32_t*)(base + o_fh);
-    c.res = (uint32_t*)(base + o_res); c.dst = d_dst; c.dst_cap = dst_cap;
-    ZK_CUDA_OK(cudaMemsetAsync(c.res, 0, ZKC_RES_HDR * 4, stream));
+    c.vblocks = a.blocks; c.psum = (unsigned long long*)(base + o_psum); c.next = (uint32_t*)(base + o_next);
+    c.starts = (uint32_t*)(base + o_starts); c.frames = (ZkcFrame*)a.frames; c.res = a.res;
+    ZK_CUDA_OK(cudaMemsetAsync(a.res, 0, ZKC_RES_HDR * 4, stream));
     cudaStream_t ss;
     if ((rc = zkc_side_stream(ws, stream, p.side, &ss))) return rc;
-    rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo0), (ZkcFrame*)(base + o_fr0), {nullptr, n, ZKC_BLOCK, nb}, nb, nullptr);
-    if (!rc) rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo1), (ZkcFrame*)(base + o_fr1), {nullptr, n, (uint32_t)n, 1}, nb, nullptr);
+    uint32_t* vcount = (uint32_t*)(base + o_cnt);
+    rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo0), (ZkcFrame*)(base + o_fr0), vcount, {nullptr, n, ZKC_BLOCK, nb}, nb, nullptr);
+    if (!rc) rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo1), (ZkcFrame*)(base + o_fr1), vcount + 2, {nullptr, n, (uint32_t)n, 1}, nb, nullptr);
     if (rc) return rc;
     // variant passes.  d = 0: frames of one block, so every block opens its frame (prefix staging included); d >= 1: one frame
     // over the pass, with the wide tier's history capped at d blocks below V - 1
     for (uint32_t d = 0; d < V; d++) {
-        ZkEncodeArgs a;
-        a.src = d_src; a.n = n; a.n_blocks = nb; a.n_frames = d == 0 ? nb : 1;
-        a.geo = (const ZkcGeo*)(base + (d == 0 ? o_geo0 : o_geo1)); a.frames = (const ZkcFrame*)(base + (d == 0 ? o_fr0 : o_fr1));
-        a.level = lvl; a.checksum = c.checksum;
-        a.blocks = (ZkcBlock*)(base + o_blocks) + (size_t)d * nb;
-        a.seq_ll = (uint16_t*)(base + o_ll); a.seq_ml = (uint16_t*)(base + o_ml); a.seq_off = (uint32_t*)(base + o_off);
-        a.lits = base + o_lits; a.stage = base + o_stage + (size_t)d * nb * ZKC_SLOT; a.seqsec = base + o_seqsec;
-        a.frame_csize = nullptr; a.frame_off = nullptr; a.frame_hash = nullptr;
-        a.dst = d_dst; a.dst_cap = dst_cap; a.total = nullptr; a.error = nullptr;
-        a.prefix = d_prefix; a.prefix_len = 0; a.ptail = 0; a.pstage = base + o_pst;
-        a.hist_cap = d >= 1 && d + 1 < V ? (size_t)d * ZKC_BLOCK : ~(size_t)0;
-        a.hc = nullptr;
-        if (d == 0 && pfx) {
-            a.prefix_len = prefix_len; a.ptail = prefix_len < ZKC_BLOCK ? prefix_len : ZKC_BLOCK;
-            ZK_LAUNCH(zk_prefix_stage_kernel, nb, 256, 0, stream, a);
+        ZkEncodeArgs v = a;
+        v.geo = (const ZkcGeo*)(base + (d == 0 ? o_geo0 : o_geo1)); v.frames = (const ZkcFrame*)(base + (d == 0 ? o_fr0 : o_fr1));
+        v.n_frames = d == 0 ? nb : 1;
+        v.hist_cap = d >= 1 && d + 1 < V ? (size_t)d * ZKC_BLOCK : ~(size_t)0;
+        v.blocks = a.blocks + (size_t)d * nb; v.stage = a.stage + (size_t)d * nb * ZKC_SLOT;
+        if (d >= 1) v.prefix_len = v.ptail = 0;
+        else if (pt) {
+            ZK_LAUNCH(zk_prefix_stage_kernel, nb, 256, 0, stream, v);
             ws->launches += 1;
         }
-        rc = zkc_run_blocks(ws, stream, ss, a, nullptr);
+        rc = zkc_run_blocks(ws, stream, ss, v, nullptr);
         if (rc) return rc;
         ws->launches += 4;
     }
@@ -1786,12 +1686,15 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     ZK_LAUNCH(zk_csize_psum_kernel, 1, 1024, 0, stream, c);
     ZK_LAUNCH(zk_csize_next_kernel, (nb + 255) / 256, 256, 0, stream, c);
     ZK_LAUNCH(zk_csize_walk_kernel, 1, 1024, walk_smem, stream, c);
-    ZK_LAUNCH(zk_csize_frame_kernel, (nb + 3) / 4, 128, 0, stream, c);
-    ZK_LAUNCH(zk_csize_scan_kernel, 1, 1024, 0, stream, c);
-    ZK_LAUNCH(zk_csize_gather_kernel, (nb + 3) / 4, 128, 0, stream, c);
+    ZK_LAUNCH(zk_geo_starts_kernel, (nb + 255) / 256, 256, 0, stream, c);
+    ZK_LAUNCH(zk_geo_block_kernel, (nb + 255) / 256, 256, 0, stream, (ZkcGeo*)a.geo, a.frames, (const uint32_t*)a.res);
+    if (p.checksum) ZK_LAUNCH(zk_frame_hash_kernel, (nb + 3) / 4, 128, 0, stream, a);
+    ZK_LAUNCH(zk_frame_size_kernel, (nb + 3) / 4, 128, 0, stream, a);
+    ZK_LAUNCH(zk_frame_scan_kernel, 1, 1024, 0, stream, a);
+    ZK_LAUNCH(zk_frame_gather_kernel, (nb + 3) / 4, 128, 0, stream, a);
     ws->prof.end(7, stream);
-    ws->launches += 6;
-    ZK_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, c.res, res_words * 4, cudaMemcpyDeviceToHost, stream));
+    ws->launches += 8 + (p.checksum ? 1 : 0);
+    ZK_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, a.res, (ZKC_RES_HDR + 2 * (size_t)nb) * 4, cudaMemcpyDeviceToHost, stream));
     if ((rc = zk_sync_check(stream))) return rc;
     ws->prof.harvest();
     const uint32_t* h = ws->h_sizes;
@@ -1801,7 +1704,7 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     unsigned long long total; memcpy(&total, h + 4, 8);
     out->total = (size_t)total;
     out->c_sizes = h + ZKC_RES_HDR;
-    out->starts = h + ZKC_RES_HDR + nb;
+    out->d_sizes = h + ZKC_RES_HDR + nb;
     return 0;
 }
 

@@ -69,7 +69,7 @@ struct ZkCsizeOut {
     uint32_t n_frames = 0;
     size_t consumed = 0, total = 0;      // input bytes the frames cover; bytes written
     const uint32_t* c_sizes = nullptr;   // n_frames compressed sizes
-    const uint32_t* starts = nullptr;    // n_frames + 1 first blocks (32 KiB units from d_src); the last one is the end of the last frame
+    const uint32_t* d_sizes = nullptr;   // n_frames input sizes
 };
 int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t target, const ZkEncodeParams& p, int final_,
                     int at_end, uint8_t* d_dst, size_t dst_cap, ZkCsizeOut* out);
