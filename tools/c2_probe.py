@@ -1,6 +1,6 @@
-"""Per-kernel device time of compression on the H100: K-C1 `zk_match_kernel`, K-C2s `zk_seq_enc_kernel`, K-C2l `zk_lit_enc_kernel` and
-K-C2f `zk_block_finish_kernel`, per GiB, for device-resident compression (zk_compress_frames_dev) of the bench's 1 GiB mix in 2 MiB frames
-at levels 1, 3 and -1 (the level -1 literal kernel does no Huffman work, so its K-C2s time is the sequence side alone).  K-C2s and K-C2l
+"""Per-kernel device time of compression on the H100: K-C1 `zk_match_kernel` (`zk_match_wide_kernel` from level 13,
+`zk_match_fast_kernel` below 0), K-C2s `zk_seq_enc_kernel`, K-C2l `zk_lit_enc_kernel` and K-C2f `zk_block_finish_kernel`, per GiB, for
+device-resident compression (zk_compress_frames_dev) of the bench's 1 GiB mix in 2 MiB frames at levels 1, 3 and -1 (the level -1 literal kernel does no Huffman work, so its K-C2s time is the sequence side alone).  K-C2s and K-C2l
 run side by side on two streams; the longer of the two ends the K-C2 profile slot.  Every step starts with an L2 flush, as in bench.py.
 Kernel durations come from torch.profiler with CUDA activities, in a run of its own; the card's name, power limit and SM clock are read
 (read-only nvidia-smi queries) in the same call.  --lib compares another build of the library on the same card.  Prints one JSON object.
@@ -24,7 +24,7 @@ import zeekstd_b200 as zk  # noqa: E402
 from zeekstd_b200 import _native as N  # noqa: E402
 
 GIB = 1 << 30
-KERNELS = ["zk_match_kernel", "zk_match_fast_kernel", "zk_seq_enc_kernel", "zk_lit_enc_kernel", "zk_block_finish_kernel"]
+KERNELS = ["zk_match_kernel", "zk_match_wide_kernel", "zk_match_fast_kernel", "zk_seq_enc_kernel", "zk_lit_enc_kernel", "zk_block_finish_kernel"]
 
 
 def card() -> dict:

@@ -202,7 +202,8 @@ __device__ __forceinline__ void zkc_extend_fwd(const uint8_t* sb, uint32_t mpos,
 }
 
 // Offset_Value of a sequence (A.5) for the fast tier, updating the repeat-offset history r0..r2 as the decoder will: the rule of
-// zk_match_body.inc, which keeps its own inline copy (as a call it costs the level-1 kernel two registers)
+// zkc_match_block, which keeps its own inline copy.  As a call there it compiles to different code, and the level-1 kernel took 10.84-10.94
+// ms per GiB of the bench mix instead of 10.68-10.77 (H100 80GB HBM3, 700 W)
 __device__ __forceinline__ uint32_t zkc_offset_value(uint32_t off, uint32_t ll, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& known) {
     uint32_t ov = off + 3;
     if (off != r0 && off != r1 && off != r2 && off + 1 != r0) {           // the common case: an explicit offset
@@ -242,24 +243,190 @@ __global__ void __launch_bounds__(256) zk_prefix_stage_kernel(ZkEncodeArgs a) {
     for (uint32_t i = threadIdx.x; i < 64; i += blockDim.x) d[a.ptail + len + i] = 0;
 }
 
-// DFAST (level >= 4): a second table indexed by a hash of EIGHT bytes is probed first -- its candidates are long matches by
-// construction, the 5-byte table catches the rest (the idea of zstd's double-fast strategy); two tables of 2^HLOG entries per warp.
+// inserts the history sb[0, lo32) into the table, and into the 8-byte table when DFAST, so that matches can reach into it.  Several
+// lanes may hash to the same slot: the highest position wins, as sequential insertion would leave it (keeps the compressed bytes
+// deterministic)
+template <int HLOG, bool DFAST, typename PosT>
+__device__ __forceinline__ void zkc_insert_history(const uint8_t* sb, uint32_t lo32, int lane, PosT* table, PosT* tableL = nullptr) {
+    for (uint32_t p0 = 0; p0 < lo32; p0 += 32) {
+        const uint32_t p = p0 + lane;
+        const unsigned long long v8 = p < lo32 ? zkc_ld8(sb + p) : 0ull;
+        const uint32_t hh = p < lo32 ? zkc_hash5<HLOG>(v8) : (0xFFFF0000u | (uint32_t)lane);
+        const uint32_t same = __match_any_sync(0xFFFFFFFFu, hh);
+        if (p < lo32 && lane == 31 - __clz((int)same)) table[hh] = (PosT)p;
+        if (DFAST) {
+            const uint32_t hl = p < lo32 ? zkc_hash8<HLOG>(v8) : (0xFFFF0000u | (uint32_t)lane);
+            const uint32_t sameL = __match_any_sync(0xFFFFFFFFu, hl);
+            if (p < lo32 && lane == 31 - __clz((int)sameL)) tableL[hl] = (PosT)p;
+        }
+    }
+    __syncwarp();
+}
+
+// The match finder of levels 1-15, run by one warp on block b.  table: the warp's 2^HLOG-entry hash table; an entry is a position, an
+// offset from the start of the history, so u16 entries need history + block < 64 KiB.  HIST_BYTES: how far before the block the history
+// reaches.  DFAST (level >= 4): tableL, a second table of 2^HLOG entries indexed by a hash of EIGHT bytes, is probed first -- its candidates
+// are long matches by construction, the 5-byte table catches the rest (the idea of zstd's double-fast strategy); tableL is not touched
+// otherwise.
+template <int HLOG, bool DFAST, typename PosT, uint32_t HIST_BYTES>
+__device__ __forceinline__ void zkc_match_block(const ZkEncodeArgs& a, uint32_t b, int lane, PosT* table, PosT* tableL) {
+    size_t lo, hi, fstart;
+    const ZkcGeo g = zkc_block_range(a, b, lo, hi, fstart);
+    // history: up to HIST_BYTES of the same frame before `lo` are searchable, capped by a.hist_cap; the first block of a frame
+    // searches the tail of the prefix instead, through its staged copy
+    const bool pfx = a.ptail != 0 && lo == fstart;
+    const size_t hist = a.hist_cap < HIST_BYTES ? a.hist_cap : HIST_BYTES;
+    const size_t base = lo - fstart >= hist ? lo - hist : fstart;
+    const uint8_t* sb = pfx ? a.pstage + (size_t)g.frame * ZKC_PSLOT : a.src + base;
+    const uint32_t lo32 = pfx ? a.ptail : (uint32_t)(lo - base), hi32 = lo32 + (uint32_t)(hi - lo);
+    for (int i = lane; i < ((DFAST ? 2 : 1) << HLOG); i += 32) table[i] = 0;
+    __syncwarp();
+    const uint32_t len = hi32 - lo32;
+    uint16_t* o_ll = a.seq_ll + (size_t)b * ZKC_MAXSEQ; uint16_t* o_ml = a.seq_ml + (size_t)b * ZKC_MAXSEQ;
+    uint32_t* o_off = a.seq_off + (size_t)b * ZKC_MAXSEQ;
+    uint8_t* o_lit = a.lits + (size_t)b * ZKC_BLOCK;
+    uint32_t nseq = 0, nlit = 0;
+    uint32_t ip = lo32;                                     // every literal byte below ip has been written to o_lit
+    if (len >= 16) {
+        const uint32_t mflimit = hi32 - 8;                  // last position where 8 bytes can be read
+        const uint32_t lt_mask = (1u << lane) - 1u;
+        const bool lazy = a.level >= 2;
+        // pre-insert the history so matches can reach into the previous block (or the prefix)
+        if (a.level >= 2 || pfx) zkc_insert_history<HLOG, DFAST>(sb, lo32, lane, table, tableL);
+        uint32_t anchor = lo32;
+        uint32_t rep = 0;                                   // last emitted offset (0 = none)
+        // repeat-offset history (A.5) as the decoder will hold it: blocks are coded independently, so repeat codes are used
+        // only once three explicit offsets have been coded in this block (the history is then certain); the first block of a
+        // frame starts from the known {1,4,8}.  o_off receives Offset_Values (1..3 = repeat codes, offset + 3 otherwise).
+        uint32_t r0 = 1, r1 = 4, r2 = 8, known = lo == fstart ? 3u : 0u;
+        uint32_t misses = 0;                                // consecutive windows without a match: widen the stride (incompressible data)
+        uint32_t s_ll = 0, s_ml = 0, s_off = 0, flushed = 0; // staged sequences: slot nseq - flushed lives in that lane
+        for (;;) {
+            const uint32_t stride = 1u + min(misses >> 3, 3u);
+            if (ip + 32u * stride > mflimit) {
+                if (stride == 1) break;
+                misses = 0; continue;                       // the tail may still fit a stride-1 window
+            }
+            const uint32_t wb = ip;
+            const uint32_t p = wb + (uint32_t)lane * stride;
+            if (lane < 2) zk_prefetch_l1(sb + min(wb + 256u + 128u * (uint32_t)lane, hi32 - 1u));
+            const unsigned long long cur = zkc_ld8(sb + p);
+            const uint32_t h = zkc_hash5<HLOG>(cur);
+            const uint32_t cand = table[h];
+            uint32_t hl = 0, candL = 0;
+            if (DFAST) { hl = zkc_hash8<HLOG>(cur); candL = tableL[hl]; }
+            __syncwarp();
+            // several lanes may hash to the same slot: the highest position wins, as sequential insertion would leave it
+            // (keeps the compressed bytes deterministic)
+            const uint32_t same = __match_any_sync(0xFFFFFFFFu, h);
+            if (lane == 31 - __clz((int)same)) table[h] = (PosT)p;
+            if (DFAST) { const uint32_t sameL = __match_any_sync(0xFFFFFFFFu, hl); if (lane == 31 - __clz((int)sameL)) tableL[hl] = (PosT)p; }
+            // candidate from the hash table(s), and the repeat-offset candidate
+            uint32_t moff = 0, mlen0 = 0;
+            if (cand < p) {
+                const unsigned long long x = zkc_ld8(sb + cand) ^ cur;
+                const uint32_t m = x ? (uint32_t)(__ffsll((long long)x) - 1) >> 3 : 8;
+                if (m >= ZKC_MINMATCH) { moff = p - cand; mlen0 = m; }
+            }
+            if (DFAST && candL < p && candL != cand) {
+                const unsigned long long x = zkc_ld8(sb + candL) ^ cur;
+                const uint32_t m = x ? (uint32_t)(__ffsll((long long)x) - 1) >> 3 : 8;
+                if (m >= ZKC_MINMATCH && m > mlen0) { moff = p - candL; mlen0 = m; }       // both 8 long: the nearer one (5-byte table) is kept
+            }
+            if (rep && p >= rep) {
+                const unsigned long long x = zkc_ld8(sb + p - rep) ^ cur;
+                const uint32_t m = x ? (uint32_t)(__ffsll((long long)x) - 1) >> 3 : 8;
+                if (m >= 4 && m + 1 >= mlen0) { moff = rep; mlen0 = m; }
+            }
+            const uint32_t found = __ballot_sync(0xFFFFFFFFu, mlen0 != 0);
+            if (stride > 1) {
+                if (found) { misses = 0; continue; }        // compressible again: redo this window at stride 1
+                // the whole window is literals, straight from the registers
+                uint8_t* o = o_lit + nlit + (uint32_t)lane * stride;
+                o[0] = (uint8_t)cur; o[1] = (uint8_t)(cur >> 8);
+                if (stride > 2) o[2] = (uint8_t)(cur >> 16);
+                if (stride > 3) o[3] = (uint8_t)(cur >> 24);
+                nlit += 32u * stride; ip = wb + 32u * stride; misses++;
+                continue;
+            }
+            if (!found) {
+                o_lit[nlit + lane] = (uint8_t)cur;
+                nlit += 32u; ip = wb + 32u; misses++;
+                continue;
+            }
+            misses = 0;
+            // take every non-overlapping match of this window, left to right (one memory round trip serves them all)
+            const uint32_t packed = (moff << 4) | mlen0;
+            // a stride-1 window yields at most 8 sequences (matches are >= 4 bytes): make room in the 32 staging lanes first
+            if (nseq - flushed > 24u) {
+                if ((uint32_t)lane < nseq - flushed) { const uint32_t at = flushed + (uint32_t)lane; o_ll[at] = (uint16_t)s_ll; o_ml[at] = (uint16_t)s_ml; o_off[at] = s_off; }
+                flushed = nseq;
+            }
+            uint32_t next_lane = 0;
+            bool cov = false;                               // this lane's byte is covered by a selected match
+            while (next_lane < 32) {
+                const uint32_t m = found & (0xFFFFFFFFu << next_lane);
+                if (!m) break;
+                int f = __ffs((int)m) - 1;
+                uint32_t mo = __shfl_sync(0xFFFFFFFFu, packed, f);          // (offset << 4) | length
+                // one step of lazy matching: a clearly longer match starting at the next position wins (one more literal)
+                if (lazy && (mo & 15u) < 8 && f < 31 && ((found >> (f + 1)) & 1u)) {
+                    const uint32_t mo2 = __shfl_sync(0xFFFFFFFFu, packed, f + 1);
+                    if ((mo2 & 15u) > (mo & 15u) + 1) { f++; mo = mo2; }
+                }
+                uint32_t ml = mo & 15u;
+                const uint32_t off = mo >> 4;
+                const uint32_t mpos = wb + (uint32_t)f;
+                if (ml == 8) zkc_extend_fwd(sb, mpos, off, hi32, lane, ml);
+                // emit: literals [anchor, mpos) are already / will be placed by the windows that hold them
+                const uint32_t ll = mpos - anchor;
+                // after every sequence r0 == off; a repeat of r0 itself (ll != 0) leaves the history alone, every other
+                // case shifts (r0 -> r1) and drops r2, except the r1 hit, which swaps the first two
+                uint32_t ov = off + 3;
+                if (off != r0 && off != r1 && off != r2 && off + 1 != r0) {           // the common case: an explicit offset
+                    r2 = r1; r1 = r0; r0 = off; known += known < 3;
+                } else {
+                    bool hit0 = false, hit1 = false;
+                    if (known == 3) {
+                        const bool e0 = off == r0, e1 = off == r1, e2 = off == r2, em = r0 > 1 && off == r0 - 1;
+                        if (ll != 0) { if (e0) { ov = 1; hit0 = true; } else if (e1) { ov = 2; hit1 = true; } else if (e2) ov = 3; }
+                        else { if (e1) { ov = 1; hit1 = true; } else if (e2) ov = 2; else if (em) ov = 3; }
+                    } else known++;
+                    if (!hit0) { r2 = hit1 ? r2 : r1; r1 = r0; r0 = off; }
+                }
+                if (lane == (int)(nseq - flushed)) { s_ll = ll; s_ml = ml - 3; s_off = ov; }
+                nseq++;
+                cov = cov || (p - mpos < ml);               // unsigned: mpos <= p < mpos + ml
+                anchor = mpos + ml; rep = off;
+                next_lane = anchor - wb;                    // >= 32: the match runs past the window
+            }
+            const uint32_t lm = __ballot_sync(0xFFFFFFFFu, !cov);
+            if (!cov) o_lit[nlit + __popc(lm & lt_mask)] = (uint8_t)cur;
+            nlit += (uint32_t)__popc(lm);
+            ip = anchor > wb + 32u ? anchor : wb + 32u;
+        }
+        if ((uint32_t)lane < nseq - flushed) {
+            const uint32_t at = flushed + (uint32_t)lane;
+            o_ll[at] = (uint16_t)s_ll; o_ml[at] = (uint16_t)s_ml; o_off[at] = s_off;
+        }
+    }
+    const uint32_t rest = hi32 - ip;
+    for (uint32_t i = lane; i < rest; i += 32) o_lit[nlit + i] = sb[ip + i];
+    nlit += rest;
+    if (lane == 0) { a.blocks[b].nseq = nseq; a.blocks[b].nlit = nlit; }
+}
+
+// levels 1-12: a history of one block, u16 positions, NW warps per CTA with their tables in static shared memory
 template <int HLOG, int NW, bool DFAST>
 __global__ void __launch_bounds__(NW * 32) zk_match_kernel(ZkEncodeArgs a) {
     __shared__ uint16_t tables[NW][(DFAST ? 2 : 1) << HLOG];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t b = blockIdx.x * NW + warp;
     if (b >= a.n_blocks) return;
-    uint16_t* table = tables[warp];
-    uint16_t* tableL = table + (1 << HLOG);                // only touched when DFAST
-#define ZKM_POS_T uint16_t
-#define ZKM_HIST_BYTES ZKC_BLOCK
-#include "zk_match_body.inc"
-#undef ZKM_POS_T
-#undef ZKM_HIST_BYTES
+    zkc_match_block<HLOG, DFAST, uint16_t, ZKC_BLOCK>(a, b, lane, tables[warp], tables[warp] + (1 << HLOG));
 }
 
-// Wide-history tier (level >= ZKC_WIDE_LEVEL): the same body with a history of ZKC_WIDE_HIST blocks of the frame instead of one -- the frame
+// Wide-history tier (level >= ZKC_WIDE_LEVEL): the same match finder with a history of ZKC_WIDE_HIST blocks of the frame instead of one -- the frame
 // header then announces a 256 KiB window (zk_frame_gather_kernel) --, 32-bit positions, and one table of 2^HLOG entries in DYNAMIC shared memory
 // (128 KiB at HLOG 15: one warp-CTA per SM).  Every block still finds its matches alone and pre-inserts its whole history first, so a block costs
 // several times a level-3 block: a tier for ratio (2.50 on the reference's corpus against 2.40 in a 64 KiB window), not for speed.
@@ -269,25 +436,18 @@ __global__ void __launch_bounds__(NW * 32) zk_match_kernel(ZkEncodeArgs a) {
 template <int HLOG>
 __global__ void __launch_bounds__(32) zk_match_wide_kernel(ZkEncodeArgs a) {
     ZK_DYN_SMEM(wide_tab);
-    constexpr bool DFAST = false;
-    const int warp = 0, lane = threadIdx.x & 31;
     const uint32_t b = blockIdx.x;
     if (b >= a.n_blocks) return;
-    uint32_t* table = (uint32_t*)wide_tab;
-    uint32_t* tableL = table;                               // never touched (DFAST is false)
-    (void)warp; (void)tableL;
-#define ZKM_POS_T uint32_t
-#define ZKM_HIST_BYTES ((size_t)ZKC_WIDE_HIST * ZKC_BLOCK)
-#include "zk_match_body.inc"
-#undef ZKM_POS_T
-#undef ZKM_HIST_BYTES
+    zkc_match_block<HLOG, false, uint32_t, ZKC_WIDE_HIST * ZKC_BLOCK>(a, b, threadIdx.x & 31, (uint32_t*)wide_tab, nullptr);
 }
 
 // Fast tier (level < 0, zstd's negative levels; acceleration A = -level): level 1's table, warps and history, with sparse probing.  Lane i of
 // a window probes position ip + i * s, where s = A + 1 + (windows since the last match) / ZKC_FAST_GROW, so long stretches without a match
 // are crossed ever faster.  Lanes whose probe lies past the last position where 8 bytes can be read idle for that window; only probed positions
 // are inserted.  A hit is extended forward as in the other tiers and backward down to the end of the previous sequence, which recovers the
-// start a sparse probe missed.  Literals are copied from the input when a sequence (or the block) ends.
+// start a sparse probe missed.  Literals are copied from the input when a sequence (or the block) ends.  The window setup and the sequence
+// staging repeat zkc_match_block's: shared with it as functions, they made the level-1 kernel compile to different code that took 11.19-11.28
+// ms per GiB of the bench mix instead of 10.64-10.67 (H100 80GB HBM3, 700 W).
 #define ZKC_FAST_GROW 8
 #define ZKC_MIN_LEVEL (-131072)          // ZSTD_minCLevel(): lower levels clamp to it
 template <int HLOG, int NW>
@@ -314,15 +474,7 @@ __global__ void __launch_bounds__(NW * 32) zk_match_fast_kernel(ZkEncodeArgs a) 
     if (hi32 - lo32 >= 16) {
         const uint32_t mflimit = hi32 - 8;                  // last position where 8 bytes can be read
         const uint32_t step0 = (uint32_t)(-a.level) + 1u;
-        if (pfx) {                                          // the prefix tail, as at level 1
-            for (uint32_t p0 = 0; p0 < lo32; p0 += 32) {
-                const uint32_t p = p0 + lane;
-                const uint32_t hh = p < lo32 ? zkc_hash5<HLOG>(zkc_ld8(sb + p)) : (0xFFFF0000u | (uint32_t)lane);
-                const uint32_t same = __match_any_sync(0xFFFFFFFFu, hh);
-                if (p < lo32 && lane == 31 - __clz((int)same)) table[hh] = (uint16_t)p;
-            }
-            __syncwarp();
-        }
+        if (pfx) zkc_insert_history<HLOG, false>(sb, lo32, lane, table);       // the prefix tail, as at level 1
         uint32_t rep = 0, r0 = 1, r1 = 4, r2 = 8, known = lo == fstart ? 3u : 0u;
         uint32_t misses = 0;                                // windows since the last match
         uint32_t s_ll = 0, s_ml = 0, s_off = 0, flushed = 0; // staged sequences: slot nseq - flushed lives in that lane
