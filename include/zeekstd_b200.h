@@ -249,6 +249,34 @@ int32_t zk_compress_frames_sized_long_dev(zk_ctx* ctx, const void* d_src, const 
                                           int32_t checksum, void* d_dst, size_t dst_cap, uint32_t* c_sizes, size_t* dst_len,
                                           void* cuda_stream);
 
+/*
+ * Per-frame prefixes (batched deltas, seekable patches): frames of caller-chosen sizes, frame f matched against its own range
+ * prefix[ranges[2f] .. ranges[2f+1]) of one prefix buffer -- each object against its own previous version, or each frame of a new image
+ * against the slice of the old image around it -- in one batch instead of one call per frame.
+ *   - Frame bytes: frame f is exactly what zk_compress_frames_sized (ldm and long_mode 0), zk_compress_frames_sized_ldm (ldm != 0) or
+ *     zk_compress_frames_sized_long (long_mode != 0) writes for frame f alone with its range as the prefix, at every level, with either
+ *     checksum setting, Window_Descriptor included.  Exceptions: under ldm, a frame whose range is empty is what zk_compress_frames_sized
+ *     writes for it at level 16 with no prefix, and an empty frame (size 0) is level 16's empty frame.
+ *   - Tiers: with ldm or long_mode set and a non-empty prefix buffer, every frame runs the high-level tier (level 16's bytes), whatever
+ *     its range, so one call never mixes tiers; without either flag a frame with an empty range is the plain frame at `level`.
+ *   - ranges == NULL gives every frame the whole buffer: the call then equals zk_compress_frames_sized / _sized_ldm / _sized_long on the
+ *     same arguments.  A range with lo > hi or hi > prefix_len, or a prefix_len above 2^31 - 1, returns ZK_ERR_INVALID_ARG.  Empty frames,
+ *     more than ZK_SEEKABLE_MAX_FRAMES frames and a short dst_cap behave as in zk_compress_frames_sized; n_frames == 0 writes nothing.
+ *   - The prefix buffer is uploaded once per call.  With ldm or long_mode, every distinct range is indexed once (its last min(length,
+ *     2^27 - 1) bytes, about 1 byte of device scratch per indexed byte); the call cuts its batch so that this stays bounded, and a frame
+ *     whose range is 2^31 - 1 bytes long always runs.
+ * zk_decompress_frames_prefixes decodes entry e (every zstd frame in it) against prefix[ranges[2e] .. ranges[2e+1]): exactly as
+ * zk_decompress_frames_prefix decodes that entry alone with its range as the prefix, d_need, checksum verification and every error code
+ * included (an offset that reaches before the start of the entry's range is -20, corruption_detected).  ranges == NULL: every entry
+ * against the whole buffer, which is zk_decompress_frames_prefix.  Range checks as above.  HOST pointers.
+ */
+int32_t zk_compress_frames_sized_prefixes(zk_ctx* ctx, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                          int32_t checksum, const uint8_t* prefix, size_t prefix_len, const uint64_t* ranges,
+                                          int32_t ldm, int32_t long_mode, uint8_t* dst, size_t dst_cap, uint32_t* c_sizes, size_t* dst_len);
+int32_t zk_decompress_frames_prefixes(zk_ctx* ctx, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n_frames,
+                                      uint8_t* dst, const uint32_t* d_need, int32_t verify_checksum, int32_t* status,
+                                      const uint8_t* prefix, size_t prefix_len, const uint64_t* ranges);
+
 /* ------------------------------------------------------------------ SeekTable (lib/src/seek_table.rs) */
 typedef struct zk_seek_table zk_seek_table;
 typedef enum { ZK_FORMAT_HEAD = 0, ZK_FORMAT_FOOT = 1 } zk_format; /* seek_table.rs:228-241 */

@@ -161,10 +161,12 @@ class Context:
         return dst[: dl.value], cs[: nf.value].copy(), ds[: nf.value].copy()
 
     def compress_frames_sized(self, data, frame_sizes, level: int = 0, checksum: bool = False, prefix=None, long_distance: bool = False,
-                              long_mode: bool = False):
+                              long_mode: bool = False, prefix_ranges=None):
         """frames of caller-chosen sizes in one batch: frame f covers the next frame_sizes[f] bytes of data (their sum is its length)
         -> (compressed bytes (np.uint8), c_sizes, d_sizes).  Each frame is what compress_frames makes of its bytes alone
-        (long_distance and long_mode as there)."""
+        (long_distance and long_mode as there).  prefix_ranges (n x 2 integers): frame f's prefix is only
+        prefix[prefix_ranges[f][0]:prefix_ranges[f][1]] (zk_compress_frames_sized_prefixes), and the frame is what this call makes of it
+        alone with that slice as the prefix."""
         addr, n, keep = _buf(data)
         ds = np.ascontiguousarray(frame_sizes, dtype=np.uint32).reshape(-1)
         if int(np.sum(ds, dtype=np.uint64)) != n:
@@ -176,6 +178,12 @@ class Context:
         cs = np.zeros(ds.size, dtype=np.uint32)
         dl = c_size_t()
         paddr, pn, pkeep = _buf(prefix) if prefix is not None else (None, 0, None)
+        if prefix_ranges is not None:
+            rg = _ranges(prefix_ranges, ds.size)
+            _check(lib.zk_compress_frames_sized_prefixes(self._h, addr, dsp, ds.size, level, int(checksum), paddr, pn,
+                                                         rg.ctypes.data_as(_native.u64p), int(long_distance), int(long_mode), dst.ctypes.data,
+                                                         cap, cs.ctypes.data_as(_native.u32p), byref(dl)), lib)
+            return dst[: dl.value], cs, ds.copy()
         fn = lib.zk_compress_frames_sized_long if long_mode else lib.zk_compress_frames_sized_ldm if long_distance else lib.zk_compress_frames_sized
         _check(fn(self._h, addr, dsp, ds.size, level, int(checksum), paddr, pn, dst.ctypes.data, cap,
                                             cs.ctypes.data_as(_native.u32p), byref(dl)), lib)
@@ -216,10 +224,13 @@ class Context:
                                           byref(used)), lib)
         return dst[: dl.value], cs[: nf.value].copy(), ds[: nf.value].copy(), int(used.value)
 
-    def decompress_frames(self, comp, c_off, d_off, verify_checksum: bool = True, out: np.ndarray | None = None, need=None, prefix=None):
+    def decompress_frames(self, comp, c_off, d_off, verify_checksum: bool = True, out: np.ndarray | None = None, need=None, prefix=None,
+                          prefix_ranges=None):
         """decode frames given N+1 cumulative offsets -> (np.uint8 output, per-frame status, rc).
         need (optional, one uint32 per frame): only that many leading bytes of each frame are wanted (range reads,
-        zk_decompress_frames_upto): the rest of a frame's output range is then unspecified and its checksum is not verified."""
+        zk_decompress_frames_upto): the rest of a frame's output range is then unspecified and its checksum is not verified.
+        prefix_ranges (n x 2 integers): entry e is decoded against prefix[prefix_ranges[e][0]:prefix_ranges[e][1]] only
+        (zk_decompress_frames_prefixes)."""
         addr, n, keep = _buf(comp)
         co = np.ascontiguousarray(c_off, dtype=np.uint64); do = np.ascontiguousarray(d_off, dtype=np.uint64)
         nf = len(co) - 1
@@ -233,10 +244,28 @@ class Context:
         if nd is not None and len(nd) != nf:
             raise ValueError("need: one entry per frame")
         paddr, pn, pkeep = _buf(prefix) if prefix is not None else (None, 0, None)
+        if prefix_ranges is not None:
+            rg = _ranges(prefix_ranges, nf)
+            rc = self.lib.zk_decompress_frames_prefixes(self._h, addr, co.ctypes.data_as(_native.u64p), do.ctypes.data_as(_native.u64p), nf,
+                                                        out.ctypes.data, None if nd is None else nd.ctypes.data_as(_native.u32p),
+                                                        int(verify_checksum), st.ctypes.data_as(_native.i32p), paddr, pn,
+                                                        rg.ctypes.data_as(_native.u64p))
+            return out[:total], st[:nf], rc
         rc = self.lib.zk_decompress_frames_prefix(self._h, addr, co.ctypes.data_as(_native.u64p), do.ctypes.data_as(_native.u64p), nf,
                                                   out.ctypes.data, None if nd is None else nd.ctypes.data_as(_native.u32p),
                                                   int(verify_checksum), st.ctypes.data_as(_native.i32p), paddr, pn)
         return out[:total], st[:nf], rc
+
+
+def _ranges(prefix_ranges, n: int) -> np.ndarray:
+    """n (lo, hi) prefix ranges -> a C-contiguous n x 2 np.uint64 array"""
+    rg = np.asarray(prefix_ranges)
+    if rg.size and (rg.dtype.kind not in "iu" or int(rg.min()) < 0):
+        raise ValueError("prefix_ranges: non-negative integers")
+    rg = np.ascontiguousarray(rg, dtype=np.uint64).reshape(-1, 2) if rg.size else np.zeros((0, 2), dtype=np.uint64)
+    if len(rg) != n:
+        raise ValueError(f"prefix_ranges: one (lo, hi) pair per frame, {n} expected, {len(rg)} given")
+    return rg if n else np.zeros((1, 2), dtype=np.uint64)
 
 
 _default_ctx: Context | None = None

@@ -7,6 +7,7 @@
 #include <time.h>
 #include <stdlib.h>
 #include <string.h>
+#include <set>
 #include <vector>
 
 static thread_local char zk_tls_cuda_msg[256] = "";
@@ -176,6 +177,21 @@ static int32_t zk_upload_prefix(zk_ctx* c, const uint8_t* prefix, size_t len, co
     return 0;
 }
 
+// per-frame prefixes: n ranges [ranges[2i], ranges[2i + 1]) of a prefix buffer of len bytes -> *out (two words per range); NULL: none (every
+// frame has the whole buffer)
+static int32_t zk_prefix_ranges(const uint64_t* ranges, uint32_t n, size_t len, std::vector<uint32_t>* out) {
+    out->clear();
+    if (!ranges) return 0;
+    if (len > 0x7FFFFFFFull) return ZK_ERR_INVALID_ARG;
+    out->resize(2 * (size_t)n);
+    for (uint32_t i = 0; i < n; i++) {
+        const uint64_t lo = ranges[2 * i], hi = ranges[2 * i + 1];
+        if (lo > hi || hi > len) return ZK_ERR_INVALID_ARG;
+        (*out)[2 * i] = (uint32_t)lo; (*out)[2 * i + 1] = (uint32_t)hi;
+    }
+    return 0;
+}
+
 // ---------------------------------------------------------------------------------------------
 // decompress
 // ---------------------------------------------------------------------------------------------
@@ -258,6 +274,7 @@ static int zk_dec_sub_enqueue(zk_ctx* c, int si, ZkSubDec& sb, const ZkDecCall& 
     if (tr) tr->mark(us, k, 1);
     ZkDecodeParams p = q.p;
     if (p.need) p.need += f;
+    if (p.ranges) p.ranges += 2 * (size_t)f;
     rc = zk_decode_enqueue(&s.dws, s.stream, s.d_in, sb.c_rel.data(), sb.d_rel.data(), cnt, s.d_out, q.verify, p);
     if (rc) return rc;
     if (tr) tr->mark(s.stream, k, 2);
@@ -296,10 +313,20 @@ extern "C" int32_t zk_decompress_frames_upto(zk_ctx* c, const uint8_t* comp, con
 extern "C" int32_t zk_decompress_frames_prefix(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n,
                                                uint8_t* dst, const uint32_t* d_need, int32_t verify, int32_t* status,
                                                const uint8_t* prefix, size_t prefix_len) {
+    return zk_decompress_frames_prefixes(c, comp, c_off, d_off, n, dst, d_need, verify, status, prefix, prefix_len, nullptr);
+}
+
+// entry e decoded against its own range of the prefix buffer; ranges == NULL: every entry against the whole buffer
+extern "C" int32_t zk_decompress_frames_prefixes(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n,
+                                                 uint8_t* dst, const uint32_t* d_need, int32_t verify, int32_t* status,
+                                                 const uint8_t* prefix, size_t prefix_len, const uint64_t* ranges) {
     if (!c) return ZK_ERR_INVALID_ARG;
     ZkDecCall q = {comp, c_off, d_off, dst, verify, status, ZkDecodeParams()};
-    int32_t rc = zk_upload_prefix(c, prefix, prefix_len, &q.p.prefix, &q.p.prefix_len);
+    std::vector<uint32_t> rw;
+    int32_t rc = zk_prefix_ranges(ranges, n, prefix_len, &rw);
+    if (!rc) rc = zk_upload_prefix(c, prefix, prefix_len, &q.p.prefix, &q.p.prefix_len);
     if (rc) return rc;
+    if (q.p.prefix && ranges) q.p.ranges = rw.data();
     if (n && (!comp || !c_off || !d_off || !dst)) return ZK_ERR_INVALID_ARG;
     if (n == 0) return 0;
     ZK_CUDA_OK(cudaSetDevice(c->device));
@@ -349,7 +376,8 @@ struct ZkCompressReq {
     bool host = true;                                       // src and dst in host memory; else device memory, worked on `stream`
     cudaStream_t stream = nullptr;                          // nullptr: slot 0's
     const uint8_t* prefix = nullptr; size_t prefix_len = 0; // host memory
-    ZkEncodeParams params;                                  // its prefix: the device copy of `prefix`
+    const uint64_t* ranges = nullptr;                       // sized: frame f's prefix is prefix[ranges[2f], ranges[2f + 1]) (NULL: all of it)
+    ZkEncodeParams params;                                  // its prefix: the device copy of `prefix`, and the ranges as 32-bit words
     int32_t final_ = 1;                                     // Compressed / ContentDefined: no more input follows this call's
     uint8_t* dst = nullptr; size_t dst_cap = 0;
     uint32_t* c_sizes = nullptr; uint32_t* d_sizes = nullptr; uint32_t frames_cap = 0; uint32_t* n_frames = nullptr;
@@ -374,6 +402,27 @@ static int32_t zk_compress_dev_subs(zk_ctx* c, const ZkFrames& fr, const uint8_t
 }
 
 struct ZkSubEnc { uint32_t f0 = 0, cnt = 0; size_t in_off = 0, in_len = 0, out_pos = 0; bool busy = false; };
+
+// Long-distance matching indexes every distinct prefix range of a sub-batch once, at about one byte of scratch per indexed byte (the last
+// min(length, 2^27 - 1) bytes of the range): the sub-batch [f0, end) ends early where the ranges it indexes would pass max(sub_bytes, 2^27)
+// bytes.  It keeps at least one frame, so a frame with a prefix of any length runs.  *in_len: the input bytes of what is kept
+static uint32_t zk_ldm_sub_end(const ZkFrames& fr, const uint32_t* ranges, uint32_t f0, uint32_t end, size_t sub_bytes, size_t* in_len) {
+    const size_t reach = (1u << 27) - 1u, budget = sub_bytes > reach + 1 ? sub_bytes : reach + 1;
+    std::set<unsigned long long> seen;
+    size_t indexed = 0, bytes = 0;
+    uint32_t f = f0;
+    for (; f < end; f++) {
+        const uint32_t lo = ranges[2 * (size_t)f], hi = ranges[2 * (size_t)f + 1];
+        if (hi > lo && seen.insert((unsigned long long)lo << 32 | hi).second) {
+            const size_t add = hi - lo < reach ? hi - lo : reach;
+            if (f > f0 && indexed + add > budget) break;
+            indexed += add;
+        }
+        bytes += fr.size(f);
+    }
+    *in_len = bytes;
+    return f;
+}
 
 // host input and output: sub-batches on up to ZK_HOST_SLOTS_ENC slots, output placed in order
 static int32_t zk_compress_host_run(zk_ctx* c, const ZkFrames& fr, const ZkCompressReq& q, size_t sub_bytes, size_t* dst_len) {
@@ -411,7 +460,10 @@ static int32_t zk_compress_host_run(zk_ctx* c, const ZkFrames& fr, const ZkCompr
         }
         ZkSlot& s = c->slot[si]; ZkSubEnc& sb = sub[si];
         if (cudaStreamSynchronize(s.stream) != cudaSuccess) { err = ZK_ERR_CUDA; break; }   // its previous D2H must be done before d_out is reused
-        const uint32_t end = fr.next_sub(f0, sub_bytes, &sb.in_len);
+        uint32_t end = fr.next_sub(f0, sub_bytes, &sb.in_len);
+        if (p.ranges && (p.ldm || p.long_mode)) end = zk_ldm_sub_end(fr, p.ranges, f0, end, sub_bytes, &sb.in_len);
+        ZkEncodeParams sp = p;
+        if (p.ranges) sp.ranges = p.ranges + 2 * (size_t)f0;
         sb.f0 = f0; sb.cnt = end - f0; sb.in_off = in_off;
         const ZkFrames sf = fr.sub(f0, sb.cnt, sb.in_len);
         const size_t bound = sf.bound();
@@ -420,7 +472,7 @@ static int32_t zk_compress_host_run(zk_ctx* c, const ZkFrames& fr, const ZkCompr
         sub_k[si] = (int)k; tr.mark(s.stream, (int)k, 0);
         if (sb.in_len && cudaMemcpyAsync(s.d_in, q.src + sb.in_off, sb.in_len, cudaMemcpyHostToDevice, s.stream) != cudaSuccess) { err = ZK_ERR_CUDA; break; }
         tr.mark(s.stream, (int)k, 1);
-        rc = zk_encode_enqueue(&s.ews, s.stream, s.d_in, sf, p, s.d_out, bound);
+        rc = zk_encode_enqueue(&s.ews, s.stream, s.d_in, sf, sp, s.d_out, bound);
         if (rc) { err = rc; break; }
         tr.mark(s.stream, (int)k, 2);
         sb.busy = true; n_inflight++;
@@ -536,6 +588,7 @@ static int32_t zk_cdc_passes(zk_ctx* c, const ZkCompressReq& q, cudaStream_t st,
 static int32_t zk_compress(zk_ctx* c, ZkCompressReq q) {
     ZkFrames fr = {};
     int32_t rc = 0;
+    std::vector<uint32_t> range_words;
     if (q.policy == ZK_FRAMES_UNIFORM) {
         if (!c) return ZK_ERR_INVALID_ARG;
         if ((rc = zk_upload_prefix(c, q.prefix, q.prefix_len, &q.params.prefix, &q.params.prefix_len))) return rc;
@@ -555,7 +608,9 @@ static int32_t zk_compress(zk_ctx* c, ZkCompressReq q) {
         if (q.n && !q.src) return ZK_ERR_INVALID_ARG;
         if (q.dst_len) *q.dst_len = 0;
         if (q.count == 0) return 0;                         // (no frame, unlike the uniform layout of no input)
+        if ((rc = zk_prefix_ranges(q.ranges, q.count, q.prefix_len, &range_words))) return rc;
         if ((rc = zk_upload_prefix(c, q.prefix, q.prefix_len, &q.params.prefix, &q.params.prefix_len))) return rc;
+        if (q.params.prefix && q.ranges) q.params.ranges = range_words.data();
         fr = {q.sizes, q.n, 0, q.count};
     } else {
         if (!c || !q.dst || (q.n && !q.src)) return ZK_ERR_INVALID_ARG;
@@ -689,6 +744,19 @@ extern "C" int32_t zk_compress_frames_sized_long(zk_ctx* c, const uint8_t* src, 
     ZkCompressReq q;
     q.policy = ZK_FRAMES_SIZED; q.sizes = frame_sizes; q.count = n_frames; q.src = src; q.prefix = prefix; q.prefix_len = prefix_len;
     q.params.level = level; q.params.checksum = checksum; q.params.long_mode = true;
+    q.dst = dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.dst_len = dst_len;
+    return zk_compress(c, q);
+}
+
+// frames of caller-chosen sizes, frame f against its own range of one prefix buffer: what the sized call (or its _ldm / _long variant)
+// writes for frame f alone with that range as its prefix
+extern "C" int32_t zk_compress_frames_sized_prefixes(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                                     int32_t checksum, const uint8_t* prefix, size_t prefix_len, const uint64_t* ranges, int32_t ldm,
+                                                     int32_t long_mode, uint8_t* dst, size_t dst_cap, uint32_t* c_sizes, size_t* dst_len) {
+    ZkCompressReq q;
+    q.policy = ZK_FRAMES_SIZED; q.sizes = frame_sizes; q.count = n_frames; q.src = src; q.prefix = prefix; q.prefix_len = prefix_len;
+    q.ranges = ranges;
+    q.params.level = level; q.params.checksum = checksum; q.params.ldm = ldm != 0; q.params.long_mode = long_mode != 0;
     q.dst = dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.dst_len = dst_len;
     return zk_compress(c, q);
 }

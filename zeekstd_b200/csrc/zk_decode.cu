@@ -1259,16 +1259,23 @@ __device__ __forceinline__ void zk_chunk_literals(const ZkRing& rg, const uint8_
     }
 }
 
+// Prefix mode: the prefix of an entry's zstd frames, its range of the prefix buffer (ZkDecodeArgs::pranges): `len` bytes that end at `end`
+struct ZkPrefixSlice { const uint8_t* end; uint32_t len; };
+__device__ __forceinline__ ZkPrefixSlice zk_entry_prefix(const ZkDecodeArgs& a, uint32_t e) {
+    const uint32_t lo = a.pranges[2 * e], hi = a.pranges[2 * e + 1];
+    return {a.prefix + hi, hi - lo};
+}
+
 // Prefix mode: the part of a match that lies before its frame's first byte (zstart) comes from the raw-content prefix that
-// precedes every zstd frame.  That part is constant data with no dependency, copied at once by its lane; what is left of the
-// match, if anything, starts at the frame's first byte with the same offset and is an ordinary match.  TO_RING: destination
+// precedes every zstd frame of the entry.  That part is constant data with no dependency, copied at once by its lane; what is left
+// of the match, if anything, starts at the frame's first byte with the same offset and is an ordinary match.  TO_RING: destination
 // is the ring, else HBM directly.
 template <bool TO_RING>
-__device__ __forceinline__ void zk_prefix_part(const ZkRing& rg, const ZkDecodeArgs& a, bool valid, uint32_t zstart, uint32_t off,
+__device__ __forceinline__ void zk_prefix_part(const ZkRing& rg, const ZkPrefixSlice& px, bool valid, uint32_t zstart, uint32_t off,
                                                uint32_t& md, uint32_t& ml) {
     if (valid && ml > 0 && off > md - zstart) {
         const uint32_t back = off - (md - zstart), la = ml < back ? ml : back;
-        const uint8_t* ps = a.prefix + (a.prefix_len - back);
+        const uint8_t* ps = px.end - back;
         for (uint32_t i = 0; i < la; i++) { if (TO_RING) rg.at(md + i) = ps[i]; else rg.out[md + i] = ps[i]; }
         md += la; ml -= la;
     }
@@ -1305,10 +1312,11 @@ struct ZkLaneSeq {
 
 // Load lane `lane`'s sequence of chunk j of a block (sequences seq_base + [32j, 32j + 32) of nseq); le0 / oe0 are lane 0's
 // predecessor ends (those of sequence 32j - 1, 0 for the first chunk).  Resolves a symbolic offset and checks the offset
-// against the output of the frame before it (and the prefix).  Returns, on every lane, whether some lane's offset is bad.
+// against the output of the frame before it (and the entry's prefix, px).  Returns, on every lane, whether some lane's offset is bad.
 template <bool PREFIX>
 __device__ __forceinline__ bool zk_lane_seq(ZkLaneSeq& q, const ZkDecodeArgs& a, uint32_t seq_base, uint32_t nseq, const ZkRepOffsets& rep,
-                                            uint32_t j, uint32_t pos, uint32_t zstart, uint32_t le0, uint32_t oe0, int lane) {
+                                            uint32_t j, uint32_t pos, uint32_t zstart, uint32_t le0, uint32_t oe0, int lane,
+                                            const ZkPrefixSlice& px) {
     const uint32_t s = j * 32 + lane;
     q.valid = s < nseq;
     const uint32_t sc = q.valid ? s : nseq - 1;
@@ -1325,7 +1333,7 @@ __device__ __forceinline__ bool zk_lane_seq(ZkLaneSeq& q, const ZkDecodeArgs& a,
             const uint32_t r = rep.slot(offv), dl = ZK_SYM_DELTA(offv);
             bad = r <= dl; q.off = r - dl;
         }
-        if (q.off == 0 || q.off > q.md - zstart + (PREFIX ? a.prefix_len : 0u)) bad = true;
+        if (q.off == 0 || q.off > q.md - zstart + (PREFIX ? px.len : 0u)) bad = true;
     }
     return __any_sync(0xFFFFFFFFu, bad);
 }
@@ -1366,7 +1374,7 @@ __device__ __forceinline__ void zk_trailing_literals(const ZkRing& rg, uint32_t 
 // the ring is reloaded with its last half ring.  Literal runs of 256 bytes or more are copied by the whole warp, shorter ones
 // byte-parallel; within the chunk, a match goes once every earlier match that its source overlaps is written.
 template <bool PREFIX>
-__device__ __forceinline__ void zk_direct_chunk(const ZkRing& rg, const ZkDecodeArgs& a, uint32_t lit_kind, uint32_t lit_byte, const uint8_t* lit, ZkLaneSeq& q,
+__device__ __forceinline__ void zk_direct_chunk(const ZkRing& rg, const ZkPrefixSlice& px, uint32_t lit_kind, uint32_t lit_byte, const uint8_t* lit, ZkLaneSeq& q,
                                                 uint32_t zstart, uint32_t chunk_end, uint32_t half, int lane) {
     uint8_t* out = rg.out;
     uint32_t longlit = __ballot_sync(0xFFFFFFFFu, q.valid && q.ll >= 256);
@@ -1384,7 +1392,7 @@ __device__ __forceinline__ void zk_direct_chunk(const ZkRing& rg, const ZkDecode
             else zk_warp_copy(out + d, lit + sp, n, lane);
         }
     }
-    if (PREFIX) zk_prefix_part<false>(rg, a, q.valid, zstart, q.off, q.md, q.ml);
+    if (PREFIX) zk_prefix_part<false>(rg, px, q.valid, zstart, q.off, q.md, q.ml);
     __syncwarp();
     const uint32_t need_end = q.md - q.off + (q.ml < q.off ? q.ml : q.off);
     uint32_t pending = __ballot_sync(0xFFFFFFFFu, q.valid && q.ml > 0);
@@ -1519,6 +1527,7 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, W = blockDim.x >> 5;
     const ZkBlock head = a.blocks[first_bidx];
     const uint32_t e = head.entry;
+    const ZkPrefixSlice px = PREFIX ? zk_entry_prefix(a, e) : ZkPrefixSlice{nullptr, 0u};
     const ZkEntry ent = a.entries[e];
     const uint32_t pos0 = head.out_pos;
     if (threadIdx.x == 0) { sm.done_pos = pos0; sm.done_chunk = 0; sm.flushed_pos = pos0; sm.flushed_chunk = 0; sm.abort_code = 0; sm.abort_block = 0xFFFFFFFFu; }
@@ -1573,7 +1582,7 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
             uint32_t le0 = 0, oe0 = 0;
             if (lane == 0 && j) { le0 = s_lit[j * 32 - 1]; oe0 = s_out[j * 32 - 1]; }
             ZkLaneSeq q;
-            if (zk_lane_seq<PREFIX>(q, a, blk.seq_base, blk.nseq, rep, j, pos, zstart, le0, oe0, lane)) { zk_d2_abort(sm, ZKZ_CORRUPTION, bi); break; }
+            if (zk_lane_seq<PREFIX>(q, a, blk.seq_base, blk.nseq, rep, j, pos, zstart, le0, oe0, lane, px)) { zk_d2_abort(sm, ZKZ_CORRUPTION, bi); break; }
             const uint32_t chunk_start = pos + __shfl_sync(0xFFFFFFFFu, q.oe_prev, 0);
             const uint32_t chunk_end = pos + __shfl_sync(0xFFFFFFFFu, q.oe, min(31u, blk.nseq - 1 - j * 32));
             const bool direct = chunk_end - chunk_start > half;
@@ -1601,7 +1610,7 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
 
             if (direct) {
                 // ======== huge chunk: HBM -> HBM, alone in flight (it is the oldest chunk)
-                zk_direct_chunk<PREFIX>(rg, a, blk.lit_kind, blk.lit_byte, lit, q, zstart, chunk_end, half, lane);
+                zk_direct_chunk<PREFIX>(rg, px, blk.lit_kind, blk.lit_byte, lit, q, zstart, chunk_end, half, lane);
                 zk_d2_mark_done(sm, c, lane);
                 zk_d2_mark_flushed(sm, c, lane);
                 continue;
@@ -1610,7 +1619,7 @@ __device__ __forceinline__ void zk_exec_segment(ZkD2Smem& sm, const ZkDecodeArgs
             // ======== normal chunk: build the output in the ring, then flush
             // literal runs: no dependencies (HBM scratch -> ring)
             zk_chunk_literals<true>(rg, lit, blk.lit_kind, blk.lit_byte, q.le, q.le_prev, q.o_lit, lane);
-            if (PREFIX) zk_prefix_part<true>(rg, a, q.valid, zstart, q.off, q.md, q.ml);
+            if (PREFIX) zk_prefix_part<true>(rg, px, q.valid, zstart, q.off, q.md, q.ml);
             {   // all literal runs are in place: sequences without a match (and the lanes past the last one) are complete
                 const uint32_t withm = __ballot_sync(0xFFFFFFFFu, q.valid && q.ml > 0);
                 zk_d2_progress(sm, c, ~withm, lane);
@@ -1752,6 +1761,7 @@ template <bool PREFIX>
 __device__ __forceinline__ void zk_exec_warp_segment(const ZkDecodeArgs& a, uint8_t* win, uint32_t first_bidx, int lane) {
     const ZkBlock& head = a.blocks[first_bidx];
     const uint32_t e = head.entry, pos0 = head.out_pos;
+    const ZkPrefixSlice px = PREFIX ? zk_entry_prefix(a, e) : ZkPrefixSlice{nullptr, 0u};
     const ZkEntry ent = a.entries[e];
     uint8_t* out = a.dst + a.d_off[e];
     const uint8_t* ebase = a.comp + a.c_off[e];
@@ -1779,15 +1789,15 @@ __device__ __forceinline__ void zk_exec_warp_segment(const ZkDecodeArgs& a, uint
         for (uint32_t j = 0; j * 32 < nseq; j++) {
             // ---------------- 32 sequences, one per lane
             ZkLaneSeq q;
-            if (zk_lane_seq<PREFIX>(q, a, seq_base, nseq, rep, j, pos, zstart, le_last, oe_last, lane)) { bad_block = bi; break; }
+            if (zk_lane_seq<PREFIX>(q, a, seq_base, nseq, rep, j, pos, zstart, le_last, oe_last, lane, px)) { bad_block = bi; break; }
             le_last = __shfl_sync(0xFFFFFFFFu, q.le, 31); oe_last = __shfl_sync(0xFFFFFFFFu, q.oe, 31);
             const uint32_t chunk_start = pos + __shfl_sync(0xFFFFFFFFu, q.oe_prev, 0), chunk_end = pos + oe_last;
             if (chunk_end - chunk_start > half) {
-                zk_direct_chunk<PREFIX>(rg, a, lit_kind, lit_byte, lit, q, zstart, chunk_end, half, lane);
+                zk_direct_chunk<PREFIX>(rg, px, lit_kind, lit_byte, lit, q, zstart, chunk_end, half, lane);
                 __syncwarp();
                 continue;
             }
-            if (PREFIX) zk_prefix_part<true>(rg, a, q.valid, zstart, q.off, q.md, q.ml);
+            if (PREFIX) zk_prefix_part<true>(rg, px, q.valid, zstart, q.off, q.md, q.ml);
             const uint32_t src0 = q.md - q.off, need_end = src0 + (q.ml < q.off ? q.ml : q.off);
             const bool near_src = src0 + half >= chunk_start;
             zk_chunk_literals<true>(rg, lit, lit_kind, lit_byte, q.le, q.le_prev, q.o_lit, lane);
@@ -1885,9 +1895,10 @@ __global__ void __launch_bounds__(128) zk_xxh64_kernel(ZkDecodeArgs a) {
 
 void zk_decode_ws_free(ZkDecodeWs* ws) {
     void* ptrs[] = { ws->blocks, ws->entries, ws->counters, ws->lit, ws->seq_lit_end, ws->seq_out_end, ws->seq_off, ws->c_off, ws->d_off,
-                     ws->huf_list, ws->seq_list, ws->seg_list, ws->d_need };
+                     ws->huf_list, ws->seq_list, ws->seg_list, ws->d_need, ws->d_pr };
     for (void* p : ptrs) if (p) cudaFree(p);
     if (ws->h_need) cudaFreeHost(ws->h_need);
+    if (ws->h_pr) cudaFreeHost(ws->h_pr);
     if (ws->h_entries) cudaFreeHost(ws->h_entries);
     if (ws->h_counters) cudaFreeHost(ws->h_counters);
     if (ws->h_off) cudaFreeHost(ws->h_off);
@@ -1936,8 +1947,12 @@ static int zk_decode_ensure(ZkDecodeWs* ws, uint32_t n, size_t need_blocks, size
         if (cudaMallocHost((void**)&ws->h_off, 2 * (c + 1) * 8) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
         if (ws->d_need) { cudaFree(ws->d_need); ws->d_need = nullptr; }
         if (ws->h_need) { cudaFreeHost(ws->h_need); ws->h_need = nullptr; }
+        if (ws->d_pr) { cudaFree(ws->d_pr); ws->d_pr = nullptr; }
+        if (ws->h_pr) { cudaFreeHost(ws->h_pr); ws->h_pr = nullptr; }
         if (cudaMalloc((void**)&ws->d_need, (c + 1) * 4) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
         if (cudaMallocHost((void**)&ws->h_need, (c + 1) * 4) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
+        if (cudaMalloc((void**)&ws->d_pr, c * 8) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
+        if (cudaMallocHost((void**)&ws->h_pr, c * 8) != cudaSuccess) return -(int)ZKZ_MEMORY_ALLOCATION;
         ws->cap_entries = c;
     }
     if (!ws->counters) {
@@ -1984,7 +1999,14 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     a.huf_list = ws->huf_list; a.seq_list = ws->seq_list; a.seg_list = ws->seg_list;
     a.cap_blocks = ws->cap_blocks; a.cap_lit = ws->cap_lit - 64; a.cap_seq = ws->cap_seq;
     a.d_need = nullptr;
-    a.prefix = p.prefix; a.prefix_len = p.prefix ? p.prefix_len : 0;
+    a.prefix = p.prefix; a.pranges = nullptr;
+    if (p.prefix) {                              // every entry's range of the prefix buffer (the whole buffer without p.ranges)
+        for (uint32_t i = 0; i < n; i++) {
+            ws->h_pr[2 * i] = p.ranges ? p.ranges[2 * i] : 0u; ws->h_pr[2 * i + 1] = p.ranges ? p.ranges[2 * i + 1] : p.prefix_len;
+        }
+        ZK_CUDA_OK(cudaMemcpyAsync(ws->d_pr, ws->h_pr, (size_t)n * 8, cudaMemcpyHostToDevice, us));
+        a.pranges = ws->d_pr;
+    }
     if (p.need) {
         memcpy(ws->h_need, p.need, (size_t)n * 4);
         ZK_CUDA_OK(cudaMemcpyAsync(ws->d_need, ws->h_need, (size_t)n * 4, cudaMemcpyHostToDevice, us));
@@ -2088,7 +2110,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     while (ring > 8 * 1024 && (size_t)ring * (size_t)per_sm > 200 * 1024) ring >>= 1;
     if (ws->ring_override) ring = ws->ring_override;
     // prefix mode: the same executors, built with the prefix split
-    const bool prefix = a.prefix_len != 0;
+    const bool prefix = a.prefix != nullptr;
     if (a.exec_short) {          // short segments first, on single warps; the CTAs below then pull only long ones
         uint32_t gw = (uint32_t)sms * 8u;
         const size_t need_w = est_blocks / ZK_XW_WARPS + 1;

@@ -18,7 +18,8 @@ struct ZkDecodeArgs {                 // kernel parameter block (by value)
                                               // front, short ones from the back: together never more than cap_blocks)
     uint32_t exec_short;                      // segments of at most this many output bytes run on one warp each; 0 = none
     unsigned long long cap_blocks, cap_lit, cap_seq;
-    const uint8_t* prefix; uint32_t prefix_len;   // raw-content prefix of every zstd frame (Decoder::decompress_with_prefix, decode.rs:211-214, 246-255); device pointer or nullptr
+    const uint8_t* prefix;            // the buffer of the raw-content prefixes of the zstd frames (Decoder::decompress_with_prefix, decode.rs:211-214, 246-255); device pointer or nullptr
+    const uint32_t* pranges;          // device, two per entry: every zstd frame of entry e has the prefix prefix[pranges[2e], pranges[2e + 1])
     const uint32_t* d_need;           // per entry: only this many leading bytes are wanted (range reads); nullptr = everything
 };
 
@@ -30,6 +31,7 @@ struct ZkDecodeWs {                   // HBM scratch owned by a zk_ctx, grown on
     uint32_t* seq_lit_end = nullptr; uint32_t* seq_out_end = nullptr; uint32_t* seq_off = nullptr; size_t cap_seq = 0;
     uint64_t* c_off = nullptr; uint64_t* d_off = nullptr;
     uint32_t* d_need = nullptr; uint32_t* h_need = nullptr;
+    uint32_t* d_pr = nullptr; uint32_t* h_pr = nullptr;     // prefix mode: the entries' prefix ranges (ZkDecodeArgs::pranges)
     uint32_t* huf_list = nullptr; uint32_t* seq_list = nullptr; uint32_t* seg_list = nullptr;
     bool attr_set = false; uint32_t ring_override = 0;
     uint32_t exec_warps = 0;          // ZK_EXEC_WARPS: warps per K-D2 CTA (at most 16); 0 = chosen from the entries per SM
@@ -53,7 +55,8 @@ struct ZkDecodeWs {                   // HBM scratch owned by a zk_ctx, grown on
 
 // What a call asks of every batch it enqueues
 struct ZkDecodeParams {
-    const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device memory: the raw-content prefix of every zstd frame (nullptr: none)
+    const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device memory: the prefix buffer of the zstd frames (nullptr: none)
+    const uint32_t* ranges = nullptr; // host, two per entry: the prefix of entry e's frames is prefix[ranges[2e], ranges[2e + 1]); nullptr: all of it
     const uint32_t* need = nullptr;   // host, one per entry: leading bytes wanted (ZkDecodeArgs::d_need); nullptr = everything
     int share = 1;                    // how many batches share the GPU concurrently (host pipeline depth)
     bool side = true;                 // K-D1h on the side stream; host pipelines get their concurrency from the other sub-batches instead,

@@ -18,6 +18,7 @@
 // by libzstd; the compressed bytes are NOT meant to equal libzstd's.
 #include "zk_encode.h"
 #include <string.h>
+#include <map>
 #include <vector>
 
 #define ZKC_BLOCK 32768u                 // zstd block size used by this encoder (<= Block_Maximum_Size)
@@ -47,9 +48,12 @@ struct ZkcGeo {                          // per block, 24 bytes
     uint32_t frame, k;                   // frame index, block index inside the frame
     uint32_t last;                       // 1: the last block of its frame
 };
-struct ZkcFrame {                        // per frame, 24 bytes
+struct ZkcFrame {                        // per frame, 40 bytes
     size_t start;                        // first input byte
-    uint32_t size, first_block, n_blocks, pad;
+    uint32_t size, first_block, n_blocks;
+    uint32_t tail;                       // bytes of its prefix K-C1 and K-C1h stage in front of it: min(plen, ZKC_BLOCK), 0 without a prefix
+    uint32_t plo, plen;                  // its prefix: prefix[plo, plo + plen) of the batch's prefix buffer
+    unsigned long long vpre;             // the tails of the frames before it (K-C1h's virtual layout: the frame's tail starts at start + vpre)
 };
 
 struct ZkEncodeArgs {
@@ -63,13 +67,13 @@ struct ZkEncodeArgs {
     uint8_t* seqsec;                                            // ZKC_SEQSEC per block
     // K-C3 (the frame assembly).  res: the result area of the batch (ZKC_RES_HDR).  V: variants of every block (zk_encode_csize; 1
     // elsewhere): block b of the tables is variant v = min(geo[b].k, V - 1), its record at blocks[v * n_blocks + b] and its staged bytes
-    // in slot v * n_blocks + b.  wmin, wmax, whist: the window the frames announce (zkc_carve)
+    // in slot v * n_blocks + b.  wmin, wmax, far: the window the frames announce (zkc_carve)
     uint32_t* res; unsigned long long* frame_off; uint32_t* frame_hash;
-    uint8_t* dst; size_t dst_cap; uint32_t V, wmin, wmax, whist;
-    // raw-content prefix (RawEncoder::compress_with_prefix, encode.rs:311-338: re-applied at the start of EVERY frame): the last
-    // ptail <= ZKC_BLOCK bytes of it are staged in front of a copy of each frame's first block, so that block's match finder sees
-    // one contiguous history and needs no second pointer
-    const uint8_t* prefix; uint32_t prefix_len, ptail; uint8_t* pstage;
+    uint8_t* dst; size_t dst_cap; uint32_t V, wmin, wmax, far;
+    // raw-content prefix (RawEncoder::compress_with_prefix, encode.rs:311-338: re-applied at the start of EVERY frame): the buffer
+    // every frame's prefix lies in (nullptr: no frame has one).  The last tail <= ZKC_BLOCK bytes of frame f's prefix (ZkcFrame) are
+    // staged in front of a copy of its first block, so that block's match finder sees one contiguous history and needs no second pointer
+    const uint8_t* prefix; uint8_t* pstage;
     // bytes of the frame before a block that K-C1 may search, on top of the tier's own limit: unlimited (~0) except in the size variants
     // of the wide tier (zk_encode_csize), where variant d must match the block d blocks into its frame
     size_t hist_cap;
@@ -87,58 +91,75 @@ __device__ __forceinline__ ZkcGeo zkc_block_range(const ZkEncodeArgs& a, uint32_
     return g;
 }
 
+// The prefix of a frame of the batch: prefix[plo, plo + plen), of which the last min(plen, ZKC_BLOCK) bytes are staged (none when the
+// batch has no prefix: pfx == 0)
+__device__ __forceinline__ void zkc_frame_prefix(ZkcFrame& r, uint32_t pfx, uint32_t plo, uint32_t plen) {
+    r.plo = plo; r.plen = plen; r.tail = pfx ? (plen < ZKC_BLOCK ? plen : ZKC_BLOCK) : 0u;
+}
+
 // uniform layout: frames of frame_size bytes, the last one shorter (n_frames = 1 and one empty frame when n == 0).  Every frame but the
-// last is full, so frame f starts at block f * ceil(frame_size / ZKC_BLOCK).  count: the frames and the blocks they cover
-__global__ void __launch_bounds__(256) zk_geo_uniform_kernel(ZkcFrame* fr, uint32_t* count, uint32_t n_frames, size_t n, uint32_t frame_size) {
+// last is full, so frame f starts at block f * ceil(frame_size / ZKC_BLOCK).  Every frame's prefix is the whole buffer of plen bytes.
+// count: the frames and the blocks they cover
+__global__ void __launch_bounds__(256) zk_geo_uniform_kernel(ZkcFrame* fr, uint32_t* count, uint32_t n_frames, size_t n, uint32_t frame_size,
+                                                             uint32_t pfx, uint32_t plen) {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= n_frames) return;
     const uint32_t bpf = (uint32_t)(((size_t)frame_size + ZKC_BLOCK - 1) / ZKC_BLOCK);
     const size_t start = (size_t)f * frame_size;
     const uint32_t size = (uint32_t)(n - start < frame_size ? n - start : frame_size);
     ZkcFrame r;
-    r.start = start; r.size = size; r.first_block = f * bpf; r.n_blocks = size ? (size + ZKC_BLOCK - 1) / ZKC_BLOCK : 1u; r.pad = 0;
+    r.start = start; r.size = size; r.first_block = f * bpf; r.n_blocks = size ? (size + ZKC_BLOCK - 1) / ZKC_BLOCK : 1u;
+    zkc_frame_prefix(r, pfx, 0, plen);
+    r.vpre = (unsigned long long)f * r.tail;
     fr[f] = r;
     if (f + 1 == n_frames) { count[0] = n_frames; count[1] = r.first_block + r.n_blocks; }
 }
 
-// caller-chosen sizes: frame starts and first blocks by one scan (one CTA, 1024 frames a round); count as zk_geo_uniform_kernel
-__global__ void __launch_bounds__(1024) zk_geo_sized_kernel(ZkcFrame* fr, uint32_t* count, const uint32_t* sizes, uint32_t n_frames) {
-    __shared__ unsigned long long wb[32], cb;
+// caller-chosen sizes: frame starts, first blocks and the tails before each frame by one scan (one CTA, 1024 frames a round).  ranges:
+// two per frame, its prefix [ranges[2f], ranges[2f + 1]) (nullptr: the whole buffer of plen bytes).  count as zk_geo_uniform_kernel
+__global__ void __launch_bounds__(1024) zk_geo_sized_kernel(ZkcFrame* fr, uint32_t* count, const uint32_t* sizes, uint32_t n_frames,
+                                                            const uint32_t* ranges, uint32_t pfx, uint32_t plen) {
+    __shared__ unsigned long long wb[32], wt[32], cb, ct;
     __shared__ uint32_t wk[32], ck;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) { cb = 0; ck = 0; }
+    if (threadIdx.x == 0) { cb = 0; ck = 0; ct = 0; }
     __syncthreads();
     for (uint32_t base = 0; base < n_frames; base += 1024) {
         const uint32_t f = base + threadIdx.x;
         const uint32_t d = f < n_frames ? sizes[f] : 0u;
         const uint32_t nb = f < n_frames ? (d ? (d + ZKC_BLOCK - 1) / ZKC_BLOCK : 1u) : 0u;
-        unsigned long long xb = d; uint32_t xk = nb;
+        ZkcFrame r;
+        zkc_frame_prefix(r, f < n_frames ? pfx : 0u, ranges && f < n_frames ? ranges[2 * f] : 0u,
+                         ranges && f < n_frames ? ranges[2 * f + 1] - ranges[2 * f] : plen);
+        unsigned long long xb = d, xt = r.tail; uint32_t xk = nb;
 #pragma unroll
         for (int s = 1; s < 32; s <<= 1) {
-            const unsigned long long tb = __shfl_up_sync(0xFFFFFFFFu, xb, s); const uint32_t tk = __shfl_up_sync(0xFFFFFFFFu, xk, s);
-            if (lane >= s) { xb += tb; xk += tk; }
+            const unsigned long long tb = __shfl_up_sync(0xFFFFFFFFu, xb, s), tt = __shfl_up_sync(0xFFFFFFFFu, xt, s);
+            const uint32_t tk = __shfl_up_sync(0xFFFFFFFFu, xk, s);
+            if (lane >= s) { xb += tb; xk += tk; xt += tt; }
         }
-        if (lane == 31) { wb[warp] = xb; wk[warp] = xk; }
+        if (lane == 31) { wb[warp] = xb; wk[warp] = xk; wt[warp] = xt; }
         __syncthreads();
         if (warp == 0) {
-            unsigned long long yb = wb[lane]; uint32_t yk = wk[lane];
+            unsigned long long yb = wb[lane], yt = wt[lane]; uint32_t yk = wk[lane];
 #pragma unroll
             for (int s = 1; s < 32; s <<= 1) {
-                const unsigned long long tb = __shfl_up_sync(0xFFFFFFFFu, yb, s); const uint32_t tk = __shfl_up_sync(0xFFFFFFFFu, yk, s);
-                if (lane >= s) { yb += tb; yk += tk; }
+                const unsigned long long tb = __shfl_up_sync(0xFFFFFFFFu, yb, s), tt = __shfl_up_sync(0xFFFFFFFFu, yt, s);
+                const uint32_t tk = __shfl_up_sync(0xFFFFFFFFu, yk, s);
+                if (lane >= s) { yb += tb; yk += tk; yt += tt; }
             }
-            wb[lane] = yb; wk[lane] = yk;
+            wb[lane] = yb; wk[lane] = yk; wt[lane] = yt;
         }
         __syncthreads();
         if (f < n_frames) {
-            ZkcFrame r;
             r.start = cb + (warp ? wb[warp - 1] : 0ull) + xb - d; r.size = d;
-            r.first_block = ck + (warp ? wk[warp - 1] : 0u) + xk - nb; r.n_blocks = nb; r.pad = 0;
+            r.first_block = ck + (warp ? wk[warp - 1] : 0u) + xk - nb; r.n_blocks = nb;
+            r.vpre = ct + (warp ? wt[warp - 1] : 0ull) + xt - r.tail;
             fr[f] = r;
             if (f + 1 == n_frames) { count[0] = n_frames; count[1] = r.first_block + nb; }
         }
         __syncthreads();
-        if (threadIdx.x == 0) { cb += wb[31]; ck += wk[31]; }
+        if (threadIdx.x == 0) { cb += wb[31]; ck += wk[31]; ct += wt[31]; }
         __syncthreads();
     }
 }
@@ -231,16 +252,16 @@ __device__ __forceinline__ void zkc_warp_copy(uint8_t* __restrict__ d, const uin
     if ((uint32_t)lane < n - n8) d[n8 + lane] = s[n8 + lane];
 }
 
-// prefix mode: [tail of the prefix | first block of frame f] -> pstage slot f (one CTA per frame)
+// prefix mode: [tail of frame f's prefix | first block of frame f] -> pstage slot f (one CTA per frame)
 __global__ void __launch_bounds__(256) zk_prefix_stage_kernel(ZkEncodeArgs a) {
     const uint32_t f = blockIdx.x;
-    const size_t fstart = a.frames[f].start;
-    const uint32_t len = a.geo[a.frames[f].first_block].len;
+    const ZkcFrame F = a.frames[f];
+    const uint32_t len = a.geo[F.first_block].len;
     uint8_t* d = a.pstage + (size_t)f * ZKC_PSLOT;
-    const uint8_t* pt = a.prefix + (a.prefix_len - a.ptail);
-    for (uint32_t i = threadIdx.x; i < a.ptail; i += blockDim.x) d[i] = pt[i];
-    for (uint32_t i = threadIdx.x; i < len; i += blockDim.x) d[a.ptail + i] = a.src[fstart + i];
-    for (uint32_t i = threadIdx.x; i < 64; i += blockDim.x) d[a.ptail + len + i] = 0;
+    const uint8_t* pt = a.prefix + (F.plo + F.plen - F.tail);
+    for (uint32_t i = threadIdx.x; i < F.tail; i += blockDim.x) d[i] = pt[i];
+    for (uint32_t i = threadIdx.x; i < len; i += blockDim.x) d[F.tail + i] = a.src[F.start + i];
+    for (uint32_t i = threadIdx.x; i < 64; i += blockDim.x) d[F.tail + len + i] = 0;
 }
 
 // inserts the history sb[0, lo32) into the table, and into the 8-byte table when DFAST, so that matches can reach into it.  Several
@@ -273,12 +294,13 @@ __device__ __forceinline__ void zkc_match_block(const ZkEncodeArgs& a, uint32_t 
     size_t lo, hi, fstart;
     const ZkcGeo g = zkc_block_range(a, b, lo, hi, fstart);
     // history: up to HIST_BYTES of the same frame before `lo` are searchable, capped by a.hist_cap; the first block of a frame
-    // searches the tail of the prefix instead, through its staged copy
-    const bool pfx = a.ptail != 0 && lo == fstart;
+    // searches the tail of its prefix instead, through its staged copy
+    const uint32_t ptail = a.prefix && lo == fstart ? a.frames[g.frame].tail : 0u;
+    const bool pfx = ptail != 0;
     const size_t hist = a.hist_cap < HIST_BYTES ? a.hist_cap : HIST_BYTES;
     const size_t base = lo - fstart >= hist ? lo - hist : fstart;
     const uint8_t* sb = pfx ? a.pstage + (size_t)g.frame * ZKC_PSLOT : a.src + base;
-    const uint32_t lo32 = pfx ? a.ptail : (uint32_t)(lo - base), hi32 = lo32 + (uint32_t)(hi - lo);
+    const uint32_t lo32 = pfx ? ptail : (uint32_t)(lo - base), hi32 = lo32 + (uint32_t)(hi - lo);
     for (int i = lane; i < ((DFAST ? 2 : 1) << HLOG); i += 32) table[i] = 0;
     __syncwarp();
     const uint32_t len = hi32 - lo32;
@@ -459,11 +481,12 @@ __global__ void __launch_bounds__(NW * 32) zk_match_fast_kernel(ZkEncodeArgs a) 
     uint16_t* table = tables[warp];
     size_t lo, hi, fstart;
     const ZkcGeo g = zkc_block_range(a, b, lo, hi, fstart);
-    const bool pfx = a.ptail != 0 && lo == fstart;
+    const uint32_t ptail = a.prefix && lo == fstart ? a.frames[g.frame].tail : 0u;
+    const bool pfx = ptail != 0;
     const size_t hist = a.hist_cap < ZKC_BLOCK ? a.hist_cap : ZKC_BLOCK;
     const size_t base = lo - fstart >= hist ? lo - hist : fstart;
     const uint8_t* sb = pfx ? a.pstage + (size_t)g.frame * ZKC_PSLOT : a.src + base;
-    const uint32_t lo32 = pfx ? a.ptail : (uint32_t)(lo - base), hi32 = lo32 + (uint32_t)(hi - lo);
+    const uint32_t lo32 = pfx ? ptail : (uint32_t)(lo - base), hi32 = lo32 + (uint32_t)(hi - lo);
     for (int i = lane; i < (1 << HLOG); i += 32) table[i] = 0;
     __syncwarp();
     uint16_t* o_ll = a.seq_ll + (size_t)b * ZKC_MAXSEQ; uint16_t* o_ml = a.seq_ml + (size_t)b * ZKC_MAXSEQ;
@@ -1424,11 +1447,14 @@ __global__ void __launch_bounds__(128) zk_frame_gather_kernel(ZkEncodeArgs a) {
     const ZkcBlock bl = a.blocks[slot];
     uint8_t* fo = a.dst + a.frame_off[f];
     if (g.k == 0 && lane == 0) {
-        const uint32_t fcs = a.frames[f].size;
-        // the smallest Window_Size = 2^(10 + e) * (1 + m / 8) >= max(wmin, min(fcs + whist, wmax)); an empty frame holds no match, so
-        // it takes the minimum whatever the prefix
-        const size_t reach = fcs ? a.whist : 0;
-        size_t want = fcs + reach < a.wmax ? fcs + reach : a.wmax;
+        const ZkcFrame F = a.frames[f];
+        const uint32_t fcs = F.size;
+        // the smallest Window_Size = 2^(10 + e) * (1 + m / 8) >= max(wmin, min(fcs + reach, wmax)), where reach is the prefix bytes the
+        // frame's offsets may reach: its tail, or all of its prefix up to 2^27 back (a.far == 2, or 1 and a prefix); an empty frame holds
+        // no match, so it takes the minimum whatever the prefix
+        const bool far = a.far == 2 || (a.far == 1 && F.plen);
+        const size_t reach = fcs ? (far ? F.plen : F.tail) : 0, wmax = far ? 1u << 27 : a.wmax;
+        size_t want = fcs + reach < wmax ? fcs + reach : wmax;
         if (want < a.wmin) want = a.wmin;
         uint32_t e = 0, m = 0;
         while (((size_t)8 + m) << (7 + e) < want) { if (++m == 8) { m = 0; e++; } }
@@ -1484,6 +1510,7 @@ struct ZkCsizeArgs {
     uint32_t* starts;                                // nb + 1: first blocks of the frames the walk closes, then the end of the last
     ZkcFrame* frames;                                // their frame table
     uint32_t* res;                                   // the result area of the chosen frames (ZKC_RES_HDR)
+    uint32_t pfx, plen;                              // every frame's prefix: the whole buffer of plen bytes (pfx == 0: none)
 };
 
 // prefix sum of variant V-1's block sizes (one CTA)
@@ -1539,7 +1566,9 @@ __global__ void __launch_bounds__(256) zk_geo_starts_kernel(ZkCsizeArgs c) {
     const uint32_t s = c.starts[f], e = c.starts[f + 1];
     const size_t hi = (size_t)e * ZKC_BLOCK < c.n ? (size_t)e * ZKC_BLOCK : c.n;
     ZkcFrame r;
-    r.start = (size_t)s * ZKC_BLOCK; r.size = (uint32_t)(hi - r.start); r.first_block = s; r.n_blocks = e - s; r.pad = 0;
+    r.start = (size_t)s * ZKC_BLOCK; r.size = (uint32_t)(hi - r.start); r.first_block = s; r.n_blocks = e - s;
+    zkc_frame_prefix(r, c.pfx, 0, c.plen);
+    r.vpre = (unsigned long long)f * r.tail;
     c.frames[f] = r; c.res[ZKC_RES_HDR + c.nb + f] = r.size;
 }
 
@@ -1584,14 +1613,17 @@ struct ZkcHcRun;
 static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, const ZkEncodeArgs& a, const ZkcHcRun* hc);
 
 // the frame and block tables of a batch and their counts, on `stream`: the uniform layout is generated on the device, the caller's sizes
-// are uploaded to d_sizes and scanned there
+// are uploaded to d_sizes (and, with per-frame prefixes, the ranges behind them, two words per frame) and scanned there.  pfx: the batch
+// has a prefix, the buffer of plen bytes that every frame's prefix lies in (ranges == nullptr: all of it)
 static int zkc_build_geometry(ZkEncodeWs* ws, cudaStream_t stream, ZkcGeo* geo, ZkcFrame* fr, uint32_t* count, const ZkFrames& frames,
-                              uint32_t n_blocks, uint32_t* d_sizes) {
+                              uint32_t n_blocks, uint32_t* d_sizes, uint32_t pfx, uint32_t plen, const uint32_t* ranges) {
     const uint32_t n_frames = frames.count;
     if (frames.sizes) {
         ZK_CUDA_OK(cudaMemcpyAsync(d_sizes, frames.sizes, (size_t)n_frames * 4, cudaMemcpyHostToDevice, stream));
-        ZK_LAUNCH(zk_geo_sized_kernel, 1, 1024, 0, stream, fr, count, (const uint32_t*)d_sizes, n_frames);
-    } else ZK_LAUNCH(zk_geo_uniform_kernel, (n_frames + 255) / 256, 256, 0, stream, fr, count, n_frames, frames.n, frames.frame_size);
+        uint32_t* d_ranges = ranges ? d_sizes + n_frames : nullptr;
+        if (ranges) ZK_CUDA_OK(cudaMemcpyAsync(d_ranges, ranges, (size_t)n_frames * 8, cudaMemcpyHostToDevice, stream));
+        ZK_LAUNCH(zk_geo_sized_kernel, 1, 1024, 0, stream, fr, count, (const uint32_t*)d_sizes, n_frames, (const uint32_t*)d_ranges, pfx, plen);
+    } else ZK_LAUNCH(zk_geo_uniform_kernel, (n_frames + 255) / 256, 256, 0, stream, fr, count, n_frames, frames.n, frames.frame_size, pfx, plen);
     ZK_LAUNCH(zk_geo_block_kernel, (n_blocks + 255) / 256, 256, 0, stream, geo, (const ZkcFrame*)fr, (const uint32_t*)count);
     ws->launches += 2;
     return 0;
@@ -1615,10 +1647,11 @@ static int zkc_side_stream(ZkEncodeWs* ws, cudaStream_t stream, bool side, cudaS
 #include "zk_cdc.inc"
 
 // The workspace of a batch of n_frames frames over n_blocks blocks, with V variants of every block's record and staged bytes (1 except in
-// zk_encode_csize) and, with a prefix tail of pt bytes, the frames' prefix staging slots: a's scratch pointers into it from `base`
+// zk_encode_csize) and, when the frames have prefixes (pfx), their prefix staging slots: a's scratch pointers into it from `base`
 // (nullptr: only counts its bytes; the caller's own regions follow), and the fields every batch of tier `lvl` sets alike.  far: the tier
-// matches up to 2^27 bytes back (long-distance matching, long mode).  Returns the bytes it takes.
-static size_t zkc_carve(ZkEncodeArgs& a, uint8_t* base, uint32_t n_frames, size_t n_blocks, uint32_t V, int lvl, bool far, uint32_t pt,
+// matches up to 2^27 bytes back, 1 into the prefix of a frame that has one (long-distance matching), 2 also within every frame (long
+// mode).  Returns the bytes it takes.
+static size_t zkc_carve(ZkEncodeArgs& a, uint8_t* base, uint32_t n_frames, size_t n_blocks, uint32_t V, int lvl, uint32_t far, bool pfx,
                         const ZkEncodeParams& p) {
     size_t off = 0;
     auto at = [&](size_t bytes) { const size_t o = off; off = zkc_align(off + bytes); return (uint8_t*)((uintptr_t)base + o); };
@@ -1630,17 +1663,16 @@ static size_t zkc_carve(ZkEncodeArgs& a, uint8_t* base, uint32_t n_frames, size_
     a.lits = at(n_blocks * ZKC_BLOCK); a.stage = at(V * n_blocks * ZKC_SLOT + 64); a.seqsec = at(n_blocks * ZKC_SEQSEC);
     a.res = (uint32_t*)at((ZKC_RES_HDR + 2 * (size_t)n_frames) * 4);
     a.frame_off = (unsigned long long*)at((size_t)n_frames * 8); a.frame_hash = (uint32_t*)at((size_t)n_frames * 4);
-    a.pstage = at(pt ? (size_t)n_frames * ZKC_PSLOT : 0);
+    a.pstage = at(pfx ? (size_t)n_frames * ZKC_PSLOT : 0);
     a.level = lvl; a.checksum = p.checksum ? 1 : 0;
-    a.prefix = p.prefix; a.prefix_len = pt ? p.prefix_len : 0; a.ptail = pt;
+    a.prefix = pfx ? p.prefix : nullptr;
     a.hist_cap = ~(size_t)0; a.hc = nullptr;
     // the window every frame announces (zk_frame_gather_kernel): 128 KiB below the wide tier, whose offsets stay below 64 KiB; the wide
     // tier's offsets reach (ZKC_WIDE_HIST + 1) blocks back, the high-level tier's ZKC_HC_WINDOW bytes within the frame and its prefix tail.
-    // Up to 2^27 bytes back, the largest window a default libzstd decoder and this one accept (zkc_ldm_window keeps every offset within
-    // it), all of the prefix is in reach
-    a.wmin = a.wmax = 128u << 10; a.whist = pt;
-    if (far) { a.wmax = 1u << 27; a.whist = a.prefix_len; }
-    else if (lvl >= ZKC_HC_LEVEL) a.wmax = ZKC_HC_WINDOW;
+    // Up to 2^27 bytes back (far), the largest window a default libzstd decoder and this one accept (zkc_ldm_window keeps every offset
+    // within it), all of the frame's prefix is in reach
+    a.wmin = a.wmax = 128u << 10; a.far = far;
+    if (lvl >= ZKC_HC_LEVEL) a.wmax = ZKC_HC_WINDOW;
     else if (lvl >= ZKC_WIDE_LEVEL) a.wmin = a.wmax = 256u << 10;
     return off;
 }
@@ -1661,35 +1693,66 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
         n_blocks = (size_t)(n_frames - 1) * zkc_frame_blocks(fr.frame_size) + zkc_frame_blocks(n - (size_t)(n_frames - 1) * fr.frame_size);
     }
     if (n_blocks > 0x7FFFFFFFull) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
-    const uint32_t pt = p.prefix && p.prefix_len && n ? (p.prefix_len < ZKC_BLOCK ? p.prefix_len : ZKC_BLOCK) : 0u;
+    if (p.ranges && !fr.sizes) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
+    // the frames have prefixes: each one's range of the buffer (zk_geo_sized_kernel), its last ZKC_BLOCK bytes staged in front of it
+    const bool pfx = p.prefix && p.prefix_len && n;
     // long-distance matching is a part of K-C1h: with it every level runs that tier.  Long mode indexes the input too (positions are u32)
     // and matches the prefix as the long-distance switch does
     if (p.long_mode && n > 0xFFFFFFFFull) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
-    const bool ldm = (p.ldm || p.long_mode) && pt, lin = p.long_mode && n;
+    const bool ldm = (p.ldm || p.long_mode) && pfx, lin = p.long_mode && n;
     const int lvl = ldm || p.long_mode ? ZKC_HC_LEVEL : zkc_level(p.level);
+    const uint32_t far = p.long_mode ? 2u : (ldm ? 1u : 0u);
     ZkcHcRun hc;
-    const uint32_t hc_span = lvl >= ZKC_HC_LEVEL ? zkc_hc_plan(fr, (uint32_t)n_blocks, pt, hc.plan) : 0u;
-    if (ldm) hc.reach = p.prefix_len < ZKC_LDM_REACH ? p.prefix_len : ZKC_LDM_REACH;
+    uint32_t hc_span = 0;
+    if (lvl >= ZKC_HC_LEVEL) {
+        // K-C1h's passes follow the frames' tails; with long-distance matching, every distinct range is indexed once, as a region of
+        // its own: its last min(length, ZKC_LDM_REACH) bytes, at virtual positions after those of the regions before it
+        std::vector<uint32_t> tails(pfx ? n_frames : 0);
+        if (ldm) hc.fregion.assign(n_frames, ZKC_LDM_NOREGION);
+        std::map<unsigned long long, uint32_t> seen;
+        unsigned long long vtotal = 0;
+        for (uint32_t f = 0; pfx && f < n_frames; f++) {
+            const uint32_t lo = p.ranges ? p.ranges[2 * f] : 0u, hi = p.ranges ? p.ranges[2 * f + 1] : p.prefix_len;
+            tails[f] = hi - lo < ZKC_BLOCK ? hi - lo : ZKC_BLOCK;
+            if (!ldm || hi == lo) continue;
+            const unsigned long long key = (unsigned long long)lo << 32 | hi;
+            auto it = seen.find(key);
+            if (it == seen.end()) {
+                ZkcLdmRegion r;
+                r.reach = hi - lo < ZKC_LDM_REACH ? hi - lo : ZKC_LDM_REACH; r.pbase = hi - r.reach;
+                r.vbase = (uint32_t)vtotal; r.run0 = hc.runs;
+                vtotal += r.reach; hc.runs += zkc_ldm_runs(r.reach);
+                if (vtotal > 0xFFFFFFFFull) return -(int)ZKZ_PARAM_OUT_OF_BOUND;
+                it = seen.emplace(key, (uint32_t)hc.regions.size()).first;
+                hc.regions.push_back(r);
+            }
+            hc.fregion[f] = it->second;
+        }
+        hc_span = zkc_hc_plan(fr, (uint32_t)n_blocks, pfx ? tails.data() : nullptr, hc.plan);
+    }
     hc.input = lin;
+    const uint32_t n_regions = (uint32_t)hc.regions.size();
     ZkEncodeArgs a;
-    size_t off = zkc_carve(a, nullptr, n_frames, n_blocks, 1, lvl, ldm || p.long_mode, pt, p);
-    const size_t o_fsz = off; if (fr.sizes) off = zkc_align(off + (size_t)n_frames * 4);
+    size_t off = zkc_carve(a, nullptr, n_frames, n_blocks, 1, lvl, far, pfx, p);
+    const size_t o_fsz = off; if (fr.sizes) off = zkc_align(off + (size_t)n_frames * (p.ranges ? 12 : 4));
     const size_t o_hc = off;
     if (lvl >= ZKC_HC_LEVEL) off = zkc_align(off + zkc_hc_layout(hc_span, nullptr, nullptr));
     const size_t o_ldm = off;
-    if (ldm || lin) off = zkc_align(off + zkc_ldm_layout(hc.reach, lin ? (uint32_t)n_blocks * ZKC_LDM_BSLOTS : 0u, n_blocks, nullptr, nullptr, nullptr, nullptr));
+    const uint32_t in_slots = lin ? (uint32_t)n_blocks * ZKC_LDM_BSLOTS : 0u;
+    if (ldm || lin) off = zkc_align(off + zkc_ldm_layout(hc.runs * ZKC_LDM_PER_RUN, n_regions, n_frames, in_slots, n_blocks, nullptr, nullptr, nullptr, nullptr));
     int rc = zk_grow(&ws->buf, &ws->cap, off, 1);
     if (!rc) rc = zk_grow((void**)&ws->h_sizes, &ws->cap_frames, ZKC_RES_HDR + (size_t)n_frames, 4, true);
     if (rc) return rc;
     uint8_t* base = (uint8_t*)ws->buf;
-    zkc_carve(a, base, n_frames, n_blocks, 1, lvl, ldm || p.long_mode, pt, p);
+    zkc_carve(a, base, n_frames, n_blocks, 1, lvl, far, pfx, p);
     a.src = d_src; a.n = n; a.dst = d_dst; a.dst_cap = dst_cap;
     a.hc = base + o_hc;
     if (ldm || lin) hc.ldm = base + o_ldm;
     ZK_CUDA_OK(cudaMemsetAsync(a.res, 0, ZKC_RES_HDR * 4, stream));
-    rc = zkc_build_geometry(ws, stream, (ZkcGeo*)a.geo, (ZkcFrame*)a.frames, a.res, fr, (uint32_t)n_blocks, (uint32_t*)(base + o_fsz));
+    rc = zkc_build_geometry(ws, stream, (ZkcGeo*)a.geo, (ZkcFrame*)a.frames, a.res, fr, (uint32_t)n_blocks, (uint32_t*)(base + o_fsz), pfx,
+                            p.prefix_len, p.ranges);
     if (rc) return rc;
-    if (pt) {
+    if (pfx) {
         ZK_LAUNCH(zk_prefix_stage_kernel, n_frames, 256, 0, stream, a);
         ws->launches += 1;
     }
@@ -1781,11 +1844,11 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     const int lvl = zkc_level(p.level) >= ZKC_HC_LEVEL ? ZKC_WIDE_LEVEL : zkc_level(p.level);
     const uint32_t nb = (uint32_t)((n + ZKC_BLOCK - 1) / ZKC_BLOCK);
     const uint32_t V = lvl >= ZKC_WIDE_LEVEL ? ZKC_WIDE_HIST + 1 : 2;
-    const uint32_t pt = p.prefix && p.prefix_len ? (p.prefix_len < ZKC_BLOCK ? p.prefix_len : ZKC_BLOCK) : 0u;
+    const bool pfx = p.prefix && p.prefix_len;
     // the batch of the chosen frames (nb at most; the cut writes their tables and result area), the cut's arrays, and the two layouts
     // of the variants with their counts: frames of one block (d = 0), one frame over the pass (d >= 1)
     ZkEncodeArgs a;
-    size_t off = zkc_carve(a, nullptr, nb, nb, V, lvl, false, pt, p);
+    size_t off = zkc_carve(a, nullptr, nb, nb, V, lvl, 0, pfx, p);
     const size_t o_psum = off; off = zkc_align(off + ((size_t)nb + 1) * 8);
     const size_t o_next = off; off = zkc_align(off + (size_t)nb * 4);
     const size_t o_starts = off; off = zkc_align(off + ((size_t)nb + 1) * 4);
@@ -1798,19 +1861,22 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     if (!rc) rc = zk_grow((void**)&ws->h_sizes, &ws->cap_frames, ZKC_RES_HDR + 2 * (size_t)nb, 4, true);
     if (rc) return rc;
     uint8_t* base = (uint8_t*)ws->buf;
-    zkc_carve(a, base, nb, nb, V, lvl, false, pt, p);
+    zkc_carve(a, base, nb, nb, V, lvl, 0, pfx, p);
     a.src = d_src; a.n = n; a.dst = d_dst; a.dst_cap = dst_cap;
     ZkCsizeArgs c;
     c.n = n; c.nb = nb; c.V = V; c.target = target ? target : 1;
     c.end_closes = at_end && final_; c.end_lazy = at_end && !final_;
     c.vblocks = a.blocks; c.psum = (unsigned long long*)(base + o_psum); c.next = (uint32_t*)(base + o_next);
     c.starts = (uint32_t*)(base + o_starts); c.frames = (ZkcFrame*)a.frames; c.res = a.res;
+    c.pfx = pfx; c.plen = p.prefix_len;
     ZK_CUDA_OK(cudaMemsetAsync(a.res, 0, ZKC_RES_HDR * 4, stream));
     cudaStream_t ss;
     if ((rc = zkc_side_stream(ws, stream, p.side, &ss))) return rc;
     uint32_t* vcount = (uint32_t*)(base + o_cnt);
-    rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo0), (ZkcFrame*)(base + o_fr0), vcount, {nullptr, n, ZKC_BLOCK, nb}, nb, nullptr);
-    if (!rc) rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo1), (ZkcFrame*)(base + o_fr1), vcount + 2, {nullptr, n, (uint32_t)n, 1}, nb, nullptr);
+    rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo0), (ZkcFrame*)(base + o_fr0), vcount, {nullptr, n, ZKC_BLOCK, nb}, nb, nullptr, pfx,
+                            p.prefix_len, nullptr);
+    if (!rc) rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo1), (ZkcFrame*)(base + o_fr1), vcount + 2, {nullptr, n, (uint32_t)n, 1}, nb,
+                                     nullptr, 0, 0, nullptr);
     if (rc) return rc;
     // variant passes.  d = 0: frames of one block, so every block opens its frame (prefix staging included); d >= 1: one frame
     // over the pass, with the wide tier's history capped at d blocks below V - 1
@@ -1820,8 +1886,8 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
         v.n_frames = d == 0 ? nb : 1;
         v.hist_cap = d >= 1 && d + 1 < V ? (size_t)d * ZKC_BLOCK : ~(size_t)0;
         v.blocks = a.blocks + (size_t)d * nb; v.stage = a.stage + (size_t)d * nb * ZKC_SLOT;
-        if (d >= 1) v.prefix_len = v.ptail = 0;
-        else if (pt) {
+        if (d >= 1) v.prefix = nullptr;
+        else if (pfx) {
             ZK_LAUNCH(zk_prefix_stage_kernel, nb, 256, 0, stream, v);
             ws->launches += 1;
         }

@@ -18,8 +18,10 @@ struct ZkEncodeWs {                    // HBM scratch owned by a zk_ctx slot, gr
 // What a call asks of every batch it enqueues
 struct ZkEncodeParams {
     int level = 0, checksum = 0;
-    const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device memory: the raw-content prefix of every frame (nullptr: none)
-    bool ldm = false;                 // long-distance matching against the whole prefix (nothing without one)
+    const uint8_t* prefix = nullptr; uint32_t prefix_len = 0;   // device memory: the prefix buffer the frames' prefixes lie in (nullptr: none)
+    const uint32_t* ranges = nullptr; // host, two per frame of the batch: frame f's prefix is prefix[ranges[2f], ranges[2f + 1]); nullptr: the
+                                      // whole buffer for every frame
+    bool ldm = false;                 // long-distance matching against the whole of each frame's prefix (nothing without one)
     bool long_mode = false;           // long mode: every frame also matches its own bytes up to 2^27 back (and the prefix as ldm does)
     bool side = true;                 // K-C2s and the checksum on the side stream; host pipelines get their concurrency from the other
                                       // sub-batches instead, and every extra stream costs a hardware queue
