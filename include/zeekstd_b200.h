@@ -277,6 +277,44 @@ int32_t zk_decompress_frames_prefixes(zk_ctx* ctx, const uint8_t* comp, const ui
                                       uint8_t* dst, const uint32_t* d_need, int32_t verify_checksum, int32_t* status,
                                       const uint8_t* prefix, size_t prefix_len, const uint64_t* ranges);
 
+/*
+ * The content-defined cut alone (FrameSizePolicy::ContentDefined(size), the rule of zk_compress_frames_cdc): frame_sizes, *n_frames and
+ * *consumed are exactly the d_sizes, frame count and consumed of zk_compress_frames_cdc on the same src, n, size and final, at any level;
+ * nothing is compressed.  frames_cap >= n / 1024 + 1 always suffices; less than a call needs returns -70 (dstSize_tooSmall).  HOST pointers.
+ */
+int32_t zk_cut_frames_cdc(zk_ctx* ctx, const uint8_t* src, size_t n, uint32_t size, int32_t final, uint32_t* frame_sizes,
+                          uint32_t frames_cap, uint32_t* n_frames, size_t* consumed);
+
+/*
+ * Compress a new version against the archive of the previous one: every frame whose bytes an old entry already holds is copied from the
+ * old archive, only the others are compressed.  src and frame_sizes as in zk_compress_frames_sized; long_mode != 0 compresses as
+ * zk_compress_frames_sized_long (frames are independent there too).  The old archive: old_comp (old_len bytes) with old_n entries, entry g at
+ * old_comp[old_c_off[g] .. old_c_off[g+1]) decoding to old_d_off[g+1] - old_d_off[g] bytes (the offsets of zk_decompress_frames, HOST
+ * arrays of old_n + 1 entries).  Writes the frames back to back into dst, c_sizes[f], and reused[f]: the old entry frame f copies, or
+ * 0xFFFFFFFF.  The rule for frame f:
+ *   1. Old entry g is a candidate when its decompressed size equals frame_sizes[f], it decodes without error (checksum verified), the
+ *      Content_Checksum_flag of its first zstd frame equals checksum != 0, and key(g) == key(f).  key(x) is XXH64 (seed 0) of the
+ *      little-endian 8-byte XXH64s of x's consecutive 32 KiB chunks (the last one may be shorter; no bytes: the XXH64 of nothing).
+ *   2. Frame f copies the lowest-index candidate verbatim iff its decoded bytes equal frame f's bytes, compared byte by byte: equality is
+ *      proven, never assumed from the key.  With no candidate, or when the bytes differ, frame f is what zk_compress_frames_sized (or
+ *      _sized_long) writes for it; no further candidate is tried.
+ * So the result always restores src, and it equals zk_compress_frames_sized[_long] on the same arguments byte for byte whenever the
+ * entries it copies were written by this codec at the same level, checksum flag and mode.  Entries written otherwise (another level,
+ * libzstd) still decode to the frame's bytes and are copied as they are.  An old entry that fails to decode is not a candidate, never an
+ * error of the call.  There is no prefix, no long-distance switch and no Compressed(n) variant: a copied frame's bytes must depend on its
+ * own bytes alone.  ZK_REUSE_KEY_BITS (environment, tests; default 64) keeps only that many low bits of every key.
+ * Old offsets that decrease, or an old_c_off[old_n] above old_len, return ZK_ERR_INVALID_ARG; other argument errors are those of
+ * zk_compress_frames_sized.  dst_cap >= zk_compress_bound_sized(frame_sizes, n_frames) + old_c_off[old_n] - old_c_off[0] suffices when
+ * every old entry is at most zk_compress_bound_sized of its own decompressed size (as this codec's entries are) or is copied at most once;
+ * a dst_cap below what the frames need returns -70 (dstSize_tooSmall).  c_sizes and reused may be NULL.  Runs unpipelined; the old
+ * entries of a matching size are decoded twice (once to index them, once to compare them), so device memory stays bounded by the
+ * sub-batch, never by the old archive.  HOST pointers.
+ */
+int32_t zk_compress_frames_sized_reuse(zk_ctx* ctx, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                       int32_t checksum, int32_t long_mode, const uint8_t* old_comp, size_t old_len,
+                                       const uint64_t* old_c_off, const uint64_t* old_d_off, uint32_t old_n, uint8_t* dst, size_t dst_cap,
+                                       uint32_t* c_sizes, uint32_t* reused, size_t* dst_len);
+
 /* ------------------------------------------------------------------ SeekTable (lib/src/seek_table.rs) */
 typedef struct zk_seek_table zk_seek_table;
 typedef enum { ZK_FORMAT_HEAD = 0, ZK_FORMAT_FOOT = 1 } zk_format; /* seek_table.rs:228-241 */

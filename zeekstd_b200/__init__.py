@@ -224,6 +224,40 @@ class Context:
                                           byref(used)), lib)
         return dst[: dl.value], cs[: nf.value].copy(), ds[: nf.value].copy(), int(used.value)
 
+    def cut_frames_cdc(self, data, size: int, final: bool = True):
+        """the frame sizes of FrameSizePolicy::ContentDefined(size) without compressing -> (d_sizes (np.uint32), consumed): exactly what
+        compress_frames_cdc returns for the same data, size and final (zk_cut_frames_cdc)."""
+        addr, n, keep = _buf(data)
+        nfmax = n // 1024 + 1
+        ds = np.zeros(nfmax, dtype=np.uint32)
+        nf = c_uint32(); used = c_size_t()
+        _check(self.lib.zk_cut_frames_cdc(self._h, addr, n, size, int(final), ds.ctypes.data_as(_native.u32p), nfmax, byref(nf), byref(used)),
+               self.lib)
+        return ds[: nf.value].copy(), int(used.value)
+
+    def compress_frames_reuse(self, data, frame_sizes, old, level: int = 0, checksum: bool = False, long_mode: bool = False):
+        """compress_frames_sized(data, frame_sizes, level, checksum, long_mode=long_mode), copying every frame whose bytes an entry of the
+        old seekable archive `old` (bytes ending in its Foot seek table) already holds -> (compressed bytes (np.uint8), c_sizes, reused):
+        reused[f] is the old entry frame f copies, or 0xFFFFFFFF.  The rule (include/zeekstd_b200.h, zk_compress_frames_sized_reuse): the
+        lowest-index old entry of frame f's size, checksum flag and key is copied verbatim iff its decoded bytes equal the frame's."""
+        addr, n, keep = _buf(data)
+        ds = np.ascontiguousarray(frame_sizes, dtype=np.uint32).reshape(-1)
+        if int(np.sum(ds, dtype=np.uint64)) != n:
+            raise ValueError(f"frame sizes add up to {int(np.sum(ds, dtype=np.uint64))} bytes, the input has {n}")
+        oaddr, on, okeep = _buf(old)
+        co, do = SeekTable.from_bytes(old, Format.Foot, self.lib).offsets()
+        lib = self.lib
+        dsp = ds.ctypes.data_as(_native.u32p)
+        cap = lib.zk_compress_bound_sized(dsp, ds.size) + int(co[-1] - co[0])
+        dst = np.empty(cap + 64, dtype=np.uint8)
+        cs = np.zeros(ds.size, dtype=np.uint32); ru = np.zeros(ds.size, dtype=np.uint32)
+        dl = c_size_t()
+        _check(lib.zk_compress_frames_sized_reuse(self._h, addr, dsp, ds.size, level, int(checksum), int(long_mode), oaddr, on,
+                                                  co.ctypes.data_as(_native.u64p), do.ctypes.data_as(_native.u64p), len(co) - 1,
+                                                  dst.ctypes.data, cap, cs.ctypes.data_as(_native.u32p), ru.ctypes.data_as(_native.u32p),
+                                                  byref(dl)), lib)
+        return dst[: dl.value], cs, ru
+
     def decompress_frames(self, comp, c_off, d_off, verify_checksum: bool = True, out: np.ndarray | None = None, need=None, prefix=None,
                           prefix_ranges=None):
         """decode frames given N+1 cumulative offsets -> (np.uint8 output, per-frame status, rc).

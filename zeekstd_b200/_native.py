@@ -91,6 +91,9 @@ _SIGS = {
                                                     c_int32, c_int32, c_void_p, c_size_t, u32p, POINTER(c_size_t)]),
     "zk_decompress_frames_prefixes": (c_int32, [c_void_p, c_void_p, u64p, u64p, c_uint32, c_void_p, u32p, c_int32, i32p, c_void_p,
                                                 c_size_t, u64p]),
+    "zk_cut_frames_cdc": (c_int32, [c_void_p, c_void_p, c_size_t, c_uint32, c_int32, u32p, c_uint32, u32p, POINTER(c_size_t)]),
+    "zk_compress_frames_sized_reuse": (c_int32, [c_void_p, c_void_p, u32p, c_uint32, c_int32, c_int32, c_int32, c_void_p, c_size_t, u64p,
+                                                 u64p, c_uint32, c_void_p, c_size_t, u32p, u32p, POINTER(c_size_t)]),
     # seek table
     "zk_seek_table_new": (c_void_p, []),
     "zk_seek_table_free": (None, [c_void_p]),

@@ -1,6 +1,7 @@
 """Command-line front end with the reference CLI's arguments and behaviour (SURVEY.md 8f.4), over the GPU codec.
 
-    python -m zeekstd_b200 [compress] [-l N] [-s 2M] [--frame-size-policy ..] [--patch-from F [--long]] [--long-mode] [INPUT] [-o OUT]
+    python -m zeekstd_b200 [compress] [-l N] [-s 2M] [--frame-size-policy ..] [--patch-from F [--long]] [--long-mode] [--reuse-from OLD.zst]
+                           [INPUT] [-o OUT]
     python -m zeekstd_b200 decompress [--from N | --from-frame I] [--to N|end | --to-frame I|end] [--patch-apply F] INPUT [-o OUT]
     python -m zeekstd_b200 list [--from-frame I] [--to-frame I|end | --num-frames N] [-d] [--seek-table-format head|foot] INPUT
 
@@ -20,6 +21,8 @@ window; with `--patch-from` it also matches the whole of F as `--long` does.  It
 `--frame-size-policy uncompressed`.  `--mmap-prefix` / `--no-mmap-prefix` choose between np.memmap and a read.  `--frame-size-policy content` (an
 extension of this codec) ends frames where a rolling hash of the data says so, about `-s` bytes apart on average, so that an edit
 of the input changes only the frames around it and rsync, dedup stores and range-fetching clients can reuse the rest.
+`--reuse-from OLD.zst` (an extension of this codec) compresses a new version against the archive of the previous one: every frame
+whose bytes a frame of OLD.zst holds is copied from it, only the others are compressed; with `uncompressed` or `content` frames.
 """
 from __future__ import annotations
 
@@ -157,6 +160,10 @@ def build_parser() -> argparse.ArgumentParser:
                    help="Match every frame also against its own bytes up to 128 MiB back (zstd --long), and with --patch-from against the "
                         "whole reference file as --long does: large frames find far repeats. Every compression level then runs as level 16; "
                         "needs --frame-size-policy uncompressed.")
+    c.add_argument("--reuse-from", default=None, metavar="OLD.zst",
+                   help="The archive of a previous version of the input (ending in its seek table): every frame whose bytes one of its "
+                        "frames already holds is copied from it, only the others are compressed. The output is what compress writes "
+                        "when OLD.zst was written with the same settings. Needs --frame-size-policy uncompressed or content.")
     c.add_argument("input_file", nargs="?", default="-")
     c.add_argument("-o", "--output-file", default=None)
 
@@ -331,6 +338,13 @@ def _run_compress(zk, ns, fmt_bytes) -> int:
         raise CliError("--long needs --frame-size-policy uncompressed")
     if ns.long_mode and ns.frame_size_policy in ("compressed", "content"):
         raise CliError("--long-mode needs --frame-size-policy uncompressed")
+    if ns.reuse_from is not None:
+        if ns.patch_from:
+            raise CliError("--reuse-from cannot be used with --patch-from: a copied frame must depend on its own bytes alone")
+        if ns.frame_size_policy == "compressed":
+            raise CliError("--reuse-from needs --frame-size-policy uncompressed or content")
+        if ns.frame_size == 0:
+            raise CliError("--reuse-from needs a frame size above 0")
     prefix_len = os.path.getsize(ns.patch_from) if ns.patch_from and os.path.exists(ns.patch_from) else None
     st_file = None
     if ns.seek_table_file is not None:
@@ -342,6 +356,8 @@ def _run_compress(zk, ns, fmt_bytes) -> int:
     bar = _Progress(in_len, fmt_bytes, not ns.quiet and not ns.no_progress)
     writer = _new_writer(out_path, in_path, ns.quiet, ns.force)
 
+    if ns.reuse_from is not None:
+        return _run_compress_reuse(zk, ns, fmt_bytes, reader, writer, in_path, out_path, st_file)
     policy = {"compressed": zk.FrameSizePolicy.Compressed, "uncompressed": zk.FrameSizePolicy.Uncompressed,
               "content": zk.FrameSizePolicy.ContentDefined}[ns.frame_size_policy](ns.frame_size)
     enc = (zk.EncodeOptions().frame_size_policy(policy).checksum_flag(not ns.no_checksum)
@@ -378,6 +394,64 @@ def _run_compress(zk, ns, fmt_bytes) -> int:
     if not ns.quiet:
         ratio = 100.0 / read * written if read else float("nan")
         sys.stderr.write(f"{in_path or 'STDIN'} : {ratio:.2f}% ( {fmt_bytes(read)} => {fmt_bytes(written)}, {out_path or 'STDOUT'})\n")
+    return 0
+
+
+def _load_whole(path, what: str):
+    """a file's bytes, memory-mapped from MMAP_THRESHOLD bytes on"""
+    try:
+        if os.path.getsize(path) >= MMAP_THRESHOLD:
+            return np.memmap(path, dtype=np.uint8, mode="r")
+        return np.fromfile(path, dtype=np.uint8)
+    except OSError as e:
+        raise CliError(f"Failed to read {what}: {e}")
+
+
+def _run_compress_reuse(zk, ns, fmt_bytes, reader, writer, in_path, out_path, st_file) -> int:
+    """compress with --reuse-from: the whole input in one batch call (Context.compress_frames_reuse) with the frame sizes the encoder's
+    policy gives, then the archive and seek table exactly as the encoder writes them"""
+    if in_path is not None and os.path.isfile(in_path):
+        reader.close()
+        data = _load_whole(in_path, "input file")
+    else:
+        data = np.frombuffer(reader.read(), dtype=np.uint8)
+    old = _load_whole(ns.reuse_from, "--reuse-from archive")
+    ctx = zk.default_context()
+    n = int(data.size)
+    if ns.frame_size_policy == "content":
+        sizes, _ = ctx.cut_frames_cdc(data, ns.frame_size)
+    else:
+        fs = min(ns.frame_size, zk.SEEKABLE_MAX_FRAME_SIZE)
+        sizes = np.full(n // fs, fs, dtype=np.uint32)
+        if n % fs or n == 0:
+            sizes = np.append(sizes, np.uint32(n % fs))
+    try:
+        zk.SeekTable.from_bytes(old, zk.Format.Foot)
+    except zk.Error as e:
+        raise CliError(f"{ns.reuse_from}: not a seekable archive ending in its seek table: {e}")
+    comp, cs, reused = ctx.compress_frames_reuse(data, sizes, old, ns.compression_level, not ns.no_checksum, ns.long_mode)
+    table = zk.SeekTable()
+    for c, d in zip(cs.tolist(), sizes.tolist()):
+        table.log_frame(c, d)
+    writer.write(comp.tobytes())
+    written = int(comp.size)
+    if st_file is not None:
+        blob = table.into_format_serializer(zk.Format.Head).to_bytes()
+        st_file.write(blob)
+        st_file.close()
+    else:
+        blob = table.into_serializer().to_bytes()
+        writer.write(blob)
+    written += len(blob)
+    if writer is not sys.stdout.buffer:
+        writer.close()
+    else:
+        writer.flush()
+    if not ns.quiet:
+        n_reused = int(np.count_nonzero(reused != 0xFFFFFFFF))
+        sys.stderr.write(f"reused {n_reused} of {len(sizes)} frames\n")
+        ratio = 100.0 / n * written if n else float("nan")
+        sys.stderr.write(f"{in_path or 'STDIN'} : {ratio:.2f}% ( {fmt_bytes(n)} => {fmt_bytes(written)}, {out_path or 'STDOUT'})\n")
     return 0
 
 

@@ -8,6 +8,8 @@
 #include <stdlib.h>
 #include <string.h>
 #include <set>
+#include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 static thread_local char zk_tls_cuda_msg[256] = "";
@@ -125,6 +127,7 @@ extern "C" void zk_ctx_destroy(zk_ctx* c) {
     if (c->up) cudaStreamDestroy(c->up);
     if (c->down) cudaStreamDestroy(c->down);
     if (c->d_prefix) cudaFree(c->d_prefix);
+    for (int i = 0; i < 4; i++) if (c->d_reuse[i]) cudaFree(c->d_reuse[i]);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
     delete c;
@@ -519,7 +522,7 @@ static int32_t zk_frame_passes(zk_ctx* c, const ZkCompressReq& q, cudaStream_t s
         const int at_end = pos + len == q.n;
         const uint8_t* d_in = q.src + pos; uint8_t* d_out = q.dst + out; size_t cap = q.dst_cap - out;
         if (q.host) {
-            cap = zk_encode_bound(len, min_frame);
+            cap = q.dst ? zk_encode_bound(len, min_frame) : 0;     // no dst: a cut without compression (zk_cut_frames_cdc)
             int rc = zk_slot_ensure(&s, len + 32, cap + 32);
             if (rc) return rc;
             ZK_CUDA_OK(cudaMemcpyAsync(s.d_in, q.src + pos, len, cudaMemcpyHostToDevice, st));
@@ -536,7 +539,7 @@ static int32_t zk_frame_passes(zk_ctx* c, const ZkCompressReq& q, cudaStream_t s
         if (r.n_frames > q.frames_cap - nf) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
         if (q.host) {
             if (r.total > q.dst_cap - out) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
-            ZK_CUDA_OK(cudaMemcpy(q.dst + out, s.d_out, r.total, cudaMemcpyDeviceToHost));
+            if (r.total) ZK_CUDA_OK(cudaMemcpy(q.dst + out, s.d_out, r.total, cudaMemcpyDeviceToHost));
         }
         if (q.c_sizes) memcpy(q.c_sizes + nf, r.c_sizes, (size_t)r.n_frames * 4);
         if (q.d_sizes) memcpy(q.d_sizes + nf, r.d_sizes, (size_t)r.n_frames * 4);
@@ -562,7 +565,8 @@ static int32_t zk_csize_passes(zk_ctx* c, const ZkCompressReq& q, cudaStream_t s
 }
 
 // ContentDefined(size): each pass is cut on the GPU (zk_encode_cdc), then its closed frames are compressed from the same device memory by
-// the sized path, in sub-batches of at most the first pass's length.  A pass of mx bytes always closes a frame.
+// the sized path, in sub-batches of at most the first pass's length (q.dst == nullptr: not at all, zk_cut_frames_cdc).  A pass of mx
+// bytes always closes a frame.
 // ZK_CDC_CAP (tests): candidate positions kept per pass (default pass / 64 + 1); fewer only makes a pass cover less.
 static int32_t zk_cdc_passes(zk_ctx* c, const ZkCompressReq& q, cudaStream_t st, size_t first_pass) {
     const ZkCdcRule rule = zk_cdc_rule(q.size);
@@ -572,6 +576,7 @@ static int32_t zk_cdc_passes(zk_ctx* c, const ZkCompressReq& q, cudaStream_t st,
         ZkCdcOut r;
         int32_t rc = zk_encode_cdc(&c->slot[0].ews, st, d_in, len, q.size, q.final_, at_end, cand_cap, &r);
         if (rc || r.n_frames == 0) return rc;
+        if (!q.dst) { o->n_frames = r.n_frames; o->consumed = r.consumed; o->d_sizes = r.sizes; return 0; }    // the cut alone
         ds.assign(r.sizes, r.sizes + r.n_frames);
         cs.resize(r.n_frames);
         const ZkFrames fr = {ds.data(), r.consumed, 0, r.n_frames};
@@ -829,4 +834,253 @@ extern "C" int32_t zk_compress_frames_cdc_dev(zk_ctx* c, const void* d_src, size
     q.dst = (uint8_t*)d_dst; q.dst_cap = dst_cap; q.c_sizes = c_sizes; q.d_sizes = d_sizes; q.frames_cap = frames_cap; q.n_frames = n_frames;
     q.dst_len = dst_len; q.consumed = consumed;
     return zk_compress(c, q);
+}
+
+// the content-defined cut alone: the d_sizes and consumed of zk_compress_frames_cdc, from the same passes (zk_cdc_passes) without dst
+extern "C" int32_t zk_cut_frames_cdc(zk_ctx* c, const uint8_t* src, size_t n, uint32_t size, int32_t final_, uint32_t* frame_sizes,
+                                     uint32_t frames_cap, uint32_t* n_frames, size_t* consumed) {
+    if (!c || (n && !src)) return ZK_ERR_INVALID_ARG;
+    if (consumed) *consumed = 0;
+    if (n_frames) *n_frames = 0;
+    if (n == 0) {                                           // one empty frame when final, as zk_compress_frames_cdc makes of no input
+        if (!final_) return 0;
+        if (frames_cap < 1 || !frame_sizes) return frames_cap < 1 ? ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL) : ZK_ERR_INVALID_ARG;
+        frame_sizes[0] = 0;
+        if (n_frames) *n_frames = 1;
+        return 0;
+    }
+    if (!frame_sizes) return ZK_ERR_INVALID_ARG;
+    ZK_CUDA_OK(cudaSetDevice(c->device));
+    ZkCompressReq q;
+    q.policy = ZK_FRAMES_CONTENT; q.size = size; q.src = src; q.n = n; q.final_ = final_;
+    q.d_sizes = frame_sizes; q.frames_cap = frames_cap; q.n_frames = n_frames; q.consumed = consumed;
+    return zk_cdc_passes(c, q, c->slot[0].stream, zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20));
+}
+
+// ---------------------------------------------------------------------------------------------
+// Reuse (DESIGN §3.8): compress a new version against the previous archive.  Frame f copies the lowest-index old entry of its size,
+// checksum flag and key when the entry's decoded bytes equal f's bytes (compared on the GPU); every other frame is compressed by the sized
+// path.  Unpipelined, on slot 0.
+//   pass A  the old entries whose decoded size is some new frame's size (and whose flag matches), decoded in sub-batches of at most
+//           ZK_HOST_SUB_BYTES of output: their keys go into a host map (size, key) -> lowest index
+//   pass B  per sub-batch of at most ZK_HOST_SUB_BYTES_ENC of input: the frames' keys, the candidates decoded again and compared, the
+//           changed frames gathered and compressed, the output assembled in frame order and copied down
+// ---------------------------------------------------------------------------------------------
+struct ZkReuseKey {
+    uint32_t size; unsigned long long key;
+    bool operator==(const ZkReuseKey& o) const { return size == o.size && key == o.key; }
+};
+struct ZkReuseKeyHash {
+    size_t operator()(const ZkReuseKey& k) const { return (size_t)(k.key ^ (unsigned long long)k.size * 0x9E3779B97F4A7C15ull); }
+};
+
+struct ZkOldArchive { const uint8_t* comp; const uint64_t* c_off; const uint64_t* d_off; };
+
+static uint32_t zk_le32(const uint8_t* p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
+
+// the Content_Checksum_flag of the first zstd frame of an entry (skippable frames before it are passed over): 0 or 1, -1 if it has none
+static int zk_entry_checksum_flag(const uint8_t* p, size_t len) {
+    size_t pos = 0;
+    while (pos + 5 <= len) {
+        const uint32_t magic = zk_le32(p + pos);
+        if (magic == ZK_MAGIC) return (p[pos + 4] >> 2) & 1;
+        if ((magic & ZK_SKIPPABLE_MASK) != ZK_SKIPPABLE_MAGIC || pos + 8 > len) return -1;
+        pos += 8 + (size_t)zk_le32(p + pos + 4);
+    }
+    return -1;
+}
+
+// a device buffer of the context's reuse staging, grown to at least `need` bytes plus padding
+static int32_t zk_reuse_buf(zk_ctx* c, int i, size_t need, uint8_t** out) {
+    const int rc = zk_grow(&c->d_reuse[i], &c->cap_reuse[i], need + 64, 1);
+    *out = (uint8_t*)c->d_reuse[i];
+    return rc;
+}
+
+// old entries list[0, m): their bytes uploaded back to back (runs of consecutive entries in one copy) into buffer 0 and decoded, with
+// checksum verification, into buffer 1 -> *c_rel / *d_rel (m + 1 offsets in those buffers), per-entry statuses in *status
+static int32_t zk_reuse_decode(zk_ctx* c, const ZkOldArchive& o, const uint32_t* list, uint32_t m, std::vector<uint64_t>* c_rel,
+                               std::vector<uint64_t>* d_rel, std::vector<int32_t>* status, uint8_t** comp, uint8_t** dec) {
+    c_rel->assign(m + 1, 0); d_rel->assign(m + 1, 0); status->assign(m, 0);
+    for (uint32_t k = 0; k < m; k++) {
+        const uint32_t g = list[k];
+        (*c_rel)[k + 1] = (*c_rel)[k] + (o.c_off[g + 1] - o.c_off[g]);
+        (*d_rel)[k + 1] = (*d_rel)[k] + (o.d_off[g + 1] - o.d_off[g]);
+    }
+    int32_t rc = zk_reuse_buf(c, 0, (*c_rel)[m], comp);
+    if (!rc) rc = zk_reuse_buf(c, 1, (*d_rel)[m], dec);
+    if (rc || m == 0) return rc;
+    ZkSlot& s = c->slot[0];
+    for (uint32_t k0 = 0; k0 < m;) {
+        uint32_t k1 = k0 + 1;
+        while (k1 < m && list[k1] == list[k1 - 1] + 1) k1++;
+        const size_t bytes = (size_t)((*c_rel)[k1] - (*c_rel)[k0]);
+        if (bytes) ZK_CUDA_OK(cudaMemcpyAsync(*comp + (*c_rel)[k0], o.comp + o.c_off[list[k0]], bytes, cudaMemcpyHostToDevice, s.stream));
+        k0 = k1;
+    }
+    rc = zk_decode_batch(&s.dws, s.stream, *comp, c_rel->data(), d_rel->data(), m, *dec, 1, ZkDecodeParams(), status->data());
+    if (rc == ZK_INT_CUDA || rc == -(int)ZKZ_MEMORY_ALLOCATION) return rc;
+    return 0;                                               // an entry that fails to decode is only not a candidate
+}
+
+extern "C" int32_t zk_compress_frames_sized_reuse(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                                  int32_t checksum, int32_t long_mode, const uint8_t* old_comp, size_t old_len,
+                                                  const uint64_t* old_c_off, const uint64_t* old_d_off, uint32_t old_n, uint8_t* dst,
+                                                  size_t dst_cap, uint32_t* c_sizes, uint32_t* reused, size_t* dst_len) {
+    // the argument checks of zk_compress_frames_sized, then the old archive's
+    if (!c || (n_frames && (!frame_sizes || !dst))) return ZK_ERR_INVALID_ARG;
+    if (n_frames > ZK_SEEKABLE_MAX_FRAMES) return ZK_ERR_FRAME_INDEX_TOO_LARGE;
+    size_t n = 0;
+    for (uint32_t f = 0; f < n_frames; f++) {
+        if (frame_sizes[f] > ZK_SEEKABLE_MAX_FRAME_SIZE) return ZK_ERR_ZSTD(ZKZ_PARAM_OUT_OF_BOUND);
+        n += frame_sizes[f];
+    }
+    if (n && !src) return ZK_ERR_INVALID_ARG;
+    if (dst_len) *dst_len = 0;
+    if (old_n && (!old_comp || !old_c_off || !old_d_off)) return ZK_ERR_INVALID_ARG;
+    if (old_c_off && old_d_off) {
+        for (uint32_t g = 0; g < old_n; g++)
+            if (old_c_off[g + 1] < old_c_off[g] || old_d_off[g + 1] < old_d_off[g]) return ZK_ERR_INVALID_ARG;
+        if (old_c_off[old_n] > old_len) return ZK_ERR_INVALID_ARG;
+    }
+    if (n_frames == 0) return 0;
+    ZK_CUDA_OK(cudaSetDevice(c->device));
+    ZkSlot& s = c->slot[0];
+    const cudaStream_t st = s.stream;
+    const ZkOldArchive o = {old_comp, old_c_off, old_d_off};
+    const size_t bits = zk_env_size("ZK_REUSE_KEY_BITS", 64);          // tests: keep only the key's low bits (0: every key is equal)
+    const unsigned long long kmask = bits >= 64 ? ~0ull : (1ull << bits) - 1;
+    const bool trace = getenv("ZK_E2E_TRACE") != nullptr;
+    double t_index = 0, t_match = 0, t_comp = 0, t_asm = 0, t = ZkTrace::now();
+    auto lap = [&](double* acc) { const double u = ZkTrace::now(); *acc += u - t; t = u; };
+    int32_t rc = 0;
+    std::vector<uint64_t> c_rel, d_rel;
+    std::vector<int32_t> status;
+    std::vector<ZkReuseSpan> spans;
+    uint8_t *b_comp = nullptr, *b_dec = nullptr, *b_gather = nullptr, *b_out = nullptr;
+
+    // pass A: index the old entries that could match a new frame
+    std::unordered_set<uint32_t> want(frame_sizes, frame_sizes + n_frames);
+    std::vector<uint32_t> sel;
+    for (uint32_t g = 0; g < old_n; g++) {
+        const uint64_t d = old_d_off[g + 1] - old_d_off[g];
+        if (d <= ZK_SEEKABLE_MAX_FRAME_SIZE && want.count((uint32_t)d) &&
+            zk_entry_checksum_flag(old_comp + old_c_off[g], (size_t)(old_c_off[g + 1] - old_c_off[g])) == (checksum ? 1 : 0))
+            sel.push_back(g);
+    }
+    std::unordered_map<ZkReuseKey, uint32_t, ZkReuseKeyHash> index;
+    const size_t dec_sub = zk_env_size("ZK_HOST_SUB_BYTES", (size_t)128 << 20);
+    std::vector<unsigned long long> keys;
+    for (size_t i0 = 0; i0 < sel.size();) {
+        size_t i1 = i0 + 1, bytes = (size_t)(old_d_off[sel[i0] + 1] - old_d_off[sel[i0]]);
+        while (i1 < sel.size() && i1 - i0 < (1u << 20) && bytes + (old_d_off[sel[i1] + 1] - old_d_off[sel[i1]]) <= dec_sub)
+            bytes += (size_t)(old_d_off[sel[i1] + 1] - old_d_off[sel[i1]]), i1++;
+        const uint32_t m = (uint32_t)(i1 - i0);
+        if ((rc = zk_reuse_decode(c, o, &sel[i0], m, &c_rel, &d_rel, &status, &b_comp, &b_dec))) return rc;
+        spans.clear();
+        std::vector<uint32_t> ok;
+        for (uint32_t k = 0; k < m; k++)
+            if (status[k] == 0) { spans.push_back({d_rel[k], 0, (uint32_t)(d_rel[k + 1] - d_rel[k])}); ok.push_back(k); }
+        keys.resize(spans.size());
+        if ((rc = zk_reuse_run(&s.ews, st, ZK_REUSE_KEYS, b_dec, nullptr, spans.data(), (uint32_t)spans.size(), keys.data()))) return rc;
+        for (size_t j = 0; j < ok.size(); j++) index.emplace(ZkReuseKey{spans[j].len, keys[j] & kmask}, sel[i0 + ok[j]]);   // lowest index kept
+        i0 = i1;
+    }
+    lap(&t_index);
+
+    // pass B: the new frames, sub-batch by sub-batch
+    ZkEncodeParams p;
+    p.level = level; p.checksum = checksum; p.long_mode = long_mode != 0;
+    p.side = zk_env_size("ZK_HOST_SIDE", 1) != 0;
+    const ZkFrames fr = {frame_sizes, n, 0, n_frames};
+    const size_t enc_sub = zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20);
+    const uint32_t NONE = 0xFFFFFFFFu;
+    std::vector<uint32_t> fo, cand, list, eq, chg_sizes, chg_cs, flags;
+    size_t in_off = 0, out_pos = 0;
+    for (uint32_t f0 = 0; f0 < n_frames;) {
+        size_t in_len = 0;
+        const uint32_t end = fr.next_sub(f0, enc_sub, &in_len), cnt = end - f0;
+        if ((rc = zk_slot_ensure(&s, in_len + 64, 0))) return rc;
+        if (in_len) ZK_CUDA_OK(cudaMemcpyAsync(s.d_in, src + in_off, in_len, cudaMemcpyHostToDevice, st));
+        // the frames' keys, and each one's candidate
+        fo.assign(cnt + 1, 0);
+        spans.resize(cnt);
+        for (uint32_t k = 0; k < cnt; k++) { fo[k + 1] = fo[k] + frame_sizes[f0 + k]; spans[k] = {fo[k], 0, frame_sizes[f0 + k]}; }
+        keys.resize(cnt);
+        if ((rc = zk_reuse_run(&s.ews, st, ZK_REUSE_KEYS, s.d_in, nullptr, spans.data(), cnt, keys.data()))) return rc;
+        cand.assign(cnt, NONE); list.clear();
+        for (uint32_t k = 0; k < cnt; k++) {
+            const auto it = index.find(ZkReuseKey{frame_sizes[f0 + k], keys[k] & kmask});
+            if (it != index.end()) { cand[k] = (uint32_t)list.size(); list.push_back(it->second); }
+        }
+        // the candidates decoded and compared with their frames
+        if ((rc = zk_reuse_decode(c, o, list.data(), (uint32_t)list.size(), &c_rel, &d_rel, &status, &b_comp, &b_dec))) return rc;
+        spans.clear();
+        for (uint32_t k = 0; k < cnt; k++)
+            if (cand[k] != NONE) spans.push_back({d_rel[cand[k]], fo[k], frame_sizes[f0 + k]});
+        flags.resize(spans.size());
+        if ((rc = zk_reuse_run(&s.ews, st, ZK_REUSE_COMPARE, b_dec, s.d_in, spans.data(), (uint32_t)spans.size(), flags.data()))) return rc;
+        eq.assign(cnt, 0); chg_sizes.clear();
+        size_t chg_bytes = 0;
+        for (uint32_t k = 0, j = 0; k < cnt; k++) {
+            if (cand[k] != NONE) { eq[k] = flags[j] != 0 && status[cand[k]] == 0; j++; }
+            if (!eq[k]) { chg_sizes.push_back(frame_sizes[f0 + k]); chg_bytes += frame_sizes[f0 + k]; }
+        }
+        lap(&t_match);
+        // the changed frames gathered (unless all of them changed) and compressed
+        const uint32_t n_chg = (uint32_t)chg_sizes.size();
+        size_t produced = 0;
+        chg_cs.assign(n_chg, 0);
+        if (n_chg) {
+            const uint8_t* from = s.d_in;
+            if (n_chg < cnt) {
+                if ((rc = zk_reuse_buf(c, 2, chg_bytes, &b_gather))) return rc;
+                spans.clear();
+                size_t pos = 0;
+                for (uint32_t k = 0; k < cnt; k++)
+                    if (!eq[k]) { spans.push_back({fo[k], pos, frame_sizes[f0 + k]}); pos += frame_sizes[f0 + k]; }
+                if ((rc = zk_reuse_run(&s.ews, st, ZK_REUSE_COPY, s.d_in, b_gather, spans.data(), (uint32_t)spans.size(), nullptr))) return rc;
+                from = b_gather;
+            }
+            const ZkFrames cf = {chg_sizes.data(), chg_bytes, 0, n_chg};
+            const size_t bound = cf.bound();
+            if ((rc = zk_slot_ensure(&s, in_len + 64, bound + 64))) return rc;
+            rc = zk_encode_enqueue(&s.ews, st, from, cf, p, s.d_out, bound);
+            if (!rc) rc = zk_encode_collect(&s.ews, st, chg_cs.data(), &produced);
+            if (rc) return rc;
+        }
+        lap(&t_comp);
+        // the output in frame order: old entries from their staged bytes, the rest from the compressed changed frames
+        size_t sub_out = 0;
+        for (uint32_t k = 0, j = 0; k < cnt; k++) {
+            const uint32_t f = f0 + k;
+            const uint32_t cs = eq[k] ? (uint32_t)(c_rel[cand[k] + 1] - c_rel[cand[k]]) : chg_cs[j++];
+            if (c_sizes) c_sizes[f] = cs;
+            if (reused) reused[f] = eq[k] ? list[cand[k]] : NONE;
+            sub_out += cs;
+        }
+        if (sub_out > dst_cap - out_pos) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
+        const uint8_t* down = s.d_out;
+        if (n_chg < cnt) {
+            if ((rc = zk_reuse_buf(c, 3, sub_out, &b_out))) return rc;
+            std::vector<ZkReuseSpan> from_new;                // one launch per source buffer
+            spans.clear();
+            size_t pos = 0, cpos = 0;
+            for (uint32_t k = 0, j = 0; k < cnt; k++) {
+                const uint32_t cs = eq[k] ? (uint32_t)(c_rel[cand[k] + 1] - c_rel[cand[k]]) : chg_cs[j++];
+                if (eq[k]) spans.push_back({c_rel[cand[k]], pos, cs});
+                else { from_new.push_back({cpos, pos, cs}); cpos += cs; }
+                pos += cs;
+            }
+            if ((rc = zk_reuse_run(&s.ews, st, ZK_REUSE_COPY, b_comp, b_out, spans.data(), (uint32_t)spans.size(), nullptr))) return rc;
+            if ((rc = zk_reuse_run(&s.ews, st, ZK_REUSE_COPY, s.d_out, b_out, from_new.data(), (uint32_t)from_new.size(), nullptr))) return rc;
+            down = b_out;
+        }
+        if (sub_out) ZK_CUDA_OK(cudaMemcpy(dst + out_pos, down, sub_out, cudaMemcpyDeviceToHost));
+        lap(&t_asm);
+        out_pos += sub_out; in_off += in_len; f0 = end;
+    }
+    if (dst_len) *dst_len = out_pos;
+    if (trace) fprintf(stderr, "reuse index %.3f match %.3f compress %.3f assemble %.3f ms\n", t_index, t_match, t_comp, t_asm);
+    return 0;
 }

@@ -1596,6 +1596,7 @@ size_t ZkFrames::bound() const { return sizes ? zk_encode_bound_sized(sizes, cou
 void zk_encode_ws_free(ZkEncodeWs* ws) {
     if (ws->buf) cudaFree(ws->buf);
     if (ws->cut) cudaFree(ws->cut);
+    if (ws->reuse) cudaFree(ws->reuse);
     if (ws->h_sizes) cudaFreeHost(ws->h_sizes);
     if (ws->side) cudaStreamDestroy(ws->side);
     if (ws->ev_a) cudaEventDestroy(ws->ev_a);
@@ -1985,3 +1986,5 @@ int zk_encode_cdc(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, siz
     out->sizes = ws->h_sizes + ZKC_CDC_RES_HDR;
     return 0;
 }
+
+#include "zk_reuse.inc"

@@ -5,6 +5,7 @@
 struct ZkEncodeWs {                    // HBM scratch owned by a zk_ctx slot, grown on demand
     void* buf = nullptr; size_t cap = 0;
     void* cut = nullptr; size_t cut_cap = 0;              // content-defined cut (zk_encode_cdc): kept apart from buf, which the frames of a cut then use
+    void* reuse = nullptr; size_t reuse_cap = 0;          // span tables and results of zk_reuse_run
     uint32_t* h_sizes = nullptr; size_t cap_frames = 0;   // pinned: per-frame compressed sizes
     int sm_count = 0;
     unsigned long long launches = 0;
@@ -90,3 +91,14 @@ struct ZkCdcOut {
 };
 int zk_encode_cdc(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, uint32_t size, int final_, int at_end, uint32_t cap,
                   ZkCdcOut* out);
+
+// zk_compress_frames_sized_reuse (zk_reuse.inc): one launch over n spans, each split into 32 KiB work items.  Span s covers
+// a_buf[a, a + len) and b_buf[b, b + len) (device buffers with 16 readable bytes after their last span; spans start at any byte).
+//   ZK_REUSE_KEYS     out (host, n words): the key of the a side, XXH64 of the little-endian XXH64s of its consecutive 32 KiB chunks
+//   ZK_REUSE_COMPARE  out (host, n u32): non-zero iff the a side equals the b side
+//   ZK_REUSE_COPY     the a side to the b side (the two must not overlap); out unused
+// Synchronous on `stream`.
+enum ZkReuseOp { ZK_REUSE_KEYS, ZK_REUSE_COMPARE, ZK_REUSE_COPY };
+struct ZkReuseSpan { unsigned long long a, b; uint32_t len; };
+int zk_reuse_run(ZkEncodeWs* ws, cudaStream_t stream, ZkReuseOp op, const uint8_t* a_buf, uint8_t* b_buf, const ZkReuseSpan* spans, uint32_t n,
+                 void* out);
