@@ -105,6 +105,8 @@ extern "C" int32_t zk_ctx_create(int32_t device_ordinal, uint32_t flags, zk_ctx*
         c->slot[i].ews.sm_count = c->sm_count;
     }
     cudaEventCreate(&c->ev0); cudaEventCreate(&c->ev1);
+    cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming);
+    for (int i = 0; i < ZK_SLOTS; i++) cudaEventCreateWithFlags(&c->ev_join[i], cudaEventDisableTiming);
     if (zk_env_size("ZK_HOST_COPY_STREAMS", 1) != 0) {
         cudaStreamCreateWithFlags(&c->up, cudaStreamNonBlocking); cudaStreamCreateWithFlags(&c->down, cudaStreamNonBlocking);
     }
@@ -130,6 +132,9 @@ extern "C" void zk_ctx_destroy(zk_ctx* c) {
     for (int i = 0; i < 4; i++) if (c->d_reuse[i]) cudaFree(c->d_reuse[i]);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
+    if (c->ev_fork) cudaEventDestroy(c->ev_fork);
+    for (int i = 0; i < ZK_SLOTS; i++) if (c->ev_join[i]) cudaEventDestroy(c->ev_join[i]);
+    if (c->d_chain) cudaFree(c->d_chain);
     delete c;
 }
 
@@ -205,29 +210,30 @@ static uint32_t zk_next_sub(const uint64_t* d_off, uint32_t first, uint32_t n, s
     return e;
 }
 
-extern "C" int32_t zk_decompress_frames_dev(zk_ctx* c, const void* d_comp, const uint64_t* c_off, const uint64_t* d_off,
-                                            uint32_t n, void* d_dst, int32_t verify, int32_t* status, void* cuda_stream) {
-    if (!c || (n && (!d_comp || !c_off || !d_off || !d_dst))) return ZK_ERR_INVALID_ARG;
-    if (n == 0) return 0;
-    ZK_CUDA_OK(cudaSetDevice(c->device));
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : c->slot[0].stream;
-    const size_t sub_bytes = zk_env_size("ZK_DEV_SUB_BYTES", (size_t)1 << 30);
-    ZkDecodeParams p;                                       // device-resident data: nothing to copy but offsets and statuses
-    p.side = zk_env_size("ZK_DEV_SIDE", 1) != 0;
-    cudaEventRecord(c->ev0, st);
-    int32_t worst = 0;
-    for (uint32_t first = 0; first < n;) {
-        uint32_t end = zk_next_sub(d_off, first, n, sub_bytes, 1u << 20);
-        int rc = zk_decode_batch(&c->slot[0].dws, st, (const uint8_t*)d_comp, c_off + first, d_off + first, end - first, (uint8_t*)d_dst,
-                                 verify, p, status ? status + first : nullptr);
-        if (rc && !worst) worst = rc;
-        if (rc == ZK_INT_CUDA || rc == -(int)ZKZ_MEMORY_ALLOCATION) return rc;
-        first = end;
+// Device-pointer calls run their sub-batches on the first ns slot streams: those start after the work the caller's stream st holds so far
+// (zk_dev_fork), and st continues after all of theirs (zk_dev_join)
+static int32_t zk_dev_fork(zk_ctx* c, cudaStream_t st, int ns) {
+    ZK_CUDA_OK(cudaEventRecord(c->ev_fork, st));
+    for (int i = 0; i < ns; i++) if (c->slot[i].stream != st) ZK_CUDA_OK(cudaStreamWaitEvent(c->slot[i].stream, c->ev_fork, 0));
+    return 0;
+}
+static int32_t zk_dev_join(zk_ctx* c, cudaStream_t st, int ns) {
+    for (int i = 0; i < ns; i++) {
+        if (c->slot[i].stream == st) continue;
+        ZK_CUDA_OK(cudaEventRecord(c->ev_join[i], c->slot[i].stream));
+        ZK_CUDA_OK(cudaStreamWaitEvent(st, c->ev_join[i], 0));
     }
-    cudaEventRecord(c->ev1, st);
-    cudaEventSynchronize(c->ev1);
-    cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1);
-    return worst;
+    return 0;
+}
+
+// input (compress) or output (decompress) bytes per sub-batch of the device-pointer paths, and the sub-batches in flight (tuning knobs,
+// swept by tools/pipeline_probe.py; DESIGN §6).  Compress runs four sub-batches of 256 MiB at once: the drain of each stage of one overlaps
+// the kernels of the others.  Decompress keeps one sub-batch of up to 1 GiB: concurrent sub-batches were slower than it at every size.
+// The passes of the cut policies, each of which ends in a host synchronisation, start at the decompress size
+static size_t zk_dev_sub_bytes(bool enc) { return zk_env_size("ZK_DEV_SUB_BYTES", enc ? (size_t)256 << 20 : (size_t)1 << 30); }
+static int zk_dev_slots(bool enc) {
+    const size_t v = zk_env_size("ZK_DEV_SLOTS", enc ? 4 : 1);
+    return (int)(v < 1 ? 1 : (v > ZK_SLOTS ? ZK_SLOTS : v));
 }
 
 // ZK_E2E_TRACE=1: per-sub-batch timeline of the host-pointer paths (CUDA events on the slot streams), printed to stderr.
@@ -255,10 +261,11 @@ struct ZkTrace {
     }
 };
 
-// one host-pointer decompress call
+// one decompress call
 struct ZkDecCall {
     const uint8_t* comp; const uint64_t* c_off; const uint64_t* d_off; uint8_t* dst; int verify; int32_t* status;
     ZkDecodeParams p;                                       // p.need: the whole call's
+    bool host = true;                                       // comp and dst in host memory, copied through the slots; else device memory
 };
 struct ZkSubDec { uint32_t first = 0, count = 0; std::vector<uint64_t> c_rel, d_rel; bool busy = false; };
 
@@ -266,6 +273,11 @@ static int zk_dec_sub_enqueue(zk_ctx* c, int si, ZkSubDec& sb, const ZkDecCall& 
     ZkSlot& s = c->slot[si];
     uint32_t f = sb.first, cnt = sb.count;
     const uint64_t* c_off = q.c_off; const uint64_t* d_off = q.d_off;
+    if (!q.host) {                                          // decoded in place: the offsets stay those of the whole call
+        const int rc = zk_decode_enqueue(&s.dws, s.stream, q.comp, c_off + f, d_off + f, cnt, q.dst, q.verify, q.p);
+        sb.busy = rc == 0;
+        return rc;
+    }
     size_t cbytes = (size_t)(c_off[f + cnt] - c_off[f]), obytes = (size_t)(d_off[f + cnt] - d_off[f]);
     int rc = zk_slot_ensure(&s, cbytes + 32, obytes + 32);
     if (rc) return rc;
@@ -303,6 +315,8 @@ static int zk_dec_sub_finish(zk_ctx* c, int si, ZkSubDec& sb, const ZkDecCall& q
     return rc;
 }
 
+static int32_t zk_dec_run(zk_ctx* c, const ZkDecCall& q, uint32_t n, size_t sub_bytes, int ns, uint32_t ramp);
+
 extern "C" int32_t zk_decompress_frames(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off,
                                         uint32_t n, uint8_t* dst, int32_t verify, int32_t* status) {
     return zk_decompress_frames_upto(c, comp, c_off, d_off, n, dst, nullptr, verify, status);
@@ -338,31 +352,56 @@ extern "C" int32_t zk_decompress_frames_prefixes(zk_ctx* c, const uint8_t* comp,
     q.p.share = (int)zk_env_size("ZK_HOST_SHARE", 3);
     q.p.side = zk_env_size("ZK_HOST_SIDE", 1) != 0;
     q.p.up = c->up; q.p.down = c->down;
+    // ZK_HOST_RAMP=r (default 0): the first r sub-batches are 1/2^r ... 1/2 of the full size, so that the output copy could start
+    // earlier.  It gave no gain when it was tried: a sub-batch of any size spends about one frame latency in
+    // K-D2, so a small first sub-batch is not done much sooner than a full one
+    return zk_dec_run(c, q, n, sub_bytes, zk_host_slots(false), (uint32_t)zk_env_size("ZK_HOST_RAMP", 0));
+}
+
+// the sub-batches of a decompress call, dealt round-robin over ns slots; the first `ramp` are 1/2^ramp ... 1/2 of sub_bytes.  Returns 0
+// or the first failure in the order of the entries
+static int32_t zk_dec_run(zk_ctx* c, const ZkDecCall& q, uint32_t n, size_t sub_bytes, int ns, uint32_t ramp) {
     ZkSubDec sub[ZK_SLOTS];
-    const int NS = zk_host_slots(false);
-    const uint32_t ramp = (uint32_t)zk_env_size("ZK_HOST_RAMP", 0);            // the first `ramp` sub-batches are 1/2^ramp ... 1/2 of the full size
-    int32_t worst = 0;
+    int32_t worst = 0, rc;
     uint32_t k = 0;
     ZkTrace tr; tr.begin(c->slot[0].stream);
     for (uint32_t first = 0; first < n; k++) {
-        int si = (int)(k % NS);
+        int si = (int)(k % ns);
         rc = zk_dec_sub_finish(c, si, sub[si], q);
         if (rc && !worst) worst = rc;
-        // ZK_HOST_RAMP=r (default 0): the first r sub-batches are 1/2^r ... 1/2 of the full size, so that the output copy could start
-        // earlier.  It gave no gain when it was tried: a sub-batch of any size spends about one frame latency in
-        // K-D2, so a small first sub-batch is not done much sooner than a full one
         const size_t this_sub = k < ramp ? sub_bytes >> (ramp - k) : sub_bytes;
-        uint32_t end = zk_next_sub(d_off, first, n, this_sub, 1u << 20);
+        uint32_t end = zk_next_sub(q.d_off, first, n, this_sub, 1u << 20);
         sub[si].first = first; sub[si].count = end - first;
         rc = zk_dec_sub_enqueue(c, si, sub[si], q, &tr, (int)k);
         if (rc) { if (!worst) worst = rc; break; }
         first = end;
     }
-    for (int si = 0; si < ZK_SLOTS; si++) {
-        rc = zk_dec_sub_finish(c, si, sub[si], q);
+    for (uint32_t j = 0; j < (uint32_t)ns; j++) {         // oldest first
+        rc = zk_dec_sub_finish(c, (int)((k + j) % ns), sub[(k + j) % ns], q);
         if (rc && !worst) worst = rc;
     }
     tr.end("dec");
+    return worst;
+}
+
+// device-resident archive and output: sub-batches decoded in place on the slot streams, between the caller stream's work before and after
+extern "C" int32_t zk_decompress_frames_dev(zk_ctx* c, const void* d_comp, const uint64_t* c_off, const uint64_t* d_off,
+                                            uint32_t n, void* d_dst, int32_t verify, int32_t* status, void* cuda_stream) {
+    if (!c || (n && (!d_comp || !c_off || !d_off || !d_dst))) return ZK_ERR_INVALID_ARG;
+    if (n == 0) return 0;
+    ZK_CUDA_OK(cudaSetDevice(c->device));
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : c->slot[0].stream;
+    ZkDecCall q = {(const uint8_t*)d_comp, c_off, d_off, (uint8_t*)d_dst, verify, status, ZkDecodeParams(), false};
+    const int ns = zk_dev_slots(false);
+    q.p.side = zk_env_size("ZK_DEV_SIDE", 1) != 0;
+    q.p.share = (int)zk_env_size("ZK_DEV_SHARE", 1);
+    ZK_CUDA_OK(cudaEventRecord(c->ev0, st));
+    int32_t rc = zk_dev_fork(c, st, ns);
+    const int32_t worst = rc ? rc : zk_dec_run(c, q, n, zk_dev_sub_bytes(false), ns, 0);
+    if ((rc = zk_dev_join(c, st, ns))) return rc;
+    ZK_CUDA_OK(cudaEventRecord(c->ev1, st));
+    ZK_CUDA_OK(cudaEventSynchronize(c->ev1));
+    cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1);
     return worst;
 }
 
@@ -387,23 +426,6 @@ struct ZkCompressReq {
     size_t* dst_len = nullptr; size_t* consumed = nullptr;
 };
 
-// device-resident input and output: sub-batches of at most sub_bytes input (which bound the scratch, about 4x that) one after the other on st
-static int32_t zk_compress_dev_subs(zk_ctx* c, const ZkFrames& fr, const uint8_t* d_src, const ZkEncodeParams& p, uint8_t* d_dst,
-                                    size_t dst_cap, uint32_t* c_sizes, size_t* dst_len, cudaStream_t st, size_t sub_bytes) {
-    size_t out_pos = 0, in_off = 0;
-    for (uint32_t f0 = 0; f0 < fr.count;) {
-        size_t in_len = 0;
-        const uint32_t end = fr.next_sub(f0, sub_bytes, &in_len);
-        size_t produced = 0;
-        int rc = zk_encode_enqueue(&c->slot[0].ews, st, d_src + in_off, fr.sub(f0, end - f0, in_len), p, d_dst + out_pos, dst_cap - out_pos);
-        if (!rc) rc = zk_encode_collect(&c->slot[0].ews, st, c_sizes ? c_sizes + f0 : nullptr, &produced);
-        if (rc) return rc;
-        out_pos += produced; in_off += in_len; f0 = end;
-    }
-    *dst_len = out_pos;
-    return 0;
-}
-
 struct ZkSubEnc { uint32_t f0 = 0, cnt = 0; size_t in_off = 0, in_len = 0, out_pos = 0; bool busy = false; };
 
 // Long-distance matching indexes every distinct prefix range of a sub-batch once, at about one byte of scratch per indexed byte (the last
@@ -427,15 +449,23 @@ static uint32_t zk_ldm_sub_end(const ZkFrames& fr, const uint32_t* ranges, uint3
     return f;
 }
 
-// host input and output: sub-batches on up to ZK_HOST_SLOTS_ENC slots, output placed in order
-static int32_t zk_compress_host_run(zk_ctx* c, const ZkFrames& fr, const ZkCompressReq& q, size_t sub_bytes, size_t* dst_len) {
-    ZkEncodeParams p = q.params;
-    p.side = zk_env_size("ZK_HOST_SIDE", 1) != 0;
-    // The compressed size of a sub-batch is only known when it completes, so output positions are assigned in
-    // order at completion time: H2D and kernels of later sub-batches overlap the D2H of earlier ones.
+// The sub-batches of a compress call (at most sub_bytes of input each, which bounds the scratch at about 4x that), dealt round-robin over ns
+// slots.  A sub-batch's compressed size is only known when it completes.  host: src and dst in host memory; each sub-batch is copied up to
+// its slot and its frames back at the position the ones before it end, assigned in order as they complete, so the copies of one overlap
+// the kernels of others.  Else device memory: the slots start after the work of the caller's stream st, and every sub-batch writes its
+// frames to dst itself, at the offset the frame scan of the one before left on the device (ZkEncodeParams::chain), so only that scan
+// waits for the sub-batch before; st continues after all of them
+static int32_t zk_compress_run(zk_ctx* c, const ZkFrames& fr, const uint8_t* src, const ZkEncodeParams& p, uint8_t* dst, size_t dst_cap,
+                               uint32_t* c_sizes, bool host, size_t sub_bytes, int ns, cudaStream_t st, size_t* dst_len) {
+    unsigned long long* chain = nullptr;
+    if (!host) {
+        if (const int rc = zk_grow(&c->d_chain, &c->cap_chain, ((size_t)fr.count + 1) * 8, 1)) return rc;
+        chain = (unsigned long long*)c->d_chain;
+        ZK_CUDA_OK(cudaMemsetAsync(chain, 0, 8, st));
+        if (const int rc = zk_dev_fork(c, st, ns)) return rc;
+    }
     ZkSubEnc sub[ZK_SLOTS];
     size_t out_pos = 0, in_off = 0; int32_t err = 0;
-    std::vector<uint32_t> tmp_sizes(q.c_sizes ? 0 : fr.count);
     ZkTrace tr; tr.begin(c->slot[0].stream);
     int sub_k[ZK_SLOTS] = {0};
     auto finish = [&](int si) -> int {
@@ -443,21 +473,22 @@ static int32_t zk_compress_host_run(zk_ctx* c, const ZkFrames& fr, const ZkCompr
         if (!sb.busy) return 0;
         sb.busy = false;
         size_t produced = 0;
-        int rc = zk_encode_collect(&s.ews, s.stream, (q.c_sizes ? q.c_sizes : tmp_sizes.data()) + sb.f0, &produced);
+        int rc = zk_encode_collect(&s.ews, s.stream, c_sizes ? c_sizes + sb.f0 : nullptr, &produced);
         if (rc) return rc;
-        if (out_pos + produced > q.dst_cap) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
-        tr.mark(s.stream, sub_k[si], 3);
-        if (cudaMemcpyAsync(q.dst + out_pos, s.d_out, produced, cudaMemcpyDeviceToHost, s.stream) != cudaSuccess) return ZK_ERR_CUDA;
-        tr.mark(s.stream, sub_k[si], 4);
+        if (host) {
+            if (out_pos + produced > dst_cap) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
+            tr.mark(s.stream, sub_k[si], 3);
+            if (cudaMemcpyAsync(dst + out_pos, s.d_out, produced, cudaMemcpyDeviceToHost, s.stream) != cudaSuccess) return ZK_ERR_CUDA;
+            tr.mark(s.stream, sub_k[si], 4);
+        }
         out_pos += produced;
         return 0;
     };
     uint32_t k = 0;
-    const int NS = zk_host_slots(true);
     int n_inflight = 0;                                     // completion must follow submission order
     for (uint32_t f0 = 0; f0 < fr.count && !err; k++) {
-        const int si = (int)(k % NS);
-        if (n_inflight == NS) {                             // oldest in flight is exactly slot si
+        const int si = (int)(k % ns);
+        if (n_inflight == ns) {                             // oldest in flight is exactly slot si
             err = finish(si); n_inflight--;
             if (err) break;
         }
@@ -469,25 +500,33 @@ static int32_t zk_compress_host_run(zk_ctx* c, const ZkFrames& fr, const ZkCompr
         if (p.ranges) sp.ranges = p.ranges + 2 * (size_t)f0;
         sb.f0 = f0; sb.cnt = end - f0; sb.in_off = in_off;
         const ZkFrames sf = fr.sub(f0, sb.cnt, sb.in_len);
-        const size_t bound = sf.bound();
-        int rc = zk_slot_ensure(&s, sb.in_len + 32, bound + 32);
-        if (rc) { err = rc; break; }
-        sub_k[si] = (int)k; tr.mark(s.stream, (int)k, 0);
-        if (sb.in_len && cudaMemcpyAsync(s.d_in, q.src + sb.in_off, sb.in_len, cudaMemcpyHostToDevice, s.stream) != cudaSuccess) { err = ZK_ERR_CUDA; break; }
-        tr.mark(s.stream, (int)k, 1);
-        rc = zk_encode_enqueue(&s.ews, s.stream, s.d_in, sf, sp, s.d_out, bound);
+        int rc = 0;
+        if (host) {
+            const size_t bound = sf.bound();
+            rc = zk_slot_ensure(&s, sb.in_len + 32, bound + 32);
+            if (rc) { err = rc; break; }
+            sub_k[si] = (int)k; tr.mark(s.stream, (int)k, 0);
+            if (sb.in_len && cudaMemcpyAsync(s.d_in, src + sb.in_off, sb.in_len, cudaMemcpyHostToDevice, s.stream) != cudaSuccess) { err = ZK_ERR_CUDA; break; }
+            tr.mark(s.stream, (int)k, 1);
+            rc = zk_encode_enqueue(&s.ews, s.stream, s.d_in, sf, sp, s.d_out, bound);
+        } else {
+            sp.chain = chain + k;
+            sp.chain_wait = k ? c->slot[(k - 1) % ns].ews.ev_chain : nullptr;
+            rc = zk_encode_enqueue(&s.ews, s.stream, src + sb.in_off, sf, sp, dst, dst_cap);
+        }
         if (rc) { err = rc; break; }
         tr.mark(s.stream, (int)k, 2);
         sb.busy = true; n_inflight++;
         f0 = end; in_off += sb.in_len;
     }
     // drain in submission order
-    for (uint32_t j = 0; j < (uint32_t)NS && !err; j++) {
-        const int si = (int)((k + j) % NS);                // oldest first
+    for (uint32_t j = 0; j < (uint32_t)ns && !err; j++) {
+        const int si = (int)((k + j) % ns);                // oldest first
         int rc = finish(si);
         if (rc) err = rc;
     }
     for (int si = 0; si < ZK_SLOTS; si++) cudaStreamSynchronize(c->slot[si].stream);
+    if (!host && !err) err = zk_dev_join(c, st, ns);
     tr.end("enc");
     if (err) return err;
     *dst_len = out_pos;
@@ -565,10 +604,10 @@ static int32_t zk_csize_passes(zk_ctx* c, const ZkCompressReq& q, cudaStream_t s
 }
 
 // ContentDefined(size): each pass is cut on the GPU (zk_encode_cdc), then its closed frames are compressed from the same device memory by
-// the sized path, in sub-batches of at most the first pass's length (q.dst == nullptr: not at all, zk_cut_frames_cdc).  A pass of mx
+// the sized path, in sub-batches of at most sub_bytes (q.dst == nullptr: not at all, zk_cut_frames_cdc).  A pass of mx
 // bytes always closes a frame.
 // ZK_CDC_CAP (tests): candidate positions kept per pass (default pass / 64 + 1); fewer only makes a pass cover less.
-static int32_t zk_cdc_passes(zk_ctx* c, const ZkCompressReq& q, cudaStream_t st, size_t first_pass) {
+static int32_t zk_cdc_passes(zk_ctx* c, const ZkCompressReq& q, cudaStream_t st, size_t first_pass, size_t sub_bytes) {
     const ZkCdcRule rule = zk_cdc_rule(q.size);
     const uint32_t cand_cap = (uint32_t)zk_env_size("ZK_CDC_CAP", 0);
     std::vector<uint32_t> ds, cs;
@@ -580,7 +619,7 @@ static int32_t zk_cdc_passes(zk_ctx* c, const ZkCompressReq& q, cudaStream_t st,
         ds.assign(r.sizes, r.sizes + r.n_frames);
         cs.resize(r.n_frames);
         const ZkFrames fr = {ds.data(), r.consumed, 0, r.n_frames};
-        rc = zk_compress_dev_subs(c, fr, d_in, q.params, d_out, cap, cs.data(), &o->total, st, first_pass);
+        rc = zk_compress_run(c, fr, d_in, q.params, d_out, cap, cs.data(), false, sub_bytes, zk_dev_slots(true), st, &o->total);
         if (rc) return rc;
         o->n_frames = r.n_frames; o->consumed = r.consumed; o->c_sizes = cs.data(); o->d_sizes = ds.data();
         return 0;
@@ -630,13 +669,18 @@ static int32_t zk_compress(zk_ctx* c, ZkCompressReq q) {
     ZK_CUDA_OK(cudaSetDevice(c->device));
     const cudaStream_t st = q.stream ? q.stream : c->slot[0].stream;
     // tuning knobs: input bytes per sub-batch, and the first pass of the cut policies (tools/knobs_round.sh sweeps the host one)
-    const size_t sub_bytes = q.host ? zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20) : zk_env_size("ZK_DEV_SUB_BYTES", (size_t)1 << 30);
+    const size_t sub_bytes = q.host ? zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20) : zk_dev_sub_bytes(true);
     if (!q.host) cudaEventRecord(c->ev0, st);
     size_t out_len = 0;
-    if (q.policy == ZK_FRAMES_COMPRESSED) rc = zk_csize_passes(c, q, st, sub_bytes);
-    else if (q.policy == ZK_FRAMES_CONTENT) rc = zk_cdc_passes(c, q, st, sub_bytes);
-    else if (q.host) rc = zk_compress_host_run(c, fr, q, sub_bytes, &out_len);
-    else rc = zk_compress_dev_subs(c, fr, q.src, q.params, q.dst, q.dst_cap, q.c_sizes, &out_len, st, sub_bytes);
+    const size_t first_pass = q.host ? sub_bytes : zk_dev_sub_bytes(false);
+    if (q.policy == ZK_FRAMES_COMPRESSED) rc = zk_csize_passes(c, q, st, first_pass);
+    else if (q.policy == ZK_FRAMES_CONTENT) rc = zk_cdc_passes(c, q, st, first_pass, sub_bytes);
+    else {
+        ZkEncodeParams p = q.params;
+        if (q.host) p.side = zk_env_size("ZK_HOST_SIDE", 1) != 0;
+        rc = zk_compress_run(c, fr, q.src, p, q.dst, q.dst_cap, q.c_sizes, q.host, sub_bytes, q.host ? zk_host_slots(true) : zk_dev_slots(true), st,
+                             &out_len);
+    }
     if (rc) return rc;
     if (!q.host) {                                          // zk_ctx_last_device_ms: the device paths only
         cudaEventRecord(c->ev1, st);
@@ -854,7 +898,8 @@ extern "C" int32_t zk_cut_frames_cdc(zk_ctx* c, const uint8_t* src, size_t n, ui
     ZkCompressReq q;
     q.policy = ZK_FRAMES_CONTENT; q.size = size; q.src = src; q.n = n; q.final_ = final_;
     q.d_sizes = frame_sizes; q.frames_cap = frames_cap; q.n_frames = n_frames; q.consumed = consumed;
-    return zk_cdc_passes(c, q, c->slot[0].stream, zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20));
+    const size_t pass = zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20);
+    return zk_cdc_passes(c, q, c->slot[0].stream, pass, pass);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -19,6 +19,9 @@ struct zk_ctx {
     int sm_count = 132;
     ZkSlot slot[ZK_SLOTS];
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    cudaEvent_t ev_fork = nullptr, ev_join[ZK_SLOTS] = {};    // device-pointer calls: the slot streams start after, and the caller's stream
+                                                          // continues after, the work of the caller's stream
+    void* d_chain = nullptr; size_t cap_chain = 0;        // device-pointer compress: the output offset of every sub-batch (ZkEncodeParams::chain)
     cudaStream_t up = nullptr, down = nullptr;            // dedicated copy streams of the host-pointer decompress pipeline
     float last_ms = 0.f;
     void* d_prefix = nullptr; size_t cap_prefix = 0;      // device copy of the raw-content prefix of the calls that take one

@@ -2111,16 +2111,25 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     if (ws->ring_override) ring = ws->ring_override;
     // prefix mode: the same executors, built with the prefix split
     const bool prefix = a.prefix != nullptr;
-    if (a.exec_short) {          // short segments first, on single warps; the CTAs below then pull only long ones
+    void (*cta_kernel)(ZkDecodeArgs, uint32_t) = small_regs ? (prefix ? zk_exec_kernel_w5<true> : zk_exec_kernel_w5<false>)
+                                                            : (prefix ? zk_exec_kernel<true> : zk_exec_kernel<false>);
+    // Long segments run on the side stream beside the short ones: segments never wait for each other, so the CTA executor's long serial
+    // chains start with the warp executor's work instead of after its drain.  They are launched first, so their CTAs are resident first
+    const bool beside = a.exec_short && hs != stream;
+    if (beside) {
+        ZK_CUDA_OK(cudaEventRecord(ws->ev_scan, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(hs, ws->ev_scan, 0));     // after the plan
+        ZK_LAUNCH(cta_kernel, n, W * 32, ring, hs, a, ring);
+        ZK_CUDA_OK(cudaEventRecord(ws->ev_huf, hs));
+    }
+    if (a.exec_short) {          // short segments on single warps; the CTAs pull only long ones
         uint32_t gw = (uint32_t)sms * 8u;
         const size_t need_w = est_blocks / ZK_XW_WARPS + 1;
         if (need_w < gw) gw = (uint32_t)need_w;
         void (*warp_kernel)(ZkDecodeArgs) = prefix ? zk_exec_warp_kernel<true> : zk_exec_warp_kernel<false>;
         ZK_LAUNCH(warp_kernel, gw, 32 * ZK_XW_WARPS, ZK_XW_WARPS * ZK_XW_WIN, stream, a);
     }
-    void (*cta_kernel)(ZkDecodeArgs, uint32_t) = small_regs ? (prefix ? zk_exec_kernel_w5<true> : zk_exec_kernel_w5<false>)
-                                                            : (prefix ? zk_exec_kernel<true> : zk_exec_kernel<false>);
-    ZK_LAUNCH(cta_kernel, n, W * 32, ring, stream, a, ring);
+    if (beside) ZK_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_huf, 0));
+    else ZK_LAUNCH(cta_kernel, n, W * 32, ring, stream, a, ring);
     ws->prof.end(3, stream);
     if (verify_checksum) { ws->prof.begin(4, stream); ZK_LAUNCH(zk_xxh64_kernel, (n + 3) / 4, 128, 0, stream, a); ws->prof.end(4, stream); }
     if (ds != stream) { ZK_CUDA_OK(cudaEventRecord(ws->ev_done, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(ds, ws->ev_done, 0)); }

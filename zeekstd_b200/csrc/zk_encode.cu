@@ -1428,11 +1428,17 @@ __device__ __forceinline__ unsigned long long zkc_cta_scan(uint32_t n, X x, Put 
     return carry;
 }
 
-// frame offsets and the total (one CTA)
-__global__ void __launch_bounds__(1024) zk_frame_scan_kernel(ZkEncodeArgs a) {
+// frame offsets and the total (one CTA); with a chain (ZkEncodeParams::chain), the frames follow the chain[0] bytes the batches before
+// wrote, and chain[1] receives the end of this batch's
+__global__ void __launch_bounds__(1024) zk_frame_scan_kernel(ZkEncodeArgs a, unsigned long long* chain) {
+    const unsigned long long base = chain ? chain[0] : 0ull;
     const unsigned long long total = zkc_cta_scan(a.res[0], [&](uint32_t f) { return (unsigned long long)a.res[ZKC_RES_HDR + f]; },
-                                                  [&](uint32_t f, unsigned long long o) { a.frame_off[f] = o; });
-    if (threadIdx.x == 0) { *(unsigned long long*)(a.res + 4) = total; if (total > a.dst_cap) a.res[2] = ZKZ_DST_TOO_SMALL; }
+                                                  [&](uint32_t f, unsigned long long o) { a.frame_off[f] = base + o; });
+    if (threadIdx.x == 0) {
+        *(unsigned long long*)(a.res + 4) = total;
+        if (base + total > a.dst_cap) a.res[2] = ZKZ_DST_TOO_SMALL;
+        if (chain) chain[1] = base + total;
+    }
 }
 
 // gather: one warp per block copies its staged bytes to the final position and sets Last_Block (a variant was staged with its own
@@ -1602,6 +1608,7 @@ void zk_encode_ws_free(ZkEncodeWs* ws) {
     if (ws->ev_a) cudaEventDestroy(ws->ev_a);
     if (ws->ev_b) cudaEventDestroy(ws->ev_b);
     if (ws->ev_c) cudaEventDestroy(ws->ev_c);
+    if (ws->ev_chain) cudaEventDestroy(ws->ev_chain);
     ws->prof.destroy();
     *ws = ZkEncodeWs();
 }
@@ -1770,7 +1777,12 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     ws->prof.begin(7, stream);
     if (p.checksum && ss == stream) ZK_LAUNCH(zk_frame_hash_kernel, (n_frames + 3) / 4, 128, 0, stream, a);   // else: already done on the side stream (joined by ev_b)
     ZK_LAUNCH(zk_frame_size_kernel, (n_frames + 3) / 4, 128, 0, stream, a);
-    ZK_LAUNCH(zk_frame_scan_kernel, 1, 1024, 0, stream, a);
+    if (p.chain_wait) ZK_CUDA_OK(cudaStreamWaitEvent(stream, p.chain_wait, 0));     // the scan of the batch before wrote chain[0]
+    ZK_LAUNCH(zk_frame_scan_kernel, 1, 1024, 0, stream, a, p.chain);
+    if (p.chain) {
+        if (!ws->ev_chain) ZK_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_chain, cudaEventDisableTiming));
+        ZK_CUDA_OK(cudaEventRecord(ws->ev_chain, stream));
+    }
     ZK_LAUNCH(zk_frame_gather_kernel, (uint32_t)((n_blocks + 3) / 4), 128, 0, stream, a);
     ws->prof.end(7, stream);
     ZK_CUDA_OK(cudaMemcpyAsync(ws->h_sizes, a.res, (ZKC_RES_HDR + (size_t)n_frames) * 4, cudaMemcpyDeviceToHost, stream));
@@ -1909,7 +1921,7 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     ZK_LAUNCH(zk_geo_block_kernel, (nb + 255) / 256, 256, 0, stream, (ZkcGeo*)a.geo, a.frames, (const uint32_t*)a.res);
     if (p.checksum) ZK_LAUNCH(zk_frame_hash_kernel, (nb + 3) / 4, 128, 0, stream, a);
     ZK_LAUNCH(zk_frame_size_kernel, (nb + 3) / 4, 128, 0, stream, a);
-    ZK_LAUNCH(zk_frame_scan_kernel, 1, 1024, 0, stream, a);
+    ZK_LAUNCH(zk_frame_scan_kernel, 1, 1024, 0, stream, a, (unsigned long long*)nullptr);
     ZK_LAUNCH(zk_frame_gather_kernel, (nb + 3) / 4, 128, 0, stream, a);
     ws->prof.end(7, stream);
     ws->launches += 8 + (p.checksum ? 1 : 0);

@@ -13,6 +13,7 @@ struct ZkEncodeWs {                    // HBM scratch owned by a zk_ctx slot, gr
     bool attr_set = false, attr_set_wide = false, attr_set_walk = false, attr_set_hc = false, attr_set_cdc = false;
     int prio = 0;                     // CUDA stream priority of the side stream (matches the slot's stream)
     cudaStream_t side = nullptr; cudaEvent_t ev_a = nullptr, ev_b = nullptr, ev_c = nullptr;   // K-C2s runs beside K-C2l
+    cudaEvent_t ev_chain = nullptr;   // recorded after the last batch's frame scan when it had a chain (ZkEncodeParams::chain)
     ZkProf prof;
 };
 
@@ -26,6 +27,11 @@ struct ZkEncodeParams {
     bool long_mode = false;           // long mode: every frame also matches its own bytes up to 2^27 back (and the prefix as ldm does)
     bool side = true;                 // K-C2s and the checksum on the side stream; host pipelines get their concurrency from the other
                                       // sub-batches instead, and every extra stream costs a hardware queue
+    // batches that write one output one after another, each enqueued before the one before it completed: chain[0] (device) holds the
+    // bytes before the batch's frames, which it writes from d_dst + chain[0] on, and its frame scan writes chain[1] after waiting for
+    // chain_wait (that of the batch before: its ZkEncodeWs::ev_chain; nullptr: none).  dst_cap bounds the whole output
+    unsigned long long* chain = nullptr;
+    cudaEvent_t chain_wait = nullptr;
 };
 
 // The frames of a batch: the caller's sizes (each <= 1 GiB; 0: an empty frame), or the uniform layout of n bytes (frame_size bytes each, the
