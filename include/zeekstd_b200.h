@@ -43,6 +43,7 @@ extern "C" {
 #define ZK_SEEKABLE_MAX_FRAME_SIZE 0x40000000u
 #define ZK_SKIPPABLE_HEADER_SIZE 8u
 #define ZK_DEFAULT_FRAME_SIZE 0x200000u /* FrameSizePolicy::default(), encode.rs:33-39 */
+#define ZK_PATCH_SLICES_MAGIC 0x184D2A5Bu /* the skippable frame of a seekable patch's slices (zk_patch_slices_write) */
 
 /* Compression levels (the `level` argument of every compress entry point and of zk_encode_options_compression_level), as in libzstd:
  *   0                 the default, level 3;
@@ -77,6 +78,8 @@ void zk_ctx_destroy(zk_ctx* ctx);
 uint64_t zk_ctx_kernel_launches(const zk_ctx* ctx);
 /* number of execution segments (independent runs of blocks of a seek-table entry) the decoder has run so far */
 uint64_t zk_ctx_decode_segments(const zk_ctx* ctx);
+/* prefix bytes this context has copied to the device so far, by every call that takes a prefix */
+uint64_t zk_ctx_prefix_bytes_uploaded(const zk_ctx* ctx);
 /* kernel-only device time (ms, CUDA events on the context's stream) of the most recent batch call */
 float zk_ctx_last_device_ms(const zk_ctx* ctx);
 const char* zk_version(void);
@@ -268,7 +271,10 @@ int32_t zk_compress_frames_sized_long_dev(zk_ctx* ctx, const void* d_src, const 
  * zk_decompress_frames_prefixes decodes entry e (every zstd frame in it) against prefix[ranges[2e] .. ranges[2e+1]): exactly as
  * zk_decompress_frames_prefix decodes that entry alone with its range as the prefix, d_need, checksum verification and every error code
  * included (an offset that reaches before the start of the entry's range is -20, corruption_detected).  ranges == NULL: every entry
- * against the whole buffer, which is zk_decompress_frames_prefix.  Range checks as above.  HOST pointers.
+ * against the whole buffer, which is zk_decompress_frames_prefix.  With ranges, only the hull of the non-empty ranges of the entries it
+ * decodes goes to the device, in groups of consecutive entries whose hull is at most 1 GiB, so the buffer may be of any size (host
+ * memory, mmapped files included) and only a single range is limited to 2^31 - 1 bytes; a range with lo > hi or hi > prefix_len returns
+ * ZK_ERR_INVALID_ARG.  HOST pointers.
  */
 int32_t zk_compress_frames_sized_prefixes(zk_ctx* ctx, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
                                           int32_t checksum, const uint8_t* prefix, size_t prefix_len, const uint64_t* ranges,
@@ -276,6 +282,37 @@ int32_t zk_compress_frames_sized_prefixes(zk_ctx* ctx, const uint8_t* src, const
 int32_t zk_decompress_frames_prefixes(zk_ctx* ctx, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n_frames,
                                       uint8_t* dst, const uint32_t* d_need, int32_t verify_checksum, int32_t* status,
                                       const uint8_t* prefix, size_t prefix_len, const uint64_t* ranges);
+
+/*
+ * Seekable patches (DESIGN §3.4): every frame of NEW matched against the slice of OLD that holds its content, so OLD may be of any size, a
+ * frame's offsets never exceed 2^27 (a default libzstd DCtx restores it with ZSTD_DCtx_refPrefix(OLD[lo, hi))), and one frame restores
+ * from its slice alone.
+ *   zk_patch_ranges: frame f covers the next frame_sizes[f] bytes of new_src -> its slice [ranges[2f], ranges[2f+1]) of old.  The slices are
+ *     a pure function of old, new, the frame sizes and margin (not of how the work is split): an anchor is a position p >= 63 whose gear hash
+ *     of the 64 bytes ending at p (the hash of zk_compress_frames_cdc) is >= 2^64 - floor((2^64 - 1) / 65536); each anchor c of frame
+ *     f = [a, b) takes OLD's anchor of the same hash nearest to c (the lower on a tie); with (c1, o1) the first match and (c2, o2) the last,
+ *     the slice is [o1 - (c1 - a) - margin, o2 + (b - c2) + margin) when o2 >= o1 and |(o2 - o1) - (c2 - c1)| <= b - a, else
+ *     [o1 - (c1 - a) - margin, o1 + (b - c1) + margin); with no match [a - margin, b + margin); clamped to [0, old_len) and then cut to at
+ *     most 2^27 - (b - a) bytes around (o1 + o2) / 2 (o1 for a move; without a match, the clamped slice's centre).  old_len and margin
+ *     below 2^62.  Both buffers in HOST memory (old may be mmapped); they stream through the device in pieces of at most 1 GiB.
+ *   zk_compress_frames_patch: frame f is exactly what zk_compress_frames_sized_prefixes(ldm = 1) writes for frame f alone with old as the
+ *     buffer and its range (level 16's tier; an empty range: level 16's frame without a prefix).  Consecutive frames whose ranges' hull is
+ *     at most 1 GiB run as one such call on that hull of old, so old may be of any size.  Argument errors as in the sized call; a range
+ *     with lo > hi or hi > old_len returns ZK_ERR_INVALID_ARG.
+ *   The archive records the slices in one skippable frame at the start of entry 0 (its compressed size includes it):
+ *     u32 ZK_PATCH_SLICES_MAGIC, u32 payload size, "ZKSLICE1", u64 old_len, u32 n, n x (u64 lo, u64 hi), little-endian.
+ *   zk_patch_slices_write writes it (zk_patch_slices_size(n) bytes; a short dst_cap is -70); zk_patch_slices_read parses it from the start
+ *     of src and validates every field: the magic, the payload size, the tag, n == n_frames (the seek table's frame count), lo <= hi <=
+ *     old_len; anything else is ZK_ERR_INVALID_ARG.  ranges (2 n_frames) may be NULL; *frame_len: the frame's bytes.
+ */
+int32_t zk_patch_ranges(zk_ctx* ctx, const uint8_t* new_src, const uint32_t* frame_sizes, uint32_t n_frames, const uint8_t* old,
+                        uint64_t old_len, uint64_t margin, uint64_t* ranges);
+int32_t zk_compress_frames_patch(zk_ctx* ctx, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                 int32_t checksum, const uint8_t* old, uint64_t old_len, const uint64_t* ranges, uint8_t* dst, size_t dst_cap,
+                                 uint32_t* c_sizes, size_t* dst_len);
+size_t zk_patch_slices_size(uint32_t n_frames);
+int32_t zk_patch_slices_write(uint64_t old_len, const uint64_t* ranges, uint32_t n_frames, uint8_t* dst, size_t dst_cap, size_t* written);
+int32_t zk_patch_slices_read(const uint8_t* src, size_t len, uint32_t n_frames, uint64_t* old_len, uint64_t* ranges, size_t* frame_len);
 
 /*
  * The content-defined cut alone (FrameSizePolicy::ContentDefined(size), the rule of zk_compress_frames_cdc): frame_sizes, *n_frames and
@@ -438,6 +475,10 @@ int32_t zk_decoder_decompress(zk_decoder* d, uint8_t* buf, size_t len, size_t* p
 /* Decoder::decompress_with_prefix: every frame is decoded against the raw-content prefix (decode.rs:211-214, 246-255) */
 int32_t zk_decoder_decompress_with_prefix(zk_decoder* d, uint8_t* buf, size_t len, const uint8_t* prefix,
                                           size_t prefix_len, size_t* produced);            /* :201-270 */
+/* the same with entry e decoded against prefix[ranges[2e] .. ranges[2e+1]) (ranges: two per seek-table entry, as zk_decompress_frames_prefixes
+ * takes them): a seekable patch read with its slices; each window of frames uploads only the hull of its own entries' ranges */
+int32_t zk_decoder_decompress_with_prefix_ranges(zk_decoder* d, uint8_t* buf, size_t len, const uint8_t* prefix, size_t prefix_len,
+                                                 const uint64_t* ranges, size_t* produced);
 void zk_decoder_reset(zk_decoder* d);                                                    /* :346-350 */
 int32_t zk_decoder_set_lower_frame(zk_decoder* d, uint32_t index, uint64_t* offset);    /* :367 */
 int32_t zk_decoder_set_upper_frame(zk_decoder* d, uint32_t index, uint64_t* offset);    /* :383 */

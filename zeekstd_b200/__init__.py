@@ -291,6 +291,91 @@ class Context:
         return out[:total], st[:nf], rc
 
 
+    # ---- seekable patches ------------------------------------------------------------------------
+    @property
+    def prefix_bytes_uploaded(self) -> int:
+        """prefix bytes this context has copied to the device so far (zk_ctx_prefix_bytes_uploaded)"""
+        return int(self.lib.zk_ctx_prefix_bytes_uploaded(self._h))
+
+    def patch_ranges(self, new, frame_sizes, old, margin: int | None = None) -> np.ndarray:
+        """the slice of `old` each frame of `new` is matched against in a seekable patch -> n x 2 np.uint64 (lo, hi), found on the GPU by
+        content anchors (the rule: include/zeekstd_b200.h, zk_patch_ranges).  margin: bytes added on each side (default: the largest frame
+        size, which is the frame size of uniform frames)"""
+        addr, n, keep = _buf(new)
+        ds = np.ascontiguousarray(frame_sizes, dtype=np.uint32).reshape(-1)
+        if int(np.sum(ds, dtype=np.uint64)) != n:
+            raise ValueError(f"frame sizes add up to {int(np.sum(ds, dtype=np.uint64))} bytes, the input has {n}")
+        oaddr, on, okeep = _buf(old)
+        m = int(ds.max()) if margin is None and ds.size else int(margin or 0)
+        rg = np.zeros((max(ds.size, 1), 2), dtype=np.uint64)
+        _check(self.lib.zk_patch_ranges(self._h, addr, ds.ctypes.data_as(_native.u32p), ds.size, oaddr, on, m,
+                                        rg.ctypes.data_as(_native.u64p)), self.lib)
+        return rg[: ds.size]
+
+    def compress_frames_patch(self, new, frame_sizes, old, ranges, level: int = 0, checksum: bool = False):
+        """frame f of `new` against old[ranges[f][0]:ranges[f][1]] with long-distance matching, for an `old` of any size
+        (zk_compress_frames_patch) -> (compressed bytes (np.uint8), c_sizes, d_sizes).  Frame f is what compress_frames_sized(frame alone,
+        prefix=old, long_distance=True, prefix_ranges=[ranges[f]]) writes"""
+        addr, n, keep = _buf(new)
+        ds = np.ascontiguousarray(frame_sizes, dtype=np.uint32).reshape(-1)
+        if int(np.sum(ds, dtype=np.uint64)) != n:
+            raise ValueError(f"frame sizes add up to {int(np.sum(ds, dtype=np.uint64))} bytes, the input has {n}")
+        oaddr, on, okeep = _buf(old)
+        rg = _ranges(ranges, ds.size)
+        dsp = ds.ctypes.data_as(_native.u32p)
+        cap = self.lib.zk_compress_bound_sized(dsp, ds.size)
+        dst = np.empty(cap + 64, dtype=np.uint8)
+        cs = np.zeros(max(ds.size, 1), dtype=np.uint32)
+        dl = c_size_t()
+        _check(self.lib.zk_compress_frames_patch(self._h, addr, dsp, ds.size, level, int(checksum), oaddr, on, rg.ctypes.data_as(_native.u64p),
+                                                 dst.ctypes.data, cap, cs.ctypes.data_as(_native.u32p), byref(dl)), self.lib)
+        return dst[: dl.value], cs[: ds.size], ds.copy()
+
+    def compress_patch_slices(self, new, frame_sizes, old, level: int = 0, checksum: bool = False, margin: int | None = None) -> bytes:
+        """a seekable patch of `new` against `old` -> the archive's bytes: the slice frame (the ranges of patch_ranges), then the frames
+        of compress_frames_patch, then the Foot seek table.  Entry 0's compressed size includes the slice frame."""
+        ds = np.ascontiguousarray(frame_sizes, dtype=np.uint32).reshape(-1)
+        if ds.size == 0:
+            raise ValueError("a seekable patch has at least one frame")
+        rg = self.patch_ranges(new, ds, old, margin)
+        comp, cs, _ = self.compress_frames_patch(new, ds, old, rg, level, checksum)
+        head = patch_slices_write(_buf(old)[1], rg, self.lib)
+        table = SeekTable(lib=self.lib)
+        for f, (c, d) in enumerate(zip(cs.tolist(), ds.tolist())):
+            table.log_frame(c + (len(head) if f == 0 else 0), d)
+        return head + comp.tobytes() + table.into_serializer().to_bytes()
+
+
+PATCH_SLICES_MAGIC = 0x184D2A5B
+
+
+def patch_slices_size(n_frames: int) -> int:
+    """bytes of the slice frame of a seekable patch of n_frames frames"""
+    return 28 + 16 * n_frames
+
+
+def patch_slices_read(buf, n_frames: int, lib=None):
+    """the slice frame at the start of a seekable patch's first entry -> (old_len, ranges (n_frames x 2 np.uint64), frame length).  Raises
+    Error (ZK_ERR_INVALID_ARG) for anything that is not a valid slice frame of n_frames slices (zk_patch_slices_read)"""
+    lib = lib or _native.default_lib()
+    addr, n, keep = _buf(buf)
+    rg = np.zeros((max(n_frames, 1), 2), dtype=np.uint64)
+    ol = c_uint64(); fl = c_size_t()
+    _check(lib.zk_patch_slices_read(addr, n, n_frames, byref(ol), rg.ctypes.data_as(_native.u64p), byref(fl)), lib)
+    return int(ol.value), rg[:n_frames], int(fl.value)
+
+
+def patch_slices_write(old_len: int, ranges, lib=None) -> bytes:
+    """the slice frame of a seekable patch whose frames have these (lo, hi) ranges of an OLD of old_len bytes (zk_patch_slices_write)"""
+    lib = lib or _native.default_lib()
+    rg = np.ascontiguousarray(np.asarray(ranges, dtype=np.uint64).reshape(-1, 2))
+    out = np.zeros(lib.zk_patch_slices_size(len(rg)), dtype=np.uint8)
+    w = c_size_t()
+    _check(lib.zk_patch_slices_write(old_len, rg.ctypes.data_as(_native.u64p) if rg.size else None, len(rg), out.ctypes.data, out.size,
+                                     byref(w)), lib)
+    return out[: w.value].tobytes()
+
+
 def _ranges(prefix_ranges, n: int) -> np.ndarray:
     """n (lo, hi) prefix ranges -> a C-contiguous n x 2 np.uint64 array"""
     rg = np.asarray(prefix_ranges)
@@ -700,8 +785,10 @@ class Decoder(io.RawIOBase):
         _check(self.lib.zk_decoder_decompress(self._h, arr, len(mv), byref(p)), self.lib)
         return int(p.value)
 
-    def decompress_with_prefix(self, buf, prefix=None) -> int:
-        """decode.rs:201-270: every frame is decoded against the raw-content prefix"""
+    def decompress_with_prefix(self, buf, prefix=None, ranges=None) -> int:
+        """decode.rs:201-270: every frame is decoded against the raw-content prefix.  ranges (one (lo, hi) pair per seek-table entry): entry
+        e is decoded against prefix[lo:hi] only, and only the slices of the frames read go to the device (a seekable patch,
+        zk_decoder_decompress_with_prefix_ranges)"""
         if prefix is None:
             return self.decompress(buf)
         mv = memoryview(buf)
@@ -711,7 +798,13 @@ class Decoder(io.RawIOBase):
         paddr, pn, pkeep = _buf(prefix)
         self._prefix_keep = pkeep
         p = c_size_t()
-        _check(self.lib.zk_decoder_decompress_with_prefix(self._h, arr, len(mv), paddr, pn, byref(p)), self.lib)
+        if ranges is None:
+            _check(self.lib.zk_decoder_decompress_with_prefix(self._h, arr, len(mv), paddr, pn, byref(p)), self.lib)
+        else:
+            if getattr(self, "_ranges_src", None) is not ranges:    # the same array on every call keeps the decoded window valid
+                self._ranges_src, self._ranges = ranges, _ranges(ranges, self.seek_table().num_frames())
+            _check(self.lib.zk_decoder_decompress_with_prefix_ranges(self._h, arr, len(mv), paddr, pn, self._ranges.ctypes.data_as(_native.u64p),
+                                                                     byref(p)), self.lib)
         return int(p.value)
 
     def readable(self): return True

@@ -1,6 +1,6 @@
 """Command-line front end with the reference CLI's arguments and behaviour (SURVEY.md 8f.4), over the GPU codec.
 
-    python -m zeekstd_b200 [compress] [-l N] [-s 2M] [--frame-size-policy ..] [--patch-from F [--long]] [--long-mode] [--reuse-from OLD.zst]
+    python -m zeekstd_b200 [compress] [-l N] [-s 2M] [--frame-size-policy ..] [--patch-from F [--long | --patch-slices]] [--long-mode] [--reuse-from OLD.zst]
                            [INPUT] [-o OUT]
     python -m zeekstd_b200 decompress [--from N | --from-frame I] [--to N|end | --to-frame I|end] [--patch-apply F] INPUT [-o OUT]
     python -m zeekstd_b200 list [--from-frame I] [--to-frame I|end | --num-frames N] [-d] [--seek-table-format head|foot] INPUT
@@ -23,6 +23,9 @@ extension of this codec) ends frames where a rolling hash of the data says so, a
 of the input changes only the frames around it and rsync, dedup stores and range-fetching clients can reuse the rest.
 `--reuse-from OLD.zst` (an extension of this codec) compresses a new version against the archive of the previous one: every frame
 whose bytes a frame of OLD.zst holds is copied from it, only the others are compressed; with `uncompressed` or `content` frames.
+`--patch-from F --patch-slices` (an extension of this codec) writes a seekable patch against an F of any size: every frame is matched
+against its own slice of F, found by content anchors and recorded in a skippable frame at the start of the archive, and `decompress
+--patch-apply F` reads only the slices of the frames it restores.
 """
 from __future__ import annotations
 
@@ -160,6 +163,12 @@ def build_parser() -> argparse.ArgumentParser:
                    help="Match every frame also against its own bytes up to 128 MiB back (zstd --long), and with --patch-from against the "
                         "whole reference file as --long does: large frames find far repeats. Every compression level then runs as level 16; "
                         "needs --frame-size-policy uncompressed.")
+    c.add_argument("--patch-slices", action="store_true",
+                   help="With --patch-from: a seekable patch. Every frame is matched against its own slice of the reference file, found by "
+                        "content anchors, so the file may be of any size and one frame restores from its slice alone. Implies long-distance "
+                        "matching (level 16's tier); needs --frame-size-policy uncompressed or content.")
+    c.add_argument("--patch-margin", type=byte_value, default=None,
+                   help="With --patch-slices: bytes added on each side of a frame's slice (default: the frame size).")
     c.add_argument("--reuse-from", default=None, metavar="OLD.zst",
                    help="The archive of a previous version of the input (ending in its seek table): every frame whose bytes one of its "
                         "frames already holds is copied from it, only the others are compressed. The output is what compress writes "
@@ -338,6 +347,19 @@ def _run_compress(zk, ns, fmt_bytes) -> int:
         raise CliError("--long needs --frame-size-policy uncompressed")
     if ns.long_mode and ns.frame_size_policy in ("compressed", "content"):
         raise CliError("--long-mode needs --frame-size-policy uncompressed")
+    if ns.patch_slices:
+        if not ns.patch_from:
+            raise CliError("--patch-slices needs --patch-from: the slices are taken from the reference file")
+        if ns.frame_size_policy == "compressed":
+            raise CliError("--patch-slices needs --frame-size-policy uncompressed or content")
+        if ns.long_mode:
+            raise CliError("--patch-slices cannot be used with --long-mode: a frame is matched against its slice of the reference file only")
+        if ns.reuse_from is not None:
+            raise CliError("--patch-slices cannot be used with --reuse-from: a copied frame must depend on its own bytes alone")
+        if ns.frame_size == 0:
+            raise CliError("--patch-slices needs a frame size above 0")
+    elif ns.patch_margin is not None:
+        raise CliError("--patch-margin needs --patch-slices")
     if ns.reuse_from is not None:
         if ns.patch_from:
             raise CliError("--reuse-from cannot be used with --patch-from: a copied frame must depend on its own bytes alone")
@@ -358,6 +380,8 @@ def _run_compress(zk, ns, fmt_bytes) -> int:
 
     if ns.reuse_from is not None:
         return _run_compress_reuse(zk, ns, fmt_bytes, reader, writer, in_path, out_path, st_file)
+    if ns.patch_slices:
+        return _run_compress_slices(zk, ns, fmt_bytes, reader, writer, in_path, out_path, st_file)
     policy = {"compressed": zk.FrameSizePolicy.Compressed, "uncompressed": zk.FrameSizePolicy.Uncompressed,
               "content": zk.FrameSizePolicy.ContentDefined}[ns.frame_size_policy](ns.frame_size)
     enc = (zk.EncodeOptions().frame_size_policy(policy).checksum_flag(not ns.no_checksum)
@@ -405,6 +429,65 @@ def _load_whole(path, what: str):
         return np.fromfile(path, dtype=np.uint8)
     except OSError as e:
         raise CliError(f"Failed to read {what}: {e}")
+
+
+def _policy_sizes(zk, ctx, ns, data):
+    """the frame sizes the encoder's policy gives the whole input (uncompressed or content)"""
+    n = int(data.size)
+    if ns.frame_size_policy == "content":
+        return ctx.cut_frames_cdc(data, ns.frame_size)[0]
+    fs = min(ns.frame_size, zk.SEEKABLE_MAX_FRAME_SIZE)
+    sizes = np.full(n // fs, fs, dtype=np.uint32)
+    if n % fs or n == 0:
+        sizes = np.append(sizes, np.uint32(n % fs))
+    return sizes
+
+
+def _write_archive(zk, ns, writer, st_file, parts, table) -> int:
+    """the frames' bytes, then the seek table (Foot, or Head into its own file) -> bytes written"""
+    written = 0
+    for part in parts:
+        writer.write(part)
+        written += len(part)
+    if st_file is not None:
+        blob = table.into_format_serializer(zk.Format.Head).to_bytes()
+        st_file.write(blob)
+        st_file.close()
+    else:
+        blob = table.into_serializer().to_bytes()
+        writer.write(blob)
+    written += len(blob)
+    if writer is not sys.stdout.buffer:
+        writer.close()
+    else:
+        writer.flush()
+    return written
+
+
+def _run_compress_slices(zk, ns, fmt_bytes, reader, writer, in_path, out_path, st_file) -> int:
+    """compress with --patch-slices: the whole input in one seekable patch (Context.patch_ranges, Context.compress_frames_patch); entry 0
+    starts with the slice frame"""
+    if in_path is not None and os.path.isfile(in_path):
+        reader.close()
+        data = _load_whole(in_path, "input file")
+    else:
+        data = np.frombuffer(reader.read(), dtype=np.uint8)
+    old = _load_whole(ns.patch_from, "prefix (patch) file")
+    ctx = zk.default_context()
+    sizes = _policy_sizes(zk, ctx, ns, data)
+    margin = ns.frame_size if ns.patch_margin is None else ns.patch_margin
+    ranges = ctx.patch_ranges(data, sizes, old, margin)
+    comp, cs, _ = ctx.compress_frames_patch(data, sizes, old, ranges, ns.compression_level, not ns.no_checksum)
+    head = zk.patch_slices_write(int(old.size), ranges)
+    table = zk.SeekTable()
+    for f, (c, d) in enumerate(zip(cs.tolist(), sizes.tolist())):
+        table.log_frame(c + (len(head) if f == 0 else 0), d)
+    written = _write_archive(zk, ns, writer, st_file, [head, comp.tobytes()], table)
+    if not ns.quiet:
+        n = int(data.size)
+        ratio = 100.0 / n * written if n else float("nan")
+        sys.stderr.write(f"{in_path or 'STDIN'} : {ratio:.2f}% ( {fmt_bytes(n)} => {fmt_bytes(written)}, {out_path or 'STDOUT'})\n")
+    return 0
 
 
 def _run_compress_reuse(zk, ns, fmt_bytes, reader, writer, in_path, out_path, st_file) -> int:
@@ -486,19 +569,35 @@ def _run_decompress(zk, ns, fmt_bytes) -> int:
             limit = table.size_decomp() if ns.to is None else ns.to
     except zk.Error as e:
         raise CliError(f"Failed to get decompression offset limit: {e}")
+    # a seekable patch: entry 0 starts with the slice frame, which holds every frame's slice of the reference file
+    ranges = None
+    n_frames = table.num_frames()
+    if n_frames:
+        head = src.read(zk.patch_slices_size(n_frames))
+        src.seek(0)
+        if len(head) >= 4 and int.from_bytes(head[:4], "little") == zk.PATCH_SLICES_MAGIC:
+            if not ns.patch_apply:
+                raise CliError("this archive is a seekable patch; pass --patch-apply")
+            try:
+                old_len, ranges, _ = zk.patch_slices_read(head, n_frames)
+            except zk.Error as e:
+                raise CliError(f"Failed to read the slices of the seekable patch: {e}")
+            if prefix_len != old_len:
+                raise CliError(f"{ns.patch_apply} has {prefix_len} bytes, the seekable patch was made against {old_len} bytes")
     bar = _Progress(limit, fmt_bytes, not ns.quiet and not ns.no_progress, pos=offset)
     try:
         dec = zk.DecodeOptions(src).seek_table(table).offset(offset).offset_limit(limit).into_decoder()
     except zk.Error as e:
         raise CliError(f"Failed to create decoder: {e}")
-    prefix = _load_prefix(ns.patch_apply, _use_mmap(ns, prefix_len))
+    # the slices of a patch are read from a mapping: only those of the frames decoded are paged in
+    prefix = _load_prefix(ns.patch_apply, ranges is not None or _use_mmap(ns, prefix_len))
 
     buf = bytearray(OUT_CHUNK)
     view = memoryview(buf)
     written = 0
     while True:
         try:
-            n = dec.decompress_with_prefix(view, prefix)
+            n = dec.decompress_with_prefix(view, prefix, ranges)
         except zk.Error as e:
             raise CliError(f"Failed to decompress data: {e}")
         if n == 0:

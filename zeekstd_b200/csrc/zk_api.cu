@@ -145,6 +145,7 @@ extern "C" uint64_t zk_ctx_decode_segments(const zk_ctx* c) {
     return n;
 }
 extern "C" float zk_ctx_last_device_ms(const zk_ctx* c) { return c ? c->last_ms : 0.f; }
+extern "C" uint64_t zk_ctx_prefix_bytes_uploaded(const zk_ctx* c) { return c ? c->prefix_uploaded : 0; }
 extern "C" size_t zk_compress_bound(size_t n, uint32_t frame_size) { return zk_encode_bound(n, frame_size); }
 
 extern "C" void zk_ctx_profile(zk_ctx* c, int32_t enable) {
@@ -181,6 +182,7 @@ static int32_t zk_upload_prefix(zk_ctx* c, const uint8_t* prefix, size_t len, co
     if (rc) return rc;
     for (int i = 0; i < ZK_SLOTS; i++) if (c->slot[i].stream) cudaStreamSynchronize(c->slot[i].stream);    // nobody reads the old prefix any more
     ZK_CUDA_OK(cudaMemcpy(c->d_prefix, prefix, len, cudaMemcpyHostToDevice));
+    c->prefix_uploaded += len;
     *d_prefix = (const uint8_t*)c->d_prefix; *d_len = (uint32_t)len;
     return 0;
 }
@@ -333,11 +335,68 @@ extern "C" int32_t zk_decompress_frames_prefix(zk_ctx* c, const uint8_t* comp, c
     return zk_decompress_frames_prefixes(c, comp, c_off, d_off, n, dst, d_need, verify, status, prefix, prefix_len, nullptr);
 }
 
-// entry e decoded against its own range of the prefix buffer; ranges == NULL: every entry against the whole buffer
+// ZK_PATCH_GROUP_BYTES (tests; default 1 GiB): the most prefix bytes one group of entries of the ranged calls uploads at once
+static uint64_t zk_patch_group_bytes() { return zk_env_size("ZK_PATCH_GROUP_BYTES", (size_t)1 << 30); }
+
+// The ranged calls work on groups of consecutive entries: from f0 on, as many as keep the hull of their non-empty ranges within `group`
+// bytes, at least one -> the group's end; *hlo, *hhi: the hull (equal: every range of the group is empty)
+static uint32_t zk_hull_group(const uint64_t* ranges, uint32_t f0, uint32_t n, uint64_t group, uint64_t* hlo, uint64_t* hhi) {
+    uint64_t lo = 0, hi = 0;
+    bool any = false;
+    uint32_t f = f0;
+    for (; f < n; f++) {
+        const uint64_t a = ranges[2 * (size_t)f], b = ranges[2 * (size_t)f + 1];
+        if (a == b) continue;
+        const uint64_t nlo = any && lo < a ? lo : a, nhi = any && hi > b ? hi : b;
+        if (f > f0 && any && nhi - nlo > group) break;
+        lo = nlo; hi = nhi; any = true;
+    }
+    *hlo = lo; *hhi = hi;
+    return f;
+}
+// the ranges of entries [f0, end) rebased to the hull that starts at hlo (an empty range becomes (0, 0))
+static void zk_rebase_ranges(const uint64_t* ranges, uint32_t f0, uint32_t end, uint64_t hlo, std::vector<uint64_t>* out) {
+    out->assign(2 * (size_t)(end - f0), 0);
+    for (uint32_t f = f0; f < end; f++) {
+        const uint64_t a = ranges[2 * (size_t)f], b = ranges[2 * (size_t)f + 1];
+        if (a != b) { (*out)[2 * (size_t)(f - f0)] = a - hlo; (*out)[2 * (size_t)(f - f0) + 1] = b - hlo; }
+    }
+}
+
+static int32_t zk_decompress_prefixes_one(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n, uint8_t* dst,
+                                          const uint32_t* d_need, int32_t verify, int32_t* status, const uint8_t* prefix, size_t prefix_len,
+                                          const uint64_t* ranges);
+
+// entry e decoded against its own range of the prefix buffer; ranges == NULL: every entry against the whole buffer.  With ranges, the
+// entries run in groups (zk_hull_group), each with only the hull of its ranges on the device, so the buffer may be of any size
 extern "C" int32_t zk_decompress_frames_prefixes(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n,
                                                  uint8_t* dst, const uint32_t* d_need, int32_t verify, int32_t* status,
                                                  const uint8_t* prefix, size_t prefix_len, const uint64_t* ranges) {
     if (!c) return ZK_ERR_INVALID_ARG;
+    if (!ranges || !prefix || prefix_len == 0)
+        return zk_decompress_prefixes_one(c, comp, c_off, d_off, n, dst, d_need, verify, status, prefix, prefix_len, ranges);
+    for (uint32_t i = 0; i < n; i++)
+        if (ranges[2 * (size_t)i] > ranges[2 * (size_t)i + 1] || ranges[2 * (size_t)i + 1] > prefix_len) return ZK_ERR_INVALID_ARG;
+    if (n && (!comp || !c_off || !d_off || !dst)) return ZK_ERR_INVALID_ARG;
+    const uint64_t group = zk_patch_group_bytes();
+    std::vector<uint64_t> rb;
+    int32_t worst = 0;
+    for (uint32_t f0 = 0; f0 < n;) {
+        uint64_t hlo, hhi;
+        const uint32_t end = zk_hull_group(ranges, f0, n, group, &hlo, &hhi);
+        zk_rebase_ranges(ranges, f0, end, hlo, &rb);
+        const int32_t rc = zk_decompress_prefixes_one(c, comp, c_off + f0, d_off + f0, end - f0, dst, d_need ? d_need + f0 : nullptr, verify,
+                                                      status ? status + f0 : nullptr, prefix + hlo, (size_t)(hhi - hlo), rb.data());
+        if (rc && !ZK_IS_ZSTD_ERR(rc)) return rc;         // the call failed; a frame's status does not stop the other groups
+        if (rc && !worst) worst = rc;
+        f0 = end;
+    }
+    return worst;
+}
+
+static int32_t zk_decompress_prefixes_one(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n, uint8_t* dst,
+                                          const uint32_t* d_need, int32_t verify, int32_t* status, const uint8_t* prefix, size_t prefix_len,
+                                          const uint64_t* ranges) {
     ZkDecCall q = {comp, c_off, d_off, dst, verify, status, ZkDecodeParams()};
     std::vector<uint32_t> rw;
     int32_t rc = zk_prefix_ranges(ranges, n, prefix_len, &rw);
@@ -1127,5 +1186,130 @@ extern "C" int32_t zk_compress_frames_sized_reuse(zk_ctx* c, const uint8_t* src,
     }
     if (dst_len) *dst_len = out_pos;
     if (trace) fprintf(stderr, "reuse index %.3f match %.3f compress %.3f assemble %.3f ms\n", t_index, t_match, t_comp, t_asm);
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Seekable patches (DESIGN §3.4): every frame of NEW against the slice of OLD its content anchors point at (zk_patch.inc), for an OLD of any
+// size.  OLD and NEW stream through slot 0 in pieces; only the anchor tables and one group's hull of OLD are ever on the device.
+// ---------------------------------------------------------------------------------------------
+// ZK_PATCH_PIECE_BYTES (tests; default 1 GiB): the bytes of OLD or NEW one anchor pass uploads; pieces overlap by 63 bytes
+static size_t zk_patch_piece_bytes() {
+    const size_t v = zk_env_size("ZK_PATCH_PIECE_BYTES", (size_t)1 << 30);
+    return v < 4096 ? 4096 : (v > ((size_t)1 << 30) ? (size_t)1 << 30 : v);
+}
+
+// the anchors of len bytes of host memory, piece by piece on slot 0
+static int32_t zk_patch_scan(zk_ctx* c, const uint8_t* src, uint64_t len, std::vector<unsigned long long>* keys,
+                             std::vector<unsigned long long>* pos) {
+    ZkSlot& s = c->slot[0];
+    const size_t piece = zk_patch_piece_bytes();
+    for (uint64_t s0 = 0; s0 < len;) {
+        const uint64_t e = len - s0 < piece ? len : s0 + piece;
+        const size_t n = (size_t)(e - s0);
+        int32_t rc = zk_slot_ensure(&s, n + 32, 0);
+        if (rc) return rc;
+        ZK_CUDA_OK(cudaMemcpyAsync(s.d_in, src + s0, n, cudaMemcpyHostToDevice, s.stream));
+        if ((rc = zk_patch_anchors(&s.ews, s.stream, s.d_in, n, s0, keys, pos))) return rc;
+        if (e == len) break;
+        s0 = e - 63;                                          // the next piece's first anchor is at e: its hash needs the 63 bytes before
+    }
+    return 0;
+}
+
+extern "C" int32_t zk_patch_ranges(zk_ctx* c, const uint8_t* new_src, const uint32_t* frame_sizes, uint32_t n_frames, const uint8_t* old,
+                                   uint64_t old_len, uint64_t margin, uint64_t* ranges) {
+    if (!c || (n_frames && (!frame_sizes || !ranges)) || (old_len && !old)) return ZK_ERR_INVALID_ARG;
+    if (old_len >= (1ull << 62) || margin >= (1ull << 62)) return ZK_ERR_INVALID_ARG;
+    ZkPatchTables t;
+    t.fa.assign((size_t)n_frames + 1, 0);
+    for (uint32_t f = 0; f < n_frames; f++) t.fa[f + 1] = t.fa[f] + frame_sizes[f];
+    const uint64_t n = t.fa[n_frames];
+    if (n && !new_src) return ZK_ERR_INVALID_ARG;
+    if (n_frames == 0) return 0;
+    ZK_CUDA_OK(cudaSetDevice(c->device));
+    int32_t rc = zk_patch_scan(c, old, old_len, &t.okeys, &t.opos);
+    if (!rc) rc = zk_patch_scan(c, new_src, n, &t.nkeys, &t.npos);
+    if (rc) return rc;
+    if (t.okeys.size() > 0xFFFFFFF0ull || t.nkeys.size() > 0xFFFFFFF0ull) return ZK_ERR_INVALID_ARG;
+    t.fanc.assign((size_t)n_frames + 1, 0);
+    for (uint32_t f = 0, i = 0; f <= n_frames; f++) {
+        while (i < t.npos.size() && t.npos[i] < t.fa[f]) i++;
+        t.fanc[f] = f == n_frames ? (uint32_t)t.npos.size() : i;
+    }
+    return zk_patch_join(&c->slot[0].ews, c->slot[0].stream, t, n_frames, old_len, margin, (unsigned long long*)ranges);
+}
+
+// frames of NEW against their ranges of OLD, in groups of consecutive frames whose hull of OLD is at most ZK_PATCH_GROUP_BYTES: each group is one
+// zk_compress_frames_sized_prefixes call (ldm = 1) on its hull, with the ranges rebased, so no frame's bytes depend on the grouping.  A group
+// whose ranges are all empty is level 16's plain frames, which is what that call writes for a frame with an empty range.
+extern "C" int32_t zk_compress_frames_patch(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                            int32_t checksum, const uint8_t* old, uint64_t old_len, const uint64_t* ranges, uint8_t* dst,
+                                            size_t dst_cap, uint32_t* c_sizes, size_t* dst_len) {
+    if (!c || (n_frames && (!frame_sizes || !ranges || !dst)) || (old_len && !old)) return ZK_ERR_INVALID_ARG;
+    if (dst_len) *dst_len = 0;
+    for (uint32_t f = 0; f < n_frames; f++)
+        if (ranges[2 * (size_t)f] > ranges[2 * (size_t)f + 1] || ranges[2 * (size_t)f + 1] > old_len) return ZK_ERR_INVALID_ARG;
+    const uint64_t group = zk_patch_group_bytes();
+    std::vector<uint64_t> rb;
+    std::vector<uint32_t> cs(n_frames);
+    size_t out = 0, in = 0;
+    for (uint32_t f0 = 0; f0 < n_frames;) {
+        uint64_t hlo, hhi;
+        const uint32_t end = zk_hull_group(ranges, f0, n_frames, group, &hlo, &hhi);
+        zk_rebase_ranges(ranges, f0, end, hlo, &rb);
+        size_t len = 0, bytes = 0;
+        for (uint32_t f = f0; f < end; f++) bytes += frame_sizes[f];
+        const int32_t rc = hhi > hlo
+            ? zk_compress_frames_sized_prefixes(c, src ? src + in : nullptr, frame_sizes + f0, end - f0, level, checksum, old + hlo, (size_t)(hhi - hlo),
+                                                rb.data(), 1, 0, dst + out, dst_cap - out, cs.data() + f0, &len)
+            : zk_compress_frames_sized(c, src ? src + in : nullptr, frame_sizes + f0, end - f0, 16, checksum, nullptr, 0, dst + out,
+                                       dst_cap - out, cs.data() + f0, &len);
+        if (rc) return rc;
+        out += len; in += bytes; f0 = end;
+    }
+    if (c_sizes && n_frames) memcpy(c_sizes, cs.data(), (size_t)n_frames * 4);
+    if (dst_len) *dst_len = out;
+    return 0;
+}
+
+// the slice frame (a skippable frame at the start of entry 0): magic, payload size, "ZKSLICE1", u64 old_len, u32 n, n x (u64 lo, u64 hi)
+static const uint8_t zk_slice_tag[8] = {'Z', 'K', 'S', 'L', 'I', 'C', 'E', '1'};
+static void zk_put_le(uint8_t* p, uint64_t v, int bytes) { for (int i = 0; i < bytes; i++) p[i] = (uint8_t)(v >> (8 * i)); }
+static uint64_t zk_get_le(const uint8_t* p, int bytes) { uint64_t v = 0; for (int i = 0; i < bytes; i++) v |= (uint64_t)p[i] << (8 * i); return v; }
+
+extern "C" size_t zk_patch_slices_size(uint32_t n_frames) { return 8 + 20 + 16 * (size_t)n_frames; }
+
+extern "C" int32_t zk_patch_slices_write(uint64_t old_len, const uint64_t* ranges, uint32_t n_frames, uint8_t* dst, size_t dst_cap,
+                                         size_t* written) {
+    if ((n_frames && !ranges) || !dst || n_frames > ZK_SEEKABLE_MAX_FRAMES) return ZK_ERR_INVALID_ARG;
+    for (uint32_t f = 0; f < n_frames; f++)
+        if (ranges[2 * (size_t)f] > ranges[2 * (size_t)f + 1] || ranges[2 * (size_t)f + 1] > old_len) return ZK_ERR_INVALID_ARG;
+    const size_t total = zk_patch_slices_size(n_frames);
+    if (dst_cap < total) return ZK_ERR_ZSTD(ZKZ_DST_TOO_SMALL);
+    zk_put_le(dst, ZK_PATCH_SLICES_MAGIC, 4);
+    zk_put_le(dst + 4, total - 8, 4);
+    memcpy(dst + 8, zk_slice_tag, 8);
+    zk_put_le(dst + 16, old_len, 8);
+    zk_put_le(dst + 24, n_frames, 4);
+    for (size_t i = 0; i < 2 * (size_t)n_frames; i++) zk_put_le(dst + 28 + 8 * i, ranges[i], 8);
+    if (written) *written = total;
+    return 0;
+}
+
+extern "C" int32_t zk_patch_slices_read(const uint8_t* src, size_t len, uint32_t n_frames, uint64_t* old_len, uint64_t* ranges,
+                                        size_t* frame_len) {
+    if (!src || len < 28 || n_frames > ZK_SEEKABLE_MAX_FRAMES) return ZK_ERR_INVALID_ARG;
+    const size_t total = zk_patch_slices_size(n_frames);
+    if (zk_get_le(src, 4) != ZK_PATCH_SLICES_MAGIC || zk_get_le(src + 4, 4) != total - 8 || len < total) return ZK_ERR_INVALID_ARG;
+    if (memcmp(src + 8, zk_slice_tag, 8) != 0 || zk_get_le(src + 24, 4) != n_frames) return ZK_ERR_INVALID_ARG;
+    const uint64_t ol = zk_get_le(src + 16, 8);
+    for (uint32_t f = 0; f < n_frames; f++) {
+        const uint64_t lo = zk_get_le(src + 28 + 16 * (size_t)f, 8), hi = zk_get_le(src + 36 + 16 * (size_t)f, 8);
+        if (lo > hi || hi > ol) return ZK_ERR_INVALID_ARG;
+        if (ranges) { ranges[2 * (size_t)f] = lo; ranges[2 * (size_t)f + 1] = hi; }
+    }
+    if (old_len) *old_len = ol;
+    if (frame_len) *frame_len = total;
     return 0;
 }

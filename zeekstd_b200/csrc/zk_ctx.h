@@ -25,6 +25,7 @@ struct zk_ctx {
     cudaStream_t up = nullptr, down = nullptr;            // dedicated copy streams of the host-pointer decompress pipeline
     float last_ms = 0.f;
     void* d_prefix = nullptr; size_t cap_prefix = 0;      // device copy of the raw-content prefix of the calls that take one
+    unsigned long long prefix_uploaded = 0;               // prefix bytes copied to the device so far (zk_ctx_prefix_bytes_uploaded)
     void* d_reuse[4] = {}; size_t cap_reuse[4] = {};      // zk_compress_frames_sized_reuse: old entries, their decoded bytes, the changed
                                                           // frames, the assembled output
     unsigned long long launches() const {

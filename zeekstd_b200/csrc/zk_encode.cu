@@ -1603,6 +1603,7 @@ void zk_encode_ws_free(ZkEncodeWs* ws) {
     if (ws->buf) cudaFree(ws->buf);
     if (ws->cut) cudaFree(ws->cut);
     if (ws->reuse) cudaFree(ws->reuse);
+    if (ws->patch) cudaFree(ws->patch);
     if (ws->h_sizes) cudaFreeHost(ws->h_sizes);
     if (ws->side) cudaStreamDestroy(ws->side);
     if (ws->ev_a) cudaEventDestroy(ws->ev_a);
@@ -2000,3 +2001,4 @@ int zk_encode_cdc(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, siz
 }
 
 #include "zk_reuse.inc"
+#include "zk_patch.inc"

@@ -1,11 +1,13 @@
 // zk_encode.h -- host-visible interface of the batched compress path (zk_encode.cu).
 #pragma once
 #include "zk_common.cuh"
+#include <vector>
 
 struct ZkEncodeWs {                    // HBM scratch owned by a zk_ctx slot, grown on demand
     void* buf = nullptr; size_t cap = 0;
     void* cut = nullptr; size_t cut_cap = 0;              // content-defined cut (zk_encode_cdc): kept apart from buf, which the frames of a cut then use
     void* reuse = nullptr; size_t reuse_cap = 0;          // span tables and results of zk_reuse_run
+    void* patch = nullptr; size_t patch_cap = 0;          // anchors and anchor tables of zk_patch_anchors / zk_patch_join
     uint32_t* h_sizes = nullptr; size_t cap_frames = 0;   // pinned: per-frame compressed sizes
     int sm_count = 0;
     unsigned long long launches = 0;
@@ -108,3 +110,20 @@ enum ZkReuseOp { ZK_REUSE_KEYS, ZK_REUSE_COMPARE, ZK_REUSE_COPY };
 struct ZkReuseSpan { unsigned long long a, b; uint32_t len; };
 int zk_reuse_run(ZkEncodeWs* ws, cudaStream_t stream, ZkReuseOp op, const uint8_t* a_buf, uint8_t* b_buf, const ZkReuseSpan* spans, uint32_t n,
                  void* out);
+
+// Seekable patches (zk_patch.inc states the rule).  An anchor is a position p >= 63 whose 64-byte gear hash h_p is >= ZK_PATCH_THR, about one
+// per 64 KiB; its key is h_p.
+#define ZK_PATCH_THR (0ull - ~0ull / 65536ull)
+// The anchors of one piece of n <= 1 GiB bytes at d_src (16 readable bytes after it), at positions 63 .. n - 1 of the piece, appended in
+// position order to *keys / *pos (positions plus base).  Synchronous on `stream`.
+int zk_patch_anchors(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, size_t n, unsigned long long base,
+                     std::vector<unsigned long long>* keys, std::vector<unsigned long long>* pos);
+// The anchors of OLD and NEW (each in position order) and NEW's frames: frame f covers NEW [fa[f], fa[f + 1]) and holds NEW's anchors
+// [fanc[f], fanc[f + 1])
+struct ZkPatchTables {
+    std::vector<unsigned long long> okeys, opos, nkeys, npos, fa;
+    std::vector<uint32_t> fanc;
+};
+// OLD's anchors sorted by (key, position) on the device, then frame f's range of OLD -> ranges[2f], ranges[2f + 1] (host).  Synchronous.
+int zk_patch_join(ZkEncodeWs* ws, cudaStream_t stream, const ZkPatchTables& t, uint32_t n_frames, unsigned long long old_len,
+                  unsigned long long margin, unsigned long long* ranges);

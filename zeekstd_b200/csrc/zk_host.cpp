@@ -554,6 +554,7 @@ struct zk_decoder {                        // decode.rs:121-466
     uint64_t win_valid_end = 0;            // the window is decoded up to this decompressed offset (< d[win_hi] after a range read)
     size_t max_window_bytes = (size_t)256 << 20;
     const uint8_t* prefix = nullptr; size_t prefix_len = 0;   // the prefix the window was decoded with (decompress_with_prefix)
+    const uint64_t* ranges = nullptr;                          // and every entry's range of it (nullptr: the whole prefix)
 
     void reset_dctx() { read_compressed = 0; win_lo = win_hi = 0; win_valid_end = 0; window.clear(); }                           // :352-357
     int32_t check_offset(uint64_t off) const { return off > seek_table.d.back() ? ZK_ERR_OFFSET_OUT_OF_RANGE : 0; }   // :439-445
@@ -582,7 +583,8 @@ struct zk_decoder {                        // decode.rs:121-466
             need.assign(n, 0xFFFFFFFFu);
             need[n - 1] = (uint32_t)(need_end - seek_table.d[f1 - 1]);
         } else need_end = d1;
-        rc = zk_decompress_frames_prefix(ctx, comp.data(), co.data(), dof.data(), n, window.data(), need.empty() ? nullptr : need.data(), 1, nullptr, prefix, prefix_len);
+        rc = zk_decompress_frames_prefixes(ctx, comp.data(), co.data(), dof.data(), n, window.data(), need.empty() ? nullptr : need.data(), 1, nullptr,
+                                           prefix, prefix_len, ranges ? ranges + 2 * (size_t)f0 : nullptr);
         if (rc) { win_lo = win_hi = 0; win_valid_end = 0; return rc; }
         win_lo = f0; win_hi = f1; win_valid_end = need_end;
         return 0;
@@ -624,9 +626,14 @@ extern "C" int32_t zk_decoder_decompress(zk_decoder* d, uint8_t* buf, size_t len
 
 extern "C" int32_t zk_decoder_decompress_with_prefix(zk_decoder* d, uint8_t* buf, size_t len, const uint8_t* prefix, size_t prefix_len,
                                                      size_t* produced) {                                        // :201-270
-    if (prefix != d->prefix || prefix_len != d->prefix_len) {      // frames decoded under another prefix are not reusable
+    return zk_decoder_decompress_with_prefix_ranges(d, buf, len, prefix, prefix_len, nullptr, produced);
+}
+
+extern "C" int32_t zk_decoder_decompress_with_prefix_ranges(zk_decoder* d, uint8_t* buf, size_t len, const uint8_t* prefix, size_t prefix_len,
+                                                            const uint64_t* ranges, size_t* produced) {
+    if (prefix != d->prefix || prefix_len != d->prefix_len || ranges != d->ranges) {   // frames decoded under another prefix are not reusable
         d->win_lo = d->win_hi = 0; d->win_valid_end = 0;
-        d->prefix = prefix; d->prefix_len = prefix_len;
+        d->prefix = prefix; d->prefix_len = prefix_len; d->ranges = ranges;
     }
     size_t progress = 0;
     const uint32_t nframes = d->seek_table.num_frames();
