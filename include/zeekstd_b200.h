@@ -80,6 +80,8 @@ uint64_t zk_ctx_kernel_launches(const zk_ctx* ctx);
 uint64_t zk_ctx_decode_segments(const zk_ctx* ctx);
 /* prefix bytes this context has copied to the device so far, by every call that takes a prefix */
 uint64_t zk_ctx_prefix_bytes_uploaded(const zk_ctx* ctx);
+/* entries of reference archives this context has decoded so far, by the calls that take one (the _archive calls of the patch block) */
+uint64_t zk_ctx_reference_entries_decoded(const zk_ctx* ctx);
 /* kernel-only device time (ms, CUDA events on the context's stream) of the most recent batch call */
 float zk_ctx_last_device_ms(const zk_ctx* ctx);
 const char* zk_version(void);
@@ -315,6 +317,37 @@ int32_t zk_patch_slices_write(uint64_t old_len, const uint64_t* ranges, uint32_t
 int32_t zk_patch_slices_read(const uint8_t* src, size_t len, uint32_t n_frames, uint64_t* old_len, uint64_t* ranges, size_t* frame_len);
 
 /*
+ * Seekable patches against a seekable archive (DESIGN §3.4.2): the reference R is a seekable archive, ref_n entries of ref_comp (ref_len
+ * bytes) at ref_c_off / ref_d_off (ref_n + 1 offsets each, as zk_decompress_frames takes them), and OLD is its decoded content, old_len =
+ * ref_d_off[ref_n].  R may be mmapped; only the compressed entries that a call needs cross to the device, and they are decoded there, on
+ * slot 0, into the context's prefix buffer: no byte of OLD is uploaded (zk_ctx_prefix_bytes_uploaded does not grow) or copied to the host.
+ *   zk_patch_ranges_archive returns exactly zk_patch_ranges(new_src, frame_sizes, OLD, old_len, margin), whatever R's entry layout.
+ *   zk_compress_frames_patch_archive writes exactly the bytes and c_sizes of zk_compress_frames_patch(..., OLD, old_len, ranges, ...).
+ *   zk_decompress_frames_prefixes_archive gives the output, statuses and return code of zk_decompress_frames_prefixes(..., OLD, old_len,
+ *     ranges), d_need and checksum verification included; ranges == NULL: every entry against all of OLD.
+ *   zk_decoder_decompress_with_reference_archive (the Decoder block) reads a seekable patch that way.
+ * For each group of entries (zk_decompress_frames_prefixes' groups, hull [hlo, hhi) <= 1 GiB) only the entries of R whose output overlaps
+ * the hull are decoded, the last one only as far as hhi (no checksum on that partial entry, as with d_need); empty entries never are.
+ * zk_ctx_reference_entries_decoded counts them.  Full entries of R are checked against their checksums on the compress and range calls
+ * always, on the decompress call when verify_checksum is set.
+ * An entry of R that fails to decode: every entry being decompressed whose range overlaps its output gets its status (the return code is
+ * the first non-zero status, as in the raw-reference call; the others decode normally); the compress and range calls return it.
+ * ZK_ERR_INVALID_ARG: R's offsets decrease, ref_d_off[0] != 0, ref_c_off[ref_n] > ref_len, a range with lo > hi or hi > old_len, or R is
+ * itself a seekable patch (ZK_PATCH_SLICES_MAGIC at ref_c_off[0]: chains are not resolved).  Other argument errors as in the raw calls.
+ */
+int32_t zk_patch_ranges_archive(zk_ctx* ctx, const uint8_t* new_src, const uint32_t* frame_sizes, uint32_t n_frames, const uint8_t* ref_comp,
+                                size_t ref_len, const uint64_t* ref_c_off, const uint64_t* ref_d_off, uint32_t ref_n, uint64_t margin,
+                                uint64_t* ranges);
+int32_t zk_compress_frames_patch_archive(zk_ctx* ctx, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                         int32_t checksum, const uint8_t* ref_comp, size_t ref_len, const uint64_t* ref_c_off,
+                                         const uint64_t* ref_d_off, uint32_t ref_n, const uint64_t* ranges, uint8_t* dst, size_t dst_cap,
+                                         uint32_t* c_sizes, size_t* dst_len);
+int32_t zk_decompress_frames_prefixes_archive(zk_ctx* ctx, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n,
+                                              uint8_t* dst, const uint32_t* d_need, int32_t verify_checksum, int32_t* status,
+                                              const uint8_t* ref_comp, size_t ref_len, const uint64_t* ref_c_off, const uint64_t* ref_d_off,
+                                              uint32_t ref_n, const uint64_t* ranges);
+
+/*
  * The content-defined cut alone (FrameSizePolicy::ContentDefined(size), the rule of zk_compress_frames_cdc): frame_sizes, *n_frames and
  * *consumed are exactly the d_sizes, frame count and consumed of zk_compress_frames_cdc on the same src, n, size and final, at any level;
  * nothing is compressed.  frames_cap >= n / 1024 + 1 always suffices; less than a call needs returns -70 (dstSize_tooSmall).  HOST pointers.
@@ -479,6 +512,11 @@ int32_t zk_decoder_decompress_with_prefix(zk_decoder* d, uint8_t* buf, size_t le
  * takes them): a seekable patch read with its slices; each window of frames uploads only the hull of its own entries' ranges */
 int32_t zk_decoder_decompress_with_prefix_ranges(zk_decoder* d, uint8_t* buf, size_t len, const uint8_t* prefix, size_t prefix_len,
                                                  const uint64_t* ranges, size_t* produced);
+/* the same with the prefix being the decoded content of the reference archive R (zk_decompress_frames_prefixes_archive's arguments): each
+ * window of frames decodes only the entries of R under its own entries' ranges */
+int32_t zk_decoder_decompress_with_reference_archive(zk_decoder* d, uint8_t* buf, size_t len, const uint8_t* ref_comp, size_t ref_len,
+                                                     const uint64_t* ref_c_off, const uint64_t* ref_d_off, uint32_t ref_n,
+                                                     const uint64_t* ranges, size_t* produced);
 void zk_decoder_reset(zk_decoder* d);                                                    /* :346-350 */
 int32_t zk_decoder_set_lower_frame(zk_decoder* d, uint32_t index, uint64_t* offset);    /* :367 */
 int32_t zk_decoder_set_upper_frame(zk_decoder* d, uint32_t index, uint64_t* offset);    /* :383 */

@@ -264,7 +264,8 @@ class Context:
         need (optional, one uint32 per frame): only that many leading bytes of each frame are wanted (range reads,
         zk_decompress_frames_upto): the rest of a frame's output range is then unspecified and its checksum is not verified.
         prefix_ranges (n x 2 integers): entry e is decoded against prefix[prefix_ranges[e][0]:prefix_ranges[e][1]] only
-        (zk_decompress_frames_prefixes)."""
+        (zk_decompress_frames_prefixes).  prefix may be a ReferenceArchive: its decoded content is the prefix, and only the entries
+        under the ranges are decoded, on the GPU (zk_decompress_frames_prefixes_archive)."""
         addr, n, keep = _buf(comp)
         co = np.ascontiguousarray(c_off, dtype=np.uint64); do = np.ascontiguousarray(d_off, dtype=np.uint64)
         nf = len(co) - 1
@@ -277,6 +278,13 @@ class Context:
         nd = None if need is None else np.ascontiguousarray(need, dtype=np.uint32)
         if nd is not None and len(nd) != nf:
             raise ValueError("need: one entry per frame")
+        if isinstance(prefix, ReferenceArchive):
+            rg = None if prefix_ranges is None else _ranges(prefix_ranges, nf)
+            rc = self.lib.zk_decompress_frames_prefixes_archive(self._h, addr, co.ctypes.data_as(_native.u64p), do.ctypes.data_as(_native.u64p),
+                                                                nf, out.ctypes.data, None if nd is None else nd.ctypes.data_as(_native.u32p),
+                                                                int(verify_checksum), st.ctypes.data_as(_native.i32p), *prefix._args(),
+                                                                None if rg is None else rg.ctypes.data_as(_native.u64p))
+            return out[:total], st[:nf], rc
         paddr, pn, pkeep = _buf(prefix) if prefix is not None else (None, 0, None)
         if prefix_ranges is not None:
             rg = _ranges(prefix_ranges, nf)
@@ -297,17 +305,27 @@ class Context:
         """prefix bytes this context has copied to the device so far (zk_ctx_prefix_bytes_uploaded)"""
         return int(self.lib.zk_ctx_prefix_bytes_uploaded(self._h))
 
+    @property
+    def reference_entries_decoded(self) -> int:
+        """entries of reference archives this context has decoded so far (zk_ctx_reference_entries_decoded)"""
+        return int(self.lib.zk_ctx_reference_entries_decoded(self._h))
+
     def patch_ranges(self, new, frame_sizes, old, margin: int | None = None) -> np.ndarray:
         """the slice of `old` each frame of `new` is matched against in a seekable patch -> n x 2 np.uint64 (lo, hi), found on the GPU by
         content anchors (the rule: include/zeekstd_b200.h, zk_patch_ranges).  margin: bytes added on each side (default: the largest frame
-        size, which is the frame size of uniform frames)"""
+        size, which is the frame size of uniform frames).  old may be a ReferenceArchive: the same ranges, with OLD decoded on the GPU
+        (zk_patch_ranges_archive)"""
         addr, n, keep = _buf(new)
         ds = np.ascontiguousarray(frame_sizes, dtype=np.uint32).reshape(-1)
         if int(np.sum(ds, dtype=np.uint64)) != n:
             raise ValueError(f"frame sizes add up to {int(np.sum(ds, dtype=np.uint64))} bytes, the input has {n}")
-        oaddr, on, okeep = _buf(old)
         m = int(ds.max()) if margin is None and ds.size else int(margin or 0)
         rg = np.zeros((max(ds.size, 1), 2), dtype=np.uint64)
+        if isinstance(old, ReferenceArchive):
+            _check(self.lib.zk_patch_ranges_archive(self._h, addr, ds.ctypes.data_as(_native.u32p), ds.size, *old._args(), m,
+                                                    rg.ctypes.data_as(_native.u64p)), self.lib)
+            return rg[: ds.size]
+        oaddr, on, okeep = _buf(old)
         _check(self.lib.zk_patch_ranges(self._h, addr, ds.ctypes.data_as(_native.u32p), ds.size, oaddr, on, m,
                                         rg.ctypes.data_as(_native.u64p)), self.lib)
         return rg[: ds.size]
@@ -315,31 +333,38 @@ class Context:
     def compress_frames_patch(self, new, frame_sizes, old, ranges, level: int = 0, checksum: bool = False):
         """frame f of `new` against old[ranges[f][0]:ranges[f][1]] with long-distance matching, for an `old` of any size
         (zk_compress_frames_patch) -> (compressed bytes (np.uint8), c_sizes, d_sizes).  Frame f is what compress_frames_sized(frame alone,
-        prefix=old, long_distance=True, prefix_ranges=[ranges[f]]) writes"""
+        prefix=old, long_distance=True, prefix_ranges=[ranges[f]]) writes.  old may be a ReferenceArchive: the same bytes, with each group's
+        slices of OLD decoded on the GPU (zk_compress_frames_patch_archive)"""
         addr, n, keep = _buf(new)
         ds = np.ascontiguousarray(frame_sizes, dtype=np.uint32).reshape(-1)
         if int(np.sum(ds, dtype=np.uint64)) != n:
             raise ValueError(f"frame sizes add up to {int(np.sum(ds, dtype=np.uint64))} bytes, the input has {n}")
-        oaddr, on, okeep = _buf(old)
         rg = _ranges(ranges, ds.size)
         dsp = ds.ctypes.data_as(_native.u32p)
         cap = self.lib.zk_compress_bound_sized(dsp, ds.size)
         dst = np.empty(cap + 64, dtype=np.uint8)
         cs = np.zeros(max(ds.size, 1), dtype=np.uint32)
         dl = c_size_t()
+        if isinstance(old, ReferenceArchive):
+            _check(self.lib.zk_compress_frames_patch_archive(self._h, addr, dsp, ds.size, level, int(checksum), *old._args(),
+                                                             rg.ctypes.data_as(_native.u64p), dst.ctypes.data, cap, cs.ctypes.data_as(_native.u32p),
+                                                             byref(dl)), self.lib)
+            return dst[: dl.value], cs[: ds.size], ds.copy()
+        oaddr, on, okeep = _buf(old)
         _check(self.lib.zk_compress_frames_patch(self._h, addr, dsp, ds.size, level, int(checksum), oaddr, on, rg.ctypes.data_as(_native.u64p),
                                                  dst.ctypes.data, cap, cs.ctypes.data_as(_native.u32p), byref(dl)), self.lib)
         return dst[: dl.value], cs[: ds.size], ds.copy()
 
     def compress_patch_slices(self, new, frame_sizes, old, level: int = 0, checksum: bool = False, margin: int | None = None) -> bytes:
         """a seekable patch of `new` against `old` -> the archive's bytes: the slice frame (the ranges of patch_ranges), then the frames
-        of compress_frames_patch, then the Foot seek table.  Entry 0's compressed size includes the slice frame."""
+        of compress_frames_patch, then the Foot seek table.  Entry 0's compressed size includes the slice frame.  old may be a
+        ReferenceArchive: the same bytes."""
         ds = np.ascontiguousarray(frame_sizes, dtype=np.uint32).reshape(-1)
         if ds.size == 0:
             raise ValueError("a seekable patch has at least one frame")
         rg = self.patch_ranges(new, ds, old, margin)
         comp, cs, _ = self.compress_frames_patch(new, ds, old, rg, level, checksum)
-        head = patch_slices_write(_buf(old)[1], rg, self.lib)
+        head = patch_slices_write(old.old_len if isinstance(old, ReferenceArchive) else _buf(old)[1], rg, self.lib)
         table = SeekTable(lib=self.lib)
         for f, (c, d) in enumerate(zip(cs.tolist(), ds.tolist())):
             table.log_frame(c + (len(head) if f == 0 else 0), d)
@@ -347,6 +372,47 @@ class Context:
 
 
 PATCH_SLICES_MAGIC = 0x184D2A5B
+
+
+class ReferenceArchive:
+    """a seekable archive as the reference (OLD) of a seekable patch: OLD is its decoded content, and the patch calls that take one decode
+    on the GPU only the entries of it they need (DESIGN §3.4.2).  data: the archive's bytes or a mapping of it (kept, not copied).  Its
+    entries come from the Foot seek table at its end (the default), from seek_table (a SeekTable, or the bytes of one in `format`, e.g.
+    a stand-alone Head table), or from explicit c_off / d_off (n + 1 offsets each, as Context.decompress_frames takes them).  A seekable
+    patch (the slice frame at the start of its first entry) is refused: chains of patches are not resolved."""
+
+    def __init__(self, data, seek_table=None, format: int = Format.Foot, c_off=None, d_off=None, lib=None):
+        self.lib = lib or _native.default_lib()
+        self._addr, self._len, self._keep = _buf(data)
+        if c_off is not None or d_off is not None:
+            if c_off is None or d_off is None:
+                raise ValueError("c_off and d_off go together")
+            co, do = np.ascontiguousarray(c_off, dtype=np.uint64), np.ascontiguousarray(d_off, dtype=np.uint64)
+            if co.ndim != 1 or co.size == 0 or co.shape != do.shape:
+                raise ValueError("c_off, d_off: n + 1 offsets each")
+        else:
+            if seek_table is None:
+                seek_table = SeekTable.from_bytes(data, format, self.lib)
+            elif not isinstance(seek_table, SeekTable):
+                seek_table = SeekTable.from_bytes(seek_table, format, self.lib)
+            co, do = seek_table.offsets()
+        self.c_off, self.d_off = co, do
+        c0 = int(co[0])
+        view = self._keep if isinstance(self._keep, np.ndarray) else self._keep[0]
+        if int(co[-1]) - c0 >= 4 and c0 + 4 <= self._len and int.from_bytes(view[c0:c0 + 4].tobytes(), "little") == PATCH_SLICES_MAGIC:
+            raise ValueError("the reference archive is a seekable patch; restore it first")
+
+    @property
+    def n_entries(self) -> int: return len(self.c_off) - 1
+
+    @property
+    def old_len(self) -> int:
+        """bytes of OLD, the archive's decoded content"""
+        return int(self.d_off[-1])
+
+    def _args(self):
+        """the (ref_comp, ref_len, ref_c_off, ref_d_off, ref_n) arguments of the _archive calls"""
+        return (self._addr, self._len, self.c_off.ctypes.data_as(_native.u64p), self.d_off.ctypes.data_as(_native.u64p), self.n_entries)
 
 
 def patch_slices_size(n_frames: int) -> int:
@@ -788,16 +854,26 @@ class Decoder(io.RawIOBase):
     def decompress_with_prefix(self, buf, prefix=None, ranges=None) -> int:
         """decode.rs:201-270: every frame is decoded against the raw-content prefix.  ranges (one (lo, hi) pair per seek-table entry): entry
         e is decoded against prefix[lo:hi] only, and only the slices of the frames read go to the device (a seekable patch,
-        zk_decoder_decompress_with_prefix_ranges)"""
+        zk_decoder_decompress_with_prefix_ranges).  prefix may be a ReferenceArchive: each window of frames then decodes only the entries
+        of it under its ranges, on the GPU (zk_decoder_decompress_with_reference_archive)"""
         if prefix is None:
             return self.decompress(buf)
         mv = memoryview(buf)
         if len(mv) == 0:
             return 0
         arr = (ctypes.c_uint8 * len(mv)).from_buffer(mv)
+        p = c_size_t()
+        if isinstance(prefix, ReferenceArchive):
+            self._prefix_keep = prefix
+            rp = None
+            if ranges is not None:
+                if getattr(self, "_ranges_src", None) is not ranges:    # the same array on every call keeps the decoded window valid
+                    self._ranges_src, self._ranges = ranges, _ranges(ranges, self.seek_table().num_frames())
+                rp = self._ranges.ctypes.data_as(_native.u64p)
+            _check(self.lib.zk_decoder_decompress_with_reference_archive(self._h, arr, len(mv), *prefix._args(), rp, byref(p)), self.lib)
+            return int(p.value)
         paddr, pn, pkeep = _buf(prefix)
         self._prefix_keep = pkeep
-        p = c_size_t()
         if ranges is None:
             _check(self.lib.zk_decoder_decompress_with_prefix(self._h, arr, len(mv), paddr, pn, byref(p)), self.lib)
         else:

@@ -49,6 +49,7 @@ _SIGS = {
     "zk_ctx_decode_segments": (c_uint64, [c_void_p]),
     "zk_ctx_last_device_ms": (c_float, [c_void_p]),
     "zk_ctx_prefix_bytes_uploaded": (c_uint64, [c_void_p]),
+    "zk_ctx_reference_entries_decoded": (c_uint64, [c_void_p]),
     "zk_compress_bound": (c_size_t, [c_size_t, c_uint32]),
     "zk_ctx_profile": (None, [c_void_p, c_int32]),
     "zk_ctx_profile_read": (None, [c_void_p, POINTER(c_float), u32p]),
@@ -98,6 +99,11 @@ _SIGS = {
     "zk_patch_slices_size": (c_size_t, [c_uint32]),
     "zk_patch_slices_write": (c_int32, [c_uint64, u64p, c_uint32, c_void_p, c_size_t, POINTER(c_size_t)]),
     "zk_patch_slices_read": (c_int32, [c_void_p, c_size_t, c_uint32, u64p, u64p, POINTER(c_size_t)]),
+    "zk_patch_ranges_archive": (c_int32, [c_void_p, c_void_p, u32p, c_uint32, c_void_p, c_size_t, u64p, u64p, c_uint32, c_uint64, u64p]),
+    "zk_compress_frames_patch_archive": (c_int32, [c_void_p, c_void_p, u32p, c_uint32, c_int32, c_int32, c_void_p, c_size_t, u64p, u64p,
+                                                   c_uint32, u64p, c_void_p, c_size_t, u32p, POINTER(c_size_t)]),
+    "zk_decompress_frames_prefixes_archive": (c_int32, [c_void_p, c_void_p, u64p, u64p, c_uint32, c_void_p, u32p, c_int32, i32p, c_void_p,
+                                                        c_size_t, u64p, u64p, c_uint32, u64p]),
     "zk_cut_frames_cdc": (c_int32, [c_void_p, c_void_p, c_size_t, c_uint32, c_int32, u32p, c_uint32, u32p, POINTER(c_size_t)]),
     "zk_compress_frames_sized_reuse": (c_int32, [c_void_p, c_void_p, u32p, c_uint32, c_int32, c_int32, c_int32, c_void_p, c_size_t, u64p,
                                                  u64p, c_uint32, c_void_p, c_size_t, u32p, u32p, POINTER(c_size_t)]),
@@ -169,6 +175,8 @@ _SIGS = {
     "zk_decoder_decompress": (c_int32, [c_void_p, c_void_p, c_size_t, POINTER(c_size_t)]),
     "zk_decoder_decompress_with_prefix": (c_int32, [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, POINTER(c_size_t)]),
     "zk_decoder_decompress_with_prefix_ranges": (c_int32, [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, u64p, POINTER(c_size_t)]),
+    "zk_decoder_decompress_with_reference_archive": (c_int32, [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, u64p, u64p, c_uint32, u64p,
+                                                               POINTER(c_size_t)]),
     "zk_decoder_reset": (None, [c_void_p]),
     "zk_decoder_set_lower_frame": (c_int32, [c_void_p, c_uint32, u64p]),
     "zk_decoder_set_upper_frame": (c_int32, [c_void_p, c_uint32, u64p]),

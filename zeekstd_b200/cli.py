@@ -1,8 +1,8 @@
 """Command-line front end with the reference CLI's arguments and behaviour (SURVEY.md 8f.4), over the GPU codec.
 
-    python -m zeekstd_b200 [compress] [-l N] [-s 2M] [--frame-size-policy ..] [--patch-from F [--long | --patch-slices]] [--long-mode] [--reuse-from OLD.zst]
-                           [INPUT] [-o OUT]
-    python -m zeekstd_b200 decompress [--from N | --from-frame I] [--to N|end | --to-frame I|end] [--patch-apply F] INPUT [-o OUT]
+    python -m zeekstd_b200 [compress] [-l N] [-s 2M] [--frame-size-policy ..] [--patch-from F [--long | --patch-slices [--patch-archive]]]
+                           [--long-mode] [--reuse-from OLD.zst] [INPUT] [-o OUT]
+    python -m zeekstd_b200 decompress [--from N | --from-frame I] [--to N|end | --to-frame I|end] [--patch-apply F [--patch-archive]] INPUT [-o OUT]
     python -m zeekstd_b200 list [--from-frame I] [--to-frame I|end | --num-frames N] [-d] [--seek-table-format head|foot] INPUT
 
 What each piece follows in the reference: argument set and value parsers cli/src/args.rs:10-329; sub-commands, output
@@ -25,7 +25,9 @@ of the input changes only the frames around it and rsync, dedup stores and range
 whose bytes a frame of OLD.zst holds is copied from it, only the others are compressed; with `uncompressed` or `content` frames.
 `--patch-from F --patch-slices` (an extension of this codec) writes a seekable patch against an F of any size: every frame is matched
 against its own slice of F, found by content anchors and recorded in a skippable frame at the start of the archive, and `decompress
---patch-apply F` reads only the slices of the frames it restores.
+--patch-apply F` reads only the slices of the frames it restores.  With `--patch-archive` (also an extension) F is a seekable archive
+whose decoded content is the reference: it is decoded on the GPU, and only the entries under the slices a command needs are.  The flag
+is explicit because a raw reference file may itself be a .zst file.
 """
 from __future__ import annotations
 
@@ -169,6 +171,9 @@ def build_parser() -> argparse.ArgumentParser:
                         "matching (level 16's tier); needs --frame-size-policy uncompressed or content.")
     c.add_argument("--patch-margin", type=byte_value, default=None,
                    help="With --patch-slices: bytes added on each side of a frame's slice (default: the frame size).")
+    c.add_argument("--patch-archive", action="store_true",
+                   help="With --patch-slices: the --patch-from file is a seekable archive, and the reference is its decoded content, "
+                        "decoded on the GPU entry by entry. The patch is the one made against the decoded file.")
     c.add_argument("--reuse-from", default=None, metavar="OLD.zst",
                    help="The archive of a previous version of the input (ending in its seek table): every frame whose bytes one of its "
                         "frames already holds is copied from it, only the others are compressed. The output is what compress writes "
@@ -185,6 +190,9 @@ def build_parser() -> argparse.ArgumentParser:
     g1.add_argument("--to", type=offset_limit, default="end", help="Accepts the special value 'end'.")
     g1.add_argument("--to-frame", type=last_frame, default=None)
     d.add_argument("--patch-apply", default=None)
+    d.add_argument("--patch-archive", action="store_true",
+                   help="With --patch-apply: the reference is a seekable archive; only its entries under the slices of the frames restored "
+                        "are decoded, on the GPU.")
     d.add_argument("input_file")
     d.add_argument("-o", "--output-file", default=None)
 
@@ -260,6 +268,20 @@ def _new_writer(out_path, in_path, quiet: bool, force: bool):
     if not force and sys.stdout.isatty():
         raise CliError("stdout is a terminal, aborting")
     return sys.stdout.buffer
+
+
+def _load_reference(zk, path):
+    """a reference archive (--patch-archive): the file mapped, its Foot seek table parsed"""
+    try:
+        data = np.memmap(path, dtype=np.uint8, mode="r") if os.path.getsize(path) > 0 else np.zeros(0, dtype=np.uint8)
+    except OSError as e:
+        raise CliError(f"Failed to load reference archive: {e}")
+    try:
+        return zk.ReferenceArchive(data)
+    except zk.Error as e:
+        raise CliError(f"Failed to parse the seek table of {path}: {e}")
+    except ValueError:
+        raise CliError(f"{path} is a seekable patch; restore it first")
 
 
 def _load_prefix(path, use_mmap: bool):
@@ -360,6 +382,8 @@ def _run_compress(zk, ns, fmt_bytes) -> int:
             raise CliError("--patch-slices needs a frame size above 0")
     elif ns.patch_margin is not None:
         raise CliError("--patch-margin needs --patch-slices")
+    if ns.patch_archive and (not ns.patch_slices or ns.long):
+        raise CliError("--patch-archive needs --patch-from and --patch-slices: whole-prefix patches against an archive are not supported")
     if ns.reuse_from is not None:
         if ns.patch_from:
             raise CliError("--reuse-from cannot be used with --patch-from: a copied frame must depend on its own bytes alone")
@@ -368,6 +392,7 @@ def _run_compress(zk, ns, fmt_bytes) -> int:
         if ns.frame_size == 0:
             raise CliError("--reuse-from needs a frame size above 0")
     prefix_len = os.path.getsize(ns.patch_from) if ns.patch_from and os.path.exists(ns.patch_from) else None
+    ns.reference = _load_reference(zk, ns.patch_from) if ns.patch_archive else None
     st_file = None
     if ns.seek_table_file is not None:
         try:
@@ -472,13 +497,13 @@ def _run_compress_slices(zk, ns, fmt_bytes, reader, writer, in_path, out_path, s
         data = _load_whole(in_path, "input file")
     else:
         data = np.frombuffer(reader.read(), dtype=np.uint8)
-    old = _load_whole(ns.patch_from, "prefix (patch) file")
+    old = ns.reference if ns.reference is not None else _load_whole(ns.patch_from, "prefix (patch) file")
     ctx = zk.default_context()
     sizes = _policy_sizes(zk, ctx, ns, data)
     margin = ns.frame_size if ns.patch_margin is None else ns.patch_margin
     ranges = ctx.patch_ranges(data, sizes, old, margin)
     comp, cs, _ = ctx.compress_frames_patch(data, sizes, old, ranges, ns.compression_level, not ns.no_checksum)
-    head = zk.patch_slices_write(int(old.size), ranges)
+    head = zk.patch_slices_write(old.old_len if ns.reference is not None else int(old.size), ranges)
     table = zk.SeekTable()
     for f, (c, d) in enumerate(zip(cs.tolist(), sizes.tolist())):
         table.log_frame(c + (len(head) if f == 0 else 0), d)
@@ -541,7 +566,12 @@ def _run_compress_reuse(zk, ns, fmt_bytes, reader, writer, in_path, out_path, st
 def _run_decompress(zk, ns, fmt_bytes) -> int:
     in_path = ns.input_file
     out_path = _out_path(ns, in_path)
+    if ns.patch_archive and not ns.patch_apply:
+        raise CliError("--patch-archive needs --patch-apply: it says that the reference file is a seekable archive")
+    reference = _load_reference(zk, ns.patch_apply) if ns.patch_archive else None
     prefix_len = os.path.getsize(ns.patch_apply) if ns.patch_apply and os.path.exists(ns.patch_apply) else None
+    if reference is not None:
+        prefix_len = reference.old_len
     writer = _new_writer(out_path, in_path, ns.quiet, ns.force)
     try:
         src = open(in_path, "rb")
@@ -583,14 +613,18 @@ def _run_decompress(zk, ns, fmt_bytes) -> int:
             except zk.Error as e:
                 raise CliError(f"Failed to read the slices of the seekable patch: {e}")
             if prefix_len != old_len:
-                raise CliError(f"{ns.patch_apply} has {prefix_len} bytes, the seekable patch was made against {old_len} bytes")
+                has = "decodes to" if reference is not None else "has"
+                raise CliError(f"{ns.patch_apply} {has} {prefix_len} bytes, the seekable patch was made against {old_len} bytes")
+    if reference is not None and ranges is None:
+        raise CliError("--patch-archive needs a seekable patch (compress --patch-slices): whole-prefix patches against an archive are not supported")
     bar = _Progress(limit, fmt_bytes, not ns.quiet and not ns.no_progress, pos=offset)
     try:
         dec = zk.DecodeOptions(src).seek_table(table).offset(offset).offset_limit(limit).into_decoder()
     except zk.Error as e:
         raise CliError(f"Failed to create decoder: {e}")
-    # the slices of a patch are read from a mapping: only those of the frames decoded are paged in
-    prefix = _load_prefix(ns.patch_apply, ranges is not None or _use_mmap(ns, prefix_len))
+    # the slices of a patch are read from a mapping: only those of the frames decoded are paged in (of a reference archive, only the
+    # entries under them are decoded)
+    prefix = reference if reference is not None else _load_prefix(ns.patch_apply, ranges is not None or _use_mmap(ns, prefix_len))
 
     buf = bytearray(OUT_CHUNK)
     view = memoryview(buf)

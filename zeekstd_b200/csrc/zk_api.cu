@@ -7,6 +7,7 @@
 #include <time.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include <set>
 #include <unordered_map>
 #include <unordered_set>
@@ -146,6 +147,7 @@ extern "C" uint64_t zk_ctx_decode_segments(const zk_ctx* c) {
 }
 extern "C" float zk_ctx_last_device_ms(const zk_ctx* c) { return c ? c->last_ms : 0.f; }
 extern "C" uint64_t zk_ctx_prefix_bytes_uploaded(const zk_ctx* c) { return c ? c->prefix_uploaded : 0; }
+extern "C" uint64_t zk_ctx_reference_entries_decoded(const zk_ctx* c) { return c ? c->ref_decoded : 0; }
 extern "C" size_t zk_compress_bound(size_t n, uint32_t frame_size) { return zk_encode_bound(n, frame_size); }
 
 extern "C" void zk_ctx_profile(zk_ctx* c, int32_t enable) {
@@ -184,6 +186,14 @@ static int32_t zk_upload_prefix(zk_ctx* c, const uint8_t* prefix, size_t len, co
     ZK_CUDA_OK(cudaMemcpy(c->d_prefix, prefix, len, cudaMemcpyHostToDevice));
     c->prefix_uploaded += len;
     *d_prefix = (const uint8_t*)c->d_prefix; *d_len = (uint32_t)len;
+    return 0;
+}
+// the same for a prefix already in device memory (a reference archive decoded into the prefix arena): nothing is copied
+static int32_t zk_device_prefix(const uint8_t* prefix, size_t len, const uint8_t** d_prefix, uint32_t* d_len) {
+    *d_prefix = nullptr; *d_len = 0;
+    if (!prefix || len == 0) return 0;
+    if (len > 0x7FFFFFFFull) return ZK_ERR_INVALID_ARG;
+    *d_prefix = prefix; *d_len = (uint32_t)len;
     return 0;
 }
 
@@ -365,7 +375,7 @@ static void zk_rebase_ranges(const uint64_t* ranges, uint32_t f0, uint32_t end, 
 
 static int32_t zk_decompress_prefixes_one(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n, uint8_t* dst,
                                           const uint32_t* d_need, int32_t verify, int32_t* status, const uint8_t* prefix, size_t prefix_len,
-                                          const uint64_t* ranges);
+                                          const uint64_t* ranges, bool prefix_dev = false);
 
 // entry e decoded against its own range of the prefix buffer; ranges == NULL: every entry against the whole buffer.  With ranges, the
 // entries run in groups (zk_hull_group), each with only the hull of its ranges on the device, so the buffer may be of any size
@@ -394,13 +404,15 @@ extern "C" int32_t zk_decompress_frames_prefixes(zk_ctx* c, const uint8_t* comp,
     return worst;
 }
 
+// prefix_dev: the prefix is already in device memory (zk_device_prefix); else host memory, uploaded (zk_upload_prefix)
 static int32_t zk_decompress_prefixes_one(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n, uint8_t* dst,
                                           const uint32_t* d_need, int32_t verify, int32_t* status, const uint8_t* prefix, size_t prefix_len,
-                                          const uint64_t* ranges) {
+                                          const uint64_t* ranges, bool prefix_dev) {
     ZkDecCall q = {comp, c_off, d_off, dst, verify, status, ZkDecodeParams()};
     std::vector<uint32_t> rw;
     int32_t rc = zk_prefix_ranges(ranges, n, prefix_len, &rw);
-    if (!rc) rc = zk_upload_prefix(c, prefix, prefix_len, &q.p.prefix, &q.p.prefix_len);
+    if (!rc) rc = prefix_dev ? zk_device_prefix(prefix, prefix_len, &q.p.prefix, &q.p.prefix_len)
+                             : zk_upload_prefix(c, prefix, prefix_len, &q.p.prefix, &q.p.prefix_len);
     if (rc) return rc;
     if (q.p.prefix && ranges) q.p.ranges = rw.data();
     if (n && (!comp || !c_off || !d_off || !dst)) return ZK_ERR_INVALID_ARG;
@@ -477,6 +489,7 @@ struct ZkCompressReq {
     bool host = true;                                       // src and dst in host memory; else device memory, worked on `stream`
     cudaStream_t stream = nullptr;                          // nullptr: slot 0's
     const uint8_t* prefix = nullptr; size_t prefix_len = 0; // host memory
+    bool prefix_dev = false;                                // sized: `prefix` is device memory already (zk_device_prefix), not uploaded
     const uint64_t* ranges = nullptr;                       // sized: frame f's prefix is prefix[ranges[2f], ranges[2f + 1]) (NULL: all of it)
     ZkEncodeParams params;                                  // its prefix: the device copy of `prefix`, and the ranges as 32-bit words
     int32_t final_ = 1;                                     // Compressed / ContentDefined: no more input follows this call's
@@ -712,7 +725,9 @@ static int32_t zk_compress(zk_ctx* c, ZkCompressReq q) {
         if (q.dst_len) *q.dst_len = 0;
         if (q.count == 0) return 0;                         // (no frame, unlike the uniform layout of no input)
         if ((rc = zk_prefix_ranges(q.ranges, q.count, q.prefix_len, &range_words))) return rc;
-        if ((rc = zk_upload_prefix(c, q.prefix, q.prefix_len, &q.params.prefix, &q.params.prefix_len))) return rc;
+        rc = q.prefix_dev ? zk_device_prefix(q.prefix, q.prefix_len, &q.params.prefix, &q.params.prefix_len)
+                          : zk_upload_prefix(c, q.prefix, q.prefix_len, &q.params.prefix, &q.params.prefix_len);
+        if (rc) return rc;
         if (q.params.prefix && q.ranges) q.params.ranges = range_words.data();
         fr = {q.sizes, q.n, 0, q.count};
     } else {
@@ -1312,4 +1327,245 @@ extern "C" int32_t zk_patch_slices_read(const uint8_t* src, size_t len, uint32_t
     if (old_len) *old_len = ol;
     if (frame_len) *frame_len = total;
     return 0;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Seekable patches against a seekable archive (DESIGN §3.4.2): OLD is the decoded content of a reference archive R, and the calls above
+// run on it without OLD ever being on the host.  For each group of entries (zk_hull_group), the entries of R whose output overlaps the
+// group's hull are decoded on slot 0 straight into the prefix arena (c->d_prefix), the last one only as far as the hull's end, and the
+// prefix machinery reads the hull from there (zk_device_prefix).  The anchor pass decodes R in runs of whole entries instead.
+// ---------------------------------------------------------------------------------------------
+struct ZkRefArchive { const uint8_t* comp; size_t len; const uint64_t* c_off; const uint64_t* d_off; uint32_t n; };
+
+// decoded OLD starts this far into the prefix arena: the anchor pass puts the 63 bytes before a run in front of it
+#define ZK_REF_HEAD 64u
+
+// R's arguments: offsets that never decrease, OLD starting at 0, entries within R's bytes, and not a seekable patch itself (chains are
+// not resolved) -> 0 or ZK_ERR_INVALID_ARG.  *old_len: OLD's length
+static int32_t zk_ref_check(const ZkRefArchive& r, uint64_t* old_len) {
+    if (!r.c_off || !r.d_off || (r.n && !r.comp) || r.d_off[0] != 0) return ZK_ERR_INVALID_ARG;
+    for (uint32_t g = 0; g < r.n; g++)
+        if (r.c_off[g + 1] < r.c_off[g] || r.d_off[g + 1] < r.d_off[g]) return ZK_ERR_INVALID_ARG;
+    if (r.c_off[r.n] > r.len) return ZK_ERR_INVALID_ARG;
+    if (r.c_off[r.n] - r.c_off[0] >= 4 && zk_le32(r.comp + r.c_off[0]) == ZK_PATCH_SLICES_MAGIC) return ZK_ERR_INVALID_ARG;
+    *old_len = r.d_off[r.n];
+    return 0;
+}
+
+// OLD [lo, hi) (lo < hi) made resident: the non-empty entries of R whose output overlaps it, list[0, m), uploaded back to back through
+// slot 0 and decoded into the prefix arena from ZK_REF_HEAD on, the last one only as far as hi (need: no checksum on it).  *base: the
+// OLD offset of arena byte ZK_REF_HEAD; (*status)[k]: entry list[k]'s status.  Returns 0 or a failure of the call itself.  Device memory:
+// the decoded bytes from the first entry's start to hi, plus the rest of the block that holds hi (the decoder stops at a block's end)
+static int32_t zk_ref_decode(zk_ctx* c, const ZkRefArchive& r, uint64_t lo, uint64_t hi, int verify, uint64_t* base,
+                             std::vector<uint32_t>* list, std::vector<int32_t>* status) {
+    list->clear();
+    uint32_t g = (uint32_t)(std::upper_bound(r.d_off, r.d_off + r.n + 1, lo) - r.d_off) - 1;    // the entry that holds lo
+    for (; g < r.n && r.d_off[g] < hi; g++)
+        if (r.d_off[g + 1] > r.d_off[g]) list->push_back(g);
+    const uint32_t m = (uint32_t)list->size();
+    std::vector<uint64_t> c_rel(m + 1, 0), d_rel(m + 1, 0);
+    for (uint32_t k = 0; k < m; k++) {
+        c_rel[k + 1] = c_rel[k] + (r.c_off[(*list)[k] + 1] - r.c_off[(*list)[k]]);
+        d_rel[k + 1] = d_rel[k] + (r.d_off[(*list)[k] + 1] - r.d_off[(*list)[k]]);
+    }
+    *base = r.d_off[(*list)[0]];
+    const uint32_t last = (*list)[m - 1];
+    std::vector<uint32_t> need;
+    if (r.d_off[last + 1] > hi) { need.assign(m, 0xFFFFFFFFu); need[m - 1] = (uint32_t)(hi - r.d_off[last]); }
+    const uint64_t block = 128u << 10, end = r.d_off[last + 1] - hi > block ? hi + block : r.d_off[last + 1];
+    ZkSlot& s = c->slot[0];
+    int32_t rc = zk_slot_ensure(&s, (size_t)c_rel[m] + 32, 0);
+    if (rc) return rc;
+    for (int i = 0; i < ZK_SLOTS; i++) if (c->slot[i].stream) cudaStreamSynchronize(c->slot[i].stream);    // nobody reads the arena any more
+    if ((rc = zk_grow(&c->d_prefix, &c->cap_prefix, ZK_REF_HEAD + (size_t)(end - *base) + 64, 1))) return rc;
+    for (uint32_t k0 = 0; k0 < m;) {                        // runs of consecutive entries in one copy
+        uint32_t k1 = k0 + 1;
+        while (k1 < m && (*list)[k1] == (*list)[k1 - 1] + 1) k1++;
+        const size_t bytes = (size_t)(c_rel[k1] - c_rel[k0]);
+        if (bytes) ZK_CUDA_OK(cudaMemcpyAsync(s.d_in + c_rel[k0], r.comp + r.c_off[(*list)[k0]], bytes, cudaMemcpyHostToDevice, s.stream));
+        k0 = k1;
+    }
+    ZkDecodeParams p;
+    if (!need.empty()) p.need = need.data();
+    status->assign(m, 0);
+    rc = zk_decode_batch(&s.dws, s.stream, s.d_in, c_rel.data(), d_rel.data(), m, (uint8_t*)c->d_prefix + ZK_REF_HEAD, verify, p, status->data());
+    c->ref_decoded += m;
+    if (rc == ZK_INT_CUDA || rc == -(int)ZKZ_MEMORY_ALLOCATION) return rc;
+    return 0;                                               // an entry that fails to decode: its status
+}
+
+// the first entry of *list (decoded by zk_ref_decode) with a non-zero status whose output overlaps [lo, hi) -> that status, else 0
+static int32_t zk_ref_failure(const ZkRefArchive& r, const std::vector<uint32_t>& list, const std::vector<int32_t>& status, uint64_t lo,
+                              uint64_t hi) {
+    for (size_t k = 0; k < list.size(); k++)
+        if (status[k] && r.d_off[list[k]] < hi && r.d_off[list[k] + 1] > lo) return status[k];
+    return 0;
+}
+
+// OLD [lo, hi) as a device prefix, for the calls that cannot use a partly decoded OLD: the first failing entry's status is the call's
+static int32_t zk_ref_prefix(zk_ctx* c, const ZkRefArchive& r, uint64_t lo, uint64_t hi, const uint8_t** prefix) {
+    std::vector<uint32_t> list;
+    std::vector<int32_t> status;
+    uint64_t base = 0;
+    int32_t rc = zk_ref_decode(c, r, lo, hi, 1, &base, &list, &status);
+    if (!rc) rc = zk_ref_failure(r, list, status, lo, hi);
+    *prefix = (const uint8_t*)c->d_prefix + ZK_REF_HEAD + (lo - base);
+    return rc;
+}
+
+extern "C" int32_t zk_decompress_frames_prefixes_archive(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n,
+                                                         uint8_t* dst, const uint32_t* d_need, int32_t verify, int32_t* status,
+                                                         const uint8_t* ref_comp, size_t ref_len, const uint64_t* ref_c_off,
+                                                         const uint64_t* ref_d_off, uint32_t ref_n, const uint64_t* ranges) {
+    if (!c) return ZK_ERR_INVALID_ARG;
+    const ZkRefArchive r = {ref_comp, ref_len, ref_c_off, ref_d_off, ref_n};
+    uint64_t old_len = 0;
+    int32_t rc = zk_ref_check(r, &old_len);
+    if (rc) return rc;
+    std::vector<uint64_t> whole;                            // no ranges: every entry against all of OLD
+    if (!ranges) {
+        whole.assign(2 * (size_t)n, 0);
+        for (uint32_t i = 0; i < n; i++) whole[2 * (size_t)i + 1] = old_len;
+        ranges = whole.data();
+    }
+    for (uint32_t i = 0; i < n; i++)
+        if (ranges[2 * (size_t)i] > ranges[2 * (size_t)i + 1] || ranges[2 * (size_t)i + 1] > old_len) return ZK_ERR_INVALID_ARG;
+    if (n && (!comp || !c_off || !d_off || !dst)) return ZK_ERR_INVALID_ARG;
+    if (n == 0) return 0;
+    ZK_CUDA_OK(cudaSetDevice(c->device));
+    const uint64_t group = zk_patch_group_bytes();
+    std::vector<uint64_t> rb;
+    std::vector<uint32_t> list;
+    std::vector<int32_t> rst, st(n, 0), fail;
+    for (uint32_t f0 = 0; f0 < n;) {
+        uint64_t hlo, hhi, base = 0;
+        const uint32_t end = zk_hull_group(ranges, f0, n, group, &hlo, &hhi);
+        zk_rebase_ranges(ranges, f0, end, hlo, &rb);
+        list.clear();
+        if (hhi > hlo && (rc = zk_ref_decode(c, r, hlo, hhi, verify, &base, &list, &rst))) return rc;
+        const uint8_t* prefix = hhi > hlo ? (const uint8_t*)c->d_prefix + ZK_REF_HEAD + (hlo - base) : nullptr;
+        // an entry whose range overlaps a reference entry that failed takes its status; the others run in runs of consecutive entries
+        fail.assign(end - f0, 0);
+        for (uint32_t f = f0; f < end; f++)
+            if (ranges[2 * (size_t)f] < ranges[2 * (size_t)f + 1])
+                fail[f - f0] = zk_ref_failure(r, list, rst, ranges[2 * (size_t)f], ranges[2 * (size_t)f + 1]);
+        for (uint32_t a = f0; a < end;) {
+            if (fail[a - f0]) { st[a] = fail[a - f0]; a++; continue; }
+            uint32_t b = a + 1;
+            while (b < end && !fail[b - f0]) b++;
+            rc = zk_decompress_prefixes_one(c, comp, c_off + a, d_off + a, b - a, dst, d_need ? d_need + a : nullptr, verify, st.data() + a,
+                                            prefix, (size_t)(hhi - hlo), rb.data() + 2 * (size_t)(a - f0), true);
+            if (rc && !ZK_IS_ZSTD_ERR(rc)) return rc;       // the call failed; a frame's status does not stop the other groups
+            a = b;
+        }
+        f0 = end;
+    }
+    if (status) memcpy(status, st.data(), (size_t)n * 4);
+    for (uint32_t i = 0; i < n; i++) if (st[i]) return st[i];
+    return 0;
+}
+
+// frames of NEW against their ranges of OLD: zk_compress_frames_patch's groups, each hull decoded from R into the prefix arena
+extern "C" int32_t zk_compress_frames_patch_archive(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                                    int32_t checksum, const uint8_t* ref_comp, size_t ref_len, const uint64_t* ref_c_off,
+                                                    const uint64_t* ref_d_off, uint32_t ref_n, const uint64_t* ranges, uint8_t* dst,
+                                                    size_t dst_cap, uint32_t* c_sizes, size_t* dst_len) {
+    if (!c || (n_frames && (!frame_sizes || !ranges || !dst))) return ZK_ERR_INVALID_ARG;
+    const ZkRefArchive r = {ref_comp, ref_len, ref_c_off, ref_d_off, ref_n};
+    uint64_t old_len = 0;
+    int32_t rc = zk_ref_check(r, &old_len);
+    if (rc) return rc;
+    if (dst_len) *dst_len = 0;
+    for (uint32_t f = 0; f < n_frames; f++)
+        if (ranges[2 * (size_t)f] > ranges[2 * (size_t)f + 1] || ranges[2 * (size_t)f + 1] > old_len) return ZK_ERR_INVALID_ARG;
+    if (n_frames) ZK_CUDA_OK(cudaSetDevice(c->device));
+    const uint64_t group = zk_patch_group_bytes();
+    std::vector<uint64_t> rb;
+    std::vector<uint32_t> cs(n_frames);
+    size_t out = 0, in = 0;
+    for (uint32_t f0 = 0; f0 < n_frames;) {
+        uint64_t hlo, hhi;
+        const uint32_t end = zk_hull_group(ranges, f0, n_frames, group, &hlo, &hhi);
+        zk_rebase_ranges(ranges, f0, end, hlo, &rb);
+        size_t len = 0, bytes = 0;
+        for (uint32_t f = f0; f < end; f++) bytes += frame_sizes[f];
+        if (hhi > hlo) {
+            ZkCompressReq q;                                // zk_compress_frames_sized_prefixes(ldm = 1) on the decoded hull
+            q.policy = ZK_FRAMES_SIZED; q.sizes = frame_sizes + f0; q.count = end - f0; q.src = src ? src + in : nullptr;
+            if ((rc = zk_ref_prefix(c, r, hlo, hhi, &q.prefix))) return rc;
+            q.prefix_len = (size_t)(hhi - hlo); q.prefix_dev = true; q.ranges = rb.data();
+            q.params.level = level; q.params.checksum = checksum; q.params.ldm = true;
+            q.dst = dst + out; q.dst_cap = dst_cap - out; q.c_sizes = cs.data() + f0; q.dst_len = &len;
+            rc = zk_compress(c, q);
+        } else {
+            rc = zk_compress_frames_sized(c, src ? src + in : nullptr, frame_sizes + f0, end - f0, 16, checksum, nullptr, 0, dst + out,
+                                          dst_cap - out, cs.data() + f0, &len);
+        }
+        if (rc) return rc;
+        out += len; in += bytes; f0 = end;
+    }
+    if (c_sizes && n_frames) memcpy(c_sizes, cs.data(), (size_t)n_frames * 4);
+    if (dst_len) *dst_len = out;
+    return 0;
+}
+
+// the anchors of OLD = R's decoded content: R in runs of whole entries of at most ZK_PATCH_PIECE_BYTES (a larger entry alone), each run
+// decoded into the prefix arena with the 63 bytes of OLD before it copied in front, so every anchor is found once, as the raw pass finds it
+static int32_t zk_patch_scan_archive(zk_ctx* c, const ZkRefArchive& r, std::vector<unsigned long long>* keys, std::vector<unsigned long long>* pos) {
+    ZkSlot& s = c->slot[0];
+    const size_t piece = zk_patch_piece_bytes();
+    const size_t most = (size_t)1 << 30;                    // zk_patch_anchors' largest piece
+    int32_t rc = zk_slot_ensure(&s, 0, ZK_REF_HEAD);        // d_out: the tail of the run before, kept while the arena is reused
+    if (rc) return rc;
+    size_t ov = 0;
+    for (uint32_t g0 = 0; g0 < r.n;) {
+        uint32_t g1 = g0 + 1;
+        while (g1 < r.n && r.d_off[g1 + 1] - r.d_off[g0] <= piece) g1++;
+        const uint64_t lo = r.d_off[g0], hi = r.d_off[g1];
+        g0 = g1;
+        if (hi == lo) continue;
+        const uint8_t* unused;
+        if ((rc = zk_ref_prefix(c, r, lo, hi, &unused))) return rc;
+        uint8_t* run = (uint8_t*)c->d_prefix + ZK_REF_HEAD;
+        if (ov) ZK_CUDA_OK(cudaMemcpyAsync(run - ov, s.d_out, ov, cudaMemcpyDeviceToDevice, s.stream));
+        const uint64_t n = ov + (hi - lo);
+        for (uint64_t s0 = 0;;) {
+            const uint64_t e = n - s0 < most ? n : s0 + most;
+            if ((rc = zk_patch_anchors(&s.ews, s.stream, run - ov + s0, (size_t)(e - s0), lo - ov + s0, keys, pos))) return rc;
+            if (e == n) break;
+            s0 = e - 63;
+        }
+        const size_t nov = n < 63 ? (size_t)n : 63;
+        ZK_CUDA_OK(cudaMemcpyAsync(s.d_out, run + (hi - lo) - nov, nov, cudaMemcpyDeviceToDevice, s.stream));
+        ov = nov;
+    }
+    return zk_sync_check(s.stream);
+}
+
+extern "C" int32_t zk_patch_ranges_archive(zk_ctx* c, const uint8_t* new_src, const uint32_t* frame_sizes, uint32_t n_frames,
+                                           const uint8_t* ref_comp, size_t ref_len, const uint64_t* ref_c_off, const uint64_t* ref_d_off,
+                                           uint32_t ref_n, uint64_t margin, uint64_t* ranges) {
+    if (!c || (n_frames && (!frame_sizes || !ranges))) return ZK_ERR_INVALID_ARG;
+    const ZkRefArchive r = {ref_comp, ref_len, ref_c_off, ref_d_off, ref_n};
+    uint64_t old_len = 0;
+    int32_t rc = zk_ref_check(r, &old_len);
+    if (rc) return rc;
+    if (old_len >= (1ull << 62) || margin >= (1ull << 62)) return ZK_ERR_INVALID_ARG;
+    ZkPatchTables t;
+    t.fa.assign((size_t)n_frames + 1, 0);
+    for (uint32_t f = 0; f < n_frames; f++) t.fa[f + 1] = t.fa[f] + frame_sizes[f];
+    const uint64_t n = t.fa[n_frames];
+    if (n && !new_src) return ZK_ERR_INVALID_ARG;
+    if (n_frames == 0) return 0;
+    ZK_CUDA_OK(cudaSetDevice(c->device));
+    rc = zk_patch_scan_archive(c, r, &t.okeys, &t.opos);
+    if (!rc) rc = zk_patch_scan(c, new_src, n, &t.nkeys, &t.npos);
+    if (rc) return rc;
+    if (t.okeys.size() > 0xFFFFFFF0ull || t.nkeys.size() > 0xFFFFFFF0ull) return ZK_ERR_INVALID_ARG;
+    t.fanc.assign((size_t)n_frames + 1, 0);
+    for (uint32_t f = 0, i = 0; f <= n_frames; f++) {
+        while (i < t.npos.size() && t.npos[i] < t.fa[f]) i++;
+        t.fanc[f] = f == n_frames ? (uint32_t)t.npos.size() : i;
+    }
+    return zk_patch_join(&c->slot[0].ews, c->slot[0].stream, t, n_frames, old_len, margin, (unsigned long long*)ranges);
 }

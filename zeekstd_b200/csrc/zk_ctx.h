@@ -26,6 +26,7 @@ struct zk_ctx {
     float last_ms = 0.f;
     void* d_prefix = nullptr; size_t cap_prefix = 0;      // device copy of the raw-content prefix of the calls that take one
     unsigned long long prefix_uploaded = 0;               // prefix bytes copied to the device so far (zk_ctx_prefix_bytes_uploaded)
+    unsigned long long ref_decoded = 0;                   // reference-archive entries decoded so far (zk_ctx_reference_entries_decoded)
     void* d_reuse[4] = {}; size_t cap_reuse[4] = {};      // zk_compress_frames_sized_reuse: old entries, their decoded bytes, the changed
                                                           // frames, the assembled output
     unsigned long long launches() const {

@@ -555,6 +555,8 @@ struct zk_decoder {                        // decode.rs:121-466
     size_t max_window_bytes = (size_t)256 << 20;
     const uint8_t* prefix = nullptr; size_t prefix_len = 0;   // the prefix the window was decoded with (decompress_with_prefix)
     const uint64_t* ranges = nullptr;                          // and every entry's range of it (nullptr: the whole prefix)
+    bool archive = false;                                      // the prefix is the decoded content of this reference archive instead
+    const uint64_t* ref_c_off = nullptr; const uint64_t* ref_d_off = nullptr; uint32_t ref_n = 0;
 
     void reset_dctx() { read_compressed = 0; win_lo = win_hi = 0; win_valid_end = 0; window.clear(); }                           // :352-357
     int32_t check_offset(uint64_t off) const { return off > seek_table.d.back() ? ZK_ERR_OFFSET_OUT_OF_RANGE : 0; }   // :439-445
@@ -583,8 +585,11 @@ struct zk_decoder {                        // decode.rs:121-466
             need.assign(n, 0xFFFFFFFFu);
             need[n - 1] = (uint32_t)(need_end - seek_table.d[f1 - 1]);
         } else need_end = d1;
-        rc = zk_decompress_frames_prefixes(ctx, comp.data(), co.data(), dof.data(), n, window.data(), need.empty() ? nullptr : need.data(), 1, nullptr,
-                                           prefix, prefix_len, ranges ? ranges + 2 * (size_t)f0 : nullptr);
+        const uint32_t* np = need.empty() ? nullptr : need.data();
+        const uint64_t* rg = ranges ? ranges + 2 * (size_t)f0 : nullptr;
+        rc = archive ? zk_decompress_frames_prefixes_archive(ctx, comp.data(), co.data(), dof.data(), n, window.data(), np, 1, nullptr, prefix,
+                                                             prefix_len, ref_c_off, ref_d_off, ref_n, rg)
+                     : zk_decompress_frames_prefixes(ctx, comp.data(), co.data(), dof.data(), n, window.data(), np, 1, nullptr, prefix, prefix_len, rg);
         if (rc) { win_lo = win_hi = 0; win_valid_end = 0; return rc; }
         win_lo = f0; win_hi = f1; win_valid_end = need_end;
         return 0;
@@ -629,12 +634,32 @@ extern "C" int32_t zk_decoder_decompress_with_prefix(zk_decoder* d, uint8_t* buf
     return zk_decoder_decompress_with_prefix_ranges(d, buf, len, prefix, prefix_len, nullptr, produced);
 }
 
+static int32_t zk_decoder_run(zk_decoder* d, uint8_t* buf, size_t len, size_t* produced);
+
 extern "C" int32_t zk_decoder_decompress_with_prefix_ranges(zk_decoder* d, uint8_t* buf, size_t len, const uint8_t* prefix, size_t prefix_len,
                                                             const uint64_t* ranges, size_t* produced) {
-    if (prefix != d->prefix || prefix_len != d->prefix_len || ranges != d->ranges) {   // frames decoded under another prefix are not reusable
+    if (d->archive || prefix != d->prefix || prefix_len != d->prefix_len || ranges != d->ranges) {   // frames decoded under another prefix are not reusable
         d->win_lo = d->win_hi = 0; d->win_valid_end = 0;
-        d->prefix = prefix; d->prefix_len = prefix_len; d->ranges = ranges;
+        d->prefix = prefix; d->prefix_len = prefix_len; d->ranges = ranges; d->archive = false;
     }
+    return zk_decoder_run(d, buf, len, produced);
+}
+
+// the reference archive's bytes and length stand in prefix / prefix_len
+extern "C" int32_t zk_decoder_decompress_with_reference_archive(zk_decoder* d, uint8_t* buf, size_t len, const uint8_t* ref_comp, size_t ref_len,
+                                                                const uint64_t* ref_c_off, const uint64_t* ref_d_off, uint32_t ref_n,
+                                                                const uint64_t* ranges, size_t* produced) {
+    if (!d->archive || ref_comp != d->prefix || ref_len != d->prefix_len || ranges != d->ranges || ref_c_off != d->ref_c_off ||
+        ref_d_off != d->ref_d_off || ref_n != d->ref_n) {
+        d->win_lo = d->win_hi = 0; d->win_valid_end = 0;
+        d->prefix = ref_comp; d->prefix_len = ref_len; d->ranges = ranges; d->archive = true;
+        d->ref_c_off = ref_c_off; d->ref_d_off = ref_d_off; d->ref_n = ref_n;
+    }
+    return zk_decoder_run(d, buf, len, produced);
+}
+
+// decode.rs:201-270 with the prefix the decoder holds
+static int32_t zk_decoder_run(zk_decoder* d, uint8_t* buf, size_t len, size_t* produced) {
     size_t progress = 0;
     const uint32_t nframes = d->seek_table.num_frames();
     while (d->offset < d->offset_limit && progress < len && nframes) {
