@@ -44,6 +44,7 @@ extern "C" {
 #define ZK_SKIPPABLE_HEADER_SIZE 8u
 #define ZK_DEFAULT_FRAME_SIZE 0x200000u /* FrameSizePolicy::default(), encode.rs:33-39 */
 #define ZK_PATCH_SLICES_MAGIC 0x184D2A5Bu /* the skippable frame of a seekable patch's slices (zk_patch_slices_write) */
+#define ZK_CHAIN_MAX_DEPTH 32u /* the most archives in a reference chain (the _chain calls of the patch block) */
 
 /* Compression levels (the `level` argument of every compress entry point and of zk_encode_options_compression_level), as in libzstd:
  *   0                 the default, level 3;
@@ -333,7 +334,8 @@ int32_t zk_patch_slices_read(const uint8_t* src, size_t len, uint32_t n_frames, 
  * An entry of R that fails to decode: every entry being decompressed whose range overlaps its output gets its status (the return code is
  * the first non-zero status, as in the raw-reference call; the others decode normally); the compress and range calls return it.
  * ZK_ERR_INVALID_ARG: R's offsets decrease, ref_d_off[0] != 0, ref_c_off[ref_n] > ref_len, a range with lo > hi or hi > old_len, or R is
- * itself a seekable patch (ZK_PATCH_SLICES_MAGIC at ref_c_off[0]: chains are not resolved).  Other argument errors as in the raw calls.
+ * itself a seekable patch (ZK_PATCH_SLICES_MAGIC at ref_c_off[0]: such a reference goes to the _chain calls below, with its own reference
+ * under it).  Other argument errors as in the raw calls.  Each _archive call is its _chain call with depth 1.
  */
 int32_t zk_patch_ranges_archive(zk_ctx* ctx, const uint8_t* new_src, const uint32_t* frame_sizes, uint32_t n_frames, const uint8_t* ref_comp,
                                 size_t ref_len, const uint64_t* ref_c_off, const uint64_t* ref_d_off, uint32_t ref_n, uint64_t margin,
@@ -346,6 +348,37 @@ int32_t zk_decompress_frames_prefixes_archive(zk_ctx* ctx, const uint8_t* comp, 
                                               uint8_t* dst, const uint32_t* d_need, int32_t verify_checksum, int32_t* status,
                                               const uint8_t* ref_comp, size_t ref_len, const uint64_t* ref_c_off, const uint64_t* ref_d_off,
                                               uint32_t ref_n, const uint64_t* ranges);
+
+/*
+ * Seekable patch chains (DESIGN §3.4.3): the reference is a chain R_0 ... R_{depth-1} of archives (root first, 1 <= depth <=
+ * ZK_CHAIN_MAX_DEPTH), each described as the _archive calls take one (host memory; comp may be mmapped).  R_0 is a plain seekable archive;
+ * every R_i with i >= 1 is a seekable patch whose slice frame (zk_patch_slices_read, n slices) has old_len = R_{i-1}'s decoded length and is
+ * applied against R_{i-1}'s decoded content.  OLD is the decoded content of the head R_{depth-1}.  The library reads each patch level's
+ * slice frame itself.
+ *   Every _chain call returns exactly what its raw call returns on OLD (the same ranges, archive bytes, c_sizes, output, statuses and
+ *   return code); with depth 1 it is its _archive call, which runs this same code.  No byte of any level's content goes to the host.
+ *   What is decoded: Need(i, [lo, hi)) decodes the non-empty entries of R_i whose output overlaps [lo, hi) into level i's device arena, the
+ *   last one only as far as hi.  For i >= 1 their slices are grouped in list order as zk_decompress_frames_prefixes groups ranges (hull at
+ *   most 1 GiB, empty slices skipped); for each group with a non-empty hull Need(i - 1, hull) runs first, then the group's entries are
+ *   decoded against it.  The top of the chain runs Need(depth - 1, ...) where the _archive calls decode R.  zk_ctx_reference_entries_decoded
+ *   counts every entry decoded at every level, each time it is decoded.
+ *   Failures propagate upward: an entry of R_{i-1} that fails (corrupt, or a bad checksum on a full entry with verification on) gives its
+ *   status to every entry of R_i in the same group whose slice overlaps its output (the first failing entry's in list order); those are not
+ *   decoded and count as failed for level i + 1.  At the top, statuses are as in the _archive calls.  The decompress call verifies full
+ *   entries at every level when verify_checksum is set; the compress and range calls always do, and return the first failure.
+ * ZK_ERR_INVALID_ARG: depth == 0 or > ZK_CHAIN_MAX_DEPTH, a root that is a seekable patch, an R_i (i >= 1) without a valid slice frame of
+ * its entry count, an old_len that differs from R_{i-1}'s decoded length, any level failing the _archive calls' offset rules, a range
+ * past OLD's length.  Device memory: per level below the head, about its hull plus one entry plus one 128 KiB block.
+ */
+typedef struct { const uint8_t* comp; size_t len; const uint64_t* c_off; const uint64_t* d_off; uint32_t n; } zk_reference_archive;
+int32_t zk_patch_ranges_chain(zk_ctx* ctx, const uint8_t* new_src, const uint32_t* frame_sizes, uint32_t n_frames,
+                              const zk_reference_archive* chain, uint32_t depth, uint64_t margin, uint64_t* ranges);
+int32_t zk_compress_frames_patch_chain(zk_ctx* ctx, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                       int32_t checksum, const zk_reference_archive* chain, uint32_t depth, const uint64_t* ranges, uint8_t* dst,
+                                       size_t dst_cap, uint32_t* c_sizes, size_t* dst_len);
+int32_t zk_decompress_frames_prefixes_chain(zk_ctx* ctx, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n,
+                                            uint8_t* dst, const uint32_t* d_need, int32_t verify_checksum, int32_t* status,
+                                            const zk_reference_archive* chain, uint32_t depth, const uint64_t* ranges);
 
 /*
  * The content-defined cut alone (FrameSizePolicy::ContentDefined(size), the rule of zk_compress_frames_cdc): frame_sizes, *n_frames and
@@ -517,6 +550,10 @@ int32_t zk_decoder_decompress_with_prefix_ranges(zk_decoder* d, uint8_t* buf, si
 int32_t zk_decoder_decompress_with_reference_archive(zk_decoder* d, uint8_t* buf, size_t len, const uint8_t* ref_comp, size_t ref_len,
                                                      const uint64_t* ref_c_off, const uint64_t* ref_d_off, uint32_t ref_n,
                                                      const uint64_t* ranges, size_t* produced);
+/* the same with the prefix being OLD of a reference chain (zk_decompress_frames_prefixes_chain's arguments).  The decoder keeps a copy of
+ * the depth descriptors: a call whose chain differs from the previous call's at any level decodes its window again */
+int32_t zk_decoder_decompress_with_reference_chain(zk_decoder* d, uint8_t* buf, size_t len, const zk_reference_archive* chain, uint32_t depth,
+                                                   const uint64_t* ranges, size_t* produced);
 void zk_decoder_reset(zk_decoder* d);                                                    /* :346-350 */
 int32_t zk_decoder_set_lower_frame(zk_decoder* d, uint32_t index, uint64_t* offset);    /* :367 */
 int32_t zk_decoder_set_upper_frame(zk_decoder* d, uint32_t index, uint64_t* offset);    /* :383 */

@@ -265,7 +265,7 @@ class Context:
         zk_decompress_frames_upto): the rest of a frame's output range is then unspecified and its checksum is not verified.
         prefix_ranges (n x 2 integers): entry e is decoded against prefix[prefix_ranges[e][0]:prefix_ranges[e][1]] only
         (zk_decompress_frames_prefixes).  prefix may be a ReferenceArchive: its decoded content is the prefix, and only the entries
-        under the ranges are decoded, on the GPU (zk_decompress_frames_prefixes_archive)."""
+        under the ranges are decoded, on the GPU, at every level of its chain (zk_decompress_frames_prefixes_chain)."""
         addr, n, keep = _buf(comp)
         co = np.ascontiguousarray(c_off, dtype=np.uint64); do = np.ascontiguousarray(d_off, dtype=np.uint64)
         nf = len(co) - 1
@@ -280,10 +280,10 @@ class Context:
             raise ValueError("need: one entry per frame")
         if isinstance(prefix, ReferenceArchive):
             rg = None if prefix_ranges is None else _ranges(prefix_ranges, nf)
-            rc = self.lib.zk_decompress_frames_prefixes_archive(self._h, addr, co.ctypes.data_as(_native.u64p), do.ctypes.data_as(_native.u64p),
-                                                                nf, out.ctypes.data, None if nd is None else nd.ctypes.data_as(_native.u32p),
-                                                                int(verify_checksum), st.ctypes.data_as(_native.i32p), *prefix._args(),
-                                                                None if rg is None else rg.ctypes.data_as(_native.u64p))
+            rc = self.lib.zk_decompress_frames_prefixes_chain(self._h, addr, co.ctypes.data_as(_native.u64p), do.ctypes.data_as(_native.u64p),
+                                                              nf, out.ctypes.data, None if nd is None else nd.ctypes.data_as(_native.u32p),
+                                                              int(verify_checksum), st.ctypes.data_as(_native.i32p), *prefix._chain(),
+                                                              None if rg is None else rg.ctypes.data_as(_native.u64p))
             return out[:total], st[:nf], rc
         paddr, pn, pkeep = _buf(prefix) if prefix is not None else (None, 0, None)
         if prefix_ranges is not None:
@@ -314,7 +314,7 @@ class Context:
         """the slice of `old` each frame of `new` is matched against in a seekable patch -> n x 2 np.uint64 (lo, hi), found on the GPU by
         content anchors (the rule: include/zeekstd_b200.h, zk_patch_ranges).  margin: bytes added on each side (default: the largest frame
         size, which is the frame size of uniform frames).  old may be a ReferenceArchive: the same ranges, with OLD decoded on the GPU
-        (zk_patch_ranges_archive)"""
+        (zk_patch_ranges_chain)"""
         addr, n, keep = _buf(new)
         ds = np.ascontiguousarray(frame_sizes, dtype=np.uint32).reshape(-1)
         if int(np.sum(ds, dtype=np.uint64)) != n:
@@ -322,8 +322,8 @@ class Context:
         m = int(ds.max()) if margin is None and ds.size else int(margin or 0)
         rg = np.zeros((max(ds.size, 1), 2), dtype=np.uint64)
         if isinstance(old, ReferenceArchive):
-            _check(self.lib.zk_patch_ranges_archive(self._h, addr, ds.ctypes.data_as(_native.u32p), ds.size, *old._args(), m,
-                                                    rg.ctypes.data_as(_native.u64p)), self.lib)
+            _check(self.lib.zk_patch_ranges_chain(self._h, addr, ds.ctypes.data_as(_native.u32p), ds.size, *old._chain(), m,
+                                                  rg.ctypes.data_as(_native.u64p)), self.lib)
             return rg[: ds.size]
         oaddr, on, okeep = _buf(old)
         _check(self.lib.zk_patch_ranges(self._h, addr, ds.ctypes.data_as(_native.u32p), ds.size, oaddr, on, m,
@@ -334,7 +334,7 @@ class Context:
         """frame f of `new` against old[ranges[f][0]:ranges[f][1]] with long-distance matching, for an `old` of any size
         (zk_compress_frames_patch) -> (compressed bytes (np.uint8), c_sizes, d_sizes).  Frame f is what compress_frames_sized(frame alone,
         prefix=old, long_distance=True, prefix_ranges=[ranges[f]]) writes.  old may be a ReferenceArchive: the same bytes, with each group's
-        slices of OLD decoded on the GPU (zk_compress_frames_patch_archive)"""
+        slices of OLD decoded on the GPU (zk_compress_frames_patch_chain)"""
         addr, n, keep = _buf(new)
         ds = np.ascontiguousarray(frame_sizes, dtype=np.uint32).reshape(-1)
         if int(np.sum(ds, dtype=np.uint64)) != n:
@@ -346,9 +346,9 @@ class Context:
         cs = np.zeros(max(ds.size, 1), dtype=np.uint32)
         dl = c_size_t()
         if isinstance(old, ReferenceArchive):
-            _check(self.lib.zk_compress_frames_patch_archive(self._h, addr, dsp, ds.size, level, int(checksum), *old._args(),
-                                                             rg.ctypes.data_as(_native.u64p), dst.ctypes.data, cap, cs.ctypes.data_as(_native.u32p),
-                                                             byref(dl)), self.lib)
+            _check(self.lib.zk_compress_frames_patch_chain(self._h, addr, dsp, ds.size, level, int(checksum), *old._chain(),
+                                                           rg.ctypes.data_as(_native.u64p), dst.ctypes.data, cap, cs.ctypes.data_as(_native.u32p),
+                                                           byref(dl)), self.lib)
             return dst[: dl.value], cs[: ds.size], ds.copy()
         oaddr, on, okeep = _buf(old)
         _check(self.lib.zk_compress_frames_patch(self._h, addr, dsp, ds.size, level, int(checksum), oaddr, on, rg.ctypes.data_as(_native.u64p),
@@ -358,7 +358,7 @@ class Context:
     def compress_patch_slices(self, new, frame_sizes, old, level: int = 0, checksum: bool = False, margin: int | None = None) -> bytes:
         """a seekable patch of `new` against `old` -> the archive's bytes: the slice frame (the ranges of patch_ranges), then the frames
         of compress_frames_patch, then the Foot seek table.  Entry 0's compressed size includes the slice frame.  old may be a
-        ReferenceArchive: the same bytes."""
+        ReferenceArchive, chained or not: the same bytes."""
         ds = np.ascontiguousarray(frame_sizes, dtype=np.uint32).reshape(-1)
         if ds.size == 0:
             raise ValueError("a seekable patch has at least one frame")
@@ -378,10 +378,13 @@ class ReferenceArchive:
     """a seekable archive as the reference (OLD) of a seekable patch: OLD is its decoded content, and the patch calls that take one decode
     on the GPU only the entries of it they need (DESIGN §3.4.2).  data: the archive's bytes or a mapping of it (kept, not copied).  Its
     entries come from the Foot seek table at its end (the default), from seek_table (a SeekTable, or the bytes of one in `format`, e.g.
-    a stand-alone Head table), or from explicit c_off / d_off (n + 1 offsets each, as Context.decompress_frames takes them).  A seekable
-    patch (the slice frame at the start of its first entry) is refused: chains of patches are not resolved."""
+    a stand-alone Head table), or from explicit c_off / d_off (n + 1 offsets each, as Context.decompress_frames takes them).
+    A seekable patch (the slice frame at the start of its first entry) needs `base`: the ReferenceArchive of the version it was made
+    against, which may itself be a patch with a base of its own.  OLD is then the patch applied to its base's decoded content, and the
+    calls decode every level of the chain on the GPU, each only where the level above reads it (DESIGN §3.4.3).  Without `base` a patch is
+    refused; a `base` under a plain archive, or one whose decoded length is not the slice frame's old_len, is a ValueError."""
 
-    def __init__(self, data, seek_table=None, format: int = Format.Foot, c_off=None, d_off=None, lib=None):
+    def __init__(self, data, seek_table=None, format: int = Format.Foot, c_off=None, d_off=None, lib=None, base=None):
         self.lib = lib or _native.default_lib()
         self._addr, self._len, self._keep = _buf(data)
         if c_off is not None or d_off is not None:
@@ -399,8 +402,21 @@ class ReferenceArchive:
         self.c_off, self.d_off = co, do
         c0 = int(co[0])
         view = self._keep if isinstance(self._keep, np.ndarray) else self._keep[0]
-        if int(co[-1]) - c0 >= 4 and c0 + 4 <= self._len and int.from_bytes(view[c0:c0 + 4].tobytes(), "little") == PATCH_SLICES_MAGIC:
-            raise ValueError("the reference archive is a seekable patch; restore it first")
+        patch = int(co[-1]) - c0 >= 4 and c0 + 4 <= self._len and int.from_bytes(view[c0:c0 + 4].tobytes(), "little") == PATCH_SLICES_MAGIC
+        if base is None:
+            if patch:
+                raise ValueError("the reference archive is a seekable patch; restore it first")
+        elif not isinstance(base, ReferenceArchive):
+            raise ValueError("base: the ReferenceArchive of the version the patch was made against")
+        elif not patch:
+            raise ValueError("base is for a seekable patch; this reference archive is a plain one")
+        else:
+            old_len = patch_slices_read(view[c0:int(co[-1])], self.n_entries, self.lib)[0]
+            if old_len != base.old_len:
+                raise ValueError(f"the base decodes to {base.old_len} bytes, the seekable patch was made against {old_len} bytes")
+            if base.depth >= _native.CHAIN_MAX_DEPTH:
+                raise ValueError(f"a reference chain has at most {_native.CHAIN_MAX_DEPTH} levels")
+        self.base = base
 
     @property
     def n_entries(self) -> int: return len(self.c_off) - 1
@@ -410,9 +426,24 @@ class ReferenceArchive:
         """bytes of OLD, the archive's decoded content"""
         return int(self.d_off[-1])
 
-    def _args(self):
-        """the (ref_comp, ref_len, ref_c_off, ref_d_off, ref_n) arguments of the _archive calls"""
-        return (self._addr, self._len, self.c_off.ctypes.data_as(_native.u64p), self.d_off.ctypes.data_as(_native.u64p), self.n_entries)
+    @property
+    def depth(self) -> int:
+        """levels of the chain this reference heads: 1 for a plain archive"""
+        return 1 if self.base is None else self.base.depth + 1
+
+    @property
+    def chain(self) -> list:
+        """the ReferenceArchive of every level, root first (the last is this one)"""
+        return [self] if self.base is None else self.base.chain + [self]
+
+    def _chain(self):
+        """the (chain, depth) arguments of the _chain calls (the array keeps no level alive: hold self while it is used)"""
+        levels = self.chain
+        arr = (_native.ReferenceArchiveDesc * len(levels))()
+        for d, r in zip(arr, levels):
+            d.comp, d.len, d.n = r._addr, r._len, r.n_entries
+            d.c_off, d.d_off = r.c_off.ctypes.data_as(_native.u64p), r.d_off.ctypes.data_as(_native.u64p)
+        return arr, len(levels)
 
 
 def patch_slices_size(n_frames: int) -> int:
@@ -855,7 +886,7 @@ class Decoder(io.RawIOBase):
         """decode.rs:201-270: every frame is decoded against the raw-content prefix.  ranges (one (lo, hi) pair per seek-table entry): entry
         e is decoded against prefix[lo:hi] only, and only the slices of the frames read go to the device (a seekable patch,
         zk_decoder_decompress_with_prefix_ranges).  prefix may be a ReferenceArchive: each window of frames then decodes only the entries
-        of it under its ranges, on the GPU (zk_decoder_decompress_with_reference_archive)"""
+        of it under its ranges, on the GPU (zk_decoder_decompress_with_reference_chain)"""
         if prefix is None:
             return self.decompress(buf)
         mv = memoryview(buf)
@@ -870,7 +901,7 @@ class Decoder(io.RawIOBase):
                 if getattr(self, "_ranges_src", None) is not ranges:    # the same array on every call keeps the decoded window valid
                     self._ranges_src, self._ranges = ranges, _ranges(ranges, self.seek_table().num_frames())
                 rp = self._ranges.ctypes.data_as(_native.u64p)
-            _check(self.lib.zk_decoder_decompress_with_reference_archive(self._h, arr, len(mv), *prefix._args(), rp, byref(p)), self.lib)
+            _check(self.lib.zk_decoder_decompress_with_reference_chain(self._h, arr, len(mv), *prefix._chain(), rp, byref(p)), self.lib)
             return int(p.value)
         paddr, pn, pkeep = _buf(prefix)
         self._prefix_keep = pkeep

@@ -39,6 +39,14 @@ class Seekable(ctypes.Structure):
     _fields_ = [("user", c_void_p), ("set_offset", SET_OFFSET_FN), ("read", READ_FN)]
 
 
+class ReferenceArchiveDesc(ctypes.Structure):
+    """zk_reference_archive: one level of a reference chain"""
+    _fields_ = [("comp", c_void_p), ("len", c_size_t), ("c_off", u64p), ("d_off", u64p), ("n", c_uint32)]
+
+
+chainp = POINTER(ReferenceArchiveDesc)
+CHAIN_MAX_DEPTH = 32                       # ZK_CHAIN_MAX_DEPTH
+
 _SIGS = {
     "zk_error_name": (c_char_p, [c_int32]),
     "zk_version": (c_char_p, []),
@@ -104,6 +112,11 @@ _SIGS = {
                                                    c_uint32, u64p, c_void_p, c_size_t, u32p, POINTER(c_size_t)]),
     "zk_decompress_frames_prefixes_archive": (c_int32, [c_void_p, c_void_p, u64p, u64p, c_uint32, c_void_p, u32p, c_int32, i32p, c_void_p,
                                                         c_size_t, u64p, u64p, c_uint32, u64p]),
+    "zk_patch_ranges_chain": (c_int32, [c_void_p, c_void_p, u32p, c_uint32, chainp, c_uint32, c_uint64, u64p]),
+    "zk_compress_frames_patch_chain": (c_int32, [c_void_p, c_void_p, u32p, c_uint32, c_int32, c_int32, chainp, c_uint32, u64p, c_void_p,
+                                                 c_size_t, u32p, POINTER(c_size_t)]),
+    "zk_decompress_frames_prefixes_chain": (c_int32, [c_void_p, c_void_p, u64p, u64p, c_uint32, c_void_p, u32p, c_int32, i32p, chainp,
+                                                      c_uint32, u64p]),
     "zk_cut_frames_cdc": (c_int32, [c_void_p, c_void_p, c_size_t, c_uint32, c_int32, u32p, c_uint32, u32p, POINTER(c_size_t)]),
     "zk_compress_frames_sized_reuse": (c_int32, [c_void_p, c_void_p, u32p, c_uint32, c_int32, c_int32, c_int32, c_void_p, c_size_t, u64p,
                                                  u64p, c_uint32, c_void_p, c_size_t, u32p, u32p, POINTER(c_size_t)]),
@@ -177,6 +190,7 @@ _SIGS = {
     "zk_decoder_decompress_with_prefix_ranges": (c_int32, [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, u64p, POINTER(c_size_t)]),
     "zk_decoder_decompress_with_reference_archive": (c_int32, [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, u64p, u64p, c_uint32, u64p,
                                                                POINTER(c_size_t)]),
+    "zk_decoder_decompress_with_reference_chain": (c_int32, [c_void_p, c_void_p, c_size_t, chainp, c_uint32, u64p, POINTER(c_size_t)]),
     "zk_decoder_reset": (None, [c_void_p]),
     "zk_decoder_set_lower_frame": (c_int32, [c_void_p, c_uint32, u64p]),
     "zk_decoder_set_upper_frame": (c_int32, [c_void_p, c_uint32, u64p]),

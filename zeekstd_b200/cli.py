@@ -1,8 +1,10 @@
 """Command-line front end with the reference CLI's arguments and behaviour (SURVEY.md 8f.4), over the GPU codec.
 
-    python -m zeekstd_b200 [compress] [-l N] [-s 2M] [--frame-size-policy ..] [--patch-from F [--long | --patch-slices [--patch-archive]]]
-                           [--long-mode] [--reuse-from OLD.zst] [INPUT] [-o OUT]
-    python -m zeekstd_b200 decompress [--from N | --from-frame I] [--to N|end | --to-frame I|end] [--patch-apply F [--patch-archive]] INPUT [-o OUT]
+    python -m zeekstd_b200 [compress] [-l N] [-s 2M] [--frame-size-policy ..]
+                           [--patch-from F [--long | --patch-slices [--patch-archive [--patch-base B]...]]] [--long-mode]
+                           [--reuse-from OLD.zst] [INPUT] [-o OUT]
+    python -m zeekstd_b200 decompress [--from N | --from-frame I] [--to N|end | --to-frame I|end]
+                           [--patch-apply F [--patch-archive [--patch-base B]...]] INPUT [-o OUT]
     python -m zeekstd_b200 list [--from-frame I] [--to-frame I|end | --num-frames N] [-d] [--seek-table-format head|foot] INPUT
 
 What each piece follows in the reference: argument set and value parsers cli/src/args.rs:10-329; sub-commands, output
@@ -27,7 +29,9 @@ whose bytes a frame of OLD.zst holds is copied from it, only the others are comp
 against its own slice of F, found by content anchors and recorded in a skippable frame at the start of the archive, and `decompress
 --patch-apply F` reads only the slices of the frames it restores.  With `--patch-archive` (also an extension) F is a seekable archive
 whose decoded content is the reference: it is decoded on the GPU, and only the entries under the slices a command needs are.  The flag
-is explicit because a raw reference file may itself be a .zst file.
+is explicit because a raw reference file may itself be a .zst file.  When F is itself a seekable patch, `--patch-base B` names the
+archive it was made against, and is repeated for B's own reference, nearest first, down to a plain seekable archive: every level of
+that chain is decoded on the GPU, each only where the level above reads it, and no version is restored on the host.
 """
 from __future__ import annotations
 
@@ -174,6 +178,9 @@ def build_parser() -> argparse.ArgumentParser:
     c.add_argument("--patch-archive", action="store_true",
                    help="With --patch-slices: the --patch-from file is a seekable archive, and the reference is its decoded content, "
                         "decoded on the GPU entry by entry. The patch is the one made against the decoded file.")
+    c.add_argument("--patch-base", action="append", default=None, metavar="FILE",
+                   help="With --patch-archive, when the --patch-from archive is itself a seekable patch: the archive it was made against. "
+                        "Repeat it for that file's own reference, nearest first, ending at a plain seekable archive.")
     c.add_argument("--reuse-from", default=None, metavar="OLD.zst",
                    help="The archive of a previous version of the input (ending in its seek table): every frame whose bytes one of its "
                         "frames already holds is copied from it, only the others are compressed. The output is what compress writes "
@@ -193,6 +200,9 @@ def build_parser() -> argparse.ArgumentParser:
     d.add_argument("--patch-archive", action="store_true",
                    help="With --patch-apply: the reference is a seekable archive; only its entries under the slices of the frames restored "
                         "are decoded, on the GPU.")
+    d.add_argument("--patch-base", action="append", default=None, metavar="FILE",
+                   help="With --patch-archive, when the --patch-apply archive is itself a seekable patch: the archive it was made against. "
+                        "Repeat it for that file's own reference, nearest first, ending at a plain seekable archive.")
     d.add_argument("input_file")
     d.add_argument("-o", "--output-file", default=None)
 
@@ -270,18 +280,40 @@ def _new_writer(out_path, in_path, quiet: bool, force: bool):
     return sys.stdout.buffer
 
 
-def _load_reference(zk, path):
-    """a reference archive (--patch-archive): the file mapped, its Foot seek table parsed"""
-    try:
-        data = np.memmap(path, dtype=np.uint8, mode="r") if os.path.getsize(path) > 0 else np.zeros(0, dtype=np.uint8)
-    except OSError as e:
-        raise CliError(f"Failed to load reference archive: {e}")
-    try:
-        return zk.ReferenceArchive(data)
-    except zk.Error as e:
-        raise CliError(f"Failed to parse the seek table of {path}: {e}")
-    except ValueError:
-        raise CliError(f"{path} is a seekable patch; restore it first")
+def _load_reference(zk, path, bases=None):
+    """a reference archive (--patch-archive): the file mapped, its Foot seek table parsed.  bases (--patch-base, nearest first): when it
+    is a seekable patch, the chain of archives under it, ending at a plain one"""
+    paths = [path] + list(bases or [])
+    ref = None
+    for i in range(len(paths) - 1, -1, -1):                # root first
+        p = paths[i]
+        try:
+            data = np.memmap(p, dtype=np.uint8, mode="r") if os.path.getsize(p) > 0 else np.zeros(0, dtype=np.uint8)
+        except OSError as e:
+            raise CliError(f"Failed to load reference archive: {e}")
+        try:
+            table = zk.SeekTable.from_bytes(data, zk.Format.Foot)
+        except zk.Error as e:
+            raise CliError(f"Failed to parse the seek table of {p}: {e}")
+        co, _ = table.offsets()
+        c0, c1 = int(co[0]), int(co[-1])
+        patch = c1 - c0 >= 4 and c0 + 4 <= data.size and int.from_bytes(data[c0:c0 + 4].tobytes(), "little") == zk.PATCH_SLICES_MAGIC
+        if ref is None and patch:
+            raise CliError(f"{p} is a seekable patch; restore it first")
+        if ref is not None:
+            if not patch:
+                raise CliError(f"{p} is not a seekable patch: --patch-base {paths[i + 1]} goes only after a seekable patch")
+            try:
+                old_len = zk.patch_slices_read(data[c0:c1], table.num_frames())[0]
+            except zk.Error as e:
+                raise CliError(f"Failed to read the slices of the seekable patch {p}: {e}")
+            if old_len != ref.old_len:
+                raise CliError(f"{paths[i + 1]} decodes to {ref.old_len} bytes, the seekable patch {p} was made against {old_len} bytes")
+        try:
+            ref = zk.ReferenceArchive(data, seek_table=table, base=ref)
+        except ValueError as e:
+            raise CliError(str(e))
+    return ref
 
 
 def _load_prefix(path, use_mmap: bool):
@@ -382,6 +414,8 @@ def _run_compress(zk, ns, fmt_bytes) -> int:
             raise CliError("--patch-slices needs a frame size above 0")
     elif ns.patch_margin is not None:
         raise CliError("--patch-margin needs --patch-slices")
+    if ns.patch_base and not ns.patch_archive:
+        raise CliError("--patch-base needs --patch-archive: it names the reference archive's own reference")
     if ns.patch_archive and (not ns.patch_slices or ns.long):
         raise CliError("--patch-archive needs --patch-from and --patch-slices: whole-prefix patches against an archive are not supported")
     if ns.reuse_from is not None:
@@ -392,7 +426,7 @@ def _run_compress(zk, ns, fmt_bytes) -> int:
         if ns.frame_size == 0:
             raise CliError("--reuse-from needs a frame size above 0")
     prefix_len = os.path.getsize(ns.patch_from) if ns.patch_from and os.path.exists(ns.patch_from) else None
-    ns.reference = _load_reference(zk, ns.patch_from) if ns.patch_archive else None
+    ns.reference = _load_reference(zk, ns.patch_from, ns.patch_base) if ns.patch_archive else None
     st_file = None
     if ns.seek_table_file is not None:
         try:
@@ -566,9 +600,11 @@ def _run_compress_reuse(zk, ns, fmt_bytes, reader, writer, in_path, out_path, st
 def _run_decompress(zk, ns, fmt_bytes) -> int:
     in_path = ns.input_file
     out_path = _out_path(ns, in_path)
+    if ns.patch_base and not ns.patch_archive:
+        raise CliError("--patch-base needs --patch-archive: it names the reference archive's own reference")
     if ns.patch_archive and not ns.patch_apply:
         raise CliError("--patch-archive needs --patch-apply: it says that the reference file is a seekable archive")
-    reference = _load_reference(zk, ns.patch_apply) if ns.patch_archive else None
+    reference = _load_reference(zk, ns.patch_apply, ns.patch_base) if ns.patch_archive else None
     prefix_len = os.path.getsize(ns.patch_apply) if ns.patch_apply and os.path.exists(ns.patch_apply) else None
     if reference is not None:
         prefix_len = reference.old_len

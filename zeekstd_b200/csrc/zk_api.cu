@@ -130,6 +130,7 @@ extern "C" void zk_ctx_destroy(zk_ctx* c) {
     if (c->up) cudaStreamDestroy(c->up);
     if (c->down) cudaStreamDestroy(c->down);
     if (c->d_prefix) cudaFree(c->d_prefix);
+    for (unsigned i = 0; i < ZK_CHAIN_MAX_DEPTH - 1; i++) if (c->d_level[i]) cudaFree(c->d_level[i]);
     for (int i = 0; i < 4; i++) if (c->d_reuse[i]) cudaFree(c->d_reuse[i]);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
@@ -1330,97 +1331,183 @@ extern "C" int32_t zk_patch_slices_read(const uint8_t* src, size_t len, uint32_t
 }
 
 // ---------------------------------------------------------------------------------------------
-// Seekable patches against a seekable archive (DESIGN §3.4.2): OLD is the decoded content of a reference archive R, and the calls above
-// run on it without OLD ever being on the host.  For each group of entries (zk_hull_group), the entries of R whose output overlaps the
-// group's hull are decoded on slot 0 straight into the prefix arena (c->d_prefix), the last one only as far as the hull's end, and the
-// prefix machinery reads the hull from there (zk_device_prefix).  The anchor pass decodes R in runs of whole entries instead.
+// Seekable patches against a seekable archive or a chain of them (DESIGN §3.4.2, §3.4.3): OLD is the decoded content of the head of a
+// reference chain R_0 <- R_1 <- ... <- R_{d-1} (R_0 a plain archive, every other level a seekable patch of the level below), and the calls
+// above run on it without any level's content ever being on the host.  For each group of entries (zk_hull_group), the entries of the head
+// whose output overlaps the group's hull are decoded on slot 0 straight into the prefix arena (c->d_prefix), the last one only as far as
+// the hull's end, and the prefix machinery reads the hull from there (zk_device_prefix).  A patch level first has the level below it decode
+// the hulls of its entries' slices into that level's own arena (c->d_level), recursively.  The anchor pass decodes the head in runs of
+// whole entries instead.  The _archive calls are the chain of one level.
 // ---------------------------------------------------------------------------------------------
-struct ZkRefArchive { const uint8_t* comp; size_t len; const uint64_t* c_off; const uint64_t* d_off; uint32_t n; };
 
-// decoded OLD starts this far into the prefix arena: the anchor pass puts the 63 bytes before a run in front of it
+// decoded content starts this far into a level's arena: the anchor pass puts the 63 bytes before a run in front of it
 #define ZK_REF_HEAD 64u
 
-// R's arguments: offsets that never decrease, OLD starting at 0, entries within R's bytes, and not a seekable patch itself (chains are
-// not resolved) -> 0 or ZK_ERR_INVALID_ARG.  *old_len: OLD's length
-static int32_t zk_ref_check(const ZkRefArchive& r, uint64_t* old_len) {
+// one level of a chain, and what the latest zk_ref_decode of it left in its arena
+struct ZkRefLevel {
+    zk_reference_archive r = {};
+    std::vector<uint64_t> slices;                           // a patch level: entry g reads [slices[2g], slices[2g + 1]) of the level below
+    void** arena = nullptr; size_t* cap = nullptr;          // the level's device arena
+    std::vector<uint32_t> list;                             // the entries decoded last, in order,
+    std::vector<int32_t> status;                            // their statuses (a failure below them included),
+    uint64_t base = 0;                                      // and the content offset of arena byte ZK_REF_HEAD
+};
+typedef std::vector<ZkRefLevel> ZkChain;
+
+// R's offsets: never decreasing, content starting at 0, entries within R's bytes -> 0 or ZK_ERR_INVALID_ARG.  *len: the decoded length
+static int32_t zk_ref_check(const zk_reference_archive& r, uint64_t* len) {
     if (!r.c_off || !r.d_off || (r.n && !r.comp) || r.d_off[0] != 0) return ZK_ERR_INVALID_ARG;
     for (uint32_t g = 0; g < r.n; g++)
         if (r.c_off[g + 1] < r.c_off[g] || r.d_off[g + 1] < r.d_off[g]) return ZK_ERR_INVALID_ARG;
     if (r.c_off[r.n] > r.len) return ZK_ERR_INVALID_ARG;
-    if (r.c_off[r.n] - r.c_off[0] >= 4 && zk_le32(r.comp + r.c_off[0]) == ZK_PATCH_SLICES_MAGIC) return ZK_ERR_INVALID_ARG;
-    *old_len = r.d_off[r.n];
+    *len = r.d_off[r.n];
     return 0;
 }
 
-// OLD [lo, hi) (lo < hi) made resident: the non-empty entries of R whose output overlaps it, list[0, m), uploaded back to back through
-// slot 0 and decoded into the prefix arena from ZK_REF_HEAD on, the last one only as far as hi (need: no checksum on it).  *base: the
-// OLD offset of arena byte ZK_REF_HEAD; (*status)[k]: entry list[k]'s status.  Returns 0 or a failure of the call itself.  Device memory:
-// the decoded bytes from the first entry's start to hi, plus the rest of the block that holds hi (the decoder stops at a block's end)
-static int32_t zk_ref_decode(zk_ctx* c, const ZkRefArchive& r, uint64_t lo, uint64_t hi, int verify, uint64_t* base,
-                             std::vector<uint32_t>* list, std::vector<int32_t>* status) {
-    list->clear();
-    uint32_t g = (uint32_t)(std::upper_bound(r.d_off, r.d_off + r.n + 1, lo) - r.d_off) - 1;    // the entry that holds lo
-    for (; g < r.n && r.d_off[g] < hi; g++)
-        if (r.d_off[g + 1] > r.d_off[g]) list->push_back(g);
-    const uint32_t m = (uint32_t)list->size();
-    std::vector<uint64_t> c_rel(m + 1, 0), d_rel(m + 1, 0);
-    for (uint32_t k = 0; k < m; k++) {
-        c_rel[k + 1] = c_rel[k] + (r.c_off[(*list)[k] + 1] - r.c_off[(*list)[k]]);
-        d_rel[k + 1] = d_rel[k] + (r.d_off[(*list)[k] + 1] - r.d_off[(*list)[k]]);
+// R starts with a slice frame: a seekable patch
+static bool zk_ref_is_patch(const zk_reference_archive& r) {
+    return r.c_off[r.n] - r.c_off[0] >= 4 && zk_le32(r.comp + r.c_off[0]) == ZK_PATCH_SLICES_MAGIC;
+}
+
+// chain[0, depth) checked and read (the slice frame of every patch level) -> *ch; *old_len: the head's decoded length.  ZK_ERR_INVALID_ARG:
+// a depth of 0 or above ZK_CHAIN_MAX_DEPTH, a level with bad offsets, a root that is a patch, a patch level without a valid slice frame of
+// its entry count or whose old_len is not the decoded length of the level below
+static int32_t zk_chain_open(zk_ctx* c, const zk_reference_archive* chain, uint32_t depth, ZkChain* ch, uint64_t* old_len) {
+    if (!chain || depth == 0 || depth > ZK_CHAIN_MAX_DEPTH) return ZK_ERR_INVALID_ARG;
+    ch->assign(depth, ZkRefLevel());
+    uint64_t below = 0;
+    for (uint32_t i = 0; i < depth; i++) {
+        ZkRefLevel& l = (*ch)[i];
+        l.r = chain[i];
+        uint64_t len = 0, ol = 0;
+        int32_t rc = zk_ref_check(l.r, &len);
+        if (rc) return rc;
+        if (i == 0 ? zk_ref_is_patch(l.r) : !zk_ref_is_patch(l.r)) return ZK_ERR_INVALID_ARG;
+        if (i > 0) {
+            l.slices.assign(2 * (size_t)l.r.n, 0);
+            rc = zk_patch_slices_read(l.r.comp + l.r.c_off[0], (size_t)(l.r.c_off[l.r.n] - l.r.c_off[0]), l.r.n, &ol, l.slices.data(), nullptr);
+            if (rc || ol != below) return ZK_ERR_INVALID_ARG;
+        }
+        l.arena = i + 1 == depth ? &c->d_prefix : &c->d_level[i];
+        l.cap = i + 1 == depth ? &c->cap_prefix : &c->cap_level[i];
+        below = len;
     }
-    *base = r.d_off[(*list)[0]];
-    const uint32_t last = (*list)[m - 1];
-    std::vector<uint32_t> need;
-    if (r.d_off[last + 1] > hi) { need.assign(m, 0xFFFFFFFFu); need[m - 1] = (uint32_t)(hi - r.d_off[last]); }
-    const uint64_t block = 128u << 10, end = r.d_off[last + 1] - hi > block ? hi + block : r.d_off[last + 1];
+    *old_len = below;
+    return 0;
+}
+
+// the first entry of l.list (decoded by zk_ref_decode) with a non-zero status whose output overlaps [lo, hi) -> that status, else 0
+static int32_t zk_ref_failure(const ZkRefLevel& l, uint64_t lo, uint64_t hi) {
+    for (size_t k = 0; k < l.list.size(); k++)
+        if (l.status[k] && l.r.d_off[l.list[k] + 1] > lo && l.r.d_off[l.list[k]] < hi) return l.status[k];
+    return 0;
+}
+
+// entries l.list[a, b) uploaded back to back through slot 0 (runs of consecutive entries in one copy) and decoded into the level's arena,
+// entry list[k] at d_rel[k], against p's prefix; need: one per entry of the list (empty: every entry whole) -> l.status[a, b).  Returns 0
+// or a failure of the call itself (an entry that fails to decode: its status)
+static int32_t zk_ref_run(zk_ctx* c, ZkRefLevel& l, uint32_t a, uint32_t b, const std::vector<uint64_t>& d_rel, int verify,
+                          const std::vector<uint32_t>& need, ZkDecodeParams p) {
+    const zk_reference_archive& r = l.r;
+    const uint32_t m = b - a;
+    std::vector<uint64_t> c_rel(m + 1, 0);
+    for (uint32_t k = 0; k < m; k++) c_rel[k + 1] = c_rel[k] + (r.c_off[l.list[a + k] + 1] - r.c_off[l.list[a + k]]);
     ZkSlot& s = c->slot[0];
     int32_t rc = zk_slot_ensure(&s, (size_t)c_rel[m] + 32, 0);
     if (rc) return rc;
-    for (int i = 0; i < ZK_SLOTS; i++) if (c->slot[i].stream) cudaStreamSynchronize(c->slot[i].stream);    // nobody reads the arena any more
-    if ((rc = zk_grow(&c->d_prefix, &c->cap_prefix, ZK_REF_HEAD + (size_t)(end - *base) + 64, 1))) return rc;
-    for (uint32_t k0 = 0; k0 < m;) {                        // runs of consecutive entries in one copy
+    for (uint32_t k0 = 0; k0 < m;) {
         uint32_t k1 = k0 + 1;
-        while (k1 < m && (*list)[k1] == (*list)[k1 - 1] + 1) k1++;
+        while (k1 < m && l.list[a + k1] == l.list[a + k1 - 1] + 1) k1++;
         const size_t bytes = (size_t)(c_rel[k1] - c_rel[k0]);
-        if (bytes) ZK_CUDA_OK(cudaMemcpyAsync(s.d_in + c_rel[k0], r.comp + r.c_off[(*list)[k0]], bytes, cudaMemcpyHostToDevice, s.stream));
+        if (bytes) ZK_CUDA_OK(cudaMemcpyAsync(s.d_in + c_rel[k0], r.comp + r.c_off[l.list[a + k0]], bytes, cudaMemcpyHostToDevice, s.stream));
         k0 = k1;
     }
-    ZkDecodeParams p;
-    if (!need.empty()) p.need = need.data();
-    status->assign(m, 0);
-    rc = zk_decode_batch(&s.dws, s.stream, s.d_in, c_rel.data(), d_rel.data(), m, (uint8_t*)c->d_prefix + ZK_REF_HEAD, verify, p, status->data());
+    if (!need.empty()) p.need = need.data() + a;
+    rc = zk_decode_batch(&s.dws, s.stream, s.d_in, c_rel.data(), d_rel.data() + a, m, (uint8_t*)*l.arena + ZK_REF_HEAD, verify, p,
+                         l.status.data() + a);
     c->ref_decoded += m;
     if (rc == ZK_INT_CUDA || rc == -(int)ZKZ_MEMORY_ALLOCATION) return rc;
-    return 0;                                               // an entry that fails to decode: its status
+    return 0;
 }
 
-// the first entry of *list (decoded by zk_ref_decode) with a non-zero status whose output overlaps [lo, hi) -> that status, else 0
-static int32_t zk_ref_failure(const ZkRefArchive& r, const std::vector<uint32_t>& list, const std::vector<int32_t>& status, uint64_t lo,
-                              uint64_t hi) {
-    for (size_t k = 0; k < list.size(); k++)
-        if (status[k] && r.d_off[list[k]] < hi && r.d_off[list[k] + 1] > lo) return status[k];
+// Need(i, [lo, hi)), lo < hi: level i's content [lo, hi) made resident.  The non-empty entries of R_i whose output overlaps it, l.list, are
+// decoded into the level's arena from ZK_REF_HEAD on (l.base: the content offset there), the last one only as far as hi (need: no checksum
+// on it).  A patch level groups its entries' slices (zk_hull_group, empty slices skipped); per group with a non-empty hull, Need(i - 1,
+// hull) runs first and the group's entries are then decoded against it, rebased.  An entry whose slice overlaps an entry below that failed
+// takes that status and is not decoded.  Returns 0 or a failure of the call itself.  Device memory, per level: the decoded bytes from the
+// first entry's start to hi, plus the rest of the block that holds hi (the decoder stops at a block's end)
+static int32_t zk_ref_decode(zk_ctx* c, ZkChain& ch, uint32_t i, uint64_t lo, uint64_t hi, int verify) {
+    ZkRefLevel& l = ch[i];
+    const zk_reference_archive& r = l.r;
+    l.list.clear();
+    uint32_t g = (uint32_t)(std::upper_bound(r.d_off, r.d_off + r.n + 1, lo) - r.d_off) - 1;    // the entry that holds lo
+    for (; g < r.n && r.d_off[g] < hi; g++)
+        if (r.d_off[g + 1] > r.d_off[g]) l.list.push_back(g);
+    const uint32_t m = (uint32_t)l.list.size();
+    const uint32_t last = l.list[m - 1];
+    l.base = r.d_off[l.list[0]];
+    std::vector<uint64_t> d_rel(m + 1);
+    for (uint32_t k = 0; k < m; k++) d_rel[k] = r.d_off[l.list[k]] - l.base;
+    d_rel[m] = r.d_off[last + 1] - l.base;
+    std::vector<uint32_t> need;
+    if (r.d_off[last + 1] > hi) { need.assign(m, 0xFFFFFFFFu); need[m - 1] = (uint32_t)(hi - r.d_off[last]); }
+    const uint64_t block = 128u << 10, end = r.d_off[last + 1] - hi > block ? hi + block : r.d_off[last + 1];
+    for (int k = 0; k < ZK_SLOTS; k++) if (c->slot[k].stream) cudaStreamSynchronize(c->slot[k].stream);    // nobody reads the arena any more
+    int32_t rc = zk_grow(l.arena, l.cap, ZK_REF_HEAD + (size_t)(end - l.base) + 64, 1);
+    if (rc) return rc;
+    l.status.assign(m, 0);
+    if (i == 0) return zk_ref_run(c, l, 0, m, d_rel, verify, need, ZkDecodeParams());
+    std::vector<uint64_t> sl(2 * (size_t)m), rb;
+    for (uint32_t k = 0; k < m; k++) { sl[2 * (size_t)k] = l.slices[2 * (size_t)l.list[k]]; sl[2 * (size_t)k + 1] = l.slices[2 * (size_t)l.list[k] + 1]; }
+    const ZkRefLevel& below = ch[i - 1];
+    const uint64_t group = zk_patch_group_bytes();
+    std::vector<int32_t> fail;
+    std::vector<uint32_t> rw;
+    for (uint32_t k0 = 0; k0 < m;) {
+        uint64_t hlo, hhi;
+        const uint32_t k1 = zk_hull_group(sl.data(), k0, m, group, &hlo, &hhi);
+        zk_rebase_ranges(sl.data(), k0, k1, hlo, &rb);
+        ZkDecodeParams p;
+        fail.assign(k1 - k0, 0);
+        if (hhi > hlo) {
+            if ((rc = zk_ref_decode(c, ch, i - 1, hlo, hhi, verify))) return rc;
+            if ((rc = zk_device_prefix((const uint8_t*)*below.arena + ZK_REF_HEAD + (hlo - below.base), (size_t)(hhi - hlo), &p.prefix,
+                                       &p.prefix_len))) return rc;
+            for (uint32_t k = k0; k < k1; k++)
+                if (sl[2 * (size_t)k] < sl[2 * (size_t)k + 1]) fail[k - k0] = zk_ref_failure(below, sl[2 * (size_t)k], sl[2 * (size_t)k + 1]);
+        }
+        for (uint32_t a = k0; a < k1;) {                    // runs of entries whose slices decoded
+            if (fail[a - k0]) { l.status[a] = fail[a - k0]; a++; continue; }
+            uint32_t b = a + 1;
+            while (b < k1 && !fail[b - k0]) b++;
+            if (p.prefix) {
+                if ((rc = zk_prefix_ranges(rb.data() + 2 * (size_t)(a - k0), b - a, (size_t)(hhi - hlo), &rw))) return rc;
+                p.ranges = rw.data();
+            }
+            if ((rc = zk_ref_run(c, l, a, b, d_rel, verify, need, p))) return rc;
+            a = b;
+        }
+        k0 = k1;
+    }
     return 0;
 }
 
 // OLD [lo, hi) as a device prefix, for the calls that cannot use a partly decoded OLD: the first failing entry's status is the call's
-static int32_t zk_ref_prefix(zk_ctx* c, const ZkRefArchive& r, uint64_t lo, uint64_t hi, const uint8_t** prefix) {
-    std::vector<uint32_t> list;
-    std::vector<int32_t> status;
-    uint64_t base = 0;
-    int32_t rc = zk_ref_decode(c, r, lo, hi, 1, &base, &list, &status);
-    if (!rc) rc = zk_ref_failure(r, list, status, lo, hi);
-    *prefix = (const uint8_t*)c->d_prefix + ZK_REF_HEAD + (lo - base);
+static int32_t zk_ref_prefix(zk_ctx* c, ZkChain& ch, uint64_t lo, uint64_t hi, const uint8_t** prefix) {
+    const ZkRefLevel& h = ch.back();
+    int32_t rc = zk_ref_decode(c, ch, (uint32_t)ch.size() - 1, lo, hi, 1);
+    if (!rc) rc = zk_ref_failure(h, lo, hi);
+    *prefix = (const uint8_t*)c->d_prefix + ZK_REF_HEAD + (lo - h.base);
     return rc;
 }
 
-extern "C" int32_t zk_decompress_frames_prefixes_archive(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n,
-                                                         uint8_t* dst, const uint32_t* d_need, int32_t verify, int32_t* status,
-                                                         const uint8_t* ref_comp, size_t ref_len, const uint64_t* ref_c_off,
-                                                         const uint64_t* ref_d_off, uint32_t ref_n, const uint64_t* ranges) {
+extern "C" int32_t zk_decompress_frames_prefixes_chain(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n,
+                                                       uint8_t* dst, const uint32_t* d_need, int32_t verify, int32_t* status,
+                                                       const zk_reference_archive* chain, uint32_t depth, const uint64_t* ranges) {
     if (!c) return ZK_ERR_INVALID_ARG;
-    const ZkRefArchive r = {ref_comp, ref_len, ref_c_off, ref_d_off, ref_n};
+    ZkChain ch;
     uint64_t old_len = 0;
-    int32_t rc = zk_ref_check(r, &old_len);
+    int32_t rc = zk_chain_open(c, chain, depth, &ch, &old_len);
     if (rc) return rc;
     std::vector<uint64_t> whole;                            // no ranges: every entry against all of OLD
     if (!ranges) {
@@ -1434,21 +1521,20 @@ extern "C" int32_t zk_decompress_frames_prefixes_archive(zk_ctx* c, const uint8_
     if (n == 0) return 0;
     ZK_CUDA_OK(cudaSetDevice(c->device));
     const uint64_t group = zk_patch_group_bytes();
+    const ZkRefLevel& h = ch.back();
     std::vector<uint64_t> rb;
-    std::vector<uint32_t> list;
-    std::vector<int32_t> rst, st(n, 0), fail;
+    std::vector<int32_t> st(n, 0), fail;
     for (uint32_t f0 = 0; f0 < n;) {
-        uint64_t hlo, hhi, base = 0;
+        uint64_t hlo, hhi;
         const uint32_t end = zk_hull_group(ranges, f0, n, group, &hlo, &hhi);
         zk_rebase_ranges(ranges, f0, end, hlo, &rb);
-        list.clear();
-        if (hhi > hlo && (rc = zk_ref_decode(c, r, hlo, hhi, verify, &base, &list, &rst))) return rc;
-        const uint8_t* prefix = hhi > hlo ? (const uint8_t*)c->d_prefix + ZK_REF_HEAD + (hlo - base) : nullptr;
+        ch.back().list.clear();
+        if (hhi > hlo && (rc = zk_ref_decode(c, ch, depth - 1, hlo, hhi, verify))) return rc;
+        const uint8_t* prefix = hhi > hlo ? (const uint8_t*)c->d_prefix + ZK_REF_HEAD + (hlo - h.base) : nullptr;
         // an entry whose range overlaps a reference entry that failed takes its status; the others run in runs of consecutive entries
         fail.assign(end - f0, 0);
         for (uint32_t f = f0; f < end; f++)
-            if (ranges[2 * (size_t)f] < ranges[2 * (size_t)f + 1])
-                fail[f - f0] = zk_ref_failure(r, list, rst, ranges[2 * (size_t)f], ranges[2 * (size_t)f + 1]);
+            if (ranges[2 * (size_t)f] < ranges[2 * (size_t)f + 1]) fail[f - f0] = zk_ref_failure(h, ranges[2 * (size_t)f], ranges[2 * (size_t)f + 1]);
         for (uint32_t a = f0; a < end;) {
             if (fail[a - f0]) { st[a] = fail[a - f0]; a++; continue; }
             uint32_t b = a + 1;
@@ -1465,15 +1551,22 @@ extern "C" int32_t zk_decompress_frames_prefixes_archive(zk_ctx* c, const uint8_
     return 0;
 }
 
-// frames of NEW against their ranges of OLD: zk_compress_frames_patch's groups, each hull decoded from R into the prefix arena
-extern "C" int32_t zk_compress_frames_patch_archive(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
-                                                    int32_t checksum, const uint8_t* ref_comp, size_t ref_len, const uint64_t* ref_c_off,
-                                                    const uint64_t* ref_d_off, uint32_t ref_n, const uint64_t* ranges, uint8_t* dst,
-                                                    size_t dst_cap, uint32_t* c_sizes, size_t* dst_len) {
+extern "C" int32_t zk_decompress_frames_prefixes_archive(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n,
+                                                         uint8_t* dst, const uint32_t* d_need, int32_t verify, int32_t* status,
+                                                         const uint8_t* ref_comp, size_t ref_len, const uint64_t* ref_c_off,
+                                                         const uint64_t* ref_d_off, uint32_t ref_n, const uint64_t* ranges) {
+    const zk_reference_archive r = {ref_comp, ref_len, ref_c_off, ref_d_off, ref_n};
+    return zk_decompress_frames_prefixes_chain(c, comp, c_off, d_off, n, dst, d_need, verify, status, &r, 1, ranges);
+}
+
+// frames of NEW against their ranges of OLD: zk_compress_frames_patch's groups, each hull decoded from the chain into the prefix arena
+extern "C" int32_t zk_compress_frames_patch_chain(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                                  int32_t checksum, const zk_reference_archive* chain, uint32_t depth, const uint64_t* ranges,
+                                                  uint8_t* dst, size_t dst_cap, uint32_t* c_sizes, size_t* dst_len) {
     if (!c || (n_frames && (!frame_sizes || !ranges || !dst))) return ZK_ERR_INVALID_ARG;
-    const ZkRefArchive r = {ref_comp, ref_len, ref_c_off, ref_d_off, ref_n};
+    ZkChain ch;
     uint64_t old_len = 0;
-    int32_t rc = zk_ref_check(r, &old_len);
+    int32_t rc = zk_chain_open(c, chain, depth, &ch, &old_len);
     if (rc) return rc;
     if (dst_len) *dst_len = 0;
     for (uint32_t f = 0; f < n_frames; f++)
@@ -1492,7 +1585,7 @@ extern "C" int32_t zk_compress_frames_patch_archive(zk_ctx* c, const uint8_t* sr
         if (hhi > hlo) {
             ZkCompressReq q;                                // zk_compress_frames_sized_prefixes(ldm = 1) on the decoded hull
             q.policy = ZK_FRAMES_SIZED; q.sizes = frame_sizes + f0; q.count = end - f0; q.src = src ? src + in : nullptr;
-            if ((rc = zk_ref_prefix(c, r, hlo, hhi, &q.prefix))) return rc;
+            if ((rc = zk_ref_prefix(c, ch, hlo, hhi, &q.prefix))) return rc;
             q.prefix_len = (size_t)(hhi - hlo); q.prefix_dev = true; q.ranges = rb.data();
             q.params.level = level; q.params.checksum = checksum; q.params.ldm = true;
             q.dst = dst + out; q.dst_cap = dst_cap - out; q.c_sizes = cs.data() + f0; q.dst_len = &len;
@@ -1509,10 +1602,20 @@ extern "C" int32_t zk_compress_frames_patch_archive(zk_ctx* c, const uint8_t* sr
     return 0;
 }
 
-// the anchors of OLD = R's decoded content: R in runs of whole entries of at most ZK_PATCH_PIECE_BYTES (a larger entry alone), each run
-// decoded into the prefix arena with the 63 bytes of OLD before it copied in front, so every anchor is found once, as the raw pass finds it
-static int32_t zk_patch_scan_archive(zk_ctx* c, const ZkRefArchive& r, std::vector<unsigned long long>* keys, std::vector<unsigned long long>* pos) {
+extern "C" int32_t zk_compress_frames_patch_archive(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                                    int32_t checksum, const uint8_t* ref_comp, size_t ref_len, const uint64_t* ref_c_off,
+                                                    const uint64_t* ref_d_off, uint32_t ref_n, const uint64_t* ranges, uint8_t* dst,
+                                                    size_t dst_cap, uint32_t* c_sizes, size_t* dst_len) {
+    const zk_reference_archive r = {ref_comp, ref_len, ref_c_off, ref_d_off, ref_n};
+    return zk_compress_frames_patch_chain(c, src, frame_sizes, n_frames, level, checksum, &r, 1, ranges, dst, dst_cap, c_sizes, dst_len);
+}
+
+// the anchors of OLD = the head's decoded content: the head in runs of whole entries of at most ZK_PATCH_PIECE_BYTES (a larger entry
+// alone), each run decoded into the prefix arena with the 63 bytes of OLD before it copied in front, so every anchor is found once, as
+// the raw pass finds it
+static int32_t zk_patch_scan_archive(zk_ctx* c, ZkChain& ch, std::vector<unsigned long long>* keys, std::vector<unsigned long long>* pos) {
     ZkSlot& s = c->slot[0];
+    const zk_reference_archive& r = ch.back().r;
     const size_t piece = zk_patch_piece_bytes();
     const size_t most = (size_t)1 << 30;                    // zk_patch_anchors' largest piece
     int32_t rc = zk_slot_ensure(&s, 0, ZK_REF_HEAD);        // d_out: the tail of the run before, kept while the arena is reused
@@ -1525,7 +1628,7 @@ static int32_t zk_patch_scan_archive(zk_ctx* c, const ZkRefArchive& r, std::vect
         g0 = g1;
         if (hi == lo) continue;
         const uint8_t* unused;
-        if ((rc = zk_ref_prefix(c, r, lo, hi, &unused))) return rc;
+        if ((rc = zk_ref_prefix(c, ch, lo, hi, &unused))) return rc;
         uint8_t* run = (uint8_t*)c->d_prefix + ZK_REF_HEAD;
         if (ov) ZK_CUDA_OK(cudaMemcpyAsync(run - ov, s.d_out, ov, cudaMemcpyDeviceToDevice, s.stream));
         const uint64_t n = ov + (hi - lo);
@@ -1542,13 +1645,12 @@ static int32_t zk_patch_scan_archive(zk_ctx* c, const ZkRefArchive& r, std::vect
     return zk_sync_check(s.stream);
 }
 
-extern "C" int32_t zk_patch_ranges_archive(zk_ctx* c, const uint8_t* new_src, const uint32_t* frame_sizes, uint32_t n_frames,
-                                           const uint8_t* ref_comp, size_t ref_len, const uint64_t* ref_c_off, const uint64_t* ref_d_off,
-                                           uint32_t ref_n, uint64_t margin, uint64_t* ranges) {
+extern "C" int32_t zk_patch_ranges_chain(zk_ctx* c, const uint8_t* new_src, const uint32_t* frame_sizes, uint32_t n_frames,
+                                         const zk_reference_archive* chain, uint32_t depth, uint64_t margin, uint64_t* ranges) {
     if (!c || (n_frames && (!frame_sizes || !ranges))) return ZK_ERR_INVALID_ARG;
-    const ZkRefArchive r = {ref_comp, ref_len, ref_c_off, ref_d_off, ref_n};
+    ZkChain ch;
     uint64_t old_len = 0;
-    int32_t rc = zk_ref_check(r, &old_len);
+    int32_t rc = zk_chain_open(c, chain, depth, &ch, &old_len);
     if (rc) return rc;
     if (old_len >= (1ull << 62) || margin >= (1ull << 62)) return ZK_ERR_INVALID_ARG;
     ZkPatchTables t;
@@ -1558,7 +1660,7 @@ extern "C" int32_t zk_patch_ranges_archive(zk_ctx* c, const uint8_t* new_src, co
     if (n && !new_src) return ZK_ERR_INVALID_ARG;
     if (n_frames == 0) return 0;
     ZK_CUDA_OK(cudaSetDevice(c->device));
-    rc = zk_patch_scan_archive(c, r, &t.okeys, &t.opos);
+    rc = zk_patch_scan_archive(c, ch, &t.okeys, &t.opos);
     if (!rc) rc = zk_patch_scan(c, new_src, n, &t.nkeys, &t.npos);
     if (rc) return rc;
     if (t.okeys.size() > 0xFFFFFFF0ull || t.nkeys.size() > 0xFFFFFFF0ull) return ZK_ERR_INVALID_ARG;
@@ -1568,4 +1670,11 @@ extern "C" int32_t zk_patch_ranges_archive(zk_ctx* c, const uint8_t* new_src, co
         t.fanc[f] = f == n_frames ? (uint32_t)t.npos.size() : i;
     }
     return zk_patch_join(&c->slot[0].ews, c->slot[0].stream, t, n_frames, old_len, margin, (unsigned long long*)ranges);
+}
+
+extern "C" int32_t zk_patch_ranges_archive(zk_ctx* c, const uint8_t* new_src, const uint32_t* frame_sizes, uint32_t n_frames,
+                                           const uint8_t* ref_comp, size_t ref_len, const uint64_t* ref_c_off, const uint64_t* ref_d_off,
+                                           uint32_t ref_n, uint64_t margin, uint64_t* ranges) {
+    const zk_reference_archive r = {ref_comp, ref_len, ref_c_off, ref_d_off, ref_n};
+    return zk_patch_ranges_chain(c, new_src, frame_sizes, n_frames, &r, 1, margin, ranges);
 }

@@ -3,6 +3,7 @@
 #pragma once
 #include "zk_decode.h"
 #include "zk_encode.h"
+#include "../../include/zeekstd_b200.h"
 
 #define ZK_SLOTS 8                        // pipeline depth of the host<->device paths (H2D | kernels | D2H overlap)
 
@@ -27,6 +28,8 @@ struct zk_ctx {
     void* d_prefix = nullptr; size_t cap_prefix = 0;      // device copy of the raw-content prefix of the calls that take one
     unsigned long long prefix_uploaded = 0;               // prefix bytes copied to the device so far (zk_ctx_prefix_bytes_uploaded)
     unsigned long long ref_decoded = 0;                   // reference-archive entries decoded so far (zk_ctx_reference_entries_decoded)
+    void* d_level[ZK_CHAIN_MAX_DEPTH - 1] = {};           // a reference chain's arenas below its head (level i's decoded content; the
+    size_t cap_level[ZK_CHAIN_MAX_DEPTH - 1] = {};        // head's is d_prefix)
     void* d_reuse[4] = {}; size_t cap_reuse[4] = {};      // zk_compress_frames_sized_reuse: old entries, their decoded bytes, the changed
                                                           // frames, the assembled output
     unsigned long long launches() const {

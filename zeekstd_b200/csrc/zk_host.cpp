@@ -555,8 +555,8 @@ struct zk_decoder {                        // decode.rs:121-466
     size_t max_window_bytes = (size_t)256 << 20;
     const uint8_t* prefix = nullptr; size_t prefix_len = 0;   // the prefix the window was decoded with (decompress_with_prefix)
     const uint64_t* ranges = nullptr;                          // and every entry's range of it (nullptr: the whole prefix)
-    bool archive = false;                                      // the prefix is the decoded content of this reference archive instead
-    const uint64_t* ref_c_off = nullptr; const uint64_t* ref_d_off = nullptr; uint32_t ref_n = 0;
+    bool archive = false;                                      // the prefix is OLD of this reference chain instead (a copy of its
+    std::vector<zk_reference_archive> chain;                   // descriptors, root first)
 
     void reset_dctx() { read_compressed = 0; win_lo = win_hi = 0; win_valid_end = 0; window.clear(); }                           // :352-357
     int32_t check_offset(uint64_t off) const { return off > seek_table.d.back() ? ZK_ERR_OFFSET_OUT_OF_RANGE : 0; }   // :439-445
@@ -587,8 +587,8 @@ struct zk_decoder {                        // decode.rs:121-466
         } else need_end = d1;
         const uint32_t* np = need.empty() ? nullptr : need.data();
         const uint64_t* rg = ranges ? ranges + 2 * (size_t)f0 : nullptr;
-        rc = archive ? zk_decompress_frames_prefixes_archive(ctx, comp.data(), co.data(), dof.data(), n, window.data(), np, 1, nullptr, prefix,
-                                                             prefix_len, ref_c_off, ref_d_off, ref_n, rg)
+        rc = archive ? zk_decompress_frames_prefixes_chain(ctx, comp.data(), co.data(), dof.data(), n, window.data(), np, 1, nullptr, chain.data(),
+                                                           (uint32_t)chain.size(), rg)
                      : zk_decompress_frames_prefixes(ctx, comp.data(), co.data(), dof.data(), n, window.data(), np, 1, nullptr, prefix, prefix_len, rg);
         if (rc) { win_lo = win_hi = 0; win_valid_end = 0; return rc; }
         win_lo = f0; win_hi = f1; win_valid_end = need_end;
@@ -645,15 +645,26 @@ extern "C" int32_t zk_decoder_decompress_with_prefix_ranges(zk_decoder* d, uint8
     return zk_decoder_run(d, buf, len, produced);
 }
 
-// the reference archive's bytes and length stand in prefix / prefix_len
 extern "C" int32_t zk_decoder_decompress_with_reference_archive(zk_decoder* d, uint8_t* buf, size_t len, const uint8_t* ref_comp, size_t ref_len,
                                                                 const uint64_t* ref_c_off, const uint64_t* ref_d_off, uint32_t ref_n,
                                                                 const uint64_t* ranges, size_t* produced) {
-    if (!d->archive || ref_comp != d->prefix || ref_len != d->prefix_len || ranges != d->ranges || ref_c_off != d->ref_c_off ||
-        ref_d_off != d->ref_d_off || ref_n != d->ref_n) {
+    const zk_reference_archive r = {ref_comp, ref_len, ref_c_off, ref_d_off, ref_n};
+    return zk_decoder_decompress_with_reference_chain(d, buf, len, &r, 1, ranges, produced);
+}
+
+// the window stays valid while the ranges and every level's descriptor are the ones it was decoded with
+extern "C" int32_t zk_decoder_decompress_with_reference_chain(zk_decoder* d, uint8_t* buf, size_t len, const zk_reference_archive* chain, uint32_t depth,
+                                                              const uint64_t* ranges, size_t* produced) {
+    if (!chain || depth == 0 || depth > ZK_CHAIN_MAX_DEPTH) return ZK_ERR_INVALID_ARG;
+    bool same = d->archive && ranges == d->ranges && depth == d->chain.size();
+    for (uint32_t i = 0; same && i < depth; i++) {
+        const zk_reference_archive &a = chain[i], &b = d->chain[i];
+        same = a.comp == b.comp && a.len == b.len && a.c_off == b.c_off && a.d_off == b.d_off && a.n == b.n;
+    }
+    if (!same) {
         d->win_lo = d->win_hi = 0; d->win_valid_end = 0;
-        d->prefix = ref_comp; d->prefix_len = ref_len; d->ranges = ranges; d->archive = true;
-        d->ref_c_off = ref_c_off; d->ref_d_off = ref_d_off; d->ref_n = ref_n;
+        d->prefix = nullptr; d->prefix_len = 0; d->ranges = ranges; d->archive = true;
+        d->chain.assign(chain, chain + depth);
     }
     return zk_decoder_run(d, buf, len, produced);
 }
