@@ -103,6 +103,7 @@ extern "C" int32_t zk_ctx_create(int32_t device_ordinal, uint32_t flags, zk_ctx*
         c->slot[i].dws.exec_short = (uint32_t)zk_env_size("ZK_EXEC_SHORT", 128 << 10);
         c->slot[i].dws.seq2_ctas = (uint32_t)zk_env_size("ZK_SEQ2_CTAS", 0);
         c->slot[i].dws.huf_ctas = (uint32_t)zk_env_size("ZK_HUF_CTAS", 0);
+        c->slot[i].dws.order = zk_env_size("ZK_DEC_ORDER", 1) != 0 ? 1u : 0u;
         c->slot[i].ews.sm_count = c->sm_count;
     }
     cudaEventCreate(&c->ev0); cudaEventCreate(&c->ev1);

@@ -9,6 +9,7 @@
 //   K-D1s zk_seq2_kernel       one chain / block    : FSE sequence decode (4 chains per warp, TMA-staged bitstreams);
 //         zk_seq2_full_kernel                       the same for blocks whose tables need more cells than zk_seq2_kernel holds
 //   K-D1h zk_huf_kernel        one LANE  / stream   : Huffman literal decode (4 lanes per 4-stream block, two-level table)
+//   K-D0o / K-D1o zk_order_kernel  one CTA / list   : the work lists of K-D1s / K-D1h (after K-D0) and of K-D2 (after K-D1p), heaviest first
 //   K-D1p zk_plan_kernel       one warp / entry     : output positions, the serial walk's checks, execution segments
 //   K-D2w zk_exec_warp_kernel  one warp / segment   : short segments, strictly in order through a per-warp window
 //   K-D2 zk_exec_kernel[_w5]   one CTA  / segment   : long segments, sequence execution through a shared-memory ring
@@ -891,6 +892,89 @@ __global__ void __launch_bounds__(32) zk_huf_kernel(ZkDecodeArgs a) {
 }
 
 // =============================================================================================
+// K-D0o / K-D1o: work order -- heaviest item first.
+//
+// Every persistent decode stage pulls its items from a work counter, so it lasts about as long as its heaviest item plus
+// however late that item was pulled.  Handing out the items by cost, heaviest first (LPT), bounds a stage near the larger
+// of its longest item and the mean load per worker, and gives the 4 chains of a K-D1s warp and the 8 blocks of a K-D1h
+// warp similar costs.  The key is bucketed into quarter octaves of log2(1 + cost) and the list counting-sorted, one CTA
+// per list; the order inside a bucket is whatever the shared-memory atomics give, which no output depends on.
+//   K-D0o (after the scan):  seq_list by nseq, huf_list by lit_size
+//   K-D1o (after the plan):  both halves of seg_list by seg_key
+// The ordered lists keep the layout of the ones they are made from and are what the consumers receive as their lists.
+// =============================================================================================
+#define ZK_ORD_ALPHA 16u            // segment cost: ZK_ORD_ALPHA x sequences + output bytes
+#define ZK_ORD_BUCKETS 128u         // 4 per octave of a 32-bit key
+#define ZK_ORD_THREADS 1024u
+#define ZK_ORD_UNROLL 4u
+
+__device__ __forceinline__ uint32_t zk_ord_bucket(uint32_t cost) {
+    const unsigned long long v = (unsigned long long)cost + 1u;
+    const uint32_t hb = 63u - (uint32_t)__clzll((long long)v);
+    const uint32_t frac = hb >= 2 ? (uint32_t)(v >> (hb - 2)) & 3u : (uint32_t)(v << (2 - hb)) & 3u;
+    const uint32_t b = 4u * hb + frac;
+    return b < ZK_ORD_BUCKETS ? b : ZK_ORD_BUCKETS - 1u;
+}
+
+// src / dst: the list, item i at base + dir * i; key of item i: keys ? keys[base + dir * i] : the field of blocks[src item]
+template <int FIELD>
+__device__ void zk_order_list(const ZkDecodeArgs& a, const uint32_t* src, uint32_t* dst, const uint32_t* keys, uint32_t n,
+                              uint64_t base, int dir) {
+    __shared__ uint32_t hist[ZK_ORD_BUCKETS];
+    for (uint32_t b = threadIdx.x; b < ZK_ORD_BUCKETS; b += blockDim.x) hist[b] = 0;
+    __syncthreads();
+    auto bucket = [&](uint32_t i) -> uint32_t {
+        const uint64_t at = base + (int64_t)dir * i;
+        if (keys) return zk_ord_bucket(keys[at]);
+        const uint32_t bidx = src[at];
+        if (bidx >= a.cap_blocks) return 0;            // (every reserved slot is written by the scan kernel)
+        return zk_ord_bucket(FIELD == 0 ? a.blocks[bidx].nseq : a.blocks[bidx].lit_size);
+    };
+    for (uint32_t i0 = threadIdx.x; i0 < n; i0 += ZK_ORD_UNROLL * blockDim.x) {
+        uint32_t bk[ZK_ORD_UNROLL];
+#pragma unroll
+        for (uint32_t u = 0; u < ZK_ORD_UNROLL; u++) { const uint32_t i = i0 + u * blockDim.x; bk[u] = i < n ? bucket(i) : 0u; }
+#pragma unroll
+        for (uint32_t u = 0; u < ZK_ORD_UNROLL; u++) if (i0 + u * blockDim.x < n) atomicAdd(&hist[bk[u]], 1u);
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {                            // exclusive scan from the heaviest bucket down: where each bucket starts
+        const uint32_t lane = threadIdx.x, per = ZK_ORD_BUCKETS / 32u;
+        uint32_t h[ZK_ORD_BUCKETS / 32u], sum = 0;
+        for (uint32_t k = 0; k < per; k++) { h[k] = hist[ZK_ORD_BUCKETS - 1u - (lane * per + k)]; sum += h[k]; }
+        uint32_t incl = sum;
+        for (int d = 1; d < 32; d <<= 1) { const uint32_t x = __shfl_up_sync(0xFFFFFFFFu, incl, d); if ((int)lane >= d) incl += x; }
+        uint32_t run = incl - sum;
+        for (uint32_t k = 0; k < per; k++) { hist[ZK_ORD_BUCKETS - 1u - (lane * per + k)] = run; run += h[k]; }
+    }
+    __syncthreads();
+    for (uint32_t i0 = threadIdx.x; i0 < n; i0 += ZK_ORD_UNROLL * blockDim.x) {
+        uint32_t bk[ZK_ORD_UNROLL];
+#pragma unroll
+        for (uint32_t u = 0; u < ZK_ORD_UNROLL; u++) { const uint32_t i = i0 + u * blockDim.x; bk[u] = i < n ? bucket(i) : 0u; }
+#pragma unroll
+        for (uint32_t u = 0; u < ZK_ORD_UNROLL; u++) {
+            const uint32_t i = i0 + u * blockDim.x;
+            if (i >= n) continue;
+            const uint32_t pos = atomicAdd(&hist[bk[u]], 1u);
+            dst[base + (int64_t)dir * pos] = src[base + (int64_t)dir * i];
+        }
+    }
+}
+
+// Two CTAs: the lists of one stage side by side.  o holds the ordered lists (ZkDecodeWs::ord_list).
+__global__ void __launch_bounds__(ZK_ORD_THREADS) zk_order_kernel(ZkDecodeArgs a, ZkDecodeArgs o, int segs) {
+    if (a.counters->overflow) return;
+    if (segs) {
+        if (blockIdx.x == 0) zk_order_list<2>(a, a.seg_list, o.seg_list, a.seg_key, a.counters->n_long, 0, 1);
+        else zk_order_list<2>(a, a.seg_list, o.seg_list, a.seg_key, a.counters->n_short, a.cap_blocks - 1, -1);
+    } else {
+        if (blockIdx.x == 0) zk_order_list<0>(a, a.seq_list, o.seq_list, nullptr, a.counters->n_seq_blocks, 0, 1);
+        else zk_order_list<1>(a, a.huf_list, o.huf_list, nullptr, a.counters->n_huf_blocks, 0, 1);
+    }
+}
+
+// =============================================================================================
 // K-D1p: execution plan -- one warp per entry.
 //
 // The serial walk over an entry's blocks is cut into SEGMENTS: runs of consecutive blocks that read nothing written
@@ -982,14 +1066,15 @@ __global__ void __launch_bounds__(128) zk_plan_kernel(ZkDecodeArgs a) {
     uint32_t nseg = 0;
     __syncwarp();
     uint32_t seg_end = run ? blocks[run - 1].out_pos + blocks[run - 1].regen : 0u;      // output end of the first segment after this tile
+    uint32_t seg_send = run ? blocks[run - 1].seq_base + blocks[run - 1].nseq : 0u;    // and its sequence end (seq_base runs on per entry)
     for (uint32_t t = run ? (run - 1) & ~31u : 0; run; t -= 32) {
         const uint32_t bi = t + (uint32_t)lane;
         const bool in = bi < run;
         long long lo = 0x7FFFFFFFFFFFFFFFll;
-        uint32_t flags = 0, op = 0; bool conc = false;
+        uint32_t flags = 0, op = 0, sb = 0; bool conc = false;
         if (in) {
             const ZkBlock& b = blocks[bi];
-            flags = b.flags; op = b.out_pos;
+            flags = b.flags; op = b.out_pos; sb = b.seq_base;
             lo = b.back == ZK_BACK_UNKNOWN ? -0x7FFFFFFFFFFFFFFFll : (long long)op - (long long)b.back;
             conc = !((b.rep_out[0] | b.rep_out[1] | b.rep_out[2]) & ZK_SYM);
         }
@@ -1006,7 +1091,10 @@ __global__ void __launch_bounds__(128) zk_plan_kernel(ZkDecodeArgs a) {
             // a segment ends where the next one starts (in this tile, else seg_end); short ones go to the single-warp list
             const uint32_t later = m & (0xFFFFFFFEu << lane);
             const uint32_t nxp = __shfl_sync(0xFFFFFFFFu, op, later ? __ffs((int)later) - 1 : 0);
-            const uint32_t end = later ? nxp : seg_end;
+            const uint32_t nxs = __shfl_sync(0xFFFFFFFFu, sb, later ? __ffs((int)later) - 1 : 0);
+            const uint32_t end = later ? nxp : seg_end, send = later ? nxs : seg_send;
+            const unsigned long long cost = (unsigned long long)ZK_ORD_ALPHA * (send - sb) + (end - op);
+            const uint32_t key = cost > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)cost;
             const uint32_t ms = __ballot_sync(0xFFFFFFFFu, start && a.exec_short && end - op <= a.exec_short), mlong = m & ~ms;
             uint32_t base_l = 0, base_s = 0;
             if (lane == 0) {
@@ -1015,10 +1103,13 @@ __global__ void __launch_bounds__(128) zk_plan_kernel(ZkDecodeArgs a) {
             }
             base_l = __shfl_sync(0xFFFFFFFFu, base_l, 0); base_s = __shfl_sync(0xFFFFFFFFu, base_s, 0);
             const uint32_t below = (1u << lane) - 1u;
-            if ((ms >> lane) & 1u) a.seg_list[a.cap_blocks - 1 - (base_s + __popc(ms & below))] = ent.first_block + bi;
-            else if (start) a.seg_list[base_l + __popc(mlong & below)] = ent.first_block + bi;
+            if (start) {
+                const uint64_t at = ((ms >> lane) & 1u) ? a.cap_blocks - 1 - (base_s + __popc(ms & below)) : base_l + __popc(mlong & below);
+                a.seg_list[at] = ent.first_block + bi; a.seg_key[at] = key;
+            }
             nseg += __popc(m);
             seg_end = __shfl_sync(0xFFFFFFFFu, op, __ffs((int)m) - 1);
+            seg_send = __shfl_sync(0xFFFFFFFFu, sb, __ffs((int)m) - 1);
         }
         low = __shfl_sync(0xFFFFFFFFu, lo, 0);
         if (t == 0) break;
@@ -1895,7 +1986,7 @@ __global__ void __launch_bounds__(128) zk_xxh64_kernel(ZkDecodeArgs a) {
 
 void zk_decode_ws_free(ZkDecodeWs* ws) {
     void* ptrs[] = { ws->blocks, ws->entries, ws->counters, ws->lit, ws->seq_lit_end, ws->seq_out_end, ws->seq_off, ws->c_off, ws->d_off,
-                     ws->huf_list, ws->seq_list, ws->seg_list, ws->d_need, ws->d_pr };
+                     ws->huf_list, ws->seq_list, ws->seg_list, ws->ord_list, ws->seg_key, ws->d_need, ws->d_pr };
     for (void* p : ptrs) if (p) cudaFree(p);
     if (ws->h_need) cudaFreeHost(ws->h_need);
     if (ws->h_pr) cudaFreeHost(ws->h_pr);
@@ -1916,14 +2007,19 @@ static int zk_decode_ensure(ZkDecodeWs* ws, uint32_t n, size_t need_blocks, size
     int rc;
     size_t cap;
     if (ws->cap_blocks < need_blocks || !ws->blocks) {
-        size_t c1 = ws->cap_blocks, c2 = ws->cap_blocks, c3 = ws->cap_blocks, c4 = ws->cap_blocks;
+        size_t c1 = ws->cap_blocks, c2 = ws->cap_blocks, c3 = ws->cap_blocks, c4 = ws->cap_blocks, c5 = ws->cap_blocks, c6 = ws->cap_blocks;
         if ((rc = zk_grow((void**)&ws->blocks, &c1, need_blocks, sizeof(ZkBlock)))) return rc;
         if ((rc = zk_grow((void**)&ws->huf_list, &c2, need_blocks, 4))) return rc;
         if ((rc = zk_grow((void**)&ws->seq_list, &c3, 2 * need_blocks, 4))) return rc;   // two lists (ZkDecodeArgs::seq_list)
         c3 /= 2;
         if ((rc = zk_grow((void**)&ws->seg_list, &c4, need_blocks, 4))) return rc;
+        if ((rc = zk_grow((void**)&ws->ord_list, &c5, 4 * need_blocks, 4))) return rc;   // ordered seq (two lists), huf, seg
+        c5 /= 4;
+        if ((rc = zk_grow((void**)&ws->seg_key, &c6, need_blocks, 4))) return rc;
         ws->cap_blocks = c1 < c2 ? (c1 < c3 ? c1 : c3) : (c2 < c3 ? c2 : c3);
         if (c4 < ws->cap_blocks) ws->cap_blocks = c4;
+        if (c5 < ws->cap_blocks) ws->cap_blocks = c5;
+        if (c6 < ws->cap_blocks) ws->cap_blocks = c6;
     }
     cap = ws->cap_lit; if ((rc = zk_grow((void**)&ws->lit, &cap, need_lit + 64, 1))) return rc; ws->cap_lit = cap;
     if (ws->cap_seq < need_seq || !ws->seq_off) {
@@ -1998,7 +2094,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     a.lit = ws->lit; a.seq_lit_end = ws->seq_lit_end; a.seq_out_end = ws->seq_out_end; a.seq_off = ws->seq_off;
     a.huf_list = ws->huf_list; a.seq_list = ws->seq_list; a.seg_list = ws->seg_list;
     a.cap_blocks = ws->cap_blocks; a.cap_lit = ws->cap_lit - 64; a.cap_seq = ws->cap_seq;
-    a.d_need = nullptr;
+    a.d_need = nullptr; a.seg_key = ws->seg_key;
     a.prefix = p.prefix; a.pranges = nullptr;
     if (p.prefix) {                              // every entry's range of the prefix buffer (the whole buffer without p.ranges)
         for (uint32_t i = 0; i < n; i++) {
@@ -2013,8 +2109,12 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
         a.d_need = ws->d_need;
     }
     if (us != stream) { ZK_CUDA_OK(cudaEventRecord(ws->ev_up, us)); ZK_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_up, 0)); }   // also orders the caller's upload of the compressed bytes
+    // the consumers of the work lists get `o`: the lists as filled, or their copies ordered heaviest first (K-D0o, K-D1o)
+    ZkDecodeArgs o = a;
+    if (ws->order) { o.seq_list = ws->ord_list; o.huf_list = ws->ord_list + 2 * ws->cap_blocks; o.seg_list = ws->ord_list + 3 * ws->cap_blocks; }
     ws->prof.begin(0, stream);
     ZK_LAUNCH(zk_scan_kernel, (n + 127) / 128, 128, 0, stream, a);
+    if (ws->order) ZK_LAUNCH(zk_order_kernel, 2, ZK_ORD_THREADS, 0, stream, a, o, 0);
     ws->prof.end(0, stream);
     // entropy stage: persistent warp-CTAs pulling groups of blocks from a work counter
     size_t est_blocks = (size_t)(total_d / ZK_BLOCK_MAX) + n;
@@ -2073,7 +2173,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
         ZK_CUDA_OK(cudaStreamWaitEvent(hs, ws->ev_scan, 0));
     }
     ws->prof.begin(2, hs);
-    ZK_LAUNCH(zk_huf_kernel, gh, 32, huf_smem + ws->huf_pad, hs, a);
+    ZK_LAUNCH(zk_huf_kernel, gh, 32, huf_smem + ws->huf_pad, hs, o);
     ws->prof.end(2, hs);
     if (hs != stream) ZK_CUDA_OK(cudaEventRecord(ws->ev_huf, hs));
     ws->prof.begin(1, stream);
@@ -2081,9 +2181,9 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
         uint32_t g2 = (uint32_t)sms * (ws->seq2_ctas ? ws->seq2_ctas : ws->seq2_fit);
         const size_t need2 = est_blocks / ZK_S2_NCH + 1;
         if (need2 < g2) g2 = (uint32_t)need2;
-        ZK_LAUNCH(zk_seq2_kernel, g2, 32, seq2_smem, stream, a);
+        ZK_LAUNCH(zk_seq2_kernel, g2, 32, seq2_smem, stream, o);
         // the blocks it passed on (none in this codec's own archives: the CTAs exit at their first work-counter read)
-        ZK_LAUNCH(zk_seq2_full_kernel, (uint32_t)sms, 32, seq2f_smem, stream, a);
+        ZK_LAUNCH(zk_seq2_full_kernel, (uint32_t)sms, 32, seq2f_smem, stream, o);
     }
     ws->prof.end(1, stream);
     if (hs != stream) ZK_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_huf, 0));
@@ -2094,9 +2194,10 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     int per_sm = (int)(((unsigned long long)n * (unsigned)(p.share > 0 ? p.share : 1) + (uint32_t)sms - 1) / (uint32_t)sms);
     if (per_sm < 1) per_sm = 1;
     int W = (int)ws->exec_warps;
-    a.exec_short = ws->exec_short;
+    a.exec_short = o.exec_short = ws->exec_short;
     ws->prof.begin(3, stream);                   // (the exec slot includes the plan kernel)
     ZK_LAUNCH(zk_plan_kernel, (n + 3) / 4, 128, 0, stream, a);
+    if (ws->order) ZK_LAUNCH(zk_order_kernel, 2, ZK_ORD_THREADS, 0, stream, a, o, 1);
     // 126 registers/thread -> 16 warps per SM; from four entries per SM on, the 96-register build of the same body
     // (20 warps per SM, <= 5 per entry) keeps every entry of the batch resident with one more warp each.  One CTA per
     // entry; the CTAs then share the batch's segments (K-D1p).
@@ -2117,8 +2218,8 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     // chains start with the warp executor's work instead of after its drain.  They are launched first, so their CTAs are resident first
     const bool beside = a.exec_short && hs != stream;
     if (beside) {
-        ZK_CUDA_OK(cudaEventRecord(ws->ev_scan, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(hs, ws->ev_scan, 0));     // after the plan
-        ZK_LAUNCH(cta_kernel, n, W * 32, ring, hs, a, ring);
+        ZK_CUDA_OK(cudaEventRecord(ws->ev_scan, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(hs, ws->ev_scan, 0));     // after the plan (and K-D1o)
+        ZK_LAUNCH(cta_kernel, n, W * 32, ring, hs, o, ring);
         ZK_CUDA_OK(cudaEventRecord(ws->ev_huf, hs));
     }
     if (a.exec_short) {          // short segments on single warps; the CTAs pull only long ones
@@ -2126,16 +2227,16 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
         const size_t need_w = est_blocks / ZK_XW_WARPS + 1;
         if (need_w < gw) gw = (uint32_t)need_w;
         void (*warp_kernel)(ZkDecodeArgs) = prefix ? zk_exec_warp_kernel<true> : zk_exec_warp_kernel<false>;
-        ZK_LAUNCH(warp_kernel, gw, 32 * ZK_XW_WARPS, ZK_XW_WARPS * ZK_XW_WIN, stream, a);
+        ZK_LAUNCH(warp_kernel, gw, 32 * ZK_XW_WARPS, ZK_XW_WARPS * ZK_XW_WIN, stream, o);
     }
     if (beside) ZK_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_huf, 0));
-    else ZK_LAUNCH(cta_kernel, n, W * 32, ring, stream, a, ring);
+    else ZK_LAUNCH(cta_kernel, n, W * 32, ring, stream, o, ring);
     ws->prof.end(3, stream);
     if (verify_checksum) { ws->prof.begin(4, stream); ZK_LAUNCH(zk_xxh64_kernel, (n + 3) / 4, 128, 0, stream, a); ws->prof.end(4, stream); }
     if (ds != stream) { ZK_CUDA_OK(cudaEventRecord(ws->ev_done, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(ds, ws->ev_done, 0)); }
     ZK_CUDA_OK(cudaMemcpyAsync(ws->h_entries, ws->entries, (size_t)n * sizeof(ZkEntry), cudaMemcpyDeviceToHost, ds));
     ZK_CUDA_OK(cudaMemcpyAsync(ws->h_counters, ws->counters, sizeof(ZkCounters), cudaMemcpyDeviceToHost, ds));
-    ws->launches += 6 + (a.exec_short ? 1 : 0) + (verify_checksum ? 1 : 0);
+    ws->launches += 6 + (a.exec_short ? 1 : 0) + (verify_checksum ? 1 : 0) + (ws->order ? 2 : 0);
     ws->pending_n = n;
     return 0;
 }

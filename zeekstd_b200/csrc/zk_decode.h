@@ -21,6 +21,7 @@ struct ZkDecodeArgs {                 // kernel parameter block (by value)
     const uint8_t* prefix;            // the buffer of the raw-content prefixes of the zstd frames (Decoder::decompress_with_prefix, decode.rs:211-214, 246-255); device pointer or nullptr
     const uint32_t* pranges;          // device, two per entry: every zstd frame of entry e has the prefix prefix[pranges[2e], pranges[2e + 1])
     const uint32_t* d_need;           // per entry: only this many leading bytes are wanted (range reads); nullptr = everything
+    uint32_t* seg_key;                // beside seg_list, same positions: the segment's cost, ZK_ORD_ALPHA x sequences + output bytes
 };
 
 struct ZkDecodeWs {                   // HBM scratch owned by a zk_ctx, grown on demand, reused across batches
@@ -33,6 +34,9 @@ struct ZkDecodeWs {                   // HBM scratch owned by a zk_ctx, grown on
     uint32_t* d_need = nullptr; uint32_t* h_need = nullptr;
     uint32_t* d_pr = nullptr; uint32_t* h_pr = nullptr;     // prefix mode: the entries' prefix ranges (ZkDecodeArgs::pranges)
     uint32_t* huf_list = nullptr; uint32_t* seq_list = nullptr; uint32_t* seg_list = nullptr;
+    uint32_t* ord_list = nullptr;     // the three work lists ordered by cost (seq 2 x cap_blocks, huf, seg), read by their consumers
+    uint32_t* seg_key = nullptr;
+    uint32_t order = 1;               // ZK_DEC_ORDER: 1 = run every work list heaviest first (zk_order_kernel), 0 = in the order it was filled
     bool attr_set = false; uint32_t ring_override = 0;
     uint32_t exec_warps = 0;          // ZK_EXEC_WARPS: warps per K-D2 CTA (at most 16); 0 = chosen from the entries per SM
     uint32_t seq2_ctas = 0;           // ZK_SEQ2_CTAS: persistent K-D1s CTAs per SM; 0 = seq2_fit
