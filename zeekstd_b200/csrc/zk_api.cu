@@ -375,46 +375,15 @@ static void zk_rebase_ranges(const uint64_t* ranges, uint32_t f0, uint32_t end, 
     }
 }
 
+// entry e decoded against its own range [ranges[2e], ranges[2e + 1]) of a prefix of prefix_len bytes (ranges == NULL: all of it), which
+// is already in device memory at d_prefix (nullptr: no prefix, the ranges are only checked)
 static int32_t zk_decompress_prefixes_one(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n, uint8_t* dst,
-                                          const uint32_t* d_need, int32_t verify, int32_t* status, const uint8_t* prefix, size_t prefix_len,
-                                          const uint64_t* ranges, bool prefix_dev = false);
-
-// entry e decoded against its own range of the prefix buffer; ranges == NULL: every entry against the whole buffer.  With ranges, the
-// entries run in groups (zk_hull_group), each with only the hull of its ranges on the device, so the buffer may be of any size
-extern "C" int32_t zk_decompress_frames_prefixes(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n,
-                                                 uint8_t* dst, const uint32_t* d_need, int32_t verify, int32_t* status,
-                                                 const uint8_t* prefix, size_t prefix_len, const uint64_t* ranges) {
-    if (!c) return ZK_ERR_INVALID_ARG;
-    if (!ranges || !prefix || prefix_len == 0)
-        return zk_decompress_prefixes_one(c, comp, c_off, d_off, n, dst, d_need, verify, status, prefix, prefix_len, ranges);
-    for (uint32_t i = 0; i < n; i++)
-        if (ranges[2 * (size_t)i] > ranges[2 * (size_t)i + 1] || ranges[2 * (size_t)i + 1] > prefix_len) return ZK_ERR_INVALID_ARG;
-    if (n && (!comp || !c_off || !d_off || !dst)) return ZK_ERR_INVALID_ARG;
-    const uint64_t group = zk_patch_group_bytes();
-    std::vector<uint64_t> rb;
-    int32_t worst = 0;
-    for (uint32_t f0 = 0; f0 < n;) {
-        uint64_t hlo, hhi;
-        const uint32_t end = zk_hull_group(ranges, f0, n, group, &hlo, &hhi);
-        zk_rebase_ranges(ranges, f0, end, hlo, &rb);
-        const int32_t rc = zk_decompress_prefixes_one(c, comp, c_off + f0, d_off + f0, end - f0, dst, d_need ? d_need + f0 : nullptr, verify,
-                                                      status ? status + f0 : nullptr, prefix + hlo, (size_t)(hhi - hlo), rb.data());
-        if (rc && !ZK_IS_ZSTD_ERR(rc)) return rc;         // the call failed; a frame's status does not stop the other groups
-        if (rc && !worst) worst = rc;
-        f0 = end;
-    }
-    return worst;
-}
-
-// prefix_dev: the prefix is already in device memory (zk_device_prefix); else host memory, uploaded (zk_upload_prefix)
-static int32_t zk_decompress_prefixes_one(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n, uint8_t* dst,
-                                          const uint32_t* d_need, int32_t verify, int32_t* status, const uint8_t* prefix, size_t prefix_len,
-                                          const uint64_t* ranges, bool prefix_dev) {
+                                          const uint32_t* d_need, int32_t verify, int32_t* status, const uint8_t* d_prefix, size_t prefix_len,
+                                          const uint64_t* ranges) {
     ZkDecCall q = {comp, c_off, d_off, dst, verify, status, ZkDecodeParams()};
     std::vector<uint32_t> rw;
     int32_t rc = zk_prefix_ranges(ranges, n, prefix_len, &rw);
-    if (!rc) rc = prefix_dev ? zk_device_prefix(prefix, prefix_len, &q.p.prefix, &q.p.prefix_len)
-                             : zk_upload_prefix(c, prefix, prefix_len, &q.p.prefix, &q.p.prefix_len);
+    if (!rc) rc = zk_device_prefix(d_prefix, prefix_len, &q.p.prefix, &q.p.prefix_len);
     if (rc) return rc;
     if (q.p.prefix && ranges) q.p.ranges = rw.data();
     if (n && (!comp || !c_off || !d_off || !dst)) return ZK_ERR_INVALID_ARG;
@@ -995,8 +964,6 @@ struct ZkReuseKeyHash {
     size_t operator()(const ZkReuseKey& k) const { return (size_t)(k.key ^ (unsigned long long)k.size * 0x9E3779B97F4A7C15ull); }
 };
 
-struct ZkOldArchive { const uint8_t* comp; const uint64_t* c_off; const uint64_t* d_off; };
-
 static uint32_t zk_le32(const uint8_t* p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
 
 // the Content_Checksum_flag of the first zstd frame of an entry (skippable frames before it are passed over): 0 or 1, -1 if it has none
@@ -1018,9 +985,23 @@ static int32_t zk_reuse_buf(zk_ctx* c, int i, size_t need, uint8_t** out) {
     return rc;
 }
 
-// old entries list[0, m): their bytes uploaded back to back (runs of consecutive entries in one copy) into buffer 0 and decoded, with
-// checksum verification, into buffer 1 -> *c_rel / *d_rel (m + 1 offsets in those buffers), per-entry statuses in *status
-static int32_t zk_reuse_decode(zk_ctx* c, const ZkOldArchive& o, const uint32_t* list, uint32_t m, std::vector<uint64_t>* c_rel,
+// entries list[0, m) of a host archive copied back to back into device memory d on st, entry list[k] at d + c_rel[k]: a run of
+// consecutive entries in one copy
+static int32_t zk_upload_entries(const zk_reference_archive& r, const uint32_t* list, uint32_t m, const uint64_t* c_rel, uint8_t* d,
+                                 cudaStream_t st) {
+    for (uint32_t k0 = 0; k0 < m;) {
+        uint32_t k1 = k0 + 1;
+        while (k1 < m && list[k1] == list[k1 - 1] + 1) k1++;
+        const size_t bytes = (size_t)(c_rel[k1] - c_rel[k0]);
+        if (bytes) ZK_CUDA_OK(cudaMemcpyAsync(d + c_rel[k0], r.comp + r.c_off[list[k0]], bytes, cudaMemcpyHostToDevice, st));
+        k0 = k1;
+    }
+    return 0;
+}
+
+// old entries list[0, m): their bytes uploaded back to back into buffer 0 and decoded, with checksum verification, into buffer 1
+// -> *c_rel / *d_rel (m + 1 offsets in those buffers), per-entry statuses in *status
+static int32_t zk_reuse_decode(zk_ctx* c, const zk_reference_archive& o, const uint32_t* list, uint32_t m, std::vector<uint64_t>* c_rel,
                                std::vector<uint64_t>* d_rel, std::vector<int32_t>* status, uint8_t** comp, uint8_t** dec) {
     c_rel->assign(m + 1, 0); d_rel->assign(m + 1, 0); status->assign(m, 0);
     for (uint32_t k = 0; k < m; k++) {
@@ -1032,13 +1013,7 @@ static int32_t zk_reuse_decode(zk_ctx* c, const ZkOldArchive& o, const uint32_t*
     if (!rc) rc = zk_reuse_buf(c, 1, (*d_rel)[m], dec);
     if (rc || m == 0) return rc;
     ZkSlot& s = c->slot[0];
-    for (uint32_t k0 = 0; k0 < m;) {
-        uint32_t k1 = k0 + 1;
-        while (k1 < m && list[k1] == list[k1 - 1] + 1) k1++;
-        const size_t bytes = (size_t)((*c_rel)[k1] - (*c_rel)[k0]);
-        if (bytes) ZK_CUDA_OK(cudaMemcpyAsync(*comp + (*c_rel)[k0], o.comp + o.c_off[list[k0]], bytes, cudaMemcpyHostToDevice, s.stream));
-        k0 = k1;
-    }
+    if ((rc = zk_upload_entries(o, list, m, c_rel->data(), *comp, s.stream))) return rc;
     rc = zk_decode_batch(&s.dws, s.stream, *comp, c_rel->data(), d_rel->data(), m, *dec, 1, ZkDecodeParams(), status->data());
     if (rc == ZK_INT_CUDA || rc == -(int)ZKZ_MEMORY_ALLOCATION) return rc;
     return 0;                                               // an entry that fails to decode is only not a candidate
@@ -1068,7 +1043,7 @@ extern "C" int32_t zk_compress_frames_sized_reuse(zk_ctx* c, const uint8_t* src,
     ZK_CUDA_OK(cudaSetDevice(c->device));
     ZkSlot& s = c->slot[0];
     const cudaStream_t st = s.stream;
-    const ZkOldArchive o = {old_comp, old_c_off, old_d_off};
+    const zk_reference_archive o = {old_comp, old_len, old_c_off, old_d_off, old_n};
     const size_t bits = zk_env_size("ZK_REUSE_KEY_BITS", 64);          // tests: keep only the key's low bits (0: every key is equal)
     const unsigned long long kmask = bits >= 64 ? ~0ull : (1ull << bits) - 1;
     const bool trace = getenv("ZK_E2E_TRACE") != nullptr;
@@ -1234,62 +1209,6 @@ static int32_t zk_patch_scan(zk_ctx* c, const uint8_t* src, uint64_t len, std::v
     return 0;
 }
 
-extern "C" int32_t zk_patch_ranges(zk_ctx* c, const uint8_t* new_src, const uint32_t* frame_sizes, uint32_t n_frames, const uint8_t* old,
-                                   uint64_t old_len, uint64_t margin, uint64_t* ranges) {
-    if (!c || (n_frames && (!frame_sizes || !ranges)) || (old_len && !old)) return ZK_ERR_INVALID_ARG;
-    if (old_len >= (1ull << 62) || margin >= (1ull << 62)) return ZK_ERR_INVALID_ARG;
-    ZkPatchTables t;
-    t.fa.assign((size_t)n_frames + 1, 0);
-    for (uint32_t f = 0; f < n_frames; f++) t.fa[f + 1] = t.fa[f] + frame_sizes[f];
-    const uint64_t n = t.fa[n_frames];
-    if (n && !new_src) return ZK_ERR_INVALID_ARG;
-    if (n_frames == 0) return 0;
-    ZK_CUDA_OK(cudaSetDevice(c->device));
-    int32_t rc = zk_patch_scan(c, old, old_len, &t.okeys, &t.opos);
-    if (!rc) rc = zk_patch_scan(c, new_src, n, &t.nkeys, &t.npos);
-    if (rc) return rc;
-    if (t.okeys.size() > 0xFFFFFFF0ull || t.nkeys.size() > 0xFFFFFFF0ull) return ZK_ERR_INVALID_ARG;
-    t.fanc.assign((size_t)n_frames + 1, 0);
-    for (uint32_t f = 0, i = 0; f <= n_frames; f++) {
-        while (i < t.npos.size() && t.npos[i] < t.fa[f]) i++;
-        t.fanc[f] = f == n_frames ? (uint32_t)t.npos.size() : i;
-    }
-    return zk_patch_join(&c->slot[0].ews, c->slot[0].stream, t, n_frames, old_len, margin, (unsigned long long*)ranges);
-}
-
-// frames of NEW against their ranges of OLD, in groups of consecutive frames whose hull of OLD is at most ZK_PATCH_GROUP_BYTES: each group is one
-// zk_compress_frames_sized_prefixes call (ldm = 1) on its hull, with the ranges rebased, so no frame's bytes depend on the grouping.  A group
-// whose ranges are all empty is level 16's plain frames, which is what that call writes for a frame with an empty range.
-extern "C" int32_t zk_compress_frames_patch(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
-                                            int32_t checksum, const uint8_t* old, uint64_t old_len, const uint64_t* ranges, uint8_t* dst,
-                                            size_t dst_cap, uint32_t* c_sizes, size_t* dst_len) {
-    if (!c || (n_frames && (!frame_sizes || !ranges || !dst)) || (old_len && !old)) return ZK_ERR_INVALID_ARG;
-    if (dst_len) *dst_len = 0;
-    for (uint32_t f = 0; f < n_frames; f++)
-        if (ranges[2 * (size_t)f] > ranges[2 * (size_t)f + 1] || ranges[2 * (size_t)f + 1] > old_len) return ZK_ERR_INVALID_ARG;
-    const uint64_t group = zk_patch_group_bytes();
-    std::vector<uint64_t> rb;
-    std::vector<uint32_t> cs(n_frames);
-    size_t out = 0, in = 0;
-    for (uint32_t f0 = 0; f0 < n_frames;) {
-        uint64_t hlo, hhi;
-        const uint32_t end = zk_hull_group(ranges, f0, n_frames, group, &hlo, &hhi);
-        zk_rebase_ranges(ranges, f0, end, hlo, &rb);
-        size_t len = 0, bytes = 0;
-        for (uint32_t f = f0; f < end; f++) bytes += frame_sizes[f];
-        const int32_t rc = hhi > hlo
-            ? zk_compress_frames_sized_prefixes(c, src ? src + in : nullptr, frame_sizes + f0, end - f0, level, checksum, old + hlo, (size_t)(hhi - hlo),
-                                                rb.data(), 1, 0, dst + out, dst_cap - out, cs.data() + f0, &len)
-            : zk_compress_frames_sized(c, src ? src + in : nullptr, frame_sizes + f0, end - f0, 16, checksum, nullptr, 0, dst + out,
-                                       dst_cap - out, cs.data() + f0, &len);
-        if (rc) return rc;
-        out += len; in += bytes; f0 = end;
-    }
-    if (c_sizes && n_frames) memcpy(c_sizes, cs.data(), (size_t)n_frames * 4);
-    if (dst_len) *dst_len = out;
-    return 0;
-}
-
 // the slice frame (a skippable frame at the start of entry 0): magic, payload size, "ZKSLICE1", u64 old_len, u32 n, n x (u64 lo, u64 hi)
 static const uint8_t zk_slice_tag[8] = {'Z', 'K', 'S', 'L', 'I', 'C', 'E', '1'};
 static void zk_put_le(uint8_t* p, uint64_t v, int bytes) { for (int i = 0; i < bytes; i++) p[i] = (uint8_t)(v >> (8 * i)); }
@@ -1332,13 +1251,14 @@ extern "C" int32_t zk_patch_slices_read(const uint8_t* src, size_t len, uint32_t
 }
 
 // ---------------------------------------------------------------------------------------------
-// Seekable patches against a seekable archive or a chain of them (DESIGN §3.4.2, §3.4.3): OLD is the decoded content of the head of a
-// reference chain R_0 <- R_1 <- ... <- R_{d-1} (R_0 a plain archive, every other level a seekable patch of the level below), and the calls
-// above run on it without any level's content ever being on the host.  For each group of entries (zk_hull_group), the entries of the head
-// whose output overlaps the group's hull are decoded on slot 0 straight into the prefix arena (c->d_prefix), the last one only as far as
-// the hull's end, and the prefix machinery reads the hull from there (zk_device_prefix).  A patch level first has the level below it decode
-// the hulls of its entries' slices into that level's own arena (c->d_level), recursively.  The anchor pass decodes the head in runs of
-// whole entries instead.  The _archive calls are the chain of one level.
+// The reference of a seekable patch (DESIGN §3.4.1-§3.4.3): OLD is the content of the head of a reference chain R_0 <- R_1 <- ... <- R_{d-1}.
+// The root R_0 is OLD's raw bytes in host memory (the raw calls, d = 1) or a plain archive; every other level is a seekable patch of the
+// level below.  Every call works on groups of its entries (zk_hull_group) in one loop, zk_ref_groups: Need(head, hull) makes the group's
+// hull resident in the prefix arena (c->d_prefix), and the prefix machinery reads it from there (zk_device_prefix).  Need of a raw root
+// copies the hull up.  Need of an archive decodes, on slot 0, the entries whose output overlaps the hull, the last one only as far as the
+// hull's end.  Need of a patch level runs the same loop on its own entries against the level below; each level below the head has its own
+// arena (c->d_level).  The anchor pass reads OLD whole instead: a raw root in pieces, any other head decoded in runs of whole entries.
+// The _archive calls are the chain of one level.
 // ---------------------------------------------------------------------------------------------
 
 // decoded content starts this far into a level's arena: the anchor pass puts the 63 bytes before a run in front of it
@@ -1347,11 +1267,12 @@ extern "C" int32_t zk_patch_slices_read(const uint8_t* src, size_t len, uint32_t
 // one level of a chain, and what the latest zk_ref_decode of it left in its arena
 struct ZkRefLevel {
     zk_reference_archive r = {};
+    bool raw = false;                                       // a raw root: r.comp holds OLD's r.len bytes, and r has no entries
     std::vector<uint64_t> slices;                           // a patch level: entry g reads [slices[2g], slices[2g + 1]) of the level below
     void** arena = nullptr; size_t* cap = nullptr;          // the level's device arena
     std::vector<uint32_t> list;                             // the entries decoded last, in order,
     std::vector<int32_t> status;                            // their statuses (a failure below them included),
-    uint64_t base = 0;                                      // and the content offset of arena byte ZK_REF_HEAD
+    uint64_t base = 0;                                      // and the content offset of arena byte ZK_REF_HEAD (a raw root: of byte 0)
 };
 typedef std::vector<ZkRefLevel> ZkChain;
 
@@ -1397,16 +1318,25 @@ static int32_t zk_chain_open(zk_ctx* c, const zk_reference_archive* chain, uint3
     return 0;
 }
 
-// the first entry of l.list (decoded by zk_ref_decode) with a non-zero status whose output overlaps [lo, hi) -> that status, else 0
+// OLD's old_len bytes in host memory -> *ch, the chain of one raw root, resident in the prefix arena
+static void zk_chain_raw(zk_ctx* c, const uint8_t* old, uint64_t old_len, ZkChain* ch) {
+    ch->assign(1, ZkRefLevel());
+    ZkRefLevel& l = ch->front();
+    l.r.comp = old; l.r.len = (size_t)old_len; l.raw = true;
+    l.arena = &c->d_prefix; l.cap = &c->cap_prefix;
+}
+
+// the first entry of l.list (decoded by zk_ref_decode) with a non-zero status whose output overlaps [lo, hi) -> that status, else 0 (a raw
+// root has no entries: always 0)
 static int32_t zk_ref_failure(const ZkRefLevel& l, uint64_t lo, uint64_t hi) {
     for (size_t k = 0; k < l.list.size(); k++)
         if (l.status[k] && l.r.d_off[l.list[k] + 1] > lo && l.r.d_off[l.list[k]] < hi) return l.status[k];
     return 0;
 }
 
-// entries l.list[a, b) uploaded back to back through slot 0 (runs of consecutive entries in one copy) and decoded into the level's arena,
-// entry list[k] at d_rel[k], against p's prefix; need: one per entry of the list (empty: every entry whole) -> l.status[a, b).  Returns 0
-// or a failure of the call itself (an entry that fails to decode: its status)
+// entries l.list[a, b) uploaded back to back through slot 0 and decoded into the level's arena, entry list[k] at d_rel[k], against p's
+// prefix; need: one per entry of the list (empty: every entry whole) -> l.status[a, b).  Returns 0 or a failure of the call itself (an entry
+// that fails to decode: its status)
 static int32_t zk_ref_run(zk_ctx* c, ZkRefLevel& l, uint32_t a, uint32_t b, const std::vector<uint64_t>& d_rel, int verify,
                           const std::vector<uint32_t>& need, ZkDecodeParams p) {
     const zk_reference_archive& r = l.r;
@@ -1415,14 +1345,8 @@ static int32_t zk_ref_run(zk_ctx* c, ZkRefLevel& l, uint32_t a, uint32_t b, cons
     for (uint32_t k = 0; k < m; k++) c_rel[k + 1] = c_rel[k] + (r.c_off[l.list[a + k] + 1] - r.c_off[l.list[a + k]]);
     ZkSlot& s = c->slot[0];
     int32_t rc = zk_slot_ensure(&s, (size_t)c_rel[m] + 32, 0);
+    if (!rc) rc = zk_upload_entries(r, l.list.data() + a, m, c_rel.data(), s.d_in, s.stream);
     if (rc) return rc;
-    for (uint32_t k0 = 0; k0 < m;) {
-        uint32_t k1 = k0 + 1;
-        while (k1 < m && l.list[a + k1] == l.list[a + k1 - 1] + 1) k1++;
-        const size_t bytes = (size_t)(c_rel[k1] - c_rel[k0]);
-        if (bytes) ZK_CUDA_OK(cudaMemcpyAsync(s.d_in + c_rel[k0], r.comp + r.c_off[l.list[a + k0]], bytes, cudaMemcpyHostToDevice, s.stream));
-        k0 = k1;
-    }
     if (!need.empty()) p.need = need.data() + a;
     rc = zk_decode_batch(&s.dws, s.stream, s.d_in, c_rel.data(), d_rel.data() + a, m, (uint8_t*)*l.arena + ZK_REF_HEAD, verify, p,
                          l.status.data() + a);
@@ -1431,15 +1355,60 @@ static int32_t zk_ref_run(zk_ctx* c, ZkRefLevel& l, uint32_t a, uint32_t b, cons
     return 0;
 }
 
-// Need(i, [lo, hi)), lo < hi: level i's content [lo, hi) made resident.  The non-empty entries of R_i whose output overlaps it, l.list, are
-// decoded into the level's arena from ZK_REF_HEAD on (l.base: the content offset there), the last one only as far as hi (need: no checksum
-// on it).  A patch level groups its entries' slices (zk_hull_group, empty slices skipped); per group with a non-empty hull, Need(i - 1,
-// hull) runs first and the group's entries are then decoded against it, rebased.  An entry whose slice overlaps an entry below that failed
-// takes that status and is not decoded.  Returns 0 or a failure of the call itself.  Device memory, per level: the decoded bytes from the
-// first entry's start to hi, plus the rest of the block that holds hi (the decoder stops at a block's end)
+static int32_t zk_ref_decode(zk_ctx* c, ZkChain& ch, uint32_t i, uint64_t lo, uint64_t hi, int verify);
+
+// The group loop of every call on a reference: entries [0, n), entry k reading [ranges[2k], ranges[2k + 1]) of level i's content, in groups
+// (zk_hull_group).  Per group, Need(i, hull) runs when the hull is not empty; then run(a, b, prefix, len, rebased) gets each run [a, b) of
+// the group's entries with the hull on the device (prefix, len; nullptr, 0 for an empty hull) and the run's ranges rebased to it.
+// status: an entry whose range overlaps a failed entry of level i takes that status there and is in no run.  status == nullptr: a failed
+// entry anywhere under the hull fails the call, and the group is one run.  Returns 0 or a failure of the call itself (run's included)
+template <class Run>
+static int32_t zk_ref_groups(zk_ctx* c, ZkChain& ch, uint32_t i, const uint64_t* ranges, uint32_t n, int verify, int32_t* status,
+                             const Run& run) {
+    const ZkRefLevel& below = ch[i];
+    const uint64_t group = zk_patch_group_bytes();
+    std::vector<uint64_t> rb;
+    std::vector<int32_t> fail;
+    int32_t rc;
+    for (uint32_t f0 = 0; f0 < n;) {
+        uint64_t hlo, hhi;
+        const uint32_t end = zk_hull_group(ranges, f0, n, group, &hlo, &hhi);
+        zk_rebase_ranges(ranges, f0, end, hlo, &rb);
+        const uint8_t* prefix = nullptr;
+        fail.assign(end - f0, 0);
+        if (hhi > hlo) {
+            if ((rc = zk_ref_decode(c, ch, i, hlo, hhi, verify))) return rc;
+            prefix = (const uint8_t*)*below.arena + (below.raw ? 0 : ZK_REF_HEAD) + (hlo - below.base);
+            if (!status && (rc = zk_ref_failure(below, hlo, hhi))) return rc;
+            for (uint32_t f = f0; status && f < end; f++)
+                if (ranges[2 * (size_t)f] < ranges[2 * (size_t)f + 1]) fail[f - f0] = zk_ref_failure(below, ranges[2 * (size_t)f], ranges[2 * (size_t)f + 1]);
+        }
+        for (uint32_t a = f0; a < end;) {
+            if (fail[a - f0]) { status[a] = fail[a - f0]; a++; continue; }
+            uint32_t b = a + 1;
+            while (b < end && !fail[b - f0]) b++;
+            if ((rc = run(a, b, prefix, hhi - hlo, rb.data() + 2 * (size_t)(a - f0)))) return rc;
+            a = b;
+        }
+        f0 = end;
+    }
+    return 0;
+}
+
+// Need(i, [lo, hi)), lo < hi: level i's content [lo, hi) made resident in its arena from ZK_REF_HEAD on (l.base: the content offset there).
+// A raw root uploads it as any prefix (zk_upload_prefix: at the arena's start, with the 64 bytes of padding the kernels' wide loads read
+// past its end); it has no entries, so nothing of it fails to decode.  Any other level decodes its non-empty entries whose output overlaps
+// it, l.list, the last one only as far as hi (need: no checksum on it); a patch level decodes them in the group loop against level i - 1,
+// its entries' slices as their ranges.  Returns 0 or a failure of the call itself.  Device memory, per level: a raw root's hull, or the
+// decoded bytes from the first entry's start to hi, plus the rest of the block that holds hi (the decoder stops at a block's end)
 static int32_t zk_ref_decode(zk_ctx* c, ZkChain& ch, uint32_t i, uint64_t lo, uint64_t hi, int verify) {
     ZkRefLevel& l = ch[i];
     const zk_reference_archive& r = l.r;
+    if (l.raw) {                                            // the arena is c->d_prefix
+        const uint8_t* d_prefix; uint32_t d_len;
+        l.base = lo;
+        return zk_upload_prefix(c, r.comp + lo, (size_t)(hi - lo), &d_prefix, &d_len);
+    }
     l.list.clear();
     uint32_t g = (uint32_t)(std::upper_bound(r.d_off, r.d_off + r.n + 1, lo) - r.d_off) - 1;    // the entry that holds lo
     for (; g < r.n && r.d_off[g] < hi; g++)
@@ -1458,48 +1427,56 @@ static int32_t zk_ref_decode(zk_ctx* c, ZkChain& ch, uint32_t i, uint64_t lo, ui
     if (rc) return rc;
     l.status.assign(m, 0);
     if (i == 0) return zk_ref_run(c, l, 0, m, d_rel, verify, need, ZkDecodeParams());
-    std::vector<uint64_t> sl(2 * (size_t)m), rb;
+    std::vector<uint64_t> sl(2 * (size_t)m);
     for (uint32_t k = 0; k < m; k++) { sl[2 * (size_t)k] = l.slices[2 * (size_t)l.list[k]]; sl[2 * (size_t)k + 1] = l.slices[2 * (size_t)l.list[k] + 1]; }
-    const ZkRefLevel& below = ch[i - 1];
-    const uint64_t group = zk_patch_group_bytes();
-    std::vector<int32_t> fail;
     std::vector<uint32_t> rw;
-    for (uint32_t k0 = 0; k0 < m;) {
-        uint64_t hlo, hhi;
-        const uint32_t k1 = zk_hull_group(sl.data(), k0, m, group, &hlo, &hhi);
-        zk_rebase_ranges(sl.data(), k0, k1, hlo, &rb);
+    auto run = [&](uint32_t a, uint32_t b, const uint8_t* prefix, uint64_t len, const uint64_t* rb) -> int32_t {
         ZkDecodeParams p;
-        fail.assign(k1 - k0, 0);
-        if (hhi > hlo) {
-            if ((rc = zk_ref_decode(c, ch, i - 1, hlo, hhi, verify))) return rc;
-            if ((rc = zk_device_prefix((const uint8_t*)*below.arena + ZK_REF_HEAD + (hlo - below.base), (size_t)(hhi - hlo), &p.prefix,
-                                       &p.prefix_len))) return rc;
-            for (uint32_t k = k0; k < k1; k++)
-                if (sl[2 * (size_t)k] < sl[2 * (size_t)k + 1]) fail[k - k0] = zk_ref_failure(below, sl[2 * (size_t)k], sl[2 * (size_t)k + 1]);
-        }
-        for (uint32_t a = k0; a < k1;) {                    // runs of entries whose slices decoded
-            if (fail[a - k0]) { l.status[a] = fail[a - k0]; a++; continue; }
-            uint32_t b = a + 1;
-            while (b < k1 && !fail[b - k0]) b++;
-            if (p.prefix) {
-                if ((rc = zk_prefix_ranges(rb.data() + 2 * (size_t)(a - k0), b - a, (size_t)(hhi - hlo), &rw))) return rc;
-                p.ranges = rw.data();
-            }
-            if ((rc = zk_ref_run(c, l, a, b, d_rel, verify, need, p))) return rc;
-            a = b;
-        }
-        k0 = k1;
-    }
-    return 0;
+        int32_t rc = zk_device_prefix(prefix, (size_t)len, &p.prefix, &p.prefix_len);
+        if (!rc && p.prefix && !(rc = zk_prefix_ranges(rb, b - a, (size_t)len, &rw))) p.ranges = rw.data();
+        return rc ? rc : zk_ref_run(c, l, a, b, d_rel, verify, need, p);
+    };
+    return zk_ref_groups(c, ch, i - 1, sl.data(), m, verify, l.status.data(), run);
 }
 
-// OLD [lo, hi) as a device prefix, for the calls that cannot use a partly decoded OLD: the first failing entry's status is the call's
-static int32_t zk_ref_prefix(zk_ctx* c, ZkChain& ch, uint64_t lo, uint64_t hi, const uint8_t** prefix) {
-    const ZkRefLevel& h = ch.back();
-    int32_t rc = zk_ref_decode(c, ch, (uint32_t)ch.size() - 1, lo, hi, 1);
-    if (!rc) rc = zk_ref_failure(h, lo, hi);
-    *prefix = (const uint8_t*)c->d_prefix + ZK_REF_HEAD + (lo - h.base);
-    return rc;
+// the decompress calls with ranges of a non-empty OLD: a call failure leaves `status` as it was
+static int32_t zk_ref_decompress(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n, uint8_t* dst,
+                                 const uint32_t* d_need, int32_t verify, int32_t* status, ZkChain& ch, uint64_t old_len, const uint64_t* ranges) {
+    for (uint32_t i = 0; i < n; i++)
+        if (ranges[2 * (size_t)i] > ranges[2 * (size_t)i + 1] || ranges[2 * (size_t)i + 1] > old_len) return ZK_ERR_INVALID_ARG;
+    if (n && (!comp || !c_off || !d_off || !dst)) return ZK_ERR_INVALID_ARG;
+    if (n == 0) return 0;
+    ZK_CUDA_OK(cudaSetDevice(c->device));
+    std::vector<int32_t> st(n, 0);
+    int32_t worst = 0;                                      // a failure with no entry status (decode scratch that could not grow)
+    auto run = [&](uint32_t a, uint32_t b, const uint8_t* prefix, uint64_t len, const uint64_t* rb) -> int32_t {
+        const int32_t rc = zk_decompress_prefixes_one(c, comp, c_off + a, d_off + a, b - a, dst, d_need ? d_need + a : nullptr, verify,
+                                                      st.data() + a, prefix, (size_t)len, rb);
+        if (rc && !ZK_IS_ZSTD_ERR(rc)) return rc;           // the call failed; a frame's status does not stop the other groups
+        if (rc && !worst) worst = rc;
+        return 0;
+    };
+    const int32_t rc = zk_ref_groups(c, ch, (uint32_t)ch.size() - 1, ranges, n, verify, st.data(), run);
+    if (rc) return rc;
+    if (status) memcpy(status, st.data(), (size_t)n * 4);
+    for (uint32_t i = 0; i < n; i++) if (st[i]) return st[i];
+    return worst;
+}
+
+// entry e decoded against its own range of the prefix buffer; ranges == NULL: every entry against the whole buffer.  With ranges, the
+// entries run in groups, each with only the hull of its ranges on the device, so the buffer may be of any size
+extern "C" int32_t zk_decompress_frames_prefixes(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n,
+                                                 uint8_t* dst, const uint32_t* d_need, int32_t verify, int32_t* status,
+                                                 const uint8_t* prefix, size_t prefix_len, const uint64_t* ranges) {
+    if (!c) return ZK_ERR_INVALID_ARG;
+    if (!ranges || !prefix || prefix_len == 0) {
+        const uint8_t* d_prefix; uint32_t d_len;
+        const int32_t rc = zk_upload_prefix(c, prefix, prefix_len, &d_prefix, &d_len);
+        return rc ? rc : zk_decompress_prefixes_one(c, comp, c_off, d_off, n, dst, d_need, verify, status, d_prefix, prefix_len, ranges);
+    }
+    ZkChain ch;
+    zk_chain_raw(c, prefix, prefix_len, &ch);
+    return zk_ref_decompress(c, comp, c_off, d_off, n, dst, d_need, verify, status, ch, prefix_len, ranges);
 }
 
 extern "C" int32_t zk_decompress_frames_prefixes_chain(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n,
@@ -1508,7 +1485,7 @@ extern "C" int32_t zk_decompress_frames_prefixes_chain(zk_ctx* c, const uint8_t*
     if (!c) return ZK_ERR_INVALID_ARG;
     ZkChain ch;
     uint64_t old_len = 0;
-    int32_t rc = zk_chain_open(c, chain, depth, &ch, &old_len);
+    const int32_t rc = zk_chain_open(c, chain, depth, &ch, &old_len);
     if (rc) return rc;
     std::vector<uint64_t> whole;                            // no ranges: every entry against all of OLD
     if (!ranges) {
@@ -1516,40 +1493,7 @@ extern "C" int32_t zk_decompress_frames_prefixes_chain(zk_ctx* c, const uint8_t*
         for (uint32_t i = 0; i < n; i++) whole[2 * (size_t)i + 1] = old_len;
         ranges = whole.data();
     }
-    for (uint32_t i = 0; i < n; i++)
-        if (ranges[2 * (size_t)i] > ranges[2 * (size_t)i + 1] || ranges[2 * (size_t)i + 1] > old_len) return ZK_ERR_INVALID_ARG;
-    if (n && (!comp || !c_off || !d_off || !dst)) return ZK_ERR_INVALID_ARG;
-    if (n == 0) return 0;
-    ZK_CUDA_OK(cudaSetDevice(c->device));
-    const uint64_t group = zk_patch_group_bytes();
-    const ZkRefLevel& h = ch.back();
-    std::vector<uint64_t> rb;
-    std::vector<int32_t> st(n, 0), fail;
-    for (uint32_t f0 = 0; f0 < n;) {
-        uint64_t hlo, hhi;
-        const uint32_t end = zk_hull_group(ranges, f0, n, group, &hlo, &hhi);
-        zk_rebase_ranges(ranges, f0, end, hlo, &rb);
-        ch.back().list.clear();
-        if (hhi > hlo && (rc = zk_ref_decode(c, ch, depth - 1, hlo, hhi, verify))) return rc;
-        const uint8_t* prefix = hhi > hlo ? (const uint8_t*)c->d_prefix + ZK_REF_HEAD + (hlo - h.base) : nullptr;
-        // an entry whose range overlaps a reference entry that failed takes its status; the others run in runs of consecutive entries
-        fail.assign(end - f0, 0);
-        for (uint32_t f = f0; f < end; f++)
-            if (ranges[2 * (size_t)f] < ranges[2 * (size_t)f + 1]) fail[f - f0] = zk_ref_failure(h, ranges[2 * (size_t)f], ranges[2 * (size_t)f + 1]);
-        for (uint32_t a = f0; a < end;) {
-            if (fail[a - f0]) { st[a] = fail[a - f0]; a++; continue; }
-            uint32_t b = a + 1;
-            while (b < end && !fail[b - f0]) b++;
-            rc = zk_decompress_prefixes_one(c, comp, c_off + a, d_off + a, b - a, dst, d_need ? d_need + a : nullptr, verify, st.data() + a,
-                                            prefix, (size_t)(hhi - hlo), rb.data() + 2 * (size_t)(a - f0), true);
-            if (rc && !ZK_IS_ZSTD_ERR(rc)) return rc;       // the call failed; a frame's status does not stop the other groups
-            a = b;
-        }
-        f0 = end;
-    }
-    if (status) memcpy(status, st.data(), (size_t)n * 4);
-    for (uint32_t i = 0; i < n; i++) if (st[i]) return st[i];
-    return 0;
+    return zk_ref_decompress(c, comp, c_off, d_off, n, dst, d_need, verify, status, ch, old_len, ranges);
 }
 
 extern "C" int32_t zk_decompress_frames_prefixes_archive(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off, uint32_t n,
@@ -1560,47 +1504,61 @@ extern "C" int32_t zk_decompress_frames_prefixes_archive(zk_ctx* c, const uint8_
     return zk_decompress_frames_prefixes_chain(c, comp, c_off, d_off, n, dst, d_need, verify, status, &r, 1, ranges);
 }
 
-// frames of NEW against their ranges of OLD: zk_compress_frames_patch's groups, each hull decoded from the chain into the prefix arena
+// frames of NEW against their ranges of OLD, group by group: each group is one zk_compress_frames_sized_prefixes call (ldm = 1) on its hull,
+// with the ranges rebased, so no frame's bytes depend on the grouping.  A group whose ranges are all empty is level 16's plain frames, which
+// is what that call writes for a frame with an empty range.  A reference entry that fails under a hull fails the call
+static int32_t zk_ref_compress(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level, int32_t checksum,
+                               ZkChain& ch, uint64_t old_len, const uint64_t* ranges, uint8_t* dst, size_t dst_cap, uint32_t* c_sizes,
+                               size_t* dst_len) {
+    if (dst_len) *dst_len = 0;
+    for (uint32_t f = 0; f < n_frames; f++)
+        if (ranges[2 * (size_t)f] > ranges[2 * (size_t)f + 1] || ranges[2 * (size_t)f + 1] > old_len) return ZK_ERR_INVALID_ARG;
+    if (n_frames) ZK_CUDA_OK(cudaSetDevice(c->device));
+    std::vector<uint32_t> cs(n_frames);
+    size_t out = 0, in = 0;
+    auto run = [&](uint32_t a, uint32_t b, const uint8_t* prefix, uint64_t len, const uint64_t* rb) -> int32_t {
+        size_t got = 0, bytes = 0;
+        for (uint32_t f = a; f < b; f++) bytes += frame_sizes[f];
+        int32_t rc;
+        if (prefix) {
+            ZkCompressReq q;
+            q.policy = ZK_FRAMES_SIZED; q.sizes = frame_sizes + a; q.count = b - a; q.src = src ? src + in : nullptr;
+            q.prefix = prefix; q.prefix_len = (size_t)len; q.prefix_dev = true; q.ranges = rb;
+            q.params.level = level; q.params.checksum = checksum; q.params.ldm = true;
+            q.dst = dst + out; q.dst_cap = dst_cap - out; q.c_sizes = cs.data() + a; q.dst_len = &got;
+            rc = zk_compress(c, q);
+        } else {
+            rc = zk_compress_frames_sized(c, src ? src + in : nullptr, frame_sizes + a, b - a, 16, checksum, nullptr, 0, dst + out, dst_cap - out,
+                                          cs.data() + a, &got);
+        }
+        out += got; in += bytes;
+        return rc;
+    };
+    const int32_t rc = zk_ref_groups(c, ch, (uint32_t)ch.size() - 1, ranges, n_frames, 1, nullptr, run);
+    if (rc) return rc;
+    if (c_sizes && n_frames) memcpy(c_sizes, cs.data(), (size_t)n_frames * 4);
+    if (dst_len) *dst_len = out;
+    return 0;
+}
+
+extern "C" int32_t zk_compress_frames_patch(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
+                                            int32_t checksum, const uint8_t* old, uint64_t old_len, const uint64_t* ranges, uint8_t* dst,
+                                            size_t dst_cap, uint32_t* c_sizes, size_t* dst_len) {
+    if (!c || (n_frames && (!frame_sizes || !ranges || !dst)) || (old_len && !old)) return ZK_ERR_INVALID_ARG;
+    ZkChain ch;
+    zk_chain_raw(c, old, old_len, &ch);
+    return zk_ref_compress(c, src, frame_sizes, n_frames, level, checksum, ch, old_len, ranges, dst, dst_cap, c_sizes, dst_len);
+}
+
 extern "C" int32_t zk_compress_frames_patch_chain(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
                                                   int32_t checksum, const zk_reference_archive* chain, uint32_t depth, const uint64_t* ranges,
                                                   uint8_t* dst, size_t dst_cap, uint32_t* c_sizes, size_t* dst_len) {
     if (!c || (n_frames && (!frame_sizes || !ranges || !dst))) return ZK_ERR_INVALID_ARG;
     ZkChain ch;
     uint64_t old_len = 0;
-    int32_t rc = zk_chain_open(c, chain, depth, &ch, &old_len);
+    const int32_t rc = zk_chain_open(c, chain, depth, &ch, &old_len);
     if (rc) return rc;
-    if (dst_len) *dst_len = 0;
-    for (uint32_t f = 0; f < n_frames; f++)
-        if (ranges[2 * (size_t)f] > ranges[2 * (size_t)f + 1] || ranges[2 * (size_t)f + 1] > old_len) return ZK_ERR_INVALID_ARG;
-    if (n_frames) ZK_CUDA_OK(cudaSetDevice(c->device));
-    const uint64_t group = zk_patch_group_bytes();
-    std::vector<uint64_t> rb;
-    std::vector<uint32_t> cs(n_frames);
-    size_t out = 0, in = 0;
-    for (uint32_t f0 = 0; f0 < n_frames;) {
-        uint64_t hlo, hhi;
-        const uint32_t end = zk_hull_group(ranges, f0, n_frames, group, &hlo, &hhi);
-        zk_rebase_ranges(ranges, f0, end, hlo, &rb);
-        size_t len = 0, bytes = 0;
-        for (uint32_t f = f0; f < end; f++) bytes += frame_sizes[f];
-        if (hhi > hlo) {
-            ZkCompressReq q;                                // zk_compress_frames_sized_prefixes(ldm = 1) on the decoded hull
-            q.policy = ZK_FRAMES_SIZED; q.sizes = frame_sizes + f0; q.count = end - f0; q.src = src ? src + in : nullptr;
-            if ((rc = zk_ref_prefix(c, ch, hlo, hhi, &q.prefix))) return rc;
-            q.prefix_len = (size_t)(hhi - hlo); q.prefix_dev = true; q.ranges = rb.data();
-            q.params.level = level; q.params.checksum = checksum; q.params.ldm = true;
-            q.dst = dst + out; q.dst_cap = dst_cap - out; q.c_sizes = cs.data() + f0; q.dst_len = &len;
-            rc = zk_compress(c, q);
-        } else {
-            rc = zk_compress_frames_sized(c, src ? src + in : nullptr, frame_sizes + f0, end - f0, 16, checksum, nullptr, 0, dst + out,
-                                          dst_cap - out, cs.data() + f0, &len);
-        }
-        if (rc) return rc;
-        out += len; in += bytes; f0 = end;
-    }
-    if (c_sizes && n_frames) memcpy(c_sizes, cs.data(), (size_t)n_frames * 4);
-    if (dst_len) *dst_len = out;
-    return 0;
+    return zk_ref_compress(c, src, frame_sizes, n_frames, level, checksum, ch, old_len, ranges, dst, dst_cap, c_sizes, dst_len);
 }
 
 extern "C" int32_t zk_compress_frames_patch_archive(zk_ctx* c, const uint8_t* src, const uint32_t* frame_sizes, uint32_t n_frames, int32_t level,
@@ -1628,8 +1586,8 @@ static int32_t zk_patch_scan_archive(zk_ctx* c, ZkChain& ch, std::vector<unsigne
         const uint64_t lo = r.d_off[g0], hi = r.d_off[g1];
         g0 = g1;
         if (hi == lo) continue;
-        const uint8_t* unused;
-        if ((rc = zk_ref_prefix(c, ch, lo, hi, &unused))) return rc;
+        rc = zk_ref_decode(c, ch, (uint32_t)ch.size() - 1, lo, hi, 1);
+        if (rc || (rc = zk_ref_failure(ch.back(), lo, hi))) return rc;
         uint8_t* run = (uint8_t*)c->d_prefix + ZK_REF_HEAD;
         if (ov) ZK_CUDA_OK(cudaMemcpyAsync(run - ov, s.d_out, ov, cudaMemcpyDeviceToDevice, s.stream));
         const uint64_t n = ov + (hi - lo);
@@ -1646,13 +1604,10 @@ static int32_t zk_patch_scan_archive(zk_ctx* c, ZkChain& ch, std::vector<unsigne
     return zk_sync_check(s.stream);
 }
 
-extern "C" int32_t zk_patch_ranges_chain(zk_ctx* c, const uint8_t* new_src, const uint32_t* frame_sizes, uint32_t n_frames,
-                                         const zk_reference_archive* chain, uint32_t depth, uint64_t margin, uint64_t* ranges) {
-    if (!c || (n_frames && (!frame_sizes || !ranges))) return ZK_ERR_INVALID_ARG;
-    ZkChain ch;
-    uint64_t old_len = 0;
-    int32_t rc = zk_chain_open(c, chain, depth, &ch, &old_len);
-    if (rc) return rc;
+// the anchors of OLD and NEW, then their join.  OLD's anchors: a raw root's bytes piece by piece through slot 0 (zk_patch_scan; not prefix
+// bytes), any other head decoded (zk_patch_scan_archive)
+static int32_t zk_ref_ranges(zk_ctx* c, ZkChain& ch, uint64_t old_len, const uint8_t* new_src, const uint32_t* frame_sizes, uint32_t n_frames,
+                             uint64_t margin, uint64_t* ranges) {
     if (old_len >= (1ull << 62) || margin >= (1ull << 62)) return ZK_ERR_INVALID_ARG;
     ZkPatchTables t;
     t.fa.assign((size_t)n_frames + 1, 0);
@@ -1661,7 +1616,8 @@ extern "C" int32_t zk_patch_ranges_chain(zk_ctx* c, const uint8_t* new_src, cons
     if (n && !new_src) return ZK_ERR_INVALID_ARG;
     if (n_frames == 0) return 0;
     ZK_CUDA_OK(cudaSetDevice(c->device));
-    rc = zk_patch_scan_archive(c, ch, &t.okeys, &t.opos);
+    const ZkRefLevel& h = ch.back();
+    int32_t rc = h.raw ? zk_patch_scan(c, h.r.comp, old_len, &t.okeys, &t.opos) : zk_patch_scan_archive(c, ch, &t.okeys, &t.opos);
     if (!rc) rc = zk_patch_scan(c, new_src, n, &t.nkeys, &t.npos);
     if (rc) return rc;
     if (t.okeys.size() > 0xFFFFFFF0ull || t.nkeys.size() > 0xFFFFFFF0ull) return ZK_ERR_INVALID_ARG;
@@ -1671,6 +1627,24 @@ extern "C" int32_t zk_patch_ranges_chain(zk_ctx* c, const uint8_t* new_src, cons
         t.fanc[f] = f == n_frames ? (uint32_t)t.npos.size() : i;
     }
     return zk_patch_join(&c->slot[0].ews, c->slot[0].stream, t, n_frames, old_len, margin, (unsigned long long*)ranges);
+}
+
+extern "C" int32_t zk_patch_ranges(zk_ctx* c, const uint8_t* new_src, const uint32_t* frame_sizes, uint32_t n_frames, const uint8_t* old,
+                                   uint64_t old_len, uint64_t margin, uint64_t* ranges) {
+    if (!c || (n_frames && (!frame_sizes || !ranges)) || (old_len && !old)) return ZK_ERR_INVALID_ARG;
+    ZkChain ch;
+    zk_chain_raw(c, old, old_len, &ch);
+    return zk_ref_ranges(c, ch, old_len, new_src, frame_sizes, n_frames, margin, ranges);
+}
+
+extern "C" int32_t zk_patch_ranges_chain(zk_ctx* c, const uint8_t* new_src, const uint32_t* frame_sizes, uint32_t n_frames,
+                                         const zk_reference_archive* chain, uint32_t depth, uint64_t margin, uint64_t* ranges) {
+    if (!c || (n_frames && (!frame_sizes || !ranges))) return ZK_ERR_INVALID_ARG;
+    ZkChain ch;
+    uint64_t old_len = 0;
+    const int32_t rc = zk_chain_open(c, chain, depth, &ch, &old_len);
+    if (rc) return rc;
+    return zk_ref_ranges(c, ch, old_len, new_src, frame_sizes, n_frames, margin, ranges);
 }
 
 extern "C" int32_t zk_patch_ranges_archive(zk_ctx* c, const uint8_t* new_src, const uint32_t* frame_sizes, uint32_t n_frames,
