@@ -9,10 +9,10 @@ intercept of a line in the sub-batch count): b is what each sub-batch's stage pa
 b's over a direction's chain is the most that overlapping the sub-batches of a call can win at that count.  The card's name, power limit and
 SM clock are read (read-only nvidia-smi queries) in the same call.  Prints one JSON object; --out also writes it.
 
---slots / --share sweep the pipelined calls as well (ZK_DEV_SLOTS sub-batches in flight, ZK_DEV_SHARE: the share of the machine each
-decode sizes its persistent kernels for); the fits are made of the one-slot rows, where the sub-batches run one after another.
+--slots sweeps the pipelined calls as well (ZK_DEV_SLOTS sub-batches in flight); the fits are made of the one-slot rows, where the
+sub-batches run one after another.
 
-usage: python tools/pipeline_probe.py [--bytes N] [--subs 64,128,256,512,1024] [--slots 1] [--share 1] [--levels 1,3c] [--reps 5] [--out FILE]"""
+usage: python tools/pipeline_probe.py [--bytes N] [--subs 64,128,256,512,1024] [--slots 1] [--levels 1,3c] [--reps 5] [--out FILE]"""
 import argparse
 import ctypes
 import json
@@ -97,14 +97,11 @@ def main():
     ap.add_argument("--bytes", type=int, default=bench.WORKLOAD_BYTES)
     ap.add_argument("--subs", default="64,128,256,512,1024", help="ZK_DEV_SUB_BYTES settings in MiB")
     ap.add_argument("--slots", default="1", help="ZK_DEV_SLOTS settings")
-    ap.add_argument("--share", default="1", help="ZK_DEV_SHARE settings (0: the slot count)")
     ap.add_argument("--levels", default="1,3c", help="levels; a trailing c: with checksum")
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
-    settings = [(int(s) * MIB, int(k), int(h) or int(k)) for k in args.slots.split(",") for h in sorted(set(args.share.split(",")))
-                for s in args.subs.split(",")]
-    settings = sorted(set(settings), key=lambda t: (t[1], t[2], t[0]))
+    settings = sorted({(int(s) * MIB, int(k)) for k in args.slots.split(",") for s in args.subs.split(",")}, key=lambda t: (t[1], t[0]))
     dev = torch.device("cuda", 0)
     lib = N.load()
     ctx = zk.Context(0, lib)
@@ -114,7 +111,7 @@ def main():
     lib.zk_ctx_profile(ctx._h, 1)
     res = {"card": card(), "bytes": args.bytes, "frame": FRAME, "reps": args.reps, "configs": {}}
     def use(st):
-        os.environ["ZK_DEV_SUB_BYTES"], os.environ["ZK_DEV_SLOTS"], os.environ["ZK_DEV_SHARE"] = (str(v) for v in st)
+        os.environ["ZK_DEV_SUB_BYTES"], os.environ["ZK_DEV_SLOTS"] = (str(v) for v in st)
 
     for lv in args.levels.split(","):
         level, ck = int(lv.rstrip("c")), lv.endswith("c")
@@ -129,16 +126,16 @@ def main():
         table = []
         for st in settings:
             r = rows[st]
-            table.append({"sub_MiB": st[0] // MIB, "slots": st[1], "share": st[2], "sub_batches": subs_of(args.bytes, st[0]),
+            table.append({"sub_MiB": st[0] // MIB, "slots": st[1], "sub_batches": subs_of(args.bytes, st[0]),
                           "compress_ms": float(np.median([v[0] for v in r])), "decompress_ms": float(np.median([v[2] for v in r])),
                           "compress_ms_range": [min(v[0] for v in r), max(v[0] for v in r)],
                           "decompress_ms_range": [min(v[2] for v in r), max(v[2] for v in r)],
                           "stage_ms": {SLOTS[i]: float(np.median([(v[1][i] if i in COMPRESS else v[3][i]) for v in r])) for i in range(8)},
                           "compressed_bytes": r[-1][4]})
-        serial = [t for t in table if t["slots"] == 1 and t["share"] == 1]
+        serial = [t for t in table if t["slots"] == 1]
         best = {d: min(table, key=lambda t: t[f"{d}_ms"]) for d in ("compress", "decompress")}
         cfg = res["configs"][f"level {level}" + (" + checksum" if ck else "")] = {
-            "table": table, "best": {d: {k: best[d][k] for k in ("sub_MiB", "slots", "share", f"{d}_ms")} for d in best}}
+            "table": table, "best": {d: {k: best[d][k] for k in ("sub_MiB", "slots", f"{d}_ms")} for d in best}}
         ks = [t["sub_batches"] for t in serial]
         if len(set(ks)) < 2 or 1 not in ks:
             continue

@@ -19,19 +19,15 @@ void zk_note_cuda_error(const char* what, int code) {
 }
 extern "C" const char* zk_last_cuda_error(void) { return zk_tls_cuda_msg; }
 
-static int zk_host_slots(bool enc);
 static size_t zk_env_size(const char* name, size_t dflt) {
     const char* s = getenv(name);
     if (!s || !*s) return dflt;
     return (size_t)strtoull(s, nullptr, 10);
 }
 
-// sub-batches in flight of the host-pointer pipelines (tuning knobs, swept by tools/e2e_sweep4.sh): decompress wants many
-// (its exec stage is latency-bound per frame), compress few (its kernels fill the machine from one 128 MiB sub-batch)
-static int zk_host_slots(bool enc) {
-    size_t v = zk_env_size(enc ? "ZK_HOST_SLOTS_ENC" : "ZK_HOST_SLOTS", enc ? 4 : 8);
-    return (int)(v < 1 ? 1 : (v > ZK_SLOTS ? ZK_SLOTS : v));
-}
+// sub-batches in flight of the host-pointer pipelines: decompress wants many (its exec stage is latency-bound per frame), compress few
+// (its kernels fill the machine from one sub-batch)
+static int zk_host_slots(bool enc) { return enc ? 4 : 8; }
 
 extern "C" const char* zk_version(void) {
 #ifdef ZK_EMUL
@@ -87,31 +83,25 @@ extern "C" int32_t zk_ctx_create(int32_t device_ordinal, uint32_t flags, zk_ctx*
     zk_ctx* c = new zk_ctx();
     c->device = device_ordinal;
     c->sm_count = prop.multiProcessorCount > 0 ? prop.multiProcessorCount : 132;
-    // ZK_HOST_PRIO (default 1): slot i runs at stream priority (greatest + i): concurrent sub-batches of the host pipelines then
-    // complete staggered (oldest slot first) instead of all at once, which keeps the D2H engine busy from early on
+    // slot i runs at stream priority (greatest + i): concurrent sub-batches of the host pipelines then complete staggered (oldest slot
+    // first) instead of all at once, which keeps the D2H engine busy from early on
     int least = 0, greatest = 0;
-    const bool use_prio = zk_env_size("ZK_HOST_PRIO", 1) != 0;
-    if (use_prio) cudaDeviceGetStreamPriorityRange(&least, &greatest);
+    cudaDeviceGetStreamPriorityRange(&least, &greatest);
     for (int i = 0; i < ZK_SLOTS; i++) {
-        const int prio = use_prio ? (greatest + i < least ? greatest + i : least) : 0;
+        const int prio = greatest + i < least ? greatest + i : least;
         if (cudaStreamCreateWithPriority(&c->slot[i].stream, cudaStreamNonBlocking, prio) != cudaSuccess) { delete c; return ZK_ERR_NO_DEVICE; }
         c->slot[i].dws.prio = c->slot[i].ews.prio = prio;
         c->slot[i].dws.sm_count = c->sm_count;
         c->slot[i].dws.ring_override = (uint32_t)zk_env_size("ZK_RING_BYTES", 0);   // tuning / tests: power of two >= 1024
         c->slot[i].dws.exec_warps = (uint32_t)zk_env_size("ZK_EXEC_WARPS", 0);
-        c->slot[i].dws.huf_pad = (uint32_t)zk_env_size("ZK_HUF_PAD", 0);
         c->slot[i].dws.exec_short = (uint32_t)zk_env_size("ZK_EXEC_SHORT", 128 << 10);
-        c->slot[i].dws.seq2_ctas = (uint32_t)zk_env_size("ZK_SEQ2_CTAS", 0);
-        c->slot[i].dws.huf_ctas = (uint32_t)zk_env_size("ZK_HUF_CTAS", 0);
         c->slot[i].dws.order = zk_env_size("ZK_DEC_ORDER", 1) != 0 ? 1u : 0u;
         c->slot[i].ews.sm_count = c->sm_count;
     }
     cudaEventCreate(&c->ev0); cudaEventCreate(&c->ev1);
     cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming);
     for (int i = 0; i < ZK_SLOTS; i++) cudaEventCreateWithFlags(&c->ev_join[i], cudaEventDisableTiming);
-    if (zk_env_size("ZK_HOST_COPY_STREAMS", 1) != 0) {
-        cudaStreamCreateWithFlags(&c->up, cudaStreamNonBlocking); cudaStreamCreateWithFlags(&c->down, cudaStreamNonBlocking);
-    }
+    cudaStreamCreateWithFlags(&c->up, cudaStreamNonBlocking); cudaStreamCreateWithFlags(&c->down, cudaStreamNonBlocking);
     *out = c;
     return 0;
 }
@@ -329,7 +319,7 @@ static int zk_dec_sub_finish(zk_ctx* c, int si, ZkSubDec& sb, const ZkDecCall& q
     return rc;
 }
 
-static int32_t zk_dec_run(zk_ctx* c, const ZkDecCall& q, uint32_t n, size_t sub_bytes, int ns, uint32_t ramp);
+static int32_t zk_dec_run(zk_ctx* c, const ZkDecCall& q, uint32_t n, size_t sub_bytes, int ns);
 
 extern "C" int32_t zk_decompress_frames(zk_ctx* c, const uint8_t* comp, const uint64_t* c_off, const uint64_t* d_off,
                                         uint32_t n, uint8_t* dst, int32_t verify, int32_t* status) {
@@ -389,20 +379,15 @@ static int32_t zk_decompress_prefixes_one(zk_ctx* c, const uint8_t* comp, const 
     if (n && (!comp || !c_off || !d_off || !dst)) return ZK_ERR_INVALID_ARG;
     if (n == 0) return 0;
     ZK_CUDA_OK(cudaSetDevice(c->device));
-    const size_t sub_bytes = zk_env_size("ZK_HOST_SUB_BYTES", (size_t)128 << 20);     // tuning knob (tools/e2e_sweep2.sh sweeps it)
+    const size_t sub_bytes = zk_env_size("ZK_HOST_SUB_BYTES", (size_t)128 << 20);     // output bytes per sub-batch (tests set less)
     q.p.need = d_need;
-    q.p.share = (int)zk_env_size("ZK_HOST_SHARE", 3);
-    q.p.side = zk_env_size("ZK_HOST_SIDE", 1) != 0;
+    q.p.share = 3;                                          // K-D2 sized as if three sub-batches shared the GPU
     q.p.up = c->up; q.p.down = c->down;
-    // ZK_HOST_RAMP=r (default 0): the first r sub-batches are 1/2^r ... 1/2 of the full size, so that the output copy could start
-    // earlier.  It gave no gain when it was tried: a sub-batch of any size spends about one frame latency in
-    // K-D2, so a small first sub-batch is not done much sooner than a full one
-    return zk_dec_run(c, q, n, sub_bytes, zk_host_slots(false), (uint32_t)zk_env_size("ZK_HOST_RAMP", 0));
+    return zk_dec_run(c, q, n, sub_bytes, zk_host_slots(false));
 }
 
-// the sub-batches of a decompress call, dealt round-robin over ns slots; the first `ramp` are 1/2^ramp ... 1/2 of sub_bytes.  Returns 0
-// or the first failure in the order of the entries
-static int32_t zk_dec_run(zk_ctx* c, const ZkDecCall& q, uint32_t n, size_t sub_bytes, int ns, uint32_t ramp) {
+// the sub-batches of a decompress call, dealt round-robin over ns slots.  Returns 0 or the first failure in the order of the entries
+static int32_t zk_dec_run(zk_ctx* c, const ZkDecCall& q, uint32_t n, size_t sub_bytes, int ns) {
     ZkSubDec sub[ZK_SLOTS];
     int32_t worst = 0, rc;
     uint32_t k = 0;
@@ -411,8 +396,7 @@ static int32_t zk_dec_run(zk_ctx* c, const ZkDecCall& q, uint32_t n, size_t sub_
         int si = (int)(k % ns);
         rc = zk_dec_sub_finish(c, si, sub[si], q);
         if (rc && !worst) worst = rc;
-        const size_t this_sub = k < ramp ? sub_bytes >> (ramp - k) : sub_bytes;
-        uint32_t end = zk_next_sub(q.d_off, first, n, this_sub, 1u << 20);
+        uint32_t end = zk_next_sub(q.d_off, first, n, sub_bytes, 1u << 20);
         sub[si].first = first; sub[si].count = end - first;
         rc = zk_dec_sub_enqueue(c, si, sub[si], q, &tr, (int)k);
         if (rc) { if (!worst) worst = rc; break; }
@@ -435,11 +419,9 @@ extern "C" int32_t zk_decompress_frames_dev(zk_ctx* c, const void* d_comp, const
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : c->slot[0].stream;
     ZkDecCall q = {(const uint8_t*)d_comp, c_off, d_off, (uint8_t*)d_dst, verify, status, ZkDecodeParams(), false};
     const int ns = zk_dev_slots(false);
-    q.p.side = zk_env_size("ZK_DEV_SIDE", 1) != 0;
-    q.p.share = (int)zk_env_size("ZK_DEV_SHARE", 1);
     ZK_CUDA_OK(cudaEventRecord(c->ev0, st));
     int32_t rc = zk_dev_fork(c, st, ns);
-    const int32_t worst = rc ? rc : zk_dec_run(c, q, n, zk_dev_sub_bytes(false), ns, 0);
+    const int32_t worst = rc ? rc : zk_dec_run(c, q, n, zk_dev_sub_bytes(false), ns);
     if ((rc = zk_dev_join(c, st, ns))) return rc;
     ZK_CUDA_OK(cudaEventRecord(c->ev1, st));
     ZK_CUDA_OK(cudaEventSynchronize(c->ev1));
@@ -713,19 +695,15 @@ static int32_t zk_compress(zk_ctx* c, ZkCompressReq q) {
     }
     ZK_CUDA_OK(cudaSetDevice(c->device));
     const cudaStream_t st = q.stream ? q.stream : c->slot[0].stream;
-    // tuning knobs: input bytes per sub-batch, and the first pass of the cut policies (tools/knobs_round.sh sweeps the host one)
+    // input bytes per sub-batch, and the first pass of the cut policies (tests set less)
     const size_t sub_bytes = q.host ? zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20) : zk_dev_sub_bytes(true);
     if (!q.host) cudaEventRecord(c->ev0, st);
     size_t out_len = 0;
     const size_t first_pass = q.host ? sub_bytes : zk_dev_sub_bytes(false);
     if (q.policy == ZK_FRAMES_COMPRESSED) rc = zk_csize_passes(c, q, st, first_pass);
     else if (q.policy == ZK_FRAMES_CONTENT) rc = zk_cdc_passes(c, q, st, first_pass, sub_bytes);
-    else {
-        ZkEncodeParams p = q.params;
-        if (q.host) p.side = zk_env_size("ZK_HOST_SIDE", 1) != 0;
-        rc = zk_compress_run(c, fr, q.src, p, q.dst, q.dst_cap, q.c_sizes, q.host, sub_bytes, q.host ? zk_host_slots(true) : zk_dev_slots(true), st,
-                             &out_len);
-    }
+    else rc = zk_compress_run(c, fr, q.src, q.params, q.dst, q.dst_cap, q.c_sizes, q.host, sub_bytes,
+                              q.host ? zk_host_slots(true) : zk_dev_slots(true), st, &out_len);
     if (rc) return rc;
     if (!q.host) {                                          // zk_ctx_last_device_ms: the device paths only
         cudaEventRecord(c->ev1, st);
@@ -1087,7 +1065,6 @@ extern "C" int32_t zk_compress_frames_sized_reuse(zk_ctx* c, const uint8_t* src,
     // pass B: the new frames, sub-batch by sub-batch
     ZkEncodeParams p;
     p.level = level; p.checksum = checksum; p.long_mode = long_mode != 0;
-    p.side = zk_env_size("ZK_HOST_SIDE", 1) != 0;
     const ZkFrames fr = {frame_sizes, n, 0, n_frames};
     const size_t enc_sub = zk_env_size("ZK_HOST_SUB_BYTES_ENC", (size_t)96 << 20);
     const uint32_t NONE = 0xFFFFFFFFu;

@@ -2118,23 +2118,23 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     ws->prof.end(0, stream);
     // entropy stage: persistent warp-CTAs pulling groups of blocks from a work counter
     size_t est_blocks = (size_t)(total_d / ZK_BLOCK_MAX) + n;
-    const size_t huf_smem = sizeof(ZkHufTab) * ZK_HUF_SLOTS + sizeof(ZkHufScratch);
+    constexpr size_t huf_smem = sizeof(ZkHufTab) * ZK_HUF_SLOTS + sizeof(ZkHufScratch);
+    static_assert(huf_smem <= 48 * 1024, "K-D1h launches without a shared-memory opt-in");
     const size_t seq2_smem = ((sizeof(ZkSeqTabs) + 127) & ~(size_t)127) + sizeof(ZkSeq2Chain<ZK_SEQ_CELLS_COMPACT>) * ZK_S2_NCH;
     const size_t seq2f_smem = ((sizeof(ZkSeqTabs) + 127) & ~(size_t)127) + sizeof(ZkSeq2Chain<ZK_SEQ_CELLS_FULL>) * ZK_S2_NCH;
     if (!ws->attr_set) {
         ZK_CUDA_OK(cudaFuncSetAttribute(zk_seq2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)seq2_smem));
         ZK_CUDA_OK(cudaFuncSetAttribute(zk_seq2_full_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)seq2f_smem));
-        ZK_CUDA_OK(cudaFuncSetAttribute(zk_huf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)huf_smem + 65536));
         ZK_CUDA_OK(cudaFuncSetAttribute(zk_exec_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
         ZK_CUDA_OK(cudaFuncSetAttribute(zk_exec_kernel_w5<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
         ZK_CUDA_OK(cudaFuncSetAttribute(zk_exec_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
         ZK_CUDA_OK(cudaFuncSetAttribute(zk_exec_kernel_w5<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
         ws->attr_set = true;
     }
-    if (!ws->huf_fit) {                          // K-D1h CTAs that fit on an SM by their shared memory (+ the tuning pad)
+    if (!ws->huf_fit) {                          // K-D1h CTAs that fit on an SM by their shared memory
 #ifndef ZK_EMUL
         int fit = 0;
-        ZK_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fit, zk_huf_kernel, 32, huf_smem + ws->huf_pad));
+        ZK_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fit, zk_huf_kernel, 32, huf_smem));
         ws->huf_fit = fit > 0 ? (uint32_t)fit : 1u;
 #else
         ws->huf_fit = 16;                        // (no SM to fill)
@@ -2143,7 +2143,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     // Half of them: K-D1s runs beside K-D1h, and the two only overlap when both fit on the SM (DESIGN §6).  K-D1s gets the CTAs
     // that fit in three quarters of an SM's shared memory (7 on H100: the best of 5-8 measured beside K-D1h's grid), at most
     // what the occupancy query allows; the CTAs of either kernel that do not fit beside the other's start as those finish.
-    const uint32_t huf_ctas = ws->huf_ctas ? ws->huf_ctas : (ws->huf_fit > 1 ? ws->huf_fit / 2 : 1u);
+    const uint32_t huf_ctas = ws->huf_fit > 1 ? ws->huf_fit / 2 : 1u;
     if (!ws->seq2_fit) {
 #ifndef ZK_EMUL
         int dev = 0, fit = 0, sm_smem = 0, reserved = 0;
@@ -2161,24 +2161,21 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     const size_t need_h = est_blocks / ZK_HUF_SLOTS + 1;
     if (need_h < gh) gh = (uint32_t)need_h;
     // the two entropy kernels are independent: run the Huffman one on a side stream
-    cudaStream_t hs = stream;
-    if (p.side) {
-        if (!ws->side) {
-            ZK_CUDA_OK(cudaStreamCreateWithPriority(&ws->side, cudaStreamNonBlocking, ws->prio));
-            ZK_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_scan, cudaEventDisableTiming));
-            ZK_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_huf, cudaEventDisableTiming));
-        }
-        hs = ws->side;
-        ZK_CUDA_OK(cudaEventRecord(ws->ev_scan, stream));
-        ZK_CUDA_OK(cudaStreamWaitEvent(hs, ws->ev_scan, 0));
+    if (!ws->side) {
+        ZK_CUDA_OK(cudaStreamCreateWithPriority(&ws->side, cudaStreamNonBlocking, ws->prio));
+        ZK_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_scan, cudaEventDisableTiming));
+        ZK_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_huf, cudaEventDisableTiming));
     }
+    const cudaStream_t hs = ws->side;
+    ZK_CUDA_OK(cudaEventRecord(ws->ev_scan, stream));
+    ZK_CUDA_OK(cudaStreamWaitEvent(hs, ws->ev_scan, 0));
     ws->prof.begin(2, hs);
-    ZK_LAUNCH(zk_huf_kernel, gh, 32, huf_smem + ws->huf_pad, hs, o);
+    ZK_LAUNCH(zk_huf_kernel, gh, 32, huf_smem, hs, o);
     ws->prof.end(2, hs);
-    if (hs != stream) ZK_CUDA_OK(cudaEventRecord(ws->ev_huf, hs));
+    ZK_CUDA_OK(cudaEventRecord(ws->ev_huf, hs));
     ws->prof.begin(1, stream);
     {
-        uint32_t g2 = (uint32_t)sms * (ws->seq2_ctas ? ws->seq2_ctas : ws->seq2_fit);
+        uint32_t g2 = (uint32_t)sms * ws->seq2_fit;
         const size_t need2 = est_blocks / ZK_S2_NCH + 1;
         if (need2 < g2) g2 = (uint32_t)need2;
         ZK_LAUNCH(zk_seq2_kernel, g2, 32, seq2_smem, stream, o);
@@ -2186,7 +2183,7 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
         ZK_LAUNCH(zk_seq2_full_kernel, (uint32_t)sms, 32, seq2f_smem, stream, o);
     }
     ws->prof.end(1, stream);
-    if (hs != stream) ZK_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_huf, 0));
+    ZK_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_huf, 0));
     // exec stage: ring size / warps per entry chosen from how many entries share the machine
     // Each entry is one serial dependency chain, so throughput comes from entries in flight: pick warps per
     // CTA and ring size such that (if possible) every entry of the batch is resident at once.
@@ -2215,22 +2212,20 @@ int zk_decode_enqueue(ZkDecodeWs* ws, cudaStream_t stream, const uint8_t* d_comp
     void (*cta_kernel)(ZkDecodeArgs, uint32_t) = small_regs ? (prefix ? zk_exec_kernel_w5<true> : zk_exec_kernel_w5<false>)
                                                             : (prefix ? zk_exec_kernel<true> : zk_exec_kernel<false>);
     // Long segments run on the side stream beside the short ones: segments never wait for each other, so the CTA executor's long serial
-    // chains start with the warp executor's work instead of after its drain.  They are launched first, so their CTAs are resident first
-    const bool beside = a.exec_short && hs != stream;
-    if (beside) {
+    // chains start with the warp executor's work instead of after its drain.  They are launched first, so their CTAs are resident first.
+    // Without short segments every segment runs on the CTAs, on `stream`
+    if (a.exec_short) {
         ZK_CUDA_OK(cudaEventRecord(ws->ev_scan, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(hs, ws->ev_scan, 0));     // after the plan (and K-D1o)
         ZK_LAUNCH(cta_kernel, n, W * 32, ring, hs, o, ring);
         ZK_CUDA_OK(cudaEventRecord(ws->ev_huf, hs));
-    }
-    if (a.exec_short) {          // short segments on single warps; the CTAs pull only long ones
+        // short segments on single warps; the CTAs pull only long ones
         uint32_t gw = (uint32_t)sms * 8u;
         const size_t need_w = est_blocks / ZK_XW_WARPS + 1;
         if (need_w < gw) gw = (uint32_t)need_w;
         void (*warp_kernel)(ZkDecodeArgs) = prefix ? zk_exec_warp_kernel<true> : zk_exec_warp_kernel<false>;
         ZK_LAUNCH(warp_kernel, gw, 32 * ZK_XW_WARPS, ZK_XW_WARPS * ZK_XW_WIN, stream, o);
-    }
-    if (beside) ZK_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_huf, 0));
-    else ZK_LAUNCH(cta_kernel, n, W * 32, ring, stream, o, ring);
+        ZK_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_huf, 0));
+    } else ZK_LAUNCH(cta_kernel, n, W * 32, ring, stream, o, ring);
     ws->prof.end(3, stream);
     if (verify_checksum) { ws->prof.begin(4, stream); ZK_LAUNCH(zk_xxh64_kernel, (n + 3) / 4, 128, 0, stream, a); ws->prof.end(4, stream); }
     if (ds != stream) { ZK_CUDA_OK(cudaEventRecord(ws->ev_done, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(ds, ws->ev_done, 0)); }

@@ -39,12 +39,9 @@ struct ZkDecodeWs {                   // HBM scratch owned by a zk_ctx, grown on
     uint32_t order = 1;               // ZK_DEC_ORDER: 1 = run every work list heaviest first (zk_order_kernel), 0 = in the order it was filled
     bool attr_set = false; uint32_t ring_override = 0;
     uint32_t exec_warps = 0;          // ZK_EXEC_WARPS: warps per K-D2 CTA (at most 16); 0 = chosen from the entries per SM
-    uint32_t seq2_ctas = 0;           // ZK_SEQ2_CTAS: persistent K-D1s CTAs per SM; 0 = seq2_fit
     uint32_t seq2_fit = 0;            // K-D1s CTAs in three quarters of an SM's shared memory (queried at the first launch; DESIGN §6)
     uint32_t exec_short = 128 << 10;  // ZK_EXEC_SHORT: output bytes up to which a segment runs on one warp (zk_exec_warp_kernel); 0 = CTAs only
-    uint32_t huf_pad = 0;             // extra dynamic smem per Huffman CTA: fewer resident CTAs -> more L1 for the streams (tuning)
     int prio = 0;                     // CUDA stream priority of the side stream (matches the slot's stream)
-    uint32_t huf_ctas = 0;            // persistent K-D1h CTAs per SM (tuning: ZK_HUF_CTAS); 0: half of huf_fit
     uint32_t huf_fit = 0;             // K-D1h CTAs that fit on an SM (occupancy query at the first launch; 0 = not asked yet)
     cudaEvent_t ev_up = nullptr, ev_done = nullptr, ev_down = nullptr;
     cudaStream_t side = nullptr; cudaEvent_t ev_scan = nullptr, ev_huf = nullptr;   // Huffman kernel runs beside the FSE kernel
@@ -63,8 +60,6 @@ struct ZkDecodeParams {
     const uint32_t* ranges = nullptr; // host, two per entry: the prefix of entry e's frames is prefix[ranges[2e], ranges[2e + 1]); nullptr: all of it
     const uint32_t* need = nullptr;   // host, one per entry: leading bytes wanted (ZkDecodeArgs::d_need); nullptr = everything
     int share = 1;                    // how many batches share the GPU concurrently (host pipeline depth)
-    bool side = true;                 // K-D1h on the side stream; host pipelines get their concurrency from the other sub-batches instead,
-                                      // and every extra stream costs a hardware queue
     cudaStream_t up = nullptr, down = nullptr;      // host pipelines: dedicated upload / download streams (not owned); nullptr = everything on `stream`
 };
 

@@ -1638,10 +1638,8 @@ static int zkc_build_geometry(ZkEncodeWs* ws, cudaStream_t stream, ZkcGeo* geo, 
     return 0;
 }
 
-// the stream K-C2s and the checksum run on: the workspace's side stream (created at its first use), or `stream` itself without one
-static int zkc_side_stream(ZkEncodeWs* ws, cudaStream_t stream, bool side, cudaStream_t* ss) {
-    *ss = stream;
-    if (!side) return 0;
+// the stream K-C2s and the checksum run on: the workspace's side stream, created at its first use
+static int zkc_side_stream(ZkEncodeWs* ws, cudaStream_t* ss) {
     if (!ws->side) {
         ZK_CUDA_OK(cudaStreamCreateWithPriority(&ws->side, cudaStreamNonBlocking, ws->prio));
         ZK_CUDA_OK(cudaEventCreateWithFlags(&ws->ev_a, cudaEventDisableTiming));
@@ -1768,15 +1766,14 @@ int zk_encode_enqueue(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src,
     // the content checksum only needs the input: it runs beside the match finder on the side stream (one warp per frame, bound
     // by the latency of its four serial chains, so it leaves the machine to K-C1)
     cudaStream_t ss;
-    if ((rc = zkc_side_stream(ws, stream, p.side, &ss))) return rc;
-    if (p.checksum && ss != stream) {
+    if ((rc = zkc_side_stream(ws, &ss))) return rc;
+    if (p.checksum) {                                       // joined by ev_b in zkc_run_blocks
         ZK_CUDA_OK(cudaEventRecord(ws->ev_c, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(ss, ws->ev_c, 0));     // after whatever produced the input
         ZK_LAUNCH(zk_frame_hash_kernel, (n_frames + 3) / 4, 128, 0, ss, a);
     }
     rc = zkc_run_blocks(ws, stream, ss, a, &hc);
     if (rc) return rc;
     ws->prof.begin(7, stream);
-    if (p.checksum && ss == stream) ZK_LAUNCH(zk_frame_hash_kernel, (n_frames + 3) / 4, 128, 0, stream, a);   // else: already done on the side stream (joined by ev_b)
     ZK_LAUNCH(zk_frame_size_kernel, (n_frames + 3) / 4, 128, 0, stream, a);
     if (p.chain_wait) ZK_CUDA_OK(cudaStreamWaitEvent(stream, p.chain_wait, 0));     // the scan of the batch before wrote chain[0]
     ZK_LAUNCH(zk_frame_scan_kernel, 1, 1024, 0, stream, a, p.chain);
@@ -1820,12 +1817,12 @@ static int zkc_run_blocks(ZkEncodeWs* ws, cudaStream_t stream, cudaStream_t ss, 
     if (!ws->attr_set) { ZK_CUDA_OK(cudaFuncSetAttribute(zk_seq_enc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)seq_smem)); ws->attr_set = true; }
     // the two entropy kernels are independent and both latency-bound: run them side by side, join in zk_block_finish_kernel
     ws->prof.begin(6, stream);
-    if (ss != stream) { ZK_CUDA_OK(cudaEventRecord(ws->ev_a, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(ss, ws->ev_a, 0)); }
+    ZK_CUDA_OK(cudaEventRecord(ws->ev_a, stream)); ZK_CUDA_OK(cudaStreamWaitEvent(ss, ws->ev_a, 0));
     ZK_LAUNCH(zk_seq_enc_kernel, (uint32_t)((n_blocks + ZKC_SW - 1) / ZKC_SW), 32 * ZKC_SW, seq_smem, ss, a);
-    if (ss != stream) ZK_CUDA_OK(cudaEventRecord(ws->ev_b, ss));
+    ZK_CUDA_OK(cudaEventRecord(ws->ev_b, ss));
     if (a.level < 0) ZK_LAUNCH((zk_lit_enc_kernel<false, 1>), (uint32_t)n_blocks, 32, 0, stream, a);
     else ZK_LAUNCH((zk_lit_enc_kernel<true, ZKC_LW>), (uint32_t)((n_blocks + ZKC_LW - 1) / ZKC_LW), 32 * ZKC_LW, 0, stream, a);
-    if (ss != stream) ZK_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_b, 0));
+    ZK_CUDA_OK(cudaStreamWaitEvent(stream, ws->ev_b, 0));
     ZK_LAUNCH(zk_block_finish_kernel, (uint32_t)((n_blocks + 3) / 4), 128, 0, stream, a);
     ws->prof.end(6, stream);
     return 0;
@@ -1885,7 +1882,7 @@ int zk_encode_csize(ZkEncodeWs* ws, cudaStream_t stream, const uint8_t* d_src, s
     c.pfx = pfx; c.plen = p.prefix_len;
     ZK_CUDA_OK(cudaMemsetAsync(a.res, 0, ZKC_RES_HDR * 4, stream));
     cudaStream_t ss;
-    if ((rc = zkc_side_stream(ws, stream, p.side, &ss))) return rc;
+    if ((rc = zkc_side_stream(ws, &ss))) return rc;
     uint32_t* vcount = (uint32_t*)(base + o_cnt);
     rc = zkc_build_geometry(ws, stream, (ZkcGeo*)(base + o_geo0), (ZkcFrame*)(base + o_fr0), vcount, {nullptr, n, ZKC_BLOCK, nb}, nb, nullptr, pfx,
                             p.prefix_len, nullptr);

@@ -27,8 +27,6 @@ struct ZkEncodeParams {
                                       // whole buffer for every frame
     bool ldm = false;                 // long-distance matching against the whole of each frame's prefix (nothing without one)
     bool long_mode = false;           // long mode: every frame also matches its own bytes up to 2^27 back (and the prefix as ldm does)
-    bool side = true;                 // K-C2s and the checksum on the side stream; host pipelines get their concurrency from the other
-                                      // sub-batches instead, and every extra stream costs a hardware queue
     // batches that write one output one after another, each enqueued before the one before it completed: chain[0] (device) holds the
     // bytes before the batch's frames, which it writes from d_dst + chain[0] on, and its frame scan writes chain[1] after waiting for
     // chain_wait (that of the batch before: its ZkEncodeWs::ev_chain; nullptr: none).  dst_cap bounds the whole output

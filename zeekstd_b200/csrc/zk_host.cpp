@@ -380,7 +380,7 @@ struct zk_encoder {
     uint64_t written_compressed = 0;
     std::vector<uint8_t> batch;            // complete + partial frames not yet compressed (Uncompressed policy)
     std::vector<uint8_t> stage;
-    size_t batch_frames = 8192;            // a GPU call takes the buffered complete frames once there are this many ...
+    static constexpr size_t batch_frames = 8192;   // a GPU call takes the buffered complete frames once there are this many ...
     size_t batch_bytes = (size_t)128 << 20; // ... or this many bytes of them (64 frames of 2 MiB; thousands of small ones: one launch sequence serves them all)
     const uint8_t* prefix = nullptr; size_t prefix_len = 0;   // prefix of the frames in `batch` (compress_with_prefix)
     size_t csize_at = (size_t)128 << 20;   // Compressed(n), ContentDefined(n): buffered bytes at which the next cut runs (doubles while a cut closes no frame)
@@ -446,8 +446,6 @@ extern "C" int32_t zk_encode_options_into_encoder(zk_encode_options* o, zk_write
     if (!e) return ZK_ERR_ZSTD(64);
     e->raw.ctx = o->ctx; e->raw.kind = o->kind; e->raw.size = o->size; e->raw.checksum = o->checksum; e->raw.level = o->level; e->raw.ldm = o->ldm; e->raw.lmode = o->lmode;
     e->write = write; e->flush = flush; e->user = user;
-    const char* bf = getenv("ZK_ENCODER_BATCH_FRAMES");
-    if (bf && atoi(bf) > 0) e->batch_frames = (size_t)atoi(bf);
     delete o;
     *out = e;
     return 0;
@@ -552,7 +550,7 @@ struct zk_decoder {                        // decode.rs:121-466
     // mirroring "no reset when seeking forward in the same frame", decode.rs:407-410)
     uint32_t win_lo = 0, win_hi = 0; std::vector<uint8_t> window; std::vector<uint8_t> comp;
     uint64_t win_valid_end = 0;            // the window is decoded up to this decompressed offset (< d[win_hi] after a range read)
-    size_t max_window_bytes = (size_t)256 << 20;
+    static constexpr size_t max_window_bytes = (size_t)256 << 20;
     const uint8_t* prefix = nullptr; size_t prefix_len = 0;   // the prefix the window was decoded with (decompress_with_prefix)
     const uint64_t* ranges = nullptr;                          // and every entry's range of it (nullptr: the whole prefix)
     bool archive = false;                                      // the prefix is OLD of this reference chain instead (a copy of its
@@ -618,8 +616,6 @@ extern "C" int32_t zk_decode_options_into_decoder(zk_decode_options* o, zk_decod
     delete o;
     if (rc) { delete d; return rc; }
     d->offset = offset; d->offset_limit = limit;
-    const char* mw = getenv("ZK_DECODER_WINDOW_BYTES");
-    if (mw && atoll(mw) > 0) d->max_window_bytes = (size_t)atoll(mw);
     *out = d;
     return 0;
 }
